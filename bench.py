@@ -55,15 +55,16 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region, and the card's name and power
+    limit: a rate is only comparable with one measured on the same card at the same limit."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,name,power.limit")
 
     def __init__(self, gpu_index: int):
         self.rows = []
@@ -89,6 +90,8 @@ class ClockSampler:
         time.sleep(0.25)
         self.proc.terminate()
         sm, smax, reasons = [], [], set()
+        gpu = {"gpu_name": self.rows[0][9] if self.rows and len(self.rows[0]) > 10 else None,
+               "power_limit_w": self.rows[0][10] if self.rows and len(self.rows[0]) > 10 else None}
         for r in self.rows:
             try:
                 sm.append(float(r[1])); smax.append(float(r[2]))
@@ -98,7 +101,7 @@ class ClockSampler:
                 if val.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(smax) if smax else None,
-                "samples": len(sm), "reasons": sorted(reasons)}
+                "samples": len(sm), "reasons": sorted(reasons), **gpu}
 
 
 def workload_config(gpus: int, chunks: int) -> dict:
@@ -107,7 +110,7 @@ def workload_config(gpus: int, chunks: int) -> dict:
                         "encode + key-table insert",
             "chunk_bytes": CHUNK, "chunks_per_gpu_per_step": chunks, "pshift": PSHIFT, "accel": ACCEL,
             "sharding": f"chunk k -> rank k mod {gpus}" if gpus > 1 else "single GPU",
-            "l2": "per-step input (1 GiB) is larger than the 126 MB L2; no explicit flush"}
+            "l2": "per-step input (1 GiB) is larger than the 50 MB L2 of an H100; no explicit flush"}
 
 
 # -------------------------------------------------------------------------------------------------
@@ -462,6 +465,26 @@ def run_config_4(args, E, O, torch, dist, rank, world, local, d_pages, threads, 
     return res
 
 
+def dump_outputs(out_dir: str, eng, u, l, lens, sample: int = 128) -> None:
+    """What the last timed step computed, as its caller receives it, for output-for-output comparison
+    of two builds: the stored length of every chunk, every chunk's EF128 fingerprint (as 32-bit
+    words, exact in float64) and the stored records {data_prefix, LZ4 block} of a fixed, seeded
+    sample of `sample` chunks (zero past each record's end; ~34 MB in float32)."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "stored_lengths.npy"), lens.astype(np.float64))
+    fps, ok = eng.read_fingerprints(u, l)
+    assert ok.all(), "a chunk of the last timed step has no fingerprint"
+    words = np.stack([fps[:, 0] >> np.uint64(32), fps[:, 0] & np.uint64(0xFFFFFFFF),
+                      fps[:, 1] >> np.uint64(32), fps[:, 1] & np.uint64(0xFFFFFFFF)], axis=1)
+    np.save(os.path.join(out_dir, "fingerprints.npy"), words.astype(np.float64))
+    pick = np.sort(np.random.default_rng(SEED).choice(len(u), size=min(sample, len(u)), replace=False))
+    recs, rec_lens = eng.read_records_raw(u[pick], l[pick])
+    recs[np.arange(recs.shape[1])[None, :] >= rec_lens[:, None]] = 0
+    np.save(os.path.join(out_dir, "records_sample.npy"), recs.astype(np.float32))
+    np.save(os.path.join(out_dir, "records_sample_lengths.npy"), rec_lens.astype(np.float64))
+    np.save(os.path.join(out_dir, "records_sample_index.npy"), pick.astype(np.float64))
+
+
 def run_ours(args):
     import torch
     import edge_fuse_b200 as E
@@ -489,11 +512,14 @@ def run_ours(args):
     PASSES = 3                                    # device-resident, e2e synchronous, e2e write-behind
     # Arena: every put of every pass goes to a fresh address, sized for the WORST case (incompressible
     # pages) so that no put can be dropped; if K is so large that this does not fit in HBM the
-    # addresses recycle every R steps (records of equal size are then rewritten in place).
+    # addresses recycle every R steps.  A put never reuses the bytes of the record it replaces
+    # (records are immutable), so once addresses recycle the arena is compacted between steps,
+    # outside the timed windows, whenever the next step might not fit (see make_room); one step more
+    # than the R distinct steps of every pass guarantees that a compaction frees enough.
     free_b, _ = torch.cuda.mem_get_info(local)
     budget = int(free_b * 0.60) - (6 << 30)
     R = max(1, min(T, budget // (PASSES * n * WORST)))
-    arena = PASSES * R * n * WORST + (5 << 30)    # + room for the per-warp arena segments in flight
+    arena = (PASSES * R + 1) * n * WORST + (5 << 30)    # + room for the per-warp arena segments in flight
     keys_all_ranks = PASSES * R * n * world
     eng = E.Engine(pshift=PSHIFT, accel=ACCEL, capacity=keys_all_ranks, table_slots=next_pow2(2 * keys_all_ranks),
                    arena_bytes=arena, max_batch=args.max_batch, flags=E.FINGERPRINT, device=local)
@@ -519,6 +545,33 @@ def run_ours(args):
         counter[0] += 1
         return base
 
+    room = {"bound": 0, "compactions": 0, "ms": 0.0}   # bound: arena bytes in use, at most
+
+    def step_fits() -> bool:
+        """Reserves the worst case of one more step in the arena; False when it might not fit."""
+        if room["bound"] + n * WORST > arena - (5 << 30):
+            return False
+        room["bound"] += n * WORST
+        return True
+
+    def compact() -> float:
+        """Compacts the arena (no step may be in flight) and reserves the next step; -> seconds taken.
+        The new bound is the largest live size over the ranks, so that every rank decides the same
+        way and compacts before the same step."""
+        t0 = time.perf_counter()
+        torch.cuda.synchronize()
+        eng.compact()
+        used = eng.stats()["arena_used"]
+        if dist:
+            tt = torch.tensor([used], dtype=torch.float64, device="cuda")
+            dist.all_reduce(tt, op=dist.ReduceOp.MAX)
+            used = int(tt[0].item())
+        room["bound"] = used + n * WORST
+        room["compactions"] += 1
+        dt = time.perf_counter() - t0
+        room["ms"] += dt * 1e3
+        return dt
+
     def check_integrity(what: str) -> dict:
         st = eng.stats()
         expect = len(written) * n
@@ -532,9 +585,20 @@ def run_ours(args):
 
     # ---- pass 0: device-resident -> value ----
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(K)]
-    ev_all = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+    # the timed region is one window of events, or several when compactions fall between its steps
+    windows = []
     st0 = None
+    paused_s = 0.0
     for it in range(T):
+        if not step_fits():
+            xch.flush()
+            if it > W:
+                windows[-1][1].record(main)
+            dt = compact()
+            if it > W:
+                paused_s += dt
+                windows.append((torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)))
+                windows[-1][0].record(main)
         if it == W:
             xch.flush()
             sync_all()
@@ -542,7 +606,8 @@ def run_ours(args):
             sampler.start()
             st0 = eng.stats()
             t_wall0 = time.perf_counter()
-            ev_all[0].record(main)
+            windows.append((torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)))
+            windows[-1][0].record(main)
         if it >= W:
             ev[it - W][0].record(main)
         u, l = addr_for(it, 0)
@@ -550,14 +615,14 @@ def run_ours(args):
         if it >= W:
             ev[it - W][1].record(main)
     xch.flush()                                   # the last step's records are imported inside the region
-    ev_all[1].record(main)
+    windows[-1][1].record(main)
     sync_all()
-    t_wall = time.perf_counter() - t_wall0
+    t_wall = time.perf_counter() - t_wall0 - paused_s
     st1 = eng.stats()
     lens = xch.last_lens()
     u_last, l_last = addr_for(T - 1, 0)
     dev_ms_steps = [a.elapsed_time(b) for a, b in ev]
-    dev_ms_total = ev_all[0].elapsed_time(ev_all[1])
+    dev_ms_total = sum(a.elapsed_time(b) for a, b in windows)
     breakdown = xch.breakdown_ms()
     if dist:
         tt = torch.tensor([dev_ms_total, t_wall * 1e3], dtype=torch.float64, device="cuda")
@@ -574,6 +639,8 @@ def run_ours(args):
     e2e_t = []
     lens_e = None
     for it in range(T):
+        if not step_fits():
+            compact()                             # nothing in flight: the last step ended with a synchronize
         u, l = addr_for(it, 1)
         sync_all()
         t0 = time.perf_counter()
@@ -599,9 +666,17 @@ def run_ours(args):
     h_pages_b[:] = h_pages
     h_ptr2 = (h_ptr, h_ptr_b)
 
+    paused = [0.0]                                # seconds of compaction inside pipelined()
+
     def pipelined(first_step: int, count: int):
         inflight = None
         for k in range(count):
+            if not step_fits():
+                xch.flush()
+                if inflight is not None:
+                    eng.wait(inflight[0])
+                    inflight = None
+                paused[0] += compact()
             u, l = addr_for(first_step + k, 2)
             # host pages stay untouched until the step's ticket is done (mode 2): the call does not
             # wait for its own copies, so the copy engine never idles between steps
@@ -615,10 +690,11 @@ def run_ours(args):
 
     pipelined(0, W)
     sync_all()
+    paused[0] = 0.0
     t0 = time.perf_counter()
     lens_p = pipelined(W, K)
     sync_all()
-    e2e_s = (time.perf_counter() - t0) / K
+    e2e_s = (time.perf_counter() - t0 - paused[0]) / K
     assert (lens_p == lens_e).all() and (lens_p == lens).all(), "the three passes stored different lengths"
     clocks = sampler.stop()
     if dist:
@@ -631,7 +707,8 @@ def run_ours(args):
     integrity["after_write_behind_e2e_pass"] = {k: final[k] for k in ("entries", "dropped_puts")}
     integrity.update({"dropped_puts": final["dropped_puts"], "local_entries": final["entries"],
                       "expected_local_entries": len(written) * n, "remote_entries": final["remote_entries"],
-                      "distinct_steps_before_addresses_recycle": R, "arena_gib": final["arena_bytes"] / GIB,
+                      "distinct_steps_before_addresses_recycle": R,
+                      "compactions": room["compactions"], "compaction_ms": room["ms"], "arena_gib": final["arena_bytes"] / GIB,
                       "arena_used_gib": final["arena_used"] / GIB})
 
     # ---- parity gate on the measured run's own records (every rank checks its shard) ----
@@ -647,6 +724,8 @@ def run_ours(args):
     parity["what"] = ("records of the last device-resident step read back from the arena (cmb200_read_records) and its reported "
                       "stored lengths vs LZ4_compress_fast(accel 12) + data_prefix of the same pages")
     assert parity["mismatches"] == 0, f"parity gate failed: {parity}"
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, u_last, l_last, lens)
 
     # ---- roofline of the dominant kernel (k_encode) ----
     peak, peak_src = peaks()
@@ -655,17 +734,9 @@ def run_ours(args):
     stored = float(lens[lens > 0].sum())
     alg_bytes_step = n * (CHUNK + 24 + 64) + stored          # SURVEY.md §8d: 65 624 + c per chunk
     achieved = alg_bytes_step * K / (enc_ns * 1e-9) / 1e9 if enc_ns else 0.0
-    traffic, traffic_src = None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "encode_traffic.json")) as f:
-            tj = json.load(f)
-        traffic = tj["dram_bytes_per_launch"] * (n / max(1, enc_launches // K)) / tj["chunks_per_launch"]
-        traffic_src = f"static: {tj['source']} (ncu --set full capture of this launch shape; not re-measured per run)"
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": "k_encode (LZ4 encode + EF128 fingerprint along the parse + record in place + slot publish)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "peak_source": peak_src, "traffic": traffic, "traffic_source": traffic_src,
+                "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes_step / max(1, enc_launches // K),
                 "avg_launch_ms": enc_ns / 1e6 / max(1, enc_launches),
                 "read_form_frac": n * CHUNK * K / (enc_ns * 1e-9) / 1e9 / peak if enc_ns else 0.0,
@@ -745,6 +816,7 @@ def main():
     ap.add_argument("--c4-steps", type=int, default=3)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-configs", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

@@ -1,7 +1,7 @@
-"""edge_fuse_b200 — B200-native cachemap (hash -> LZ4 -> keyed lookup) behind the reference's C API.
+"""edge_fuse_b200 — H100-native cachemap (hash -> LZ4 -> keyed lookup) behind the reference's C API.
 
 The product is the shared library ``libcachemap.so.0.0`` built from ``csrc/`` (CUDA kernels for
-sm_100a + a C host layer exporting the reference's cachemap.h / filemap.h functions).  This Python
+sm_90a + a C host layer exporting the reference's cachemap.h / filemap.h functions).  This Python
 package is only a ctypes face over that C ABI for tests and benchmarks: it never computes
 anything itself and raises if the library or a CUDA device is missing — there is no CPU fallback.
 """

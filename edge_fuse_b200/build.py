@@ -1,4 +1,4 @@
-"""Builds libcachemap.so.0.0 (CUDA kernels + engine + C API) in-tree for sm_100a.
+"""Builds libcachemap.so.0.0 (CUDA kernels + engine + C API) in-tree for sm_90a (H100).
 
 nvcc cross-compiles without a GPU; the resulting shared object is git-ignored but travels to the
 GPU box with the repo snapshot.  Usage: ``python -m edge_fuse_b200.build`` or ``build()``.
@@ -15,8 +15,9 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libcachemap.so.0.0")
 
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper)
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    *GENCODE, "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-Xcompiler", "-Wno-unknown-pragmas",
 ]
 CU_SOURCES = ["kernels.cu", "engine.cu"]
@@ -68,7 +69,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                         *os.environ.get("CMB200_CC_EXTRA", "").split(), "-c",
                         os.path.join(CSRC, src), "-o", obj], check=True)
         objs.append(obj)
-    subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs,
+    subprocess.run([nvcc, "-shared", *GENCODE, "-o", LIB, *objs,
                     "-Xlinker", "-soname=libcachemap.so.0.0", "-lpthread"], check=True)
     if not out:
         link = os.path.join(HERE, "libcachemap.so")

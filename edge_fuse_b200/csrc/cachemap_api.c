@@ -1,5 +1,5 @@
 /*
- * cachemap_api.c — the reference's C API (include/cachemap.h, include/filemap.h) over the B200
+ * cachemap_api.c — the reference's C API (include/cachemap.h, include/filemap.h) over the H100
  * engine.  Host code stays C; everything heavy happens in the engine's kernels.
  *
  * What each reference function became:
@@ -499,7 +499,7 @@ filemap_ring_lookup(struct filemap *m, const cmb200_addr *addr, void *dst)
 
 /* Combining queue of the single-page calls (cachemap_get / filemap_unset from FUSE worker threads).
  *
- * A get's latency is one page's decode on one SM and a B200 decodes 148 pages at a time, so a
+ * A get's latency is one page's decode on one SM and an H100 decodes 132 pages at a time, so a
  * request is launched at once when it can be: whoever finds a free leader slot and nobody else
  * inside a launch takes everything queued (<= COMBINE_MAX) and launches it as ONE fused kernel
  * (cmb200_get_small_begin).  Kernel launches are what limits the rate with many callers (~100 k

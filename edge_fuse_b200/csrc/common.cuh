@@ -1,4 +1,4 @@
-// common.cuh — device helpers shared by the cachemap kernels (sm_100a).
+// common.cuh — device helpers shared by the cachemap kernels (sm_90a).
 //
 // Everything on this path is byte / integer work on 64 KiB chunks that live in HBM; the helpers
 // here are the unaligned-access and warp-collective building blocks the LZ4 and fingerprint

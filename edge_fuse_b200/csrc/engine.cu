@@ -1,4 +1,4 @@
-// engine.cu — host side of the B200 cachemap engine: HBM layout, batch pipelines, C ABI.
+// engine.cu — host side of the H100 cachemap engine: HBM layout, batch pipelines, C ABI.
 //
 // HBM layout per engine (one engine per GPU):
 //   key table   (slots+2) x 64 B          replaces the 32 LMDB environments (filemap.c:54-90)

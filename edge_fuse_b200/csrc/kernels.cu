@@ -1,4 +1,4 @@
-// kernels.cu — sm_100a kernels of the cachemap hot path and their launchers.
+// kernels.cu — sm_90a kernels of the cachemap hot path and their launchers.
 //
 //   k_encode      fingerprint + LZ4 block encode + arena commit, one warp per chunk  (HBM: §4)
 //   k_decode      table record -> LZ4 decode -> page, one warp per request
@@ -348,8 +348,8 @@ __device__ uint32_t commit_direct(const EncodeJob &job, uint32_t i, uint32_t idx
 // by TMA (lz4_encode_ring.cuh); shared memory = tables | rings | mbarriers.
 // FPNA: the fingerprint's streaming loads do not allocate in the L1.
 // Launch bounds = the real launch shapes (2 CTAs x 7 warps, or 1 CTA x 13 warps with the ring), so
-// that the register allocator may use what the SM has (146 / 157 registers per thread) instead of
-// rematerialising loop invariants inside the parse loop.
+// that the register allocator may use what the SM has (up to 146 / 152 registers per thread) instead
+// of rematerialising loop invariants inside the parse loop.
 constexpr int ENC_PLAIN_WARPS = 7, ENC_RING_WARPS = 13;
 template <bool WIDE, int ENC, bool FPNA>
 __global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WARPS * 32, ENC == 1 ? 1 : 2) k_encode(EncodeJob job) {
@@ -441,7 +441,7 @@ int sm_count() {
 		int dev = 0;
 		cudaGetDevice(&dev);
 		cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, dev);
-		if (g_sm_count <= 0) g_sm_count = 148;
+		if (g_sm_count <= 0) g_sm_count = 132;          // H100 SXM
 	}
 	return g_sm_count;
 }

@@ -1,4 +1,4 @@
-// kernels.h — launch interface between the engine (host C++) and the sm_100a kernels.
+// kernels.h — launch interface between the engine (host C++) and the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -36,7 +36,7 @@ __device__ __forceinline__ bool lz4_read_ext(const uint8_t *blk, uint32_t cap, u
 }
 
 // Returns bytes consumed (>0) or a negative error; uniform across the warp.
-// The kernel is issue-bound (64 warps per SM, profiles/r2_decode_blend_summary.txt), so the loop is
+// The kernel is issue-bound (64 warps per SM), so the loop is
 // written for few instructions per sequence: the common sequence — up to 32 literals with at most one
 // length byte, a match of up to 32 bytes that does not overlap itself — is one predicated byte load
 // and store per lane for the literals and one for the match; the token of the NEXT sequence and the

@@ -1,4 +1,4 @@
-// lz4_encode.cuh — byte-exact LZ4 1.8.1 block encoder, one warp per chunk (sm_100a): tables, probe
+// lz4_encode.cuh — byte-exact LZ4 1.8.1 block encoder, one warp per chunk (sm_90a): tables, probe
 // neighbourhoods and the out-of-line paths; the loop is lz4_encode_lean in lz4_encode_ring.cuh.
 //
 // Emits exactly the bytes the reference's filemap_set stores:
@@ -79,7 +79,7 @@ struct Lz4Around { uint32_t before, at, next; };
 #define CMB_LZ4_HINT_CAND 0
 #endif
 // HINT: 0 = ld.global.nc, 1 = + L1::evict_last, 2 = + L1::no_allocate, 3 = .cg, 4 = .cs, 5 = .lu,
-// 6 = .nc + L1::evict_first (tuning, profiles/r1_encode_notes.md)
+// 6 = .nc + L1::evict_first (tuning)
 template <int HINT> __device__ __forceinline__ uint32_t lz4_ldw(const uint32_t *q) {
 	uint32_t v;
 	if (HINT == 1) asm("ld.global.nc.L1::evict_last.b32 %0, [%1];" : "=r"(v) : "l"(q));

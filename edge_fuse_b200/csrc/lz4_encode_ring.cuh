@@ -1,5 +1,5 @@
 // lz4_encode_ring.cuh — the warp-per-chunk LZ4 1.8.1 encoder of lz4_encode.cuh with the page's
-// sliding window staged in shared memory by TMA (sm_100a: cp.async.bulk + mbarrier).
+// sliding window staged in shared memory by TMA (sm_90a: cp.async.bulk + mbarrier).
 //
 // Output bytes: LZ4_compress_fast of the reference (cachemap/lz4.c:532-733 behind filemap.c:124-128); what
 // changes is where the parse frontier reads the page from.  Profile of the plain kernel (round 1,

@@ -1,5 +1,5 @@
 /*
- * cachemap.h — L2 page cache front end, B200 edition.  Drop-in for the reference's
+ * cachemap.h — L2 page cache front end, H100 edition.  Drop-in for the reference's
  * cachemap/cachemap.h:33-47: the same six functions with the same meaning, so edgefs.c's
  * FUSE read()/write() callbacks (edgefs.c:1165,1191,1224) and its cachemap_create call
  * (edgefs.c:2115) compile and link against this library unchanged.

@@ -1,5 +1,5 @@
 /*
- * cachemap_b200.h — C ABI of the B200 cachemap engine (batch extension + kernel-level entries).
+ * cachemap_b200.h — C ABI of the H100 cachemap engine (batch extension + kernel-level entries).
  *
  * The drop-in surface is include/cachemap.h + include/filemap.h (same prototypes as the
  * reference's cachemap/cachemap.h:33-47 and cachemap/filemap.h:19-29).  This header is the layer

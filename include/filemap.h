@@ -1,5 +1,5 @@
 /*
- * filemap.h — keyed page store, B200 edition.  Same seven entry points as the reference's
+ * filemap.h — keyed page store, H100 edition.  Same seven entry points as the reference's
  * cachemap/filemap.h:19-29; behind them the 32 LMDB environments are replaced by one HBM key
  * table + record arena per GPU (include/cachemap_b200.h, DESIGN.md §2).
  *

@@ -101,3 +101,20 @@ def codec_cases():
     for cid in range(8):
         cases.append(("S", 65536, 12, cid))
     return cases
+
+
+# The sweep the oracle is pinned to the reference's LZ4_compress_fast with (tests/golden/ref_blocks.json):
+# (kind, nbytes, accel, seed).
+def reference_sweep_cases():
+    cases = []
+    for rep in range(2):
+        for n in (4096, 16384, 65536, 131072, 65546, 65547, 13, 12, 1, 777):
+            for accel in (12, 1, 0, 5, 200):
+                for kind in "RTZMPAX":
+                    cases.append((kind, n, accel, 10_000 * rep + n + accel + ord(kind)))
+    return cases
+
+
+# The pages the CUDA encoder is compared with the reference's blocks on (tests/golden/ref_blocks.json).
+def gpu_reference_cases():
+    return [("RTZMPAX"[i % 7], bs, 12, 9000 + i) for bs, n in ((65536, 84), (4096, 140)) for i in range(n)]

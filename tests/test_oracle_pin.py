@@ -76,22 +76,24 @@ def test_decoder_rejects_malformed(oracle):
 
 
 def test_oracle_vs_reference_live(oracle):
-    if oracle.ref() is None:
-        pytest.skip("oracle/_ref not built (no /root/reference here); golden vectors cover this")
-    assert oracle.ref().LZ4_versionString() == b"1.8.1"
-    n_cases = 0
-    for rep in range(2):
-        for n in (4096, 16384, 65536, 131072, 65546, 65547, 13, 12, 1, 777):
-            for accel in (12, 1, 0, 5, 200):
-                for kind in "RTZMPAX":
-                    page = datagen.make_page(kind, n, 10_000 * rep + n + accel + ord(kind))
-                    a = oracle.lz4_encode(page, accel)
-                    b = oracle.ref_lz4_encode(page, accel)
-                    assert a == b, (kind, n, accel)
-                    back, used = oracle.ref_lz4_decode(a, n)
-                    assert back == page.tobytes() and used == len(a)
-                    n_cases += 1
-    assert n_cases == 700
+    """The oracle against the reference's LZ4_compress_fast over a sweep of sizes, accelerations and
+    content classes: stored lengths and hashes of the reference's blocks, and the compiled reference
+    itself where oracle/_ref was built."""
+    g = load("ref_blocks.json")
+    assert g["version"] == "1.8.1"
+    cases = datagen.reference_sweep_cases()
+    assert [tuple(r[:4]) for r in g["sweep"]] == cases and len(cases) == 700
+    R = oracle.ref()
+    for kind, n, accel, seed, ref_len, ref_sha in g["sweep"]:
+        page = datagen.make_page(kind, n, seed)
+        a = oracle.lz4_encode(page, accel)
+        assert len(a) == ref_len and sha(a)[:32] == ref_sha, (kind, n, accel)
+        back, used = oracle.lz4_decode(a, n)
+        assert back == page.tobytes() and used == len(a)
+        if R is not None:
+            assert a == oracle.ref_lz4_encode(page, accel), (kind, n, accel)
+            back, used = oracle.ref_lz4_decode(a, n)
+            assert back == page.tobytes() and used == len(a)
 
 
 def test_store_model_matches_reference_trace(oracle):

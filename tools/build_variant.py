@@ -19,6 +19,6 @@ for src in B.CU_SOURCES:
     objs.append(obj)
 objs.append(os.path.join(B.OBJ, "cachemap_api.o"))
 out = os.path.join(out_dir, f"{name}.so")
-subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", out, *objs,
+subprocess.run([nvcc, "-shared", *B.GENCODE, "-o", out, *objs,
                 "-Xlinker", "-soname=libcachemap.so.0.0", "-lpthread"], check=True)
 print(out)

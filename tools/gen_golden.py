@@ -4,7 +4,7 @@
 own uint128.h).  Run in the authoring container only; the fixtures it writes are committed and
 are what pins the oracle (and, on the GPU box, the CUDA path) where /root/reference is absent.
 
-    python tools/gen_golden.py
+    python tools/gen_golden.py [lz4 keys ref_blocks exerciser store]
 """
 from __future__ import annotations
 
@@ -50,6 +50,56 @@ def gen_lz4():
         json.dump({"generator": "tools/gen_golden.py", "reference": "LZ4_compress_fast of cachemap/lz4.c (v1.8.1), "
                    "called as filemap.c:126 does", "cases": out}, f, indent=0)
     print("lz4 cases:", len(out))
+
+
+def gen_ref_blocks():
+    """Length and SHA-256 of the reference's block for every page of the oracle's sweep and of the
+    CUDA comparison, so that both comparisons run without the reference."""
+    def rows(cases):
+        out = []
+        for kind, n, accel, seed in cases:
+            page = datagen.make_page(kind, n, seed)
+            blk = O.ref_lz4_encode(page, accel)
+            back, used = O.ref_lz4_decode(blk, n)
+            assert back == page.tobytes() and used == len(blk)
+            out.append([kind, n, accel, seed, len(blk), sha(blk)[:32]])
+        return out
+    with open(os.path.join(GOLD, "ref_blocks.json"), "w") as f:
+        json.dump({"generator": "tools/gen_golden.py", "reference": "LZ4_compress_fast of cachemap/lz4.c (v1.8.1)",
+                   "version": O.ref().LZ4_versionString().decode(),
+                   "columns": ["kind", "n", "accel", "seed", "len", "sha256 (first 32 hex digits)"],
+                   "sweep": rows(datagen.reference_sweep_cases()),
+                   "gpu": rows(datagen.gpu_reference_cases())}, f, indent=0)
+    print("reference blocks written")
+
+
+def gen_exerciser(seeds=(1, 2, 3), objects=32768, pshift=15):
+    """Per-phase hit counts of tests/c/exerciser.c linked against the reference's library."""
+    import re
+    ref = os.path.join(ROOT, "oracle", "_ref", "libcachemap_ref.so")
+    exe = os.path.join(ROOT, "oracle", "_ref", "exerciser_ref")
+    subprocess.run(["gcc", "-O2", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "c", "exerciser.c"),
+                    "-o", exe, ref, f"-Wl,-rpath,{os.path.dirname(ref)}", "-lpthread"], check=True)
+    runs = []
+    for seed in seeds:
+        for attempt in range(8):                   # the reference can hang at start-up (SURVEY.md §5)
+            with tempfile.TemporaryDirectory(dir="/dev/shm" if os.path.isdir("/dev/shm") else None) as d:
+                try:
+                    out = subprocess.run([exe, d, str(objects), str(pshift), str(seed)], capture_output=True,
+                                         text=True, timeout=60).stdout
+                    break
+                except subprocess.TimeoutExpired:
+                    continue
+        else:
+            raise RuntimeError("the reference exerciser hung at start-up in every attempt")
+        phases = {m.group(1): [int(m.group(2)), int(m.group(3))] for m in re.finditer(r"phase (\w+) hits (\d+) of (\d+)", out)}
+        entries = [int(x) for x in re.findall(r"entries_after_\w+ (\d+)", out)]
+        assert len(phases) == 5, out
+        runs.append({"seed": seed, "phases": phases, "entries": entries})
+    with open(os.path.join(GOLD, "ref_exerciser.json"), "w") as f:
+        json.dump({"generator": "tools/gen_golden.py: tests/c/exerciser.c linked against libcachemap_ref.so (LMDB on tmpfs)",
+                   "objects": objects, "pshift": pshift, "runs": runs}, f, indent=1)
+    print("exerciser runs:", runs)
 
 
 def gen_keys():
@@ -136,6 +186,7 @@ def gen_store():
 if __name__ == "__main__":
     assert O.ref() is not None, "oracle/_ref/libcachemap_ref.so missing: run make -C oracle"
     os.makedirs(GOLD, exist_ok=True)
-    gen_lz4()
-    gen_keys()
-    gen_store()
+    steps = {"lz4": gen_lz4, "keys": gen_keys, "ref_blocks": gen_ref_blocks, "exerciser": gen_exerciser,
+             "store": gen_store}                   # gen_store ends the process: keep it last
+    for name in sys.argv[1:] or steps:
+        steps[name]()

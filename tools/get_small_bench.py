@@ -25,7 +25,7 @@ for k, cls in enumerate("RTZM"):
     out, st = eng.get_small(u, l)
     assert (st == E.HIT).all() and (out == pages).all()
     row = {}
-    for m in (1, 8, 32, 148, 256):
+    for m in (1, 8, 32, 132, 256):
         for name, fn in (("small", lambda: eng.get_small(u[:m], l[:m], out=hp)), ("batch", lambda: eng.get(u[:m], l[:m], out=hp))):
             fn(); fn()
             reps = 20

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """A small pass over every hot kernel (ring encoder incl. long matches and ragged sizes, k_decode,
 k_get_small with its decode pipeline, eviction sampling, compaction + table rebuild) meant to be
-run under `compute-sanitizer --tool memcheck` (tools: profiles/r2_memcheck.log)."""
+run under `compute-sanitizer --tool memcheck`."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
