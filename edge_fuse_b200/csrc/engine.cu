@@ -103,6 +103,7 @@ struct cmb200_engine {
 	int32_t *d_lens = nullptr, *d_status = nullptr;
 	uint64_t *d_fps = nullptr, *d_recoff = nullptr;
 	unsigned int *d_work = nullptr;
+	uint32_t *d_order = nullptr;         // the encoder's longest-first chunk lists (encode_order_words(max_batch))
 	uint32_t *d_import_slot = nullptr;   // slot scratch of cmb200_import_records_dev
 	size_t import_slot_cap = 0;
 	// page-locked staging for the small per-chunk arrays, so that no copy ever blocks the host
@@ -178,7 +179,7 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	}
 	cudaFree(e->d_recoff_out);
 	for (int r = 0; r < GET_MAX_PEERS; r++) if (e->peer_base[r]) cudaIpcCloseMemHandle((void *)e->peer_base[r]);
-	cudaFree(e->d_lens); cudaFree(e->d_status); cudaFree(e->d_fps); cudaFree(e->d_recoff); cudaFree(e->d_work); cudaFree(e->d_import_slot);
+	cudaFree(e->d_lens); cudaFree(e->d_status); cudaFree(e->d_fps); cudaFree(e->d_recoff); cudaFree(e->d_work); cudaFree(e->d_order); cudaFree(e->d_import_slot);
 	for (int i = 0; i < 2; i++) {
 		if (e->landed[i]) cudaEventDestroy(e->landed[i]);
 		if (e->consumed[i]) cudaEventDestroy(e->consumed[i]);
@@ -293,6 +294,7 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 		ENG_CHECK(cudaMalloc(&e->d_fps, B * 16));
 		ENG_CHECK(cudaMalloc(&e->d_recoff, B * 8));
 		ENG_CHECK(cudaMalloc(&e->d_work, 64));
+		ENG_CHECK(cudaMalloc(&e->d_order, encode_order_words((uint32_t)B) * 4));
 		ENG_CHECK(cudaMallocHost(&e->h_meta, cmb200_engine::META_CAP * 33));
 		for (auto &ln : e->lane) {
 			ENG_CHECK(cudaMallocHost(&ln.h_status, cmb200_engine::GET_SMALL_MAX * 4));
@@ -468,6 +470,7 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		job.rec_out = e->d_recoff_out + at;
 		job.fps = (e->flags & CMB200_FINGERPRINT) ? e->d_fps : nullptr;
 		job.work = e->d_work;
+		job.order = e->d_order;
 		job.slot_idx = e->d_slot;
 		job.addr = d_addr + 2 * at;
 		job.ts = ts ? d_ts + at : nullptr;
@@ -483,12 +486,13 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		}
 		CMB_CHECK(cudaEventRecord(ev0, e->st));
 		if (trace && nb < 16) cudaEventRecord(tr[2][nb], e->st);
-		if (launch_encode(job, e->st)) return -1;
+		const int encode_kernels = launch_encode(job, e->st);
+		if (encode_kernels < 0) return -1;
 		if (trace && nb < 16) cudaEventRecord(tr[3][nb], e->st);
 		CMB_CHECK(cudaEventRecord(ev1, e->st));
 		if (!pages_on_dev) CMB_CHECK(cudaEventRecord(e->consumed[buf], e->st));
 		e->seq += (unsigned long long)m * e->seq_stride;
-		e->stats.kernel_launches += 2;
+		e->stats.kernel_launches += 1 + encode_kernels;
 	}
 	e->stats.put_chunks += n;
 	if (recs && recs->out) {
@@ -1218,8 +1222,9 @@ extern "C" int cmb200_lz4_encode_batch(int device, const void *pages_host, size_
 	size_t bound = (size_t)nbytes + nbytes / 255 + 16;
 	size_t sstride = (bound + 15) & ~(size_t)15;
 	if (out_stride < bound) { set_error_msg("encode_batch: out_stride below LZ4_compressBound"); return -1; }
-	DevBuf d_in, d_stage, d_lens, d_fps, d_work;
-	if (d_in.alloc(n * stride) || d_stage.alloc(n * sstride) || d_lens.alloc(n * 4) || d_fps.alloc(n * 16) || d_work.alloc(64)) return -1;
+	DevBuf d_in, d_stage, d_lens, d_fps, d_work, d_order;
+	if (d_in.alloc(n * stride) || d_stage.alloc(n * sstride) || d_lens.alloc(n * 4) || d_fps.alloc(n * 16) || d_work.alloc(64) ||
+	    d_order.alloc(encode_order_words((uint32_t)n) * 4)) return -1;
 	CMB_CHECK(cudaMemcpy(d_in.p, pages_host, n * stride, cudaMemcpyHostToDevice));
 	EncodeJob job{};
 	job.pages = d_in.as<uint8_t>(); job.page_stride = stride; job.nbytes = nbytes; job.n = (uint32_t)n;
@@ -1229,7 +1234,8 @@ extern "C" int cmb200_lz4_encode_batch(int device, const void *pages_host, size_
 	job.lens = d_lens.as<int32_t>();
 	job.fps = fp_out ? d_fps.as<uint64_t>() : nullptr;
 	job.work = d_work.as<unsigned int>();
-	if (launch_encode(job, 0)) return -1;
+	job.order = d_order.as<uint32_t>();
+	if (launch_encode(job, 0) < 0) return -1;
 	CMB_CHECK(cudaMemcpy(lens_out, d_lens.p, n * 4, cudaMemcpyDeviceToHost));
 	if (fp_out) CMB_CHECK(cudaMemcpy(fp_out, d_fps.p, n * 16, cudaMemcpyDeviceToHost));
 	CMB_CHECK(cudaMemcpy2D(blocks_out_host, out_stride, d_stage.p, sstride, bound < out_stride ? bound : out_stride, n,

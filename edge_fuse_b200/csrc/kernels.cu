@@ -344,6 +344,115 @@ __device__ uint32_t commit_direct(const EncodeJob &job, uint32_t i, uint32_t idx
 	return need;
 }
 
+// ---- longest-first handout ---------------------------------------------------------------------
+// A launch ends when its last chunk does, and chunk costs differ by about 10x (DESIGN.md §4): with
+// chunks taken in index order, the warps that run dry wait for whoever drew a costly chunk last.
+// k_cost rates each chunk before the encode and puts it in one of ENC_BUCKETS lists; k_encode's
+// tickets then walk the lists from the costliest down, so the launch ends on cheap chunks.
+//
+// The rate comes from a 1 KiB sample, 8 windows of 128 bytes spread over the page (lane L holds
+// bytes [32 (L & 3), +32) of window L >> 2), scanned like the encoder scans the page: a 4-byte
+// sequence that occurs elsewhere in the sample is a match, and a match whose previous byte also
+// matches at the same distance continues a sequence instead of starting one.  Estimated LZ4 loop
+// iterations = sequence starts + match-less positions / (COST_LIT x accel).  Zero pages and repeats
+// rate cheap (few starts), incompressible pages too (the probe step skips through them).  A page
+// whose sequences are all further apart than the sample sees (source text) rates low; that costs
+// balance, never a result.  Only page bytes and slot liveness go into it; a chunk that a later
+// chunk of the batch rewrites is not encoded at all and goes last.
+// COST_LIT and COST_FULL: least-squares fit of the per-chunk durations of tools/encode_timeline.py
+// on an H100 80GB HBM3 (400 W), bench stream and tree files (DESIGN.md §4).
+constexpr uint32_t COST_WARPS = 8, COST_TAB = 2048, COST_POS = 125;   // positions rated per window
+constexpr float COST_LIT = 1.0f / 14.0f;       // a match-less position weighs 1 / (14 accel) sequence starts
+constexpr float COST_FULL = 160.0f;            // estimate at and above which a chunk goes in the top bucket
+#ifdef CMB_ENC_TIMELINE        /* diagnostic builds only (tools/encode_timeline.py) */
+__device__ unsigned long long *g_enc_timeline;   // per chunk {warp slot, start ns, end ns, estimate}
+__device__ __forceinline__ unsigned long long enc_clock() {
+	unsigned long long t;
+	asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+	return t;
+}
+#endif
+__global__ void __launch_bounds__(COST_WARPS * 32, 4) k_cost(EncodeJob job) {
+	__shared__ __align__(16) uint32_t smp[COST_WARPS][256 + 4];           // the sample (+ the word a gram may touch past it)
+	// gram hash -> a sample position with that hash; whatever an entry holds (another gram, a position
+	// of the previous chunk) is checked against the sample itself, so the table is never cleared
+	__shared__ uint16_t tab[COST_WARPS][COST_TAB];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	uint32_t *s = smp[warp];
+	uint16_t *h = tab[warp];
+	const uint8_t *sb = reinterpret_cast<const uint8_t *>(s);
+	const uint32_t o0 = ((uint32_t)lane & 3u) * 32u;                      // offset of this lane's bytes in its window
+	const uint32_t win_stride = (job.nbytes / 8u) & ~15u;
+	for (uint32_t i = blockIdx.x * COST_WARPS + warp; i < job.n; i += gridDim.x * COST_WARPS) {
+		// the sample is loaded before liveness is known: the two round trips overlap
+		const uint4 *src = reinterpret_cast<const uint4 *>(job.pages + (size_t)i * job.page_stride + (lane >> 2) * win_stride + o0);
+		const uint4 a = __ldg(src), c = __ldg(src + 1);
+		bool live = true;
+		if (job.slot_idx) {
+			const uint32_t idx = job.slot_idx[i];
+			live = idx != 0xffffffffu && job.table.slots[idx].seq == job.seq0 + job.seq_stride * i;
+		}
+		uint32_t bucket = 0;
+		[[maybe_unused]] uint32_t est = 0;                                 // {starts, match-less positions}, timeline builds report it
+		if (live) {
+			const uint32_t w[9] = {a.x, a.y, a.z, a.w, c.x, c.y, c.z, c.w, __shfl_down_sync(CMB_FULL, a.x, 1)};
+			__syncwarp();                                             // the previous chunk's reads of s and h are done
+			reinterpret_cast<uint4 *>(s)[2 * lane] = a;
+			reinterpret_cast<uint4 *>(s)[2 * lane + 1] = c;
+			// every position enters the table (one writer per entry survives), then every position looks
+			// its gram up: a gram seen r times finds r - 1 partners, as a serial scan would
+#pragma unroll
+			for (uint32_t k = 0; k < 32; k++) {
+				if (o0 + k >= COST_POS) break;
+				const uint32_t g = __funnelshift_r(w[k >> 2], w[(k >> 2) + 1], (k & 3u) * 8u);
+				h[(g * 2654435761u) >> 21] = (uint16_t)((uint32_t)lane * 32u + k);
+			}
+			__syncwarp();
+			uint32_t starts = 0, lits = 0;
+#pragma unroll
+			for (uint32_t k = 0; k < 32; k++) {
+				if (o0 + k >= COST_POS) break;
+				const uint32_t p = (uint32_t)lane * 32u + k;
+				const uint32_t g = __funnelshift_r(w[k >> 2], w[(k >> 2) + 1], (k & 3u) * 8u);
+				const uint32_t q = h[(g * 2654435761u) >> 21] & 1023u;
+				const bool m = q != p && (q & 127u) < COST_POS && __funnelshift_r(s[q >> 2], s[(q >> 2) + 1], (q & 3u) * 8u) == g;
+				const bool cont = m && o0 + k > 0u && (q & 127u) > 0u && sb[p - 1] == sb[q - 1];
+				starts += m && !cont;
+				lits += !m;
+			}
+#pragma unroll
+			for (int d = 16; d > 0; d >>= 1) {
+				starts += __shfl_xor_sync(CMB_FULL, starts, d);
+				lits += __shfl_xor_sync(CMB_FULL, lits, d);
+			}
+			const float cost = (float)starts + COST_LIT * (float)lits / (float)job.accel;
+			bucket = min(ENC_BUCKETS - 1u, (uint32_t)(cost * ((float)ENC_BUCKETS / COST_FULL)));
+			est = starts << 16 | lits;
+		}
+		if (lane == 0) {
+			const uint32_t pos = atomicAdd(&job.work[1 + bucket], 1u);
+			job.order[(size_t)bucket * job.n + pos] = i;
+#ifdef CMB_ENC_TIMELINE
+			if (g_enc_timeline) g_enc_timeline[4 * (size_t)i + 3] = (unsigned long long)bucket << 32 | est;
+#endif
+		}
+	}
+}
+
+// Ticket t of an ordered launch -> chunk: the buckets' sizes in descending cost order, prefix-summed
+// across lanes 0..ENC_BUCKETS-1, tell which list t falls in (once per chunk, out of the parse loop).
+__device__ __noinline__ uint32_t enc_ticket_chunk(const unsigned int *work, const uint32_t *order, uint32_t n, uint32_t t, int lane) {
+	uint32_t cum = lane < (int)ENC_BUCKETS ? work[ENC_BUCKETS - lane] : 0u;   // lane k: bucket ENC_BUCKETS-1-k
+#pragma unroll
+	for (int d = 1; d < (int)ENC_BUCKETS; d <<= 1) {
+		const uint32_t v = __shfl_up_sync(CMB_FULL, cum, d);
+		if (lane >= d) cum += v;
+	}
+	const int k = __ffs(__ballot_sync(CMB_FULL, lane < (int)ENC_BUCKETS && t < cum)) - 1;   // t < n = the sum
+	const uint32_t before = __shfl_sync(CMB_FULL, cum, (k + 31) & 31);
+	return order[(size_t)(ENC_BUCKETS - 1 - k) * n + (t - (k ? before : 0u))];
+}
+
 // ENC 0: page read through the L1.  ENC 1: parse frontier staged in a per-warp shared-memory ring
 // by TMA (lz4_encode_ring.cuh); shared memory = tables | rings | mbarriers.
 // FPNA: the fingerprint's streaming loads do not allocate in the L1.
@@ -367,10 +476,22 @@ __global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WAR
 	const uint32_t worst = (uint32_t)((24u + job.stage_stride + 15u) & ~15ull);
 	unsigned long long seg_cur = 0, seg_end = 0;                         // lane 0's copy is the truth
 	if (direct && lane == 0) { seg_cur = job.arena.seg[2 * gw]; seg_end = job.arena.seg[2 * gw + 1]; }
+#ifdef CMB_ENC_TIMELINE
+	uint32_t prev = ~0u;
+#endif
 	for (;;) {
 		uint32_t i = 0;
 		if (lane == 0) i = atomicAdd(job.work, 1u);
 		i = __shfl_sync(CMB_FULL, i, 0);
+		if (i < job.n && job.order) i = enc_ticket_chunk(job.work, job.order, job.n, i, lane);
+#ifdef CMB_ENC_TIMELINE
+		if (lane == 0 && g_enc_timeline) {               // a chunk ends where the warp draws its next ticket
+			const unsigned long long t = enc_clock();
+			if (prev != ~0u) g_enc_timeline[4 * (size_t)prev + 2] = t;
+			if (i < job.n) { g_enc_timeline[4 * (size_t)i] = gw; g_enc_timeline[4 * (size_t)i + 1] = t; }
+			prev = i;
+		}
+#endif
 		if (i >= job.n) break;
 		const bool store = job.slot_idx != nullptr;
 		uint32_t idx = 0;
@@ -467,11 +588,14 @@ static int launch_encode_kernel(K kern, const EncodeJob &job, int warps, int cta
 	return 0;
 }
 
+static int enc_plain_warps() { static const int w = env_int("CMB200_ENC_WARPS", ENC_PLAIN_WARPS, 1, ENC_PLAIN_WARPS); return w; }
+static int enc_plain_ctas() { static const int c = env_int("CMB200_ENC_CTAS_PER_SM", 2, 1, 2); return c; }
+static int enc_ring_warps() { static const int w = env_int("CMB200_RING_WARPS", ENC_RING_WARPS, 1, ENC_RING_WARPS); return w; }
+
 // Plain organisation: residency is bounded by shared memory, one 16 KiB position table per chunk,
 // 14 of them in the 227 KiB of an SM (2 CTAs x 7 warps); chunks handed out dynamically.
 static int launch_encode_warps(const EncodeJob &job, cudaStream_t st, bool fpna) {
-	static int warps = env_int("CMB200_ENC_WARPS", ENC_PLAIN_WARPS, 1, ENC_PLAIN_WARPS);
-	static int ctas = env_int("CMB200_ENC_CTAS_PER_SM", 2, 1, 2);
+	const int warps = enc_plain_warps(), ctas = enc_plain_ctas();
 	const size_t smem = (size_t)warps * LZ4_TABLE_BYTES;
 	const bool wide = job.nbytes >= LZ4_NARROW_LIMIT;
 	if (wide) return fpna ? launch_encode_kernel(k_encode<true, 0, true>, job, warps, ctas, smem, st)
@@ -483,7 +607,7 @@ static int launch_encode_warps(const EncodeJob &job, cudaStream_t st, bool fpna)
 // Ring organisation (lz4_encode_ring.cuh): table + 1 KiB TMA ring + mbarriers per warp, 13 chunks
 // per SM in one CTA.
 static int launch_encode_ring(const EncodeJob &job, cudaStream_t st, bool fpna) {
-	static int warps = env_int("CMB200_RING_WARPS", ENC_RING_WARPS, 1, ENC_RING_WARPS);
+	const int warps = enc_ring_warps();
 	const size_t smem = (size_t)warps * RING_WARP_SMEM;
 	const bool wide = job.nbytes >= LZ4_NARROW_LIMIT;
 	if (wide) return fpna ? launch_encode_kernel(k_encode<true, 1, true>, job, warps, 1, smem, st)
@@ -502,13 +626,27 @@ int launch_encode(const EncodeJob &job_in, cudaStream_t st) {
 	static int mode = env_int("CMB200_ENC_MODE", 2, 0, 2);
 	static int fpna = env_int("CMB200_FP_NOALLOC", 1, 0, 1);
 	EncodeJob job = job_in;
-	CMB_CHECK(cudaMemsetAsync(job.work, 0, sizeof(unsigned int), st));
+	const bool aligned = (reinterpret_cast<uintptr_t>(job.pages) & 15u) == 0 && (job.page_stride & 15u) == 0;
 	// the ring holds what 30 probes at accel <= 12 reach and TMA wants 16-byte aligned pages
-	const bool ring_ok = job.accel >= 1 && job.accel <= RING_MAX_ACCEL && job.nbytes < (1u << 24) &&
-	    (reinterpret_cast<uintptr_t>(job.pages) & 15u) == 0 && (job.page_stride & 15u) == 0;
-	if (mode == 2 && ring_ok) return launch_encode_ring(job, st, fpna != 0);
-	return launch_encode_warps(job, st, fpna != 0);
+	const bool ring = mode == 2 && job.accel >= 1 && job.accel <= RING_MAX_ACCEL && job.nbytes < (1u << 24) && aligned;
+	// Longest-first handout when chunks wait for a warp at all (more chunks than resident warps) and
+	// are encoded (a raw store costs the same per chunk); the sample wants >= 1 KiB aligned pages.
+	const uint32_t resident = (uint32_t)sm_count() * (ring ? enc_ring_warps() : enc_plain_ctas() * enc_plain_warps());
+	if (job.n <= resident || job.accel == 0 || job.nbytes < 1024u || !aligned) job.order = nullptr;
+	CMB_CHECK(cudaMemsetAsync(job.work, 0, (job.order ? 1 + ENC_BUCKETS : 1) * sizeof(unsigned int), st));
+	if (job.order) {
+		k_cost<<<(job.n + COST_WARPS - 1) / COST_WARPS, COST_WARPS * 32, 0, st>>>(job);   // a warp per chunk
+		CMB_CHECK(cudaGetLastError());
+	}
+	if ((ring ? launch_encode_ring(job, st, fpna != 0) : launch_encode_warps(job, st, fpna != 0)) != 0) return -1;
+	return job.order ? 2 : 1;
 }
+
+#ifdef CMB_ENC_TIMELINE
+extern "C" int cmb200_enc_timeline(void *buf) {       // n x 4 u64, see g_enc_timeline; null = off
+	return cudaMemcpyToSymbol(g_enc_timeline, &buf, sizeof(buf)) == cudaSuccess ? 0 : -1;
+}
+#endif
 
 // ------------------------------------------------------------------------------------------
 // decode

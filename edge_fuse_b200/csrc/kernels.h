@@ -81,7 +81,8 @@ struct EncodeJob {
 	int32_t *lens;           // out: block length, -1 = chunk skipped (superseded inside the batch)
 	unsigned long long *rec_out; // out, optional: arena offset of the stored record per chunk (~0 = dropped)
 	uint64_t *fps;           // out, optional: 2 x u64 per chunk {hi, lo}
-	unsigned int *work;      // dynamic work counter (zeroed by the launcher)
+	unsigned int *work;      // 1 + ENC_BUCKETS words: the ticket counter, then the bucket sizes (zeroed by the launcher)
+	uint32_t *order;         // scratch of encode_order_words(n): chunk lists of the longest-first handout (launch_encode)
 	// store mode (all null/0 for codec-only use)
 	const uint32_t *slot_idx; // per chunk, from the upsert kernel; 0xffffffff = invalid address
 	const unsigned long long *addr; // per chunk {u,l}
@@ -92,7 +93,12 @@ struct EncodeJob {
 	ArenaView arena;
 };
 
-int launch_encode(const EncodeJob &job, cudaStream_t st);
+// Longest-first handout (DESIGN.md §4): when a launch has more chunks than resident encoder warps,
+// k_cost rates every chunk from a sample of its bytes and appends it to the list of its cost bucket;
+// the tickets of k_encode then walk the buckets from the costliest down.
+constexpr uint32_t ENC_BUCKETS = 8;
+inline size_t encode_order_words(uint32_t n) { return (size_t)ENC_BUCKETS * n; }
+int launch_encode(const EncodeJob &job, cudaStream_t st);   // -> kernels launched (0..2), < 0 on error
 
 struct DecodeJob {
 	uint32_t n;
