@@ -39,16 +39,6 @@ def _newer(src_paths, target) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """CMB200_NVCC_EXTRA (e.g. "-DCMB_OUT_HINT=1") adds nvcc flags (CMB200_CC_EXTRA: flags for the C layer) and CMB200_BUILD_OUT names the
-    output file: a differently tuned build of the same library next to the default one, loaded by
-    setting CMB200_LIB (tuning experiments; the default build takes neither)."""
-    global LIB, OBJ
-    extra = os.environ.get("CMB200_NVCC_EXTRA", "").split()
-    out = os.environ.get("CMB200_BUILD_OUT")
-    if out:
-        LIB = os.path.join(HERE, out)
-        OBJ = os.path.join(HERE, "build_" + out.replace(".", "_"))
-        force = True
     os.makedirs(OBJ, exist_ok=True)
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)]
     deps += [os.path.join(HERE, "..", "include", f) for f in os.listdir(os.path.join(HERE, "..", "include"))]
@@ -58,24 +48,22 @@ def build(force: bool = False, verbose: bool = False) -> str:
     objs = []
     for src in CU_SOURCES:
         obj = os.path.join(OBJ, src.replace(".cu", ".o"))
-        cmd = [nvcc, *NVCC_FLAGS, *extra, "-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         subprocess.run(cmd, check=True)
         objs.append(obj)
     for src in C_SOURCES:
         obj = os.path.join(OBJ, src.replace(".c", ".o"))
-        subprocess.run(["gcc", "-std=gnu11", "-O2", "-fPIC", "-Wall", "-Wextra", "-pthread",
-                        *os.environ.get("CMB200_CC_EXTRA", "").split(), "-c",
+        subprocess.run(["gcc", "-std=gnu11", "-O2", "-fPIC", "-Wall", "-Wextra", "-pthread", "-c",
                         os.path.join(CSRC, src), "-o", obj], check=True)
         objs.append(obj)
     subprocess.run([nvcc, "-shared", *GENCODE, "-o", LIB, *objs,
                     "-Xlinker", "-soname=libcachemap.so.0.0", "-lpthread"], check=True)
-    if not out:
-        link = os.path.join(HERE, "libcachemap.so")
-        if os.path.lexists(link):
-            os.remove(link)
-        os.symlink("libcachemap.so.0.0", link)
+    link = os.path.join(HERE, "libcachemap.so")
+    if os.path.lexists(link):
+        os.remove(link)
+    os.symlink("libcachemap.so.0.0", link)
     return LIB
 
 

@@ -35,13 +35,9 @@
 #include "../../include/cachemap_b200.h"
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
-#ifndef LEADERS
-#define LEADERS 32
-#endif                          /* batches of gets that may be in flight at once, each on its own engine lane
-                                 * (<= the engine's CMB_GET_LANES); see the combining queue below */
-#ifndef GET_CALLERS
+#define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
+                                 * (<= the engine's GET_LANES); see the combining queue below */
 #define GET_CALLERS 32          /* callers inside the combining queue at once; the rest sleep at its door */
-#endif
 #define FLUSH_MAX 4096          /* pages the flusher hands over per GPU batch */
 #define PNUM_SHIFT 44           /* cachemap.c:155 */
 

@@ -29,19 +29,8 @@ __device__ __forceinline__ uint32_t ldg32(const uint8_t *p) {
 }
 __device__ __forceinline__ uint32_t ldg8(const uint8_t *p) { return __ldg(p); }
 
-// Byte store of encoder output.  CMB_OUT_HINT selects the cache policy of the bytes the encoder
-// writes into the arena (written once, never read by the kernel): 0 = default, 1 = st.global.cs
-// (streaming: first to leave the L2, which the parse wants for the pages it comes back to).
-#ifndef CMB_OUT_HINT
-#define CMB_OUT_HINT 0
-#endif
-__device__ __forceinline__ void st_out8(uint8_t *p, uint32_t v) {
-#if CMB_OUT_HINT == 1
-	asm volatile("st.global.cs.u8 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-#else
-	*p = (uint8_t)v;
-#endif
-}
+// Byte store of encoder output.
+__device__ __forceinline__ void st_out8(uint8_t *p, uint32_t v) { *p = (uint8_t)v; }
 
 // Little-endian 32-bit read at an arbitrary byte offset `pos` of a 4-byte-aligned base.
 // `lim4` is the chunk length rounded up to 4: the second word is only touched when it lies

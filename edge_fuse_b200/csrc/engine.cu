@@ -49,10 +49,7 @@ struct cmb200_engine {
 	// callers of cmb200_get_small): each takes one LANE — a stream plus page-locked request / status
 	// words — and the open side of get_gate; what moves records or peer mappings (compaction, peers,
 	// destroy) closes get_gate.
-#ifndef CMB_GET_LANES
-#define CMB_GET_LANES 32
-#endif
-	static constexpr int GET_LANES = CMB_GET_LANES;
+	static constexpr int GET_LANES = 32;
 	struct GetLane { std::atomic<int> busy{0}; cudaStream_t st = nullptr; int32_t *h_status = nullptr; cmb200_addr *h_addr = nullptr; };
 	GetLane lane[GET_LANES];
 	// A small get may be begun by one thread and ended by another (cmb200_get_small_begin / _end), so
@@ -209,21 +206,15 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 	e->accel = cfg->accel < 0 ? 1 : (cfg->accel > (1 << 20) ? (1 << 20) : cfg->accel);   // lz4.c:740
 	e->capacity = cfg->capacity;
 	e->max_batch = cfg->max_batch ? cfg->max_batch : 4096;
-	{
-		// host pages are pipelined in smaller steps than a resident batch is launched in: the first
-		// copy of a call cannot overlap anything, while a launch wants many chunks per warp
-		const char *hb = getenv("CMB200_HOST_BATCH");
-		uint32_t v = hb ? (uint32_t)strtoul(hb, nullptr, 0) : 4096u;
-		e->host_batch = v && v < e->max_batch ? v : e->max_batch;
-	}
+	// host pages are pipelined in smaller steps than a resident batch is launched in: the first
+	// copy of a call cannot overlap anything, while a launch wants many chunks per warp
+	e->host_batch = e->max_batch < 4096u ? e->max_batch : 4096u;
 	e->flags = cfg->flags;
 	const uint64_t B = e->max_batch;
 	{
 		uint64_t slots = cfg->table_slots ? next_pow2(cfg->table_slots) : next_pow2(4 * (cfg->capacity ? cfg->capacity : 1024));
 		if (slots < 1024) slots = 1024;
-		const char *cap_env = getenv("CMB200_MAX_TABLE_SLOTS");
-		uint64_t max_slots = cap_env ? next_pow2(strtoull(cap_env, nullptr, 0)) : (1ull << 27);
-		if (slots > max_slots) slots = max_slots;
+		if (slots > (1ull << 27)) slots = 1ull << 27;
 		e->table.cap = slots;
 		ENG_CHECK(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
 		ENG_CHECK(cudaStreamCreateWithFlags(&e->copy, cudaStreamNonBlocking));
@@ -437,9 +428,6 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 	}
 	size_t nb = 0;
 	int last_buf = 0;
-	static const bool trace = getenv("CMB200_TRACE") != nullptr;
-	cudaEvent_t tr[4][16];
-	if (trace) for (int i = 0; i < 4; i++) for (int j = 0; j < 16; j++) cudaEventCreate(&tr[i][j]);
 	for (size_t at = 0; at < n; at += B, nb++) {
 		// (splitting the last step into smaller ones to shorten the un-overlapped tail was tried:
 		// launches below ~4096 chunks run below PCIe rate, so the tail got longer, not shorter)
@@ -453,10 +441,8 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 			e->ring_pos++;
 			last_buf = buf;
 			CMB_CHECK(cudaStreamWaitEvent(e->copy, e->consumed[buf], 0));
-			if (trace && nb < 16) cudaEventRecord(tr[0][nb], e->copy);
 			CMB_CHECK(cudaMemcpyAsync(e->d_pages[buf], pages + at * e->bsize, (size_t)m * e->bsize,
 			    cudaMemcpyHostToDevice, e->copy));
-			if (trace && nb < 16) cudaEventRecord(tr[1][nb], e->copy);
 			CMB_CHECK(cudaEventRecord(e->landed[buf], e->copy));
 			CMB_CHECK(cudaStreamWaitEvent(e->st, e->landed[buf], 0));
 			d_in = e->d_pages[buf];
@@ -485,10 +471,8 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 			ev0 = e->t0[nb % e->RING]; ev1 = e->t1[nb % e->RING];
 		}
 		CMB_CHECK(cudaEventRecord(ev0, e->st));
-		if (trace && nb < 16) cudaEventRecord(tr[2][nb], e->st);
 		const int encode_kernels = launch_encode(job, e->st);
 		if (encode_kernels < 0) return -1;
-		if (trace && nb < 16) cudaEventRecord(tr[3][nb], e->st);
 		CMB_CHECK(cudaEventRecord(ev1, e->st));
 		if (!pages_on_dev) CMB_CHECK(cudaEventRecord(e->consumed[buf], e->st));
 		e->seq += (unsigned long long)m * e->seq_stride;
@@ -512,21 +496,22 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 	}
 	if (lens_out) CMB_CHECK(cudaMemcpyAsync(h_lens, e->d_lens, n * 4, cudaMemcpyDeviceToHost, e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
-	if (trace) {
-		for (size_t k = 0; k < nb && k < 16 && !pages_on_dev; k++) {
-			float a = 0, b = 0, c = 0, d = 0;
-			cudaEventElapsedTime(&a, tr[0][0], tr[0][k]); cudaEventElapsedTime(&b, tr[0][0], tr[1][k]);
-			cudaEventElapsedTime(&c, tr[0][0], tr[2][k]); cudaEventElapsedTime(&d, tr[0][0], tr[3][k]);
-			fprintf(stderr, "sub-batch %zu: copy %.2f-%.2f ms  encode %.2f-%.2f ms\n", k, a, b, c, d);
-		}
-		for (int i = 0; i < 4; i++) for (int j = 0; j < 16; j++) cudaEventDestroy(tr[i][j]);
-	}
 	if (lens_out) memcpy(lens_out, h_lens, n * 4);
 	for (size_t k = 0; k < nb && k < (size_t)e->RING; k++) {
 		float ms = 0;
 		CMB_CHECK(cudaEventElapsedTime(&ms, e->t0[k], e->t1[k]));
 		e->stats.encode_kernel_ns += (uint64_t)(ms * 1e6);
 		e->stats.encode_kernel_launches++;
+	}
+	return 0;
+}
+
+// The encoder reads device pages with 16-byte loads (TMA ring, fingerprint stripes): a device page
+// pointer is checked before anything is queued.  Page strides (1 << pshift, pshift >= 6) are multiples of 64.
+static int check_dev_pages(const void *pages, const char *what) {
+	if (reinterpret_cast<uintptr_t>(pages) & 15u) {
+		snprintf(g_err, sizeof(g_err), "%s: device pages must be 16-byte aligned", what);
+		return -1;
 	}
 	return 0;
 }
@@ -560,6 +545,7 @@ extern "C" int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *ad
     const void *pages, int pages_on_dev, const uint64_t *ts, uint32_t rank, void *records_dev_out,
     int32_t *lens_out, uint64_t *ticket) {
 	if (n > cmb200_engine::META_CAP) { set_error_msg("cmb200_put_step: more than 262144 chunks in one step"); return -1; }
+	if (pages_on_dev == 1 && check_dev_pages(pages, "cmb200_put_step")) return -1;
 	std::lock_guard<std::mutex> g(e->mu);
 	CMB_CHECK(cudaSetDevice(e->device));
 	uint64_t t = e->tickets;
@@ -602,6 +588,7 @@ extern "C" int cmb200_wait(cmb200_engine *e, uint64_t ticket) {
 }
 extern "C" int cmb200_put_batch_dev(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     const void *pages_dev, const uint64_t *ts, int32_t *lens_out) {
+	if (check_dev_pages(pages_dev, "cmb200_put_batch_dev")) return -1;
 	return put_impl(e, n, addr, valid, (const uint8_t *)pages_dev, true, ts, lens_out, nullptr);
 }
 

@@ -26,16 +26,13 @@ __device__ __forceinline__ uint64_t ef_av(uint64_t h) {
 
 struct EfLane { uint64_t a, b, s0, s1, s2, s3; };
 
-// 16-byte page load of the fingerprint pass.  Every page byte is absorbed exactly once, so in the
-// fused encoder the stripes are pure streaming traffic: NOALLOC keeps them out of the L1, which the
-// parse needs for its match-candidate reads (ld.global.nc.L1::no_allocate).
-template <bool NOALLOC> __device__ __forceinline__ uint4 ef_ld16(const uint4 *p) {
-	if (NOALLOC) {
-		uint4 v;
-		asm("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-		return v;
-	}
-	return __ldg(p);
+// 16-byte page load of the fused fingerprint.  Every page byte is absorbed exactly once, so in the
+// encoder the stripes are pure streaming traffic: they stay out of the L1, which the parse needs for
+// its match-candidate reads (ld.global.nc.L1::no_allocate).
+__device__ __forceinline__ uint4 ef_ld16(const uint4 *p) {
+	uint4 v;
+	asm("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+	return v;
 }
 
 __device__ __forceinline__ void ef_init(EfLane &L, int lane) {
@@ -100,8 +97,8 @@ __device__ __forceinline__ void warp_fingerprint128(const uint8_t *src, uint32_t
 // EF128 computed along the frontier of another pass over the same page (the LZ4 parse): stripes
 // are absorbed in order as the caller's position advances, one stripe requested ahead of need, so
 // the page crosses HBM once and the stripe loads double as a prefetch for the parse that follows
-// them.  Same result as warp_fingerprint128.
-template <bool NOALLOC = false> struct EfFrontierT {
+// them.  Same result as warp_fingerprint128; `src` 16-byte aligned.
+struct EfFrontier {
 	EfLane L;
 	uint4 ahead;          // stripe `next`, already requested
 	uint32_t next;        // next stripe to absorb
@@ -111,7 +108,7 @@ template <bool NOALLOC = false> struct EfFrontierT {
 		ef_init(L, lane);
 		next = 0;
 		full = n >> 9;
-		ahead = full ? ef_ld16<NOALLOC>(reinterpret_cast<const uint4 *>(src) + lane) : make_uint4(0, 0, 0, 0);
+		ahead = full ? ef_ld16(reinterpret_cast<const uint4 *>(src) + lane) : make_uint4(0, 0, 0, 0);
 	}
 	__device__ __forceinline__ void take(const uint4 &x) {
 		ef_absorb(L, (uint64_t)x.x | ((uint64_t)x.y << 32), (uint64_t)x.z | ((uint64_t)x.w << 32));
@@ -126,19 +123,19 @@ template <bool NOALLOC = false> struct EfFrontierT {
 		take(ahead);
 		// a long match jumped ahead: single stripes up to a scramble boundary, then 16 stripes per
 		// step with 16 loads in flight, then the remainder
-		while (next < target && (next & 15u)) { const uint4 x = ef_ld16<NOALLOC>(v + (size_t)next * 32); take(x); }
+		while (next < target && (next & 15u)) { const uint4 x = ef_ld16(v + (size_t)next * 32); take(x); }
 		while (target - next >= 16u) {
 			uint4 x[16];
 #pragma unroll
-			for (int k = 0; k < 16; k++) x[k] = ef_ld16<NOALLOC>(v + (size_t)(next + k) * 32);
+			for (int k = 0; k < 16; k++) x[k] = ef_ld16(v + (size_t)(next + k) * 32);
 #pragma unroll
 			for (int k = 0; k < 16; k++)
 				ef_absorb(L, (uint64_t)x[k].x | ((uint64_t)x[k].y << 32), (uint64_t)x[k].z | ((uint64_t)x[k].w << 32));
 			ef_scramble(L);
 			next += 16;
 		}
-		while (next < target) { const uint4 x = ef_ld16<NOALLOC>(v + (size_t)next * 32); take(x); }
-		if (next < full) ahead = ef_ld16<NOALLOC>(v + (size_t)next * 32);
+		while (next < target) { const uint4 x = ef_ld16(v + (size_t)next * 32); take(x); }
+		if (next < full) ahead = ef_ld16(v + (size_t)next * 32);
 	}
 	// absorb the rest of the page (incl. a zero-padded partial stripe) and fold the lanes
 	__device__ __forceinline__ void finish(const uint8_t *src, uint32_t n, int lane, uint64_t &hi, uint64_t &lo) {
@@ -163,6 +160,5 @@ template <bool NOALLOC = false> struct EfFrontierT {
 		hi = ef_av(~((uint64_t)n * 0xC2B2AE3D27D4EB4FULL) + w);
 	}
 };
-typedef EfFrontierT<false> EfFrontier;
 
 }  // namespace cmb

@@ -5,8 +5,6 @@
 //   k_fingerprint EF128 alone
 //   k_compose / k_upsert / k_lookup / k_unset / k_sample   the HBM key table
 //   k_streamgen   synthetic benchmark input
-#include <stdio.h>
-#include <stdlib.h>
 #include "kernels.h"
 #include "common.cuh"
 #include "fingerprint.cuh"
@@ -455,13 +453,12 @@ __device__ __noinline__ uint32_t enc_ticket_chunk(const unsigned int *work, cons
 
 // ENC 0: page read through the L1.  ENC 1: parse frontier staged in a per-warp shared-memory ring
 // by TMA (lz4_encode_ring.cuh); shared memory = tables | rings | mbarriers.
-// FPNA: the fingerprint's streaming loads do not allocate in the L1.
 // Launch bounds = the real launch shapes (2 CTAs x 7 warps, or 1 CTA x 13 warps with the ring), so
 // that the register allocator may use what the SM has (up to 146 / 152 registers per thread) instead
 // of rematerialising loop invariants inside the parse loop.
-constexpr int ENC_PLAIN_WARPS = 7, ENC_RING_WARPS = 13;
-template <bool WIDE, int ENC, bool FPNA>
-__global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WARPS * 32, ENC == 1 ? 1 : 2) k_encode(EncodeJob job) {
+constexpr int ENC_PLAIN_WARPS = 7, ENC_PLAIN_CTAS = 2, ENC_RING_WARPS = 13;
+template <bool WIDE, int ENC>
+__global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WARPS * 32, ENC == 1 ? 1 : ENC_PLAIN_CTAS) k_encode(EncodeJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 	const uint32_t nwarps = blockDim.x >> 5;
@@ -535,10 +532,10 @@ __global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WAR
 		}
 		uint32_t clen, ck = 0xffffffffu;
 		if (job.fps) {                  // fingerprint along the parse frontier: the page is read once
-			clen = lz4_encode_lean<WIDE, true, FPNA, ENC == 1>(src, job.nbytes, dst, job.accel, wsm, ring, lane, fp_hi, fp_lo, ck);
+			clen = lz4_encode_lean<WIDE, true, ENC == 1>(src, job.nbytes, dst, job.accel, wsm, ring, lane, fp_hi, fp_lo, ck);
 			if (lane == 0) { job.fps[2 * (size_t)i] = fp_hi; job.fps[2 * (size_t)i + 1] = fp_lo; }
 		} else {
-			clen = lz4_encode_lean<WIDE, false, false, ENC == 1>(src, job.nbytes, dst, job.accel, wsm, ring, lane, fp_hi, fp_lo, ck);
+			clen = lz4_encode_lean<WIDE, false, ENC == 1>(src, job.nbytes, dst, job.accel, wsm, ring, lane, fp_hi, fp_lo, ck);
 		}
 		if (lane == 0) job.lens[i] = (int32_t)clen;
 		if (store) {
@@ -567,19 +564,17 @@ int sm_count() {
 	return g_sm_count;
 }
 
-static int env_int(const char *name, int dflt, int lo, int hi) {
-	const char *v = getenv(name);
-	if (!v || !*v) return dflt;
-	int x = atoi(v);
-	return x < lo ? lo : x > hi ? hi : x;
-}
-
-template <class K>
-static int launch_encode_kernel(K kern, const EncodeJob &job, int warps, int ctas_per_sm, size_t smem, cudaStream_t st) {
+// Launches k_encode in one of its two organisations (chunks handed out dynamically in both):
+//   plain: residency is bounded by shared memory, one 16 KiB position table per chunk, 14 of them in
+//          the 227 KiB of an SM (2 CTAs x 7 warps);
+//   ring (lz4_encode_ring.cuh): table + 1 KiB TMA ring + mbarriers per warp, 13 chunks per SM in one CTA.
+static int launch_encode_kernel(const EncodeJob &job, bool ring, cudaStream_t st) {
+	const bool wide = job.nbytes >= LZ4_NARROW_LIMIT;
+	void (*const kern)(EncodeJob) = ring ? (wide ? k_encode<true, 1> : k_encode<false, 1>)
+	                                     : (wide ? k_encode<true, 0> : k_encode<false, 0>);
+	const int warps = ring ? ENC_RING_WARPS : ENC_PLAIN_WARPS, ctas_per_sm = ring ? 1 : ENC_PLAIN_CTAS;
+	const size_t smem = (size_t)warps * (ring ? RING_WARP_SMEM : LZ4_TABLE_BYTES);
 	CMB_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-	// what the tables leave of the 256 KiB per SM is L1 for the page reads; -1 = driver's choice
-	static int carve = env_int("CMB200_ENC_CARVEOUT", -1, -1, 100);
-	if (carve >= 0) CMB_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
 	uint32_t grid = (uint32_t)(sm_count() * ctas_per_sm);
 	uint32_t need = (job.n + warps - 1) / warps;
 	if (grid > need) grid = need;
@@ -588,57 +583,23 @@ static int launch_encode_kernel(K kern, const EncodeJob &job, int warps, int cta
 	return 0;
 }
 
-static int enc_plain_warps() { static const int w = env_int("CMB200_ENC_WARPS", ENC_PLAIN_WARPS, 1, ENC_PLAIN_WARPS); return w; }
-static int enc_plain_ctas() { static const int c = env_int("CMB200_ENC_CTAS_PER_SM", 2, 1, 2); return c; }
-static int enc_ring_warps() { static const int w = env_int("CMB200_RING_WARPS", ENC_RING_WARPS, 1, ENC_RING_WARPS); return w; }
-
-// Plain organisation: residency is bounded by shared memory, one 16 KiB position table per chunk,
-// 14 of them in the 227 KiB of an SM (2 CTAs x 7 warps); chunks handed out dynamically.
-static int launch_encode_warps(const EncodeJob &job, cudaStream_t st, bool fpna) {
-	const int warps = enc_plain_warps(), ctas = enc_plain_ctas();
-	const size_t smem = (size_t)warps * LZ4_TABLE_BYTES;
-	const bool wide = job.nbytes >= LZ4_NARROW_LIMIT;
-	if (wide) return fpna ? launch_encode_kernel(k_encode<true, 0, true>, job, warps, ctas, smem, st)
-	                      : launch_encode_kernel(k_encode<true, 0, false>, job, warps, ctas, smem, st);
-	return fpna ? launch_encode_kernel(k_encode<false, 0, true>, job, warps, ctas, smem, st)
-	            : launch_encode_kernel(k_encode<false, 0, false>, job, warps, ctas, smem, st);
-}
-
-// Ring organisation (lz4_encode_ring.cuh): table + 1 KiB TMA ring + mbarriers per warp, 13 chunks
-// per SM in one CTA.
-static int launch_encode_ring(const EncodeJob &job, cudaStream_t st, bool fpna) {
-	const int warps = enc_ring_warps();
-	const size_t smem = (size_t)warps * RING_WARP_SMEM;
-	const bool wide = job.nbytes >= LZ4_NARROW_LIMIT;
-	if (wide) return fpna ? launch_encode_kernel(k_encode<true, 1, true>, job, warps, 1, smem, st)
-	                      : launch_encode_kernel(k_encode<true, 1, false>, job, warps, 1, smem, st);
-	return fpna ? launch_encode_kernel(k_encode<false, 1, true>, job, warps, 1, smem, st)
-	            : launch_encode_kernel(k_encode<false, 1, false>, job, warps, 1, smem, st);
-}
-
 int launch_encode(const EncodeJob &job_in, cudaStream_t st) {
 	if (job_in.n == 0) return 0;
-	// One encoder loop (lz4_encode_lean), two data paths with identical output:
-	//   2 "ring" (default): the parse frontier staged in a per-warp shared-memory ring by TMA
-	//               (lz4_encode_ring.cuh), 13 chunks per SM in one CTA;
-	//   0 "plain":  the page read through the L1, 14 chunks per SM — also what accelerations above
-	//               12 and unaligned page buffers use.
-	static int mode = env_int("CMB200_ENC_MODE", 2, 0, 2);
-	static int fpna = env_int("CMB200_FP_NOALLOC", 1, 0, 1);
+	// One encoder loop (lz4_encode_lean), two data paths with identical output: the ring, where it
+	// holds what 30 probes reach (accel <= 12), and the page read through the L1 for every other
+	// acceleration.  Both need the 16-byte aligned pages EncodeJob asks for (TMA, fingerprint loads).
 	EncodeJob job = job_in;
-	const bool aligned = (reinterpret_cast<uintptr_t>(job.pages) & 15u) == 0 && (job.page_stride & 15u) == 0;
-	// the ring holds what 30 probes at accel <= 12 reach and TMA wants 16-byte aligned pages
-	const bool ring = mode == 2 && job.accel >= 1 && job.accel <= RING_MAX_ACCEL && job.nbytes < (1u << 24) && aligned;
+	const bool ring = job.accel >= 1 && job.accel <= RING_MAX_ACCEL && job.nbytes < (1u << 24);
 	// Longest-first handout when chunks wait for a warp at all (more chunks than resident warps) and
-	// are encoded (a raw store costs the same per chunk); the sample wants >= 1 KiB aligned pages.
-	const uint32_t resident = (uint32_t)sm_count() * (ring ? enc_ring_warps() : enc_plain_ctas() * enc_plain_warps());
-	if (job.n <= resident || job.accel == 0 || job.nbytes < 1024u || !aligned) job.order = nullptr;
+	// are encoded (a raw store costs the same per chunk); the sample wants >= 1 KiB pages.
+	const uint32_t resident = (uint32_t)sm_count() * (ring ? ENC_RING_WARPS : ENC_PLAIN_CTAS * ENC_PLAIN_WARPS);
+	if (job.n <= resident || job.accel == 0 || job.nbytes < 1024u) job.order = nullptr;
 	CMB_CHECK(cudaMemsetAsync(job.work, 0, (job.order ? 1 + ENC_BUCKETS : 1) * sizeof(unsigned int), st));
 	if (job.order) {
 		k_cost<<<(job.n + COST_WARPS - 1) / COST_WARPS, COST_WARPS * 32, 0, st>>>(job);   // a warp per chunk
 		CMB_CHECK(cudaGetLastError());
 	}
-	if ((ring ? launch_encode_ring(job, st, fpna != 0) : launch_encode_warps(job, st, fpna != 0)) != 0) return -1;
+	if (launch_encode_kernel(job, ring, st) != 0) return -1;
 	return job.order ? 2 : 1;
 }
 
@@ -761,7 +722,7 @@ __device__ void gs_region_give(const GetJob &job, uint32_t r) { atomicAnd(&job.p
 __device__ void gs_sections(const GetJob &job, GetShared *sh, DecodeCta *dc, uint32_t clen, bool local) {
 	const uint32_t n = job.nbytes, S = n / DC_CHAINS;
 	bool use = false;
-	if (local && job.table.ckpt && CMB_GET_CKPT) {
+	if (local && job.table.ckpt) {
 		const uint32_t *ck = job.table.ckpt + (size_t)sh->idx * CKPT_WORDS;
 		const uint32_t want = ckpt_tag(sh->off, clen);
 		if (ldv32(ck) == want) {
@@ -806,16 +767,8 @@ __device__ bool gs_sections_fit(const DecodeCta *dc, uint32_t clen, uint32_t n) 
 	return dc->ip1[prev] == clen && dc->op1[prev] == n;          // filemap.c:244-248: consumed == compressed_length
 }
 
-#ifdef CMB_GS_TRACE            /* diagnostic builds only: cycle stamps of the phases, printed by CTA 0 */
-#define GS_STAMP(k) do { if (tid == 0) stamp[k] = clock64(); } while (0)
-#else
-#define GS_STAMP(k) do { } while (0)
-#endif
 __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
-#ifdef CMB_GS_TRACE
-	long long stamp[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-#endif
 	GetShared *sh = reinterpret_cast<GetShared *>(smem);
 	DecodeCta *dc = reinterpret_cast<DecodeCta *>(smem + 128);
 	uint8_t *rec = smem + GS_CTRL;
@@ -827,7 +780,6 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	uint8_t *out = job.out + (size_t)i * job.nbytes;
 	const uint32_t s_bar = smem_addr(&sh->bar);
 	if (job.valid && !job.valid[i]) { if (tid == 0) job.status[i] = ST_INVALID; return; }
-	GS_STAMP(0);
 	if (tid == 0) {
 		sh->region = 0xffffffffu;
 		mbar_init(s_bar, 1u);
@@ -886,7 +838,6 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 			break;
 		}
 		// ---- LZ4 block -> page, both in shared memory (lz4_decode_cta.cuh) ----
-		GS_STAMP(1);
 		if (tid == 0) {
 			if (sh->region == 0xffffffffu) sh->region = gs_region_take(job);
 			gs_sections(job, sh, dc, clen, st == ST_HIT);
@@ -897,7 +848,6 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 		const uint32_t stride = dc_stride(job.nbytes);
 		const uint32_t blk_s = smem_addr(rec + 24), page_s = smem_addr(page);
 		bool good = false;
-		GS_STAMP(2);
 		for (int pass = 0; pass < 2 && !good; pass++) {
 			const bool many = sh->sections > 1u;
 			if (dc->ip0[warp] != 0xffffffffu)
@@ -912,28 +862,15 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 			__syncthreads();
 		}
 		if (!good) { result = ST_BAD_DECODE; break; }             // filemap.c:244-248
-		GS_STAMP(3);
-#ifndef CMB_DC_SKIP_LIT       /* diagnostic builds only: what a phase costs */
 		dc_literals(dc, desc, stride, blk_s, page_s, rec + 24, page, warp, lane);
-#endif
 		__syncthreads();
-		GS_STAMP(4);
-#ifndef CMB_DC_SKIP_MATCH
 		if (warp == 0) dc_matches(dc, desc, stride, page_s, lane);
-#endif
 		__syncthreads();
-		GS_STAMP(5);
 		for (uint32_t k = tid; k < job.nbytes / 16u; k += GS_THREADS)
 			reinterpret_cast<uint4 *>(out)[k] = reinterpret_cast<const uint4 *>(page)[k];
-		GS_STAMP(6);
 		result = ST_HIT;
 		break;
 	}
-#ifdef CMB_GS_TRACE
-	if (tid == 0 && blockIdx.x == 0 && stamp[6])
-		printf("gs_trace clen %u sections %u: stage %lld sections %lld parse %lld literals %lld matches %lld out %lld (cycles)\n", sh->clen, sh->sections,
-		    stamp[1] - stamp[0], stamp[2] - stamp[1], stamp[3] - stamp[2], stamp[4] - stamp[3], stamp[5] - stamp[4], stamp[6] - stamp[5]);
-#endif
 	// status may live in page-locked host memory that the caller polls: the page first, then the status
 	// (every thread's stores happen before the barrier, thread 0's system-wide fence after it is cumulative)
 	__syncthreads();

@@ -40,9 +40,6 @@ struct TableView {
 // that sixteenth.  Written by the encoder (kernels.cu:ckpt_store), read by k_get_small.
 constexpr uint32_t CKPT_WORDS = 16;
 constexpr uint32_t CKPT_POS_BITS = 13;       // n/16 <= 8192 for pages up to 128 KiB
-#ifndef CMB_GET_CKPT
-#define CMB_GET_CKPT 1
-#endif
 __host__ __device__ inline uint32_t ckpt_tag(unsigned long long rec_off, uint32_t clen) {
 	return 0x80000000u | (((uint32_t)(rec_off >> 4) ^ (clen * 0x9E3779B1u)) & 0x7fffffffu);
 }
@@ -72,7 +69,7 @@ enum LookupStatus : int32_t {
 
 struct EncodeJob {
 	const uint8_t *pages;    // n chunks, `page_stride` apart, 16-byte aligned
-	uint64_t page_stride;
+	uint64_t page_stride;    // a multiple of 16
 	uint32_t nbytes;         // chunk length
 	uint32_t n;
 	uint32_t accel;          // 0 = store raw (cachemap.h comp_accel==0)

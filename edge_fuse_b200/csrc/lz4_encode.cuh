@@ -72,33 +72,13 @@ template <> struct Lz4Table<true> {
 // aligned loads (page buffers are padded past their end; the word before the page start is never
 // needed because backward extension is capped by the position itself).
 struct Lz4Around { uint32_t before, at, next; };
-#ifndef CMB_LZ4_HINT_PROBE
-#define CMB_LZ4_HINT_PROBE 0
-#endif
-#ifndef CMB_LZ4_HINT_CAND
-#define CMB_LZ4_HINT_CAND 0
-#endif
-// HINT: 0 = ld.global.nc, 1 = + L1::evict_last, 2 = + L1::no_allocate, 3 = .cg, 4 = .cs, 5 = .lu,
-// 6 = .nc + L1::evict_first (tuning)
-template <int HINT> __device__ __forceinline__ uint32_t lz4_ldw(const uint32_t *q) {
-	uint32_t v;
-	if (HINT == 1) asm("ld.global.nc.L1::evict_last.b32 %0, [%1];" : "=r"(v) : "l"(q));
-	else if (HINT == 2) asm("ld.global.nc.L1::no_allocate.b32 %0, [%1];" : "=r"(v) : "l"(q));
-	else if (HINT == 3) v = __ldcg(q);
-	else if (HINT == 4) v = __ldcs(q);
-	else if (HINT == 5) v = __ldlu(q);
-	else if (HINT == 6) asm("ld.global.nc.L1::evict_first.b32 %0, [%1];" : "=r"(v) : "l"(q));
-	else v = __ldg(q);
-	return v;
-}
-template <int HINT = 0>
 __device__ __forceinline__ Lz4Around lz4_around(const uint8_t *src, uint32_t p) {
 	const uint32_t a = p & ~3u, sh = (p & 3u) * 8u;
 	const uint32_t *q = reinterpret_cast<const uint32_t *>(src + a);
 	// p < 4: the word before the page does not exist and is not needed (backward extension is capped
 	// by the position), so the first word is read twice instead of branching
-	const uint32_t w0 = lz4_ldw<HINT>(q - (a != 0u));
-	const uint32_t w1 = lz4_ldw<HINT>(q), w2 = lz4_ldw<HINT>(q + 1), w3 = lz4_ldw<HINT>(q + 2);
+	const uint32_t w0 = __ldg(q - (a != 0u));
+	const uint32_t w1 = __ldg(q), w2 = __ldg(q + 1), w3 = __ldg(q + 2);
 	Lz4Around r;
 	r.before = __funnelshift_r(w0, w1, sh);
 	r.at = __funnelshift_r(w1, w2, sh);

@@ -159,7 +159,7 @@ __device__ __forceinline__ Lz4Around ring_around(const uint8_t *ring, uint32_t p
 
 // Encodes src[0,n) into dst; returns the block length (uniform across the warp).  tab_smem = this
 // warp's LZ4_TABLE_BYTES of shared memory; src must be 4-byte aligned and readable up to 16 bytes
-// past src + n (the library's page buffers are contiguous and padded).  With FP the EF128
+// past src + n (the library's page buffers are contiguous and padded); with FP, 16-byte aligned.  With FP the EF128
 // fingerprint of the page is computed along the way (EfFrontier): parse and fingerprint then read
 // the page from HBM once.  RING: the probe neighbourhoods and literal bytes come from the warp's TMA ring
 // (accel <= RING_MAX_ACCEL, src 16-byte aligned, `ring` set up by this warp); otherwise from global
@@ -172,7 +172,7 @@ __device__ __forceinline__ Lz4Around ring_around(const uint8_t *ring, uint32_t p
 // chain per warp every instruction of the body costs issue time whether or not the next sequence
 // depends on it): everything that changes only every few hundred bytes — the fingerprint frontier,
 // the ring — hangs off ONE comparison of the anchor with the position of the next such event.
-template <bool WIDE, bool FP, bool FP_NOALLOC, bool RING>
+template <bool WIDE, bool FP, bool RING>
 __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n, uint8_t *__restrict__ dst,
     uint32_t accel, uint8_t *tab_smem, PageRing &ring, int lane, uint64_t &fp_hi, uint64_t &fp_lo, uint32_t &ck) {
 	Lz4Table<WIDE> tab;
@@ -185,7 +185,7 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 	const uint32_t ck_span = n / CKPT_WORDS;
 	uint32_t ck_k = 1, ck_at = ck_span ? ck_span : 0xffffffffu;
 	ck = 0xffffffffu;
-	EfFrontierT<FP_NOALLOC> fp;
+	EfFrontier fp;
 	if (FP) fp.start(src, n, lane);
 
 	// lz4.c:739 — table cleared per call: an untouched slot aliases position 0.
@@ -222,16 +222,9 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 		// few probes).  So a chunk whose recent batches all hit early runs 16-lane batches (refill,
 		// re-test, 14 probes); a 16-lane batch that finds nothing continues in lz4_search_slow from slot
 		// 16 and the chunk goes back to 32 lanes for a while.  Same probes in the same order either way.
-#ifndef CMB_LZ4_NARROW
-#define CMB_LZ4_NARROW 1
-#endif
-#ifndef CMB_LZ4_NARROW_W
-#define CMB_LZ4_NARROW_W 16u
-#endif
-#ifndef CMB_LZ4_NARROW_HIT
-#define CMB_LZ4_NARROW_HIT 12
-#endif
-		uint32_t width = 32u, calm = 0u;                                    // lanes per batch; batches in a row that hit below lane 12
+		constexpr uint32_t NARROW_W = 16u;                                 // lanes of a narrow batch
+		constexpr int NARROW_HIT = 12;                                     // a hit at or above this lane widens the batch again
+		uint32_t width = 32u, calm = 0u;                                    // lanes per batch; batches in a row that hit below NARROW_HIT
 		uint32_t next_event = 0, ring_next = 0;                            // anchor at which the frontiers move next / a checkpoint is due
 		for (;;) {
 			if (anchor >= next_event) {
@@ -286,7 +279,7 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 			} else {
 				litbyte = ldg8(src + min(anchor + (uint32_t)lane, n - 1u));
 				litbyte2 = ldg8(src + min(anchor + 32u + (uint32_t)lane, n - 1u));
-				ai = lz4_around<CMB_LZ4_HINT_PROBE>(src, pos);
+				ai = lz4_around(src, pos);
 			}
 
 			// ---- unified batch ----
@@ -296,7 +289,7 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 			__syncwarp();
 			if (en) tab.put(h, pos);                                // speculative commit
 			__syncwarp();
-			const Lz4Around ac = lz4_around<CMB_LZ4_HINT_CAND>(src, cand);   // latency overlaps the read-back
+			const Lz4Around ac = lz4_around(src, cand);   // latency overlaps the read-back
 			const uint32_t seen = tab.get(h);
 			__syncwarp();                                           // read-backs done before any undo store
 			const bool foreign = en && seen != (WIDE ? pos : (pos & 0xffffu));
@@ -327,10 +320,8 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 				fwd = __shfl_sync(CMB_FULL, nf, w);
 				back = __shfl_sync(CMB_FULL, nb, w);
 				retest_hit = w == 1;
-				if (CMB_LZ4_NARROW) {
-					calm = w < CMB_LZ4_NARROW_HIT ? calm + 1u : 0u;
-					if (w >= CMB_LZ4_NARROW_HIT) width = 32u; else if (calm >= 8u) width = CMB_LZ4_NARROW_W;
-				}
+				calm = w < NARROW_HIT ? calm + 1u : 0u;
+				if (w >= NARROW_HIT) width = 32u; else if (calm >= 8u) width = NARROW_W;
 				if (fwd == 4u || back == 4u) {                      // longer than the neighbourhoods show: rare
 					if (fwd == 4u) fwd = 4u + lz4_count_long(src, ip + 8u, match + 8u, mlimit, lim4, lane);
 					if (back == 4u && ip >= anchor + 5u && match >= 5u)
@@ -341,7 +332,7 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 				// lanes of this batch that were held back only by the end margin (not by the batch width)
 				const uint32_t enmask = __ballot_sync(CMB_FULL, en || special || (uint32_t)lane >= width);
 				const uint32_t w0 = width;
-				if (CMB_LZ4_NARROW) { width = 32u; calm = 0u; }
+				width = 32u; calm = 0u;
 				if (foreigns) {
 					if (en) tab.put(h, cand);
 					__syncwarp();

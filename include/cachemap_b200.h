@@ -40,7 +40,7 @@ typedef struct cmb200_config {
 	uint64_t arena_bytes;   /* HBM arena for records, 0 = sized from capacity and free memory */
 	uint64_t table_slots;   /* key-table slots (power of two), 0 = 4 x capacity rounded up */
 	uint32_t max_batch;     /* chunks per kernel launch, 0 = 4096 (host pages are pipelined in
-	                         * steps of min(max_batch, CMB200_HOST_BATCH = 4096) chunks) */
+	                         * steps of min(max_batch, 4096) chunks) */
 	uint32_t flags;
 } cmb200_config;
 
@@ -72,7 +72,9 @@ int cmb200_sync(cmb200_engine *e);
 /* filemap_set for n chunks (cachemap/filemap.c:112-158): pages = n x (1<<pshift) bytes.
  * valid (nullable) = per-chunk flag, 0 skips the chunk (rejected address).  ts (nullable) = the
  * LMDB attribute.  Chunks are applied in array order: a later chunk with the same key wins.
- * lens_out (nullable, host) receives each stored compressed_length, or -1 for skipped chunks. */
+ * lens_out (nullable, host) receives each stored compressed_length, or -1 for skipped chunks.
+ * pages_dev (cmb200_put_batch_dev) must be 16-byte aligned, as cmb200_dev_alloc and cudaMalloc
+ * memory is; any other pointer fails with -1 before anything is stored. */
 int cmb200_put_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     const void *pages_host, const uint64_t *ts, int32_t *lens_out);
 int cmb200_put_batch_dev(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
@@ -128,7 +130,8 @@ int cmb200_get_stats(cmb200_engine *e, cmb200_stats *out);
  * asynchronous.  Like cmb200_put_batch_async (pages on the host, pages_on_dev = 0), or with the
  * pages in page-locked host memory that the caller leaves untouched until the ticket is done
  * (pages_on_dev = 2: the call returns without waiting for its own copies, so the next step can be
- * queued behind them at once), or device resident (pages_on_dev = 1, same lifetime rule),
+ * queued behind them at once), or device resident (pages_on_dev = 1, same lifetime rule, and
+ * 16-byte aligned as for cmb200_put_batch_dev),
  * and additionally writes one 32-byte exchange record per chunk — {u, l, global stream position,
  * rank << 32 | stored length (negative: nothing stored)} — to records_dev_out (device memory,
  * n x 32 bytes) on the engine's stream.  The caller all-gathers those records (NCCL, on that

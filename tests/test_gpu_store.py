@@ -594,6 +594,41 @@ def test_put_step_records_and_device_import(E, gpu, oracle):
     E.lib().cmb200_host_free(hp)
 
 
+def test_device_pages_must_be_16_byte_aligned(E, gpu, oracle):
+    """The encoder reads device pages with 16-byte loads, so put_batch_dev and put_step(on_dev=1)
+    refuse a pointer that is only 4-byte aligned before anything is queued: no kernel is launched
+    and the store is unchanged.  The same pages at a 16-byte aligned address store the reference's
+    records."""
+    n = 8
+    eng = E.Engine(pshift=16, accel=12, capacity=1024, arena_bytes=64 << 20, max_batch=64, flags=E.FINGERPRINT)
+    pages = np.stack([E.gen_chunk_host(5, c, 65536) for c in range(n)])
+    d_pages = eng.dev_alloc(n * 65536 + 256)
+    d_rec = eng.dev_alloc(n * 32)
+    u = np.full(n, 77, dtype=np.uint64)
+    l = np.arange(n, dtype=np.uint64)
+    keys = ("entries", "put_chunks", "dropped_puts", "kernel_launches")
+    before = eng.stats()
+    eng.h2d(d_pages + 4, pages)
+    with pytest.raises(RuntimeError, match="16-byte aligned"):
+        eng.put(u, l, d_pages + 4, on_dev=True)
+    with pytest.raises(RuntimeError, match="16-byte aligned"):
+        eng.put_step(u, l, d_pages + 4, on_dev=True, records_dev=d_rec)
+    eng.sync()
+    after = eng.stats()
+    assert {k: after[k] for k in keys} == {k: before[k] for k in keys}
+    eng.h2d(d_pages + 16, pages)
+    eng.put(u, l, d_pages + 16, on_dev=True)
+    eng.wait(eng.put_step(u, l + np.uint64(n), d_pages + 16, on_dev=True, records_dev=d_rec))
+    assert eng.entries() == 2 * n
+    recs = eng.read_records(np.concatenate([u, u]), np.concatenate([l, l + np.uint64(n)]))
+    for i in range(2 * n):
+        blk = oracle.lz4_encode(pages[i % n], 12)
+        assert recs[i] == oracle.record_prefix(77, i, len(blk)) + blk, i
+    for p in (d_pages, d_rec):
+        eng.dev_free(p)
+    eng.close()
+
+
 def test_arena_compaction_reclaims_deleted_and_outgrown_records(E, gpu, oracle):
     """cmb200_compact slides the live records down: arena_used falls to the live bytes, garbage to
     zero, and every record, timestamp and fingerprint is what it was (staged and in-place paths)."""

@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Builds a tuning variant of libcachemap.so.0.0 with extra -D flags into
-edge_fuse_b200/build/variants/<name>.so (select it with CMB200_LIB=<path>).
+"""Builds a variant of libcachemap.so.0.0 with extra -D flags into
+edge_fuse_b200/build/variants/<name>.so (select it with CMB200_LIB=<path>), e.g. the encoder
+timeline build that tools/encode_timeline.py reads:
 
-    python tools/build_variant.py probe_last -DCMB_LZ4_HINT_PROBE=1
+    python tools/build_variant.py timeline -DCMB_ENC_TIMELINE
 """
 import os, subprocess, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
