@@ -34,6 +34,13 @@
 #include "../../include/cachemap.h"
 #include "../../include/cachemap_b200.h"
 
+/* The host tier is optional in the engine this layer links against: libcachemap's engine defines
+ * these, an engine without a tier (such as the CPU stand-in the host-layer tests link) does not, and
+ * then they are null and CMB200_HOST_TIER_MB is refused. */
+#pragma weak cmb200_host_tier_enable
+#pragma weak cmb200_demote_batch
+#pragma weak cmb200_host_tier_stats
+
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
                                  * (<= the engine's GET_LANES); see the combining queue below */
@@ -72,6 +79,7 @@ struct filemap {
 	pthread_mutex_t init_mu;
 	int init_state;         /* 0 = not yet, 1 = ready, -1 = failed */
 	cmb200_engine *eng;
+	int host_tier;          /* the engine has a host tier (CMB200_HOST_TIER_MB): a full arena demotes instead of evicting */
 	uint8_t *h_stage;       /* page-locked, LEADERS x COMBINE_MAX pages: the stage buffer of each leader slot */
 	int leader_busy[LEADERS];       /* a batch is in flight in this slot (under q_mu) */
 	int batch_left[LEADERS];        /* its requesters that have not taken their answer yet (atomic) */
@@ -136,6 +144,15 @@ filemap_engine_ready(struct filemap *m)
 		cfg.max_batch = (uint32_t)env_long("CMB200_MAX_BATCH", 0);
 		cfg.flags = env_long("CMB200_FINGERPRINT", 0) ? CMB200_FINGERPRINT : 0;
 		m->eng = cmb200_engine_create(&cfg);
+		const long tier_mb = env_long("CMB200_HOST_TIER_MB", 0);
+		if (m->eng && tier_mb > 0) {
+			if (!cmb200_host_tier_enable)
+				fprintf(stderr, "cachemap_b200: no host tier of %ld MiB: the engine has none\n", tier_mb);
+			else if (cmb200_host_tier_enable(m->eng, (uint64_t)tier_mb << 20) == 0)
+				m->host_tier = 1;
+			else
+				fprintf(stderr, "cachemap_b200: no host tier of %ld MiB: %s\n", tier_mb, cmb200_last_error());
+		}
 		if (m->eng) {
 			m->h_stage = cmb200_host_alloc((size_t)LEADERS * COMBINE_MAX * m->bsize);
 			/* ring of 256 MiB by default, at least 64 pages.  The size sets the batch the flusher can form
@@ -329,6 +346,71 @@ filemap_evict_n(struct filemap *m, uint64_t want)
 	return gone;
 }
 
+struct aged { uint64_t ts; cmb200_addr a; };
+
+static int
+aged_cmp(const void *x, const void *y)
+{
+	const uint64_t a = ((const struct aged *)x)->ts, b = ((const struct aged *)y)->ts;
+	return a < b ? -1 : a > b;
+}
+
+/* Moves up to `want` arena records to the host tier.  The candidates are drawn as filemap_evict_n
+ * draws them (3 per record wanted) and go oldest first; keys already in the tier are passed over, so
+ * a round goes on down its candidates until `want` have moved.  When few records are left in the
+ * arena a round may find none: it draws again, up to 16 times in a row.  Returns how many moved. */
+static uint64_t
+filemap_demote_n(struct filemap *m, uint64_t want)
+{
+	uint64_t moved = 0;
+	int idle = 0;
+	while (moved < want && idle < 16) {
+		uint64_t need = want - moved;
+		if (need > 4096)
+			need = 4096;
+		const uint64_t nd = 3 * need;
+		uint64_t *draws = malloc(nd * sizeof(uint64_t));
+		uint64_t *ts = malloc(nd * sizeof(uint64_t));
+		int32_t *ok = malloc(nd * sizeof(int32_t));
+		cmb200_addr *cand = malloc(nd * sizeof(cmb200_addr));
+		struct aged *old = malloc(nd * sizeof(struct aged));
+		cmb200_addr *victim = malloc(nd * sizeof(cmb200_addr));
+		uint64_t round = 0;
+		if (draws && ts && ok && cand && old && victim) {
+			for (uint64_t i = 0; i < nd; i++) {
+				uint64_t r = 0;
+				for (int b = 0; b < 64; b += 30)        /* filemap.c:271-274 */
+					r = r * ((uint64_t)RAND_MAX + 1) + (uint64_t)rand();
+				draws[i] = r;
+			}
+			if (cmb200_sample(m->eng, (size_t)nd, draws, cand, ts, ok) == 0) {
+				uint64_t nv = 0;
+				for (uint64_t i = 0; i < nd; i++)
+					if (ok[i] > 0)
+						old[nv++] = (struct aged){ ts[i], cand[i] };
+				qsort(old, (size_t)nv, sizeof(struct aged), aged_cmp);
+				for (uint64_t k = 0; k < nv && moved < want;) {
+					uint64_t take = want - moved < nv - k ? want - moved : nv - k, got = 0;
+					for (uint64_t j = 0; j < take; j++)
+						victim[j] = old[k + j].a;
+					if (cmb200_demote_batch(m->eng, (size_t)take, victim, &got) != 0) {
+						fprintf(stderr, "cachemap_b200: demotion to the host tier failed: %s\n", cmb200_last_error());
+						break;
+					}
+					moved += got;
+					round += got;
+					k += take;
+				}
+			} else {
+				fprintf(stderr, "cachemap_b200: demotion could not sample the store: %s\n", cmb200_last_error());
+			}
+		}
+		free(draws); free(ts); free(ok); free(cand); free(old); free(victim);
+		idle = round ? 0 : idle + 1;
+	}
+	return moved;
+}
+
 /* Before `incoming` puts: while entries + incoming > capacity, evict (cachemap.c:17-45); loops
  * until the count fits or nothing more can be retired. */
 static void
@@ -351,7 +433,9 @@ filemap_evict(struct filemap *m, uint64_t incoming)
 /* The arena is a bump allocator; deleted and outgrown records stay behind as garbage until
  * cmb200_compact slides the live ones down.  When `incoming` worst-case records would not fit:
  * compact if that frees enough; otherwise the live data itself fills the arena (the store was
- * sized in pages, the arena is bytes), so evict by bytes as well and compact what that frees.
+ * sized in pages, the arena is bytes).  With a host tier that can take what must move, the oldest
+ * records are demoted to it and the arena compacted, so the store keeps `capacity` pages as the
+ * reference's LMDB files do; otherwise evict by bytes as well and compact what that frees.
  * Only when even that fails does a put get dropped, as a full LMDB map drops it
  * (filemap.c:143-145,154-157). */
 static void
@@ -377,10 +461,24 @@ filemap_check_arena(struct filemap *m, uint64_t incoming)
 		}
 		if (st.entries == 0)
 			return;
-		/* live records fill the arena: retire enough of them (average record size, plus a margin) */
+		/* live records fill the arena: move or retire enough of them (average record size, plus a margin) */
 		const uint64_t live = st.arena_used > st.arena_garbage ? st.arena_used - st.arena_garbage : 1;
-		const uint64_t avg = live / st.entries ? live / st.entries : 1;
 		const uint64_t shortfall = need - (free_b + st.arena_garbage < need ? free_b + st.arena_garbage : need);
+		struct cmb200_host_tier_stats ht;
+		if (m->host_tier && cmb200_host_tier_stats(m->eng, &ht) == 0 && shortfall <= ht.bytes) {
+			if (st.entries <= ht.records)
+				return;         /* every live record is in the tier already: evicting frees no arena bytes */
+			const uint64_t in_arena = st.entries - ht.records;
+			const uint64_t avg = live / in_arena ? live / in_arena : 1;
+			uint64_t victims = shortfall / avg + shortfall / avg / 8 + 16;
+			if (victims > in_arena)
+				victims = in_arena;
+			if (filemap_demote_n(m, victims) == 0)
+				return;
+			evicted = 1;
+			continue;
+		}
+		const uint64_t avg = live / st.entries ? live / st.entries : 1;
 		uint64_t victims = shortfall / avg + shortfall / avg / 8 + 16;
 		if (victims > st.entries)
 			victims = st.entries;

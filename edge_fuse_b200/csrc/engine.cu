@@ -5,16 +5,20 @@
 //   arena       bump-allocated records    {24-byte data_prefix, LZ4 block | raw page}
 //   page ring   2 x max_batch x bsize     double-buffered landing zone for host pages
 //   stage       one (bsize+1024) row per resident encoder warp: block before it is packed into the arena
+// Host tier (optional, cmb200_host_tier_enable): page-locked, device-mapped host memory holding records
+// demoted from the arena, a ring in demotion order (DESIGN.md §2).
 // A put batch is: H2D copy (copy stream)  ->  k_upsert  ->  k_encode (fingerprint + LZ4 + arena
 // commit + table publish), sub-batch k+1's copy overlapping sub-batch k's kernels.
 // A get batch is: k_lookup -> k_decode -> D2H copy.
 #include <algorithm>
 #include <atomic>
+#include <deque>
 #include <mutex>
 #include <shared_mutex>
 #include <sched.h>
 #include <string>
 #include <new>
+#include <unordered_set>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -125,6 +129,21 @@ struct cmb200_engine {
 	size_t meta_cap = 0;                 // entries per copy
 	std::mutex mu;
 	cmb200_stats stats{};
+	// host tier: a ring of records in demotion order.  Log position p lies at tier offset p % size; a
+	// record never straddles the end of the ring (the rest of the lap is skipped).
+	struct HostTier {
+		uint8_t *host = nullptr;             // cudaHostAlloc(mapped); null = no tier
+		uint8_t *dev = nullptr;              // its device address
+		uint64_t size = 0;
+		uint64_t head = 0;                   // log position of the next record
+		std::deque<std::pair<uint64_t, uint32_t>> log;   // {position, bytes} of each record not yet overwritten, oldest first
+		uint64_t demoted_records = 0, demoted_bytes = 0;
+		unsigned long long *d_ctr = nullptr; // device: [0] records retired by wrap-around, [1] host-tier hits
+		unsigned long long *d_retire = nullptr;   // {u, l, location, bytes} per record a wrap overwrites
+		size_t retire_cap = 0;
+		DemoteEntry *d_moves = nullptr;      // max_batch entries
+	} tier;
+	std::atomic<bool> multi_gpu{false};  // a multi-GPU call was made: no host tier from then on
 };
 
 #define ENG_CHECK(expr)                                                 \
@@ -176,6 +195,8 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	}
 	cudaFree(e->d_recoff_out);
 	for (int r = 0; r < GET_MAX_PEERS; r++) if (e->peer_base[r]) cudaIpcCloseMemHandle((void *)e->peer_base[r]);
+	if (e->tier.host) cudaFreeHost(e->tier.host);
+	cudaFree(e->tier.d_ctr); cudaFree(e->tier.d_retire); cudaFree(e->tier.d_moves);
 	cudaFree(e->d_lens); cudaFree(e->d_status); cudaFree(e->d_fps); cudaFree(e->d_recoff); cudaFree(e->d_work); cudaFree(e->d_order); cudaFree(e->d_import_slot);
 	for (int i = 0; i < 2; i++) {
 		if (e->landed[i]) cudaEventDestroy(e->landed[i]);
@@ -263,6 +284,7 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 		e->arena.garbage = e->d_counters + 3;
 		e->arena.dropped = e->d_counters + 4;
 		e->table.remote = e->d_counters + 5;
+		e->arena.tier = e->d_counters + 6;
 
 		e->stage_stride = ((uint64_t)e->bsize + 1024 + 15) & ~15ull;        // filemap.c:120 dest[bsize+1024]
 		ENG_CHECK(cudaMalloc(&e->d_pages[0], (uint64_t)e->host_batch * e->bsize + 256));
@@ -516,6 +538,17 @@ static int check_dev_pages(const void *pages, const char *what) {
 	return 0;
 }
 
+// The multi-GPU calls and the host tier exclude each other: the exchange records and peer reads know
+// arena locations only.
+static int multi_gpu_call(cmb200_engine *e, const char *what) {
+	if (e->tier.host) {
+		snprintf(g_err, sizeof(g_err), "%s: not available on an engine with a host tier", what);
+		return -1;
+	}
+	e->multi_gpu = true;
+	return 0;
+}
+
 static int put_impl(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     const uint8_t *pages, bool pages_on_dev, const uint64_t *ts, int32_t *lens_out, uint64_t *ticket) {
 	std::lock_guard<std::mutex> g(e->mu);
@@ -544,6 +577,7 @@ extern "C" int cmb200_put_batch_async(cmb200_engine *e, size_t n, const cmb200_a
 extern "C" int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     const void *pages, int pages_on_dev, const uint64_t *ts, uint32_t rank, void *records_dev_out,
     int32_t *lens_out, uint64_t *ticket) {
+	if (multi_gpu_call(e, "cmb200_put_step")) return -1;
 	if (n > cmb200_engine::META_CAP) { set_error_msg("cmb200_put_step: more than 262144 chunks in one step"); return -1; }
 	if (pages_on_dev == 1 && check_dev_pages(pages, "cmb200_put_step")) return -1;
 	std::lock_guard<std::mutex> g(e->mu);
@@ -557,6 +591,7 @@ extern "C" int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *ad
 
 extern "C" int cmb200_import_records_dev(cmb200_engine *e, size_t n_total, const void *records_dev, uint32_t my_rank) {
 	std::lock_guard<std::mutex> g(e->mu);
+	if (multi_gpu_call(e, "cmb200_import_records_dev")) return -1;
 	CMB_CHECK(cudaSetDevice(e->device));
 	if (n_total == 0) return 0;
 	if (n_total > 0xffffffffull) { set_error_msg("cmb200_import_records_dev: too many records"); return -1; }
@@ -615,6 +650,7 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		DecodeJob job{};
 		job.n = m; job.nbytes = e->bsize; job.pages = d_out; job.status = e->d_status + at;
 		job.rec_off = e->d_recoff; job.vlen = e->d_vlen; job.arena = e->arena.base;
+		job.host = e->tier.dev; job.host_hits = e->tier.d_ctr + 1;
 		CMB_CHECK(cudaEventRecord(e->t0[nb % e->RING], e->st));
 		if (launch_decode(job, e->st)) return -1;
 		CMB_CHECK(cudaEventRecord(e->t1[nb % e->RING], e->st));
@@ -685,6 +721,7 @@ extern "C" int cmb200_get_batch_dev(cmb200_engine *e, size_t n, const cmb200_add
 
 extern "C" int cmb200_set_stream_order(cmb200_engine *e, uint64_t next_seq, uint64_t stride) {
 	std::lock_guard<std::mutex> g(e->mu);
+	if (multi_gpu_call(e, "cmb200_set_stream_order")) return -1;
 	if (stride == 0) { set_error_msg("stream order: stride must be >= 1"); return -1; }
 	e->seq = next_seq; e->seq_stride = stride;
 	return 0;
@@ -693,6 +730,7 @@ extern "C" int cmb200_set_stream_order(cmb200_engine *e, uint64_t next_seq, uint
 extern "C" int cmb200_import_remote(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint32_t *owner,
     const uint64_t *seq, const uint64_t *loc, int on_dev) {
 	std::lock_guard<std::mutex> g(e->mu);
+	if (multi_gpu_call(e, "cmb200_import_remote")) return -1;
 	CMB_CHECK(cudaSetDevice(e->device));
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
@@ -752,6 +790,7 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	for (size_t i = 0; i < n; i++) hs[i] = SMALL_PENDING;
 	GetJob job{};
 	job.table = e->table; job.arena = e->arena.base; job.arena_size = e->arena.size;
+	job.host = e->tier.dev; job.host_size = e->tier.size; job.host_hits = e->tier.d_ctr + 1;
 	job.addr = (const unsigned long long *)ln->h_addr; job.valid = nullptr; job.n = (uint32_t)n; job.nbytes = e->bsize;
 	job.out = (uint8_t *)pages_out;                          // device memory or page-locked host memory (UVA)
 	job.status = ln->h_status;
@@ -824,6 +863,10 @@ extern "C" int cmb200_close_peers(cmb200_engine *e) {
 }
 
 extern "C" int cmb200_arena_ipc_handle(cmb200_engine *e, void *handle64, uint64_t *arena_bytes_out) {
+	{
+		std::lock_guard<std::mutex> g(e->mu);
+		if (multi_gpu_call(e, "cmb200_arena_ipc_handle")) return -1;
+	}
 	CMB_CHECK(cudaSetDevice(e->device));
 	cudaIpcMemHandle_t h;
 	static_assert(sizeof(h) == 64, "cudaIpcMemHandle_t is 64 bytes");
@@ -834,6 +877,10 @@ extern "C" int cmb200_arena_ipc_handle(cmb200_engine *e, void *handle64, uint64_
 }
 
 extern "C" int cmb200_open_peer(cmb200_engine *e, uint32_t rank, const void *handle64, uint64_t arena_bytes) {
+	{
+		std::lock_guard<std::mutex> g(e->mu);
+		if (multi_gpu_call(e, "cmb200_open_peer")) return -1;
+	}
 	if (rank >= GET_MAX_PEERS) { set_error_msg("cmb200_open_peer: rank out of range"); return -1; }
 	cmb200_engine::GateClosed g(e->get_gate);
 	CMB_CHECK(cudaSetDevice(e->device));
@@ -929,7 +976,8 @@ extern "C" int cmb200_read_records(cmb200_engine *e, size_t n, const cmb200_addr
 			uint32_t clen = vl[i] - 1;
 			size_t total = 24 + (clen ? clen : e->bsize);
 			if (total > stride) { set_error_msg("cmb200_read_records: stride too small"); return -1; }
-			CMB_CHECK(cudaMemcpyAsync((uint8_t *)out_host + (at + i) * stride, e->arena.base + off[i], total,
+			if (off[i] & REC_HOST) memcpy((uint8_t *)out_host + (at + i) * stride, e->tier.host + (off[i] & ~REC_HOST), total);
+			else CMB_CHECK(cudaMemcpyAsync((uint8_t *)out_host + (at + i) * stride, e->arena.base + off[i], total,
 			    cudaMemcpyDeviceToHost, e->st));
 			len_out[at + i] = (int32_t)total;
 		}
@@ -992,7 +1040,7 @@ extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records
 	DevBuf d_list, d_count;
 	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
 	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
-	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, e->st)) return -1;
+	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, false, e->st)) return -1;
 	unsigned long long count = 0;
 	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
@@ -1014,6 +1062,15 @@ extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records
 	static const uint8_t zeros[16] = {0};
 	size_t k = 0;
 	while (ok && k < list.size()) {
+		if (list[k].rec_off & REC_HOST) {
+			// host-tier records sort last and are written straight from the tier
+			const ExportEntry &x = list[k++];
+			SnapRecord r{x.ts, x.fp_hi, x.fp_lo, x.len, 0};
+			const size_t padn = (16 - (x.len & 15)) & 15;
+			ok = fwrite(&r, sizeof(r), 1, f) == 1 && fwrite(e->tier.host + (x.rec_off & ~REC_HOST), x.len, 1, f) == 1 &&
+			    (padn == 0 || fwrite(zeros, padn, 1, f) == 1);
+			continue;
+		}
 		// one window of the arena starting at record k; the records wholly inside it are written out
 		const unsigned long long w0 = list[k].rec_off;
 		unsigned long long w1 = w0 + SNAP_WINDOW;
@@ -1035,6 +1092,8 @@ extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records
 	if (records_out) *records_out = count;
 	return 0;
 }
+
+static int demote_arena_all(cmb200_engine *e);
 
 extern "C" int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out) {
 	std::lock_guard<std::mutex> g(e->mu);
@@ -1082,6 +1141,11 @@ extern "C" int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records
 		}
 		if (rc) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); break; }
 		if (m == 0) { rc = -1; set_error_msg("cmb200_load: record larger than the staging buffer"); break; }
+		if (e->tier.host) {
+			unsigned long long c[8];
+			if (read_counters(e, c)) { rc = -1; break; }
+			if (c[2] + used > e->arena.size && demote_arena_all(e)) { rc = -1; break; }
+		}
 		const bool fail =
 		    cudaMemcpyAsync(e->d_pages[0], blob, used, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
 		    cudaMemcpyAsync(e->d_addr, addr.data(), m * 16, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
@@ -1114,8 +1178,8 @@ extern "C" int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records
 // page-ring buffers, repoints the slots and resets the bump pointer and the per-warp segments.
 // Stop-the-world on the engine's stream, at HBM speed; callers trigger it when the arena is about
 // to overflow although a good part of it is garbage (filemap_make_room, cmb200_compact).
-extern "C" int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out) {
-	std::lock_guard<std::mutex> g(e->mu);
+// (e->mu held)
+static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 	cmb200_engine::GateClosed gg(e->get_gate);          // records move: no small get may be reading the arena
 	unsigned long long c[8];
 	if (read_counters(e, c)) return -1;
@@ -1125,7 +1189,8 @@ extern "C" int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out) {
 	DevBuf d_list, d_count, d_moves;
 	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
 	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
-	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, e->st)) return -1;
+	// arena records only: the host tier is a ring and is never compacted
+	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, true, e->st)) return -1;
 	unsigned long long count = 0;
 	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
@@ -1181,6 +1246,190 @@ extern "C" int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out) {
 			cudaFree(fresh.slots);
 		}
 	}
+	return 0;
+}
+
+extern "C" int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	return compact_locked(e, reclaimed_out);
+}
+
+// ---- host tier ---------------------------------------------------------------------------------
+// Records demoted from the arena live in page-locked, device-mapped host memory, in the arena's
+// record format.  The tier is a ring in demotion order: it is never compacted, and a lap that comes
+// round again first retires (unsets) the keys whose records it overwrites.
+
+extern "C" int cmb200_host_tier_enable(cmb200_engine *e, uint64_t bytes) {
+	std::lock_guard<std::mutex> g(e->mu);
+	if (e->tier.host) { set_error_msg("cmb200_host_tier_enable: the engine already has a host tier"); return -1; }
+	if (e->multi_gpu) { set_error_msg("cmb200_host_tier_enable: not available after a multi-GPU call"); return -1; }
+	if (e->seq != 1) { set_error_msg("cmb200_host_tier_enable: must be called before the first put"); return -1; }
+	bytes = (bytes + 4095) & ~4095ull;
+	if (bytes < 4ull * e->stage_stride) { set_error_msg("cmb200_host_tier_enable: fewer bytes than four worst-case records"); return -1; }
+	CMB_CHECK(cudaSetDevice(e->device));
+	cmb200_engine::HostTier &t = e->tier;
+	if (cudaMalloc(&t.d_ctr, 2 * sizeof(unsigned long long)) != cudaSuccess ||
+	    cudaMalloc(&t.d_moves, (size_t)e->max_batch * sizeof(DemoteEntry)) != cudaSuccess ||
+	    cudaMemset(t.d_ctr, 0, 2 * sizeof(unsigned long long)) != cudaSuccess ||
+	    cudaHostAlloc(&t.host, bytes, cudaHostAllocMapped) != cudaSuccess ||
+	    cudaHostGetDevicePointer(&t.dev, t.host, 0) != cudaSuccess) {
+		cmb_set_error("cmb200_host_tier_enable", cudaGetLastError(), __FILE__, __LINE__);
+		if (t.host) cudaFreeHost(t.host);
+		cudaFree(t.d_ctr); cudaFree(t.d_moves);
+		t = cmb200_engine::HostTier{};
+		return -1;
+	}
+	t.size = bytes;
+	return 0;
+}
+
+// Moves one group of records (their tier region [start, end) is at most one lap and fits the bounce
+// buffer) to the tier: gather -> retire what the region overwrites -> one or two D2H copies -> publish.
+static int demote_group(cmb200_engine *e, const std::vector<DemoteEntry> &grp,
+    const std::vector<std::pair<uint64_t, uint32_t>> &placed, uint64_t start, uint64_t end) {
+	cmb200_engine::HostTier &t = e->tier;
+	uint8_t *bounce = e->d_pages[0];
+	const uint32_t n = (uint32_t)grp.size();
+	CMB_CHECK(cudaMemcpyAsync(t.d_moves, grp.data(), n * sizeof(DemoteEntry), cudaMemcpyHostToDevice, e->st));
+	if (launch_demote_gather(e->arena, t.d_moves, n, bounce, e->st)) return -1;
+	// every record that starts before end - size lies where this region is about to be written
+	std::vector<unsigned long long> ret;
+	while (!t.log.empty() && t.log.front().first + t.size < end) {
+		const uint64_t p = t.log.front().first, at = p % t.size;
+		const unsigned long long *pre = reinterpret_cast<const unsigned long long *>(t.host + at);
+		ret.insert(ret.end(), {pre[0], pre[1], REC_HOST | at, t.log.front().second});
+		t.log.pop_front();
+	}
+	const bool overwrite = end > t.size;        // the region holds bytes of an earlier lap
+	if (overwrite) e->get_gate.close();          // no small get may be reading what is overwritten
+	int rc = 0;
+	const size_t nr = ret.size() / 4;
+	if (nr > t.retire_cap) {
+		if (cudaStreamSynchronize(e->st) != cudaSuccess) rc = -1;
+		cudaFree(t.d_retire);
+		t.d_retire = nullptr; t.retire_cap = 0;
+		if (rc == 0 && cudaMalloc(&t.d_retire, nr * 32) == cudaSuccess) t.retire_cap = nr;
+		else rc = -1;
+	}
+	const uint64_t a0 = start % t.size, bytes = end - start, first = std::min(bytes, t.size - a0);
+	if (rc == 0 && nr) {
+		rc = cudaMemcpyAsync(t.d_retire, ret.data(), nr * 32, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
+		    launch_tier_retire(e->table, e->arena, t.d_retire, (uint32_t)nr, t.d_ctr, e->st) ? -1 : 0;
+		e->stats.kernel_launches++;
+	}
+	if (rc == 0 && (cudaMemcpyAsync(t.host + a0, bounce, first, cudaMemcpyDeviceToHost, e->st) != cudaSuccess ||
+	    (bytes > first && cudaMemcpyAsync(t.host, bounce + first, bytes - first, cudaMemcpyDeviceToHost, e->st) != cudaSuccess)))
+		rc = -1;
+	if (rc == 0 && launch_demote_publish(e->table, e->arena, t.d_moves, n, e->st)) rc = -1;
+	if (cudaStreamSynchronize(e->st) != cudaSuccess) rc = -1;
+	if (overwrite) e->get_gate.reopen();
+	if (rc) { cmb_set_error("host tier demotion", cudaGetLastError(), __FILE__, __LINE__); return -1; }
+	t.log.insert(t.log.end(), placed.begin(), placed.end());
+	t.head = end;
+	t.demoted_records += n;
+	for (const DemoteEntry &d : grp) t.demoted_bytes += d.len;
+	e->stats.kernel_launches += 2;
+	return 0;
+}
+
+// Demotes the arena records {offset, length} (distinct, e->mu held) in the given order.
+static int demote_records(cmb200_engine *e, const std::vector<std::pair<unsigned long long, uint32_t>> &recs) {
+	cmb200_engine::HostTier &t = e->tier;
+	const uint64_t cap = std::min<uint64_t>(t.size, (uint64_t)e->host_batch * e->bsize);   // bounce = one page-ring buffer
+	size_t k = 0;
+	std::vector<DemoteEntry> grp;
+	std::vector<std::pair<uint64_t, uint32_t>> placed;
+	while (k < recs.size()) {
+		grp.clear(); placed.clear();
+		const uint64_t start = t.head;
+		uint64_t pos = start;
+		while (k < recs.size() && grp.size() < e->max_batch) {
+			const uint32_t len = recs[k].second, need = (len + 15u) & ~15u;
+			uint64_t p = pos;
+			if (p % t.size + need > t.size) p += t.size - p % t.size;     // no record straddles the end of the ring
+			if (p + need - start > cap) break;
+			grp.push_back(DemoteEntry{recs[k].first, p % t.size, p - start, len, 0});
+			placed.emplace_back(p, need);
+			pos = p + need;
+			k++;
+		}
+		if (grp.empty()) { set_error_msg("cmb200_demote_batch: record larger than the bounce buffer"); return -1; }
+		if (demote_group(e, grp, placed, start, pos)) return -1;
+	}
+	return 0;
+}
+
+extern "C" int cmb200_demote_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *demoted_out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	if (demoted_out) *demoted_out = 0;
+	if (!e->tier.host) { set_error_msg("cmb200_demote_batch: the engine has no host tier"); return -1; }
+	CMB_CHECK(cudaSetDevice(e->device));
+	harvest_pending(e, true);
+	std::vector<int32_t> st(e->max_batch);
+	std::vector<uint64_t> off(e->max_batch);
+	std::vector<uint32_t> vl(e->max_batch);
+	std::vector<std::pair<unsigned long long, uint32_t>> recs;
+	uint64_t done = 0;
+	for (size_t at = 0; at < n; at += e->max_batch) {
+		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
+		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
+		if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(st.data(), e->d_status, m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemcpyAsync(off.data(), e->d_recoff, m * 8, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemcpyAsync(vl.data(), e->d_vlen, m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		e->stats.kernel_launches++;
+		// absent, remote and host-tier keys are skipped; a key named twice moves once
+		recs.clear();
+		std::unordered_set<uint64_t> seen;
+		for (uint32_t i = 0; i < m; i++) {
+			if (st[i] != ST_HIT || (off[i] & REC_HOST) || !seen.insert(off[i]).second) continue;
+			const uint32_t clen = vl[i] - 1u;
+			recs.emplace_back(off[i], 24u + (clen ? clen : e->bsize));
+		}
+		if (demote_records(e, recs)) return -1;
+		done += recs.size();
+	}
+	if (demoted_out) *demoted_out = done;
+	return 0;
+}
+
+// Moves every arena record to the host tier and compacts the arena (e->mu held): a snapshot that does
+// not fit the arena continues into the tier.
+static int demote_arena_all(cmb200_engine *e) {
+	unsigned long long c[8];
+	if (read_counters(e, c)) return -1;
+	const unsigned long long cap_out = c[0] + 16;
+	DevBuf d_list, d_count;
+	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
+	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
+	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, true, e->st)) return -1;
+	unsigned long long count = 0;
+	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	if (count > cap_out) count = cap_out;
+	std::vector<ExportEntry> list(count);
+	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list.p, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
+	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
+	std::vector<std::pair<unsigned long long, uint32_t>> recs;
+	for (const ExportEntry &x : list) recs.emplace_back(x.rec_off, x.len);
+	if (demote_records(e, recs)) return -1;
+	return compact_locked(e, nullptr);
+}
+
+extern "C" int cmb200_host_tier_stats(cmb200_engine *e, struct cmb200_host_tier_stats *out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	memset(out, 0, sizeof(*out));
+	const cmb200_engine::HostTier &t = e->tier;
+	if (!t.host) return 0;
+	unsigned long long c[8], d[2];
+	if (read_counters(e, c)) return -1;
+	CMB_CHECK(cudaMemcpy(d, t.d_ctr, sizeof(d), cudaMemcpyDeviceToHost));
+	out->bytes = t.size;
+	out->used = t.log.empty() ? 0 : t.head - t.log.front().first;
+	out->records = c[7]; out->garbage = c[6];
+	out->demoted_records = t.demoted_records; out->demoted_bytes = t.demoted_bytes;
+	out->retired_records = d[0]; out->hits = d[1];
 	return 0;
 }
 

@@ -159,6 +159,16 @@ __global__ void k_lookup(TableView t, const unsigned long long *addr, const uint
 	if (ts_out) ts_out[i] = ts;
 }
 
+// The bytes a slot's record held (s.alloc) become garbage of the tier they are in.
+__device__ __forceinline__ void slot_release(const ArenaView &a, const Slot &s) {
+	if (s.rec_off & REC_HOST) {
+		atomicAdd(a.tier, (unsigned long long)s.alloc);
+		atomicAdd(a.tier + 1, (unsigned long long)-1ll);
+	} else {
+		atomicAdd(a.garbage, (unsigned long long)s.alloc);
+	}
+}
+
 // filemap_unset (filemap.c:188-215): delete by key, whatever address the record holds.
 __global__ void k_unset(TableView t, ArenaView a, const unsigned long long *addr, uint32_t n) {
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -170,7 +180,7 @@ __global__ void k_unset(TableView t, ArenaView a, const unsigned long long *addr
 	uint32_t old = atomicExch(&s.vlen, 0u);
 	if (old == 0) return;
 	atomicAdd(t.entries, (unsigned long long)-1ll);
-	atomicAdd(a.garbage, (unsigned long long)s.alloc);
+	slot_release(a, s);
 	s.alloc = 0;
 	s.owner = 0;
 	if (idx < t.cap) {
@@ -242,12 +252,16 @@ __global__ void __launch_bounds__(256) k_sample_scan(TableView t, const unsigned
 // Points the slot at a finished record (one thread).  Order: location first, then the length that
 // makes the slot valid; readers on other streams take the length and the address from the record's
 // own prefix and only the location from the slot (k_get_small).
+// Invariant: rec_off is the only word of a slot that such a reader trusts, and it is always written
+// with ONE 8-byte store.  Demotion to the host tier (k_demote_publish) changes nothing else (vlen,
+// addr and ts stay), so a reader sees the old arena location or the new host location, never a mix;
+// the arena bytes stay intact until the next compaction, which closes get_gate.
 __device__ __forceinline__ void slot_publish(const EncodeJob &job, Slot &s, uint32_t i, uint32_t idx, unsigned long long off,
     uint32_t need, uint32_t clen, unsigned long long au, unsigned long long al, uint64_t fp_hi, uint64_t fp_lo) {
 	// whatever checkpoints the slot has describe the record it is leaving (ckpt_store renews them)
 	if (job.table.ckpt) *reinterpret_cast<volatile uint32_t *>(&job.table.ckpt[(size_t)idx * CKPT_WORDS]) = 0u;
 	if (s.owner) { atomicAdd(job.table.remote, (unsigned long long)-1ll); s.owner = 0; }   // now newest here (alloc held the remote length)
-	else if (s.alloc) atomicAdd(job.arena.garbage, (unsigned long long)s.alloc);         // the record this one replaces
+	else if (s.alloc) slot_release(job.arena, s);                                          // the record this one replaces
 	s.addr_u = au; s.addr_l = al;
 	s.ts = job.ts ? job.ts[i] : 0;
 	if (job.table.fp) { job.table.fp[2 * (size_t)idx] = fp_hi; job.table.fp[2 * (size_t)idx + 1] = fp_lo; }
@@ -620,7 +634,10 @@ __global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) {
 	uint8_t *out = job.pages + (size_t)i * job.nbytes;
 	if (job.rec_off) {                                  // store mode
 		if (job.status[i] != ST_HIT) return;
-		const uint8_t *rec = job.arena + job.rec_off[i];
+		const unsigned long long off = job.rec_off[i];
+		// host tier: mapped host memory, read over PCIe
+		const uint8_t *rec = (off & REC_HOST) ? job.host + (off & ~REC_HOST) : job.arena + off;
+		if ((off & REC_HOST) && lane == 0) atomicAdd(job.host_hits, 1ull);
 		uint32_t clen = job.vlen[i] - 1u;
 		if (clen == 0) {                            // raw page (filemap.c:249-251)
 			warp_copy_ro(out, rec + 24, job.nbytes, lane);
@@ -788,6 +805,7 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	}
 	uint32_t phase = 0;
 	int32_t result = ST_MISS;
+	bool from_host = false;                                     // the record read last came from the host tier
 	for (int attempt = 0; attempt < 4; attempt++) {
 		if (tid == 0) gs_lookup(job, u, l, sh);
 		__syncthreads();
@@ -800,6 +818,9 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 		const uint32_t tx = (24u + plen + 15u) & ~15u;
 		const uint8_t *base = job.arena;
 		uint64_t limit = job.arena_size + 256u;                  // every arena is allocated with 256 bytes of slack
+		from_host = st == ST_HIT && (off & REC_HOST);
+		if (from_host) { base = job.host; limit = job.host_size; }
+		const unsigned long long roff = off & ~REC_HOST;
 		bool ok = clen <= job.nbytes + 1024u && (off & 15u) == 0;
 		if (st == ST_REMOTE) {
 			base = owner - 1u < GET_MAX_PEERS ? job.peer[owner - 1u] : nullptr;
@@ -807,14 +828,15 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 			ok = ok && base != nullptr && clen != 0xffffffffu;
 			if (!ok) break;                                      // no path to the owner's arena: REMOTE is the answer
 		}
-		if (!ok || off + tx > limit) { result = ST_MISS; break; }
-		if (st == ST_HIT) {
+		if (!ok || roff + tx > limit) { result = ST_MISS; break; }
+		if (st == ST_HIT && !from_host) {
 			if (tid == 0) { mbar_expect_tx(s_bar, tx); tma_load_1d(smem_addr(rec), base + off, tx, s_bar); }
 			while (!mbar_try_wait(s_bar, phase)) {}
 			phase ^= 1u;
 		} else {
-			// the owner's arena over NVLink: plain 16-byte loads, no local L2 (peer lines are not cached there)
-			const uint4 *src = reinterpret_cast<const uint4 *>(base + off);
+			// the owner's arena over NVLink, or the host tier over PCIe: plain 16-byte loads (TMA is not
+			// used on mapped host memory), no local L2 (peer lines are not cached there)
+			const uint4 *src = reinterpret_cast<const uint4 *>(base + roff);
 			for (uint32_t k = tid; k < tx / 16u; k += GS_THREADS) reinterpret_cast<uint4 *>(rec)[k] = __ldcg(src + k);
 			__syncthreads();
 		}
@@ -876,6 +898,7 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	__syncthreads();
 	if (tid == 0) {
 		if (sh->region != 0xffffffffu) gs_region_give(job, sh->region);
+		if (result == ST_HIT && from_host) atomicAdd(job.host_hits, 1ull);
 		__threadfence_system();
 		*reinterpret_cast<volatile int32_t *>(&job.status[i]) = result;
 	}
@@ -1101,11 +1124,12 @@ int launch_read_fp(TableView t, const unsigned long long *addr, uint32_t n, uint
 }
 // ---- snapshot -----------------------------------------------------------------------------
 __global__ void k_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
-    unsigned long long max_out) {
+    unsigned long long max_out, bool arena_only) {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= t.cap + 2) return;
 	const Slot &s = t.slots[i];
 	if (s.vlen == 0 || s.owner != 0) return;        // empty / deleted / the record lives on another GPU
+	if (arena_only && (s.rec_off & REC_HOST)) return;
 	if (i < t.cap && (s.key == KEY_EMPTY || s.key == KEY_TOMB)) return;
 	const unsigned long long j = atomicAdd(count, 1ull);
 	if (j >= max_out) return;
@@ -1117,9 +1141,9 @@ __global__ void k_export_list(TableView t, uint32_t bsize, ExportEntry *out, uns
 	out[j] = e;
 }
 int launch_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
-    unsigned long long max_out, cudaStream_t st) {
+    unsigned long long max_out, bool arena_only, cudaStream_t st) {
 	const uint64_t n = t.cap + 2;
-	k_export_list<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, bsize, out, count, max_out);
+	k_export_list<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, bsize, out, count, max_out, arena_only);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
@@ -1173,6 +1197,88 @@ int launch_compact_window(TableView t, ArenaView a, const MoveEntry *moves, uint
 	k_compact_gather<<<(n * 32 + 255) / 256, 256, 0, st>>>(a, moves, n, bounce);
 	CMB_CHECK(cudaGetLastError());
 	k_compact_scatter<<<(n * 32 + 255) / 256, 256, 0, st>>>(t, a, moves, n, bounce);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+// ---- host tier ---------------------------------------------------------------------------------
+// Demotion: gather the records into the bounce buffer in tier order (one warp per record), let the copy
+// engine move the buffer to the tier, then repoint the slots.
+__global__ void __launch_bounds__(256) k_demote_gather(ArenaView a, const DemoteEntry *d, uint32_t n, uint8_t *bounce) {
+	const int lane = threadIdx.x & 31;
+	const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	if (i >= n) return;
+	const DemoteEntry m = d[i];
+	warp_copy_rw(bounce + m.bounce_off, a.base + m.old_off, m.len, lane);
+}
+__global__ void k_demote_publish(TableView t, ArenaView a, const DemoteEntry *d, uint32_t n) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const DemoteEntry m = d[i];
+	// the arena copy is intact until the next compaction: its prefix names the key
+	const unsigned long long *pre = reinterpret_cast<const unsigned long long *>(a.base + m.old_off);
+	const uint32_t idx = table_find(t, fnv_addr(pre[0], pre[1]));
+	if (idx == 0xffffffffu) return;
+	Slot &s = t.slots[idx];
+	if (s.vlen == 0 || s.owner != 0 || s.rec_off != m.old_off) return;   // not the record that was copied
+	const uint32_t clen = s.vlen - 1u;
+	const unsigned long long loc = REC_HOST | m.host_off;
+	atomicAdd(a.garbage, (unsigned long long)s.alloc);
+	atomicAdd(a.tier + 1, 1ull);
+	s.alloc = (m.len + 15u) & ~15u;
+	*reinterpret_cast<volatile unsigned long long *>(&s.rec_off) = loc;      // the one store readers trust
+	if (t.ckpt) {
+		// the block is unchanged, so are its checkpoints: only the tag moves to the new location
+		uint32_t *w = t.ckpt + (size_t)idx * CKPT_WORDS;
+		if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(m.old_off, clen)) {
+			__threadfence();
+			*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(loc, clen);
+		}
+	}
+}
+int launch_demote_gather(ArenaView a, const DemoteEntry *d, uint32_t n, uint8_t *bounce, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_demote_gather<<<(n * 32 + 255) / 256, 256, 0, st>>>(a, d, n, bounce);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_demote_publish(TableView t, ArenaView a, const DemoteEntry *d, uint32_t n, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_demote_publish<<<GRID1D(n), 0, st>>>(t, a, d, n);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+// Conditional unset of the records a wrap of the tier overwrites: rec[4i..4i+3] = {u, l, location, bytes}.
+__global__ void k_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
+    unsigned long long *retired) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const unsigned long long loc = rec[4 * (size_t)i + 2], bytes = rec[4 * (size_t)i + 3];
+	const uint32_t idx = table_find(t, fnv_addr(rec[4 * (size_t)i], rec[4 * (size_t)i + 1]));
+	if (idx != 0xffffffffu) {
+		Slot &s = t.slots[idx];
+		// a location names one record, so no two requests of a batch can both match
+		if (s.vlen != 0 && s.rec_off == loc) {
+			s.vlen = 0;
+			atomicAdd(t.entries, (unsigned long long)-1ll);        // an eviction, counted as k_unset counts it
+			atomicAdd(a.tier + 1, (unsigned long long)-1ll);
+			s.alloc = 0;
+			s.owner = 0;
+			if (idx < t.cap) {
+				s.key = KEY_TOMB;
+				atomicAdd(t.tombs, 1ull);
+			}
+			atomicAdd(retired, 1ull);
+			return;
+		}
+	}
+	atomicAdd(a.tier, 0ull - bytes);                         // a dead record: its bytes leave the tier's garbage
+}
+int launch_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
+    unsigned long long *retired, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_tier_retire<<<GRID1D(n), 0, st>>>(t, a, rec, n, retired);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

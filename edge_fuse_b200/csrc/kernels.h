@@ -12,9 +12,10 @@ struct Slot {
 	unsigned long long key;      // 0 = never used, ~0 = deleted; those two key values live in side slots
 	unsigned long long addr_u;   // stored address, verified on get (filemap.c:236-240)
 	unsigned long long addr_l;
-	unsigned long long rec_off;  // arena offset of {24-byte data_prefix, payload} (filemap.c:140-147)
+	unsigned long long rec_off;  // location of {24-byte data_prefix, payload} (filemap.c:140-147): arena
+	                             // offset, or REC_HOST | offset in the host tier
 	uint32_t vlen;               // 0 = no valid record, else compressed_length + 1 (0+1 = raw page)
-	uint32_t alloc;              // arena bytes reserved at rec_off
+	uint32_t alloc;              // bytes reserved at rec_off (arena or host tier)
 	unsigned long long ts;       // LMDB node attribute of the reference
 	unsigned long long seq;      // stream order of the last put that claimed this key
 	unsigned long long owner;    // 0 = record (if any) is in this GPU's arena; r+1 = key last written on rank r
@@ -23,6 +24,11 @@ static_assert(sizeof(Slot) == 64, "slot layout");
 
 constexpr unsigned long long KEY_EMPTY = 0ull;
 constexpr unsigned long long KEY_TOMB = ~0ull;
+
+// Bit 63 of Slot::rec_off: the record lives in the host tier (page-locked, device-mapped host memory)
+// at offset rec_off & ~REC_HOST, in the same format as in the arena.  A record moves from the arena
+// to the host tier only (cmb200_demote_batch), by one 8-byte store of rec_off.
+constexpr unsigned long long REC_HOST = 1ull << 63;
 
 struct TableView {
 	Slot *slots;                 // cap + 2 entries; [cap] holds key 0, [cap+1] holds key ~0
@@ -40,8 +46,10 @@ struct TableView {
 // that sixteenth.  Written by the encoder (kernels.cu:ckpt_store), read by k_get_small.
 constexpr uint32_t CKPT_WORDS = 16;
 constexpr uint32_t CKPT_POS_BITS = 13;       // n/16 <= 8192 for pages up to 128 KiB
+// Bit 30 of the tag is the record's tier, so a tag never names a record in the other tier.
 __host__ __device__ inline uint32_t ckpt_tag(unsigned long long rec_off, uint32_t clen) {
-	return 0x80000000u | (((uint32_t)(rec_off >> 4) ^ (clen * 0x9E3779B1u)) & 0x7fffffffu);
+	return 0x80000000u | ((uint32_t)(rec_off >> 33) & 0x40000000u) |
+	    (((uint32_t)(rec_off >> 4) ^ (clen * 0x9E3779B1u)) & 0x3fffffffu);
 }
 
 #define ARENA_SEG_SLOTS 4096u    // resident encoder warps that can own an arena segment
@@ -52,6 +60,7 @@ struct ArenaView {
 	unsigned long long *head;     // bump pointer
 	unsigned long long *garbage;  // bytes orphaned by relocated / deleted records
 	unsigned long long *dropped;  // puts dropped because the arena was full (filemap.c:154-157 analogue)
+	unsigned long long *tier;     // host tier: [0] = garbage bytes, [1] = live records
 	// direct encode (large arenas): every resident encoder warp owns a segment of the arena and
 	// writes blocks straight into it; seg[2w] = cursor, seg[2w+1] = end of warp slot w's segment
 	unsigned long long *seg;
@@ -110,6 +119,8 @@ struct DecodeJob {
 	const uint64_t *rec_off;     // per request, from lookup
 	const uint32_t *vlen;
 	const uint8_t *arena;
+	const uint8_t *host;         // device address of the host tier (null: no tier)
+	unsigned long long *host_hits;
 };
 int launch_decode(const DecodeJob &job, cudaStream_t st);
 
@@ -123,6 +134,9 @@ struct GetJob {
 	TableView table;
 	const uint8_t *arena;
 	uint64_t arena_size;
+	const uint8_t *host;              // device address of the host tier (null: no tier)
+	uint64_t host_size;
+	unsigned long long *host_hits;
 	const unsigned long long *addr;   // n x {u, l}
 	const uint8_t *valid;             // optional
 	uint32_t n;
@@ -204,8 +218,9 @@ struct ExportEntry {
 	uint32_t slot;
 };
 static_assert(sizeof(ExportEntry) == 40, "export entry layout");
+// arena_only: leave out the records of the host tier (compaction moves arena records only)
 int launch_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
-    unsigned long long max_out, cudaStream_t st);
+    unsigned long long max_out, bool arena_only, cudaStream_t st);
 // Restores n records {24-byte prefix, payload} lying at blob + off[i]; slot_idx from launch_upsert
 // on the records' addresses (job.addr / job.ts / job.table / job.arena / job.seq0 as for a put).
 int launch_restore(const EncodeJob &job, const uint8_t *blob, const unsigned long long *off,
@@ -219,6 +234,21 @@ struct MoveEntry { unsigned long long old_off, new_off; uint32_t len, slot; };
 static_assert(sizeof(MoveEntry) == 24, "move entry layout");
 int launch_compact_window(TableView t, ArenaView a, const MoveEntry *moves, uint32_t n, uint8_t *bounce,
     cudaStream_t st);
+
+// ---- host tier (cmb200_demote_batch) ----
+// One record moving from the arena to the host tier: gathered from the arena into the bounce buffer at
+// bounce_off, copied to the tier by the copy engine, then published at host_off.
+struct DemoteEntry { unsigned long long old_off, host_off, bounce_off; uint32_t len, pad; };
+static_assert(sizeof(DemoteEntry) == 32, "demote entry layout");
+int launch_demote_gather(ArenaView a, const DemoteEntry *d, uint32_t n, uint8_t *bounce, cudaStream_t st);
+// Repoints each slot that still holds old_off to REC_HOST | host_off and moves its bytes from arena
+// garbage accounting to the tier's.
+int launch_demote_publish(TableView t, ArenaView a, const DemoteEntry *d, uint32_t n, cudaStream_t st);
+// Records of the tier that are about to be overwritten: {u, l, REC_HOST | offset, bytes}.  A key whose
+// slot still points at that exact location is unset (an eviction); otherwise the bytes leave the
+// tier's garbage.  *retired counts the unset keys.
+int launch_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
+    unsigned long long *retired, cudaStream_t st);
 
 // Re-inserts every live slot of `from` into the (zeroed) table `to` of the same geometry.
 int launch_rehash(TableView from, TableView to, cudaStream_t st);

@@ -159,6 +159,31 @@ int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out);
 int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records_out);
 int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out);
 
+/* ---- host tier: records beyond the HBM arena ----------------------------------------------------
+ * The reference keeps `capacity` pages in LMDB files on SSD; here the store is an HBM arena, which can
+ * be far smaller than what `capacity` pages need.  A host tier is page-locked, device-mapped host
+ * memory that holds records demoted from the arena, byte for byte in the same format (24-byte
+ * data_prefix + payload).  Gets read them over PCIe and answer CMB200_HIT as for any record; keys,
+ * records, statuses and counters do not depend on the tier a record is in.
+ * cmb200_host_tier_enable allocates `bytes` of it: once, before the first put, and never on an engine
+ * that has made a multi-GPU call (cmb200_set_stream_order, cmb200_put_step, cmb200_import_*,
+ * cmb200_arena_ipc_handle, cmb200_open_peer); those calls in turn fail on an engine with a tier.
+ * cmb200_demote_batch moves the arena records of the named keys to the tier (*demoted_out = how many);
+ * keys that are absent, remote or already in the tier are skipped.  Their arena bytes become
+ * arena_garbage.  The tier is a ring in demotion order: when it comes round, the keys whose records
+ * it overwrites are unset, an eviction like cmb200_unset_batch (retired_records).  A record leaves
+ * the tier when it is unset, overwritten or retired; promotion back to the arena does not exist. */
+struct cmb200_host_tier_stats {
+	uint64_t bytes, used, records, garbage;     /* tier size; bytes between oldest and newest record; live records; dead bytes */
+	uint64_t demoted_records, demoted_bytes;    /* moved from the arena so far (bytes = record lengths) */
+	uint64_t retired_records;                   /* keys unset because the ring overwrote their records */
+	uint64_t hits;                              /* gets answered from the tier */
+};
+int cmb200_host_tier_enable(cmb200_engine *e, uint64_t bytes);
+int cmb200_demote_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *demoted_out);
+/* all zero for an engine without a tier */
+int cmb200_host_tier_stats(cmb200_engine *e, struct cmb200_host_tier_stats *out);
+
 /* ---- multi-GPU: chunks sharded round-robin over ranks, one replicated key index per GPU ----
  * Each rank puts its own shard with the chunks' GLOBAL stream positions as sequence numbers
  * (next_seq = position of the rank's next chunk, stride = world size), then the ranks all-gather
