@@ -72,18 +72,29 @@ template <> struct Lz4Table<true> {
 // aligned loads (page buffers are padded past their end; the word before the page start is never
 // needed because backward extension is capped by the position itself).
 struct Lz4Around { uint32_t before, at, next; };
-__device__ __forceinline__ Lz4Around lz4_around(const uint8_t *src, uint32_t p) {
-	const uint32_t a = p & ~3u, sh = (p & 3u) * 8u;
+// The same in two halves, the loads and the byte alignment, for a caller that has other work to
+// do while the loads are in flight.
+struct Lz4Words { uint32_t w0, w1, w2, w3, sh; };
+__device__ __forceinline__ Lz4Words lz4_around_load(const uint8_t *src, uint32_t p) {
+	const uint32_t a = p & ~3u;
 	const uint32_t *q = reinterpret_cast<const uint32_t *>(src + a);
 	// p < 4: the word before the page does not exist and is not needed (backward extension is capped
 	// by the position), so the first word is read twice instead of branching
-	const uint32_t w0 = __ldg(q - (a != 0u));
-	const uint32_t w1 = __ldg(q), w2 = __ldg(q + 1), w3 = __ldg(q + 2);
+	Lz4Words w;
+	w.w0 = __ldg(q - (a != 0u));
+	w.w1 = __ldg(q); w.w2 = __ldg(q + 1); w.w3 = __ldg(q + 2);
+	w.sh = (p & 3u) * 8u;
+	return w;
+}
+__device__ __forceinline__ Lz4Around lz4_around_align(const Lz4Words &w) {
 	Lz4Around r;
-	r.before = __funnelshift_r(w0, w1, sh);
-	r.at = __funnelshift_r(w1, w2, sh);
-	r.next = __funnelshift_r(w2, w3, sh);
+	r.before = __funnelshift_r(w.w0, w.w1, w.sh);
+	r.at = __funnelshift_r(w.w1, w.w2, w.sh);
+	r.next = __funnelshift_r(w.w2, w.w3, w.sh);
 	return r;
+}
+__device__ __forceinline__ Lz4Around lz4_around(const uint8_t *src, uint32_t p) {
+	return lz4_around_align(lz4_around_load(src, p));
 }
 
 // ---- rare paths, kept out of line ------------------------------------------------------------
@@ -94,6 +105,12 @@ __device__ __noinline__ uint32_t lz4_emit_len(uint8_t *dst, uint32_t op, uint32_
 	for (uint32_t i = lane; i < nff; i += 32) dst[op + i] = 0xFF;
 	if (lane == 0) dst[op + nff] = (uint8_t)(count - nff * 255u);
 	return op + nff + 1;
+}
+// The number of bytes lz4_emit_len writes for a token field that holds `count` (none below 15).
+__device__ __forceinline__ uint32_t lz4_len_bytes(uint32_t count) { return count >= 15u ? (count - 15u) / 255u + 1u : 0u; }
+// Size of a whole sequence: token, literal length bytes, literals, offset, match length bytes.
+__device__ __forceinline__ uint32_t lz4_seq_bytes(uint32_t lit, uint32_t mc) {
+	return 3u + lit + lz4_len_bytes(lit) + lz4_len_bytes(mc);
 }
 
 __device__ __noinline__ void lz4_copy_literals(uint8_t *dst, const uint8_t *src, uint32_t len, int lane) {
@@ -217,6 +234,39 @@ __device__ __noinline__ uint32_t lz4_emit_general(uint8_t *dst, uint32_t op, con
 	op += 2;
 	if (mc >= 15u) op = lz4_emit_len(dst, op, mc - 15u, lane);
 	return op;
+}
+
+// Byte store of encoder output (global memory) as ONE predicated instruction.  Inside the encoder
+// loop's conditional emit the compiler otherwise branches around each store and recomputes its
+// address behind the branch.
+__device__ __forceinline__ void st_out8_if(bool p, uint8_t *ptr, uint32_t v) {
+	asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.u32 q, %2, 0;\n\t@q st.global.u8 [%0], %1;\n\t}" ::"l"(
+	                 __cvta_generic_to_global(ptr)), "r"(v), "r"((uint32_t)p)
+	             : "memory");
+}
+
+// Writes one sequence — token, literal run, offset and match length (lz4.c:625-683) — at dst[op..),
+// lz4_seq_bytes(lit, mc) bytes.  A run of at most 64 literals comes from registers (b0 = src[from +
+// lane], b1 = src[from + 32 + lane], loaded by the batch that found the match) and is written by
+// predicated lane stores; longer runs and long lengths go to lz4_emit_general, which reads the
+// literals from the page in global memory.
+__device__ __forceinline__ void lz4_emit_seq(uint8_t *dst, const uint8_t *src, uint32_t op, uint32_t from, uint32_t lit,
+    uint32_t off, uint32_t mc, uint32_t b0, uint32_t b1, int lane) {
+	if (lit <= 64u && mc < 15u + 255u) {
+		uint8_t *o = dst + op;
+		const uint32_t lext = lit >= 15u, mext = mc >= 15u;
+		const uint32_t hl = 1u + lext;
+		st_out8_if((uint32_t)lane < lit, o + hl + lane, b0);
+		st_out8_if((uint32_t)lane + 32u < lit, o + hl + 32u + lane, b1);
+		const uint32_t tail = hl + lit;
+		const uint32_t head4 = (min(lit, 15u) << 4) | min(mc, 15u) | (((lit - 15u) & 0xffu) << 8) | (off << 16);
+		const uint32_t val = lane < 4 ? head4 >> (8u * (uint32_t)lane) : mc - 15u;
+		const uint32_t at = lane < 2 ? (uint32_t)lane : tail + (uint32_t)lane - 2u;
+		const uint32_t owners = 0x0du | (lext << 1) | (mext << 4);
+		st_out8_if((owners >> lane) & 1u, o + at, val);
+	} else {
+		lz4_emit_general(dst, op, src, from, lit, off, mc, lane);
+	}
 }
 
 // The encoder loop itself is lz4_encode_lean (lz4_encode_ring.cuh).

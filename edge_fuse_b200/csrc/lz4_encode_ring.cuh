@@ -226,12 +226,19 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 		constexpr int NARROW_HIT = 12;                                     // a hit at or above this lane widens the batch again
 		uint32_t width = 32u, calm = 0u;                                    // lanes per batch; batches in a row that hit below NARROW_HIT
 		uint32_t next_event = 0, ring_next = 0;                            // anchor at which the frontiers move next / a checkpoint is due
+		// The sequence a batch resolves is written by the NEXT iteration, behind that batch's candidate
+		// reads: the emit's stores and arithmetic (its size included) then fill the L2 round trip instead
+		// of standing between one batch and the next.  From the top of an iteration to its deferred
+		// emit, if `started`, one sequence is pending: it starts at dst[op] and at page position
+		// anchor - LZ4_MIN_MATCH - p_mc - p_lit, and its first 64 literal bytes are in litbyte / litbyte2.
+		uint32_t p_lit = 0, p_off = 0, p_mc = 0, litbyte = 0, litbyte2 = 0;
 		for (;;) {
 			if (anchor >= next_event) {
 				// a sequence starts at or after the next checkpoint position: this is the one to note
 				while (anchor >= ck_at) {
 					const uint32_t rel = anchor - ck_at;
-					if ((uint32_t)lane == ck_k) ck = rel < ck_span ? (op << CKPT_POS_BITS) | rel : 0xffffffffu;
+					const uint32_t at = op + (started ? lz4_seq_bytes(p_lit, p_mc) : 0u);   // behind the pending one
+					if ((uint32_t)lane == ck_k) ck = rel < ck_span ? (at << CKPT_POS_BITS) | rel : 0xffffffffu;
 					ck_k++;
 					ck_at = ck_k < CKPT_WORDS ? ck_at + ck_span : 0xffffffffu;
 				}
@@ -268,19 +275,7 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 			}
 			const bool en = anchor < en_below && (uint32_t)lane < width;
 			const uint32_t pos = en ? anchor + delta2 : 0u;        // disabled lanes read (and ignore) position 0 / ring offset 0
-			// speculative literal bytes: src[anchor + lane], src[anchor + 32 + lane] (used when the run is <= 64 bytes;
-			// never stored beyond the literal run, so reading past the page end is harmless in the ring)
-			uint32_t litbyte, litbyte2;
-			Lz4Around ai;
-			if (RING) {
-				litbyte = rb[(anchor + (uint32_t)lane) & (RING_BYTES - 1u)];
-				litbyte2 = rb[(anchor + 32u + (uint32_t)lane) & (RING_BYTES - 1u)];
-				ai = ring_around(rb, pos);
-			} else {
-				litbyte = ldg8(src + min(anchor + (uint32_t)lane, n - 1u));
-				litbyte2 = ldg8(src + min(anchor + 32u + (uint32_t)lane, n - 1u));
-				ai = lz4_around(src, pos);
-			}
+			const Lz4Around ai = RING ? ring_around(rb, pos) : lz4_around(src, pos);
 
 			// ---- unified batch ----
 			const uint32_t pseq = ai.at;
@@ -289,9 +284,31 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 			__syncwarp();
 			if (en) tab.put(h, pos);                                // speculative commit
 			__syncwarp();
-			const Lz4Around ac = lz4_around(src, cand);   // latency overlaps the read-back
+			Lz4Words acw = lz4_around_load(src, cand);   // latency overlaps the read-back and the emit below
 			const uint32_t seen = tab.get(h);
 			__syncwarp();                                           // read-backs done before any undo store
+
+			// ---- deferred emit of the pending sequence, while the candidate reads are in flight ----
+			// It needs nothing of this batch: the fast path stores registers only, lz4_emit_general reads
+			// the page from global memory (never from the ring, whose buffers the loop head recycles).
+			if (started) {
+				lz4_emit_seq(dst, src, op, anchor - LZ4_MIN_MATCH - p_mc - p_lit, p_lit, p_off, p_mc, litbyte, litbyte2, lane);
+				op += lz4_seq_bytes(p_lit, p_mc);
+			}
+			// speculative literal bytes of the sequence this batch resolves: src[anchor + lane],
+			// src[anchor + 32 + lane] (used when the run is <= 64 bytes; never stored beyond the literal
+			// run, so reading past the page end is harmless in the ring)
+			if (RING) {
+				litbyte = rb[(anchor + (uint32_t)lane) & (RING_BYTES - 1u)];
+				litbyte2 = rb[(anchor + 32u + (uint32_t)lane) & (RING_BYTES - 1u)];
+			} else {
+				litbyte = ldg8(src + min(anchor + (uint32_t)lane, n - 1u));
+				litbyte2 = ldg8(src + min(anchor + 32u + (uint32_t)lane, n - 1u));
+			}
+			// The candidate words are first used here, behind the emit (the compiler would otherwise align
+			// them right after the loads, and the warp would wait for the L2 before emitting).
+			asm volatile("" : "+r"(acw.w0), "+r"(acw.w1), "+r"(acw.w2), "+r"(acw.w3));
+			const Lz4Around ac = lz4_around_align(acw);
 			const bool foreign = en && seen != (WIDE ? pos : (pos & 0xffffu));
 			bool hit = en && lane != 0 && ac.at == pseq;
 			if (WIDE) hit = hit && cand + LZ4_FAR >= pos;           // byU16: every distance fits (lz4.c:617)
@@ -340,40 +357,30 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 				} else if (enmask == CMB_FULL) {                     // the probes of this batch were not enough
 					res = lz4_search_slow<WIDE>(src, lim4, tab, anchor, 2u, accel, mflimit, w0, lane, started);
 				}
-				if (!(res >> 63)) break;                             // -> last literals
+				if (!(res >> 63)) break;                             // -> last literals (nothing pending)
 				retest_hit = (res >> 62) & 1u;
 				ip = (uint32_t)(res >> 32) & 0x3fffffffu;
 				match = (uint32_t)res;
 				fwd = lz4_count_long(src, ip + LZ4_MIN_MATCH, match + LZ4_MIN_MATCH, mlimit, lim4, lane);
 				back = retest_hit ? 0u : lz4_catchup_long(src, ip, match, anchor, lane);
 			}
-			const uint32_t off = ip - match;
-			const uint32_t mc = back + fwd;               // lz4.c:660 matchCode
-			const uint32_t lit = ip - back - anchor;
+			// ---- the sequence becomes the pending one (emitted by the next iteration) ----
+			p_off = ip - match;
+			p_mc = back + fwd;                            // lz4.c:660 matchCode
+			p_lit = ip - back - anchor;
 			const uint32_t end = ip + LZ4_MIN_MATCH + fwd;
-
-			// ---- emit: token, literal run (lz4.c:625-641), offset + match length (lz4.c:643-683) ----
-			if (lit <= 64u && mc < 15u + 255u) {
-				uint8_t *o = dst + op;
-				const uint32_t lext = lit >= 15u, mext = mc >= 15u;
-				const uint32_t hl = 1u + lext;
-				if ((uint32_t)lane < lit) st_out8(o + hl + lane, litbyte);
-				if ((uint32_t)lane + 32u < lit) st_out8(o + hl + 32u + lane, litbyte2);
-				const uint32_t tail = hl + lit;
-				const uint32_t head4 = (min(lit, 15u) << 4) | min(mc, 15u) | (((lit - 15u) & 0xffu) << 8) | (off << 16);
-				const uint32_t val = lane < 4 ? head4 >> (8u * (uint32_t)lane) : mc - 15u;
-				const uint32_t at = lane < 2 ? (uint32_t)lane : tail + (uint32_t)lane - 2u;
-				const uint32_t owners = 0x0du | (lext << 1) | (mext << 4);
-				if ((owners >> lane) & 1u) st_out8(o + at, val);
-				op += tail + 2u + mext;
-			} else {
-				op = lz4_emit_general(dst, op, src, anchor, lit, off, mc, lane);
-			}
 
 			anchor = end;
 			started = true;
 			en_below |= special_on;
 			if (end > mflimit) break;                     // lz4.c:688
+		}
+		// Still pending when the loop stopped at the end margin (anchor = end > mflimit).  A search that
+		// ran into the margin has already emitted its predecessor (its anchor is <= mflimit).  Either way
+		// the whole block is written before this function returns (and dst may be the arena).
+		if (started && anchor > mflimit) {
+			lz4_emit_seq(dst, src, op, anchor - LZ4_MIN_MATCH - p_mc - p_lit, p_lit, p_off, p_mc, litbyte, litbyte2, lane);
+			op += lz4_seq_bytes(p_lit, p_mc);
 		}
 		if (RING) ring_drain(ring);
 	}
