@@ -668,6 +668,7 @@ constexpr uint32_t GS_THREADS = DC_THREADS;       // 16 warps: one per parse sec
 constexpr uint32_t GS_CTRL = 128 + 1152;          // control block + decoder state at the start of the shared memory
 static_assert(sizeof(DecodeCta) <= 1152, "decoder state fits its slot");
 constexpr uint32_t GS_MAX_PAGE = 65536;           // record buffer + page buffer must fit 227 KiB
+constexpr uint32_t GS_PAIR_MAX_PAGE = 131072;     // k_get_small_pair: one buffer per CTA of a cluster of two
 struct GetShared {
 	unsigned long long bar;                   // mbarrier of the record copy
 	unsigned long long off;                   // arena offset of the record
@@ -681,8 +682,10 @@ struct GetShared {
 };
 static_assert(sizeof(GetShared) <= 128, "control block");
 __host__ __device__ inline uint32_t gs_recbuf(uint32_t nbytes) { return (24u + nbytes + 1024u + 31u) & ~15u; }
-bool get_small_supports(uint32_t nbytes) { return nbytes >= 64u && nbytes <= GS_MAX_PAGE && (nbytes & 15u) == 0; }
-size_t get_small_smem(uint32_t nbytes) { return GS_CTRL + gs_recbuf(nbytes) + nbytes; }
+bool get_small_supports(uint32_t nbytes) { return nbytes >= 64u && nbytes <= GS_PAIR_MAX_PAGE && (nbytes & 15u) == 0; }
+size_t get_small_smem(uint32_t nbytes) {                      // per CTA
+	return nbytes > GS_MAX_PAGE ? GS_CTRL + gs_recbuf(nbytes) : GS_CTRL + gs_recbuf(nbytes) + nbytes;
+}
 uint32_t get_small_region_entries(uint32_t nbytes) { return dc_region(nbytes); }
 
 __device__ __forceinline__ unsigned long long ldv64(const unsigned long long *p) { return *reinterpret_cast<const volatile unsigned long long *>(p); }
@@ -873,7 +876,7 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 		for (int pass = 0; pass < 2 && !good; pass++) {
 			const bool many = sh->sections > 1u;
 			if (dc->ip0[warp] != 0xffffffffu)
-				dc_parse_chain(dc, warp, blk_s, clen, job.nbytes, desc + (size_t)warp * stride,
+				dc_parse_chain<false>(dc, warp, blk_s, clen, job.nbytes, desc + (size_t)warp * stride,
 				    many ? stride : job.region_entries, lane);
 			__syncthreads();
 			good = gs_sections_fit(dc, clen, job.nbytes);
@@ -884,9 +887,9 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 			__syncthreads();
 		}
 		if (!good) { result = ST_BAD_DECODE; break; }             // filemap.c:244-248
-		dc_literals(dc, desc, stride, blk_s, page_s, rec + 24, page, warp, lane);
+		dc_literals<false>(dc, desc, stride, blk_s, page_s, rec + 24, page, warp, lane);
 		__syncthreads();
-		if (warp == 0) dc_matches(dc, desc, stride, page_s, lane);
+		if (warp == 0) dc_matches<false>(dc, desc, stride, page_s, lane);
 		__syncthreads();
 		for (uint32_t k = tid; k < job.nbytes / 16u; k += GS_THREADS)
 			reinterpret_cast<uint4 *>(out)[k] = reinterpret_cast<const uint4 *>(page)[k];
@@ -904,9 +907,194 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	}
 }
 
+// ---- pages above 64 KiB: one request per cluster of two CTAs ----------------------------------------
+// The record and the page together (264 KiB at 128 KiB pages) exceed the 227 KiB one CTA may have, so
+// the request is split over a cluster of two with the same shared-memory layout (DESIGN.md §5):
+//   rank 0, the RECORD CTA: lookup, staging, prefix check and retries exactly as k_get_small, the parse
+//           on the block in its own shared memory, then the literal phase, which stores the runs into
+//           the page CTA over DSMEM.  Raw pages go straight to `out`.  Every decision is taken here.
+//   rank 1, the PAGE CTA: holds the page at the record buffer's offset.  Given the record CTA's
+//           verdict it runs the match phase on its own shared memory, writes the page out, then the
+//           status.  It is the one CTA that answers: region release, host-tier hit, status word.
+// Two cluster barrier phases.  A: both CTAs arrive at entry, and the record CTA waits for A before
+// its first remote store, so the page CTA has started.  B: the record CTA arrives with release after
+// its last remote store and global write, the page CTA waits with acquire: literals, descriptors,
+// counts and verdict are visible before the match phase.  Only the page CTA's shared memory is
+// accessed remotely, and it waits for B, so no CTA exits while its partner can still reach it.
+struct PairVerdict {                              // the page CTA's control block, written by the record CTA
+	int32_t result;
+	uint32_t region;                          // scratch region of the descriptors (~0: none)
+	uint32_t decode;                          // 1: the literals are in the page, the matches are not
+	uint32_t from_host;                       // the record came from the host tier
+};
+static_assert(sizeof(PairVerdict) <= 128, "control block");
+
+__device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+__device__ __forceinline__ void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed;" ::: "memory"); }
+__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
+// shared::cluster address / generic address of the same location in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t dsmem_map(uint32_t a, uint32_t rank) {
+	uint32_t r;
+	asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(a), "r"(rank));
+	return r;
+}
+__device__ __forceinline__ uint8_t *dsmem_map_generic(uint8_t *p, uint32_t rank) {
+	uint64_t r;
+	asm volatile("mapa.u64 %0, %1, %2;" : "=l"(r) : "l"(p), "r"(rank));
+	return reinterpret_cast<uint8_t *>(r);
+}
+__device__ __forceinline__ void dsmem_st32(uint32_t a, uint32_t v) { asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get_small_pair(GetJob job) {
+	extern __shared__ __align__(128) uint8_t smem[];
+	DecodeCta *dc = reinterpret_cast<DecodeCta *>(smem + 128);
+	uint8_t *buf = smem + GS_CTRL;                              // record CTA: the record; page CTA: the page
+	const uint32_t i = blockIdx.x >> 1, tid = threadIdx.x, rank = cluster_rank();
+	const int lane = tid & 31;
+	const uint32_t warp = tid >> 5;
+	uint8_t *out = job.out + (size_t)i * job.nbytes;
+	const uint32_t stride = dc_stride(job.nbytes);
+	if (job.valid && !job.valid[i]) { if (rank == 1u && tid == 0) job.status[i] = ST_INVALID; return; }
+	cluster_arrive_relaxed();                                   // A
+	if (rank == 1u) {
+		const PairVerdict *v = reinterpret_cast<const PairVerdict *>(smem);
+		cluster_wait();                                     // A
+		cluster_arrive_relaxed();                           // B
+		cluster_wait();                                     // B: the record CTA is done with this CTA
+		if (v->decode) {
+			if (warp == 0) dc_matches<true>(dc, job.scratch + (size_t)v->region * job.region_entries, stride, smem_addr(buf), lane);
+			__syncthreads();
+			for (uint32_t k = tid; k < job.nbytes / 16u; k += GS_THREADS)
+				reinterpret_cast<uint4 *>(out)[k] = reinterpret_cast<const uint4 *>(buf)[k];
+		}
+		// the page first, then the status (as k_get_small; a raw page was written by the record CTA
+		// before it arrived at B, and this thread acquired B)
+		__syncthreads();
+		if (tid == 0) {
+			if (v->region != 0xffffffffu) gs_region_give(job, v->region);
+			if (v->result == ST_HIT && v->from_host) atomicAdd(job.host_hits, 1ull);
+			__threadfence_system();
+			*reinterpret_cast<volatile int32_t *>(&job.status[i]) = v->result;
+		}
+		return;
+	}
+	GetShared *sh = reinterpret_cast<GetShared *>(smem);
+	uint8_t *rec = buf;
+	const unsigned long long u = job.addr[2 * (size_t)i], l = job.addr[2 * (size_t)i + 1];
+	const uint32_t s_bar = smem_addr(&sh->bar);
+	if (tid == 0) {
+		sh->region = 0xffffffffu;
+		mbar_init(s_bar, 1u);
+		asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+		asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+	}
+	uint32_t phase = 0;
+	int32_t result = ST_MISS;
+	bool from_host = false, decode = false;
+	for (int attempt = 0; attempt < 4; attempt++) {
+		if (tid == 0) gs_lookup(job, u, l, sh);
+		__syncthreads();
+		const int32_t st = sh->st;
+		const uint32_t clen = sh->clen, owner = sh->owner;
+		const unsigned long long off = sh->off;
+		result = st;
+		if (st != ST_HIT && st != ST_REMOTE) break;
+		const uint32_t plen = clen ? clen : job.nbytes;
+		const uint32_t tx = (24u + plen + 15u) & ~15u;
+		const uint8_t *base = job.arena;
+		uint64_t limit = job.arena_size + 256u;
+		from_host = st == ST_HIT && (off & REC_HOST);
+		if (from_host) { base = job.host; limit = job.host_size; }
+		const unsigned long long roff = off & ~REC_HOST;
+		bool ok = clen <= job.nbytes + 1024u && (off & 15u) == 0;
+		if (st == ST_REMOTE) {
+			base = owner - 1u < GET_MAX_PEERS ? job.peer[owner - 1u] : nullptr;
+			limit = owner - 1u < GET_MAX_PEERS ? job.peer_size[owner - 1u] + 256u : 0;
+			ok = ok && base != nullptr && clen != 0xffffffffu;
+			if (!ok) break;
+		}
+		if (!ok || roff + tx > limit) { result = ST_MISS; break; }
+		if (st == ST_HIT && !from_host) {
+			if (tid == 0) { mbar_expect_tx(s_bar, tx); tma_load_1d(smem_addr(rec), base + off, tx, s_bar); }
+			while (!mbar_try_wait(s_bar, phase)) {}
+			phase ^= 1u;
+		} else {
+			const uint4 *src = reinterpret_cast<const uint4 *>(base + roff);
+			for (uint32_t k = tid; k < tx / 16u; k += GS_THREADS) reinterpret_cast<uint4 *>(rec)[k] = __ldcg(src + k);
+			__syncthreads();
+		}
+		const unsigned long long pu = *reinterpret_cast<const unsigned long long *>(rec);
+		const unsigned long long pl = *reinterpret_cast<const unsigned long long *>(rec + 8);
+		const uint32_t pclen = *reinterpret_cast<const uint32_t *>(rec + 16);
+		if (pu != u || pl != l || pclen != clen) {
+			result = ST_MISS;
+			__syncthreads();
+			if (st == ST_REMOTE) break;
+			continue;
+		}
+		if (clen == 0u) {
+			for (uint32_t k = tid; k < job.nbytes / 8u; k += GS_THREADS)
+				reinterpret_cast<unsigned long long *>(out)[k] = reinterpret_cast<const unsigned long long *>(rec + 24)[k];
+			result = ST_HIT;
+			break;
+		}
+		if (tid == 0) {
+			if (sh->region == 0xffffffffu) sh->region = gs_region_take(job);
+			gs_sections(job, sh, dc, clen, st == ST_HIT);
+		}
+		__syncthreads();
+		if (sh->region == 0xffffffffu) { result = ST_BAD_DECODE; break; }
+		uint4 *desc = job.scratch + (size_t)sh->region * job.region_entries;
+		const uint32_t blk_s = smem_addr(rec + 24);
+		bool good = false;
+		for (int pass = 0; pass < 2 && !good; pass++) {
+			const bool many = sh->sections > 1u;
+			if (dc->ip0[warp] != 0xffffffffu)
+				dc_parse_chain<true>(dc, warp, blk_s, clen, job.nbytes, desc + (size_t)warp * stride,
+				    many ? stride : job.region_entries, lane);
+			__syncthreads();
+			good = gs_sections_fit(dc, clen, job.nbytes);
+			if (good || !many) break;
+			__syncthreads();
+			if (tid == 0) gs_sections(job, sh, dc, clen, false);
+			__syncthreads();
+		}
+		result = good ? ST_HIT : ST_BAD_DECODE;
+		decode = good;
+		break;
+	}
+	cluster_wait();                                             // A: the page CTA has started
+	const uint32_t region = sh->region;
+	if (decode) {
+		dc_literals<true>(dc, job.scratch + (size_t)region * job.region_entries, stride, smem_addr(rec + 24),
+		    dsmem_map(smem_addr(buf), 1u), rec + 24, dsmem_map_generic(buf, 1u), warp, lane);
+		if (tid < DC_CHAINS) dsmem_st32(dsmem_map(smem_addr(&dc->cnt[tid]), 1u), dc->cnt[tid]);
+	}
+	if (tid == 0) {
+		const uint32_t v = dsmem_map(smem_addr(smem), 1u);
+		dsmem_st32(v + offsetof(PairVerdict, result), (uint32_t)result);
+		dsmem_st32(v + offsetof(PairVerdict, region), region);
+		dsmem_st32(v + offsetof(PairVerdict, decode), decode ? 1u : 0u);
+		dsmem_st32(v + offsetof(PairVerdict, from_host), from_host ? 1u : 0u);
+	}
+	cluster_arrive_release();                                   // B
+	cluster_wait();
+}
+
 int launch_get_small(const GetJob &job, cudaStream_t st) {
 	if (job.n == 0) return 0;
 	const size_t smem = get_small_smem(job.nbytes);
+	if (job.nbytes > GS_MAX_PAGE) {
+		static size_t configured_pair = 0;
+		if (smem > configured_pair) {
+			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+			configured_pair = smem;
+		}
+		k_get_small_pair<<<2u * job.n, GS_THREADS, smem, st>>>(job);
+		CMB_CHECK(cudaGetLastError());
+		return 0;
+	}
 	static size_t configured = 0;
 	if (smem > configured) {
 		CMB_CHECK(cudaFuncSetAttribute(k_get_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -917,9 +1105,20 @@ int launch_get_small(const GetJob &job, cudaStream_t st) {
 	return 0;
 }
 
-// CTAs of k_get_small that can be resident on the device at once (= scratch regions needed)
+// Requests of k_get_small (CTAs) or k_get_small_pair (clusters) that can be resident on the device at
+// once (= scratch regions needed).  Clusters of two need two SMs of one GPC.
 int get_small_residency(uint32_t nbytes) {
 	const size_t smem = get_small_smem(nbytes);
+	if (nbytes > GS_MAX_PAGE) {
+		if (cudaFuncSetAttribute(k_get_small_pair, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+		cudaLaunchConfig_t cfg = {};
+		cfg.gridDim = dim3(2u * (uint32_t)sm_count());
+		cfg.blockDim = dim3(GS_THREADS);
+		cfg.dynamicSmemBytes = smem;
+		int clusters = 0;
+		if (cudaOccupancyMaxActiveClusters(&clusters, k_get_small_pair, &cfg) != cudaSuccess) return -1;
+		return clusters;
+	}
 	if (cudaFuncSetAttribute(k_get_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
 	int per_sm = 0;
 	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_get_small, (int)GS_THREADS, smem) != cudaSuccess) return -1;

@@ -140,7 +140,7 @@ struct GetJob {
 	const unsigned long long *addr;   // n x {u, l}
 	const uint8_t *valid;             // optional
 	uint32_t n;
-	uint32_t nbytes;                  // page size, <= 65536 for this kernel
+	uint32_t nbytes;                  // page size, <= 131072; above 65536 a cluster of two CTAs per request
 	uint8_t *out;                     // n x nbytes
 	int32_t *status;                  // n
 	const uint8_t *peer[GET_MAX_PEERS];
@@ -153,7 +153,7 @@ struct GetJob {
 bool get_small_supports(uint32_t nbytes);
 size_t get_small_smem(uint32_t nbytes);
 uint32_t get_small_region_entries(uint32_t nbytes);
-int get_small_residency(uint32_t nbytes);   // CTAs resident on the device at once, < 0 on error
+int get_small_residency(uint32_t nbytes);   // requests resident on the device at once, < 0 on error
 int launch_get_small(const GetJob &job, cudaStream_t st);
 
 int launch_fingerprint(const uint8_t *pages, uint64_t stride, uint32_t nbytes, uint32_t n,

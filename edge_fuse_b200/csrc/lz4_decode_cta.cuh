@@ -1,4 +1,5 @@
-// lz4_decode_cta.cuh — one CTA decodes one LZ4 block that sits in shared memory (k_get_small).
+// lz4_decode_cta.cuh — one CTA decodes one LZ4 block that sits in shared memory (k_get_small; for
+// 128 KiB pages the page sits in a second CTA of a cluster, k_get_small_pair, see PAIR below).
 //
 // Same result as LZ4_decompress_fast (cachemap/lz4.c:1169-1344,1360-1363): exactly n bytes decoded,
 // `consumed` = bytes of the block read (lz4.c:1339), which filemap_get compares with the stored
@@ -61,6 +62,25 @@ __device__ __forceinline__ uint32_t dcs_ld32(uint32_t a) { uint32_t v; asm volat
 __device__ __forceinline__ void dcs_st32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v)); }
 __device__ __forceinline__ void dcs_st8(uint32_t a, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" ::"r"(a), "r"(v)); }
 
+// PAIR = the two-CTA decoder of 128 KiB pages (kernels.cu:k_get_small_pair): the record and the page
+// do not fit one CTA's shared memory, so the page lives in the partner CTA of a cluster of two and
+// the literal phase stores into it over DSMEM.  Its descriptors need 17 bits for match length - 4 (a
+// zero page is ONE match of ~131 060 bytes): the low 16 stay in the top half of the last word, bit 16
+// goes to bit 31 of the literal length (at most 131 072, so bits 18-31 are free).  Literal source,
+// output position and offset (< 65 536, the encoder's MAX_DISTANCE) keep their fields.
+template <bool PAIR> __device__ __forceinline__ uint32_t dc_lit_len(uint4 d) { return PAIR ? d.z & 0x7fffffffu : d.z; }
+template <bool PAIR> __device__ __forceinline__ uint32_t dc_match_len(uint4 d) {
+	return PAIR ? ((d.w >> 16) | (d.z >> 31) << 16) + 4u : (d.w >> 16) + 4u;
+}
+template <bool PAIR> __device__ __forceinline__ void dc_put8(uint32_t a, uint32_t v) {
+	if (PAIR) asm volatile("st.shared::cluster.u8 [%0], %1;" ::"r"(a), "r"(v));
+	else dcs_st8(a, v);
+}
+template <bool PAIR> __device__ __forceinline__ void dc_put32(uint32_t a, uint32_t v) {
+	if (PAIR) asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(a), "r"(v));
+	else dcs_st32(a, v);
+}
+
 // LZ4 255-run length extension at shared address blk + ip; cap = block length
 __device__ __forceinline__ bool dcs_ext(uint32_t blk, uint32_t cap, uint32_t &ip, uint32_t &len, int lane) {
 	for (;;) {
@@ -83,6 +103,7 @@ __device__ __forceinline__ bool dcs_ext(uint32_t blk, uint32_t cap, uint32_t &ip
 // past `cap` stay inside the CTA's shared memory and every use is bounds-checked).  The walk is one
 // shared-memory round trip per sequence: the token and the byte after it fix where the offset, the
 // match-length byte and the NEXT token lie, so those five bytes are requested together.
+template <bool PAIR>
 __device__ void dc_parse_chain(DecodeCta *dc, uint32_t c, uint32_t blk, uint32_t cap, uint32_t n, uint4 *desc,
     uint32_t max_desc, int lane) {
 	uint32_t ip = dc->ip0[c], op = dc->op0[c];
@@ -157,7 +178,7 @@ __device__ void dc_parse_chain(DecodeCta *dc, uint32_t c, uint32_t blk, uint32_t
 		} else {
 			mlen = 0;
 		}
-		if (lane == 0) *dnext = make_uint4(lit_src, out_pos, len, off | (mlen << 16));
+		if (lane == 0) *dnext = make_uint4(lit_src, out_pos, PAIR ? len | (mlen >> 16) << 31 : len, off | (mlen << 16));
 		dnext++;
 		cnt++;
 		if (last) break;                                     // op == n, ip == bytes consumed (lz4.c:1339)
@@ -168,7 +189,9 @@ __device__ void dc_parse_chain(DecodeCta *dc, uint32_t c, uint32_t blk, uint32_t
 	}
 }
 
-// Phase 2, all warps: batches of 32 descriptors, dealt round-robin.
+// Phase 2, all warps: batches of 32 descriptors, dealt round-robin.  PAIR: `out` / `out_g` is the
+// page in the partner CTA of the cluster (a shared::cluster address / a generic address).
+template <bool PAIR>
 __device__ void dc_literals(const DecodeCta *dc, uint4 *desc, uint32_t stride, uint32_t blk, uint32_t out,
     const uint8_t *blk_g, uint8_t *out_g, uint32_t warp, int lane) {
 	uint32_t turn = 0;
@@ -179,7 +202,7 @@ __device__ void dc_literals(const DecodeCta *dc, uint4 *desc, uint32_t stride, u
 			const bool valid = b + lane < cnt;
 			uint4 d = make_uint4(0, 0, 0, 0);
 			if (valid) d = __ldcg(desc + (size_t)c * stride + b + lane);
-			const uint32_t len = d.z;
+			const uint32_t len = dc_lit_len<PAIR>(d);
 			const uint32_t mine = len <= DC_LANE_LIT ? len : 0u;
 			const uint32_t most = __reduce_max_sync(CMB_FULL, mine);
 			const uint32_t src = blk + d.x, dst = out + d.y;
@@ -190,17 +213,17 @@ __device__ void dc_literals(const DecodeCta *dc, uint4 *desc, uint32_t stride, u
 				const uint32_t head = min(mine, (4u - (dst & 3u)) & 3u);
 				const uint32_t words = (mine - head) / 4u, tail = head + 4u * words;
 #pragma unroll
-				for (uint32_t j = 0; j < 3u; j++) if (j < head) dcs_st8(dst + j, dcs_ld8(src + j));
+				for (uint32_t j = 0; j < 3u; j++) if (j < head) dc_put8<PAIR>(dst + j, dcs_ld8(src + j));
 				const uint32_t mostw = __reduce_max_sync(CMB_FULL, words);
 				const uint32_t sa = src + head, s8 = (sa & 3u) * 8u;
 				for (uint32_t t = 0; t < mostw; t++) {
 					if (t < words) {
 						const uint32_t a = (sa & ~3u) + 4u * t;
-						dcs_st32(dst + head + 4u * t, __funnelshift_r(dcs_ld32(a), dcs_ld32(a + 4u), s8));
+						dc_put32<PAIR>(dst + head + 4u * t, __funnelshift_r(dcs_ld32(a), dcs_ld32(a + 4u), s8));
 					}
 				}
 #pragma unroll
-				for (uint32_t j = 0; j < 3u; j++) if (tail + j < mine) dcs_st8(dst + tail + j, dcs_ld8(src + tail + j));
+				for (uint32_t j = 0; j < 3u; j++) if (tail + j < mine) dc_put8<PAIR>(dst + tail + j, dcs_ld8(src + tail + j));
 			}
 			(void)most;
 			uint32_t wide = __ballot_sync(CMB_FULL, len > DC_LANE_LIT);
@@ -217,18 +240,28 @@ __device__ void dc_literals(const DecodeCta *dc, uint4 *desc, uint32_t stride, u
 			// final when the loop reaches i.  The number replaces the literal source in the descriptor.
 			const uint32_t off = d.w & 0xffffu;
 			const bool has = valid && off != 0u;
-			const uint32_t mlen = has ? (d.w >> 16) + 4u : 0u;
-			const uint32_t to = has ? d.y + d.z : 0xffffffffu, from = to - off, fe = from + mlen;
+			const uint32_t mlen = has ? dc_match_len<PAIR>(d) : 0u;
+			const uint32_t to = has ? d.y + len : 0xffffffffu, from = to - off, fe = from + mlen;
 			uint32_t wave = has ? 1u : 0u;
 			const uint32_t to0 = __shfl_sync(CMB_FULL, to, 0);             // (every lane takes part in the shuffle)
 			if (__any_sync(CMB_FULL, has && fe > to0)) {                  // somebody reads inside the batch
-				// destination and length travel in one word (both < 65 536); only the wave is a chain
-				const uint32_t key = has ? to | (mlen << 16) : 0xffffu;
+				if (PAIR) {
+					// destinations and lengths reach 17 bits: they travel in two words
 #pragma unroll
-				for (int i = 0; i < 31; i++) {
-					const uint32_t ki = __shfl_sync(CMB_FULL, key, i), wi = __shfl_sync(CMB_FULL, wave, i);
-					const uint32_t ti = ki & 0xffffu, li = ki >> 16;
-					if (lane > i && has && ti < fe && ti + li > from) wave = max(wave, wi + 1u);
+					for (int i = 0; i < 31; i++) {
+						const uint32_t ti = __shfl_sync(CMB_FULL, to, i), li = __shfl_sync(CMB_FULL, mlen, i);
+						const uint32_t wi = __shfl_sync(CMB_FULL, wave, i);
+						if (lane > i && has && ti < fe && ti + li > from) wave = max(wave, wi + 1u);
+					}
+				} else {
+					// destination and length travel in one word (both < 65 536); only the wave is a chain
+					const uint32_t key = has ? to | (mlen << 16) : 0xffffu;
+#pragma unroll
+					for (int i = 0; i < 31; i++) {
+						const uint32_t ki = __shfl_sync(CMB_FULL, key, i), wi = __shfl_sync(CMB_FULL, wave, i);
+						const uint32_t ti = ki & 0xffffu, li = ki >> 16;
+						if (lane > i && has && ti < fe && ti + li > from) wave = max(wave, wi + 1u);
+					}
 				}
 			}
 			if (valid) desc[(size_t)c * stride + b + lane].x = wave;
@@ -303,9 +336,10 @@ __device__ __forceinline__ void dc_match_wide(uint32_t to, uint32_t from, uint32
 	__syncwarp();
 }
 
-// Phase 3, one warp.  out = shared address of the page.  Every descriptor carries the wave of its
+// Phase 3, one warp.  out = shared address of the page (in this CTA also for PAIR).  Every descriptor carries the wave of its
 // match within its batch of 32 (dc_literals): the matches of one wave are copied together, a lane
 // each; long ones by the whole warp, one after the other.
+template <bool PAIR>
 __device__ void dc_matches(const DecodeCta *dc, const uint4 *desc, uint32_t stride, uint32_t out, int lane) {
 	for (uint32_t c = 0; c < DC_CHAINS; c++) {
 		const uint32_t cnt = dc->cnt[c];
@@ -317,8 +351,8 @@ __device__ void dc_matches(const DecodeCta *dc, const uint4 *desc, uint32_t stri
 			if (b + 32u + lane < cnt) nxt = __ldcg(dq + b + 32u + lane);      // next batch while this one is copied
 			const uint32_t off = d.w & 0xffffu;
 			const bool valid = b + lane < cnt && off != 0u;
-			const uint32_t len = valid ? (d.w >> 16) + 4u : 0u;
-			const uint32_t to = d.y + d.z, from = to - off;
+			const uint32_t len = valid ? dc_match_len<PAIR>(d) : 0u;
+			const uint32_t to = d.y + dc_lit_len<PAIR>(d), from = to - off;
 			const uint32_t wave = valid ? d.x : 0u;
 			const bool wide = len > DC_LANE_MATCH;
 			const uint32_t waves = __reduce_max_sync(CMB_FULL, wave);

@@ -216,8 +216,9 @@ int cmb200_close_peers(cmb200_engine *e);
  * memory (cmb200_host_alloc; the kernel writes it directly) or device memory.  Records are
  * immutable and every rewrite goes to fresh arena space, so a get that overlaps a put of the same
  * key returns the old or the new page, never a mix (the reference's LMDB snapshot reads,
- * filemap.c:223-231).  Page sizes above 64 KiB are not served by this call (-2): use
- * cmb200_get_batch.  status_out as cmb200_get_batch. */
+ * filemap.c:223-231).  Pages of 128 KiB (pshift 17) are decoded by a cluster of two CTAs per
+ * request, record in one and page in the other, with the same contract.  Page sizes above 128 KiB
+ * are not served by this call (-2): use cmb200_get_batch.  status_out as cmb200_get_batch. */
 int cmb200_get_small(cmb200_engine *e, size_t n, const cmb200_addr *addr, void *pages_out, int32_t *status_out);
 
 /* The same get in two halves, for callers that combine the requests of several threads into one
