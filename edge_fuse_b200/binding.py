@@ -36,6 +36,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_lz4_encode_batch", "cmb200_lz4_decode_batch", "cmb200_fingerprint_batch", "cmb200_fingerprint_dev",
     "cmb200_gen_chunk_host", "cmb200_gen_chunks_dev", "cmb200_gen_stream_ids", "cmb200_gen_addr",
     "cmb200_host_tier_enable", "cmb200_demote_batch", "cmb200_host_tier_stats",
+    "cmb200_promote_batch", "cmb200_host_tier_hot",
 ]
 
 
@@ -55,7 +56,8 @@ class Stats(C.Structure):
 
 class HostTierStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in (
-        "bytes", "used", "records", "garbage", "demoted_records", "demoted_bytes", "retired_records", "hits")]
+        "bytes", "used", "records", "garbage", "demoted_records", "demoted_bytes", "retired_records", "hits",
+        "promoted_records", "promoted_bytes")]
 
 
 def library_path() -> str:
@@ -148,6 +150,8 @@ def lib() -> C.CDLL:
         "cmb200_host_tier_enable": (i32, [vp, u64]),
         "cmb200_demote_batch": (i32, [vp, sz, vp, vp]),
         "cmb200_host_tier_stats": (i32, [vp, vp]),
+        "cmb200_promote_batch": (i32, [vp, sz, vp, vp]),
+        "cmb200_host_tier_hot": (i32, [vp, sz, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -312,6 +316,22 @@ class Engine:
         n = C.c_uint64(0)
         _check(lib().cmb200_demote_batch(self.h, len(addr), _ptr(addr), C.byref(n)), "cmb200_demote_batch")
         return n.value
+
+    def promote(self, u, l) -> int:
+        """cmb200_promote_batch: moves the keys' host-tier records back to free arena bytes, in order
+        while they fit -> how many moved."""
+        addr = _addr_array(u, l)
+        n = C.c_uint64(0)
+        _check(lib().cmb200_promote_batch(self.h, len(addr), _ptr(addr), C.byref(n)), "cmb200_promote_batch")
+        return n.value
+
+    def tier_hot(self, max_n: int = 4096):
+        """cmb200_host_tier_hot -> (u, l, lost): addresses read from the host tier since the last call,
+        newest first, distinct, at most max_n; lost = hits the log overwrote before this drain."""
+        addr = np.zeros((max(1, max_n), 2), dtype=np.uint64)
+        n, lost = C.c_size_t(0), C.c_uint64(0)
+        _check(lib().cmb200_host_tier_hot(self.h, max_n, _ptr(addr), C.byref(n), C.byref(lost)), "cmb200_host_tier_hot")
+        return addr[:n.value, 0].copy(), addr[:n.value, 1].copy(), lost.value
 
     def host_tier_stats(self) -> dict:
         return host_tier_stats(self.h)

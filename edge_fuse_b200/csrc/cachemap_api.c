@@ -40,6 +40,8 @@
 #pragma weak cmb200_host_tier_enable
 #pragma weak cmb200_demote_batch
 #pragma weak cmb200_host_tier_stats
+#pragma weak cmb200_promote_batch
+#pragma weak cmb200_host_tier_hot
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -47,6 +49,7 @@
 #define GET_CALLERS 32          /* callers inside the combining queue at once; the rest sleep at its door */
 #define FLUSH_MAX 4096          /* pages the flusher hands over per GPU batch */
 #define PNUM_SHIFT 44           /* cachemap.c:155 */
+#define PROMOTE_EVERY_MS 100    /* CMB200_TIER_PROMOTE: at most one promotion round this often */
 
 enum req_kind { REQ_GET, REQ_UNSET };
 enum wb_state { WB_FREE = 0, WB_FILLING, WB_READY, WB_FLUSHING };
@@ -80,6 +83,13 @@ struct filemap {
 	int init_state;         /* 0 = not yet, 1 = ready, -1 = failed */
 	cmb200_engine *eng;
 	int host_tier;          /* the engine has a host tier (CMB200_HOST_TIER_MB): a full arena demotes instead of evicting */
+	/* promotion of hot tier records back to the arena (CMB200_TIER_PROMOTE), run by the flusher */
+	uint64_t tier_promote;  /* pages per round, 0 = off */
+	cmb200_addr *promo_hot; /* tier_promote entries: the round's drained hot addresses */
+	pthread_mutex_t promo_mu;       /* the guard below (demotion runs in callers of cachemap_put_batch too) */
+	cmb200_addr *promo_guard;       /* FIFO of the last 4 x tier_promote promoted addresses: not demoted again */
+	uint64_t promo_guard_n;         /* addresses ever added; slot = index % (4 x tier_promote) */
+	struct timespec promo_last;     /* CLOCK_MONOTONIC of the last round */
 	uint8_t *h_stage;       /* page-locked, LEADERS x COMBINE_MAX pages: the stage buffer of each leader slot */
 	int leader_busy[LEADERS];       /* a batch is in flight in this slot (under q_mu) */
 	int batch_left[LEADERS];        /* its requesters that have not taken their answer yet (atomic) */
@@ -153,6 +163,17 @@ filemap_engine_ready(struct filemap *m)
 			else
 				fprintf(stderr, "cachemap_b200: no host tier of %ld MiB: %s\n", tier_mb, cmb200_last_error());
 		}
+		const long promote = env_long("CMB200_TIER_PROMOTE", 0);
+		if (m->host_tier && promote > 0) {
+			if (!cmb200_promote_batch || !cmb200_host_tier_hot)
+				fprintf(stderr, "cachemap_b200: CMB200_TIER_PROMOTE ignored: the engine cannot promote\n");
+			else {
+				m->promo_hot = malloc((size_t)promote * sizeof(cmb200_addr));
+				m->promo_guard = malloc(4 * (size_t)promote * sizeof(cmb200_addr));
+				if (m->promo_hot && m->promo_guard)
+					m->tier_promote = (uint64_t)promote;
+			}
+		}
 		if (m->eng) {
 			m->h_stage = cmb200_host_alloc((size_t)LEADERS * COMBINE_MAX * m->bsize);
 			/* ring of 256 MiB by default, at least 64 pages.  The size sets the batch the flusher can form
@@ -223,6 +244,7 @@ filemap_create(char *destdir, uint64_t n, int compress_accel, int pshift)
 	pthread_cond_init(&m->wb_work, NULL);
 	pthread_cond_init(&m->wb_idle, NULL);
 	pthread_mutex_init(&m->snap_mu, NULL);
+	pthread_mutex_init(&m->promo_mu, NULL);
 	return m;
 }
 
@@ -281,6 +303,9 @@ filemap_free(struct filemap *m)
 		cmb200_host_free(m->h_stage);
 	if (m->eng)
 		cmb200_engine_destroy(m->eng);
+	free(m->promo_hot);
+	free(m->promo_guard);
+	pthread_mutex_destroy(&m->promo_mu);
 	pthread_mutex_destroy(&m->snap_mu);
 	pthread_mutex_destroy(&m->init_mu);
 	pthread_mutex_destroy(&m->q_mu);
@@ -355,15 +380,50 @@ aged_cmp(const void *x, const void *y)
 	return a < b ? -1 : a > b;
 }
 
+static int
+addr_cmp(const void *x, const void *y)
+{
+	const cmb200_addr *a = x, *b = y;
+	if (a->u != b->u)
+		return a->u < b->u ? -1 : 1;
+	return a->l < b->l ? -1 : a->l > b->l;
+}
+
+/* Sorted copy of the addresses the last promotion rounds offered (CMB200_TIER_PROMOTE), or NULL.  A
+ * promoted record keeps its old put timestamp, so without this the next demotion, which takes the
+ * oldest of what it samples, would send it straight back to the tier. */
+static cmb200_addr *
+filemap_promo_guard(struct filemap *m, size_t *n)
+{
+	*n = 0;
+	if (!m->tier_promote)
+		return NULL;
+	pthread_mutex_lock(&m->promo_mu);
+	const uint64_t cap = 4 * m->tier_promote;
+	const size_t k = (size_t)(m->promo_guard_n < cap ? m->promo_guard_n : cap);
+	cmb200_addr *g = k ? malloc(k * sizeof(cmb200_addr)) : NULL;
+	if (g) {
+		memcpy(g, m->promo_guard, k * sizeof(cmb200_addr));
+		*n = k;
+	}
+	pthread_mutex_unlock(&m->promo_mu);
+	if (g)
+		qsort(g, *n, sizeof(cmb200_addr), addr_cmp);
+	return g;
+}
+
 /* Moves up to `want` arena records to the host tier.  The candidates are drawn as filemap_evict_n
- * draws them (3 per record wanted) and go oldest first; keys already in the tier are passed over, so
- * a round goes on down its candidates until `want` have moved.  When few records are left in the
- * arena a round may find none: it draws again, up to 16 times in a row.  Returns how many moved. */
+ * draws them (3 per record wanted) and go oldest first; keys already in the tier, and keys promotion
+ * has just brought back (filemap_promo_guard), are passed over, so a round goes on down its candidates
+ * until `want` have moved.  When few records are left in the arena a round may find none: it draws
+ * again, up to 16 times in a row.  Returns how many moved. */
 static uint64_t
 filemap_demote_n(struct filemap *m, uint64_t want)
 {
 	uint64_t moved = 0;
 	int idle = 0;
+	size_t ng = 0;
+	cmb200_addr *guard = filemap_promo_guard(m, &ng);
 	while (moved < want && idle < 16) {
 		uint64_t need = want - moved;
 		if (need > 4096)
@@ -386,7 +446,7 @@ filemap_demote_n(struct filemap *m, uint64_t want)
 			if (cmb200_sample(m->eng, (size_t)nd, draws, cand, ts, ok) == 0) {
 				uint64_t nv = 0;
 				for (uint64_t i = 0; i < nd; i++)
-					if (ok[i] > 0)
+					if (ok[i] > 0 && !(guard && bsearch(&cand[i], guard, ng, sizeof(cmb200_addr), addr_cmp)))
 						old[nv++] = (struct aged){ ts[i], cand[i] };
 				qsort(old, (size_t)nv, sizeof(struct aged), aged_cmp);
 				for (uint64_t k = 0; k < nv && moved < want;) {
@@ -408,6 +468,7 @@ filemap_demote_n(struct filemap *m, uint64_t want)
 		free(draws); free(ts); free(ok); free(cand); free(old); free(victim);
 		idle = round ? 0 : idle + 1;
 	}
+	free(guard);
 	return moved;
 }
 
@@ -437,9 +498,9 @@ filemap_evict(struct filemap *m, uint64_t incoming)
  * records are demoted to it and the arena compacted, so the store keeps `capacity` pages as the
  * reference's LMDB files do; otherwise evict by bytes as well and compact what that frees.
  * Only when even that fails does a put get dropped, as a full LMDB map drops it
- * (filemap.c:143-145,154-157). */
+ * (filemap.c:143-145,154-157).  may_evict = 0 (room for promotion): demotion and compaction only. */
 static void
-filemap_check_arena(struct filemap *m, uint64_t incoming)
+filemap_arena_room(struct filemap *m, uint64_t incoming, int may_evict)
 {
 	const uint64_t need = incoming * ((uint64_t)m->bsize + 1056);
 	int evicted = 0;
@@ -478,6 +539,8 @@ filemap_check_arena(struct filemap *m, uint64_t incoming)
 			evicted = 1;
 			continue;
 		}
+		if (!may_evict)
+			return;
 		const uint64_t avg = live / st.entries ? live / st.entries : 1;
 		uint64_t victims = shortfall / avg + shortfall / avg / 8 + 16;
 		if (victims > st.entries)
@@ -488,6 +551,52 @@ filemap_check_arena(struct filemap *m, uint64_t incoming)
 	}
 }
 
+static void
+filemap_check_arena(struct filemap *m, uint64_t incoming)
+{
+	filemap_arena_room(m, incoming, 1);
+}
+
+/* One promotion round (CMB200_TIER_PROMOTE = N): up to N addresses that gets answered from the host
+ * tier since the last round, newest first, go back to the arena.  Room is made only by demoting the
+ * oldest arena records and compacting, never by evicting; when that frees too little, the round
+ * promotes what fits.  The addresses join the guard FIFO that demotion passes over. */
+static void
+filemap_promote_round(struct filemap *m)
+{
+	clock_gettime(CLOCK_MONOTONIC, &m->promo_last);
+	size_t n = 0;
+	if (cmb200_host_tier_hot(m->eng, (size_t)m->tier_promote, m->promo_hot, &n, NULL) != 0) {
+		fprintf(stderr, "cachemap_b200: the host tier's hot log could not be read: %s\n", cmb200_last_error());
+		return;
+	}
+	if (n == 0)
+		return;
+	filemap_arena_room(m, n, 0);
+	uint64_t got = 0;
+	if (cmb200_promote_batch(m->eng, n, m->promo_hot, &got) != 0) {
+		fprintf(stderr, "cachemap_b200: promotion from the host tier failed: %s\n", cmb200_last_error());
+		return;
+	}
+	pthread_mutex_lock(&m->promo_mu);
+	const uint64_t cap = 4 * m->tier_promote;
+	for (size_t i = 0; i < n; i++)
+		m->promo_guard[m->promo_guard_n++ % cap] = m->promo_hot[i];
+	pthread_mutex_unlock(&m->promo_mu);
+}
+
+/* A promotion round is due: the knob is on and PROMOTE_EVERY_MS have passed since the last one. */
+static int
+filemap_promote_due(struct filemap *m)
+{
+	if (!m->tier_promote)
+		return 0;
+	struct timespec now;
+	clock_gettime(CLOCK_MONOTONIC, &now);
+	const int64_t ms = (int64_t)(now.tv_sec - m->promo_last.tv_sec) * 1000 + (now.tv_nsec - m->promo_last.tv_nsec) / 1000000;
+	return ms >= PROMOTE_EVERY_MS;
+}
+
 /* Before a batch of `incoming` puts: evict down to capacity, then make sure the arena has room
  * (what eviction frees is garbage until the arena is compacted). */
 static void
@@ -495,6 +604,14 @@ filemap_make_room(struct filemap *m, uint64_t incoming)
 {
 	filemap_evict(m, incoming);
 	filemap_check_arena(m, incoming);
+}
+
+static void
+timespec_add_ms(struct timespec *t, long ms)
+{
+	t->tv_nsec += ms * 1000000L;
+	t->tv_sec += t->tv_nsec / 1000000000L;
+	t->tv_nsec %= 1000000000L;
 }
 
 /* The flusher: takes the longest run of finished slots from the tail of the ring and puts it
@@ -517,6 +634,12 @@ filemap_flusher(void *arg)
 		if (count == 0) {
 			if (m->wb_stop && m->wb_tail == m->wb_head)
 				break;
+			if (filemap_promote_due(m)) {
+				pthread_mutex_unlock(&m->wb_mu);
+				filemap_promote_round(m);
+				pthread_mutex_lock(&m->wb_mu);
+				continue;
+			}
 			if (m->checkpoint_sec > 0 && m->persist) {
 				struct timespec now, until;
 				clock_gettime(CLOCK_REALTIME, &now);
@@ -528,7 +651,18 @@ filemap_flusher(void *arg)
 					continue;
 				}
 				until = now;
-				until.tv_sec += 1;
+				if (m->tier_promote)
+					timespec_add_ms(&until, PROMOTE_EVERY_MS);
+				else
+					until.tv_sec += 1;
+				m->wb_flusher_asleep = 1;
+				pthread_cond_timedwait(&m->wb_work, &m->wb_mu, &until);
+				m->wb_flusher_asleep = 0;
+			} else if (m->tier_promote) {
+				/* woken for the next promotion round at the latest */
+				struct timespec until;
+				clock_gettime(CLOCK_REALTIME, &until);
+				timespec_add_ms(&until, PROMOTE_EVERY_MS);
 				m->wb_flusher_asleep = 1;
 				pthread_cond_timedwait(&m->wb_work, &m->wb_mu, &until);
 				m->wb_flusher_asleep = 0;
@@ -563,6 +697,11 @@ filemap_flusher(void *arg)
 		m->wb_tail += count;
 		pthread_cond_broadcast(&m->wb_space);
 		pthread_cond_broadcast(&m->wb_idle);            /* waiters compare wb_tail with their own target */
+		if (filemap_promote_due(m)) {
+			pthread_mutex_unlock(&m->wb_mu);
+			filemap_promote_round(m);
+			pthread_mutex_lock(&m->wb_mu);
+		}
 	}
 	pthread_mutex_unlock(&m->wb_mu);
 	free(addr);

@@ -14,6 +14,7 @@
 #include <atomic>
 #include <deque>
 #include <mutex>
+#include <set>
 #include <shared_mutex>
 #include <sched.h>
 #include <string>
@@ -138,10 +139,16 @@ struct cmb200_engine {
 		uint64_t head = 0;                   // log position of the next record
 		std::deque<std::pair<uint64_t, uint32_t>> log;   // {position, bytes} of each record not yet overwritten, oldest first
 		uint64_t demoted_records = 0, demoted_bytes = 0;
-		unsigned long long *d_ctr = nullptr; // device: [0] records retired by wrap-around, [1] host-tier hits
+		uint64_t promoted_records = 0, promoted_bytes = 0;
+		unsigned long long *d_ctr = nullptr; // device: [0] records retired by wrap-around, [1] host-tier hits,
+		                                     // [2] head of the hot log
+		ulonglong2 *d_hot = nullptr;         // the hot log: HOT_LOG_N addresses of tier hits
+		uint64_t hot_drained = 0;            // hot-log head at the last cmb200_host_tier_hot
 		unsigned long long *d_retire = nullptr;   // {u, l, location, bytes} per record a wrap overwrites
 		size_t retire_cap = 0;
 		DemoteEntry *d_moves = nullptr;      // max_batch entries
+		PromoteEntry *d_promote = nullptr;   // max_batch entries
+		HotLog hot() const { return HotLog{d_ctr ? d_ctr + 2 : nullptr, d_hot}; }
 	} tier;
 	std::atomic<bool> multi_gpu{false};  // a multi-GPU call was made: no host tier from then on
 };
@@ -197,6 +204,7 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	for (int r = 0; r < GET_MAX_PEERS; r++) if (e->peer_base[r]) cudaIpcCloseMemHandle((void *)e->peer_base[r]);
 	if (e->tier.host) cudaFreeHost(e->tier.host);
 	cudaFree(e->tier.d_ctr); cudaFree(e->tier.d_retire); cudaFree(e->tier.d_moves);
+	cudaFree(e->tier.d_promote); cudaFree(e->tier.d_hot);
 	cudaFree(e->d_lens); cudaFree(e->d_status); cudaFree(e->d_fps); cudaFree(e->d_recoff); cudaFree(e->d_work); cudaFree(e->d_order); cudaFree(e->d_import_slot);
 	for (int i = 0; i < 2; i++) {
 		if (e->landed[i]) cudaEventDestroy(e->landed[i]);
@@ -651,6 +659,7 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		job.n = m; job.nbytes = e->bsize; job.pages = d_out; job.status = e->d_status + at;
 		job.rec_off = e->d_recoff; job.vlen = e->d_vlen; job.arena = e->arena.base;
 		job.host = e->tier.dev; job.host_hits = e->tier.d_ctr + 1;
+		job.hot = e->tier.hot(); job.addr = e->d_addr + 2 * at;
 		CMB_CHECK(cudaEventRecord(e->t0[nb % e->RING], e->st));
 		if (launch_decode(job, e->st)) return -1;
 		CMB_CHECK(cudaEventRecord(e->t1[nb % e->RING], e->st));
@@ -796,6 +805,7 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	job.status = ln->h_status;
 	for (int r = 0; r < GET_MAX_PEERS; r++) { job.peer[r] = e->peer_base[r]; job.peer_size[r] = e->peer_size[r]; }
 	job.scratch = e->d_scratch; job.region_entries = e->region_entries; job.pool_bits = e->d_pool_bits; job.pool_n = e->pool_n;
+	job.hot = e->tier.hot();
 	if (launch_get_small(job, ln->st)) { ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1; }
 	t->lane = li; t->n = (uint32_t)n; t->status = ln->h_status;
 	return 0;
@@ -1268,14 +1278,17 @@ extern "C" int cmb200_host_tier_enable(cmb200_engine *e, uint64_t bytes) {
 	if (bytes < 4ull * e->stage_stride) { set_error_msg("cmb200_host_tier_enable: fewer bytes than four worst-case records"); return -1; }
 	CMB_CHECK(cudaSetDevice(e->device));
 	cmb200_engine::HostTier &t = e->tier;
-	if (cudaMalloc(&t.d_ctr, 2 * sizeof(unsigned long long)) != cudaSuccess ||
+	if (cudaMalloc(&t.d_ctr, 3 * sizeof(unsigned long long)) != cudaSuccess ||
 	    cudaMalloc(&t.d_moves, (size_t)e->max_batch * sizeof(DemoteEntry)) != cudaSuccess ||
-	    cudaMemset(t.d_ctr, 0, 2 * sizeof(unsigned long long)) != cudaSuccess ||
+	    cudaMalloc(&t.d_promote, (size_t)e->max_batch * sizeof(PromoteEntry)) != cudaSuccess ||
+	    cudaMalloc(&t.d_hot, HOT_LOG_N * sizeof(ulonglong2)) != cudaSuccess ||
+	    cudaMemset(t.d_ctr, 0, 3 * sizeof(unsigned long long)) != cudaSuccess ||
+	    cudaMemset(t.d_hot, 0, HOT_LOG_N * sizeof(ulonglong2)) != cudaSuccess ||
 	    cudaHostAlloc(&t.host, bytes, cudaHostAllocMapped) != cudaSuccess ||
 	    cudaHostGetDevicePointer(&t.dev, t.host, 0) != cudaSuccess) {
 		cmb_set_error("cmb200_host_tier_enable", cudaGetLastError(), __FILE__, __LINE__);
 		if (t.host) cudaFreeHost(t.host);
-		cudaFree(t.d_ctr); cudaFree(t.d_moves);
+		cudaFree(t.d_ctr); cudaFree(t.d_moves); cudaFree(t.d_promote); cudaFree(t.d_hot);
 		t = cmb200_engine::HostTier{};
 		return -1;
 	}
@@ -1417,6 +1430,92 @@ static int demote_arena_all(cmb200_engine *e) {
 	return compact_locked(e, nullptr);
 }
 
+// Promotion: the tier records of the named keys go back to free arena bytes above the bump pointer, in
+// array order while they fit.  Nothing is evicted, demoted or compacted to make room; the caller does
+// that first if it wants to (the drop-in's CMB200_TIER_PROMOTE).  See slot_publish in kernels.cu for
+// why readers on other streams need no get_gate.
+extern "C" int cmb200_promote_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *promoted_out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	if (promoted_out) *promoted_out = 0;
+	cmb200_engine::HostTier &t = e->tier;
+	if (!t.host) { set_error_msg("cmb200_promote_batch: the engine has no host tier"); return -1; }
+	CMB_CHECK(cudaSetDevice(e->device));
+	harvest_pending(e, true);
+	unsigned long long c[8];
+	if (read_counters(e, c)) return -1;
+	unsigned long long head = c[2];                  // a multiple of 16; past the end when a put overflowed
+	std::vector<int32_t> st(e->max_batch);
+	std::vector<uint64_t> off(e->max_batch);
+	std::vector<uint32_t> vl(e->max_batch);
+	std::vector<PromoteEntry> plan;
+	uint64_t done = 0;
+	bool full = false;
+	for (size_t at = 0; at < n && !full; at += e->max_batch) {
+		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
+		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
+		if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(st.data(), e->d_status, m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemcpyAsync(off.data(), e->d_recoff, m * 8, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemcpyAsync(vl.data(), e->d_vlen, m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		e->stats.kernel_launches++;
+		// absent, remote and arena keys are skipped; a key named twice moves once (a later chunk's
+		// lookup runs after this chunk's promotion on the stream and finds it in the arena)
+		plan.clear();
+		std::unordered_set<uint64_t> seen;
+		for (uint32_t i = 0; i < m; i++) {
+			if (st[i] != ST_HIT || !(off[i] & REC_HOST) || !seen.insert(off[i]).second) continue;
+			const uint32_t clen = vl[i] - 1u, len = 24u + (clen ? clen : e->bsize), need = (len + 15u) & ~15u;
+			if (head + need > e->arena.size) { full = true; break; }
+			plan.push_back(PromoteEntry{off[i] & ~REC_HOST, head, len, 0});
+			head += need;
+		}
+		if (plan.empty()) continue;
+		// the bump pointer moves past the new records before any of them is published
+		CMB_CHECK(cudaMemcpyAsync(e->d_counters + 2, &head, 8, cudaMemcpyHostToDevice, e->st));
+		CMB_CHECK(cudaMemcpyAsync(t.d_promote, plan.data(), plan.size() * sizeof(PromoteEntry), cudaMemcpyHostToDevice, e->st));
+		if (launch_promote(e->table, e->arena, t.d_promote, (uint32_t)plan.size(), t.dev, e->st)) return -1;
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		e->stats.kernel_launches++;
+		done += plan.size();
+		t.promoted_records += plan.size();
+		for (const PromoteEntry &p : plan) t.promoted_bytes += p.len;
+	}
+	if (promoted_out) *promoted_out = done;
+	return 0;
+}
+
+// The hot log is read while gets go on appending to it, without the lock that puts take.  An entry
+// read half-written, or one overwritten by a later lap, yields an address that is wrong or stale;
+// that is harmless, since cmb200_promote_batch looks every address up again and checks its record.
+extern "C" int cmb200_host_tier_hot(cmb200_engine *e, size_t max, cmb200_addr *addr_out, size_t *n_out, uint64_t *lost_out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	*n_out = 0;
+	if (lost_out) *lost_out = 0;
+	cmb200_engine::HostTier &t = e->tier;
+	if (!t.host) return 0;
+	CMB_CHECK(cudaSetDevice(e->device));
+	unsigned long long head = 0;
+	std::vector<ulonglong2> ring(HOT_LOG_N);
+	CMB_CHECK(cudaMemcpyAsync(&head, t.d_ctr + 2, 8, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaMemcpyAsync(ring.data(), t.d_hot, HOT_LOG_N * sizeof(ulonglong2), cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	const uint64_t since = head - t.hot_drained;
+	const uint64_t from = since > HOT_LOG_N ? head - HOT_LOG_N : t.hot_drained;
+	if (lost_out) *lost_out = since > HOT_LOG_N ? since - HOT_LOG_N : 0;
+	t.hot_drained = head;
+	std::set<std::pair<uint64_t, uint64_t>> seen;
+	size_t k = 0;
+	for (uint64_t p = head; p > from && k < max; p--) {        // newest first
+		const ulonglong2 a = ring[(p - 1) % HOT_LOG_N];
+		if (!seen.insert({a.x, a.y}).second) continue;
+		addr_out[k].u = a.x; addr_out[k].l = a.y;
+		k++;
+	}
+	*n_out = k;
+	return 0;
+}
+
 extern "C" int cmb200_host_tier_stats(cmb200_engine *e, struct cmb200_host_tier_stats *out) {
 	std::lock_guard<std::mutex> g(e->mu);
 	memset(out, 0, sizeof(*out));
@@ -1430,6 +1529,7 @@ extern "C" int cmb200_host_tier_stats(cmb200_engine *e, struct cmb200_host_tier_
 	out->records = c[7]; out->garbage = c[6];
 	out->demoted_records = t.demoted_records; out->demoted_bytes = t.demoted_bytes;
 	out->retired_records = d[0]; out->hits = d[1];
+	out->promoted_records = t.promoted_records; out->promoted_bytes = t.promoted_bytes;
 	return 0;
 }
 

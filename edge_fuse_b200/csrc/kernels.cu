@@ -169,6 +169,14 @@ __device__ __forceinline__ void slot_release(const ArenaView &a, const Slot &s) 
 	}
 }
 
+// Appends the address of a get answered from the host tier to the hot log (one thread).  The log is
+// written without a lock: an entry read while it is being written, or one a later lap has replaced, is
+// only a hint, since cmb200_promote_batch looks every address up again and checks the record's prefix.
+__device__ __forceinline__ void hot_log(const HotLog &h, unsigned long long u, unsigned long long l) {
+	const unsigned long long k = atomicAdd(h.head, 1ull);
+	h.ring[k % HOT_LOG_N] = make_ulonglong2(u, l);
+}
+
 // filemap_unset (filemap.c:188-215): delete by key, whatever address the record holds.
 __global__ void k_unset(TableView t, ArenaView a, const unsigned long long *addr, uint32_t n) {
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -256,6 +264,11 @@ __global__ void __launch_bounds__(256) k_sample_scan(TableView t, const unsigned
 // with ONE 8-byte store.  Demotion to the host tier (k_demote_publish) changes nothing else (vlen,
 // addr and ts stay), so a reader sees the old arena location or the new host location, never a mix;
 // the arena bytes stay intact until the next compaction, which closes get_gate.
+// Promotion back to the arena (k_promote) is the same store in the other direction and needs no
+// get_gate either: a reader sees the tier location or the arena location, and both hold the same bytes.
+// The tier bytes stay intact until the ring laps them, and that lap closes get_gate (demote_group).
+// The arena bytes lie above the bump pointer as it was before the promotion, where no slot pointed, so
+// no reader can reach them before the rec_off store, which k_promote makes after a fence.
 __device__ __forceinline__ void slot_publish(const EncodeJob &job, Slot &s, uint32_t i, uint32_t idx, unsigned long long off,
     uint32_t need, uint32_t clen, unsigned long long au, unsigned long long al, uint64_t fp_hi, uint64_t fp_lo) {
 	// whatever checkpoints the slot has describe the record it is leaving (ckpt_store renews them)
@@ -637,7 +650,10 @@ __global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) {
 		const unsigned long long off = job.rec_off[i];
 		// host tier: mapped host memory, read over PCIe
 		const uint8_t *rec = (off & REC_HOST) ? job.host + (off & ~REC_HOST) : job.arena + off;
-		if ((off & REC_HOST) && lane == 0) atomicAdd(job.host_hits, 1ull);
+		if ((off & REC_HOST) && lane == 0) {
+			atomicAdd(job.host_hits, 1ull);
+			hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
+		}
 		uint32_t clen = job.vlen[i] - 1u;
 		if (clen == 0) {                            // raw page (filemap.c:249-251)
 			warp_copy_ro(out, rec + 24, job.nbytes, lane);
@@ -901,7 +917,11 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	__syncthreads();
 	if (tid == 0) {
 		if (sh->region != 0xffffffffu) gs_region_give(job, sh->region);
-		if (result == ST_HIT && from_host) atomicAdd(job.host_hits, 1ull);
+		if (result == ST_HIT && from_host) {
+			atomicAdd(job.host_hits, 1ull);
+			// loaded again rather than kept from the top: u and l live past the loop would cost registers
+			hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
+		}
 		__threadfence_system();
 		*reinterpret_cast<volatile int32_t *>(&job.status[i]) = result;
 	}
@@ -973,7 +993,10 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 		__syncthreads();
 		if (tid == 0) {
 			if (v->region != 0xffffffffu) gs_region_give(job, v->region);
-			if (v->result == ST_HIT && v->from_host) atomicAdd(job.host_hits, 1ull);
+			if (v->result == ST_HIT && v->from_host) {
+				atomicAdd(job.host_hits, 1ull);
+				hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
+			}
 			__threadfence_system();
 			*reinterpret_cast<volatile int32_t *>(&job.status[i]) = v->result;
 		}
@@ -1444,6 +1467,51 @@ int launch_demote_gather(ArenaView a, const DemoteEntry *d, uint32_t n, uint8_t 
 int launch_demote_publish(TableView t, ArenaView a, const DemoteEntry *d, uint32_t n, cudaStream_t st) {
 	if (n == 0) return 0;
 	k_demote_publish<<<GRID1D(n), 0, st>>>(t, a, d, n);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+// Promotion: one warp per record copies it from the mapped tier into the arena above the old bump
+// pointer (16-byte loads past the L1, as k_get_small reads the tier), then lane 0 repoints the slot.
+__global__ void __launch_bounds__(256) k_promote(TableView t, ArenaView a, const PromoteEntry *p, uint32_t n,
+    const uint8_t *host) {
+	const int lane = threadIdx.x & 31;
+	const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	if (i >= n) return;
+	const PromoteEntry m = p[i];
+	const uint32_t need = (m.len + 15u) & ~15u;
+	const uint4 *src = reinterpret_cast<const uint4 *>(host + m.host_off);
+	uint4 *dst = reinterpret_cast<uint4 *>(a.base + m.new_off);
+	for (uint32_t k = lane; k < need / 16u; k += 32) dst[k] = __ldcg(src + k);
+	__threadfence();                                 // the record is complete before the slot points to it
+	__syncwarp();
+	if (lane != 0) return;
+	// the record's own prefix names the key, as in k_demote_publish
+	const unsigned long long *pre = reinterpret_cast<const unsigned long long *>(a.base + m.new_off);
+	const unsigned long long loc = REC_HOST | m.host_off;
+	const uint32_t idx = table_find(t, fnv_addr(pre[0], pre[1]));
+	Slot *s = idx == 0xffffffffu ? nullptr : &t.slots[idx];
+	if (!s || s->vlen == 0 || s->owner != 0 || s->rec_off != loc) {
+		atomicAdd(a.garbage, (unsigned long long)need);          // not the record that was copied
+		return;
+	}
+	const uint32_t clen = s->vlen - 1u;
+	atomicAdd(a.tier, (unsigned long long)s->alloc);           // the tier copy is dead bytes until the ring laps it
+	atomicAdd(a.tier + 1, (unsigned long long)-1ll);
+	s->alloc = need;
+	*reinterpret_cast<volatile unsigned long long *>(&s->rec_off) = m.new_off;   // the one store readers trust
+	if (t.ckpt) {
+		// the block is unchanged, so are its checkpoints: only the tag moves to the new location
+		uint32_t *w = t.ckpt + (size_t)idx * CKPT_WORDS;
+		if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(loc, clen)) {
+			__threadfence();
+			*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(m.new_off, clen);
+		}
+	}
+}
+int launch_promote(TableView t, ArenaView a, const PromoteEntry *p, uint32_t n, const uint8_t *host, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_promote<<<(n * 32 + 255) / 256, 256, 0, st>>>(t, a, p, n, host);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

@@ -26,9 +26,19 @@ constexpr unsigned long long KEY_EMPTY = 0ull;
 constexpr unsigned long long KEY_TOMB = ~0ull;
 
 // Bit 63 of Slot::rec_off: the record lives in the host tier (page-locked, device-mapped host memory)
-// at offset rec_off & ~REC_HOST, in the same format as in the arena.  A record moves from the arena
-// to the host tier only (cmb200_demote_batch), by one 8-byte store of rec_off.
+// at offset rec_off & ~REC_HOST, in the same format as in the arena.  A record moves between the
+// tiers by one 8-byte store of rec_off: to the host tier by cmb200_demote_batch, back to the arena by
+// cmb200_promote_batch.
 constexpr unsigned long long REC_HOST = 1ull << 63;
+
+// The log of host-tier hits: a ring of the last HOT_LOG_N addresses {u, l} that a get answered from the
+// tier, appended by k_decode / k_get_small / k_get_small_pair (slot = atomicAdd(head, 1) % HOT_LOG_N,
+// one 16-byte store) and drained by cmb200_host_tier_hot.
+constexpr uint32_t HOT_LOG_N = 4096;
+struct HotLog {
+	unsigned long long *head;     // appends so far (64-bit, never wraps)
+	ulonglong2 *ring;             // HOT_LOG_N entries {u, l}
+};
 
 struct TableView {
 	Slot *slots;                 // cap + 2 entries; [cap] holds key 0, [cap+1] holds key ~0
@@ -121,6 +131,8 @@ struct DecodeJob {
 	const uint8_t *arena;
 	const uint8_t *host;         // device address of the host tier (null: no tier)
 	unsigned long long *host_hits;
+	HotLog hot;                  // where tier hits are logged (null: no tier)
+	const unsigned long long *addr;   // n x {u, l}, the requests' addresses (for the log)
 };
 int launch_decode(const DecodeJob &job, cudaStream_t st);
 
@@ -149,6 +161,8 @@ struct GetJob {
 	uint32_t region_entries;
 	uint32_t *pool_bits;              // bitmap of the regions in use
 	uint32_t pool_n;
+	HotLog hot;                       // where tier hits are logged (null: no tier); last, so that the
+	                                  // other members keep their parameter offsets
 };
 bool get_small_supports(uint32_t nbytes);
 size_t get_small_smem(uint32_t nbytes);
@@ -244,6 +258,14 @@ int launch_demote_gather(ArenaView a, const DemoteEntry *d, uint32_t n, uint8_t 
 // Repoints each slot that still holds old_off to REC_HOST | host_off and moves its bytes from arena
 // garbage accounting to the tier's.
 int launch_demote_publish(TableView t, ArenaView a, const DemoteEntry *d, uint32_t n, cudaStream_t st);
+// ---- host tier (cmb200_promote_batch) ----
+// One record moving from the host tier back to the arena: copied from host_off (one warp, 16-byte
+// loads from the mapped tier) to new_off, free arena bytes above the bump pointer.  The slot that
+// still holds REC_HOST | host_off then points at new_off and its bytes go from the tier's accounting
+// to the arena's; a slot that no longer holds it leaves the copy as arena garbage.
+struct PromoteEntry { unsigned long long host_off, new_off; uint32_t len, pad; };
+static_assert(sizeof(PromoteEntry) == 24, "promote entry layout");
+int launch_promote(TableView t, ArenaView a, const PromoteEntry *p, uint32_t n, const uint8_t *host, cudaStream_t st);
 // Records of the tier that are about to be overwritten: {u, l, REC_HOST | offset, bytes}.  A key whose
 // slot still points at that exact location is unset (an eviction); otherwise the bytes leave the
 // tier's garbage.  *retired counts the unset keys.

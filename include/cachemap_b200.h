@@ -172,17 +172,32 @@ int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out);
  * keys that are absent, remote or already in the tier are skipped.  Their arena bytes become
  * arena_garbage.  The tier is a ring in demotion order: when it comes round, the keys whose records
  * it overwrites are unset, an eviction like cmb200_unset_batch (retired_records).  A record leaves
- * the tier when it is unset, overwritten or retired; promotion back to the arena does not exist. */
+ * the tier when it is unset, overwritten, retired or promoted back to the arena (cmb200_promote_batch).
+ * A promoted record's tier bytes become tier garbage until the ring laps them; its key is not retired
+ * then.  Promotion keeps the put timestamp, which the eviction policy reads. */
 struct cmb200_host_tier_stats {
 	uint64_t bytes, used, records, garbage;     /* tier size; bytes between oldest and newest record; live records; dead bytes */
 	uint64_t demoted_records, demoted_bytes;    /* moved from the arena so far (bytes = record lengths) */
 	uint64_t retired_records;                   /* keys unset because the ring overwrote their records */
 	uint64_t hits;                              /* gets answered from the tier */
+	uint64_t promoted_records, promoted_bytes;  /* moved back to the arena so far (bytes = record lengths) */
 };
 int cmb200_host_tier_enable(cmb200_engine *e, uint64_t bytes);
 int cmb200_demote_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *demoted_out);
 /* all zero for an engine without a tier */
 int cmb200_host_tier_stats(cmb200_engine *e, struct cmb200_host_tier_stats *out);
+/* Moves the host-tier records of the named keys back into the HBM arena (*promoted_out = how many).
+ * Keys that are absent, remote or already in the arena are skipped; a key named twice moves once.
+ * Only free arena bytes are used: keys are taken in array order while their records fit between the
+ * bump pointer and the end of the arena; the rest stay in the tier (no eviction, demotion or
+ * compaction happens inside this call).  Keys, records, statuses and counters are unchanged. */
+int cmb200_promote_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *promoted_out);
+/* Addresses read from the host tier since the last call, newest first, distinct, at most max
+ * (*n_out); *lost_out (nullable) = hits that the log overwrote before they were drained.  The engine
+ * logs the last 4096 tier hits of cmb200_get_batch and cmb200_get_small in a device ring without a
+ * lock, so an address may be stale; cmb200_promote_batch checks every address it is given.  Empty
+ * for an engine without a tier. */
+int cmb200_host_tier_hot(cmb200_engine *e, size_t max, cmb200_addr *addr_out, size_t *n_out, uint64_t *lost_out);
 
 /* ---- multi-GPU: chunks sharded round-robin over ranks, one replicated key index per GPU ----
  * Each rank puts its own shard with the chunks' GLOBAL stream positions as sequence numbers

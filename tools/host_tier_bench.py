@@ -3,10 +3,13 @@
   1. demotion rate (cmb200_demote_batch), GiB/s of records, for incompressible (R) and text-like (T) pages;
   2. cmb200_get_small latency at 1..256 pages per call and cmb200_get_batch GiB/s, for the same pages in
      the HBM arena and in the host tier;
-  3. drop-in cachemap_put_batch rate with a working set 4x the arena, host tier on and off (alternated).
+  3. drop-in cachemap_put_batch rate with a working set 4x the arena, host tier on and off (alternated);
+  4. promotion rate (cmb200_promote_batch), GiB/s of records, 8 192 R or T records per call, and the
+     cmb200_get_small latency of the same keys in the tier and after their promotion.
 
 Every shape is warmed up first and every figure is repeated to show its spread.  The card's name and
-power limit are recorded with the numbers.  usage: python tools/host_tier_bench.py [--out FILE.json]"""
+power limit are recorded with the numbers.
+usage: python tools/host_tier_bench.py [--only demotion,gets,drop_in,promotion] [--out FILE.json]"""
 from __future__ import annotations
 
 import argparse
@@ -146,17 +149,78 @@ def drop_in(reps=3):
     return res
 
 
+def small_get_us(eng, u, l, k, buf, status, iters=200):
+    """cmb200_get_small of k pages per call over the keys u, l: p10 / p50 / p90 microseconds."""
+    n, times = len(u), []
+    for it in range(iters + 20):                               # 20 warm-up calls of this shape
+        at = (it * k) % (n - k)
+        addr = np.ascontiguousarray(np.stack([u[at:at + k], l[at:at + k]], axis=1))
+        t0 = time.perf_counter()
+        rc = E.lib().cmb200_get_small(eng.h, k, addr.ctypes.data, buf, status.ctypes.data)
+        dt = time.perf_counter() - t0
+        assert rc == 0 and (status[:k] == E.HIT).all()
+        if it >= 20:
+            times.append(dt * 1e6)
+    return [round(float(x), 1) for x in np.percentile(times, [10, 50, 90])]
+
+
+def promotion(kind, reps=4):
+    n = 8192                                                   # 512 MiB of pages per repetition
+    eng = E.Engine(pshift=16, accel=12, capacity=1 << 16, arena_bytes=4 << 30, max_batch=4096,
+                   host_tier_bytes=4 << 30)
+    pages = pages_of(kind, n)
+    u = np.full(n, 1, dtype=np.uint64)
+    l = np.arange(n, dtype=np.uint64)
+    eng.put(u, l, pages)
+    rates = []
+    for rep in range(reps + 1):                                # repetition 0 warms up
+        assert eng.demote(u, l) == n
+        eng.compact()                                          # the arena is empty: every record fits
+        b0 = eng.host_tier_stats()["promoted_bytes"]
+        t0 = time.perf_counter()
+        moved = eng.promote(u, l)
+        dt = time.perf_counter() - t0
+        assert moved == n
+        if rep:
+            rates.append((eng.host_tier_stats()["promoted_bytes"] - b0) / dt / GIB)
+    out, st = eng.get(u, l)
+    assert (st == E.HIT).all() and (out == pages).all()
+    # the same keys read from the tier, then after promotion
+    buf = E.lib().cmb200_host_alloc(256 * BS)
+    status = np.zeros(256, dtype=np.int32)
+    lat = {}
+    assert eng.demote(u, l) == n
+    eng.compact()
+    for k in (1, 64, 256):
+        lat[f"tier_{k}"] = small_get_us(eng, u, l, k, buf, status)
+    assert eng.promote(u, l) == n
+    for k in (1, 64, 256):
+        lat[f"promoted_{k}"] = small_get_us(eng, u, l, k, buf, status)
+    E.lib().cmb200_host_free(buf)
+    rec_kib = eng.host_tier_stats()["promoted_bytes"] / eng.host_tier_stats()["promoted_records"] / 1024
+    eng.close()
+    return {"kind": kind, "record_kib": round(rec_kib, 1), "gib_s": [round(r, 2) for r in rates], "small_us": lat}
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--only", default="demotion,gets,drop_in,promotion", help="sections to run")
     ap.add_argument("--out", help="also write the result here")
     a = ap.parse_args()
+    only = set(a.only.split(","))
     assert E.device_count() > 0, f"no CUDA device: {E.last_error()}"
     res = {"card": card()}
-    res["demotion"] = [demotion_rate("R"), demotion_rate("T")]
-    print(json.dumps(res), flush=True)
-    res["gets"] = gets()
-    print(json.dumps(res["gets"]), flush=True)
-    res["drop_in_put_4x_arena"] = drop_in()
+    if "demotion" in only:
+        res["demotion"] = [demotion_rate("R"), demotion_rate("T")]
+        print(json.dumps(res), flush=True)
+    if "gets" in only:
+        res["gets"] = gets()
+        print(json.dumps(res["gets"]), flush=True)
+    if "promotion" in only:
+        res["promotion"] = [promotion("R"), promotion("T")]
+        print(json.dumps(res["promotion"]), flush=True)
+    if "drop_in" in only:
+        res["drop_in_put_4x_arena"] = drop_in()
     if a.out:
         with open(a.out, "w") as f:
             json.dump(res, f, indent=1)
