@@ -36,7 +36,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_lz4_encode_batch", "cmb200_lz4_decode_batch", "cmb200_fingerprint_batch", "cmb200_fingerprint_dev",
     "cmb200_gen_chunk_host", "cmb200_gen_chunks_dev", "cmb200_gen_stream_ids", "cmb200_gen_addr",
     "cmb200_host_tier_enable", "cmb200_demote_batch", "cmb200_host_tier_stats",
-    "cmb200_promote_batch", "cmb200_host_tier_hot",
+    "cmb200_promote_batch", "cmb200_host_tier_hot", "cmb200_read_checkpoints",
 ]
 
 
@@ -152,6 +152,7 @@ def lib() -> C.CDLL:
         "cmb200_host_tier_stats": (i32, [vp, vp]),
         "cmb200_promote_batch": (i32, [vp, sz, vp, vp]),
         "cmb200_host_tier_hot": (i32, [vp, sz, vp, vp, vp]),
+        "cmb200_read_checkpoints": (i32, [vp, sz, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -286,6 +287,18 @@ def host_tier_stats(handle) -> dict:
     st = HostTierStats()
     _check(lib().cmb200_host_tier_stats(handle, C.byref(st)), "cmb200_host_tier_stats")
     return {n: int(getattr(st, n)) for n, _ in HostTierStats._fields_}
+
+
+def read_checkpoints(handle, u, l):
+    """cmb200_read_checkpoints of an engine handle -> (words [n, 16] uint32, ok [n] int32): word 0 is
+    the tag as stored; ok 1 = valid checkpoints, 0 = a record without them, -1 = absent, remote or
+    no side table."""
+    addr = _addr_array(u, l)
+    n = len(addr)
+    words = np.zeros((n, 16), dtype=np.uint32)
+    ok = np.zeros(n, dtype=np.int32)
+    _check(lib().cmb200_read_checkpoints(handle, n, _ptr(addr), _ptr(words), _ptr(ok)), "cmb200_read_checkpoints")
+    return words, ok
 
 
 class Engine:
@@ -473,6 +486,9 @@ class Engine:
         _check(lib().cmb200_read_fingerprints(self.h, n, _ptr(addr), _ptr(fps), _ptr(ok)),
                "cmb200_read_fingerprints")
         return fps, ok
+
+    def read_checkpoints(self, u, l):
+        return read_checkpoints(self.h, u, l)
 
     def compact(self) -> int:
         """cmb200_compact -> bytes of arena reclaimed."""

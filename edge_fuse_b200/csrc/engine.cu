@@ -1019,6 +1019,28 @@ struct DevBuf {
 	template <class T> T *as() { return (T *)p; }
 };
 
+extern "C" int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint32_t *words_out,
+    int32_t *ok_out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (!e->table.ckpt) {                                // no side table: nothing has checkpoints
+		memset(words_out, 0, n * CKPT_WORDS * 4);
+		for (size_t i = 0; i < n; i++) ok_out[i] = -1;
+		return 0;
+	}
+	DevBuf d_words;
+	if (n && d_words.alloc((size_t)e->max_batch * CKPT_WORDS * 4)) return -1;
+	for (size_t at = 0; at < n; at += e->max_batch) {
+		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
+		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
+		if (launch_read_ckpt(e->table, e->d_addr, m, d_words.as<uint32_t>(), e->d_status, e->st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(words_out + at * CKPT_WORDS, d_words.p, (size_t)m * CKPT_WORDS * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemcpyAsync(ok_out + at, e->d_status, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+	}
+	return 0;
+}
+
 // ---- snapshot: persistence of the cache directory (SURVEY.md 8 f3) ---------------------------
 //
 // The reference's store is persistent because it IS a set of LMDB files under <cachedir>
@@ -1238,18 +1260,26 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 	// linear probing never frees one by itself.
 	if (c[1] > e->table.cap / 8) {
 		TableView fresh = e->table;
-		fresh.slots = nullptr; fresh.fp = nullptr;
+		fresh.slots = nullptr; fresh.fp = nullptr; fresh.ckpt = nullptr;
 		if (cudaMalloc(&fresh.slots, (e->table.cap + 2) * sizeof(Slot)) == cudaSuccess &&
 		    (!e->table.fp || cudaMalloc(&fresh.fp, (e->table.cap + 2) * 16) == cudaSuccess)) {
 			CMB_CHECK(cudaMemsetAsync(fresh.slots, 0, (e->table.cap + 2) * sizeof(Slot), e->st));
 			if (fresh.fp) CMB_CHECK(cudaMemsetAsync(fresh.fp, 0, (e->table.cap + 2) * 16, e->st));
+			// parse checkpoints move with their slots (k_rehash); without room for a second side table
+			// they are dropped instead, and those records are walked by one warp until rewritten
+			const size_t ck_bytes = (e->table.cap + 2) * CKPT_WORDS * 4;
+			if (e->table.ckpt && cudaMalloc(&fresh.ckpt, ck_bytes) != cudaSuccess) {
+				(void)cudaGetLastError();
+				fresh.ckpt = nullptr;
+			}
+			if (fresh.ckpt) CMB_CHECK(cudaMemsetAsync(fresh.ckpt, 0, ck_bytes, e->st));
 			if (launch_rehash(e->table, fresh, e->st)) return -1;
-			// the slots have moved: their parse checkpoints are dropped (those records are walked by one warp)
-			if (e->table.ckpt) CMB_CHECK(cudaMemsetAsync(e->table.ckpt, 0, (e->table.cap + 2) * CKPT_WORDS * 4, e->st));
+			if (e->table.ckpt && !fresh.ckpt) CMB_CHECK(cudaMemsetAsync(e->table.ckpt, 0, ck_bytes, e->st));
 			CMB_CHECK(cudaMemsetAsync(e->d_counters + 1, 0, sizeof(unsigned long long), e->st));   // tombstones
 			CMB_CHECK(cudaStreamSynchronize(e->st));
 			cudaFree(e->table.slots); cudaFree(e->table.fp);
 			e->table.slots = fresh.slots; e->table.fp = fresh.fp;
+			if (fresh.ckpt) { cudaFree(e->table.ckpt); e->table.ckpt = fresh.ckpt; }
 			e->stats.kernel_launches++;
 		} else {
 			(void)cudaGetLastError();                    // no room for a second table: keep the old one

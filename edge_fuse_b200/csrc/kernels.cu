@@ -1344,6 +1344,30 @@ int launch_read_fp(TableView t, const unsigned long long *addr, uint32_t n, uint
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
+__global__ void k_read_ckpt(TableView t, const unsigned long long *addr, uint32_t n, uint32_t *words_out, int32_t *ok) {
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	unsigned long long u = addr[2 * i], l = addr[2 * i + 1];
+	uint32_t idx = table_find(t, fnv_addr(u, l));
+	int32_t found = -1;
+	uint32_t *w = words_out + (size_t)i * CKPT_WORDS;
+	for (uint32_t k = 0; k < CKPT_WORDS; k++) w[k] = 0;
+	if (idx != 0xffffffffu) {
+		const Slot &s = t.slots[idx];
+		if (s.vlen != 0 && s.owner == 0 && s.addr_u == u && s.addr_l == l) {
+			for (uint32_t k = 0; k < CKPT_WORDS; k++) w[k] = t.ckpt[(size_t)idx * CKPT_WORDS + k];
+			found = w[0] == ckpt_tag(s.rec_off, s.vlen - 1u) ? 1 : 0;
+		}
+	}
+	ok[i] = found;
+}
+int launch_read_ckpt(TableView t, const unsigned long long *addr, uint32_t n, uint32_t *words_out, int32_t *ok,
+    cudaStream_t st) {
+	if (n == 0) return 0;
+	k_read_ckpt<<<GRID1D(n), 0, st>>>(t, addr, n, words_out, ok);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
 // ---- snapshot -----------------------------------------------------------------------------
 __global__ void k_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
     unsigned long long max_out, bool arena_only) {
@@ -1370,8 +1394,67 @@ int launch_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned l
 	return 0;
 }
 
-__global__ void __launch_bounds__(256) k_restore(EncodeJob job, const uint8_t *blob, const unsigned long long *off,
+// Parse checkpoints of a block that arrives without them (a snapshot record), by walking its token
+// chain: the same words as the encoder's (lz4_encode_lean), lane k gets word k.  Every lane walks
+// the same chain out of a per-warp window of the block in shared memory, which the warp refills
+// when the walk leaves it; only [blk, blk + clen) is read.  The block is untrusted: a chain that
+// does not end exactly at (consumed == clen, output == n), or whose runs pass the page end, gives
+// false and no checkpoints.
+constexpr uint32_t RESTORE_WARPS = 8, RESTORE_WIN = 1024;
+__device__ bool restore_ckpt_walk(const uint8_t *blk, uint32_t clen, uint32_t n, uint8_t *win, int lane, uint32_t &ck) {
+	const uint32_t S = n / CKPT_WORDS;
+	uint32_t ip = 0, op = 0, k = 1, wb = 0, we = 0;
+	ck = 0xffffffffu;
+	// byte p of the block, p < clen; positions only grow along the chain
+	auto at = [&](uint32_t p) -> uint32_t {
+		if (p >= we) {
+			__syncwarp();
+			wb = p; we = min(p + RESTORE_WIN, clen);
+			for (uint32_t q = wb + (uint32_t)lane; q < we; q += 32u) win[q - wb] = blk[q];
+			__syncwarp();
+		}
+		return win[p - wb];
+	};
+	for (;;) {
+		// a sequence starts at token ip, its literals at output position op
+		for (; k < CKPT_WORDS && op >= k * S; k++)
+			if ((uint32_t)lane == k) ck = op - k * S < S ? (ip << CKPT_POS_BITS) | (op - k * S) : 0xffffffffu;
+		if (ip >= clen) return false;
+		const uint32_t tok = at(ip++);
+		uint32_t lit = tok >> 4;
+		if (lit == 15u) {
+			uint32_t b;
+			do {
+				if (ip >= clen) return false;
+				b = at(ip++);
+				lit += b;
+			} while (b == 255u && lit <= n);
+		}
+		if (lit > n - op || lit > clen - ip) return false;
+		ip += lit; op += lit;
+		if (ip == clen) break;                              // the last literals
+		if (clen - ip < 2u) return false;
+		ip += 2;                                            // match offset
+		uint32_t mlen = tok & 15u;
+		if (mlen == 15u) {
+			uint32_t b;
+			do {
+				if (ip >= clen) return false;
+				b = at(ip++);
+				mlen += b;
+			} while (b == 255u && mlen <= n);
+		}
+		if (mlen + 4u > n - op) return false;
+		op += mlen + 4u;
+	}
+	if (op != n) return false;
+	for (; k < CKPT_WORDS; k++) if ((uint32_t)lane == k) ck = 0xffffffffu;   // no sequence starts at or after k * S
+	return true;
+}
+
+__global__ void __launch_bounds__(RESTORE_WARPS * 32) k_restore(EncodeJob job, const uint8_t *blob, const unsigned long long *off,
     const uint64_t *fps, uint32_t bsize) {
+	__shared__ uint8_t win[RESTORE_WARPS][RESTORE_WIN];
 	const int lane = threadIdx.x & 31;
 	const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
 	if (i >= job.n) return;
@@ -1380,12 +1463,19 @@ __global__ void __launch_bounds__(256) k_restore(EncodeJob job, const uint8_t *b
 	const uint8_t *rec = blob + off[i];
 	const int32_t clen = *reinterpret_cast<const int32_t *>(rec + 16);   // data_prefix.compressed_length (filemap.c:9-12); off[] is 16-aligned
 	const uint32_t plen = clen > 0 ? (uint32_t)clen : bsize;
-	commit_record(job, i, idx, rec + 24, plen, clen, true, fps ? fps[2 * i] : 0ull, fps ? fps[2 * i + 1] : 0ull, lane);
+	const unsigned long long at =
+	    commit_record(job, i, idx, rec + 24, plen, clen, true, fps ? fps[2 * i] : 0ull, fps ? fps[2 * i + 1] : 0ull, lane);
+	// the encoder's checkpoints, rebuilt from the block (raw pages have none); slot_publish has zeroed
+	// the tag, so a block that does not walk leaves the record to the one-warp parse of k_get_small
+	if (at == ~0ull || clen <= 0 || !job.table.ckpt) return;
+	uint32_t ck;
+	if (restore_ckpt_walk(rec + 24, (uint32_t)clen, bsize, win[threadIdx.x >> 5], lane, ck))
+		ckpt_store(job, idx, at, (uint32_t)clen, ck, lane);
 }
 int launch_restore(const EncodeJob &job, const uint8_t *blob, const unsigned long long *off,
     const uint64_t *fps, uint32_t bsize, cudaStream_t st) {
 	if (job.n == 0) return 0;
-	k_restore<<<(job.n * 32 + 255) / 256, 256, 0, st>>>(job, blob, off, fps, bsize);
+	k_restore<<<(job.n + RESTORE_WARPS - 1) / RESTORE_WARPS, RESTORE_WARPS * 32, 0, st>>>(job, blob, off, fps, bsize);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
@@ -1411,6 +1501,15 @@ __global__ void __launch_bounds__(256) k_compact_scatter(TableView t, ArenaView 
 		Slot &s = t.slots[m.slot];
 		s.rec_off = m.new_off;
 		s.alloc = (m.len + 15u) & ~15u;
+		if (t.ckpt) {
+			// the block is unchanged, so are its checkpoints: only the tag moves (as in k_demote_publish)
+			const uint32_t clen = s.vlen - 1u;
+			uint32_t *w = t.ckpt + (size_t)m.slot * CKPT_WORDS;
+			if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(m.old_off, clen)) {
+				__threadfence();
+				*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(m.new_off, clen);
+			}
+		}
 	}
 }
 int launch_compact_window(TableView t, ArenaView a, const MoveEntry *moves, uint32_t n, uint8_t *bounce,
@@ -1571,6 +1670,9 @@ __global__ void k_rehash(TableView from, TableView to) {
 	t.addr_u = d.addr_u; t.addr_l = d.addr_l; t.rec_off = d.rec_off; t.vlen = d.vlen; t.alloc = d.alloc;
 	t.ts = d.ts; t.seq = d.seq; t.owner = d.owner;
 	if (from.fp && to.fp) { to.fp[2 * (size_t)idx] = from.fp[2 * i]; to.fp[2 * (size_t)idx + 1] = from.fp[2 * i + 1]; }
+	// the tag names rec_off and the length, which stay: the parse checkpoints move with the slot
+	if (from.ckpt && to.ckpt)
+		for (uint32_t k = 0; k < CKPT_WORDS; k++) to.ckpt[(size_t)idx * CKPT_WORDS + k] = from.ckpt[i * CKPT_WORDS + k];
 }
 int launch_rehash(TableView from, TableView to, cudaStream_t st) {
 	const uint64_t n = from.cap + 2;

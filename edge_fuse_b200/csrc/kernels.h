@@ -218,6 +218,10 @@ int launch_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned
 
 int launch_read_fp(TableView t, const unsigned long long *addr, uint32_t n, uint64_t *fp_out, int32_t *ok,
     cudaStream_t st);
+// words_out[CKPT_WORDS i + k] = checkpoint word k of the key's slot (t.ckpt must be set); ok[i] = 1: a local
+// record whose tag names it, 0: a local record without valid checkpoints, -1: absent or remote.
+int launch_read_ckpt(TableView t, const unsigned long long *addr, uint32_t n, uint32_t *words_out, int32_t *ok,
+    cudaStream_t st);
 
 int launch_streamgen(const uint64_t *cids, uint32_t n, uint64_t seed, uint32_t bsize, uint8_t *out,
     cudaStream_t st);

@@ -13,9 +13,10 @@
 //   1. PARSE    up to 16 warps walk 16 sections of the token chain at once.  Where a section starts
 //               cannot be found without walking — so the ENCODER leaves 15 checkpoints per record
 //               (block offset + output position of the first sequence at or after k/16 of the page;
-//               a side table indexed by slot, kernels.cu:ckpt_store) and a record without usable
-//               checkpoints (imported, loaded from a snapshot, moved by compaction, another GPU's)
-//               is walked by one warp.  Each sequence becomes a 16-byte descriptor in a scratch
+//               a side table indexed by slot, kernels.cu:ckpt_store; rebuilt from the block when a
+//               snapshot is loaded, kernels.cu:restore_ckpt_walk; kept by compaction and table
+//               rebuilds) and a record without usable checkpoints (a raw page, another GPU's, a
+//               loaded block whose chain does not fit) is walked by one warp.  Each sequence becomes a 16-byte descriptor in a scratch
 //               region in global memory (L2): {literal source, output position, literal length,
 //               offset | (match length - 4) << 16}; offset 0 marks the last sequence.
 //               Every section must end exactly where the next one starts, the last at

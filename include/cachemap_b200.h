@@ -155,7 +155,10 @@ int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out);
  * attribute and fingerprint — to one file (written to path.tmp, then renamed); cmb200_load puts
  * the records of such a file into the store as if they had been put in file order (existing keys
  * are overwritten).  The format (engine.cu) is independent of capacity and arena size; the page
- * size must match.  Both return 0 on success, -1 with cmb200_last_error() otherwise. */
+ * size must match.  The file holds no parse checkpoints: cmb200_load rebuilds them from each LZ4
+ * block, so a loaded record is read by cmb200_get_small as fast as a freshly put one (a block whose
+ * token chain does not add up to the page gets none and is walked by one warp).
+ * Both return 0 on success, -1 with cmb200_last_error() otherwise. */
 int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records_out);
 int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out);
 
@@ -277,6 +280,10 @@ int cmb200_fingerprint_batch(int device, const void *pages_host, size_t n, uint3
     size_t stride, uint64_t *fp_out);
 /* EF128 of n pages resident in the engine's HBM (1<<pshift bytes each); fp_out on the host. */
 int cmb200_fingerprint_dev(cmb200_engine *e, size_t n, const void *pages_dev, uint64_t *fp_out_host);
+/* Parse checkpoints of the stored records: words_out[16 i + k] = word k (word 0 = tag as stored).
+ * ok_out[i] = 1: the key's record is local and word 0 names its location and length;
+ * 0: the key has a record without valid checkpoints; -1: absent, remote, or no side table. */
+int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint32_t *words_out, int32_t *ok_out);
 
 /* ---- synthetic streams (SURVEY.md §8d), same definition on host and device ---- */
 void cmb200_gen_chunk_host(uint64_t seed, uint64_t cid, uint32_t bsize, void *out);
