@@ -558,6 +558,10 @@ __global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WAR
 			if (in_arena) dst = job.arena.base + base + 24;
 		}
 		uint32_t clen, ck = 0xffffffffu;
+#ifdef CMB_ENC_PHASES
+		if (lane == 0) s_enc_phase_row[warp] = g_enc_phases && gw % 4u == 0u ? g_enc_phases + 2u * ENC_PH_N * (size_t)i : nullptr;
+		__syncwarp();
+#endif
 		if (job.fps) {                  // fingerprint along the parse frontier: the page is read once
 			clen = lz4_encode_lean<WIDE, true, ENC == 1>(src, job.nbytes, dst, job.accel, wsm, ring, lane, fp_hi, fp_lo, ck);
 			if (lane == 0) { job.fps[2 * (size_t)i] = fp_hi; job.fps[2 * (size_t)i + 1] = fp_lo; }
@@ -633,6 +637,12 @@ int launch_encode(const EncodeJob &job_in, cudaStream_t st) {
 #ifdef CMB_ENC_TIMELINE
 extern "C" int cmb200_enc_timeline(void *buf) {       // n x 4 u64, see g_enc_timeline; null = off
 	return cudaMemcpyToSymbol(g_enc_timeline, &buf, sizeof(buf)) == cudaSuccess ? 0 : -1;
+}
+#endif
+#ifdef CMB_ENC_PHASES
+extern "C" int cmb200_enc_phases(void *buf, uint32_t *nphases) {   // n x 2 x ENC_PH_N u64, see g_enc_phases; null = off
+	if (nphases) *nphases = ENC_PH_N;
+	return cudaMemcpyToSymbol(g_enc_phases, &buf, sizeof(buf)) == cudaSuccess ? 0 : -1;
 }
 #endif
 

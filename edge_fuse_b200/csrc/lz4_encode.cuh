@@ -135,10 +135,19 @@ __device__ __noinline__ uint32_t lz4_count_long(const uint8_t *src, uint32_t a, 
 		if (pa < lim) {
 			const uint32_t avail = min(16u, lim - pa);
 			const uint32_t pb = b + total + 16u * lane;
+			// both 16-byte windows are loaded at once (one L2 round trip per step), then compared
+			uint32_t wa[5], wb[5];
+			const uint32_t qa = pa & ~3u, qb = pb & ~3u;
+#pragma unroll
+			for (uint32_t k = 0; k < 5; k++) {
+				wa[k] = qa + 4u * k < lim4 ? ldg32(src + qa + 4u * k) : 0u;
+				wb[k] = qb + 4u * k < lim4 ? ldg32(src + qb + 4u * k) : 0u;
+			}
 #pragma unroll
 			for (uint32_t j = 0; j < 4; j++) {
-				if (nb == 4u * j && 4u * j < avail) {
-					uint32_t x = read32u(src, pa + 4u * j, lim4) ^ read32u(src, pb + 4u * j, lim4);
+				if (nb == 4u * j) {
+					const uint32_t x = __funnelshift_r(wa[j], wa[j + 1], (pa & 3u) * 8u) ^
+					    __funnelshift_r(wb[j], wb[j + 1], (pb & 3u) * 8u);
 					nb += x ? (uint32_t)(__ffs(x) - 1) >> 3 : 4u;
 				}
 			}
@@ -224,7 +233,7 @@ __device__ __noinline__ uint32_t lz4_emit_general(uint8_t *dst, uint32_t op, con
 	if (lane == 0) dst[op] = (uint8_t)((min(lit, 15u) << 4) | min(mc, 15u));
 	op++;
 	if (lit >= 15u) op = lz4_emit_len(dst, op, lit - 15u, lane);
-	if (lit <= 256u) {           // the usual case here is a run of 65..200 bytes: bytes, no alignment work
+	if (lit <= 256u) {           // the usual case here is a run of 129..256 bytes: bytes, no alignment work
 		for (uint32_t i = lane; i < lit; i += 32) st_out8(dst + op + i, ldg8(src + anchor + i));
 	} else {
 		warp_copy_ro(dst + op, src + anchor, lit, lane);
@@ -246,18 +255,20 @@ __device__ __forceinline__ void st_out8_if(bool p, uint8_t *ptr, uint32_t v) {
 }
 
 // Writes one sequence — token, literal run, offset and match length (lz4.c:625-683) — at dst[op..),
-// lz4_seq_bytes(lit, mc) bytes.  A run of at most 64 literals comes from registers (b0 = src[from +
-// lane], b1 = src[from + 32 + lane], loaded by the batch that found the match) and is written by
-// predicated lane stores; longer runs and long lengths go to lz4_emit_general, which reads the
-// literals from the page in global memory.
+// lz4_seq_bytes(lit, mc) bytes.  A run of at most LZ4_LIT_REG literals comes from a register (lw =
+// src[from + 4 lane .. + 4), little-endian, loaded by the batch that found the match) and is written
+// by predicated lane stores; longer runs and long lengths go to lz4_emit_general, which reads the
+// literals from the page in global memory (an L2 round trip on the parse's path).
+constexpr uint32_t LZ4_LIT_REG = 128;
 __device__ __forceinline__ void lz4_emit_seq(uint8_t *dst, const uint8_t *src, uint32_t op, uint32_t from, uint32_t lit,
-    uint32_t off, uint32_t mc, uint32_t b0, uint32_t b1, int lane) {
-	if (lit <= 64u && mc < 15u + 255u) {
+    uint32_t off, uint32_t mc, uint32_t lw, int lane) {
+	if (lit <= LZ4_LIT_REG && mc < 15u + 255u) {
 		uint8_t *o = dst + op;
 		const uint32_t lext = lit >= 15u, mext = mc >= 15u;
 		const uint32_t hl = 1u + lext;
-		st_out8_if((uint32_t)lane < lit, o + hl + lane, b0);
-		st_out8_if((uint32_t)lane + 32u < lit, o + hl + 32u + lane, b1);
+		const uint32_t l4 = 4u * (uint32_t)lane;
+#pragma unroll
+		for (uint32_t k = 0; k < 4; k++) st_out8_if(l4 + k < lit, o + hl + l4 + k, lw >> (8u * k));
 		const uint32_t tail = hl + lit;
 		const uint32_t head4 = (min(lit, 15u) << 4) | min(mc, 15u) | (((lit - 15u) & 0xffu) << 8) | (off << 16);
 		const uint32_t val = lane < 4 ? head4 >> (8u * (uint32_t)lane) : mc - 15u;

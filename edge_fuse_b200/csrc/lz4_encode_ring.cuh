@@ -157,6 +157,44 @@ __device__ __forceinline__ Lz4Around ring_around(const uint8_t *ring, uint32_t p
 	return r;
 }
 
+#ifdef CMB_ENC_PHASES   /* diagnostic builds only (tools/encode_phases.py) */
+// Where the cycles of one parse iteration go.  Lane 0 of every fourth resident warp slot stamps
+// clock64() at fixed points of each iteration and adds the cycles since its previous stamp to the
+// phase that has just ended (a warp issues in order, so a stamp counts every stall of the
+// instructions before it).  Row per chunk: ENC_PH_N cycle sums, then ENC_PH_N counts.
+enum : uint32_t {
+	ENC_PH_HEAD,           // end of the previous iteration -> past the loop-head test (events excluded)
+	ENC_PH_EVENTS,         // checkpoint / ring / fingerprint events
+	ENC_PH_TABLE,          // ring read, hash, table get / put, candidate-load issue, read-back
+	ENC_PH_EMIT,           // deferred emit, fast path
+	ENC_PH_WAIT,           // literal bytes, candidate bytes' first use, the two ballots
+	ENC_PH_RESOLVE,        // winner, shuffles, undo stores, next anchor
+	ENC_PH_SEARCH_SLOW,    // lz4_search_slow
+	ENC_PH_COUNT_LONG,     // lz4_count_long
+	ENC_PH_CATCHUP_LONG,   // lz4_catchup_long
+	ENC_PH_EMIT_GENERAL,   // lz4_emit_general (deferred emit, long runs)
+	ENC_PH_N
+};
+__device__ unsigned long long *g_enc_phases;   // null = off
+__shared__ unsigned long long *s_enc_phase_row[32];   // per warp of the CTA: its chunk's row, or null
+struct EncPhaseClock {
+	unsigned long long *row;
+	unsigned long long t;
+	__device__ __forceinline__ void start(int lane) {
+		row = lane == 0 ? s_enc_phase_row[threadIdx.x >> 5] : nullptr;
+		t = clock64();
+	}
+	__device__ __forceinline__ void mark(uint32_t ph) {
+		const unsigned long long now = clock64();
+		if (row) { atomicAdd(row + ph, now - t); atomicAdd(row + ENC_PH_N + ph, 1ull); }
+		t = now;
+	}
+};
+#define ENC_PHASE(ph) phc.mark(ph)
+#else
+#define ENC_PHASE(ph) do {} while (0)
+#endif
+
 // Encodes src[0,n) into dst; returns the block length (uniform across the warp).  tab_smem = this
 // warp's LZ4_TABLE_BYTES of shared memory; src must be 4-byte aligned and readable up to 16 bytes
 // past src + n (the library's page buffers are contiguous and padded); with FP, 16-byte aligned.  With FP the EF128
@@ -230,10 +268,15 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 		// reads: the emit's stores and arithmetic (its size included) then fill the L2 round trip instead
 		// of standing between one batch and the next.  From the top of an iteration to its deferred
 		// emit, if `started`, one sequence is pending: it starts at dst[op] and at page position
-		// anchor - LZ4_MIN_MATCH - p_mc - p_lit, and its first 64 literal bytes are in litbyte / litbyte2.
-		uint32_t p_lit = 0, p_off = 0, p_mc = 0, litbyte = 0, litbyte2 = 0;
+		// anchor - LZ4_MIN_MATCH - p_mc - p_lit, and its first LZ4_LIT_REG literal bytes are in litw.
+		uint32_t p_lit = 0, p_off = 0, p_mc = 0, litw = 0;
+#ifdef CMB_ENC_PHASES
+		EncPhaseClock phc;
+		phc.start(lane);
+#endif
 		for (;;) {
 			if (anchor >= next_event) {
+				ENC_PHASE(ENC_PH_HEAD);
 				// a sequence starts at or after the next checkpoint position: this is the one to note
 				while (anchor >= ck_at) {
 					const uint32_t rel = anchor - ck_at;
@@ -272,7 +315,9 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 				if (FP) fp.upto(src, anchor + 512u, lane);
 				}
 				next_event = min(ring_next, ck_at);
+				ENC_PHASE(ENC_PH_EVENTS);
 			}
+			ENC_PHASE(ENC_PH_HEAD);
 			const bool en = anchor < en_below && (uint32_t)lane < width;
 			const uint32_t pos = en ? anchor + delta2 : 0u;        // disabled lanes read (and ignore) position 0 / ring offset 0
 			const Lz4Around ai = RING ? ring_around(rb, pos) : lz4_around(src, pos);
@@ -287,23 +332,30 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 			Lz4Words acw = lz4_around_load(src, cand);   // latency overlaps the read-back and the emit below
 			const uint32_t seen = tab.get(h);
 			__syncwarp();                                           // read-backs done before any undo store
+			ENC_PHASE(ENC_PH_TABLE);
 
 			// ---- deferred emit of the pending sequence, while the candidate reads are in flight ----
 			// It needs nothing of this batch: the fast path stores registers only, lz4_emit_general reads
 			// the page from global memory (never from the ring, whose buffers the loop head recycles).
 			if (started) {
-				lz4_emit_seq(dst, src, op, anchor - LZ4_MIN_MATCH - p_mc - p_lit, p_lit, p_off, p_mc, litbyte, litbyte2, lane);
+				lz4_emit_seq(dst, src, op, anchor - LZ4_MIN_MATCH - p_mc - p_lit, p_lit, p_off, p_mc, litw, lane);
 				op += lz4_seq_bytes(p_lit, p_mc);
+				ENC_PHASE(p_lit <= LZ4_LIT_REG && p_mc < 15u + 255u ? ENC_PH_EMIT : ENC_PH_EMIT_GENERAL);
 			}
-			// speculative literal bytes of the sequence this batch resolves: src[anchor + lane],
-			// src[anchor + 32 + lane] (used when the run is <= 64 bytes; never stored beyond the literal
-			// run, so reading past the page end is harmless in the ring)
-			if (RING) {
-				litbyte = rb[(anchor + (uint32_t)lane) & (RING_BYTES - 1u)];
-				litbyte2 = rb[(anchor + 32u + (uint32_t)lane) & (RING_BYTES - 1u)];
-			} else {
-				litbyte = ldg8(src + min(anchor + (uint32_t)lane, n - 1u));
-				litbyte2 = ldg8(src + min(anchor + 32u + (uint32_t)lane, n - 1u));
+			// speculative literal bytes of the sequence this batch resolves: src[anchor + 4 lane .. + 4)
+			// (used when the run is <= LZ4_LIT_REG bytes; never stored beyond the literal run, so what a
+			// lane reads past the page end does not matter).  In the ring: two aligned words inside the
+			// resident [anchor - 4, anchor + RING_AHEAD), the mirror absorbing the wrap; from the page: a
+			// lane past the end reads the last word instead (pages are padded by 16 bytes).
+			{
+				const uint32_t sh = (anchor & 3u) * 8u;
+				if (RING) {
+					const uint32_t *q = reinterpret_cast<const uint32_t *>(rb + (((anchor & ~3u) + 4u * (uint32_t)lane) & (RING_BYTES - 1u)));
+					litw = __funnelshift_r(q[0], q[1], sh);
+				} else {
+					const uint32_t a = min((anchor & ~3u) + 4u * (uint32_t)lane, (n - 1u) & ~3u);
+					litw = __funnelshift_r(ldg32(src + a), ldg32(src + a + 4u), sh);
+				}
 			}
 			// The candidate words are first used here, behind the emit (the compiler would otherwise align
 			// them right after the loads, and the warp would wait for the L2 before emitting).
@@ -328,6 +380,7 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 			uint32_t ip, match, fwd, back;
 			bool retest_hit;
 			if (low_hit - 1u < low_for - 1u) {
+				ENC_PHASE(ENC_PH_WAIT);
 				const int w = __ffs(hits) - 1;
 				const uint32_t pos_w = __shfl_sync(CMB_FULL, pos, w);
 				if (en && lane > w && !(foreign && seen <= (WIDE ? pos_w : (pos_w & 0xffffu)))) tab.put(h, cand);
@@ -340,11 +393,18 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 				calm = w < NARROW_HIT ? calm + 1u : 0u;
 				if (w >= NARROW_HIT) width = 32u; else if (calm >= 8u) width = NARROW_W;
 				if (fwd == 4u || back == 4u) {                      // longer than the neighbourhoods show: rare
-					if (fwd == 4u) fwd = 4u + lz4_count_long(src, ip + 8u, match + 8u, mlimit, lim4, lane);
-					if (back == 4u && ip >= anchor + 5u && match >= 5u)
+					ENC_PHASE(ENC_PH_RESOLVE);
+					if (fwd == 4u) {
+						fwd = 4u + lz4_count_long(src, ip + 8u, match + 8u, mlimit, lim4, lane);
+						ENC_PHASE(ENC_PH_COUNT_LONG);
+					}
+					if (back == 4u && ip >= anchor + 5u && match >= 5u) {
 						back = 4u + lz4_catchup_long(src, ip - 4u, match - 4u, anchor, lane);
+						ENC_PHASE(ENC_PH_CATCHUP_LONG);
+					}
 				}
 			} else {
+				ENC_PHASE(ENC_PH_WAIT);
 				uint64_t res = 0;
 				// lanes of this batch that were held back only by the end margin (not by the batch width)
 				const uint32_t enmask = __ballot_sync(CMB_FULL, en || special || (uint32_t)lane >= width);
@@ -357,12 +417,15 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 				} else if (enmask == CMB_FULL) {                     // the probes of this batch were not enough
 					res = lz4_search_slow<WIDE>(src, lim4, tab, anchor, 2u, accel, mflimit, w0, lane, started);
 				}
+				ENC_PHASE(ENC_PH_SEARCH_SLOW);
 				if (!(res >> 63)) break;                             // -> last literals (nothing pending)
 				retest_hit = (res >> 62) & 1u;
 				ip = (uint32_t)(res >> 32) & 0x3fffffffu;
 				match = (uint32_t)res;
 				fwd = lz4_count_long(src, ip + LZ4_MIN_MATCH, match + LZ4_MIN_MATCH, mlimit, lim4, lane);
+				ENC_PHASE(ENC_PH_COUNT_LONG);
 				back = retest_hit ? 0u : lz4_catchup_long(src, ip, match, anchor, lane);
+				ENC_PHASE(ENC_PH_CATCHUP_LONG);
 			}
 			// ---- the sequence becomes the pending one (emitted by the next iteration) ----
 			p_off = ip - match;
@@ -373,13 +436,14 @@ __device__ uint32_t lz4_encode_lean(const uint8_t *__restrict__ src, uint32_t n,
 			anchor = end;
 			started = true;
 			en_below |= special_on;
+			ENC_PHASE(ENC_PH_RESOLVE);
 			if (end > mflimit) break;                     // lz4.c:688
 		}
 		// Still pending when the loop stopped at the end margin (anchor = end > mflimit).  A search that
 		// ran into the margin has already emitted its predecessor (its anchor is <= mflimit).  Either way
 		// the whole block is written before this function returns (and dst may be the arena).
 		if (started && anchor > mflimit) {
-			lz4_emit_seq(dst, src, op, anchor - LZ4_MIN_MATCH - p_mc - p_lit, p_lit, p_off, p_mc, litbyte, litbyte2, lane);
+			lz4_emit_seq(dst, src, op, anchor - LZ4_MIN_MATCH - p_mc - p_lit, p_lit, p_off, p_mc, litw, lane);
 			op += lz4_seq_bytes(p_lit, p_mc);
 		}
 		if (RING) ring_drain(ring);
