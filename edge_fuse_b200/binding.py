@@ -18,7 +18,7 @@ EXPORTED_SYMBOLS = [
     # cachemap.h — reference cachemap/cachemap.h:33-47 + batch extension
     "cachemap_create", "cachemap_free", "cachemap_get", "cachemap_put", "cachemap_put_async",
     "cachemap_print_stats", "cachemap_put_batch", "cachemap_get_batch", "cachemap_put_batch_dev",
-    "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine",
+    "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
@@ -37,6 +37,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_gen_chunk_host", "cmb200_gen_chunks_dev", "cmb200_gen_stream_ids", "cmb200_gen_addr",
     "cmb200_host_tier_enable", "cmb200_demote_batch", "cmb200_host_tier_stats",
     "cmb200_promote_batch", "cmb200_host_tier_hot", "cmb200_read_checkpoints",
+    "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
 ]
 
 
@@ -90,6 +91,7 @@ def lib() -> C.CDLL:
         "cachemap_get_batch_dev": (None, [vp, u64, vp, vp, vp, vp, vp]),
         "cachemap_get_counters": (None, [vp, vp, vp]),
         "cachemap_engine": (vp, [vp]),
+        "cachemap_engines": (i32, [vp, vp, i32]),
         "cachemap_checkpoint": (i32, [vp]),
         "cachemap_read_range": (i32, [vp, u64, u32, u64, sz, vp]),
         "cachemap_write_range": (None, [vp, u64, u32, u64, sz, vp]),
@@ -153,6 +155,11 @@ def lib() -> C.CDLL:
         "cmb200_promote_batch": (i32, [vp, sz, vp, vp]),
         "cmb200_host_tier_hot": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_read_checkpoints": (i32, [vp, sz, vp, vp, vp]),
+        "cmb200_owner": (i32, [u64, i32]),
+        "cmb200_save_set": (i32, [vp, i32, C.c_char_p, vp]),
+        "cmb200_load_set": (i32, [vp, i32, C.c_char_p, vp]),
+        "cmb200_move_pages": (i32, [vp, sz, vp, vp, vp, vp]),
+        "cmb200_copy_peer": (i32, [vp, vp, vp, vp, sz]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -506,6 +513,12 @@ class Engine:
         _check(lib().cmb200_load(self.h, path.encode(), C.byref(n)), "cmb200_load")
         return n.value
 
+    def move_pages(self, n: int, dst_dev: int, src_dev: int, dst_idx=None, src_idx=None):
+        """cmb200_move_pages: dst[dst_idx[i] or i] = src[src_idx[i] or i], n pages in this engine's HBM."""
+        di = None if dst_idx is None else np.ascontiguousarray(dst_idx, dtype=np.uint32)
+        si = None if src_idx is None else np.ascontiguousarray(src_idx, dtype=np.uint32)
+        _check(lib().cmb200_move_pages(self.h, n, dst_dev, _ptr(di), src_dev, _ptr(si)), "cmb200_move_pages")
+
     def set_stream_order(self, next_seq: int, stride: int):
         _check(lib().cmb200_set_stream_order(self.h, next_seq, stride), "cmb200_set_stream_order")
 
@@ -557,6 +570,32 @@ class Engine:
     def gen_chunks_dev(self, seed: int, cids, out_dev: int):
         cids = np.ascontiguousarray(cids, dtype=np.uint64)
         _check(lib().cmb200_gen_chunks_dev(self.h, seed, _ptr(cids), len(cids), out_dev), "cmb200_gen_chunks_dev")
+
+
+def owner(key: int, g: int) -> int:
+    """cmb200_owner: which of g engines holds the store key `key` (FNV-1a-64 of the address)."""
+    return int(lib().cmb200_owner(key, g))
+
+
+def _handles(handles):
+    arr = (C.c_void_p * len(handles))(*handles)
+    return arr, len(handles)
+
+
+def save_set(handles, path: str) -> int:
+    """cmb200_save_set over engine handles -> records written."""
+    arr, g = _handles(handles)
+    n = C.c_uint64(0)
+    _check(lib().cmb200_save_set(arr, g, path.encode(), C.byref(n)), "cmb200_save_set")
+    return n.value
+
+
+def load_set(handles, path: str) -> int:
+    """cmb200_load_set over engine handles -> records loaded."""
+    arr, g = _handles(handles)
+    n = C.c_uint64(0)
+    _check(lib().cmb200_load_set(arr, g, path.encode(), C.byref(n)), "cmb200_load_set")
+    return n.value
 
 
 class Cachemap:
@@ -632,6 +671,12 @@ class Cachemap:
 
     def engine_handle(self) -> int:
         return int(lib().cachemap_engine(self.h) or 0)
+
+    def engine_handles(self) -> list:
+        """Every engine of the map (one per CMB200_DEVICES entry), first = engine_handle()."""
+        out = (C.c_void_p * 64)()
+        n = lib().cachemap_engines(self.h, out, 64)
+        return [int(out[i]) for i in range(min(n, 64))]
 
 
 _LIBC = None

@@ -3,7 +3,7 @@
  * engine.  Host code stays C; everything heavy happens in the engine's kernels.
  *
  * What each reference function became:
- *   filemap_create/free        cachemap/filemap.c:35-110   -> config only; engine built lazily
+ *   filemap_create/free        cachemap/filemap.c:35-110   -> config only; engines built lazily
  *   filemap_set                cachemap/filemap.c:112-158  -> WRITE-BEHIND: the page is copied into a
  *                              page-locked ring and the call returns; one flusher thread hands the
  *                              ring to the GPU in batches.  A single chunk takes the GPU 0.2-3 ms
@@ -17,7 +17,15 @@
  *   cachemap_*                 cachemap/cachemap.c:107-239 -> same logic: address composition,
  *                              timestamps, counters; evict-oldest-of-3 runs in the flusher before
  *                              each batch; put_async == put (both are write-behind now)
- * There is no CPU fallback: if the engine cannot be created the process stops with a message
+ *
+ * One map, several GPUs (CMB200_DEVICES): the reference already splits its store into 32 shards by
+ * key and no call but filemap_entries crosses shards (filemap.c:26-33).  Here the map owns one engine
+ * per listed device and every key lives on exactly one of them, cmb200_owner(key, G).  Each engine
+ * has its own write-behind ring and flusher, combining queue, host tier and promotion state (struct
+ * fm_dev); the map keeps the capacity, the counters, the eviction decision and persistence.  Without
+ * CMB200_DEVICES there is one engine on CMB200_DEVICE: G = 1 of the same code.
+ *
+ * There is no CPU fallback: if an engine cannot be created the process stops with a message
  * (set CMB200_SOFT_FAIL=1 to degrade to "every put dropped, every get a miss" instead).
  */
 #define _GNU_SOURCE
@@ -34,14 +42,25 @@
 #include "../../include/cachemap.h"
 #include "../../include/cachemap_b200.h"
 
+/* the library's external definition of the header's inline cmb200_owner */
+extern int cmb200_owner(uint64_t key, int g);
+
 /* The host tier is optional in the engine this layer links against: libcachemap's engine defines
  * these, an engine without a tier (such as the CPU stand-in the host-layer tests link) does not, and
- * then they are null and CMB200_HOST_TIER_MB is refused. */
+ * then they are null and CMB200_HOST_TIER_MB is refused.  The same holds for the calls of a sharded
+ * store: without the snapshot set calls a map does not persist, without the page moves and device
+ * memory the _dev batch calls serve G = 1 only. */
 #pragma weak cmb200_host_tier_enable
 #pragma weak cmb200_demote_batch
 #pragma weak cmb200_host_tier_stats
 #pragma weak cmb200_promote_batch
 #pragma weak cmb200_host_tier_hot
+#pragma weak cmb200_save_set
+#pragma weak cmb200_load_set
+#pragma weak cmb200_move_pages
+#pragma weak cmb200_copy_peer
+#pragma weak cmb200_dev_alloc
+#pragma weak cmb200_dev_free
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -50,6 +69,7 @@
 #define FLUSH_MAX 4096          /* pages the flusher hands over per GPU batch */
 #define PNUM_SHIFT 44           /* cachemap.c:155 */
 #define PROMOTE_EVERY_MS 100    /* CMB200_TIER_PROMOTE: at most one promotion round this often */
+#define MAX_DEVICES 64          /* engines one map may own (CMB200_DEVICES) */
 
 enum req_kind { REQ_GET, REQ_UNSET };
 enum wb_state { WB_FREE = 0, WB_FILLING, WB_READY, WB_FLUSHING };
@@ -71,16 +91,11 @@ struct wb_slot {
 	int state;
 };
 
-struct filemap {
-	uint64_t n;
-	int compress;
-	int bsize;
-	int pshift;
-	char destdir[2048];
-	uint64_t capacity;      /* eviction threshold (set by cachemap_create), 0 = none */
-	/* engine, built on first use (fork safety, SURVEY.md §3.1) */
-	pthread_mutex_t init_mu;
-	int init_state;         /* 0 = not yet, 1 = ready, -1 = failed */
+/* One engine of the map and everything that feeds it: the keys with cmb200_owner(key, G) == index. */
+struct fm_dev {
+	struct filemap *m;
+	int index;              /* position in CMB200_DEVICES */
+	int device;             /* CUDA ordinal (-1 = the current device: CMB200_DEVICES unset, CMB200_DEVICE unset) */
 	cmb200_engine *eng;
 	int host_tier;          /* the engine has a host tier (CMB200_HOST_TIER_MB): a full arena demotes instead of evicting */
 	/* promotion of hot tier records back to the arena (CMB200_TIER_PROMOTE), run by the flusher */
@@ -112,9 +127,36 @@ struct filemap {
 	pthread_t wb_thread;
 	int wb_started, wb_stop;
 	int wb_flusher_asleep;  /* the flusher waits on wb_work (under wb_mu) */
-	/* persistence: <destdir>/cachemap_b200.snap (cmb200_save / cmb200_load) */
+	pthread_mutex_t land_mu;        /* held while a put batch lands in this engine (filemap_land_begin) */
+	/* staging of this engine's share of batch calls that span engines (stage_mu): page-locked host
+	 * pages, and device buffers on the first engine's GPU and on this engine's, grown as needed */
+	pthread_mutex_t stage_mu;
+	uint8_t *h_put;
+	void *d_first, *d_own;
+	size_t d_first_bytes, d_own_bytes;
+};
+
+struct filemap {
+	uint64_t n;
+	int compress;
+	int bsize;
+	int pshift;
+	char destdir[2048];
+	uint64_t capacity;      /* eviction threshold (set by cachemap_create), 0 = none */
+	/* engines, built on first use (fork safety, SURVEY.md §3.1) */
+	pthread_mutex_t init_mu;
+	int init_state;         /* 0 = not yet, 1 = ready, -1 = failed */
+	int g;                  /* engines (G) */
+	struct fm_dev *dev[MAX_DEVICES];
+	cmb200_engine *engs[MAX_DEVICES];
+	/* eviction by count is one decision over all engines, taken under evict_mu: a batch reserves its
+	 * pages (filemap_evict) until they have landed in their engine (filemap_land_end), so that two
+	 * flushers never evict for the same excess nor both fill the same room */
+	pthread_mutex_t evict_mu;
+	uint64_t reserved;      /* (atomic) */
+	/* persistence: <destdir>/cachemap_b200.snap (cmb200_save_set / cmb200_load_set) */
 	int persist;
-	long checkpoint_sec;    /* > 0: the flusher saves a snapshot this often when puts have arrived */
+	long checkpoint_sec;    /* > 0: the first engine's flusher saves a snapshot this often when puts have arrived */
 	uint64_t puts_seen, puts_saved;
 	pthread_mutex_t snap_mu;
 };
@@ -134,7 +176,153 @@ env_long(const char *name, long dflt)
 	return (v && *v) ? strtol(v, NULL, 0) : dflt;
 }
 
+/* The engine that owns `a`. */
+static struct fm_dev *
+filemap_owner(struct filemap *m, const cmb200_addr *a)
+{
+	uint64_t key;
+	FNV_hash(a, (int)sizeof(*a), &key);                     /* filemap.c:18-24 */
+	return m->dev[cmb200_owner(key, m->g)];
+}
+
+/* CMB200_DEVICES: "all", or a comma-separated list of CUDA ordinals (one may repeat: two engines on
+ * one GPU).  Unset: one engine on CMB200_DEVICE.  Returns how many, 0 for a list that names none. */
+static int
+filemap_device_list(int *out)
+{
+	const char *v = getenv("CMB200_DEVICES");
+	if (!v || !*v) {
+		out[0] = (int)env_long("CMB200_DEVICE", -1);
+		return 1;
+	}
+	if (strcmp(v, "all") == 0) {
+		int n = cmb200_device_count();
+		if (n > MAX_DEVICES)
+			n = MAX_DEVICES;
+		for (int i = 0; i < n; i++)
+			out[i] = i;
+		return n > 0 ? n : 0;
+	}
+	int n = 0;
+	const char *p = v;
+	for (;;) {
+		char *end;
+		const long d = strtol(p, &end, 10);
+		if (end == p || d < 0 || d > 1023 || n == MAX_DEVICES)
+			return 0;
+		out[n++] = (int)d;
+		while (*end == ' ')
+			end++;
+		if (*end == '\0')
+			return n;
+		if (*end != ',')
+			return 0;
+		p = end + 1;
+	}
+}
+
 static void *filemap_flusher(void *arg);
+
+static void
+fm_dev_free(struct fm_dev *d)
+{
+	if (!d)
+		return;
+	if (d->wb_pages)
+		cmb200_host_free(d->wb_pages);
+	free(d->wb_slot);
+	if (d->h_stage)
+		cmb200_host_free(d->h_stage);
+	if (d->eng)
+		cmb200_engine_destroy(d->eng);
+	free(d->promo_hot);
+	free(d->promo_guard);
+	pthread_mutex_destroy(&d->promo_mu);
+	pthread_mutex_destroy(&d->land_mu);
+	pthread_mutex_destroy(&d->stage_mu);
+	pthread_mutex_destroy(&d->q_mu);
+	sem_destroy(&d->q_door);
+	pthread_mutex_destroy(&d->wb_mu);
+	pthread_cond_destroy(&d->wb_space);
+	pthread_cond_destroy(&d->wb_work);
+	pthread_cond_destroy(&d->wb_idle);
+	free(d);
+}
+
+/* Engine `index` of the map on CUDA device `device`, with its buffers; NULL if it cannot start.
+ * The knobs apply per engine; the table and the default arena are sized for its share of the
+ * capacity, ceil(n / G). */
+static struct fm_dev *
+fm_dev_start(struct filemap *m, int index, int device, int g)
+{
+	struct fm_dev *d = calloc(1, sizeof(*d));
+	if (!d)
+		return NULL;
+	d->m = m;
+	d->index = index;
+	d->device = device;
+	pthread_mutex_init(&d->q_mu, NULL);
+	sem_init(&d->q_door, 0, GET_CALLERS);
+	pthread_mutex_init(&d->wb_mu, NULL);
+	pthread_cond_init(&d->wb_space, NULL);
+	pthread_cond_init(&d->wb_work, NULL);
+	pthread_cond_init(&d->wb_idle, NULL);
+	pthread_mutex_init(&d->promo_mu, NULL);
+	pthread_mutex_init(&d->land_mu, NULL);
+	pthread_mutex_init(&d->stage_mu, NULL);
+
+	cmb200_config cfg;
+	memset(&cfg, 0, sizeof(cfg));
+	cfg.device = device;
+	cfg.pshift = m->pshift;
+	cfg.accel = m->compress;
+	cfg.capacity = (m->n + (uint64_t)g - 1) / (uint64_t)g;
+	cfg.arena_bytes = (uint64_t)env_long("CMB200_ARENA_MB", 0) << 20;
+	cfg.table_slots = (uint64_t)env_long("CMB200_TABLE_SLOTS", 0);
+	cfg.max_batch = (uint32_t)env_long("CMB200_MAX_BATCH", 0);
+	cfg.flags = env_long("CMB200_FINGERPRINT", 0) ? CMB200_FINGERPRINT : 0;
+	d->eng = cmb200_engine_create(&cfg);
+	const long tier_mb = env_long("CMB200_HOST_TIER_MB", 0);
+	if (d->eng && tier_mb > 0) {
+		if (!cmb200_host_tier_enable)
+			fprintf(stderr, "cachemap_b200: no host tier of %ld MiB: the engine has none\n", tier_mb);
+		else if (cmb200_host_tier_enable(d->eng, (uint64_t)tier_mb << 20) == 0)
+			d->host_tier = 1;
+		else
+			fprintf(stderr, "cachemap_b200: no host tier of %ld MiB: %s\n", tier_mb, cmb200_last_error());
+	}
+	const long promote = env_long("CMB200_TIER_PROMOTE", 0);
+	if (d->host_tier && promote > 0) {
+		if (!cmb200_promote_batch || !cmb200_host_tier_hot)
+			fprintf(stderr, "cachemap_b200: CMB200_TIER_PROMOTE ignored: the engine cannot promote\n");
+		else {
+			d->promo_hot = malloc((size_t)promote * sizeof(cmb200_addr));
+			d->promo_guard = malloc(4 * (size_t)promote * sizeof(cmb200_addr));
+			if (d->promo_hot && d->promo_guard)
+				d->tier_promote = (uint64_t)promote;
+		}
+	}
+	if (d->eng) {
+		d->h_stage = cmb200_host_alloc((size_t)LEADERS * COMBINE_MAX * m->bsize);
+		/* ring of 256 MiB by default, at least 64 pages.  The size sets the batch the flusher can form
+		 * (half the ring), and a batch below ~2 000 chunks leaves the encode kernel a partial wave
+		 * whose duration is one chunk's latency (~2 ms for a text-like page) whatever its size */
+		long slots = env_long("CMB200_WB_SLOTS", (256L << 20) / m->bsize);
+		if (slots > 0 && slots < 64)
+			slots = 64;
+		if (slots > 0) {
+			d->wb_pages = cmb200_host_alloc((size_t)slots * m->bsize);
+			d->wb_slot = calloc((size_t)slots, sizeof(struct wb_slot));
+			d->wb_n = (d->wb_pages && d->wb_slot) ? (uint64_t)slots : 0;
+		}
+	}
+	if (!d->eng || !d->h_stage) {
+		fprintf(stderr, "cachemap_b200: cannot start the GPU engine on device %d: %s\n", device, cmb200_last_error());
+		fm_dev_free(d);
+		return NULL;
+	}
+	return d;
+}
 
 static int
 filemap_engine_ready(struct filemap *m)
@@ -143,53 +331,19 @@ filemap_engine_ready(struct filemap *m)
 		return 1;
 	pthread_mutex_lock(&m->init_mu);
 	if (m->init_state == 0) {
-		cmb200_config cfg;
-		memset(&cfg, 0, sizeof(cfg));
-		cfg.device = (int)env_long("CMB200_DEVICE", -1);
-		cfg.pshift = m->pshift;
-		cfg.accel = m->compress;
-		cfg.capacity = m->n;
-		cfg.arena_bytes = (uint64_t)env_long("CMB200_ARENA_MB", 0) << 20;
-		cfg.table_slots = (uint64_t)env_long("CMB200_TABLE_SLOTS", 0);
-		cfg.max_batch = (uint32_t)env_long("CMB200_MAX_BATCH", 0);
-		cfg.flags = env_long("CMB200_FINGERPRINT", 0) ? CMB200_FINGERPRINT : 0;
-		m->eng = cmb200_engine_create(&cfg);
-		const long tier_mb = env_long("CMB200_HOST_TIER_MB", 0);
-		if (m->eng && tier_mb > 0) {
-			if (!cmb200_host_tier_enable)
-				fprintf(stderr, "cachemap_b200: no host tier of %ld MiB: the engine has none\n", tier_mb);
-			else if (cmb200_host_tier_enable(m->eng, (uint64_t)tier_mb << 20) == 0)
-				m->host_tier = 1;
-			else
-				fprintf(stderr, "cachemap_b200: no host tier of %ld MiB: %s\n", tier_mb, cmb200_last_error());
-		}
-		const long promote = env_long("CMB200_TIER_PROMOTE", 0);
-		if (m->host_tier && promote > 0) {
-			if (!cmb200_promote_batch || !cmb200_host_tier_hot)
-				fprintf(stderr, "cachemap_b200: CMB200_TIER_PROMOTE ignored: the engine cannot promote\n");
-			else {
-				m->promo_hot = malloc((size_t)promote * sizeof(cmb200_addr));
-				m->promo_guard = malloc(4 * (size_t)promote * sizeof(cmb200_addr));
-				if (m->promo_hot && m->promo_guard)
-					m->tier_promote = (uint64_t)promote;
+		int devs[MAX_DEVICES];
+		const int g = filemap_device_list(devs);
+		int started = 0;
+		if (g == 0)
+			fprintf(stderr, "cachemap_b200: CMB200_DEVICES=%s names no device\n", getenv("CMB200_DEVICES"));
+		/* all engines or none */
+		while (started < g && (m->dev[started] = fm_dev_start(m, started, devs[started], g)) != NULL)
+			started++;
+		if (g == 0 || started < g) {
+			for (int i = 0; i < started; i++) {
+				fm_dev_free(m->dev[i]);
+				m->dev[i] = NULL;
 			}
-		}
-		if (m->eng) {
-			m->h_stage = cmb200_host_alloc((size_t)LEADERS * COMBINE_MAX * m->bsize);
-			/* ring of 256 MiB by default, at least 64 pages.  The size sets the batch the flusher can form
-			 * (half the ring), and a batch below ~2 000 chunks leaves the encode kernel a partial wave
-			 * whose duration is one chunk's latency (~2 ms for a text-like page) whatever its size */
-			long slots = env_long("CMB200_WB_SLOTS", (256L << 20) / m->bsize);
-			if (slots > 0 && slots < 64)
-				slots = 64;
-			if (slots > 0) {
-				m->wb_pages = cmb200_host_alloc((size_t)slots * m->bsize);
-				m->wb_slot = calloc((size_t)slots, sizeof(struct wb_slot));
-				m->wb_n = (m->wb_pages && m->wb_slot) ? (uint64_t)slots : 0;
-			}
-		}
-		if (!m->eng || !m->h_stage) {
-			fprintf(stderr, "cachemap_b200: cannot start the GPU engine: %s\n", cmb200_last_error());
 			if (!env_long("CMB200_SOFT_FAIL", 0)) {
 				fprintf(stderr, "cachemap_b200: no CPU fallback exists; aborting "
 				    "(CMB200_SOFT_FAIL=1 turns this into dropped puts / misses)\n");
@@ -197,21 +351,30 @@ filemap_engine_ready(struct filemap *m)
 			}
 			__atomic_store_n(&m->init_state, -1, __ATOMIC_RELEASE);
 		} else {
+			m->g = g;
+			for (int i = 0; i < g; i++)
+				m->engs[i] = m->dev[i]->eng;
 			/* what the cache directory holds from an earlier run comes back first: the reference's
-			 * store is persistent (LMDB files under destdir, filemap.c:57,71-72) */
+			 * store is persistent (LMDB files under destdir, filemap.c:57,71-72).  A file saved with
+			 * any number of engines loads into this one's. */
 			m->persist = (int)env_long("CMB200_PERSIST", 1);
 			m->checkpoint_sec = env_long("CMB200_CHECKPOINT_SEC", 0);
 			char snap[2200];
 			if (m->persist && filemap_snapshot_path(m, snap, sizeof(snap)) && access(snap, R_OK) == 0) {
 				uint64_t got = 0;
-				if (cmb200_load(m->eng, snap, &got) != 0)
+				if (!cmb200_load_set)
+					fprintf(stderr, "cachemap_b200: %s ignored: the engine cannot load snapshots\n", snap);
+				else if (cmb200_load_set(m->engs, g, snap, &got) != 0)
 					fprintf(stderr, "cachemap_b200: %s ignored: %s\n", snap, cmb200_last_error());
 			}
-			/* the flusher starts here, i.e. in the process that actually caches (after any fork) */
-			if (m->wb_n && pthread_create(&m->wb_thread, NULL, filemap_flusher, m) == 0)
-				m->wb_started = 1;
-			else
-				m->wb_n = 0;
+			/* the flushers start here, i.e. in the process that actually caches (after any fork) */
+			for (int i = 0; i < g; i++) {
+				struct fm_dev *d = m->dev[i];
+				if (d->wb_n && pthread_create(&d->wb_thread, NULL, filemap_flusher, d) == 0)
+					d->wb_started = 1;
+				else
+					d->wb_n = 0;
+			}
 			__atomic_store_n(&m->init_state, 1, __ATOMIC_RELEASE);
 		}
 	}
@@ -237,14 +400,8 @@ filemap_create(char *destdir, uint64_t n, int compress_accel, int pshift)
 	m->pshift = pshift;
 	strcpy(m->destdir, destdir);
 	pthread_mutex_init(&m->init_mu, NULL);
-	pthread_mutex_init(&m->q_mu, NULL);
-	sem_init(&m->q_door, 0, GET_CALLERS);
-	pthread_mutex_init(&m->wb_mu, NULL);
-	pthread_cond_init(&m->wb_space, NULL);
-	pthread_cond_init(&m->wb_work, NULL);
-	pthread_cond_init(&m->wb_idle, NULL);
+	pthread_mutex_init(&m->evict_mu, NULL);
 	pthread_mutex_init(&m->snap_mu, NULL);
-	pthread_mutex_init(&m->promo_mu, NULL);
 	return m;
 }
 
@@ -257,9 +414,13 @@ filemap_save(struct filemap *m)
 	if (__atomic_load_n(&m->init_state, __ATOMIC_ACQUIRE) != 1 || !m->persist ||
 	    !filemap_snapshot_path(m, snap, sizeof(snap)))
 		return -1;
+	if (!cmb200_save_set) {
+		fprintf(stderr, "cachemap_b200: snapshot not written: the engine cannot save snapshots\n");
+		return -1;
+	}
 	pthread_mutex_lock(&m->snap_mu);
 	uint64_t seen = __atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED);
-	int rc = cmb200_save(m->eng, snap, NULL);
+	int rc = cmb200_save_set(m->engs, m->g, snap, NULL);
 	if (rc == 0)
 		m->puts_saved = seen;
 	else
@@ -268,19 +429,37 @@ filemap_save(struct filemap *m)
 	return rc;
 }
 
+/* Waits until every page accepted by this engine's ring so far is in its store. */
+static void
+fm_dev_drain(struct fm_dev *d)
+{
+	if (!d->wb_n)
+		return;
+	pthread_mutex_lock(&d->wb_mu);
+	/* everything accepted before this call, not "until the ring is empty": with other threads
+	 * still putting the ring may never be empty (the flusher broadcasts after every batch) */
+	const uint64_t target = d->wb_head;
+	while (d->wb_tail < target)
+		pthread_cond_wait(&d->wb_idle, &d->wb_mu);
+	pthread_mutex_unlock(&d->wb_mu);
+}
+
 /* Waits until every page accepted so far is in the GPU store. */
 static void
 filemap_drain(struct filemap *m)
 {
-	if (!m->wb_n)
-		return;
-	pthread_mutex_lock(&m->wb_mu);
-	/* everything accepted before this call, not "until the ring is empty": with other threads
-	 * still putting the ring may never be empty (the flusher broadcasts after every batch) */
-	const uint64_t target = m->wb_head;
-	while (m->wb_tail < target)
-		pthread_cond_wait(&m->wb_idle, &m->wb_mu);
-	pthread_mutex_unlock(&m->wb_mu);
+	for (int i = 0; i < m->g; i++)
+		fm_dev_drain(m->dev[i]);
+}
+
+/* Live entries over all engines. */
+static uint64_t
+filemap_count(struct filemap *m)
+{
+	uint64_t n = 0;
+	for (int i = 0; i < m->g; i++)
+		n += cmb200_entries(m->dev[i]->eng);
+	return n;
 }
 
 void
@@ -288,42 +467,125 @@ filemap_free(struct filemap *m)
 {
 	if (!m)
 		return;
-	if (m->wb_started) {
-		pthread_mutex_lock(&m->wb_mu);
-		m->wb_stop = 1;
-		pthread_cond_broadcast(&m->wb_work);
-		pthread_mutex_unlock(&m->wb_mu);
-		pthread_join(m->wb_thread, NULL);      /* drains the ring first */
+	for (int i = 0; i < m->g; i++) {
+		struct fm_dev *d = m->dev[i];
+		if (!d->wb_started)
+			continue;
+		pthread_mutex_lock(&d->wb_mu);
+		d->wb_stop = 1;
+		pthread_cond_broadcast(&d->wb_work);
+		pthread_mutex_unlock(&d->wb_mu);
+		pthread_join(d->wb_thread, NULL);      /* drains the ring first */
 	}
 	filemap_save(m);                                /* the cache directory outlives the process */
-	if (m->wb_pages)
-		cmb200_host_free(m->wb_pages);
-	free(m->wb_slot);
-	if (m->h_stage)
-		cmb200_host_free(m->h_stage);
-	if (m->eng)
-		cmb200_engine_destroy(m->eng);
-	free(m->promo_hot);
-	free(m->promo_guard);
-	pthread_mutex_destroy(&m->promo_mu);
+	for (int i = 0; i < m->g; i++) {
+		/* staging first, while every engine that allocated it is alive */
+		struct fm_dev *d = m->dev[i];
+		if (d->h_put)
+			cmb200_host_free(d->h_put);
+		if (d->d_first)
+			cmb200_dev_free(m->dev[0]->eng, d->d_first);
+		if (d->d_own)
+			cmb200_dev_free(d->eng, d->d_own);
+	}
+	for (int i = 0; i < m->g; i++)
+		fm_dev_free(m->dev[i]);
 	pthread_mutex_destroy(&m->snap_mu);
+	pthread_mutex_destroy(&m->evict_mu);
 	pthread_mutex_destroy(&m->init_mu);
-	pthread_mutex_destroy(&m->q_mu);
-	sem_destroy(&m->q_door);
-	pthread_mutex_destroy(&m->wb_mu);
-	pthread_cond_destroy(&m->wb_space);
-	pthread_cond_destroy(&m->wb_work);
-	pthread_cond_destroy(&m->wb_idle);
 	free(m);
 }
 
-/* Retires up to `want` records, each the oldest of three random live ones (cachemap.c:17-45).
- * Statistically the reference's policy; bitwise parity is undefined there (wall-clock
- * timestamps, rand()).  Returns how many entries actually went away. */
-static uint64_t
-filemap_evict_n(struct filemap *m, uint64_t want)
+/* Counting sort of n items by engine: order[] lists the items of engine 0, then of engine 1, ...,
+ * each in array order; engine k's are order[start[k] .. start[k+1]).  own[i] = engine of item i. */
+static void
+group_by_owner(int g, size_t n, const int *own, size_t *order, size_t *start)
 {
-	uint64_t before = cmb200_entries(m->eng), gone = 0;
+	for (int k = 0; k <= g; k++)
+		start[k] = 0;
+	for (size_t i = 0; i < n; i++)
+		start[own[i] + 1]++;
+	for (int k = 0; k < g; k++)
+		start[k + 1] += start[k];
+	size_t fill[MAX_DEVICES];
+	for (int k = 0; k < g; k++)
+		fill[k] = start[k];
+	for (size_t i = 0; i < n; i++)
+		order[fill[own[i]]++] = i;
+}
+
+static uint64_t
+rand64(void)
+{
+	uint64_t r = 0;
+	for (int b = 0; b < 64; b += 30)        /* filemap.c:271-274 */
+		r = r * ((uint64_t)RAND_MAX + 1) + (uint64_t)rand();
+	return r;
+}
+
+/* cmb200_sample of n draws: on engine `only`, or (only = NULL) each draw on engine cmb200_owner(r, G).
+ * own_out[i] = the engine that answered draw i.  0 = sampled, -1 = an engine failed. */
+static int
+filemap_sample(struct filemap *m, struct fm_dev *only, size_t n, const uint64_t *draws, cmb200_addr *cand,
+    uint64_t *ts, int32_t *ok, int *own_out)
+{
+	if (only) {
+		for (size_t i = 0; i < n; i++)
+			own_out[i] = only->index;
+		return cmb200_sample(only->eng, n, draws, cand, ts, ok);
+	}
+	size_t *order = malloc(n * sizeof(size_t));
+	uint64_t *r = malloc(n * sizeof(uint64_t)), *t = malloc(n * sizeof(uint64_t));
+	cmb200_addr *a = malloc(n * sizeof(cmb200_addr));
+	int32_t *o = malloc(n * sizeof(int32_t));
+	size_t start[MAX_DEVICES + 1];
+	int rc = (order && r && t && a && o) ? 0 : -1;
+	if (rc == 0) {
+		for (size_t i = 0; i < n; i++)
+			own_out[i] = cmb200_owner(draws[i], m->g);
+		group_by_owner(m->g, n, own_out, order, start);
+		for (size_t j = 0; j < n; j++)
+			r[j] = draws[order[j]];
+		for (int k = 0; k < m->g && rc == 0; k++)
+			if (start[k + 1] > start[k])
+				rc = cmb200_sample(m->dev[k]->eng, start[k + 1] - start[k], r + start[k], a + start[k], t + start[k],
+				    o + start[k]);
+		for (size_t j = 0; rc == 0 && j < n; j++) {
+			cand[order[j]] = a[j];
+			ts[order[j]] = t[j];
+			ok[order[j]] = o[j];
+		}
+	}
+	free(order); free(r); free(t); free(a); free(o);
+	return rc;
+}
+
+/* Unsets n victims, each on its engine own[i]. */
+static void
+filemap_unset_victims(struct filemap *m, size_t n, const cmb200_addr *victim, const int *own)
+{
+	cmb200_addr *v = malloc(n * sizeof(cmb200_addr));
+	if (!v)
+		return;
+	for (int k = 0; k < m->g; k++) {
+		size_t c = 0;
+		for (size_t i = 0; i < n; i++)
+			if (own[i] == k)
+				v[c++] = victim[i];
+		if (c)
+			cmb200_unset_batch(m->dev[k]->eng, c, v);
+	}
+	free(v);
+}
+
+/* Retires up to `want` records, each the oldest of three random live ones (cachemap.c:17-45): on
+ * engine `only` (arena pressure), or over the whole map (only = NULL, eviction by count; each draw on
+ * the engine its r names).  Statistically the reference's policy; bitwise parity is undefined there
+ * (wall-clock timestamps, rand()).  Returns how many entries actually went away. */
+static uint64_t
+filemap_evict_n(struct filemap *m, struct fm_dev *only, uint64_t want)
+{
+	uint64_t before = only ? cmb200_entries(only->eng) : filemap_count(m), gone = 0;
 	while (gone < want && before > 0) {
 		uint64_t need = want - gone;
 		if (need > before)
@@ -333,17 +595,15 @@ filemap_evict_n(struct filemap *m, uint64_t want)
 		uint64_t *draws = malloc(3 * need * sizeof(uint64_t));
 		uint64_t *ts = malloc(3 * need * sizeof(uint64_t));
 		int32_t *ok = malloc(3 * need * sizeof(int32_t));
+		int *own = malloc(3 * need * sizeof(int));
 		cmb200_addr *cand = malloc(3 * need * sizeof(cmb200_addr));
 		cmb200_addr *victim = malloc(need * sizeof(cmb200_addr));
+		int *vown = malloc(need * sizeof(int));
 		uint64_t nv = 0;
-		if (draws && ts && ok && cand && victim) {
-			for (uint64_t i = 0; i < 3 * need; i++) {
-				uint64_t r = 0;
-				for (int b = 0; b < 64; b += 30)        /* filemap.c:271-274 */
-					r = r * ((uint64_t)RAND_MAX + 1) + (uint64_t)rand();
-				draws[i] = r;
-			}
-			if (cmb200_sample(m->eng, (size_t)(3 * need), draws, cand, ts, ok) == 0) {
+		if (draws && ts && ok && own && cand && victim && vown) {
+			for (uint64_t i = 0; i < 3 * need; i++)
+				draws[i] = rand64();
+			if (filemap_sample(m, only, (size_t)(3 * need), draws, cand, ts, ok, own) == 0) {
 				for (uint64_t i = 0; i < need; i++) {
 					uint64_t a = ts[3 * i], b = ts[3 * i + 1], c = ts[3 * i + 2];
 					int pick;
@@ -351,18 +611,20 @@ filemap_evict_n(struct filemap *m, uint64_t want)
 						pick = (a > c) ? 2 : 0;         /* cachemap.c:29-41 */
 					else
 						pick = (b > c) ? 2 : 1;
-					if (ok[3 * i + pick] > 0)
-						victim[nv++] = cand[3 * i + pick];
+					if (ok[3 * i + pick] > 0) {
+						victim[nv] = cand[3 * i + pick];
+						vown[nv++] = own[3 * i + pick];
+					}
 				}
 				if (nv)
-					cmb200_unset_batch(m->eng, (size_t)nv, victim);
+					filemap_unset_victims(m, (size_t)nv, victim, vown);
 			} else {
 				fprintf(stderr, "cachemap_b200: eviction could not sample the store: %s\n", cmb200_last_error());
 			}
 		}
-		free(draws); free(ts); free(ok); free(cand); free(victim);
+		free(draws); free(ts); free(ok); free(own); free(cand); free(victim); free(vown);
 		/* two draws may have picked the same victim: count what really left the table */
-		uint64_t after = cmb200_entries(m->eng);
+		uint64_t after = only ? cmb200_entries(only->eng) : filemap_count(m);
 		if (nv == 0 || after >= before)
 			break;          /* no progress */
 		gone += before - after;
@@ -393,37 +655,37 @@ addr_cmp(const void *x, const void *y)
  * promoted record keeps its old put timestamp, so without this the next demotion, which takes the
  * oldest of what it samples, would send it straight back to the tier. */
 static cmb200_addr *
-filemap_promo_guard(struct filemap *m, size_t *n)
+filemap_promo_guard(struct fm_dev *d, size_t *n)
 {
 	*n = 0;
-	if (!m->tier_promote)
+	if (!d->tier_promote)
 		return NULL;
-	pthread_mutex_lock(&m->promo_mu);
-	const uint64_t cap = 4 * m->tier_promote;
-	const size_t k = (size_t)(m->promo_guard_n < cap ? m->promo_guard_n : cap);
+	pthread_mutex_lock(&d->promo_mu);
+	const uint64_t cap = 4 * d->tier_promote;
+	const size_t k = (size_t)(d->promo_guard_n < cap ? d->promo_guard_n : cap);
 	cmb200_addr *g = k ? malloc(k * sizeof(cmb200_addr)) : NULL;
 	if (g) {
-		memcpy(g, m->promo_guard, k * sizeof(cmb200_addr));
+		memcpy(g, d->promo_guard, k * sizeof(cmb200_addr));
 		*n = k;
 	}
-	pthread_mutex_unlock(&m->promo_mu);
+	pthread_mutex_unlock(&d->promo_mu);
 	if (g)
 		qsort(g, *n, sizeof(cmb200_addr), addr_cmp);
 	return g;
 }
 
-/* Moves up to `want` arena records to the host tier.  The candidates are drawn as filemap_evict_n
- * draws them (3 per record wanted) and go oldest first; keys already in the tier, and keys promotion
- * has just brought back (filemap_promo_guard), are passed over, so a round goes on down its candidates
- * until `want` have moved.  When few records are left in the arena a round may find none: it draws
- * again, up to 16 times in a row.  Returns how many moved. */
+/* Moves up to `want` arena records of engine d to its host tier.  The candidates are drawn as
+ * filemap_evict_n draws them (3 per record wanted, on this engine only) and go oldest first; keys
+ * already in the tier, and keys promotion has just brought back (filemap_promo_guard), are passed
+ * over, so a round goes on down its candidates until `want` have moved.  When few records are left in
+ * the arena a round may find none: it draws again, up to 16 times in a row.  Returns how many moved. */
 static uint64_t
-filemap_demote_n(struct filemap *m, uint64_t want)
+filemap_demote_n(struct fm_dev *d, uint64_t want)
 {
 	uint64_t moved = 0;
 	int idle = 0;
 	size_t ng = 0;
-	cmb200_addr *guard = filemap_promo_guard(m, &ng);
+	cmb200_addr *guard = filemap_promo_guard(d, &ng);
 	while (moved < want && idle < 16) {
 		uint64_t need = want - moved;
 		if (need > 4096)
@@ -437,13 +699,9 @@ filemap_demote_n(struct filemap *m, uint64_t want)
 		cmb200_addr *victim = malloc(nd * sizeof(cmb200_addr));
 		uint64_t round = 0;
 		if (draws && ts && ok && cand && old && victim) {
-			for (uint64_t i = 0; i < nd; i++) {
-				uint64_t r = 0;
-				for (int b = 0; b < 64; b += 30)        /* filemap.c:271-274 */
-					r = r * ((uint64_t)RAND_MAX + 1) + (uint64_t)rand();
-				draws[i] = r;
-			}
-			if (cmb200_sample(m->eng, (size_t)nd, draws, cand, ts, ok) == 0) {
+			for (uint64_t i = 0; i < nd; i++)
+				draws[i] = rand64();
+			if (cmb200_sample(d->eng, (size_t)nd, draws, cand, ts, ok) == 0) {
 				uint64_t nv = 0;
 				for (uint64_t i = 0; i < nd; i++)
 					if (ok[i] > 0 && !(guard && bsearch(&cand[i], guard, ng, sizeof(cmb200_addr), addr_cmp)))
@@ -453,7 +711,7 @@ filemap_demote_n(struct filemap *m, uint64_t want)
 					uint64_t take = want - moved < nv - k ? want - moved : nv - k, got = 0;
 					for (uint64_t j = 0; j < take; j++)
 						victim[j] = old[k + j].a;
-					if (cmb200_demote_batch(m->eng, (size_t)take, victim, &got) != 0) {
+					if (cmb200_demote_batch(d->eng, (size_t)take, victim, &got) != 0) {
 						fprintf(stderr, "cachemap_b200: demotion to the host tier failed: %s\n", cmb200_last_error());
 						break;
 					}
@@ -472,23 +730,56 @@ filemap_demote_n(struct filemap *m, uint64_t want)
 	return moved;
 }
 
-/* Before `incoming` puts: while entries + incoming > capacity, evict (cachemap.c:17-45); loops
- * until the count fits or nothing more can be retired. */
+/* Before a batch of `incoming` puts: while entries + incoming > capacity over all engines, evict
+ * (cachemap.c:17-45); loops until the count fits or nothing more can be retired.  Then the batch's
+ * pages are reserved until they have landed in their engine (filemap_land_end): a batch that has made
+ * its room but is not in its engine yet counts for every other batch's decision, so two flushers
+ * neither evict for the same excess nor fill the same room.  The estimate (entries + reserved) can
+ * count a batch twice, after it has landed and before its reservation is released; so when the
+ * estimate says evict, the decision takes every engine's land_mu and counts again: no batch is
+ * between the two then, and no more is evicted than the count needs. */
 static void
 filemap_evict(struct filemap *m, uint64_t incoming)
 {
 	if (!m->capacity)
 		return;
-	for (;;) {
-		uint64_t entries = cmb200_entries(m->eng);
-		if (entries + incoming <= m->capacity || entries == 0)
-			return;
-		uint64_t need = entries + incoming - m->capacity;
-		if (incoming == 1)
-			need = 1;       /* the reference evicts exactly one per put */
-		if (filemap_evict_n(m, need) == 0 || incoming == 1)
-			return;
+	pthread_mutex_lock(&m->evict_mu);
+	uint64_t entries = filemap_count(m) + __atomic_load_n(&m->reserved, __ATOMIC_RELAXED);
+	if (entries + incoming > m->capacity && entries > 0) {
+		for (int k = 0; k < m->g; k++)
+			pthread_mutex_lock(&m->dev[k]->land_mu);
+		for (;;) {
+			entries = filemap_count(m) + __atomic_load_n(&m->reserved, __ATOMIC_RELAXED);
+			if (entries + incoming <= m->capacity || entries == 0)
+				break;
+			uint64_t need = entries + incoming - m->capacity;
+			if (incoming == 1)
+				need = 1;       /* the reference evicts exactly one per put */
+			if (filemap_evict_n(m, NULL, need) == 0 || incoming == 1)
+				break;
+		}
+		for (int k = m->g - 1; k >= 0; k--)
+			pthread_mutex_unlock(&m->dev[k]->land_mu);
 	}
+	__atomic_fetch_add(&m->reserved, incoming, __ATOMIC_RELAXED);
+	pthread_mutex_unlock(&m->evict_mu);
+}
+
+/* Puts land in an engine under its land_mu, and their reservation (filemap_evict) is released before
+ * land_mu is: a decision that holds every land_mu sees each batch either reserved or in its engine,
+ * never both. */
+static void
+filemap_land_begin(struct fm_dev *d)
+{
+	pthread_mutex_lock(&d->land_mu);
+}
+
+static void
+filemap_land_end(struct fm_dev *d, uint64_t pages)
+{
+	if (d->m->capacity)
+		__atomic_fetch_sub(&d->m->reserved, pages, __ATOMIC_RELAXED);
+	pthread_mutex_unlock(&d->land_mu);
 }
 
 /* The arena is a bump allocator; deleted and outgrown records stay behind as garbage until
@@ -498,22 +789,23 @@ filemap_evict(struct filemap *m, uint64_t incoming)
  * records are demoted to it and the arena compacted, so the store keeps `capacity` pages as the
  * reference's LMDB files do; otherwise evict by bytes as well and compact what that frees.
  * Only when even that fails does a put get dropped, as a full LMDB map drops it
- * (filemap.c:143-145,154-157).  may_evict = 0 (room for promotion): demotion and compaction only. */
+ * (filemap.c:143-145,154-157).  may_evict = 0 (room for promotion): demotion and compaction only.
+ * All of it happens on engine d, the one whose arena is full. */
 static void
-filemap_arena_room(struct filemap *m, uint64_t incoming, int may_evict)
+filemap_arena_room(struct fm_dev *d, uint64_t incoming, int may_evict)
 {
-	const uint64_t need = incoming * ((uint64_t)m->bsize + 1056);
+	const uint64_t need = incoming * ((uint64_t)d->m->bsize + 1056);
 	int evicted = 0;
 	for (int attempt = 0; attempt < 6; attempt++) {
 		cmb200_stats st;
-		if (cmb200_get_stats(m->eng, &st) != 0)
+		if (cmb200_get_stats(d->eng, &st) != 0)
 			return;
 		if (st.arena_used + need <= st.arena_bytes)
 			return;
 		const uint64_t free_b = st.arena_bytes - st.arena_used;
 		if (st.arena_garbage > 0 && (free_b + st.arena_garbage >= need || evicted)) {
 			uint64_t got = 0;
-			if (cmb200_compact(m->eng, &got) != 0) {
+			if (cmb200_compact(d->eng, &got) != 0) {
 				fprintf(stderr, "cachemap_b200: arena compaction failed: %s\n", cmb200_last_error());
 				return;
 			}
@@ -526,7 +818,7 @@ filemap_arena_room(struct filemap *m, uint64_t incoming, int may_evict)
 		const uint64_t live = st.arena_used > st.arena_garbage ? st.arena_used - st.arena_garbage : 1;
 		const uint64_t shortfall = need - (free_b + st.arena_garbage < need ? free_b + st.arena_garbage : need);
 		struct cmb200_host_tier_stats ht;
-		if (m->host_tier && cmb200_host_tier_stats(m->eng, &ht) == 0 && shortfall <= ht.bytes) {
+		if (d->host_tier && cmb200_host_tier_stats(d->eng, &ht) == 0 && shortfall <= ht.bytes) {
 			if (st.entries <= ht.records)
 				return;         /* every live record is in the tier already: evicting frees no arena bytes */
 			const uint64_t in_arena = st.entries - ht.records;
@@ -534,7 +826,7 @@ filemap_arena_room(struct filemap *m, uint64_t incoming, int may_evict)
 			uint64_t victims = shortfall / avg + shortfall / avg / 8 + 16;
 			if (victims > in_arena)
 				victims = in_arena;
-			if (filemap_demote_n(m, victims) == 0)
+			if (filemap_demote_n(d, victims) == 0)
 				return;
 			evicted = 1;
 			continue;
@@ -545,16 +837,16 @@ filemap_arena_room(struct filemap *m, uint64_t incoming, int may_evict)
 		uint64_t victims = shortfall / avg + shortfall / avg / 8 + 16;
 		if (victims > st.entries)
 			victims = st.entries;
-		if (filemap_evict_n(m, victims) == 0)
+		if (filemap_evict_n(d->m, d, victims) == 0)
 			return;
 		evicted = 1;
 	}
 }
 
 static void
-filemap_check_arena(struct filemap *m, uint64_t incoming)
+filemap_check_arena(struct fm_dev *d, uint64_t incoming)
 {
-	filemap_arena_room(m, incoming, 1);
+	filemap_arena_room(d, incoming, 1);
 }
 
 /* One promotion round (CMB200_TIER_PROMOTE = N): up to N addresses that gets answered from the host
@@ -562,48 +854,49 @@ filemap_check_arena(struct filemap *m, uint64_t incoming)
  * oldest arena records and compacting, never by evicting; when that frees too little, the round
  * promotes what fits.  The addresses join the guard FIFO that demotion passes over. */
 static void
-filemap_promote_round(struct filemap *m)
+filemap_promote_round(struct fm_dev *d)
 {
-	clock_gettime(CLOCK_MONOTONIC, &m->promo_last);
+	clock_gettime(CLOCK_MONOTONIC, &d->promo_last);
 	size_t n = 0;
-	if (cmb200_host_tier_hot(m->eng, (size_t)m->tier_promote, m->promo_hot, &n, NULL) != 0) {
+	if (cmb200_host_tier_hot(d->eng, (size_t)d->tier_promote, d->promo_hot, &n, NULL) != 0) {
 		fprintf(stderr, "cachemap_b200: the host tier's hot log could not be read: %s\n", cmb200_last_error());
 		return;
 	}
 	if (n == 0)
 		return;
-	filemap_arena_room(m, n, 0);
+	filemap_arena_room(d, n, 0);
 	uint64_t got = 0;
-	if (cmb200_promote_batch(m->eng, n, m->promo_hot, &got) != 0) {
+	if (cmb200_promote_batch(d->eng, n, d->promo_hot, &got) != 0) {
 		fprintf(stderr, "cachemap_b200: promotion from the host tier failed: %s\n", cmb200_last_error());
 		return;
 	}
-	pthread_mutex_lock(&m->promo_mu);
-	const uint64_t cap = 4 * m->tier_promote;
+	pthread_mutex_lock(&d->promo_mu);
+	const uint64_t cap = 4 * d->tier_promote;
 	for (size_t i = 0; i < n; i++)
-		m->promo_guard[m->promo_guard_n++ % cap] = m->promo_hot[i];
-	pthread_mutex_unlock(&m->promo_mu);
+		d->promo_guard[d->promo_guard_n++ % cap] = d->promo_hot[i];
+	pthread_mutex_unlock(&d->promo_mu);
 }
 
 /* A promotion round is due: the knob is on and PROMOTE_EVERY_MS have passed since the last one. */
 static int
-filemap_promote_due(struct filemap *m)
+filemap_promote_due(struct fm_dev *d)
 {
-	if (!m->tier_promote)
+	if (!d->tier_promote)
 		return 0;
 	struct timespec now;
 	clock_gettime(CLOCK_MONOTONIC, &now);
-	const int64_t ms = (int64_t)(now.tv_sec - m->promo_last.tv_sec) * 1000 + (now.tv_nsec - m->promo_last.tv_nsec) / 1000000;
+	const int64_t ms = (int64_t)(now.tv_sec - d->promo_last.tv_sec) * 1000 + (now.tv_nsec - d->promo_last.tv_nsec) / 1000000;
 	return ms >= PROMOTE_EVERY_MS;
 }
 
-/* Before a batch of `incoming` puts: evict down to capacity, then make sure the arena has room
- * (what eviction frees is garbage until the arena is compacted). */
+/* Before a batch of `incoming` puts into engine d: evict the map down to capacity (and reserve the
+ * batch, see filemap_evict), then make sure d's arena has room (what eviction frees is garbage until
+ * the arena is compacted).  The put follows between filemap_land_begin and filemap_land_end. */
 static void
-filemap_make_room(struct filemap *m, uint64_t incoming)
+filemap_make_room(struct fm_dev *d, uint64_t incoming)
 {
-	filemap_evict(m, incoming);
-	filemap_check_arena(m, incoming);
+	filemap_evict(d->m, incoming);
+	filemap_check_arena(d, incoming);
 }
 
 static void
@@ -614,123 +907,135 @@ timespec_add_ms(struct timespec *t, long ms)
 	t->tv_nsec %= 1000000000L;
 }
 
-/* The flusher: takes the longest run of finished slots from the tail of the ring and puts it
- * into the GPU store as one batch (two calls when the run wraps around the ring). */
+/* The flusher of one engine: takes the longest run of finished slots from the tail of its ring and
+ * puts it into the engine as one batch (two calls when the run wraps around the ring).  The first
+ * engine's flusher also writes the CMB200_CHECKPOINT_SEC snapshots of the whole map. */
 static void *
 filemap_flusher(void *arg)
 {
-	struct filemap *m = arg;
+	struct fm_dev *d = arg;
+	struct filemap *m = d->m;
 	cmb200_addr *addr = malloc(FLUSH_MAX * sizeof(cmb200_addr));
 	uint64_t *ts = malloc(FLUSH_MAX * sizeof(uint64_t));
 	time_t last_save = time(NULL);
-	pthread_mutex_lock(&m->wb_mu);
+	const int checkpoints = m->checkpoint_sec > 0 && m->persist && d->index == 0;
+	pthread_mutex_lock(&d->wb_mu);
 	for (;;) {
 		uint64_t count = 0;
 		/* at most half the ring per batch: callers keep filling the other half while this one is on the GPU */
-		const uint64_t flush_cap = m->wb_n / 2 < FLUSH_MAX ? (m->wb_n / 2 ? m->wb_n / 2 : 1) : FLUSH_MAX;
-		while (m->wb_tail + count < m->wb_head && count < flush_cap &&
-		    m->wb_slot[(m->wb_tail + count) % m->wb_n].state == WB_READY)
+		uint64_t flush_cap = d->wb_n / 2 < FLUSH_MAX ? (d->wb_n / 2 ? d->wb_n / 2 : 1) : FLUSH_MAX;
+		/* and at most this engine's share of the capacity: the batches of all flushers in flight at once
+		 * then fit the store together */
+		if (m->capacity && flush_cap > m->capacity / (uint64_t)m->g)
+			flush_cap = m->capacity / (uint64_t)m->g ? m->capacity / (uint64_t)m->g : 1;
+		while (d->wb_tail + count < d->wb_head && count < flush_cap &&
+		    d->wb_slot[(d->wb_tail + count) % d->wb_n].state == WB_READY)
 			count++;
 		if (count == 0) {
-			if (m->wb_stop && m->wb_tail == m->wb_head)
+			if (d->wb_stop && d->wb_tail == d->wb_head)
 				break;
-			if (filemap_promote_due(m)) {
-				pthread_mutex_unlock(&m->wb_mu);
-				filemap_promote_round(m);
-				pthread_mutex_lock(&m->wb_mu);
+			if (filemap_promote_due(d)) {
+				pthread_mutex_unlock(&d->wb_mu);
+				filemap_promote_round(d);
+				pthread_mutex_lock(&d->wb_mu);
 				continue;
 			}
-			if (m->checkpoint_sec > 0 && m->persist) {
+			if (checkpoints) {
 				struct timespec now, until;
 				clock_gettime(CLOCK_REALTIME, &now);
-				if (m->puts_seen != m->puts_saved && now.tv_sec - last_save >= m->checkpoint_sec) {
-					pthread_mutex_unlock(&m->wb_mu);
+				if (__atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED) != m->puts_saved &&
+				    now.tv_sec - last_save >= m->checkpoint_sec) {
+					pthread_mutex_unlock(&d->wb_mu);
 					filemap_save(m);
-					pthread_mutex_lock(&m->wb_mu);
+					pthread_mutex_lock(&d->wb_mu);
 					last_save = now.tv_sec;
 					continue;
 				}
 				until = now;
-				if (m->tier_promote)
+				if (d->tier_promote)
 					timespec_add_ms(&until, PROMOTE_EVERY_MS);
 				else
 					until.tv_sec += 1;
-				m->wb_flusher_asleep = 1;
-				pthread_cond_timedwait(&m->wb_work, &m->wb_mu, &until);
-				m->wb_flusher_asleep = 0;
-			} else if (m->tier_promote) {
+				d->wb_flusher_asleep = 1;
+				pthread_cond_timedwait(&d->wb_work, &d->wb_mu, &until);
+				d->wb_flusher_asleep = 0;
+			} else if (d->tier_promote) {
 				/* woken for the next promotion round at the latest */
 				struct timespec until;
 				clock_gettime(CLOCK_REALTIME, &until);
 				timespec_add_ms(&until, PROMOTE_EVERY_MS);
-				m->wb_flusher_asleep = 1;
-				pthread_cond_timedwait(&m->wb_work, &m->wb_mu, &until);
-				m->wb_flusher_asleep = 0;
+				d->wb_flusher_asleep = 1;
+				pthread_cond_timedwait(&d->wb_work, &d->wb_mu, &until);
+				d->wb_flusher_asleep = 0;
 			} else {
-				m->wb_flusher_asleep = 1;
-				pthread_cond_wait(&m->wb_work, &m->wb_mu);
-				m->wb_flusher_asleep = 0;
+				d->wb_flusher_asleep = 1;
+				pthread_cond_wait(&d->wb_work, &d->wb_mu);
+				d->wb_flusher_asleep = 0;
 			}
 			continue;
 		}
 		for (uint64_t i = 0; i < count; i++) {
-			struct wb_slot *s = &m->wb_slot[(m->wb_tail + i) % m->wb_n];
+			struct wb_slot *s = &d->wb_slot[(d->wb_tail + i) % d->wb_n];
 			s->state = WB_FLUSHING;
 			addr[i] = s->addr;
 			ts[i] = s->ts;
 		}
-		const uint64_t first = m->wb_tail % m->wb_n;
-		pthread_mutex_unlock(&m->wb_mu);
+		const uint64_t first = d->wb_tail % d->wb_n;
+		pthread_mutex_unlock(&d->wb_mu);
 
 		if (addr && ts) {
-			filemap_make_room(m, count);
-			uint64_t run1 = count < m->wb_n - first ? count : m->wb_n - first;
-			cmb200_put_batch(m->eng, (size_t)run1, addr, NULL, m->wb_pages + first * (size_t)m->bsize, ts, NULL);
+			filemap_make_room(d, count);
+			filemap_land_begin(d);
+			uint64_t run1 = count < d->wb_n - first ? count : d->wb_n - first;
+			cmb200_put_batch(d->eng, (size_t)run1, addr, NULL, d->wb_pages + first * (size_t)m->bsize, ts, NULL);
 			if (run1 < count)
-				cmb200_put_batch(m->eng, (size_t)(count - run1), addr + run1, NULL, m->wb_pages, ts + run1, NULL);
+				cmb200_put_batch(d->eng, (size_t)(count - run1), addr + run1, NULL, d->wb_pages, ts + run1, NULL);
+			filemap_land_end(d, count);
 		}
 
-		pthread_mutex_lock(&m->wb_mu);
+		pthread_mutex_lock(&d->wb_mu);
 		__atomic_fetch_add(&m->puts_seen, count, __ATOMIC_RELAXED);
 		for (uint64_t i = 0; i < count; i++)
-			m->wb_slot[(m->wb_tail + i) % m->wb_n].state = WB_FREE;
-		m->wb_tail += count;
-		pthread_cond_broadcast(&m->wb_space);
-		pthread_cond_broadcast(&m->wb_idle);            /* waiters compare wb_tail with their own target */
-		if (filemap_promote_due(m)) {
-			pthread_mutex_unlock(&m->wb_mu);
-			filemap_promote_round(m);
-			pthread_mutex_lock(&m->wb_mu);
+			d->wb_slot[(d->wb_tail + i) % d->wb_n].state = WB_FREE;
+		d->wb_tail += count;
+		pthread_cond_broadcast(&d->wb_space);
+		pthread_cond_broadcast(&d->wb_idle);            /* waiters compare wb_tail with their own target */
+		if (filemap_promote_due(d)) {
+			pthread_mutex_unlock(&d->wb_mu);
+			filemap_promote_round(d);
+			pthread_mutex_lock(&d->wb_mu);
 		}
 	}
-	pthread_mutex_unlock(&m->wb_mu);
+	pthread_mutex_unlock(&d->wb_mu);
 	free(addr);
 	free(ts);
 	return NULL;
 }
 
-/* Newest copy of `addr` still in the ring -> malloc()ed page, else NULL. */
+/* Newest copy of `addr` still in its engine's ring -> malloc()ed page (or dst), else NULL. */
 static void *
-filemap_ring_lookup(struct filemap *m, const cmb200_addr *addr, void *dst)
+filemap_ring_lookup(struct fm_dev *d, const cmb200_addr *addr, void *dst)
 {
 	void *page = NULL;
-	if (!m->wb_n)
+	if (!d->wb_n)
 		return NULL;
-	pthread_mutex_lock(&m->wb_mu);
-	for (uint64_t s = m->wb_head; s > m->wb_tail; s--) {
-		struct wb_slot *w = &m->wb_slot[(s - 1) % m->wb_n];
+	const size_t bsize = (size_t)d->m->bsize;
+	pthread_mutex_lock(&d->wb_mu);
+	for (uint64_t s = d->wb_head; s > d->wb_tail; s--) {
+		struct wb_slot *w = &d->wb_slot[(s - 1) % d->wb_n];
 		if (w->state >= WB_READY && w->addr.u == addr->u && w->addr.l == addr->l) {
-			page = dst ? dst : malloc((size_t)m->bsize);
+			page = dst ? dst : malloc(bsize);
 			if (page)
-				memcpy(page, m->wb_pages + ((s - 1) % m->wb_n) * (size_t)m->bsize, (size_t)m->bsize);
+				memcpy(page, d->wb_pages + ((s - 1) % d->wb_n) * bsize, bsize);
 			break;
 		}
 	}
-	pthread_mutex_unlock(&m->wb_mu);
+	pthread_mutex_unlock(&d->wb_mu);
 	return page;
 }
 
-/* Combining queue of the single-page calls (cachemap_get / filemap_unset from FUSE worker threads).
+/* Combining queue of the single-page calls (cachemap_get / filemap_unset from FUSE worker threads),
+ * one per engine.
  *
  * A get's latency is one page's decode on one SM and an H100 decodes 132 pages at a time, so a
  * request is launched at once when it can be: whoever finds a free leader slot and nobody else
@@ -745,30 +1050,30 @@ filemap_ring_lookup(struct filemap *m, const cmb200_addr *addr, void *dst)
 static const int32_t fm_answered = CMB200_MISS;         /* status word of requests that have no page to wait for */
 
 /* Takes up to COMBINE_MAX queued requests into leader slot `ls` and launches them.  Called with q_mu
- * held and m->launching set; returns with q_mu held. */
+ * held and d->launching set; returns with q_mu held. */
 static void
-filemap_lead(struct filemap *m, int ls)
+filemap_lead(struct fm_dev *d, int ls)
 {
 	struct fm_req *batch[COMBINE_MAX];
 	cmb200_addr addr[COMBINE_MAX];
 	int idx[COMBINE_MAX];
 	int nb = 0, k;
 
-	while (m->q_head && nb < COMBINE_MAX) {
-		batch[nb++] = m->q_head;
-		m->q_head = m->q_head->next;
+	while (d->q_head && nb < COMBINE_MAX) {
+		batch[nb++] = d->q_head;
+		d->q_head = d->q_head->next;
 	}
-	if (!m->q_head)
-		m->q_tail = NULL;
-	__atomic_fetch_sub(&m->q_len, nb, __ATOMIC_RELAXED);
-	pthread_mutex_unlock(&m->q_mu);
+	if (!d->q_head)
+		d->q_tail = NULL;
+	__atomic_fetch_sub(&d->q_len, nb, __ATOMIC_RELAXED);
+	pthread_mutex_unlock(&d->q_mu);
 
 	k = 0;
 	for (int i = 0; i < nb; i++)
 		if (batch[i]->kind == REQ_UNSET)
 			addr[k++] = batch[i]->addr;
 	if (k)
-		cmb200_unset_batch(m->eng, (size_t)k, addr);    /* unsets first: they change the table the gets read by key */
+		cmb200_unset_batch(d->eng, (size_t)k, addr);    /* unsets first: they change the table the gets read by key */
 
 	k = 0;
 	for (int i = 0; i < nb; i++) {
@@ -778,28 +1083,28 @@ filemap_lead(struct filemap *m, int ls)
 		idx[k] = i;
 		k++;
 	}
-	uint8_t *stage = m->h_stage + (size_t)ls * COMBINE_MAX * (size_t)m->bsize;
-	const volatile int32_t *answers = m->sync_status[ls];
-	m->ticket[ls].lane = -1;
+	uint8_t *stage = d->h_stage + (size_t)ls * COMBINE_MAX * (size_t)d->m->bsize;
+	const volatile int32_t *answers = d->sync_status[ls];
+	d->ticket[ls].lane = -1;
 	if (k) {
 		/* the fused small-batch get: one kernel on a stream of its own, pages land in the page-locked
-		 * stage buffer directly; page sizes it does not serve (> 64 KiB) take the two-kernel batch path,
+		 * stage buffer directly; page sizes it does not serve (> 128 KiB) take the two-kernel batch path,
 		 * synchronously */
-		int rc = cmb200_get_small_begin(m->eng, (size_t)k, addr, stage, &m->ticket[ls]);
+		int rc = cmb200_get_small_begin(d->eng, (size_t)k, addr, stage, &d->ticket[ls]);
 		if (rc == 0) {
-			answers = m->ticket[ls].status;
+			answers = d->ticket[ls].status;
 		} else {
-			m->ticket[ls].lane = -1;
+			d->ticket[ls].lane = -1;
 			if (rc == -2)
-				rc = cmb200_get_batch(m->eng, (size_t)k, addr, NULL, stage, m->sync_status[ls]);
+				rc = cmb200_get_batch(d->eng, (size_t)k, addr, NULL, stage, d->sync_status[ls]);
 			if (rc != 0)
 				for (int j = 0; j < k; j++)
-					m->sync_status[ls][j] = CMB200_MISS;
+					d->sync_status[ls][j] = CMB200_MISS;
 		}
 	}
 
-	pthread_mutex_lock(&m->q_mu);
-	__atomic_store_n(&m->batch_left[ls], nb, __ATOMIC_RELEASE);
+	pthread_mutex_lock(&d->q_mu);
+	__atomic_store_n(&d->batch_left[ls], nb, __ATOMIC_RELEASE);
 	for (int j = 0; j < k; j++)
 		batch[idx[j]]->pos = j;
 	k = 0;
@@ -812,11 +1117,9 @@ filemap_lead(struct filemap *m, int ls)
 	}
 }
 
-/* Queues `count` requests (an array) and returns when all of them have been answered.  A requester
- * takes q_mu once to queue; after that it only takes it again to launch a batch itself or to sleep
- * when every slot is busy — watching for its launch and for its answer needs no lock. */
+/* Queues `count` requests (an array) on engine d.  filemap_await must follow with the same array. */
 static void
-filemap_submit_many(struct filemap *m, struct fm_req *reqs, int count)
+filemap_enqueue(struct fm_dev *d, struct fm_req *reqs, int count)
 {
 	for (int i = 0; i < count; i++) {
 		reqs[i].status = NULL;
@@ -824,17 +1127,24 @@ filemap_submit_many(struct filemap *m, struct fm_req *reqs, int count)
 		reqs[i].pos = 0;
 		reqs[i].next = i + 1 < count ? &reqs[i + 1] : NULL;
 	}
-	while (sem_wait(&m->q_door) != 0)
+	while (sem_wait(&d->q_door) != 0)
 		;
-	pthread_mutex_lock(&m->q_mu);
-	if (m->q_tail)
-		m->q_tail->next = &reqs[0];
+	pthread_mutex_lock(&d->q_mu);
+	if (d->q_tail)
+		d->q_tail->next = &reqs[0];
 	else
-		m->q_head = &reqs[0];
-	m->q_tail = &reqs[count - 1];
-	__atomic_fetch_add(&m->q_len, count, __ATOMIC_RELAXED);
-	pthread_mutex_unlock(&m->q_mu);
+		d->q_head = &reqs[0];
+	d->q_tail = &reqs[count - 1];
+	__atomic_fetch_add(&d->q_len, count, __ATOMIC_RELAXED);
+	pthread_mutex_unlock(&d->q_mu);
+}
 
+/* Returns when all `count` requests queued by filemap_enqueue have been answered.  A requester
+ * takes q_mu once to queue; after that it only takes it again to launch a batch itself or to sleep
+ * when every slot is busy — watching for its launch and for its answer needs no lock. */
+static void
+filemap_await(struct fm_dev *d, struct fm_req *reqs, int count)
+{
 	for (int i = 0; i < count; i++) {
 		struct fm_req *r = &reqs[i];
 		const volatile int32_t *answer;
@@ -844,9 +1154,9 @@ filemap_submit_many(struct filemap *m, struct fm_req *reqs, int count)
 			 * request with it or leaves it to the next launch), while every slot is busy, and — for a
 			 * short while — when a launch now would carry very few requests into one of the last free
 			 * slots: with many callers the slots are what runs out, and batches of 1 use them up. */
-			const int busy = __atomic_load_n(&m->busy_slots, __ATOMIC_RELAXED);
-			if (__atomic_load_n(&m->launching, __ATOMIC_ACQUIRE) || busy >= LEADERS ||
-			    (busy >= LEADERS / 2 && waited < 256u && 4 * __atomic_load_n(&m->q_len, __ATOMIC_RELAXED) < busy)) {
+			const int busy = __atomic_load_n(&d->busy_slots, __ATOMIC_RELAXED);
+			if (__atomic_load_n(&d->launching, __ATOMIC_ACQUIRE) || busy >= LEADERS ||
+			    (busy >= LEADERS / 2 && waited < 256u && 4 * __atomic_load_n(&d->q_len, __ATOMIC_RELAXED) < busy)) {
 #if defined(__x86_64__)
 				__builtin_ia32_pause();
 #endif
@@ -854,20 +1164,20 @@ filemap_submit_many(struct filemap *m, struct fm_req *reqs, int count)
 					sched_yield();
 				continue;
 			}
-			pthread_mutex_lock(&m->q_mu);
-			if (!r->status && !__atomic_load_n(&m->launching, __ATOMIC_RELAXED)) {
+			pthread_mutex_lock(&d->q_mu);
+			if (!r->status && !__atomic_load_n(&d->launching, __ATOMIC_RELAXED)) {
 				int ls = -1;
 				for (int k = 0; k < LEADERS; k++)
-					if (!m->leader_busy[k]) { ls = k; break; }
+					if (!d->leader_busy[k]) { ls = k; break; }
 				if (ls >= 0) {
-					__atomic_store_n(&m->launching, 1, __ATOMIC_RELAXED);  /* (read by watchers that hold no lock) */
-					m->leader_busy[ls] = 1;
-					__atomic_fetch_add(&m->busy_slots, 1, __ATOMIC_RELAXED);
-					filemap_lead(m, ls);                    /* (drops and retakes q_mu around the launch) */
-					__atomic_store_n(&m->launching, 0, __ATOMIC_RELEASE);
+					__atomic_store_n(&d->launching, 1, __ATOMIC_RELAXED);  /* (read by watchers that hold no lock) */
+					d->leader_busy[ls] = 1;
+					__atomic_fetch_add(&d->busy_slots, 1, __ATOMIC_RELAXED);
+					filemap_lead(d, ls);                    /* (drops and retakes q_mu around the launch) */
+					__atomic_store_n(&d->launching, 0, __ATOMIC_RELEASE);
 				}
 			}
-			pthread_mutex_unlock(&m->q_mu);
+			pthread_mutex_unlock(&d->q_mu);
 		}
 		const int ls = r->slot;
 
@@ -883,33 +1193,34 @@ filemap_submit_many(struct filemap *m, struct fm_req *reqs, int count)
 		/* (the acquire load above orders the page bytes after the status word) */
 		if (r->kind == REQ_GET) {
 			if (st == CMB200_HIT) {
-				r->out = r->dst ? r->dst : malloc((size_t)m->bsize);    /* filemap.c:242 */
+				const size_t bsize = (size_t)d->m->bsize;
+				r->out = r->dst ? r->dst : malloc(bsize);    /* filemap.c:242 */
 				if (r->out)
-					memcpy(r->out, m->h_stage + ((size_t)ls * COMBINE_MAX + (size_t)r->pos) * (size_t)m->bsize,
-					    (size_t)m->bsize);
+					memcpy(r->out, d->h_stage + ((size_t)ls * COMBINE_MAX + (size_t)r->pos) * bsize, bsize);
 			} else if (st == CMB200_BAD_ENTRY) {
 				r->bad_entry = 1;
 			}
 		}
 
-		if (__atomic_sub_fetch(&m->batch_left[ls], 1, __ATOMIC_ACQ_REL) == 0) {
+		if (__atomic_sub_fetch(&d->batch_left[ls], 1, __ATOMIC_ACQ_REL) == 0) {
 			/* last one out: every status word of the launch has been seen answered, so ending it does
 			 * not wait; then the slot and its stage buffer are free again */
-			if (m->ticket[ls].lane >= 0)
-				cmb200_get_small_end(m->eng, &m->ticket[ls], NULL);
-			pthread_mutex_lock(&m->q_mu);
-			m->leader_busy[ls] = 0;
-			__atomic_fetch_sub(&m->busy_slots, 1, __ATOMIC_RELEASE);
-			pthread_mutex_unlock(&m->q_mu);
+			if (d->ticket[ls].lane >= 0)
+				cmb200_get_small_end(d->eng, &d->ticket[ls], NULL);
+			pthread_mutex_lock(&d->q_mu);
+			d->leader_busy[ls] = 0;
+			__atomic_fetch_sub(&d->busy_slots, 1, __ATOMIC_RELEASE);
+			pthread_mutex_unlock(&d->q_mu);
 		}
 	}
-	sem_post(&m->q_door);
+	sem_post(&d->q_door);
 }
 
 static void
-filemap_submit(struct filemap *m, struct fm_req *req)
+filemap_submit(struct fm_dev *d, struct fm_req *req)
 {
-	filemap_submit_many(m, req, 1);
+	filemap_enqueue(d, req, 1);
+	filemap_await(d, req, 1);
 }
 
 void
@@ -918,27 +1229,30 @@ filemap_set(struct filemap *m, uint128_t *key, void *value, uint64_t attr)
 	if (!filemap_engine_ready(m))
 		return;
 	cmb200_addr a = { key->u, key->l };
-	if (!m->wb_n) {                         /* write-behind disabled: one synchronous GPU put */
-		filemap_make_room(m, 1);
-		cmb200_put_batch(m->eng, 1, &a, NULL, value, &attr, NULL);
+	struct fm_dev *d = filemap_owner(m, &a);
+	if (!d->wb_n) {                         /* write-behind disabled: one synchronous GPU put */
+		filemap_make_room(d, 1);
+		filemap_land_begin(d);
+		cmb200_put_batch(d->eng, 1, &a, NULL, value, &attr, NULL);
+		filemap_land_end(d, 1);
 		__atomic_fetch_add(&m->puts_seen, 1, __ATOMIC_RELAXED);
 		return;
 	}
-	pthread_mutex_lock(&m->wb_mu);
-	while (m->wb_head - m->wb_tail == m->wb_n)
-		pthread_cond_wait(&m->wb_space, &m->wb_mu);     /* back-pressure: the ring is full */
-	const uint64_t s = m->wb_head++;
-	struct wb_slot *w = &m->wb_slot[s % m->wb_n];
+	pthread_mutex_lock(&d->wb_mu);
+	while (d->wb_head - d->wb_tail == d->wb_n)
+		pthread_cond_wait(&d->wb_space, &d->wb_mu);     /* back-pressure: the ring is full */
+	const uint64_t s = d->wb_head++;
+	struct wb_slot *w = &d->wb_slot[s % d->wb_n];
 	w->addr = a;
 	w->ts = attr;
 	w->state = WB_FILLING;
-	pthread_mutex_unlock(&m->wb_mu);
-	memcpy(m->wb_pages + (s % m->wb_n) * (size_t)m->bsize, value, (size_t)m->bsize);
-	pthread_mutex_lock(&m->wb_mu);
+	pthread_mutex_unlock(&d->wb_mu);
+	memcpy(d->wb_pages + (s % d->wb_n) * (size_t)m->bsize, value, (size_t)m->bsize);
+	pthread_mutex_lock(&d->wb_mu);
 	w->state = WB_READY;
-	if (m->wb_flusher_asleep)               /* a busy flusher finds the page by itself when it comes back: no wake-up call per put */
-		pthread_cond_signal(&m->wb_work);
-	pthread_mutex_unlock(&m->wb_mu);
+	if (d->wb_flusher_asleep)               /* a busy flusher finds the page by itself when it comes back: no wake-up call per put */
+		pthread_cond_signal(&d->wb_work);
+	pthread_mutex_unlock(&d->wb_mu);
 }
 
 void
@@ -946,13 +1260,14 @@ filemap_unset(struct filemap *m, uint128_t *key)
 {
 	if (!filemap_engine_ready(m))
 		return;
-	filemap_drain(m);
 	struct fm_req r;
 	memset(&r, 0, sizeof(r));
 	r.kind = REQ_UNSET;
 	r.addr.u = key->u;
 	r.addr.l = key->l;
-	filemap_submit(m, &r);
+	struct fm_dev *d = filemap_owner(m, &r.addr);
+	fm_dev_drain(d);
+	filemap_submit(d, &r);
 }
 
 void *
@@ -965,12 +1280,13 @@ filemap_get(struct filemap *m, uint128_t *key)
 	r.kind = REQ_GET;
 	r.addr.u = key->u;
 	r.addr.l = key->l;
+	struct fm_dev *d = filemap_owner(m, &r.addr);
 	/* a page accepted by filemap_set but not flushed yet is served from the ring; a slot leaves
 	 * the ring only after the GPU put of its batch has completed, so nothing falls between */
-	void *page = filemap_ring_lookup(m, &r.addr, NULL);
+	void *page = filemap_ring_lookup(d, &r.addr, NULL);
 	if (page)
 		return page;
-	filemap_submit(m, &r);
+	filemap_submit(d, &r);
 	if (r.bad_entry)
 		printf("bad entry\n");          /* filemap.c:237 */
 	return r.out;
@@ -982,13 +1298,11 @@ filemap_get_rand(struct filemap *m, uint128_t *key, uint64_t *ts)
 	if (!filemap_engine_ready(m))
 		return 0;
 	filemap_drain(m);
-	/* filemap.c:271-274: a 64-bit draw built from rand() */
-	uint64_t r = 0;
-	for (int i = 0; i < 64; i += 30)
-		r = r * ((uint64_t)RAND_MAX + 1) + (uint64_t)rand();
+	/* filemap.c:271-274: a 64-bit draw built from rand(), sampled on the engine it names */
+	uint64_t r = rand64();
 	cmb200_addr a;
 	int32_t ok = 0;
-	if (cmb200_sample(m->eng, 1, &r, &a, ts, &ok) != 0 || !ok)
+	if (cmb200_sample(m->dev[cmb200_owner(r, m->g)]->eng, 1, &r, &a, ts, &ok) != 0 || !ok)
 		return 0;
 	key->u = a.u;
 	key->l = a.l;
@@ -1001,7 +1315,7 @@ filemap_entries(struct filemap *m)
 	if (!filemap_engine_ready(m))
 		return 0;
 	filemap_drain(m);
-	return cmb200_entries(m->eng);
+	return filemap_count(m);
 }
 
 /* ------------------------------------------------------------------------------------------ */
@@ -1089,7 +1403,7 @@ cachemap_free(struct cachemap *cm)
 {
 	if (!cm)
 		return;
-	filemap_free(cm->pages);                /* drains the write-behind ring (cachemap.c:218-232) */
+	filemap_free(cm->pages);                /* drains the write-behind rings (cachemap.c:218-232) */
 	free(cm);
 }
 
@@ -1108,6 +1422,7 @@ struct batch_keys {
 	cmb200_addr *addr;
 	uint8_t *valid;
 	uint64_t *ts;
+	int *own;               /* engine of each page (an invalid address goes to engine 0, which skips it) */
 };
 
 static int
@@ -1117,8 +1432,9 @@ batch_keys_build(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 	bk->addr = malloc((size_t)n * sizeof(cmb200_addr));
 	bk->valid = malloc((size_t)n);
 	bk->ts = want_ts ? malloc((size_t)n * 8) : NULL;
-	if (!bk->addr || !bk->valid || (want_ts && !bk->ts)) {
-		free(bk->addr); free(bk->valid); free(bk->ts);
+	bk->own = malloc((size_t)n * sizeof(int));
+	if (!bk->addr || !bk->valid || (want_ts && !bk->ts) || !bk->own) {
+		free(bk->addr); free(bk->valid); free(bk->ts); free(bk->own);
 		return -1;
 	}
 	uint64_t ts = want_ts ? now_ns() : 0;
@@ -1126,6 +1442,7 @@ batch_keys_build(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 		bk->valid[i] = compose_addr(cm, offset[i], nhid[i], genid ? genid[i] : 0, &bk->addr[i]) == 0;
 		if (!bk->valid[i])
 			memset(&bk->addr[i], 0, sizeof(cmb200_addr));
+		bk->own[i] = bk->valid[i] ? filemap_owner(cm->pages, &bk->addr[i])->index : 0;
 		if (want_ts)
 			bk->ts[i] = ts;
 	}
@@ -1135,45 +1452,292 @@ batch_keys_build(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 static void
 batch_keys_free(struct batch_keys *bk)
 {
-	free(bk->addr); free(bk->valid); free(bk->ts);
+	free(bk->addr); free(bk->valid); free(bk->ts); free(bk->own);
+}
+
+/* One engine's share of a batch call when the batch spans engines: its pages' keys gathered, and
+ * where its pages are in the caller's buffer.  The shares of a call run concurrently, one thread per
+ * engine, each through its engine's reusable staging buffers (struct fm_dev, stage_mu). */
+struct batch_part {
+	struct filemap *m;
+	struct fm_dev *d;
+	size_t c;
+	cmb200_addr *addr;
+	uint8_t *valid;
+	uint64_t *ts;
+	uint32_t *idx;          /* page of the caller's buffer of each */
+	int32_t *status;        /* get: status of each */
+	const uint8_t *src;     /* put: the caller's pages (host, or the first engine's GPU) */
+	uint8_t *dst;           /* get: the caller's output (host, or the first engine's GPU) */
+	int on_dev;
+	pthread_t th;
+};
+
+/* The pages order[0..c) of the batch keys, from position `at` on. */
+static int
+batch_part_gather(struct batch_part *p, const struct batch_keys *bk, const size_t *order, size_t c, uint64_t at)
+{
+	p->c = c;
+	p->addr = malloc(c * sizeof(cmb200_addr));
+	p->valid = malloc(c);
+	p->ts = bk->ts ? malloc(c * 8) : NULL;
+	p->idx = malloc(c * sizeof(uint32_t));
+	p->status = bk->ts ? NULL : malloc(c * sizeof(int32_t));
+	if (!p->addr || !p->valid || (bk->ts && !p->ts) || !p->idx || (!bk->ts && !p->status))
+		return -1;
+	for (size_t j = 0; j < c; j++) {
+		p->addr[j] = bk->addr[at + order[j]];
+		p->valid[j] = bk->valid[at + order[j]];
+		if (p->ts)
+			p->ts[j] = bk->ts[at + order[j]];
+		p->idx[j] = (uint32_t)order[j];
+	}
+	return 0;
+}
+
+static void
+batch_part_free(struct batch_part *p)
+{
+	free(p->addr); free(p->valid); free(p->ts); free(p->idx); free(p->status);
+}
+
+/* Host pages a share moves per engine call: 64 MiB of page-locked staging per engine, at most 4096
+ * pages (the engine's sub-batch). */
+static size_t
+stage_pages(const struct filemap *m)
+{
+	size_t k = ((size_t)64 << 20) / (size_t)m->bsize;
+	return k < 1 ? 1 : k > 4096 ? 4096 : k;
+}
+
+/* d->h_put, allocated on first use (stage_mu held). */
+static uint8_t *
+stage_host(struct fm_dev *d)
+{
+	if (!d->h_put)
+		d->h_put = cmb200_host_alloc(stage_pages(d->m) * (size_t)d->m->bsize);
+	return d->h_put;
+}
+
+/* A device buffer of at least `bytes` on engine e's GPU in *p, kept in the share's engine and grown as
+ * needed (stage_mu held): no allocation, and no device-wide cudaFree, per call. */
+static void *
+stage_dev(cmb200_engine *e, void **p, size_t *cap, size_t bytes)
+{
+	if (*p && *cap >= bytes)
+		return *p;
+	if (*p)
+		cmb200_dev_free(e, *p);
+	*p = cmb200_dev_alloc(e, bytes);
+	*cap = *p ? bytes : 0;
+	return *p;
+}
+
+/* Device-resident pages (the _dev calls) are on the first engine's GPU.  Engine k's pages cross to
+ * its GPU in one contiguous buffer and one peer copy: gathered on the first GPU by k_move_pages
+ * (cmb200_move_pages), then copied; nothing is copied when engine k is on the first GPU. */
+static int
+same_gpu(struct filemap *m, int k)
+{
+	return m->dev[k]->device == m->dev[0]->device;
+}
+
+static int
+dev_calls_present(void)
+{
+	return cmb200_move_pages && cmb200_copy_peer && cmb200_dev_alloc && cmb200_dev_free;
+}
+
+/* One engine's share of a put: host pages are copied into the engine's page-locked staging buffer in
+ * runs of stage_pages(); device pages are gathered on the first GPU by k_move_pages and cross in one
+ * peer copy. */
+static void *
+put_part(void *arg)
+{
+	struct batch_part *p = arg;
+	struct filemap *m = p->m;
+	struct fm_dev *d = p->d, *d0 = m->dev[0];
+	const size_t bsize = (size_t)m->bsize, bytes = p->c * bsize;
+	int rc = -1;
+	pthread_mutex_lock(&d->stage_mu);
+	filemap_check_arena(d, p->c);
+	filemap_land_begin(d);
+	if (!p->on_dev) {
+		uint8_t *h = stage_host(d);
+		const size_t sp = stage_pages(m);
+		rc = h ? 0 : -1;
+		for (size_t at = 0; rc == 0 && at < p->c; at += sp) {
+			const size_t k = p->c - at < sp ? p->c - at : sp;
+			for (size_t j = 0; j < k; j++)
+				memcpy(h + j * bsize, p->src + (size_t)p->idx[at + j] * bsize, bsize);
+			/* back when the pages have crossed to the GPU: the buffer is free for the next run */
+			uint64_t ticket;
+			rc = cmb200_put_batch_async(d->eng, k, p->addr + at, p->valid + at, h, p->ts + at, NULL, &ticket);
+		}
+	} else if (dev_calls_present()) {
+		void *g0 = stage_dev(d0->eng, &d->d_first, &d->d_first_bytes, bytes), *buf = g0;
+		rc = g0 ? cmb200_move_pages(d0->eng, p->c, g0, NULL, p->src, p->idx) : -1;
+		if (rc == 0 && !same_gpu(m, d->index)) {
+			buf = stage_dev(d->eng, &d->d_own, &d->d_own_bytes, bytes);
+			rc = buf ? cmb200_copy_peer(d->eng, buf, d0->eng, g0, bytes) : -1;
+		}
+		if (rc == 0)
+			rc = cmb200_put_batch_dev(d->eng, p->c, p->addr, p->valid, buf, p->ts, NULL);
+	}
+	filemap_land_end(d, p->c);
+	pthread_mutex_unlock(&d->stage_mu);
+	if (rc != 0)
+		fprintf(stderr, "cachemap_b200: %zu pages not stored on engine %d: %s\n", p->c, d->index, cmb200_last_error());
+	return NULL;
+}
+
+/* One engine's share of a get: decoded into the engine's staging buffer (host: in runs of
+ * stage_pages(); device: on the engine's GPU, then one peer copy to the first GPU), and the hits
+ * scattered to their places in the caller's output; a miss leaves its page untouched.  p->status
+ * stays CMB200_MISS where the engine could not answer. */
+static void *
+get_part(void *arg)
+{
+	struct batch_part *p = arg;
+	struct filemap *m = p->m;
+	struct fm_dev *d = p->d, *d0 = m->dev[0];
+	const size_t bsize = (size_t)m->bsize, bytes = p->c * bsize;
+	for (size_t j = 0; j < p->c; j++)
+		p->status[j] = CMB200_MISS;
+	pthread_mutex_lock(&d->stage_mu);
+	if (!p->on_dev) {
+		uint8_t *h = stage_host(d);
+		const size_t sp = stage_pages(m);
+		for (size_t at = 0; h && at < p->c; at += sp) {
+			const size_t k = p->c - at < sp ? p->c - at : sp;
+			if (cmb200_get_batch(d->eng, k, p->addr + at, p->valid + at, h, p->status + at) != 0) {
+				for (size_t j = 0; j < k; j++)
+					p->status[at + j] = CMB200_MISS;
+				continue;
+			}
+			for (size_t j = 0; j < k; j++)
+				if (p->status[at + j] == CMB200_HIT)
+					memcpy(p->dst + (size_t)p->idx[at + j] * bsize, h + j * bsize, bsize);
+		}
+	} else if (dev_calls_present()) {
+		uint32_t *src = malloc(p->c * sizeof(uint32_t)), *dst = malloc(p->c * sizeof(uint32_t));
+		void *gk = stage_dev(d->eng, &d->d_own, &d->d_own_bytes, bytes), *buf = gk;
+		int rc = gk && src && dst ? cmb200_get_batch_dev(d->eng, p->c, p->addr, p->valid, gk, p->status) : -1;
+		if (rc == 0 && !same_gpu(m, d->index)) {
+			buf = stage_dev(d0->eng, &d->d_first, &d->d_first_bytes, bytes);
+			rc = buf ? cmb200_copy_peer(d0->eng, buf, d->eng, gk, bytes) : -1;
+		}
+		if (rc == 0) {
+			size_t h = 0;
+			for (size_t j = 0; j < p->c; j++)
+				if (p->status[j] == CMB200_HIT) {
+					src[h] = (uint32_t)j;
+					dst[h++] = p->idx[j];
+				}
+			rc = cmb200_move_pages(d0->eng, h, p->dst, dst, buf, src);
+		}
+		if (rc != 0)
+			for (size_t j = 0; j < p->c; j++)
+				p->status[j] = CMB200_MISS;
+		free(src); free(dst);
+	}
+	pthread_mutex_unlock(&d->stage_mu);
+	return NULL;
+}
+
+/* Runs the np shares of a call at once: one thread each, the first on the caller's thread. */
+static void
+run_parts(struct batch_part *parts, int np, void *(*fn)(void *))
+{
+	int started[MAX_DEVICES];
+	for (int i = 1; i < np; i++)
+		started[i] = pthread_create(&parts[i].th, NULL, fn, &parts[i]) == 0;
+	if (np > 0)
+		fn(&parts[0]);
+	for (int i = 1; i < np; i++) {
+		if (started[i])
+			pthread_join(parts[i].th, NULL);
+		else
+			fn(&parts[i]);
+	}
 }
 
 static void
 put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const uint64_t *nhid,
     const uint32_t *genid, const void *pages, int on_dev)
 {
+	struct filemap *fm = cm->pages;
 	struct batch_keys bk;
-	if (n == 0 || !filemap_engine_ready(cm->pages))
+	if (n == 0 || !filemap_engine_ready(fm))
 		return;
 	if (batch_keys_build(cm, n, offset, nhid, genid, 1, &bk) != 0)
 		return;
-	filemap_drain(cm->pages);               /* earlier single puts land first */
-	__atomic_fetch_add(&cm->pages->puts_seen, n, __ATOMIC_RELAXED);
-	/* One GPU batch when the store has room for all of it; at capacity the batch goes in slices
-	 * with eviction before each, so that entries never run past capacity by more than a slice
+	size_t *order = malloc((size_t)n * sizeof(size_t));
+	if (!order) {
+		batch_keys_free(&bk);
+		return;
+	}
+	filemap_drain(fm);                      /* earlier single puts land first */
+	__atomic_fetch_add(&fm->puts_seen, n, __ATOMIC_RELAXED);
+	/* One GPU batch per engine when the store has room for all of it; at capacity the batch goes in
+	 * slices with eviction before each, so that entries never run past capacity by more than a slice
 	 * (the reference evicts before every single put, cachemap.c:186-197). */
 	uint64_t slice = n;
-	if (cm->capacity && cmb200_entries(cm->pages->eng) + n > cm->capacity) {
+	if (cm->capacity && filemap_count(fm) + n > cm->capacity) {
 		slice = cm->capacity / 4;
 		if (slice > 4096)
 			slice = 4096;
 		if (slice < 1)
 			slice = 1;
 	}
-	const size_t bsize = (size_t)cm->pages->bsize;
+	const size_t bsize = (size_t)fm->bsize;
 	for (uint64_t at = 0; at < n; at += slice) {
 		const uint64_t m = n - at < slice ? n - at : slice;
 		const uint8_t *pg = (const uint8_t *)pages + at * bsize;
-		filemap_make_room(cm->pages, m);
-		if (on_dev)
-			cmb200_put_batch_dev(cm->pages->eng, (size_t)m, bk.addr + at, bk.valid + at, pg, bk.ts + at, NULL);
-		else {
-			/* write-behind like cachemap_put: back when the pages have crossed to the GPU and the
-			 * caller may reuse them; whatever is called next is ordered after the encode */
-			uint64_t ticket;
-			cmb200_put_batch_async(cm->pages->eng, (size_t)m, bk.addr + at, bk.valid + at, pg, bk.ts + at, NULL, &ticket);
+		size_t start[MAX_DEVICES + 1];
+		group_by_owner(fm->g, (size_t)m, bk.own + at, order, start);
+		filemap_evict(fm, m);
+		struct batch_part parts[MAX_DEVICES];
+		int np = 0;
+		for (int k = 0; k < fm->g; k++) {
+			const size_t c = start[k + 1] - start[k];
+			if (c == 0)
+				continue;
+			struct fm_dev *d = fm->dev[k];
+			if (c == m && (k == 0 || !on_dev)) {
+				/* the whole slice is this engine's (always so with one engine): the caller's arrays as they are */
+				filemap_check_arena(d, c);
+				filemap_land_begin(d);
+				if (on_dev)
+					cmb200_put_batch_dev(d->eng, (size_t)m, bk.addr + at, bk.valid + at, pg, bk.ts + at, NULL);
+				else {
+					/* write-behind like cachemap_put: back when the pages have crossed to the GPU and the
+					 * caller may reuse them; whatever is called next is ordered after the encode */
+					uint64_t ticket;
+					cmb200_put_batch_async(d->eng, (size_t)m, bk.addr + at, bk.valid + at, pg, bk.ts + at, NULL, &ticket);
+				}
+				filemap_land_end(d, m);
+				continue;
+			}
+			struct batch_part *p = &parts[np];
+			memset(p, 0, sizeof(*p));
+			p->m = fm;
+			p->d = d;
+			p->src = pg;
+			p->on_dev = on_dev;
+			if (batch_part_gather(p, &bk, order + start[k], c, at) != 0) {
+				batch_part_free(p);
+				filemap_land_begin(d);
+				filemap_land_end(d, c);         /* (what a share cannot store gives its reservation back) */
+				continue;
+			}
+			np++;
 		}
+		run_parts(parts, np, put_part);
+		for (int i = 0; i < np; i++)
+			batch_part_free(&parts[i]);
 	}
+	free(order);
 	batch_keys_free(&bk);
 }
 
@@ -1181,33 +1745,72 @@ static void
 get_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const uint64_t *nhid,
     const uint32_t *genid, void *pages_out, uint8_t *hit_out, int on_dev)
 {
+	struct filemap *fm = cm->pages;
 	struct batch_keys bk;
 	memset(hit_out, 0, (size_t)n);
-	if (n == 0 || !filemap_engine_ready(cm->pages))
+	if (n == 0 || !filemap_engine_ready(fm))
 		return;
 	if (batch_keys_build(cm, n, offset, nhid, genid, 0, &bk) != 0)
 		return;
-	filemap_drain(cm->pages);
+	filemap_drain(fm);
 	int32_t *status = malloc((size_t)n * 4);
-	int rc = -1;
-	if (status)
-		rc = on_dev ? cmb200_get_batch_dev(cm->pages->eng, (size_t)n, bk.addr, bk.valid, pages_out, status)
-			    : cmb200_get_batch(cm->pages->eng, (size_t)n, bk.addr, bk.valid, pages_out, status);
+	size_t *order = malloc((size_t)n * sizeof(size_t));
+	size_t start[MAX_DEVICES + 1];
+	struct batch_part parts[MAX_DEVICES];
+	int np = 0;
+	if (status && order) {
+		for (uint64_t i = 0; i < n; i++)
+			status[i] = CMB200_MISS;        /* what an engine that fails leaves: no hit, no bad entry */
+		group_by_owner(fm->g, (size_t)n, bk.own, order, start);
+		for (int k = 0; k < fm->g; k++) {
+			const size_t c = start[k + 1] - start[k];
+			if (c == 0)
+				continue;
+			struct fm_dev *d = fm->dev[k];
+			if (c == n && (k == 0 || !on_dev)) {
+				/* all of it on this engine (always so with one engine): straight into the caller's arrays */
+				int rc = on_dev ? cmb200_get_batch_dev(d->eng, (size_t)n, bk.addr, bk.valid, pages_out, status)
+				                : cmb200_get_batch(d->eng, (size_t)n, bk.addr, bk.valid, pages_out, status);
+				if (rc != 0)
+					for (uint64_t i = 0; i < n; i++)
+						status[i] = CMB200_MISS;
+				continue;
+			}
+			struct batch_part *p = &parts[np];
+			memset(p, 0, sizeof(*p));
+			p->m = fm;
+			p->d = d;
+			p->dst = pages_out;
+			p->on_dev = on_dev;
+			if (batch_part_gather(p, &bk, order + start[k], c, 0) != 0) {
+				batch_part_free(p);
+				continue;
+			}
+			np++;
+		}
+		run_parts(parts, np, get_part);
+		for (int i = 0; i < np; i++) {
+			for (size_t j = 0; j < parts[i].c; j++)
+				status[parts[i].idx[j]] = parts[i].status[j];
+			batch_part_free(&parts[i]);
+		}
+	}
 	uint64_t rq = 0, ht = 0;
 	for (uint64_t i = 0; i < n; i++) {
 		if (!bk.valid[i])
 			continue;                       /* cachemap.c:173-174: not a request */
 		rq++;
-		if (rc == 0 && status[i] == CMB200_HIT) {
+		if (status && status[i] == CMB200_HIT) {
 			hit_out[i] = 1;
 			ht++;
-		} else if (rc == 0 && status[i] == CMB200_BAD_ENTRY) {
+		} else if (status && status[i] == CMB200_BAD_ENTRY) {
 			printf("bad entry\n");
 		}
 	}
 	__atomic_fetch_add(&cm->requests, rq, __ATOMIC_RELAXED);
 	__atomic_fetch_add(&cm->hits, ht, __ATOMIC_RELAXED);
 	free(status);
+	free(order);
 	batch_keys_free(&bk);
 }
 
@@ -1245,50 +1848,69 @@ int
 cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size,
     void *out_buf)
 {
-	const int pshift = cm->pages->pshift;
+	struct filemap *fm = cm->pages;
+	const int pshift = fm->pshift;
 	const uint64_t page_size = 1ULL << pshift;
 	if ((off & (page_size - 1)) || ((off + (uint64_t)size) & (page_size - 1)))     /* edgefs.c:192-203 */
 		return 0;
 	const uint64_t n = (uint64_t)size >> pshift;
 	if (n == 0)
 		return 1;
-	if (!filemap_engine_ready(cm->pages))
+	if (!filemap_engine_ready(fm))
 		return 0;
 	struct fm_req *reqs = calloc((size_t)n, sizeof(*reqs));
-	int *which = malloc((size_t)n * sizeof(int));
-	uint8_t *state = calloc((size_t)n, 1);          /* 0 miss, 1 hit, 2 invalid address */
-	if (!reqs || !which || !state) {
-		free(reqs); free(which); free(state);
+	cmb200_addr *addr = malloc((size_t)n * sizeof(cmb200_addr));
+	int *own = malloc((size_t)n * sizeof(int));
+	size_t *order = malloc((size_t)n * sizeof(size_t));
+	uint8_t *state = calloc((size_t)n, 1);          /* 0 miss, 1 hit, 2 invalid address, 3 asked of an engine */
+	if (!reqs || !addr || !own || !order || !state) {
+		free(reqs); free(addr); free(own); free(order); free(state);
 		return 0;
 	}
-	/* pages still in the write-behind ring are served from it, the rest go to the GPU as one
-	 * chain of requests (one batch unless the chain is longer than COMBINE_MAX) */
-	int k = 0;
+	/* pages still in a write-behind ring are served from it; the rest go to their engines, one chain
+	 * of requests per engine (one batch unless the chain is longer than COMBINE_MAX) */
+	size_t ask = 0;
 	for (uint64_t i = 0; i < n; i++) {
-		cmb200_addr a;
 		uint8_t *dst = (uint8_t *)out_buf + (i << pshift);
-		if (compose_addr(cm, off + (i << pshift), nhid_small, genid, &a) != 0) {
+		if (compose_addr(cm, off + (i << pshift), nhid_small, genid, &addr[ask]) != 0) {
 			state[i] = 2;
 			continue;
 		}
-		if (filemap_ring_lookup(cm->pages, &a, dst)) {
+		struct fm_dev *d = filemap_owner(fm, &addr[ask]);
+		if (filemap_ring_lookup(d, &addr[ask], dst)) {
 			state[i] = 1;
 			continue;
 		}
-		reqs[k].kind = REQ_GET;
-		reqs[k].addr = a;
-		reqs[k].dst = dst;
-		which[k] = (int)i;
-		k++;
+		state[i] = 3;
+		own[ask] = d->index;
+		order[ask] = i;         /* (page of each asked request, until grouped below) */
+		ask++;
 	}
-	if (k)
-		filemap_submit_many(cm->pages, reqs, k);
-	for (int j = 0; j < k; j++) {
-		if (reqs[j].out)
-			state[which[j]] = 1;
+	size_t start[MAX_DEVICES + 1], *page_of = malloc((ask ? ask : 1) * sizeof(size_t));
+	if (!page_of) {
+		free(reqs); free(addr); free(own); free(order); free(state);
+		return 0;
 	}
-	/* counters as the reference's loop leaves them: it stops at the first page that is not a
-	 * hit; an invalid address returns NULL without counting a request (cachemap.c:173-174) */
+	memcpy(page_of, order, ask * sizeof(size_t));
+	group_by_owner(fm->g, ask, own, order, start);
+	for (size_t j = 0; j < ask; j++) {
+		reqs[j].kind = REQ_GET;
+		reqs[j].addr = addr[order[j]];
+		reqs[j].dst = (uint8_t *)out_buf + ((uint64_t)page_of[order[j]] << pshift);
+	}
+	/* every engine's chain is queued before any is waited for, in engine order (so that two callers
+	 * never hold the door of one engine while they wait for the other's) */
+	for (int k = 0; k < fm->g; k++)
+		if (start[k + 1] > start[k])
+			filemap_enqueue(fm->dev[k], reqs + start[k], (int)(start[k + 1] - start[k]));
+	for (int k = 0; k < fm->g; k++)
+		if (start[k + 1] > start[k])
+			filemap_await(fm->dev[k], reqs + start[k], (int)(start[k + 1] - start[k]));
+	for (size_t j = 0; j < ask; j++)
+		state[page_of[order[j]]] = reqs[j].out ? 1 : 0;
+	/* counters as the reference's loop leaves them, in page order whatever engine answered which page:
+	 * it stops at the first page that is not a hit; an invalid address returns NULL without counting a
+	 * request (cachemap.c:173-174) */
 	uint64_t rq = 0, ht = 0, i = 0;
 	for (; i < n; i++) {
 		if (state[i] == 2)
@@ -1298,12 +1920,12 @@ cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 			break;
 		ht++;
 	}
-	for (int j = 0; j < k; j++)
-		if (reqs[j].bad_entry && (uint64_t)which[j] <= i)
+	for (size_t j = 0; j < ask; j++)
+		if (reqs[j].bad_entry && (uint64_t)page_of[order[j]] <= i)
 			printf("bad entry\n");                  /* filemap.c:237 */
 	__atomic_fetch_add(&cm->requests, rq, __ATOMIC_RELAXED);
 	__atomic_fetch_add(&cm->hits, ht, __ATOMIC_RELAXED);
-	free(reqs); free(which); free(state);
+	free(reqs); free(addr); free(own); free(order); free(state); free(page_of);
 	return i == n;
 }
 
@@ -1343,5 +1965,16 @@ cachemap_engine(struct cachemap *cm)
 	if (!filemap_engine_ready(cm->pages))
 		return NULL;
 	filemap_drain(cm->pages);               /* callers of the engine see every accepted put */
-	return cm->pages->eng;
+	return cm->pages->dev[0]->eng;
+}
+
+int
+cachemap_engines(struct cachemap *cm, struct cmb200_engine **out, int max)
+{
+	if (!filemap_engine_ready(cm->pages))
+		return 0;
+	filemap_drain(cm->pages);
+	for (int i = 0; i < cm->pages->g && i < max; i++)
+		out[i] = cm->pages->dev[i]->eng;
+	return cm->pages->g;
 }

@@ -25,6 +25,7 @@
 #include <string.h>
 #include <vector>
 #include "../../include/cachemap_b200.h"
+#include "../../include/uint128.h"
 #include "kernels.h"
 #include "common.cuh"
 #include "streamgen.cuh"
@@ -108,6 +109,8 @@ struct cmb200_engine {
 	uint32_t *d_order = nullptr;         // the encoder's longest-first chunk lists (encode_order_words(max_batch))
 	uint32_t *d_import_slot = nullptr;   // slot scratch of cmb200_import_records_dev
 	size_t import_slot_cap = 0;
+	uint32_t *d_move_idx = nullptr;      // index scratch of cmb200_move_pages (2 x move_idx_cap), grown, never shrunk
+	size_t move_idx_cap = 0;
 	// page-locked staging for the small per-chunk arrays, so that no copy ever blocks the host
 	// thread that is feeding the pipeline (a pageable cudaMemcpyAsync waits for the stream)
 	static constexpr size_t META_CAP = 1u << 18;   // chunks per outer slice of a call
@@ -194,6 +197,7 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	cudaFree(e->table.slots); cudaFree(e->table.fp); cudaFree(e->arena.base); cudaFree(e->arena.seg); cudaFree(e->d_counters);
 	cudaFree(e->d_pages[0]); cudaFree(e->d_pages[1]); cudaFree(e->d_stage);
 	cudaFree(e->d_addr); cudaFree(e->d_ts); cudaFree(e->d_valid); cudaFree(e->d_slot); cudaFree(e->d_vlen);
+	cudaFree(e->d_move_idx);
 	if (e->h_meta) cudaFreeHost(e->h_meta);
 	for (auto &ln : e->lane) {
 		if (ln.st) { cudaStreamSynchronize(ln.st); cudaStreamDestroy(ln.st); }
@@ -806,7 +810,7 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	for (int r = 0; r < GET_MAX_PEERS; r++) { job.peer[r] = e->peer_base[r]; job.peer_size[r] = e->peer_size[r]; }
 	job.scratch = e->d_scratch; job.region_entries = e->region_entries; job.pool_bits = e->d_pool_bits; job.pool_n = e->pool_n;
 	job.hot = e->tier.hot();
-	if (launch_get_small(job, ln->st)) { ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1; }
+	if (launch_get_small(job, e->device, ln->st)) { ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1; }
 	t->lane = li; t->n = (uint32_t)n; t->status = ln->h_status;
 	return 0;
 }
@@ -1064,8 +1068,9 @@ struct SnapRecord { uint64_t ts, fp_hi, fp_lo; uint32_t len, zero; };
 static_assert(sizeof(SnapRecord) == 32, "snapshot record header");
 static const size_t SNAP_WINDOW = 64u << 20;
 
-extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records_out) {
-	std::lock_guard<std::mutex> g(e->mu);
+// Writes every live record of e to f through the page-locked window `win` and adds to *records /
+// *bytes.  (e->mu held)  0 = written, -1 = a CUDA call failed (error set), -2 = a write failed.
+static int save_engine(cmb200_engine *e, FILE *f, uint8_t *win, uint64_t *records, uint64_t *bytes) {
 	unsigned long long c[8];
 	if (read_counters(e, c)) return -1;
 	const unsigned long long cap_out = c[0] + 16;
@@ -1080,17 +1085,10 @@ extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records
 	std::vector<ExportEntry> list(count);
 	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list.p, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
 	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
+	*records += count;
+	for (const ExportEntry &x : list) *bytes += x.len;
 
-	std::string tmp = std::string(path) + ".tmp";
-	FILE *f = fopen(tmp.c_str(), "wb");
-	if (!f) { set_error_msg("cmb200_save: cannot create the snapshot file"); return -1; }
-	SnapHeader h{};
-	memcpy(h.magic, "CMB200S1", 8);
-	h.version = 1; h.pshift = (uint32_t)e->pshift; h.records = count; h.flags = e->table.fp ? 1u : 0u;
-	for (const ExportEntry &x : list) h.bytes += x.len;
-	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
-	uint8_t *win = nullptr;
-	if (cudaMallocHost(&win, SNAP_WINDOW) != cudaSuccess) { fclose(f); remove(tmp.c_str()); set_error_msg("cmb200_save: no page-locked window"); return -1; }
+	bool ok = true;
 	static const uint8_t zeros[16] = {0};
 	size_t k = 0;
 	while (ok && k < list.size()) {
@@ -1117,90 +1115,210 @@ extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records
 			    (padn == 0 || fwrite(zeros, padn, 1, f) == 1);
 		}
 	}
+	return ok ? 0 : -2;
+}
+
+extern "C" int cmb200_save_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out) {
+	if (g < 1 || !engines) { set_error_msg("cmb200_save_set: no engines"); return -1; }
+	for (int i = 1; i < g; i++)
+		if (engines[i]->pshift != engines[0]->pshift) { set_error_msg("cmb200_save_set: engines of different page sizes"); return -1; }
+	std::string tmp = std::string(path) + ".tmp";
+	FILE *f = fopen(tmp.c_str(), "wb");
+	if (!f) { set_error_msg("cmb200_save: cannot create the snapshot file"); return -1; }
+	uint8_t *win = nullptr;
+	if (cudaMallocHost(&win, SNAP_WINDOW) != cudaSuccess) { fclose(f); remove(tmp.c_str()); set_error_msg("cmb200_save: no page-locked window"); return -1; }
+	// the header goes first with the counts zero and is written again once every section is out
+	SnapHeader h{};
+	memcpy(h.magic, "CMB200S1", 8);
+	h.version = 1; h.pshift = (uint32_t)engines[0]->pshift; h.flags = engines[0]->table.fp ? 1u : 0u;
+	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
+	int rc = 0;
+	for (int i = 0; i < g && ok && rc == 0; i++) {
+		std::lock_guard<std::mutex> lk(engines[i]->mu);
+		rc = save_engine(engines[i], f, win, &h.records, &h.bytes);
+	}
 	cudaFreeHost(win);
+	ok = ok && rc != -2 && fseek(f, 0, SEEK_SET) == 0 && fwrite(&h, sizeof(h), 1, f) == 1;
 	ok = ok && fflush(f) == 0;
 	ok = (fclose(f) == 0) && ok;
-	if (!ok || rename(tmp.c_str(), path) != 0) { remove(tmp.c_str()); set_error_msg("cmb200_save: write failed"); return -1; }
-	if (records_out) *records_out = count;
+	if (rc == -1 || !ok || rename(tmp.c_str(), path) != 0) {
+		remove(tmp.c_str());
+		if (rc != -1) set_error_msg("cmb200_save: write failed");
+		return -1;
+	}
+	if (records_out) *records_out = h.records;
 	return 0;
+}
+
+extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records_out) {
+	return cmb200_save_set(&e, 1, path, records_out);
 }
 
 static int demote_arena_all(cmb200_engine *e);
 
-extern "C" int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out) {
+// One engine's share of a load: its records are staged in page-locked memory until the batch is full
+// (<= max_batch records and <= one page-ring buffer of bytes), then put in as one upsert + k_restore.
+struct LoadBatch {
+	cmb200_engine *e = nullptr;
+	uint8_t *blob = nullptr;
+	size_t cap = 0, B = 0, used = 0, m = 0;
+	std::vector<unsigned long long> off, ts, fps;
+	std::vector<cmb200_addr> addr;
+	unsigned long long *d_off = nullptr;
+	uint64_t *d_fp = nullptr;
+	int setup(cmb200_engine *eng) {
+		e = eng;
+		CMB_CHECK(cudaSetDevice(e->device));
+		cap = (size_t)e->host_batch * e->bsize;
+		B = e->max_batch < cmb200_engine::META_CAP ? e->max_batch : cmb200_engine::META_CAP;
+		off.resize(B); ts.resize(B); fps.resize(2 * B); addr.resize(B);
+		CMB_CHECK(cudaMallocHost(&blob, cap));
+		CMB_CHECK(cudaMalloc(&d_off, B * 8));
+		CMB_CHECK(cudaMalloc(&d_fp, B * 16));
+		return 0;
+	}
+	void release() {
+		if (!e) return;
+		cudaSetDevice(e->device);
+		if (blob) cudaFreeHost(blob);
+		if (d_off) cudaFree(d_off);
+		if (d_fp) cudaFree(d_fp);
+	}
+};
+
+// Puts the staged records into their engine as if they had been put in file order.  Returns how many
+// (>= 0) or -1.
+static long long load_flush(LoadBatch &b, bool with_fp) {
+	if (b.m == 0) return 0;
+	cmb200_engine *e = b.e;
 	std::lock_guard<std::mutex> g(e->mu);
 	CMB_CHECK(cudaSetDevice(e->device));
+	const size_t m = b.m;
+	if (e->tier.host) {
+		unsigned long long c[8];
+		if (read_counters(e, c)) return -1;
+		if (c[2] + b.used > e->arena.size && demote_arena_all(e)) return -1;
+	}
+	CMB_CHECK(cudaMemcpyAsync(e->d_pages[0], b.blob, b.used, cudaMemcpyHostToDevice, e->st));
+	CMB_CHECK(cudaMemcpyAsync(e->d_addr, b.addr.data(), m * 16, cudaMemcpyHostToDevice, e->st));
+	CMB_CHECK(cudaMemcpyAsync(e->d_ts, b.ts.data(), m * 8, cudaMemcpyHostToDevice, e->st));
+	CMB_CHECK(cudaMemcpyAsync(b.d_off, b.off.data(), m * 8, cudaMemcpyHostToDevice, e->st));
+	CMB_CHECK(cudaMemcpyAsync(b.d_fp, b.fps.data(), m * 16, cudaMemcpyHostToDevice, e->st));
+	if (launch_upsert(e->table, e->d_addr, nullptr, (uint32_t)m, e->seq, e->seq_stride, e->d_slot, e->st)) return -1;
+	EncodeJob job{};
+	job.n = (uint32_t)m; job.nbytes = e->bsize;
+	job.slot_idx = e->d_slot; job.addr = e->d_addr; job.ts = e->d_ts;
+	job.seq0 = e->seq; job.seq_stride = e->seq_stride;
+	job.table = e->table; job.arena = e->arena;
+	if (launch_restore(job, e->d_pages[0], b.d_off, with_fp ? b.d_fp : nullptr, e->bsize, e->st)) return -1;
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	e->seq += (unsigned long long)m * e->seq_stride;
+	e->stats.kernel_launches += 2;
+	b.m = 0; b.used = 0;
+	return (long long)m;
+}
+
+extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out) {
 	if (records_out) *records_out = 0;
+	if (g < 1 || !engines) { set_error_msg("cmb200_load_set: no engines"); return -1; }
 	FILE *f = fopen(path, "rb");
 	if (!f) { set_error_msg("cmb200_load: no snapshot file"); return -1; }
 	SnapHeader h{};
 	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "CMB200S1", 8) != 0 || h.version != 1) {
 		fclose(f); set_error_msg("cmb200_load: not a snapshot of this library"); return -1;
 	}
-	if ((int)h.pshift != e->pshift) { fclose(f); set_error_msg("cmb200_load: snapshot has another page size"); return -1; }
-	// batches: <= max_batch records and <= one page-ring buffer of bytes
-	const size_t blob_cap = (size_t)e->host_batch * e->bsize;
-	const size_t B = e->max_batch < cmb200_engine::META_CAP ? e->max_batch : cmb200_engine::META_CAP;
-	uint8_t *blob = nullptr;
-	if (cudaMallocHost(&blob, blob_cap) != cudaSuccess) { fclose(f); set_error_msg("cmb200_load: no page-locked buffer"); return -1; }
-	std::vector<unsigned long long> off(B), ts(B), fps(2 * B);
-	std::vector<cmb200_addr> addr(B);
-	DevBuf d_off, d_fp;
+	for (int i = 0; i < g; i++)
+		if ((int)h.pshift != engines[i]->pshift) { fclose(f); set_error_msg("cmb200_load: snapshot has another page size"); return -1; }
+	const uint32_t bsize = engines[0]->bsize;
+	std::vector<LoadBatch> bs(g);
 	int rc = 0;
-	if (d_off.alloc(B * 8) || d_fp.alloc(B * 16)) rc = -1;
+	for (int i = 0; i < g && rc == 0; i++)
+		if (bs[i].setup(engines[i])) { rc = -1; set_error_msg("cmb200_load: no staging buffers"); }
 	uint64_t done = 0, loaded = 0;
-	SnapRecord pending{}; bool have_pending = false;
 	while (rc == 0 && done < h.records) {
-		size_t m = 0, used = 0;
-		while (m < B && done + m < h.records) {
-			SnapRecord r;
-			if (have_pending) { r = pending; have_pending = false; }
-			else if (fread(&r, sizeof(r), 1, f) != 1) { rc = -1; break; }
-			const size_t padded = ((size_t)r.len + 15) & ~(size_t)15;
-			if (r.len < 24 || r.len > 24u + e->bsize + 1024u) { rc = -1; break; }
-			if (used + padded > blob_cap) { pending = r; have_pending = true; break; }
-			if (fread(blob + used, padded, 1, f) != 1) { rc = -1; break; }
-			{
-				// the record must be what filemap_set would have stored (filemap.c:124-147): a foreign or
-				// corrupt file must not reach k_restore, which trusts compressed_length
-				int32_t clen;
-				memcpy(&clen, blob + used + 16, 4);
-				if (clen < 0 || (uint32_t)clen > e->bsize + 1024u || r.len != 24u + (clen ? (uint32_t)clen : e->bsize)) { rc = -1; break; }
+		// record header and address first: the address names the engine whose batch takes the bytes
+		SnapRecord r;
+		cmb200_addr a;
+		if (fread(&r, sizeof(r), 1, f) != 1 || r.len < 24 || r.len > 24u + bsize + 1024u || fread(&a, 16, 1, f) != 1) {
+			rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
+		}
+		uint64_t key;
+		FNV_hash(&a, 16, &key);
+		LoadBatch &b = bs[cmb200_owner(key, g)];
+		const size_t padded = ((size_t)r.len + 15) & ~(size_t)15;
+		if (padded > b.cap) { rc = -1; set_error_msg("cmb200_load: record larger than the staging buffer"); break; }
+		if (b.m == b.B || b.used + padded > b.cap) {
+			const long long got = load_flush(b, h.flags & 1u);
+			if (got < 0) { rc = -1; break; }
+			loaded += (uint64_t)got;
+		}
+		uint8_t *rec = b.blob + b.used;
+		memcpy(rec, &a, 16);
+		if (fread(rec + 16, padded - 16, 1, f) != 1) { rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break; }
+		{
+			// the record must be what filemap_set would have stored (filemap.c:124-147): a foreign or
+			// corrupt file must not reach k_restore, which trusts compressed_length
+			int32_t clen;
+			memcpy(&clen, rec + 16, 4);
+			if (clen < 0 || (uint32_t)clen > bsize + 1024u || r.len != 24u + (clen ? (uint32_t)clen : bsize)) {
+				rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
 			}
-			memcpy(&addr[m], blob + used, 16);      // data_prefix {u, l}
-			off[m] = used; ts[m] = r.ts; fps[2 * m] = r.fp_hi; fps[2 * m + 1] = r.fp_lo;
-			used += padded; m++;
 		}
-		if (rc) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); break; }
-		if (m == 0) { rc = -1; set_error_msg("cmb200_load: record larger than the staging buffer"); break; }
-		if (e->tier.host) {
-			unsigned long long c[8];
-			if (read_counters(e, c)) { rc = -1; break; }
-			if (c[2] + used > e->arena.size && demote_arena_all(e)) { rc = -1; break; }
-		}
-		const bool fail =
-		    cudaMemcpyAsync(e->d_pages[0], blob, used, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
-		    cudaMemcpyAsync(e->d_addr, addr.data(), m * 16, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
-		    cudaMemcpyAsync(e->d_ts, ts.data(), m * 8, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
-		    cudaMemcpyAsync(d_off.p, off.data(), m * 8, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
-		    cudaMemcpyAsync(d_fp.p, fps.data(), m * 16, cudaMemcpyHostToDevice, e->st) != cudaSuccess;
-		if (fail || launch_upsert(e->table, e->d_addr, nullptr, (uint32_t)m, e->seq, e->seq_stride, e->d_slot, e->st)) { rc = -1; break; }
-		EncodeJob job{};
-		job.n = (uint32_t)m; job.nbytes = e->bsize;
-		job.slot_idx = e->d_slot; job.addr = e->d_addr; job.ts = e->d_ts;
-		job.seq0 = e->seq; job.seq_stride = e->seq_stride;
-		job.table = e->table; job.arena = e->arena;
-		if (launch_restore(job, e->d_pages[0], d_off.as<unsigned long long>(), (h.flags & 1u) ? d_fp.as<uint64_t>() : nullptr,
-			e->bsize, e->st)) { rc = -1; break; }
-		if (cudaStreamSynchronize(e->st) != cudaSuccess) { rc = -1; break; }
-		e->seq += (unsigned long long)m * e->seq_stride;
-		e->stats.kernel_launches += 2;
-		done += m; loaded += m;
+		b.addr[b.m] = a;
+		b.off[b.m] = b.used; b.ts[b.m] = r.ts; b.fps[2 * b.m] = r.fp_hi; b.fps[2 * b.m + 1] = r.fp_lo;
+		b.used += padded; b.m++;
+		done++;
 	}
-	cudaFreeHost(blob);
+	for (int i = 0; i < g && rc == 0; i++) {
+		const long long got = load_flush(bs[i], h.flags & 1u);
+		if (got < 0) rc = -1;
+		else loaded += (uint64_t)got;
+	}
+	for (LoadBatch &b : bs) b.release();
 	fclose(f);
 	if (records_out) *records_out = loaded;
 	return rc;
+}
+
+extern "C" int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out) {
+	return cmb200_load_set(&e, 1, path, records_out);
+}
+
+// ---- pages of a sharded store (CMB200_DEVICES): gather / scatter and peer copies ----------------
+
+extern "C" int cmb200_move_pages(cmb200_engine *e, size_t n, void *dst_dev, const uint32_t *dst_idx, const void *src_dev,
+    const uint32_t *src_idx) {
+	if (n == 0) return 0;
+	if (check_dev_pages(dst_dev, "cmb200_move_pages") || check_dev_pages(src_dev, "cmb200_move_pages")) return -1;
+	if (n > 0xffffffffu) { set_error_msg("cmb200_move_pages: too many pages"); return -1; }
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	if ((dst_idx || src_idx) && n > e->move_idx_cap) {
+		// grown to the largest call so far: a cudaFree per call would synchronise the whole device
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		cudaFree(e->d_move_idx);
+		e->d_move_idx = nullptr;
+		e->move_idx_cap = 0;
+		CMB_CHECK(cudaMalloc(&e->d_move_idx, n * 8));
+		e->move_idx_cap = n;
+	}
+	uint32_t *d_dst_idx = dst_idx ? e->d_move_idx : nullptr;
+	uint32_t *d_src_idx = src_idx ? e->d_move_idx + e->move_idx_cap : nullptr;
+	if (dst_idx) CMB_CHECK(cudaMemcpyAsync(d_dst_idx, dst_idx, n * 4, cudaMemcpyHostToDevice, e->st));
+	if (src_idx) CMB_CHECK(cudaMemcpyAsync(d_src_idx, src_idx, n * 4, cudaMemcpyHostToDevice, e->st));
+	if (launch_move_pages(dst_dev, d_dst_idx, src_dev, d_src_idx, (uint32_t)n, e->bsize, e->st)) return -1;
+	e->stats.kernel_launches++;
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	return 0;
+}
+
+extern "C" int cmb200_copy_peer(cmb200_engine *dst_e, void *dst_dev, cmb200_engine *src_e, const void *src_dev, size_t bytes) {
+	if (bytes == 0) return 0;
+	std::lock_guard<std::mutex> g(src_e->mu);
+	CMB_CHECK(cudaSetDevice(src_e->device));
+	CMB_CHECK(cudaMemcpyPeerAsync(dst_dev, dst_e->device, src_dev, src_e->device, bytes, src_e->st));
+	CMB_CHECK(cudaStreamSynchronize(src_e->st));
+	return 0;
 }
 
 // ---- arena compaction -------------------------------------------------------------------------

@@ -1115,23 +1115,26 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 	cluster_wait();
 }
 
-int launch_get_small(const GetJob &job, cudaStream_t st) {
+int launch_get_small(const GetJob &job, int device, cudaStream_t st) {
 	if (job.n == 0) return 0;
 	const size_t smem = get_small_smem(job.nbytes);
+	// the attribute belongs to the device: engines on several GPUs (CMB200_DEVICES) each set their own
+	constexpr int MAX_DEV = 64;
+	const int dev = device >= 0 && device < MAX_DEV ? device : 0;
 	if (job.nbytes > GS_MAX_PAGE) {
-		static size_t configured_pair = 0;
-		if (smem > configured_pair) {
+		static size_t configured_pair[MAX_DEV] = {};
+		if (smem > configured_pair[dev]) {
 			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-			configured_pair = smem;
+			configured_pair[dev] = smem;
 		}
 		k_get_small_pair<<<2u * job.n, GS_THREADS, smem, st>>>(job);
 		CMB_CHECK(cudaGetLastError());
 		return 0;
 	}
-	static size_t configured = 0;
-	if (smem > configured) {
+	static size_t configured[MAX_DEV] = {};
+	if (smem > configured[dev]) {
 		CMB_CHECK(cudaFuncSetAttribute(k_get_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-		configured = smem;
+		configured[dev] = smem;
 	}
 	k_get_small<<<job.n, GS_THREADS, smem, st>>>(job);
 	CMB_CHECK(cudaGetLastError());
@@ -1697,6 +1700,28 @@ int launch_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned
 	k_sample<<<GRID1D(n), 0, st>>>(t, r, n, addr_out, ts_out, ok);
 	CMB_CHECK(cudaGetLastError());
 	k_sample_scan<<<n < 1024u ? n : 1024u, 256, 0, st>>>(t, r, n, addr_out, ts_out, ok);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+// ---- page moves between the engines of a sharded store (cmb200_move_pages) --------------------
+// One warp per page: 32 lanes x 16 bytes per step, so a page of nbytes takes ceil(nbytes / 512) steps.
+// The pages of one owner are gathered into a contiguous buffer before a peer copy, or scattered
+// from one after it.
+__global__ void __launch_bounds__(256) k_move_pages(uint4 *dst, const uint32_t *dst_idx, const uint4 *src,
+    const uint32_t *src_idx, uint32_t n, uint32_t nbytes) {
+	const int lane = threadIdx.x & 31;
+	const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	if (i >= n) return;
+	const size_t words = nbytes >> 4;
+	uint4 *d = dst + (size_t)(dst_idx ? dst_idx[i] : i) * words;
+	const uint4 *s = src + (size_t)(src_idx ? src_idx[i] : i) * words;
+	for (size_t w = lane; w < words; w += 32) d[w] = s[w];
+}
+int launch_move_pages(void *dst, const uint32_t *dst_idx, const void *src, const uint32_t *src_idx, uint32_t n,
+    uint32_t nbytes, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_move_pages<<<(n * 32 + 255) / 256, 256, 0, st>>>((uint4 *)dst, dst_idx, (const uint4 *)src, src_idx, n, nbytes);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

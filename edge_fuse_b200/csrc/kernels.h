@@ -168,7 +168,7 @@ bool get_small_supports(uint32_t nbytes);
 size_t get_small_smem(uint32_t nbytes);
 uint32_t get_small_region_entries(uint32_t nbytes);
 int get_small_residency(uint32_t nbytes);   // requests resident on the device at once, < 0 on error
-int launch_get_small(const GetJob &job, cudaStream_t st);
+int launch_get_small(const GetJob &job, int device, cudaStream_t st);   // device: CUDA ordinal the launch runs on
 
 int launch_fingerprint(const uint8_t *pages, uint64_t stride, uint32_t nbytes, uint32_t n,
     uint64_t *fps, cudaStream_t st);
@@ -278,6 +278,11 @@ int launch_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, 
 
 // Re-inserts every live slot of `from` into the (zeroed) table `to` of the same geometry.
 int launch_rehash(TableView from, TableView to, cudaStream_t st);
+
+// dst[dst_idx ? dst_idx[i] : i] = src[src_idx ? src_idx[i] : i] for n pages of nbytes (a multiple of
+// 16; pages 16-byte aligned; index arrays in device memory).  One warp per page.
+int launch_move_pages(void *dst, const uint32_t *dst_idx, const void *src, const uint32_t *src_idx, uint32_t n,
+    uint32_t nbytes, cudaStream_t st);
 
 int sm_count();
 

@@ -89,6 +89,10 @@ int cachemap_checkpoint(struct cachemap *cm);
 /* requests / hits counters (cachemap.c:176,181) and the engine under the map. */
 void cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hits);
 struct cmb200_engine *cachemap_engine(struct cachemap *cm);
+/* Every engine under the map, in CMB200_DEVICES order (cachemap_engine is out[0]): stores up to max
+ * of them in out and returns how many there are, 0 if none could be started.  Like cachemap_engine,
+ * returns after every accepted put is in its engine. */
+int cachemap_engines(struct cachemap *cm, struct cmb200_engine **out, int max);
 
 #ifdef __cplusplus
 }

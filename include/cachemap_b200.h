@@ -162,6 +162,33 @@ int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out);
 int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records_out);
 int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out);
 
+/* ---- a store sharded by key over several engines (CMB200_DEVICES, one engine per listed GPU) -------
+ * key = FNV-1a-64 of the 16 address bytes (FNV_hash in uint128.h; the key of filemap.c:18-24).  Of g
+ * engines, the key belongs to engine cmb200_owner(key, g): the high 32 bits of the key scaled to g, so
+ * the split is even for any g and independent of the low bits the reference's 32 shards use
+ * (filemap.c:26-33).  This is the only definition; the drop-in and the snapshot code both call it.
+ * (C99 inline: cachemap_api.c emits the external definition, so the library exports it as well.) */
+inline int cmb200_owner(uint64_t key, int g) { return (int)(((key >> 32) * (uint64_t)g) >> 32); }
+
+/* cmb200_save / cmb200_load over g engines that split the keys by cmb200_owner.  The file is the one
+ * cmb200_save writes: one header, then the records of engine 0, 1, ...  Each engine's section is a
+ * point-in-time copy of that engine (the engine is locked while it is written, the others are not);
+ * the engines hold disjoint keys, so the union is a valid store.  cmb200_load_set reads the file once
+ * and puts each record into engine cmb200_owner(key, g), whatever g the file was written with.
+ * cmb200_save and cmb200_load are these calls with g = 1. */
+int cmb200_save_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out);
+int cmb200_load_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out);
+
+/* Moves n pages of the engine's page size within the engine's device memory:
+ * dst[dst_idx ? dst_idx[i] : i] = src[src_idx ? src_idx[i] : i] (one warp per page, 16-byte loads and
+ * stores; dst and src 16-byte aligned and not overlapping; the index arrays are host memory).  Returns
+ * when the pages have moved. */
+int cmb200_move_pages(cmb200_engine *e, size_t n, void *dst_dev, const uint32_t *dst_idx, const void *src_dev,
+    const uint32_t *src_idx);
+/* Copies `bytes` from device memory of engine src_e to device memory of engine dst_e (one
+ * cudaMemcpyPeerAsync; the two may be on the same GPU).  Returns when the bytes have arrived. */
+int cmb200_copy_peer(cmb200_engine *dst_e, void *dst_dev, cmb200_engine *src_e, const void *src_dev, size_t bytes);
+
 /* ---- host tier: records beyond the HBM arena ----------------------------------------------------
  * The reference keeps `capacity` pages in LMDB files on SSD; here the store is an HBM arena, which can
  * be far smaller than what `capacity` pages need.  A host tier is page-locked, device-mapped host
