@@ -4,7 +4,7 @@
 //   key table   (slots+2) x 64 B          replaces the 32 LMDB environments (filemap.c:54-90)
 //   arena       bump-allocated records    {24-byte data_prefix, LZ4 block | raw page}
 //   page ring   2 x max_batch x bsize     double-buffered landing zone for host pages
-//   stage       one (bsize+1024) row per resident encoder warp: block before it is packed into the arena
+//   stage       one max(bsize+1024, LZ4_compressBound) row per resident encoder warp: block before it is packed into the arena
 // Host tier (optional, cmb200_host_tier_enable): page-locked, device-mapped host memory holding records
 // demoted from the arena, a ring in demotion order (DESIGN.md §2).
 // A put batch is: H2D copy (copy stream)  ->  k_upsert  ->  k_encode (fingerprint + LZ4 + arena
@@ -298,7 +298,14 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 		e->table.remote = e->d_counters + 5;
 		e->arena.tier = e->d_counters + 6;
 
-		e->stage_stride = ((uint64_t)e->bsize + 1024 + 15) & ~15ull;        // filemap.c:120 dest[bsize+1024]
+		// filemap.c:120 dest[bsize+1024], but never below LZ4_compressBound: the encoder has no output
+		// limit, and above 128 KiB pages an incompressible block is longer than bsize + 1024 (k_encode
+		// then stores the page raw, as LZ4_compress_fast's 0 would make filemap_set do)
+		{
+			const uint64_t bound = (uint64_t)e->bsize + e->bsize / 255 + 16;
+			const uint64_t row = (uint64_t)e->bsize + 1024 > bound ? (uint64_t)e->bsize + 1024 : bound;
+			e->stage_stride = (row + 15) & ~15ull;
+		}
 		ENG_CHECK(cudaMalloc(&e->d_pages[0], (uint64_t)e->host_batch * e->bsize + 256));
 		ENG_CHECK(cudaMalloc(&e->d_pages[1], (uint64_t)e->host_batch * e->bsize + 256));
 		// one stage row per resident warp / group of the encode kernels (store mode), not per chunk
@@ -331,8 +338,9 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 		if (!arena) {
 			size_t free_b = 0, total_b = 0;
 			ENG_CHECK(cudaMemGetInfo(&free_b, &total_b));
-			// capacity worst-case records (incompressible pages: 24 + bsize + bsize/255 + 16) plus 1/8
-			// headroom, so that a store at capacity still has garbage worth compacting
+			// capacity worst-case records (24 + a stage row: a stored record is never longer, since a
+			// block longer than bsize + 1024 is stored as the raw page) plus 1/8 headroom, so that a
+			// store at capacity still has garbage worth compacting
 			uint64_t want = (cfg->capacity ? cfg->capacity : 1024) * (e->stage_stride + 32);
 			want += want / 8;
 			uint64_t lim = (uint64_t)(free_b * 0.8);

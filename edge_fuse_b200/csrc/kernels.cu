@@ -496,7 +496,7 @@ __global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WAR
 		    smem + (size_t)nwarps * (LZ4_TABLE_BYTES + RING_ALLOC) + (size_t)warp * RING_MBAR_BYTES, lane);
 	const uint32_t gw = blockIdx.x * (blockDim.x >> 5) + warp;         // resident warp slot
 	const bool direct = job.slot_idx != nullptr && job.arena.seg_bytes != 0u && job.accel != 0u && gw < ARENA_SEG_SLOTS;
-	// room one chunk may need while it is being encoded: prefix + a stage row (filemap.c:120 dest[bsize+1024])
+	// room one chunk may need while it is being encoded: prefix + a stage row (>= LZ4_compressBound)
 	const uint32_t worst = (uint32_t)((24u + job.stage_stride + 15u) & ~15ull);
 	unsigned long long seg_cur = 0, seg_end = 0;                         // lane 0's copy is the truth
 	if (direct && lane == 0) { seg_cur = job.arena.seg[2 * gw]; seg_end = job.arena.seg[2 * gw + 1]; }
@@ -568,8 +568,16 @@ __global__ void __launch_bounds__(ENC == 1 ? ENC_RING_WARPS * 32 : ENC_PLAIN_WAR
 		} else {
 			clen = lz4_encode_lean<WIDE, false, ENC == 1>(src, job.nbytes, dst, job.accel, wsm, ring, lane, fp_hi, fp_lo, ck);
 		}
-		if (lane == 0) job.lens[i] = (int32_t)clen;
-		if (store) {
+		// A store keeps at most bsize + 1024 block bytes (filemap.c:126, dstCapacity): above that,
+		// LZ4_compress_fast returns 0 (only incompressible pages of more than 128 KiB get there) and
+		// the page is stored raw, as with comp_accel == 0.  The block in the stage row or the segment
+		// is dropped; a direct segment's cursor stays where it was.
+		const bool raw = store && clen > job.nbytes + 1024u;
+		if (lane == 0) job.lens[i] = raw ? 0 : (int32_t)clen;
+		if (raw) {
+			__syncwarp();
+			commit_record(job, i, idx, src, job.nbytes, 0, true, fp_hi, fp_lo, lane);
+		} else if (store) {
 			__syncwarp();
 			if (in_arena) {
 				const uint32_t used = commit_direct(job, i, idx, base, clen, fp_hi, fp_lo, lane);

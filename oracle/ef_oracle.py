@@ -250,8 +250,10 @@ class StoreModel:
         if a is None:
             return
         key = addr_key(*a)
-        if self.accel:
-            blk = lz4_encode(page, self.accel)
+        blk = lz4_encode(page, self.accel) if self.accel else None
+        # filemap_set's dstCapacity is bsize + 1024 (filemap.c:126): LZ4_compress_fast returns 0 for a
+        # longer block, and this store keeps such a page raw (DESIGN.md, f1)
+        if blk is not None and len(blk) <= self.bsize + 1024:
             self.rec[key] = (a, len(blk), blk)
         else:
             self.rec[key] = (a, 0, bytes(_u8(page)))

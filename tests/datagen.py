@@ -76,6 +76,14 @@ def make_page(kind: str, n: int, seed: int) -> np.ndarray:
     raise ValueError(kind)
 
 
+def limit_page(n: int, seed: int, zero_at: int, zero_len: int) -> np.ndarray:
+    """Random bytes with one run of zeros: the run's length sets how far the page's LZ4 block falls
+    below the block of a fully random page (tests/golden/lz4_limit.json)."""
+    p = rand_bytes(seed, n)
+    p[zero_at:zero_at + zero_len] = 0
+    return p
+
+
 def pad_rows(pages: list[np.ndarray], stride: int | None = None) -> np.ndarray:
     n = max((len(p) for p in pages), default=0)
     stride = stride or max(16, (n + 15) // 16 * 16)

@@ -40,7 +40,7 @@ def _block_words(eng, u, l, bs):
 
 
 @pytest.mark.parametrize("accel", [12, 20])
-@pytest.mark.parametrize("pshift", [12, 14, 16, 17])
+@pytest.mark.parametrize("pshift", [6, 10, 12, 14, 16, 17])
 def test_encoder_words_equal_the_definition(E, gpu, pshift, accel):
     bs, n = 1 << pshift, 16
     pages = _pages(n, bs, 100 * pshift + accel)

@@ -62,7 +62,8 @@ def test_encode_golden_vectors(E, gpu, oracle):
 
 
 def test_encode_matches_oracle_many(E, gpu, oracle):
-    for n, accel, reps in ((65536, 12, 40), (4096, 12, 64), (131072, 12, 12), (32768, 1, 16), (65536, 97, 8)):
+    for n, accel, reps in ((65536, 12, 40), (4096, 12, 64), (131072, 12, 12), (32768, 1, 16), (65536, 97, 8),
+                           (64, 12, 64), (1024, 12, 64), (1 << 18, 12, 8), (1 << 20, 12, 8)):
         pages = [datagen.make_page("RTZMPAXS"[i % 8], n, 9000 + 31 * i + n) for i in range(reps)]
         blocks, _ = _encode_group(E, pages, n, accel)
         for i, (p, b) in enumerate(zip(pages, blocks)):
@@ -89,7 +90,7 @@ def test_encode_edge_inputs(E, gpu, oracle):
 
 
 def test_decode_matches_and_consumes(E, gpu, oracle):
-    for n in (65536, 4096, 131072, 5000):
+    for n in (65536, 4096, 131072, 5000, 64, 1024, 1 << 18, 1 << 20):
         pages = [datagen.make_page("RTZMPAXS"[i % 8], n, 50 + i + n) for i in range(24)]
         blocks = [oracle.lz4_encode(p, 12) for p in pages]
         out, used = E.lz4_decode_batch(blocks, n)

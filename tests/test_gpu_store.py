@@ -130,7 +130,8 @@ def test_store_semantics_vs_model(E, gpu, oracle):
 
 
 def test_raw_mode_and_other_page_sizes(E, gpu, oracle, tmp_path):
-    for pshift, accel in ((12, 0), (13, 12), (15, 12), (17, 12), (16, 0)):
+    for pshift, accel in ((12, 0), (13, 12), (15, 12), (17, 12), (16, 0),
+                          *((ps, a) for ps in (6, 8, 10, 11, 18, 19, 20) for a in (12, 0))):
         cm = E.Cachemap(str(tmp_path), 2048, accel, pshift)
         bs = 1 << pshift
         n = 40
@@ -366,6 +367,60 @@ print("direct ok", used)
     env = dict(os.environ, CMB200_SEG_KB="320")
     out = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=900)
     assert out.returncode == 0 and "direct ok" in out.stdout, out.stdout + out.stderr
+
+
+@pytest.mark.parametrize("seg_kb", ["0", "1"])       # stage rows / arena segments of one worst-case record
+@pytest.mark.parametrize("pshift", [18, 19, 20])
+def test_incompressible_large_pages_are_stored_raw(E, gpu, oracle, tmp_path, monkeypatch, pshift, seg_kb):
+    """Above 128 KiB an incompressible page's block is longer than the bsize + 1024 bytes filemap_set
+    gives LZ4_compress_fast; the page is stored raw (compressed_length 0, DESIGN.md f1) and the block,
+    written first, stays inside its stage row or arena segment.  Random pages alternate with
+    compressible ones so that neighbouring warps encode at the same time."""
+    monkeypatch.setenv("CMB200_SEG_KB", seg_kb)
+    monkeypatch.setenv("CMB200_PERSIST", "0")
+    bs, n, nh = 1 << pshift, {18: 256, 19: 160, 20: 128}[pshift], 0xB16
+    pages = np.stack([datagen.make_page("R" if i % 2 == 0 else "TX"[i // 2 % 2], bs, 31 * pshift + i) for i in range(n)])
+    u = np.full(n, nh, dtype=np.uint64)
+    l = np.arange(n, dtype=np.uint64)
+    model = oracle.StoreModel(pshift, 12)
+    for i in range(n):
+        model.put(i << pshift, nh, 0, pages[i])
+    exp = [model.record_bytes(nh, i) for i in range(n)]
+    exp_lens = [int.from_bytes(r[16:20], "little") for r in exp]
+    assert exp_lens.count(0) >= n // 4 and min(exp_lens[1::2]) > 0
+    row = 24 + max(bs + 1024, bs + bs // 255 + 16) + 16
+    geo = dict(pshift=pshift, accel=12, capacity=1024, arena_bytes=3 * n * row + (64 << 20), max_batch=256)
+    path = str(tmp_path / "large.snap")
+    eng = E.Engine(**geo)                      # one engine at a time: the stage alone is ~17 GB at 2^20
+    try:
+        lens = eng.put(u, l, pages)
+        assert lens.tolist() == exp_lens
+        assert eng.read_records(u, l) == exp
+        out, st = eng.get(u, l)
+        assert (st == E.HIT).all() and (out == pages).all()
+        assert eng.stats()["dropped_puts"] == 0
+        assert eng.save(path) == n
+    finally:
+        eng.close()
+    eng = E.Engine(**geo)
+    try:
+        assert eng.load(path) == n
+        assert eng.read_records(u, l) == exp
+        out, st = eng.get(u, l)
+        assert (st == E.HIT).all() and (out == pages).all()
+    finally:
+        eng.close()
+    cm = E.Cachemap(str(tmp_path), 1024, 12, pshift)
+    off = l << np.uint64(pshift)
+    gen = np.zeros(n, dtype=np.uint32)
+    cm.put_batch(off, u, gen, pages)
+    out, hit = cm.get_batch(off, u, gen)
+    assert hit.all() and (out == pages).all()
+    view = E.Engine.__new__(E.Engine); view.h = cm.engine_handle(); view.bsize = bs
+    assert view.read_records(u, l) == exp
+    assert view.stats()["dropped_puts"] == 0
+    view.h = None
+    cm.free()
 
 
 @pytest.mark.gpu

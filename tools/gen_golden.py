@@ -4,7 +4,7 @@
 own uint128.h).  Run in the authoring container only; the fixtures it writes are committed and
 are what pins the oracle (and, on the GPU box, the CUDA path) where /root/reference is absent.
 
-    python tools/gen_golden.py [lz4 keys ref_blocks exerciser store]
+    python tools/gen_golden.py [lz4 keys ref_blocks limit exerciser store]
 """
 from __future__ import annotations
 
@@ -71,6 +71,34 @@ def gen_ref_blocks():
                    "sweep": rows(datagen.reference_sweep_cases()),
                    "gpu": rows(datagen.gpu_reference_cases())}, f, indent=0)
     print("reference blocks written")
+
+
+def gen_limit():
+    """The reference's LZ4_compress_fast with filemap_set's dstCapacity of n + 1024 (filemap.c:126) on
+    pages whose unlimited block is within 24 bytes of that limit (pshift 18-20), plus random pages at
+    pshift 17, where every block fits.  ref_len 0: the reference refused the page."""
+    out = []
+    for pshift in (17, 18, 19, 20):
+        n = 1 << pshift
+        for seed in range(3):
+            for accel in (12, 1):
+                base = len(O.lz4_encode(datagen.limit_page(n, 100 * pshift + seed, 0, 0), accel))
+                # a zero run near the page start (where the match search still steps byte by byte)
+                # shortens the block by about its length
+                zlens = [0] if pshift == 17 else range(max(0, base - n - 1024 - 24), base - n - 1024 + 25, 2)
+                for z in zlens:
+                    at = 16 * seed
+                    page = datagen.limit_page(n, 100 * pshift + seed, at, z)
+                    ours = len(O.lz4_encode(page, accel))
+                    if pshift > 17 and abs(ours - (n + 1024)) > 24:
+                        continue
+                    out.append([pshift, accel, 100 * pshift + seed, at, z, len(O.ref_lz4_encode(page, accel))])
+    with open(os.path.join(GOLD, "lz4_limit.json"), "w") as f:
+        json.dump({"generator": "tools/gen_golden.py", "reference": "LZ4_compress_fast(page, dst, n, n + 1024, accel) "
+                   "of cachemap/lz4.c (v1.8.1), called as filemap.c:126 does",
+                   "columns": ["pshift", "accel", "seed", "zero_at", "zero_len", "ref_len (0: refused)"],
+                   "page": "tests/datagen.py limit_page(1 << pshift, seed, zero_at, zero_len)", "cases": out}, f, indent=0)
+    print("limit cases:", len(out), "refused:", sum(1 for r in out if r[-1] == 0))
 
 
 def gen_exerciser(seeds=(1, 2, 3), objects=32768, pshift=15):
@@ -186,7 +214,7 @@ def gen_store():
 if __name__ == "__main__":
     assert O.ref() is not None, "oracle/_ref/libcachemap_ref.so missing: run make -C oracle"
     os.makedirs(GOLD, exist_ok=True)
-    steps = {"lz4": gen_lz4, "keys": gen_keys, "ref_blocks": gen_ref_blocks, "exerciser": gen_exerciser,
+    steps = {"lz4": gen_lz4, "keys": gen_keys, "ref_blocks": gen_ref_blocks, "limit": gen_limit, "exerciser": gen_exerciser,
              "store": gen_store}                   # gen_store ends the process: keep it last
     for name in sys.argv[1:] or steps:
         steps[name]()
