@@ -30,7 +30,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_put_batch", "cmb200_put_batch_dev", "cmb200_put_batch_async", "cmb200_wait", "cmb200_get_batch", "cmb200_get_batch_dev",
     "cmb200_unset_batch", "cmb200_entries", "cmb200_sample", "cmb200_read_records",
     "cmb200_read_fingerprints", "cmb200_get_stats", "cmb200_compose_keys",
-    "cmb200_set_stream_order", "cmb200_import_remote", "cmb200_locate_batch", "cmb200_save", "cmb200_load",
+    "cmb200_set_stream_order", "cmb200_locate_batch", "cmb200_save", "cmb200_load",
     "cmb200_put_step", "cmb200_import_records_dev", "cmb200_compact",
     "cmb200_get_small", "cmb200_get_small_begin", "cmb200_get_small_end", "cmb200_arena_ipc_handle", "cmb200_open_peer", "cmb200_close_peers",
     "cmb200_lz4_encode_batch", "cmb200_lz4_decode_batch", "cmb200_fingerprint_batch", "cmb200_fingerprint_dev",
@@ -132,7 +132,6 @@ def lib() -> C.CDLL:
         "cmb200_read_fingerprints": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_get_stats": (i32, [vp, vp]),
         "cmb200_set_stream_order": (i32, [vp, u64, u64]),
-        "cmb200_import_remote": (i32, [vp, sz, vp, vp, vp, vp, i32]),
         "cmb200_get_small": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_get_small_begin": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_get_small_end": (i32, [vp, vp, vp]),
@@ -521,14 +520,6 @@ class Engine:
 
     def set_stream_order(self, next_seq: int, stride: int):
         _check(lib().cmb200_set_stream_order(self.h, next_seq, stride), "cmb200_set_stream_order")
-
-    def import_remote(self, u, l, owner, seq, loc=None):
-        addr = _addr_array(u, l)
-        owner = np.ascontiguousarray(owner, dtype=np.uint32)
-        seq = np.ascontiguousarray(seq, dtype=np.uint64)
-        loc = None if loc is None else np.ascontiguousarray(loc, dtype=np.uint64)
-        _check(lib().cmb200_import_remote(self.h, len(addr), _ptr(addr), _ptr(owner), _ptr(seq), _ptr(loc), 0),
-               "cmb200_import_remote")
 
     def locate(self, u, l):
         addr = _addr_array(u, l)

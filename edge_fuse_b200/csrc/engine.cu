@@ -717,6 +717,20 @@ extern "C" int cmb200_get_batch(cmb200_engine *e, size_t n, const cmb200_addr *a
     void *pages_out_host, int32_t *status_out) {
 	return get_impl(e, n, addr, valid, (uint8_t *)pages_out_host, false, status_out);
 }
+// Looks up m <= max_batch host addresses and brings each one's status, location and vlen (stored
+// length + 1; nullable) to the host.  For ST_REMOTE the location is the owner rank (k_lookup).  The
+// callers count the launch.  (e->mu held)
+static int lookup_chunk(cmb200_engine *e, const cmb200_addr *addr, uint32_t m, int32_t *status, uint64_t *loc,
+    uint32_t *vlen) {
+	CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
+	if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
+	CMB_CHECK(cudaMemcpyAsync(status, e->d_status, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaMemcpyAsync(loc, e->d_recoff, (size_t)m * 8, cudaMemcpyDeviceToHost, e->st));
+	if (vlen) CMB_CHECK(cudaMemcpyAsync(vlen, e->d_vlen, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	return 0;
+}
+
 extern "C" int cmb200_locate_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, int32_t *status_out,
     uint64_t *owner_out) {
 	// lookup only: which requests hit here, miss, or live on another rank (owner_out = rank)
@@ -724,13 +738,9 @@ extern "C" int cmb200_locate_batch(cmb200_engine *e, size_t n, const cmb200_addr
 	CMB_CHECK(cudaSetDevice(e->device));
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
-		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
-		if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
-		CMB_CHECK(cudaMemcpyAsync(status_out + at, e->d_status, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaMemcpyAsync(owner_out + at, e->d_recoff, (size_t)m * 8, cudaMemcpyDeviceToHost, e->st));
+		if (lookup_chunk(e, addr + at, m, status_out + at, owner_out + at, nullptr)) return -1;
 		e->stats.kernel_launches++;
 	}
-	CMB_CHECK(cudaStreamSynchronize(e->st));
 	return 0;
 }
 extern "C" int cmb200_get_batch_dev(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
@@ -745,31 +755,6 @@ extern "C" int cmb200_set_stream_order(cmb200_engine *e, uint64_t next_seq, uint
 	if (multi_gpu_call(e, "cmb200_set_stream_order")) return -1;
 	if (stride == 0) { set_error_msg("stream order: stride must be >= 1"); return -1; }
 	e->seq = next_seq; e->seq_stride = stride;
-	return 0;
-}
-
-extern "C" int cmb200_import_remote(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint32_t *owner,
-    const uint64_t *seq, const uint64_t *loc, int on_dev) {
-	std::lock_guard<std::mutex> g(e->mu);
-	if (multi_gpu_call(e, "cmb200_import_remote")) return -1;
-	CMB_CHECK(cudaSetDevice(e->device));
-	for (size_t at = 0; at < n; at += e->max_batch) {
-		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
-		const unsigned long long *d_a; const uint32_t *d_o; const unsigned long long *d_s; const unsigned long long *d_l = nullptr;
-		if (on_dev) {
-			d_a = (const unsigned long long *)(addr + at); d_o = owner + at; d_s = (const unsigned long long *)(seq + at);
-			if (loc) d_l = (const unsigned long long *)(loc + at);
-		} else {
-			CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
-			CMB_CHECK(cudaMemcpyAsync(e->d_vlen, owner + at, (size_t)m * 4, cudaMemcpyHostToDevice, e->st));
-			CMB_CHECK(cudaMemcpyAsync(e->d_ts, seq + at, (size_t)m * 8, cudaMemcpyHostToDevice, e->st));
-			if (loc) CMB_CHECK(cudaMemcpyAsync(e->d_recoff, loc + at, (size_t)m * 8, cudaMemcpyHostToDevice, e->st));
-			d_a = e->d_addr; d_o = e->d_vlen; d_s = e->d_ts; d_l = loc ? (const unsigned long long *)e->d_recoff : nullptr;
-		}
-		if (launch_import(e->table, e->arena, d_a, d_o, d_s, d_l, m, e->d_slot, e->st)) return -1;
-		e->stats.kernel_launches += 2;
-	}
-	CMB_CHECK(cudaStreamSynchronize(e->st));
 	return 0;
 }
 
@@ -987,12 +972,7 @@ extern "C" int cmb200_read_records(cmb200_engine *e, size_t n, const cmb200_addr
 	std::vector<uint32_t> vl(e->max_batch);
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
-		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
-		if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
-		CMB_CHECK(cudaMemcpyAsync(st.data(), e->d_status, m * 4, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaMemcpyAsync(off.data(), e->d_recoff, m * 8, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaMemcpyAsync(vl.data(), e->d_vlen, m * 4, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaStreamSynchronize(e->st));
+		if (lookup_chunk(e, addr + at, m, st.data(), off.data(), vl.data())) return -1;
 		for (uint32_t i = 0; i < m; i++) {
 			if (st[i] != ST_HIT) { len_out[at + i] = -1; continue; }
 			uint32_t clen = vl[i] - 1;
@@ -1053,6 +1033,29 @@ extern "C" int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_
 	return 0;
 }
 
+// Every live local record (arena_only: leave out the host tier's), sorted by offset, and the counters
+// read just before the export.  (e->mu held)  0 = listed, -1 = a CUDA call failed (error set), 1 = more
+// than c[0] + 16 records were found (the store changed since the counters were read): the list holds
+// c[0] + 16 of them.
+static int live_records(cmb200_engine *e, bool arena_only, std::vector<ExportEntry> &list, unsigned long long c[8]) {
+	if (read_counters(e, c)) return -1;
+	const unsigned long long cap_out = c[0] + 16;
+	DevBuf d_list, d_count;
+	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
+	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
+	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out,
+		arena_only, e->st)) return -1;
+	unsigned long long count = 0;
+	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	const int over = count > cap_out;
+	if (over) count = cap_out;
+	list.resize(count);
+	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list.p, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
+	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
+	return over;
+}
+
 // ---- snapshot: persistence of the cache directory (SURVEY.md 8 f3) ---------------------------
 //
 // The reference's store is persistent because it IS a set of LMDB files under <cachedir>
@@ -1080,20 +1083,9 @@ static const size_t SNAP_WINDOW = 64u << 20;
 // *bytes.  (e->mu held)  0 = written, -1 = a CUDA call failed (error set), -2 = a write failed.
 static int save_engine(cmb200_engine *e, FILE *f, uint8_t *win, uint64_t *records, uint64_t *bytes) {
 	unsigned long long c[8];
-	if (read_counters(e, c)) return -1;
-	const unsigned long long cap_out = c[0] + 16;
-	DevBuf d_list, d_count;
-	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
-	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
-	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, false, e->st)) return -1;
-	unsigned long long count = 0;
-	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
-	CMB_CHECK(cudaStreamSynchronize(e->st));
-	if (count > cap_out) count = cap_out;
-	std::vector<ExportEntry> list(count);
-	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list.p, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
-	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
-	*records += count;
+	std::vector<ExportEntry> list;
+	if (live_records(e, false, list, c) < 0) return -1;
+	*records += list.size();
 	for (const ExportEntry &x : list) *bytes += x.len;
 
 	bool ok = true;
@@ -1339,23 +1331,16 @@ extern "C" int cmb200_copy_peer(cmb200_engine *dst_e, void *dst_dev, cmb200_engi
 // (e->mu held)
 static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 	cmb200_engine::GateClosed gg(e->get_gate);          // records move: no small get may be reading the arena
-	unsigned long long c[8];
-	if (read_counters(e, c)) return -1;
 	harvest_pending(e, true);
-	const unsigned long long head_before = c[2];
-	const unsigned long long cap_out = c[0] + 16;
-	DevBuf d_list, d_count, d_moves;
-	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
-	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
+	unsigned long long c[8];
+	std::vector<ExportEntry> list;
 	// arena records only: the host tier is a ring and is never compacted
-	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, true, e->st)) return -1;
-	unsigned long long count = 0;
-	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
-	CMB_CHECK(cudaStreamSynchronize(e->st));
-	if (count > cap_out) { set_error_msg("cmb200_compact: the store changed under the compaction"); return -1; }
-	std::vector<ExportEntry> list(count);
-	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list.p, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
-	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
+	const int listed = live_records(e, true, list, c);
+	if (listed < 0) return -1;
+	if (listed > 0) { set_error_msg("cmb200_compact: the store changed under the compaction"); return -1; }
+	const unsigned long long head_before = c[2];
+	const size_t count = list.size();
+	DevBuf d_moves;
 	std::vector<MoveEntry> moves(count);
 	unsigned long long at = 0;
 	for (size_t i = 0; i < count; i++) {
@@ -1541,12 +1526,7 @@ extern "C" int cmb200_demote_batch(cmb200_engine *e, size_t n, const cmb200_addr
 	uint64_t done = 0;
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
-		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
-		if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
-		CMB_CHECK(cudaMemcpyAsync(st.data(), e->d_status, m * 4, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaMemcpyAsync(off.data(), e->d_recoff, m * 8, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaMemcpyAsync(vl.data(), e->d_vlen, m * 4, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaStreamSynchronize(e->st));
+		if (lookup_chunk(e, addr + at, m, st.data(), off.data(), vl.data())) return -1;
 		e->stats.kernel_launches++;
 		// absent, remote and host-tier keys are skipped; a key named twice moves once
 		recs.clear();
@@ -1567,19 +1547,8 @@ extern "C" int cmb200_demote_batch(cmb200_engine *e, size_t n, const cmb200_addr
 // not fit the arena continues into the tier.
 static int demote_arena_all(cmb200_engine *e) {
 	unsigned long long c[8];
-	if (read_counters(e, c)) return -1;
-	const unsigned long long cap_out = c[0] + 16;
-	DevBuf d_list, d_count;
-	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
-	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
-	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out, true, e->st)) return -1;
-	unsigned long long count = 0;
-	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
-	CMB_CHECK(cudaStreamSynchronize(e->st));
-	if (count > cap_out) count = cap_out;
-	std::vector<ExportEntry> list(count);
-	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list.p, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
-	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
+	std::vector<ExportEntry> list;
+	if (live_records(e, true, list, c) < 0) return -1;
 	std::vector<std::pair<unsigned long long, uint32_t>> recs;
 	for (const ExportEntry &x : list) recs.emplace_back(x.rec_off, x.len);
 	if (demote_records(e, recs)) return -1;
@@ -1608,12 +1577,7 @@ extern "C" int cmb200_promote_batch(cmb200_engine *e, size_t n, const cmb200_add
 	bool full = false;
 	for (size_t at = 0; at < n && !full; at += e->max_batch) {
 		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
-		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
-		if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
-		CMB_CHECK(cudaMemcpyAsync(st.data(), e->d_status, m * 4, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaMemcpyAsync(off.data(), e->d_recoff, m * 8, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaMemcpyAsync(vl.data(), e->d_vlen, m * 4, cudaMemcpyDeviceToHost, e->st));
-		CMB_CHECK(cudaStreamSynchronize(e->st));
+		if (lookup_chunk(e, addr + at, m, st.data(), off.data(), vl.data())) return -1;
 		e->stats.kernel_launches++;
 		// absent, remote and arena keys are skipped; a key named twice moves once (a later chunk's
 		// lookup runs after this chunk's promotion on the stream and finds it in the arena)

@@ -300,6 +300,20 @@ __device__ __forceinline__ void ckpt_store(const EncodeJob &job, uint32_t idx, u
 	if (lane == 0) *reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(off, clen);
 }
 
+// The record of slot idx moved from old_loc to new_loc with its block unchanged (compaction, demotion,
+// promotion), so its checkpoints still hold and only the tag moves.  A tag that names another record
+// version (or none) is left alone.  The fence orders the caller's rec_off store before the new tag,
+// so a reader that sees the tag also sees the location it names.  (one thread)
+__device__ __forceinline__ void ckpt_retag(const TableView &t, uint32_t idx, unsigned long long old_loc,
+    unsigned long long new_loc, uint32_t clen) {
+	if (!t.ckpt) return;
+	uint32_t *w = t.ckpt + (size_t)idx * CKPT_WORDS;
+	if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(old_loc, clen)) {
+		__threadfence();
+		*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(new_loc, clen);
+	}
+}
+
 // Stores the finished block as a filemap record {data_prefix, block} (filemap.c:140-147) and
 // publishes it in the key table.  Called by the whole warp; lane 0 owns the bookkeeping.
 __device__ unsigned long long commit_record(const EncodeJob &job, uint32_t i, uint32_t idx, const uint8_t *payload,
@@ -1219,44 +1233,6 @@ int launch_compose(const uint64_t *offset, const uint64_t *nhid, const uint32_t 
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
-// Multi-GPU import, phase 1: claim the slot and record stream order; phase 2: the newest
-// sequence per key applies itself (a key may appear several times in one import).
-__global__ void k_import_claim(TableView t, const unsigned long long *addr, const unsigned long long *seq,
-    uint32_t n, uint32_t *slot_idx) {
-	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	uint32_t idx = table_find_or_claim(t, fnv_addr(addr[2 * i], addr[2 * i + 1]));
-	if (idx != 0xffffffffu) atomicMax(&t.slots[idx].seq, seq[i]);
-	slot_idx[i] = idx;
-}
-__global__ void k_import_apply(TableView t, ArenaView a, const unsigned long long *addr, const uint32_t *owner,
-    const unsigned long long *seq, const unsigned long long *loc, uint32_t n, const uint32_t *slot_idx) {
-	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	uint32_t idx = slot_idx[i];
-	if (idx == 0xffffffffu) return;
-	Slot &s = t.slots[idx];
-	if (s.seq != seq[i]) return;                 // an even newer put (local or imported) owns the key
-	if (s.vlen) {                                // our local record is superseded
-		atomicAdd(t.entries, (unsigned long long)-1ll);
-		atomicAdd(a.garbage, (unsigned long long)s.alloc);
-		s.vlen = 0; s.alloc = 0;
-	}
-	if (s.owner == 0) atomicAdd(t.remote, 1ull);
-	s.addr_u = addr[2 * i]; s.addr_l = addr[2 * i + 1];
-	s.rec_off = loc ? xrec_off(loc[i]) : 0ull; s.alloc = loc ? xrec_len1(loc[i]) : 0u;   // 0 = location unknown
-	__threadfence();
-	s.owner = (unsigned long long)owner[i] + 1;
-}
-int launch_import(TableView t, ArenaView a, const unsigned long long *addr, const uint32_t *owner,
-    const unsigned long long *seq, const unsigned long long *loc, uint32_t n, uint32_t *slot_idx, cudaStream_t st) {
-	if (n == 0) return 0;
-	k_import_claim<<<GRID1D(n), 0, st>>>(t, addr, seq, n, slot_idx);
-	CMB_CHECK(cudaGetLastError());
-	k_import_apply<<<GRID1D(n), 0, st>>>(t, a, addr, owner, seq, loc, n, slot_idx);
-	CMB_CHECK(cudaGetLastError());
-	return 0;
-}
 // ---- multi-GPU exchange records, device resident ------------------------------------------------
 // One 32-byte record per chunk of a put step: {u, l, global stream position, tail}; tail is
 // xrec_tail(owner rank, arena offset, stored length) (kernels.h; edge_fuse_b200/sharding.py has the
@@ -1283,6 +1259,8 @@ int launch_pack_records(const unsigned long long *addr, const int32_t *lens, con
 	return 0;
 }
 // Import straight from all-gathered records: rows of `my_rank` and rows that stored nothing are skipped.
+// Phase 1 claims the slot and records stream order; phase 2: the newest sequence per key applies
+// itself (a key may appear several times in one import).
 __global__ void k_import_claim_rec(TableView t, const unsigned long long *rec, uint32_t n, uint32_t my_rank,
     uint32_t *slot_idx) {
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1522,15 +1500,7 @@ __global__ void __launch_bounds__(256) k_compact_scatter(TableView t, ArenaView 
 		Slot &s = t.slots[m.slot];
 		s.rec_off = m.new_off;
 		s.alloc = (m.len + 15u) & ~15u;
-		if (t.ckpt) {
-			// the block is unchanged, so are its checkpoints: only the tag moves (as in k_demote_publish)
-			const uint32_t clen = s.vlen - 1u;
-			uint32_t *w = t.ckpt + (size_t)m.slot * CKPT_WORDS;
-			if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(m.old_off, clen)) {
-				__threadfence();
-				*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(m.new_off, clen);
-			}
-		}
+		ckpt_retag(t, m.slot, m.old_off, m.new_off, s.vlen - 1u);
 	}
 }
 int launch_compact_window(TableView t, ArenaView a, const MoveEntry *moves, uint32_t n, uint8_t *bounce,
@@ -1569,14 +1539,7 @@ __global__ void k_demote_publish(TableView t, ArenaView a, const DemoteEntry *d,
 	atomicAdd(a.tier + 1, 1ull);
 	s.alloc = (m.len + 15u) & ~15u;
 	*reinterpret_cast<volatile unsigned long long *>(&s.rec_off) = loc;      // the one store readers trust
-	if (t.ckpt) {
-		// the block is unchanged, so are its checkpoints: only the tag moves to the new location
-		uint32_t *w = t.ckpt + (size_t)idx * CKPT_WORDS;
-		if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(m.old_off, clen)) {
-			__threadfence();
-			*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(loc, clen);
-		}
-	}
+	ckpt_retag(t, idx, m.old_off, loc, clen);
 }
 int launch_demote_gather(ArenaView a, const DemoteEntry *d, uint32_t n, uint8_t *bounce, cudaStream_t st) {
 	if (n == 0) return 0;
@@ -1620,14 +1583,7 @@ __global__ void __launch_bounds__(256) k_promote(TableView t, ArenaView a, const
 	atomicAdd(a.tier + 1, (unsigned long long)-1ll);
 	s->alloc = need;
 	*reinterpret_cast<volatile unsigned long long *>(&s->rec_off) = m.new_off;   // the one store readers trust
-	if (t.ckpt) {
-		// the block is unchanged, so are its checkpoints: only the tag moves to the new location
-		uint32_t *w = t.ckpt + (size_t)idx * CKPT_WORDS;
-		if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(loc, clen)) {
-			__threadfence();
-			*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(m.new_off, clen);
-		}
-	}
+	ckpt_retag(t, idx, loc, m.new_off, clen);
 }
 int launch_promote(TableView t, ArenaView a, const PromoteEntry *p, uint32_t n, const uint8_t *host, cudaStream_t st) {
 	if (n == 0) return 0;

@@ -180,13 +180,9 @@ int launch_compose(const uint64_t *offset, const uint64_t *nhid, const uint32_t 
 int launch_upsert(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
     unsigned long long seq0, unsigned long long seq_stride, uint32_t *slot_idx, cudaStream_t st);
 
-// Multi-GPU index replication: records {addr, owner rank, seq} written on other GPUs.  Newest
-// sequence per key wins; a local record that loses is retired.
-int launch_import(TableView t, ArenaView a, const unsigned long long *addr, const uint32_t *owner,
-    const unsigned long long *seq, const unsigned long long *loc, uint32_t n, uint32_t *slot_idx, cudaStream_t st);
-
-// The same exchange with the records staying on the device: pack one 32-byte record per chunk of a
-// put step, import all-gathered records (rows of my_rank / rows that stored nothing are skipped).
+// Multi-GPU index replication, the records staying on the device: pack one 32-byte record per chunk
+// of a put step, import all-gathered records written on other GPUs (rows of my_rank / rows that stored
+// nothing are skipped).  Newest sequence per key wins; a local record that loses is retired.
 // Record = {u, l, global stream position, tail}; tail = owner rank << 56 | arena offset / 16 << 22 |
 // stored length + 1 (0 = the chunk stored nothing).  The location lets another GPU read the record
 // from the owner's arena over NVLink (k_get_small).

@@ -4,9 +4,10 @@ Chunk k of the global stream belongs to rank k mod world (round-robin); every ra
 stores its own chunks with no data-path collective.  What is replicated is the key index: after
 each batch the ranks all-gather one fixed-size record per stored chunk — {address u, address l,
 global stream position, owner rank | stored length} = 32 bytes — over NCCL (NVLink / NVSwitch) and
-import the other ranks' records into their table replica (cmb200_import_remote), where the highest
-stream position per key wins, i.e. the outcome of the sequential reference.  torch.distributed is
-only the transport; the table logic is in the CUDA library.
+import the other ranks' records into their table replica (cmb200_import_records_dev, straight from
+the gathered records), where the highest stream position per key wins, i.e. the outcome of the
+sequential reference.  torch.distributed is only the transport; the table logic is in the CUDA
+library.
 """
 from __future__ import annotations
 
@@ -94,26 +95,28 @@ def resolve_newest(records: np.ndarray) -> dict:
 
 
 def import_gathered(engine, gathered, rank: int) -> int:
-    """Imports the other ranks' rows of an all-gathered record tensor (CUDA tensor) into `engine`'s
-    index replica.  Returns the number of rows imported."""
-    import torch
-    rows = remote_rows(gathered, rank)
-    n = int(rows.shape[0])
+    """Imports the other ranks' rows of an all-gathered [n, 4] int64 record tensor into `engine`'s
+    index replica (cmb200_import_records_dev, which skips the rows of `rank` and the rows that stored
+    nothing).  A CUDA tensor must be on the engine's device; a CPU tensor is copied there first.  The
+    import is complete on return.  Returns the number of rows imported."""
+    _, _, _, owner, length = unpack_records(gathered)
+    n = int(((owner != rank) & (length >= 0)).sum())
     if n == 0:
         return 0
-    addr = rows[:, :2].contiguous()
-    seq = rows[:, 2].contiguous()
-    loc = rows[:, 3].contiguous()
-    owner = ((rows[:, 3] >> 56) & 0xFF).to(torch.int32).contiguous()
+    rows = gathered.contiguous()
     if rows.is_cuda:
-        torch.cuda.current_stream(rows.device).synchronize()
-        from .binding import lib, _check
-        _check(lib().cmb200_import_remote(engine.h, n, addr.data_ptr(), owner.data_ptr(), seq.data_ptr(), loc.data_ptr(), 1),
-               "cmb200_import_remote")
-    else:
-        a = addr.numpy().view(np.uint64)
-        engine.import_remote(a[:, 0], a[:, 1], owner.numpy().view(np.uint32), seq.numpy().view(np.uint64),
-                             loc.numpy().view(np.uint64))
+        import torch
+        torch.cuda.current_stream(rows.device).synchronize()      # the gather has landed before the engine reads it
+        engine.import_records_dev(rows.shape[0], rows.data_ptr(), rank)
+        engine.sync()
+        return n
+    d = engine.dev_alloc(rows.numel() * 8)
+    try:
+        engine.h2d(d, rows.numpy())
+        engine.import_records_dev(rows.shape[0], d, rank)
+        engine.sync()
+    finally:
+        engine.dev_free(d)
     return n
 
 

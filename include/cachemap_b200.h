@@ -133,10 +133,13 @@ int cmb200_get_stats(cmb200_engine *e, cmb200_stats *out);
  * queued behind them at once), or device resident (pages_on_dev = 1, same lifetime rule, and
  * 16-byte aligned as for cmb200_put_batch_dev),
  * and additionally writes one 32-byte exchange record per chunk — {u, l, global stream position,
- * rank << 32 | stored length (negative: nothing stored)} — to records_dev_out (device memory,
- * n x 32 bytes) on the engine's stream.  The caller all-gathers those records (NCCL, on that
- * stream) and hands the result to cmb200_import_records_dev, which imports the rows of the other
- * ranks into the index replica, again without a host round trip.  n <= 262144. */
+ * rank << 56 | arena offset / 16 << 22 | stored length + 1 (0: nothing stored)} — to records_dev_out
+ * (device memory, n x 32 bytes) on the engine's stream.  The caller all-gathers those records (NCCL,
+ * on that stream) and hands the result to cmb200_import_records_dev, which imports the rows of the
+ * other ranks into the index replica, again without a host round trip.  n <= 262144.
+ * cmb200_import_records_dev reads n_total such records from device memory, skips the rows of my_rank
+ * and the rows that stored nothing, and is asynchronous on the engine's stream.  The arena offset
+ * lets cmb200_get_small read a record over NVLink once cmb200_open_peer has mapped its owner's arena. */
 int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     const void *pages, int pages_on_dev, const uint64_t *ts, uint32_t rank, void *records_dev_out,
     int32_t *lens_out, uint64_t *ticket);
@@ -196,7 +199,7 @@ int cmb200_copy_peer(cmb200_engine *dst_e, void *dst_dev, cmb200_engine *src_e, 
  * data_prefix + payload).  Gets read them over PCIe and answer CMB200_HIT as for any record; keys,
  * records, statuses and counters do not depend on the tier a record is in.
  * cmb200_host_tier_enable allocates `bytes` of it: once, before the first put, and never on an engine
- * that has made a multi-GPU call (cmb200_set_stream_order, cmb200_put_step, cmb200_import_*,
+ * that has made a multi-GPU call (cmb200_set_stream_order, cmb200_put_step, cmb200_import_records_dev,
  * cmb200_arena_ipc_handle, cmb200_open_peer); those calls in turn fail on an engine with a tier.
  * cmb200_demote_batch moves the arena records of the named keys to the tier (*demoted_out = how many);
  * keys that are absent, remote or already in the tier are skipped.  Their arena bytes become
@@ -236,11 +239,6 @@ int cmb200_host_tier_hot(cmb200_engine *e, size_t max, cmb200_addr *addr_out, si
  * others' records: per key the highest sequence wins, exactly as sequential puts would resolve
  * (SURVEY.md §8e "ordering caveat"); a local record that loses is retired. */
 int cmb200_set_stream_order(cmb200_engine *e, uint64_t next_seq, uint64_t stride);
-/* loc[i] (optional) = word 3 of the exchange record of row i: owner rank << 56 | arena offset / 16
- * << 22 | stored length + 1 — where the record lies in the owner's arena, so that cmb200_get_small
- * can read it over NVLink once cmb200_open_peer has mapped that arena. */
-int cmb200_import_remote(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint32_t *owner,
-    const uint64_t *seq, const uint64_t *loc, int arrays_on_device);
 /* The other ranks' arenas as NVLink peer memory.  Every rank exports the CUDA IPC handle of its
  * arena (64 bytes; exchange them with one all-gather), and opens the handles of the ranks it wants
  * to read from.  A cmb200_get_small of a key whose newest record lives on rank r then copies the

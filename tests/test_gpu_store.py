@@ -225,9 +225,10 @@ def test_eviction_keeps_capacity(E, gpu, tmp_path):
     cm.free()
 
 
-def test_remote_index_import(E, gpu, oracle):
+def test_remote_index_import_records(E, gpu, oracle):
     """Multi-GPU index replica on one GPU: records written "elsewhere" are imported; per key the
     highest stream position wins whatever the arrival order (SURVEY.md 8e ordering caveat)."""
+    from edge_fuse_b200 import sharding
     eng = E.Engine(pshift=12, accel=12, capacity=4096, arena_bytes=32 << 20, max_batch=64)
     n = 100
     pages = np.stack([datagen.make_page("T", 4096, i) for i in range(n)])
@@ -242,9 +243,18 @@ def test_remote_index_import(E, gpu, oracle):
     rseq = np.concatenate([1001 + 2 * np.arange(50) + 2 * 200, 3 + np.arange(10), [7]]).astype(np.uint64)
     # duplicates inside one import: key 0 appears twice, the larger sequence must win
     ru = np.append(ru, np.uint64(5)); rl = np.append(rl, np.uint64(0)); rseq = np.append(rseq, np.uint64(5000))
-    owner = np.full(len(ru), 1, dtype=np.uint32); owner[-1] = 3
+    # rows 0..60 come from rank 1, the last from rank 3; no location (offset 0, length 0): only peer
+    # reads, which this test does not make, would use one
+    lens = np.zeros(len(ru), dtype=np.int64)
+    rows = np.concatenate([sharding.pack_records(ru[:-1], rl[:-1], rseq[:-1], 1, lens[:-1]),
+                           sharding.pack_records(ru[-1:], rl[-1:], rseq[-1:], 3, lens[-1:])])
     perm = np.argsort(datagen.words(9, len(ru)))      # arrival order must not matter
-    eng.import_remote(ru[perm], rl[perm], owner[perm], rseq[perm])
+    rows = rows[perm]
+    d_rows = eng.dev_alloc(rows.nbytes)
+    eng.h2d(d_rows, rows)
+    eng.import_records_dev(len(rows), d_rows, 0)
+    eng.sync()
+    eng.dev_free(d_rows)
     status, own = eng.locate(u, l)
     assert (status[:50] == E.REMOTE).all() and (status[50:] == E.HIT).all()
     assert own[0] == 3 and (own[1:50] == 1).all()
@@ -588,9 +598,8 @@ def test_engine_snapshot_roundtrip_any_geometry(E, gpu, oracle, tmp_path):
 
 def test_put_step_records_and_device_import(E, gpu, oracle):
     """cmb200_put_step packs the exchange records of a step on the device exactly as sharding.py
-    packs them on the host, and cmb200_import_records_dev applies all-gathered records like
-    cmb200_import_remote: own rows and rows that stored nothing are skipped, the newest stream
-    position per key wins."""
+    packs them on the host, and cmb200_import_records_dev applies all-gathered records: own rows and
+    rows that stored nothing are skipped, the newest stream position per key wins."""
     from edge_fuse_b200 import sharding
     n, world, rank = 512, 4, 1
     eng = E.Engine(pshift=16, accel=12, capacity=8192, arena_bytes=128 << 20, max_batch=256, flags=E.FINGERPRINT)
@@ -647,6 +656,26 @@ def test_put_step_records_and_device_import(E, gpu, oracle):
         eng.dev_free(p)
     eng.close()
     E.lib().cmb200_host_free(hp)
+
+
+def test_import_gathered_host_and_device_tensors(E, gpu):
+    """sharding.import_gathered takes an all-gathered record tensor on the host or on the device,
+    imports the other ranks' rows that stored something before it returns, and returns their number."""
+    import torch
+    from edge_fuse_b200 import sharding
+    rows = np.concatenate([
+        sharding.pack_records([7, 7], [1, 2], [10, 11], 0, [100, 100]),          # this rank's own rows
+        sharding.pack_records([7, 7], [3, 4], [12, 13], 1, [100, -1]),           # key 4 stored nothing
+        sharding.pack_records([7], [5], [14], 2, [100], rec_off=[4096]),
+    ])
+    for gathered in (torch.from_numpy(rows), torch.from_numpy(rows).cuda()):
+        eng = E.Engine(pshift=12, accel=12, capacity=1024, arena_bytes=16 << 20, max_batch=64)
+        assert sharding.import_gathered(eng, gathered[:2], 0) == 0
+        assert sharding.import_gathered(eng, gathered, 0) == 2
+        status, owner = eng.locate(np.full(5, 7, dtype=np.uint64), np.arange(1, 6, dtype=np.uint64))
+        assert list(status) == [E.MISS, E.MISS, E.REMOTE, E.MISS, E.REMOTE], gathered.device
+        assert owner[2] == 1 and owner[4] == 2 and eng.stats()["remote_entries"] == 2
+        eng.close()
 
 
 def test_device_pages_must_be_16_byte_aligned(E, gpu, oracle):
