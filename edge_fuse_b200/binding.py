@@ -10,8 +10,9 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
-MISS, HIT, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE = 0, 1, 2, 3, 4, 5
+MISS, HIT, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, CORRUPT = 0, 1, 2, 3, 4, 5, 6
 FINGERPRINT = 1
+VERIFY = 2
 
 # every symbol the headers in include/ declare (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [
@@ -38,6 +39,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_host_tier_enable", "cmb200_demote_batch", "cmb200_host_tier_stats",
     "cmb200_promote_batch", "cmb200_host_tier_hot", "cmb200_read_checkpoints",
     "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
+    "cmb200_verify_stats", "cmb200_verify_store",
 ]
 
 
@@ -59,6 +61,10 @@ class HostTierStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in (
         "bytes", "used", "records", "garbage", "demoted_records", "demoted_bytes", "retired_records", "hits",
         "promoted_records", "promoted_bytes")]
+
+
+class VerifyStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("verified", "unverified", "corrupt", "scanned", "scan_corrupt")]
 
 
 def library_path() -> str:
@@ -159,6 +165,8 @@ def lib() -> C.CDLL:
         "cmb200_load_set": (i32, [vp, i32, C.c_char_p, vp]),
         "cmb200_move_pages": (i32, [vp, sz, vp, vp, vp, vp]),
         "cmb200_copy_peer": (i32, [vp, vp, vp, vp, sz]),
+        "cmb200_verify_stats": (i32, [vp, vp]),
+        "cmb200_verify_store": (i32, [vp, sz, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -295,6 +303,13 @@ def host_tier_stats(handle) -> dict:
     return {n: int(getattr(st, n)) for n, _ in HostTierStats._fields_}
 
 
+def verify_stats(handle) -> dict:
+    """cmb200_verify_stats of an engine handle (all zero for an engine created without VERIFY)."""
+    st = VerifyStats()
+    _check(lib().cmb200_verify_stats(handle, C.byref(st)), "cmb200_verify_stats")
+    return {n: int(getattr(st, n)) for n, _ in VerifyStats._fields_}
+
+
 def read_checkpoints(handle, u, l):
     """cmb200_read_checkpoints of an engine handle -> (words [n, 16] uint32, ok [n] int32): word 0 is
     the tag as stored; ok 1 = valid checkpoints, 0 = a record without them, -1 = absent, remote or
@@ -354,6 +369,20 @@ class Engine:
 
     def host_tier_stats(self) -> dict:
         return host_tier_stats(self.h)
+
+    def verify_stats(self) -> dict:
+        return verify_stats(self.h)
+
+    def verify_store(self, max_bad: int = 4096):
+        """cmb200_verify_store -> (u, l, n_bad, checked): the addresses of the first max_bad records
+        whose page does not match its stored EF128 or does not decode, how many such records there
+        are, and how many records had a fingerprint to compare with."""
+        addr = np.zeros((max(1, max_bad), 2), dtype=np.uint64)
+        n, checked = C.c_size_t(0), C.c_uint64(0)
+        _check(lib().cmb200_verify_store(self.h, max_bad, _ptr(addr), C.byref(n), C.byref(checked)),
+               "cmb200_verify_store")
+        k = min(n.value, max_bad)
+        return addr[:k, 0].copy(), addr[:k, 1].copy(), int(n.value), int(checked.value)
 
     def close(self):
         if self.h:

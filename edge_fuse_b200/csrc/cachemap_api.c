@@ -281,6 +281,8 @@ fm_dev_start(struct filemap *m, int index, int device, int g)
 	cfg.table_slots = (uint64_t)env_long("CMB200_TABLE_SLOTS", 0);
 	cfg.max_batch = (uint32_t)env_long("CMB200_MAX_BATCH", 0);
 	cfg.flags = env_long("CMB200_FINGERPRINT", 0) ? CMB200_FINGERPRINT : 0;
+	/* every get compared with its page's EF128 on the GPU; a page that differs is a miss */
+	if (env_long("CMB200_VERIFY", 0)) cfg.flags |= CMB200_VERIFY;
 	d->eng = cmb200_engine_create(&cfg);
 	const long tier_mb = env_long("CMB200_HOST_TIER_MB", 0);
 	if (d->eng && tier_mb > 0) {

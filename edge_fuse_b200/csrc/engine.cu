@@ -154,6 +154,10 @@ struct cmb200_engine {
 		HotLog hot() const { return HotLog{d_ctr ? d_ctr + 2 : nullptr, d_hot}; }
 	} tier;
 	std::atomic<bool> multi_gpu{false};  // a multi-GPU call was made: no host tier from then on
+	// CMB200_VERIFY: device counters, VS_WORDS of the gets, then VS_WORDS of the running store scan
+	unsigned long long *d_vstat = nullptr;
+	uint32_t *d_vidx = nullptr;          // slot of each request of a verified get batch (max_batch)
+	uint64_t scanned = 0, scan_corrupt = 0;
 };
 
 #define ENG_CHECK(expr)                                                 \
@@ -193,7 +197,8 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	cudaSetDevice(e->device);
 	if (e->st) cudaStreamSynchronize(e->st);
 	if (e->copy) cudaStreamSynchronize(e->copy);
-	cudaFree(e->d_scratch); cudaFree(e->d_pool_bits); cudaFree(e->table.ckpt);
+	cudaFree(e->d_scratch); cudaFree(e->d_pool_bits); cudaFree(e->table.ckpt); cudaFree(e->table.fp_tag);
+	cudaFree(e->d_vstat); cudaFree(e->d_vidx);
 	cudaFree(e->table.slots); cudaFree(e->table.fp); cudaFree(e->arena.base); cudaFree(e->arena.seg); cudaFree(e->d_counters);
 	cudaFree(e->d_pages[0]); cudaFree(e->d_pages[1]); cudaFree(e->d_stage);
 	cudaFree(e->d_addr); cudaFree(e->d_ts); cudaFree(e->d_valid); cudaFree(e->d_slot); cudaFree(e->d_vlen);
@@ -243,6 +248,7 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 	// copy of a call cannot overlap anything, while a launch wants many chunks per warp
 	e->host_batch = e->max_batch < 4096u ? e->max_batch : 4096u;
 	e->flags = cfg->flags;
+	if (e->flags & CMB200_VERIFY) e->flags |= CMB200_FINGERPRINT;
 	const uint64_t B = e->max_batch;
 	{
 		uint64_t slots = cfg->table_slots ? next_pow2(cfg->table_slots) : next_pow2(4 * (cfg->capacity ? cfg->capacity : 1024));
@@ -273,6 +279,13 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 			ENG_CHECK(cudaMalloc(&e->table.fp, (slots + 2) * 16));
 			ENG_CHECK(cudaMemsetAsync(e->table.fp, 0, (slots + 2) * 16, e->st));
 		}
+		if (e->flags & CMB200_VERIFY) {
+			ENG_CHECK(cudaMalloc(&e->table.fp_tag, (slots + 2) * 4));
+			ENG_CHECK(cudaMemsetAsync(e->table.fp_tag, 0, (slots + 2) * 4, e->st));
+			ENG_CHECK(cudaMalloc(&e->d_vstat, 2 * VS_WORDS * sizeof(unsigned long long)));
+			ENG_CHECK(cudaMemsetAsync(e->d_vstat, 0, 2 * VS_WORDS * sizeof(unsigned long long), e->st));
+			ENG_CHECK(cudaMalloc(&e->d_vidx, B * 4));
+		}
 		if (get_small_supports(e->bsize)) {
 			// parse checkpoints per slot (64 bytes) and the descriptor scratch of the fused single-page get
 			const char *ck = getenv("CMB200_CKPT");
@@ -280,7 +293,7 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 				ENG_CHECK(cudaMalloc(&e->table.ckpt, (slots + 2) * CKPT_WORDS * 4));
 				ENG_CHECK(cudaMemsetAsync(e->table.ckpt, 0, (slots + 2) * CKPT_WORDS * 4, e->st));
 			}
-			const int resident = get_small_residency(e->bsize);
+			const int resident = get_small_residency(e->bsize, e->table.fp_tag != nullptr);
 			if (resident <= 0) { set_error_msg("k_get_small does not fit this device"); goto fail; }
 			e->pool_n = (uint32_t)resident;
 			e->region_entries = get_small_region_entries(e->bsize);
@@ -666,14 +679,15 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		uint8_t *d_out = out_on_dev ? pages_out + at * e->bsize : e->d_pages[buf];
 		if (!out_on_dev) CMB_CHECK(cudaStreamWaitEvent(e->st, e->consumed[buf], 0));   // D2H of buf finished
 		if (launch_lookup(e->table, e->d_addr + 2 * at, valid ? e->d_valid + at : nullptr, m, e->d_status + at, e->d_recoff,
-			e->d_vlen, nullptr, e->st)) return -1;
+			e->d_vlen, nullptr, e->st, e->d_vidx)) return -1;
 		DecodeJob job{};
 		job.n = m; job.nbytes = e->bsize; job.pages = d_out; job.status = e->d_status + at;
 		job.rec_off = e->d_recoff; job.vlen = e->d_vlen; job.arena = e->arena.base;
 		job.host = e->tier.dev; job.host_hits = e->tier.d_ctr + 1;
 		job.hot = e->tier.hot(); job.addr = e->d_addr + 2 * at;
+		const DecodeVerify ver{e->d_vidx, e->table.fp, e->table.fp_tag, e->d_vstat};
 		CMB_CHECK(cudaEventRecord(e->t0[nb % e->RING], e->st));
-		if (launch_decode(job, e->st)) return -1;
+		if (launch_decode(job, e->st, e->table.fp_tag ? &ver : nullptr)) return -1;
 		CMB_CHECK(cudaEventRecord(e->t1[nb % e->RING], e->st));
 		if (!out_on_dev) {
 			CMB_CHECK(cudaEventRecord(e->landed[buf], e->st));
@@ -803,6 +817,7 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	for (int r = 0; r < GET_MAX_PEERS; r++) { job.peer[r] = e->peer_base[r]; job.peer_size[r] = e->peer_size[r]; }
 	job.scratch = e->d_scratch; job.region_entries = e->region_entries; job.pool_bits = e->d_pool_bits; job.pool_n = e->pool_n;
 	job.hot = e->tier.hot();
+	job.vstat = e->d_vstat;
 	if (launch_get_small(job, e->device, ln->st)) { ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1; }
 	t->lane = li; t->n = (uint32_t)n; t->status = ln->h_status;
 	return 0;
@@ -1371,11 +1386,13 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 	// linear probing never frees one by itself.
 	if (c[1] > e->table.cap / 8) {
 		TableView fresh = e->table;
-		fresh.slots = nullptr; fresh.fp = nullptr; fresh.ckpt = nullptr;
+		fresh.slots = nullptr; fresh.fp = nullptr; fresh.ckpt = nullptr; fresh.fp_tag = nullptr;
 		if (cudaMalloc(&fresh.slots, (e->table.cap + 2) * sizeof(Slot)) == cudaSuccess &&
-		    (!e->table.fp || cudaMalloc(&fresh.fp, (e->table.cap + 2) * 16) == cudaSuccess)) {
+		    (!e->table.fp || cudaMalloc(&fresh.fp, (e->table.cap + 2) * 16) == cudaSuccess) &&
+		    (!e->table.fp_tag || cudaMalloc(&fresh.fp_tag, (e->table.cap + 2) * 4) == cudaSuccess)) {
 			CMB_CHECK(cudaMemsetAsync(fresh.slots, 0, (e->table.cap + 2) * sizeof(Slot), e->st));
 			if (fresh.fp) CMB_CHECK(cudaMemsetAsync(fresh.fp, 0, (e->table.cap + 2) * 16, e->st));
+			if (fresh.fp_tag) CMB_CHECK(cudaMemsetAsync(fresh.fp_tag, 0, (e->table.cap + 2) * 4, e->st));
 			// parse checkpoints move with their slots (k_rehash); without room for a second side table
 			// they are dropped instead, and those records are walked by one warp until rewritten
 			const size_t ck_bytes = (e->table.cap + 2) * CKPT_WORDS * 4;
@@ -1388,13 +1405,13 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 			if (e->table.ckpt && !fresh.ckpt) CMB_CHECK(cudaMemsetAsync(e->table.ckpt, 0, ck_bytes, e->st));
 			CMB_CHECK(cudaMemsetAsync(e->d_counters + 1, 0, sizeof(unsigned long long), e->st));   // tombstones
 			CMB_CHECK(cudaStreamSynchronize(e->st));
-			cudaFree(e->table.slots); cudaFree(e->table.fp);
-			e->table.slots = fresh.slots; e->table.fp = fresh.fp;
+			cudaFree(e->table.slots); cudaFree(e->table.fp); cudaFree(e->table.fp_tag);
+			e->table.slots = fresh.slots; e->table.fp = fresh.fp; e->table.fp_tag = fresh.fp_tag;
 			if (fresh.ckpt) { cudaFree(e->table.ckpt); e->table.ckpt = fresh.ckpt; }
 			e->stats.kernel_launches++;
 		} else {
 			(void)cudaGetLastError();                    // no room for a second table: keep the old one
-			cudaFree(fresh.slots);
+			cudaFree(fresh.slots); cudaFree(fresh.fp); cudaFree(fresh.fp_tag);
 		}
 	}
 	return 0;
@@ -1403,6 +1420,75 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 extern "C" int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out) {
 	std::lock_guard<std::mutex> g(e->mu);
 	return compact_locked(e, reclaimed_out);
+}
+
+// ---- verified reads (CMB200_VERIFY) ------------------------------------------------------------
+
+extern "C" int cmb200_verify_stats(cmb200_engine *e, struct cmb200_verify_stats *out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	memset(out, 0, sizeof(*out));
+	if (!e->d_vstat) return 0;
+	unsigned long long v[VS_WORDS];
+	CMB_CHECK(cudaSetDevice(e->device));
+	CMB_CHECK(cudaMemcpyAsync(v, e->d_vstat, sizeof(v), cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	out->verified = v[VS_VERIFIED]; out->unverified = v[VS_UNVERIFIED]; out->corrupt = v[VS_CORRUPT];
+	out->scanned = e->scanned; out->scan_corrupt = e->scan_corrupt;
+	return 0;
+}
+
+// Every live local record, both tiers, decoded batch by batch into the first page-ring buffer by the
+// verified k_decode (host_hits null: a scan books no tier hit), whose counters go to the second half of
+// d_vstat.  The records do not move while the engine lock is held, and small gets only read them.
+extern "C" int cmb200_verify_store(cmb200_engine *e, size_t max, cmb200_addr *bad_out, size_t *n_bad,
+    uint64_t *checked) {
+	std::lock_guard<std::mutex> g(e->mu);
+	if (n_bad) *n_bad = 0;
+	if (checked) *checked = 0;
+	if (!e->table.fp_tag) { set_error_msg("cmb200_verify_store: engine created without CMB200_VERIFY"); return -1; }
+	CMB_CHECK(cudaSetDevice(e->device));
+	harvest_pending(e, true);
+	unsigned long long c[8];
+	std::vector<ExportEntry> list;
+	const int listed = live_records(e, false, list, c);
+	if (listed < 0) return -1;
+	if (listed > 0) { set_error_msg("cmb200_verify_store: the store changed under the scan"); return -1; }
+	unsigned long long *scan = e->d_vstat + VS_WORDS;
+	CMB_CHECK(cudaMemsetAsync(scan, 0, VS_WORDS * sizeof(unsigned long long), e->st));
+	const size_t B = e->host_batch;
+	DevBuf d_list;
+	if (!list.empty() && d_list.alloc(B * sizeof(ExportEntry))) return -1;
+	std::vector<int32_t> st(B);
+	std::vector<cmb200_addr> addr(B);
+	size_t bad = 0;
+	for (size_t at = 0; at < list.size(); at += B) {
+		const uint32_t m = (uint32_t)(list.size() - at < B ? list.size() - at : B);
+		CMB_CHECK(cudaMemcpyAsync(d_list.p, list.data() + at, m * sizeof(ExportEntry), cudaMemcpyHostToDevice, e->st));
+		if (launch_scan_prep(e->table, d_list.as<ExportEntry>(), m, e->d_status, e->d_recoff, e->d_vlen, e->d_vidx,
+			e->d_addr, e->st)) return -1;
+		DecodeJob job{};
+		job.n = m; job.nbytes = e->bsize; job.pages = e->d_pages[0]; job.status = e->d_status;
+		job.rec_off = e->d_recoff; job.vlen = e->d_vlen; job.arena = e->arena.base; job.host = e->tier.dev;
+		const DecodeVerify ver{e->d_vidx, e->table.fp, e->table.fp_tag, scan};
+		if (launch_decode(job, e->st, &ver)) return -1;
+		e->stats.kernel_launches += 2;
+		CMB_CHECK(cudaMemcpyAsync(st.data(), e->d_status, m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemcpyAsync(addr.data(), e->d_addr, m * 16, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		for (uint32_t i = 0; i < m; i++) {
+			if (st[i] != CMB200_CORRUPT && st[i] != CMB200_BAD_DECODE) continue;
+			if (bad < max && bad_out) bad_out[bad] = addr[i];
+			bad++;
+		}
+	}
+	unsigned long long v[VS_WORDS];
+	CMB_CHECK(cudaMemcpyAsync(v, scan, sizeof(v), cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	e->scanned += list.size();
+	e->scan_corrupt += bad;
+	if (n_bad) *n_bad = bad;
+	if (checked) *checked = v[VS_VERIFIED] + v[VS_CORRUPT];
+	return 0;
 }
 
 // ---- host tier ---------------------------------------------------------------------------------

@@ -51,6 +51,9 @@ __device__ __forceinline__ void ef_scramble(EfLane &L) {
 }
 
 // Whole-warp call.  `src` 16-byte aligned; bytes at or beyond n read as zero.  Result on all lanes.
+// COHERENT: the page was written by the calling kernel, so it is read through the L2
+// (ld.global.cg) and never through the read-only path, which may hold stale lines.
+template <bool COHERENT = false>
 __device__ __forceinline__ void warp_fingerprint128(const uint8_t *src, uint32_t n, int lane,
     uint64_t &hi, uint64_t &lo) {
 	EfLane L;
@@ -63,7 +66,7 @@ __device__ __forceinline__ void warp_fingerprint128(const uint8_t *src, uint32_t
 	for (; s + 16 <= full; s += 16) {
 		uint4 x[16];
 #pragma unroll
-		for (int k = 0; k < 16; k++) x[k] = __ldg(v + (size_t)(s + k) * 32);
+		for (int k = 0; k < 16; k++) x[k] = COHERENT ? __ldcg(v + (size_t)(s + k) * 32) : __ldg(v + (size_t)(s + k) * 32);
 #pragma unroll
 		for (int k = 0; k < 16; k++)
 			ef_absorb(L, (uint64_t)x[k].x | ((uint64_t)x[k].y << 32),
@@ -74,17 +77,70 @@ __device__ __forceinline__ void warp_fingerprint128(const uint8_t *src, uint32_t
 		uint32_t off = s * 512 + lane * 16;
 		uint64_t x0 = 0, x1 = 0;
 		if (off + 16 <= n) {
-			uint4 x = __ldg(v + (size_t)s * 32);
+			uint4 x = COHERENT ? __ldcg(v + (size_t)s * 32) : __ldg(v + (size_t)s * 32);
 			x0 = (uint64_t)x.x | ((uint64_t)x.y << 32);
 			x1 = (uint64_t)x.z | ((uint64_t)x.w << 32);
 		} else {
 			for (uint32_t k = 0; k < 16 && off + k < n; k++) {
-				uint64_t byte = ldg8(src + off + k);
+				uint64_t byte = COHERENT ? (uint64_t)__ldcg(src + off + k) : ldg8(src + off + k);
 				if (k < 8) x0 |= byte << (8 * k); else x1 |= byte << (8 * (k - 8));
 			}
 		}
 		ef_absorb(L, x0, x1);
 		if ((s & 15u) == 15u) ef_scramble(L);
+	}
+	uint64_t u = ef_fold(L.a ^ L.s0, L.b ^ L.s1);
+	uint64_t w = ef_fold(L.a ^ L.s3, L.b ^ L.s2);
+	u = warp_sum_u64(u);
+	w = warp_sum_u64(w);
+	lo = ef_av((uint64_t)n * 0x9E3779B185EBCA87ULL + u);
+	hi = ef_av(~((uint64_t)n * 0xC2B2AE3D27D4EB4FULL) + w);
+}
+
+// EF128 split by 16-stripe groups, for a page that a whole CTA holds (k_get_small's shared memory).
+// Inside a group the absorb step only adds to a and b (mod 2^64), and what it adds depends on the
+// input and the lane's secrets alone, so with A_g = lane l's sum over group g,
+//   a after group g = scramble(a before + A_g),
+// and the groups' sums can be taken by different warps at once.  One warp then chains them: a group
+// that reaches its 16th stripe is followed by a scramble, a trailing shorter group is added without one.
+// Same result as warp_fingerprint128 for every n.
+constexpr uint32_t EF_GROUP_BYTES = 16u * 512u;
+__host__ __device__ __forceinline__ uint32_t ef_groups(uint32_t n) { return (n + EF_GROUP_BYTES - 1u) / EF_GROUP_BYTES; }
+
+// Lane sums {A, B} of group g of the n bytes at `src` (8-byte aligned, any state space the generic
+// address reaches; bytes at or beyond n read as zero).
+__device__ __forceinline__ ulonglong2 ef_group_sum(const uint8_t *src, uint32_t n, uint32_t g, int lane) {
+	EfLane G;
+	G.s0 = ef_secret(4 * lane); G.s1 = ef_secret(4 * lane + 1);
+	G.a = 0; G.b = 0;
+	const uint32_t stripes = (n + 511u) >> 9, end = min(stripes, 16u * g + 16u);
+	for (uint32_t s = 16u * g; s < end; s++) {
+		const uint32_t off = s * 512u + (uint32_t)lane * 16u;
+		uint64_t x0 = 0, x1 = 0;
+		if (off + 16u <= n) {
+			x0 = *reinterpret_cast<const uint64_t *>(src + off);
+			x1 = *reinterpret_cast<const uint64_t *>(src + off + 8u);
+		} else {
+			for (uint32_t k = 0; k < 16u && off + k < n; k++) {
+				const uint64_t byte = src[off + k];
+				if (k < 8) x0 |= byte << (8 * k); else x1 |= byte << (8 * (k - 8));
+			}
+		}
+		ef_absorb(G, x0, x1);
+	}
+	return make_ulonglong2(G.a, G.b);
+}
+
+// Whole-warp call: chains the lane sums sums[32 g + lane] of every group of an n-byte page and folds
+// them.  Result on all lanes.
+__device__ __forceinline__ void ef_group_finish(const ulonglong2 *sums, uint32_t n, int lane, uint64_t &hi, uint64_t &lo) {
+	EfLane L;
+	ef_init(L, lane);
+	const uint32_t groups = ef_groups(n), full = ((n + 511u) >> 9) >> 4;   // groups that reach their 16th stripe
+	for (uint32_t g = 0; g < groups; g++) {
+		const ulonglong2 s = sums[32u * g + (uint32_t)lane];
+		L.a += s.x; L.b += s.y;
+		if (g < full) ef_scramble(L);
 	}
 	uint64_t u = ef_fold(L.a ^ L.s0, L.b ^ L.s1);
 	uint64_t w = ef_fold(L.a ^ L.s3, L.b ^ L.s2);

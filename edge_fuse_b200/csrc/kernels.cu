@@ -128,18 +128,19 @@ __global__ void k_upsert(TableView t, const unsigned long long *addr, const uint
 }
 
 __global__ void k_lookup(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
-    int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out) {
+    int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out, uint32_t *idx_out) {
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
 	int32_t st = ST_MISS;
 	uint64_t off = 0;
 	uint32_t vl = 0;
 	unsigned long long ts = 0;
+	uint32_t idx = 0xffffffffu;
 	if (valid && !valid[i]) {
 		st = ST_INVALID;
 	} else {
 		unsigned long long u = addr[2 * i], l = addr[2 * i + 1];
-		uint32_t idx = table_find(t, fnv_addr(u, l));
+		idx = table_find(t, fnv_addr(u, l));
 		if (idx != 0xffffffffu) {
 			const Slot &s = t.slots[idx];
 			if (s.vlen != 0) {
@@ -157,6 +158,7 @@ __global__ void k_lookup(TableView t, const unsigned long long *addr, const uint
 	if (rec_off) rec_off[i] = off;
 	if (vlen) vlen[i] = vl;
 	if (ts_out) ts_out[i] = ts;
+	if (idx_out) idx_out[i] = idx;
 }
 
 // The bytes a slot's record held (s.alloc) become garbage of the tier they are in.
@@ -191,6 +193,7 @@ __global__ void k_unset(TableView t, ArenaView a, const unsigned long long *addr
 	slot_release(a, s);
 	s.alloc = 0;
 	s.owner = 0;
+	if (t.fp_tag) t.fp_tag[idx] = 0u;
 	if (idx < t.cap) {
 		s.key = KEY_TOMB;
 		atomicAdd(t.tombs, 1ull);
@@ -269,10 +272,16 @@ __global__ void __launch_bounds__(256) k_sample_scan(TableView t, const unsigned
 // The tier bytes stay intact until the ring laps them, and that lap closes get_gate (demote_group).
 // The arena bytes lie above the bump pointer as it was before the promotion, where no slot pointed, so
 // no reader can reach them before the rec_off store, which k_promote makes after a fence.
+// With CMB200_VERIFY the fingerprint is guarded like the checkpoints (ckpt_store): its tag is zeroed
+// before fp changes and names the new record only once rec_off and vlen are out, so a get on another
+// stream that staged the old record never compares it with the new fingerprint.  has_fp = false (a
+// snapshot written without fingerprints) leaves the tag zero: the record is served unverified.
 __device__ __forceinline__ void slot_publish(const EncodeJob &job, Slot &s, uint32_t i, uint32_t idx, unsigned long long off,
-    uint32_t need, uint32_t clen, unsigned long long au, unsigned long long al, uint64_t fp_hi, uint64_t fp_lo) {
+    uint32_t need, uint32_t clen, unsigned long long au, unsigned long long al, uint64_t fp_hi, uint64_t fp_lo,
+    bool has_fp = true) {
 	// whatever checkpoints the slot has describe the record it is leaving (ckpt_store renews them)
 	if (job.table.ckpt) *reinterpret_cast<volatile uint32_t *>(&job.table.ckpt[(size_t)idx * CKPT_WORDS]) = 0u;
+	if (job.table.fp_tag) { *reinterpret_cast<volatile uint32_t *>(&job.table.fp_tag[idx]) = 0u; __threadfence(); }
 	if (s.owner) { atomicAdd(job.table.remote, (unsigned long long)-1ll); s.owner = 0; }   // now newest here (alloc held the remote length)
 	else if (s.alloc) slot_release(job.arena, s);                                          // the record this one replaces
 	s.addr_u = au; s.addr_l = al;
@@ -284,6 +293,7 @@ __device__ __forceinline__ void slot_publish(const EncodeJob &job, Slot &s, uint
 	if (s.vlen == 0) atomicAdd(job.table.entries, 1ull);
 	*reinterpret_cast<volatile uint32_t *>(&s.vlen) = clen + 1u;
 	if (job.rec_out) job.rec_out[i] = off;
+	if (job.table.fp_tag && has_fp) { __threadfence(); *reinterpret_cast<volatile uint32_t *>(&job.table.fp_tag[idx]) = ckpt_tag(off, clen); }
 }
 
 // Parse checkpoints of the record just published in slot idx (whole warp; lane k holds word k, see
@@ -301,23 +311,24 @@ __device__ __forceinline__ void ckpt_store(const EncodeJob &job, uint32_t idx, u
 }
 
 // The record of slot idx moved from old_loc to new_loc with its block unchanged (compaction, demotion,
-// promotion), so its checkpoints still hold and only the tag moves.  A tag that names another record
-// version (or none) is left alone.  The fence orders the caller's rec_off store before the new tag,
-// so a reader that sees the tag also sees the location it names.  (one thread)
+// promotion), so its checkpoints and its fingerprint still hold and only their tags move.  A tag that
+// names another record version (or none) is left alone.  The fence orders the caller's rec_off store
+// before the new tag, so a reader that sees the tag also sees the location it names.  (one thread)
 __device__ __forceinline__ void ckpt_retag(const TableView &t, uint32_t idx, unsigned long long old_loc,
     unsigned long long new_loc, uint32_t clen) {
-	if (!t.ckpt) return;
-	uint32_t *w = t.ckpt + (size_t)idx * CKPT_WORDS;
-	if (*reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(old_loc, clen)) {
-		__threadfence();
-		*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(new_loc, clen);
+	uint32_t *tags[2] = {t.ckpt ? t.ckpt + (size_t)idx * CKPT_WORDS : nullptr, t.fp_tag ? t.fp_tag + idx : nullptr};
+	for (uint32_t *w : tags) {
+		if (w && *reinterpret_cast<volatile uint32_t *>(w) == ckpt_tag(old_loc, clen)) {
+			__threadfence();
+			*reinterpret_cast<volatile uint32_t *>(w) = ckpt_tag(new_loc, clen);
+		}
 	}
 }
 
 // Stores the finished block as a filemap record {data_prefix, block} (filemap.c:140-147) and
 // publishes it in the key table.  Called by the whole warp; lane 0 owns the bookkeeping.
 __device__ unsigned long long commit_record(const EncodeJob &job, uint32_t i, uint32_t idx, const uint8_t *payload,
-    uint32_t plen, int32_t clen, bool payload_ro, uint64_t fp_hi, uint64_t fp_lo, int lane) {
+    uint32_t plen, int32_t clen, bool payload_ro, uint64_t fp_hi, uint64_t fp_lo, int lane, bool has_fp = true) {
 	Slot &s = job.table.slots[idx];
 	const uint32_t need = (24u + plen + 15u) & ~15u;
 	unsigned long long off = 0;
@@ -360,7 +371,7 @@ __device__ unsigned long long commit_record(const EncodeJob &job, uint32_t i, ui
 	else warp_copy_rw(rec + 24, payload, plen, lane);
 	__threadfence();                                 // the record is complete before the slot points to it
 	__syncwarp();
-	if (lane == 0) slot_publish(job, s, i, idx, off, need, (uint32_t)clen, au, al, fp_hi, fp_lo);
+	if (lane == 0) slot_publish(job, s, i, idx, off, need, (uint32_t)clen, au, al, fp_hi, fp_lo, has_fp);
 	return off;                                      // arena offset of the record (~0: dropped)
 }
 
@@ -672,7 +683,14 @@ extern "C" int cmb200_enc_phases(void *buf, uint32_t *nphases) {   // n x 2 x EN
 // decode
 // ------------------------------------------------------------------------------------------
 
-__global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) {
+// VERIFY (CMB200_VERIFY): the warp fingerprints the page it has just written and compares it with the
+// record's EF128 when the slot's tag names this record version (the engine stream orders this kernel
+// after every put, so no writer races it); a mismatch is ST_CORRUPT.  host_hits null: a scan of the
+// store (cmb200_verify_store), which is not a get and books no tier hit.
+// The verify state is a parameter of k_decode_verify alone, so that k_decode's parameter block (and with
+// it its register allocation) stays what it is without the flag.
+template <bool VERIFY>
+__device__ __forceinline__ void decode_request(const DecodeJob &job, const DecodeVerify &v) {
 	const int lane = threadIdx.x & 31;
 	const uint32_t i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
 	if (i >= job.n) return;
@@ -682,17 +700,39 @@ __global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) {
 		const unsigned long long off = job.rec_off[i];
 		// host tier: mapped host memory, read over PCIe
 		const uint8_t *rec = (off & REC_HOST) ? job.host + (off & ~REC_HOST) : job.arena + off;
-		if ((off & REC_HOST) && lane == 0) {
+		if ((off & REC_HOST) && lane == 0 && (!VERIFY || job.host_hits)) {
 			atomicAdd(job.host_hits, 1ull);
 			hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
 		}
 		uint32_t clen = job.vlen[i] - 1u;
-		if (clen == 0) {                            // raw page (filemap.c:249-251)
-			warp_copy_ro(out, rec + 24, job.nbytes, lane);
-			return;
+		if constexpr (!VERIFY) {
+			if (clen == 0) {                            // raw page (filemap.c:249-251)
+				warp_copy_ro(out, rec + 24, job.nbytes, lane);
+				return;
+			}
+			int used = lz4_decode_warp(rec + 24, clen, out, job.nbytes, lane);
+			if (used != (int)clen && lane == 0) job.status[i] = ST_BAD_DECODE;   // filemap.c:244-248
+		} else {
+			if (clen == 0) {
+				warp_copy_ro(out, rec + 24, job.nbytes, lane);
+			} else if (lz4_decode_warp(rec + 24, clen, out, job.nbytes, lane) != (int)clen) {
+				if (lane == 0) job.status[i] = ST_BAD_DECODE;
+				return;
+			}
+			const uint32_t idx = v.idx[i];
+			if (v.fp_tag[idx] != ckpt_tag(off, clen)) {
+				if (lane == 0) atomicAdd(&v.vstat[VS_UNVERIFIED], 1ull);
+				return;
+			}
+			__syncwarp();                           // every lane's stores of the page are visible to the warp
+			uint64_t hi, lo;
+			warp_fingerprint128<true>(out, job.nbytes, lane, hi, lo);
+			const bool match = hi == v.fp[2 * (size_t)idx] && lo == v.fp[2 * (size_t)idx + 1];
+			if (lane == 0) {
+				atomicAdd(&v.vstat[match ? VS_VERIFIED : VS_CORRUPT], 1ull);
+				if (!match) job.status[i] = ST_CORRUPT;
+			}
 		}
-		int used = lz4_decode_warp(rec + 24, clen, out, job.nbytes, lane);
-		if (used != (int)clen && lane == 0) job.status[i] = ST_BAD_DECODE;   // filemap.c:244-248
 	} else {
 		int used = lz4_decode_warp(job.blocks + (size_t)i * job.block_stride, (uint32_t)job.lens[i], out,
 		    job.nbytes, lane);
@@ -700,10 +740,16 @@ __global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) {
 	}
 }
 
-int launch_decode(const DecodeJob &job, cudaStream_t st) {
+__global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) { decode_request<false>(job, DecodeVerify{}); }
+// 4 CTAs per SM rather than 8: the fingerprint's 16 loads in flight per lane need the registers that 8
+// would leave to spills.
+__global__ void __launch_bounds__(256, 4) k_decode_verify(DecodeJob job, DecodeVerify v) { decode_request<true>(job, v); }
+
+int launch_decode(const DecodeJob &job, cudaStream_t st, const DecodeVerify *verify) {
 	if (job.n == 0) return 0;
 	const int warps = 8;
-	k_decode<<<(job.n + warps - 1) / warps, warps * 32, 0, st>>>(job);
+	if (job.rec_off && verify) k_decode_verify<<<(job.n + warps - 1) / warps, warps * 32, 0, st>>>(job, *verify);
+	else k_decode<<<(job.n + warps - 1) / warps, warps * 32, 0, st>>>(job);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
@@ -727,12 +773,20 @@ struct GetShared {
 	uint32_t region;                          // scratch region this CTA holds (~0: none)
 	uint32_t sections;                        // 1 = one warp walks the block, 16 = the record's checkpoints are used
 	uint32_t ck[CKPT_WORDS];
+	unsigned long long fp[2];                 // VERIFY: the record's stored EF128 {hi, lo} ...
+	uint32_t fp_ok;                           // ... 1 = taken under a tag naming the staged record
+	uint32_t match;                           // gs_page_matches' answer
 };
 static_assert(sizeof(GetShared) <= 128, "control block");
 __host__ __device__ inline uint32_t gs_recbuf(uint32_t nbytes) { return (24u + nbytes + 1024u + 31u) & ~15u; }
 bool get_small_supports(uint32_t nbytes) { return nbytes >= 64u && nbytes <= GS_PAIR_MAX_PAGE && (nbytes & 15u) == 0; }
-size_t get_small_smem(uint32_t nbytes) {                      // per CTA
+// Shared memory per CTA: control block, record buffer, page buffer (one CTA per request); with VERIFY
+// the EF128 lane sums of the page's 16-stripe groups follow (gs_page_matches).
+__host__ __device__ inline uint32_t gs_sums_at(uint32_t nbytes) {
 	return nbytes > GS_MAX_PAGE ? GS_CTRL + gs_recbuf(nbytes) : GS_CTRL + gs_recbuf(nbytes) + nbytes;
+}
+size_t get_small_smem(uint32_t nbytes, bool verify) {
+	return gs_sums_at(nbytes) + (verify ? ef_groups(nbytes) * 32u * sizeof(ulonglong2) : 0u);
 }
 uint32_t get_small_region_entries(uint32_t nbytes) { return dc_region(nbytes); }
 
@@ -823,6 +877,40 @@ __device__ void gs_sections(const GetJob &job, GetShared *sh, DecodeCta *dc, uin
 	sh->sections = use ? DC_CHAINS : 1u;
 }
 
+// CMB200_VERIFY: the stored EF128 of the record this CTA staged (slot sh->idx, location off, length
+// clen), taken between two equal reads of the slot's fingerprint tag, and only when the tag names that
+// location and length.  Otherwise sh->fp_ok = 0 and the page is served unverified: a put of the key on
+// another stream may have replaced the fingerprint after the record was staged.  (one thread)
+__device__ void gs_fp_take(const GetJob &job, GetShared *sh, unsigned long long off, uint32_t clen, bool local) {
+	sh->fp_ok = 0u;
+	if (!local) return;                                      // a peer's record: no fingerprint travels with it
+	const uint32_t *tag = job.table.fp_tag + sh->idx;
+	const uint32_t want = ckpt_tag(off, clen);
+	if (ldv32(tag) != want) return;
+	__threadfence();
+	const unsigned long long *fp = reinterpret_cast<const unsigned long long *>(job.table.fp) + 2 * (size_t)sh->idx;
+	sh->fp[0] = ldv64(fp);
+	sh->fp[1] = ldv64(fp + 1);
+	__threadfence();
+	sh->fp_ok = ldv32(tag) == want ? 1u : 0u;
+}
+
+// Whole CTA: does the n-byte page at `src` (shared memory, 8-byte aligned) have the EF128 {hi, lo}?
+// The 16 warps take the lane sums of the page's 16-stripe groups (fingerprint.cuh: ef_group_sum) into
+// `sums`, warp 0 chains and folds them.  The answer passes through *flag and the barrier.
+__device__ bool gs_page_matches(const uint8_t *src, uint32_t n, ulonglong2 *sums, unsigned long long hi,
+    unsigned long long lo, uint32_t *flag, uint32_t warp, int lane) {
+	for (uint32_t g = warp; g < ef_groups(n); g += GS_THREADS / 32u) sums[32u * g + (uint32_t)lane] = ef_group_sum(src, n, g, lane);
+	__syncthreads();
+	if (warp == 0) {
+		uint64_t h, l;
+		ef_group_finish(sums, n, lane, h, l);
+		if (lane == 0) *flag = h == hi && l == lo ? 1u : 0u;
+	}
+	__syncthreads();
+	return *flag != 0u;
+}
+
 // Do the sections add up to the serial parse?  (one thread)
 __device__ bool gs_sections_fit(const DecodeCta *dc, uint32_t clen, uint32_t n) {
 	if (dc->err) return false;
@@ -835,6 +923,10 @@ __device__ bool gs_sections_fit(const DecodeCta *dc, uint32_t clen, uint32_t n) 
 	return dc->ip1[prev] == clen && dc->op1[prev] == n;          // filemap.c:244-248: consumed == compressed_length
 }
 
+// VERIFY (CMB200_VERIFY): the page, decoded or raw, is compared with the record's stored EF128 while it
+// is still in shared memory (gs_page_matches), so a page that does not match is never written out and
+// is answered ST_CORRUPT.
+template <bool VERIFY>
 __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
 	GetShared *sh = reinterpret_cast<GetShared *>(smem);
@@ -903,7 +995,14 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 			if (st == ST_REMOTE) break;
 			continue;
 		}
+		if (VERIFY) {
+			if (tid == 0) gs_fp_take(job, sh, off, clen, st == ST_HIT);
+			__syncthreads();
+		}
 		if (clen == 0u) {
+			if (VERIFY && sh->fp_ok &&
+			    !gs_page_matches(rec + 24, job.nbytes, reinterpret_cast<ulonglong2 *>(smem + gs_sums_at(job.nbytes)),
+			        sh->fp[0], sh->fp[1], &sh->match, warp, lane)) { result = ST_CORRUPT; break; }
 			// raw page (filemap.c:249-251); 8-byte granularity: rec + 24 is not 16-byte aligned
 			for (uint32_t k = tid; k < job.nbytes / 8u; k += GS_THREADS)
 				reinterpret_cast<unsigned long long *>(out)[k] = reinterpret_cast<const unsigned long long *>(rec + 24)[k];
@@ -939,6 +1038,9 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 		__syncthreads();
 		if (warp == 0) dc_matches<false>(dc, desc, stride, page_s, lane);
 		__syncthreads();
+		if (VERIFY && sh->fp_ok &&
+		    !gs_page_matches(page, job.nbytes, reinterpret_cast<ulonglong2 *>(smem + gs_sums_at(job.nbytes)),
+		        sh->fp[0], sh->fp[1], &sh->match, warp, lane)) { result = ST_CORRUPT; break; }
 		for (uint32_t k = tid; k < job.nbytes / 16u; k += GS_THREADS)
 			reinterpret_cast<uint4 *>(out)[k] = reinterpret_cast<const uint4 *>(page)[k];
 		result = ST_HIT;
@@ -954,6 +1056,8 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 			// loaded again rather than kept from the top: u and l live past the loop would cost registers
 			hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
 		}
+		if (VERIFY && (result == ST_HIT || result == ST_CORRUPT))
+			atomicAdd(&job.vstat[result == ST_CORRUPT ? VS_CORRUPT : sh->fp_ok ? VS_VERIFIED : VS_UNVERIFIED], 1ull);
 		__threadfence_system();
 		*reinterpret_cast<volatile int32_t *>(&job.status[i]) = result;
 	}
@@ -978,6 +1082,9 @@ struct PairVerdict {                              // the page CTA's control bloc
 	uint32_t region;                          // scratch region of the descriptors (~0: none)
 	uint32_t decode;                          // 1: the literals are in the page, the matches are not
 	uint32_t from_host;                       // the record came from the host tier
+	uint32_t fp_ok;                           // VERIFY: fp holds the record's stored EF128 (GetShared::fp_ok)
+	uint32_t match;                           // the page CTA's gs_page_matches answer
+	uint32_t fp[4];                           // {hi, lo} as 32-bit halves (DSMEM stores are 32-bit)
 };
 static_assert(sizeof(PairVerdict) <= 128, "control block");
 
@@ -998,6 +1105,9 @@ __device__ __forceinline__ uint8_t *dsmem_map_generic(uint8_t *p, uint32_t rank)
 }
 __device__ __forceinline__ void dsmem_st32(uint32_t a, uint32_t v) { asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 
+// VERIFY: the CTA that holds the page compares it with the record's stored EF128 before writing it out
+// (gs_page_matches): the page CTA for a decoded page, the record CTA for a raw one.
+template <bool VERIFY>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get_small_pair(GetJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
 	DecodeCta *dc = reinterpret_cast<DecodeCta *>(smem + 128);
@@ -1017,8 +1127,20 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 		if (v->decode) {
 			if (warp == 0) dc_matches<true>(dc, job.scratch + (size_t)v->region * job.region_entries, stride, smem_addr(buf), lane);
 			__syncthreads();
-			for (uint32_t k = tid; k < job.nbytes / 16u; k += GS_THREADS)
-				reinterpret_cast<uint4 *>(out)[k] = reinterpret_cast<const uint4 *>(buf)[k];
+			bool write = true;
+			if constexpr (VERIFY) {
+				PairVerdict *vw = reinterpret_cast<PairVerdict *>(smem);
+				if (v->fp_ok &&
+				    !gs_page_matches(buf, job.nbytes, reinterpret_cast<ulonglong2 *>(smem + gs_sums_at(job.nbytes)),
+				        (unsigned long long)v->fp[1] << 32 | v->fp[0], (unsigned long long)v->fp[3] << 32 | v->fp[2],
+				        &vw->match, warp, lane)) {
+					write = false;
+					if (tid == 0) vw->result = ST_CORRUPT;      // read below by this thread only
+				}
+			}
+			if (write)
+				for (uint32_t k = tid; k < job.nbytes / 16u; k += GS_THREADS)
+					reinterpret_cast<uint4 *>(out)[k] = reinterpret_cast<const uint4 *>(buf)[k];
 		}
 		// the page first, then the status (as k_get_small; a raw page was written by the record CTA
 		// before it arrived at B, and this thread acquired B)
@@ -1029,6 +1151,9 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 				atomicAdd(job.host_hits, 1ull);
 				hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
 			}
+			if constexpr (VERIFY)
+				if (v->result == ST_HIT || v->result == ST_CORRUPT)
+					atomicAdd(&job.vstat[v->result == ST_CORRUPT ? VS_CORRUPT : v->fp_ok ? VS_VERIFIED : VS_UNVERIFIED], 1ull);
 			__threadfence_system();
 			*reinterpret_cast<volatile int32_t *>(&job.status[i]) = v->result;
 		}
@@ -1088,7 +1213,14 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 			if (st == ST_REMOTE) break;
 			continue;
 		}
+		if (VERIFY) {
+			if (tid == 0) gs_fp_take(job, sh, off, clen, st == ST_HIT);
+			__syncthreads();
+		}
 		if (clen == 0u) {
+			if (VERIFY && sh->fp_ok &&
+			    !gs_page_matches(rec + 24, job.nbytes, reinterpret_cast<ulonglong2 *>(smem + gs_sums_at(job.nbytes)),
+			        sh->fp[0], sh->fp[1], &sh->match, warp, lane)) { result = ST_CORRUPT; break; }
 			for (uint32_t k = tid; k < job.nbytes / 8u; k += GS_THREADS)
 				reinterpret_cast<unsigned long long *>(out)[k] = reinterpret_cast<const unsigned long long *>(rec + 24)[k];
 			result = ST_HIT;
@@ -1132,55 +1264,70 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 		dsmem_st32(v + offsetof(PairVerdict, region), region);
 		dsmem_st32(v + offsetof(PairVerdict, decode), decode ? 1u : 0u);
 		dsmem_st32(v + offsetof(PairVerdict, from_host), from_host ? 1u : 0u);
+		if (VERIFY) {
+			// a raw page was checked here; fp_ok also tells the page CTA which counter the hit goes to
+			const uint32_t fp_ok = (result == ST_HIT || result == ST_CORRUPT) ? sh->fp_ok : 0u;
+			dsmem_st32(v + offsetof(PairVerdict, fp_ok), fp_ok);
+			for (uint32_t k = 0; k < 4; k++)
+				dsmem_st32(v + offsetof(PairVerdict, fp) + 4u * k, (uint32_t)(sh->fp[k >> 1] >> (32u * (k & 1u))));
+		}
 	}
 	cluster_arrive_release();                                   // B
 	cluster_wait();
 }
 
-int launch_get_small(const GetJob &job, int device, cudaStream_t st) {
-	if (job.n == 0) return 0;
-	const size_t smem = get_small_smem(job.nbytes);
+template <bool VERIFY>
+static int launch_get_small_kernel(const GetJob &job, int device, cudaStream_t st) {
+	const size_t smem = get_small_smem(job.nbytes, VERIFY);
 	// the attribute belongs to the device: engines on several GPUs (CMB200_DEVICES) each set their own
 	constexpr int MAX_DEV = 64;
 	const int dev = device >= 0 && device < MAX_DEV ? device : 0;
 	if (job.nbytes > GS_MAX_PAGE) {
 		static size_t configured_pair[MAX_DEV] = {};
 		if (smem > configured_pair[dev]) {
-			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 			configured_pair[dev] = smem;
 		}
-		k_get_small_pair<<<2u * job.n, GS_THREADS, smem, st>>>(job);
+		k_get_small_pair<VERIFY><<<2u * job.n, GS_THREADS, smem, st>>>(job);
 		CMB_CHECK(cudaGetLastError());
 		return 0;
 	}
 	static size_t configured[MAX_DEV] = {};
 	if (smem > configured[dev]) {
-		CMB_CHECK(cudaFuncSetAttribute(k_get_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+		CMB_CHECK(cudaFuncSetAttribute(k_get_small<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 		configured[dev] = smem;
 	}
-	k_get_small<<<job.n, GS_THREADS, smem, st>>>(job);
+	k_get_small<VERIFY><<<job.n, GS_THREADS, smem, st>>>(job);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
+}
+int launch_get_small(const GetJob &job, int device, cudaStream_t st) {
+	if (job.n == 0) return 0;
+	return job.table.fp_tag ? launch_get_small_kernel<true>(job, device, st) : launch_get_small_kernel<false>(job, device, st);
 }
 
 // Requests of k_get_small (CTAs) or k_get_small_pair (clusters) that can be resident on the device at
 // once (= scratch regions needed).  Clusters of two need two SMs of one GPC.
-int get_small_residency(uint32_t nbytes) {
-	const size_t smem = get_small_smem(nbytes);
+template <bool VERIFY>
+static int get_small_residency_of(uint32_t nbytes) {
+	const size_t smem = get_small_smem(nbytes, VERIFY);
 	if (nbytes > GS_MAX_PAGE) {
-		if (cudaFuncSetAttribute(k_get_small_pair, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+		if (cudaFuncSetAttribute(k_get_small_pair<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
 		cudaLaunchConfig_t cfg = {};
 		cfg.gridDim = dim3(2u * (uint32_t)sm_count());
 		cfg.blockDim = dim3(GS_THREADS);
 		cfg.dynamicSmemBytes = smem;
 		int clusters = 0;
-		if (cudaOccupancyMaxActiveClusters(&clusters, k_get_small_pair, &cfg) != cudaSuccess) return -1;
+		if (cudaOccupancyMaxActiveClusters(&clusters, k_get_small_pair<VERIFY>, &cfg) != cudaSuccess) return -1;
 		return clusters;
 	}
-	if (cudaFuncSetAttribute(k_get_small, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+	if (cudaFuncSetAttribute(k_get_small<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
 	int per_sm = 0;
-	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_get_small, (int)GS_THREADS, smem) != cudaSuccess) return -1;
+	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_get_small<VERIFY>, (int)GS_THREADS, smem) != cudaSuccess) return -1;
 	return per_sm * sm_count();
+}
+int get_small_residency(uint32_t nbytes, bool verify) {
+	return verify ? get_small_residency_of<true>(nbytes) : get_small_residency_of<false>(nbytes);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1291,6 +1438,7 @@ __global__ void k_import_apply_rec(TableView t, ArenaView a, const unsigned long
 	s.addr_u = rec[4 * (size_t)i]; s.addr_l = rec[4 * (size_t)i + 1];
 	// where the record lies in the owner's arena (vlen stays 0: no local record)
 	s.rec_off = xrec_off(tail); s.alloc = xrec_len1(tail);
+	if (t.fp_tag) t.fp_tag[idx] = 0u;                 // the exchange record carries no fingerprint
 	__threadfence();
 	s.owner = (unsigned long long)xrec_owner(tail) + 1;
 }
@@ -1312,9 +1460,9 @@ int launch_upsert(TableView t, const unsigned long long *addr, const uint8_t *va
 	return 0;
 }
 int launch_lookup(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
-    int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out, cudaStream_t st) {
+    int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out, cudaStream_t st, uint32_t *idx_out) {
 	if (n == 0) return 0;
-	k_lookup<<<GRID1D(n), 0, st>>>(t, addr, valid, n, status, rec_off, vlen, ts_out);
+	k_lookup<<<GRID1D(n), 0, st>>>(t, addr, valid, n, status, rec_off, vlen, ts_out, idx_out);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
@@ -1380,7 +1528,10 @@ __global__ void k_export_list(TableView t, uint32_t bsize, ExportEntry *out, uns
 	if (j >= max_out) return;
 	ExportEntry e;
 	e.rec_off = s.rec_off; e.ts = s.ts;
-	e.fp_hi = t.fp ? t.fp[2 * i] : 0ull; e.fp_lo = t.fp ? t.fp[2 * i + 1] : 0ull;
+	// {0, 0} = no fingerprint: a record loaded without one keeps none (with CMB200_VERIFY its tag says
+	// whether fp belongs to this record; without it, fp of such a record is {0, 0} already)
+	const bool has_fp = t.fp && (!t.fp_tag || t.fp_tag[i] == ckpt_tag(s.rec_off, s.vlen - 1u));
+	e.fp_hi = has_fp ? t.fp[2 * i] : 0ull; e.fp_lo = has_fp ? t.fp[2 * i + 1] : 0ull;
 	e.len = 24u + (s.vlen > 1u ? s.vlen - 1u : bsize);
 	e.slot = (uint32_t)i;
 	out[j] = e;
@@ -1389,6 +1540,22 @@ int launch_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned l
     unsigned long long max_out, bool arena_only, cudaStream_t st) {
 	const uint64_t n = t.cap + 2;
 	k_export_list<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, bsize, out, count, max_out, arena_only);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+__global__ void k_scan_prep(TableView t, const ExportEntry *list, uint32_t n, int32_t *status, uint64_t *rec_off,
+    uint32_t *vlen, uint32_t *idx, unsigned long long *addr) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const ExportEntry x = list[i];
+	const Slot &s = t.slots[x.slot];
+	status[i] = ST_HIT; rec_off[i] = x.rec_off; vlen[i] = s.vlen; idx[i] = x.slot;
+	addr[2 * (size_t)i] = s.addr_u; addr[2 * (size_t)i + 1] = s.addr_l;
+}
+int launch_scan_prep(TableView t, const ExportEntry *list, uint32_t n, int32_t *status, uint64_t *rec_off,
+    uint32_t *vlen, uint32_t *idx, unsigned long long *addr, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_scan_prep<<<GRID1D(n), 0, st>>>(t, list, n, status, rec_off, vlen, idx, addr);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
@@ -1462,8 +1629,11 @@ __global__ void __launch_bounds__(RESTORE_WARPS * 32) k_restore(EncodeJob job, c
 	const uint8_t *rec = blob + off[i];
 	const int32_t clen = *reinterpret_cast<const int32_t *>(rec + 16);   // data_prefix.compressed_length (filemap.c:9-12); off[] is 16-aligned
 	const uint32_t plen = clen > 0 ? (uint32_t)clen : bsize;
+	// a record saved without a fingerprint carries {0, 0} even in a file whose header says it has them
+	// (cmb200_save writes every record of the store): it stays unverified
+	const uint64_t fp_hi = fps ? fps[2 * i] : 0ull, fp_lo = fps ? fps[2 * i + 1] : 0ull;
 	const unsigned long long at =
-	    commit_record(job, i, idx, rec + 24, plen, clen, true, fps ? fps[2 * i] : 0ull, fps ? fps[2 * i + 1] : 0ull, lane);
+	    commit_record(job, i, idx, rec + 24, plen, clen, true, fp_hi, fp_lo, lane, (fp_hi | fp_lo) != 0ull);
 	// the encoder's checkpoints, rebuilt from the block (raw pages have none); slot_publish has zeroed
 	// the tag, so a block that does not walk leaves the record to the one-warp parse of k_get_small
 	if (at == ~0ull || clen <= 0 || !job.table.ckpt) return;
@@ -1608,6 +1778,7 @@ __global__ void k_tier_retire(TableView t, ArenaView a, const unsigned long long
 			atomicAdd(a.tier + 1, (unsigned long long)-1ll);
 			s.alloc = 0;
 			s.owner = 0;
+			if (t.fp_tag) t.fp_tag[idx] = 0u;
 			if (idx < t.cap) {
 				s.key = KEY_TOMB;
 				atomicAdd(t.tombs, 1ull);
@@ -1650,6 +1821,7 @@ __global__ void k_rehash(TableView from, TableView to) {
 	// the tag names rec_off and the length, which stay: the parse checkpoints move with the slot
 	if (from.ckpt && to.ckpt)
 		for (uint32_t k = 0; k < CKPT_WORDS; k++) to.ckpt[(size_t)idx * CKPT_WORDS + k] = from.ckpt[i * CKPT_WORDS + k];
+	if (from.fp_tag && to.fp_tag) to.fp_tag[idx] = from.fp_tag[i];
 }
 int launch_rehash(TableView from, TableView to, cudaStream_t st) {
 	const uint64_t n = from.cap + 2;

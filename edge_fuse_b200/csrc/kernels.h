@@ -48,6 +48,8 @@ struct TableView {
 	unsigned long long *remote;  // keys whose newest record lives on another GPU
 	uint64_t *fp;                // optional, 2 x u64 per slot {hi, lo}
 	uint32_t *ckpt;              // optional, CKPT_WORDS per slot: parse checkpoints of the slot's record
+	uint32_t *fp_tag;            // CMB200_VERIFY only, one per slot: ckpt_tag of the record version fp
+	                             // belongs to (0 = none); gets compare a page with fp only under it
 };
 
 // Parse checkpoints (lz4_decode_cta.cuh): word 0 = tag naming the record version (0 = none), word k
@@ -84,7 +86,13 @@ enum LookupStatus : int32_t {
 	ST_BAD_ENTRY = 3,    // key present with another address (filemap.c:236-240)
 	ST_BAD_DECODE = 4,   // decoder consumed != stored length (filemap.c:244-248)
 	ST_REMOTE = 5,       // multi-GPU: the key's newest record is on another rank (status - 5 is not encoded; see owner_out)
+	ST_CORRUPT = 6,      // CMB200_VERIFY: the decoded page's EF128 differs from the one stored with the record
 };
+
+// Counters of the verified gets (CMB200_VERIFY), device words: [VS_VERIFIED] hits whose page matched
+// the stored EF128, [VS_UNVERIFIED] hits without a fingerprint for that record version, [VS_CORRUPT]
+// pages that did not match.
+enum : uint32_t { VS_VERIFIED = 0, VS_UNVERIFIED = 1, VS_CORRUPT = 2, VS_WORDS = 3 };
 
 struct EncodeJob {
 	const uint8_t *pages;    // n chunks, `page_stride` apart, 16-byte aligned
@@ -134,7 +142,14 @@ struct DecodeJob {
 	HotLog hot;                  // where tier hits are logged (null: no tier)
 	const unsigned long long *addr;   // n x {u, l}, the requests' addresses (for the log)
 };
-int launch_decode(const DecodeJob &job, cudaStream_t st);
+// Store mode with CMB200_VERIFY: every decoded page is compared with its record's EF128 (k_decode_verify).
+struct DecodeVerify {
+	const uint32_t *idx;              // per request, the key's slot (from lookup)
+	const uint64_t *fp;               // the table's fingerprints and their tags
+	const uint32_t *fp_tag;
+	unsigned long long *vstat;        // VS_WORDS counters
+};
+int launch_decode(const DecodeJob &job, cudaStream_t st, const DecodeVerify *verify = nullptr);
 
 // Fused small-batch get (one CTA per request): key lookup, record staged in shared memory by TMA,
 // LZ4 decode shared -> shared, page written out with 16-byte stores (device memory or page-locked
@@ -163,11 +178,12 @@ struct GetJob {
 	uint32_t pool_n;
 	HotLog hot;                       // where tier hits are logged (null: no tier); last, so that the
 	                                  // other members keep their parameter offsets
+	unsigned long long *vstat;        // CMB200_VERIFY (table.fp_tag set): VS_WORDS counters
 };
 bool get_small_supports(uint32_t nbytes);
-size_t get_small_smem(uint32_t nbytes);
+size_t get_small_smem(uint32_t nbytes, bool verify);
 uint32_t get_small_region_entries(uint32_t nbytes);
-int get_small_residency(uint32_t nbytes);   // requests resident on the device at once, < 0 on error
+int get_small_residency(uint32_t nbytes, bool verify);   // requests resident on the device at once, < 0 on error
 int launch_get_small(const GetJob &job, int device, cudaStream_t st);   // device: CUDA ordinal the launch runs on
 
 int launch_fingerprint(const uint8_t *pages, uint64_t stride, uint32_t nbytes, uint32_t n,
@@ -203,8 +219,10 @@ int launch_import_records(TableView t, ArenaView a, const unsigned long long *re
     uint32_t *slot_idx, cudaStream_t st);
 
 int launch_lookup(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
-    int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out, cudaStream_t st);
-// After launch_lookup: status ST_REMOTE entries have their owner rank in rec_off[i].
+    int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out, cudaStream_t st,
+    uint32_t *idx_out = nullptr);
+// After launch_lookup: status ST_REMOTE entries have their owner rank in rec_off[i]; idx_out (optional)
+// gets the key's slot of every ST_HIT.
 
 int launch_unset(TableView t, ArenaView a, const unsigned long long *addr, uint32_t n, cudaStream_t st);
 
@@ -235,6 +253,10 @@ static_assert(sizeof(ExportEntry) == 40, "export entry layout");
 // arena_only: leave out the records of the host tier (compaction moves arena records only)
 int launch_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
     unsigned long long max_out, bool arena_only, cudaStream_t st);
+// cmb200_verify_store: turns n export entries into the lookup results of their keys (status ST_HIT,
+// location, vlen, slot, address), the input k_decode's verified store mode reads.
+int launch_scan_prep(TableView t, const ExportEntry *list, uint32_t n, int32_t *status, uint64_t *rec_off,
+    uint32_t *vlen, uint32_t *idx, unsigned long long *addr, cudaStream_t st);
 // Restores n records {24-byte prefix, payload} lying at blob + off[i]; slot_idx from launch_upsert
 // on the records' addresses (job.addr / job.ts / job.table / job.arena / job.seq0 as for a put).
 int launch_restore(const EncodeJob &job, const uint8_t *blob, const unsigned long long *off,

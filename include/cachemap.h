@@ -15,6 +15,9 @@
  *   - a page number that does not fit 44 bits is ignored (put) / NULL without counting (get);
  *   - no error codes: any internal failure is a dropped put or a miss.
  * New: all calls are thread-safe, and concurrent callers are combined into one GPU batch.
+ * With CMB200_VERIFY=1 in the environment every engine checks each page it serves against the
+ * page's stored EF128 fingerprint (cachemap_b200.h, CMB200_VERIFY): a page that differs is a miss,
+ * counted in `requests` and not in `hits`, so the caller fetches and puts it again.
  * struct cachemap is opaque (edgefs.c never looks inside it).
  */
 #ifndef CACHEMAP_H

@@ -31,6 +31,13 @@ typedef struct cmb200_engine cmb200_engine;
 typedef struct { uint64_t u; uint64_t l; } cmb200_addr;
 
 #define CMB200_FINGERPRINT 1u   /* compute + keep the EF128 content fingerprint of every put */
+/* Verified reads (implies CMB200_FINGERPRINT): every hit of cmb200_get_batch, cmb200_get_batch_dev,
+ * cmb200_get_small and cmb200_get_small_begin / _end has its decoded page's EF128 compared on the GPU
+ * with the fingerprint stored for that record version; a page that differs is answered
+ * CMB200_CORRUPT instead of CMB200_HIT.  A hit whose record has no fingerprint (imported from another
+ * rank, read from a peer's arena, or loaded from a snapshot written without fingerprints) is served
+ * as CMB200_HIT and counted unverified.  See cmb200_verify_stats and cmb200_verify_store. */
+#define CMB200_VERIFY 2u
 
 typedef struct cmb200_config {
 	int device;             /* CUDA ordinal, -1 = current device */
@@ -51,7 +58,10 @@ enum {
 	CMB200_INVALID = 2,     /* address rejected: not counted as a request (cachemap.c:173-174) */
 	CMB200_BAD_ENTRY = 3,   /* key present under another address: a miss (filemap.c:236-240) */
 	CMB200_BAD_DECODE = 4,  /* decoded length != stored length: a miss (filemap.c:244-248) */
-	CMB200_REMOTE = 5       /* multi-GPU: the newest record of this key lives on another rank */
+	CMB200_REMOTE = 5,      /* multi-GPU: the newest record of this key lives on another rank */
+	CMB200_CORRUPT = 6      /* CMB200_VERIFY: the decoded page differs from the stored EF128: a miss.
+	                         * The page is not written by cmb200_get_small; cmb200_get_batch(_dev) may
+	                         * have written it, as for CMB200_BAD_DECODE. */
 };
 
 const char *cmb200_last_error(void);
@@ -280,6 +290,25 @@ typedef struct cmb200_small_ticket {
 } cmb200_small_ticket;
 int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_addr *addr, void *pages_out, cmb200_small_ticket *ticket);
 int cmb200_get_small_end(cmb200_engine *e, cmb200_small_ticket *ticket, int32_t *status_out);
+
+/* ---- verified reads (CMB200_VERIFY) -------------------------------------------------------------
+ * Counters of the engine's verified gets: hits whose page matched the stored EF128, hits without a
+ * fingerprint for their record version, pages answered CMB200_CORRUPT; and of cmb200_verify_store:
+ * records decoded by the scans so far, and those among them that failed.  All zero without the flag.
+ * A call of its own rather than more fields of cmb200_stats, so that code built against an older
+ * header keeps passing the struct size it knows. */
+struct cmb200_verify_stats {
+	uint64_t verified, unverified, corrupt;
+	uint64_t scanned, scan_corrupt;
+};
+int cmb200_verify_stats(cmb200_engine *e, struct cmb200_verify_stats *out);
+/* At-rest check of every live local record, in HBM and in the host tier, including records nobody
+ * reads: each one is decoded on the GPU and its page compared with the stored EF128.  Runs on the
+ * engine's stream under its lock, as cmb200_compact does, and repairs nothing.  *n_bad = records whose
+ * page differs from its fingerprint or whose block does not decode; the first `max` of their addresses
+ * go to bad_out (the caller may cmb200_unset_batch them).  *checked = records that had a fingerprint
+ * to compare with; the others are unverified.  -1 for an engine created without CMB200_VERIFY. */
+int cmb200_verify_store(cmb200_engine *e, size_t max, cmb200_addr *bad_out, size_t *n_bad, uint64_t *checked);
 
 /* Lookup only: status_out[i] in CMB200_{MISS,HIT,BAD_ENTRY,REMOTE}; owner_out[i] = owning rank for
  * CMB200_REMOTE. */
