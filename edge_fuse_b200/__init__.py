@@ -9,5 +9,6 @@ from .binding import (  # noqa: F401
     Cachemap, Engine, lib, library_path, compose_keys, lz4_encode_batch, lz4_decode_batch,
     fingerprint_batch, gen_chunk_host, gen_stream_ids, gen_addr, device_count, last_error,
     HIT, MISS, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, FINGERPRINT, EXPORTED_SYMBOLS, engine_stats,
-    host_tier_stats, read_checkpoints, VERIFY, CORRUPT, verify_stats,
+    host_tier_stats, read_checkpoints, VERIFY, CORRUPT, verify_stats, owner, save_set, load_set,
+    snapshot_begin, snapshot_finish,
 )

@@ -39,7 +39,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_host_tier_enable", "cmb200_demote_batch", "cmb200_host_tier_stats",
     "cmb200_promote_batch", "cmb200_host_tier_hot", "cmb200_read_checkpoints",
     "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
-    "cmb200_verify_stats", "cmb200_verify_store",
+    "cmb200_verify_stats", "cmb200_verify_store", "cmb200_snapshot_begin", "cmb200_snapshot_finish",
 ]
 
 
@@ -167,6 +167,8 @@ def lib() -> C.CDLL:
         "cmb200_copy_peer": (i32, [vp, vp, vp, vp, sz]),
         "cmb200_verify_stats": (i32, [vp, vp]),
         "cmb200_verify_store": (i32, [vp, sz, vp, vp, vp]),
+        "cmb200_snapshot_begin": (vp, [vp, i32, C.c_char_p]),
+        "cmb200_snapshot_finish": (i32, [vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -541,6 +543,10 @@ class Engine:
         _check(lib().cmb200_load(self.h, path.encode(), C.byref(n)), "cmb200_load")
         return n.value
 
+    def snapshot_begin(self, path: str) -> int:
+        """cmb200_snapshot_begin of this engine alone -> handle for snapshot_finish."""
+        return snapshot_begin([self.h], path)
+
     def move_pages(self, n: int, dst_dev: int, src_dev: int, dst_idx=None, src_idx=None):
         """cmb200_move_pages: dst[dst_idx[i] or i] = src[src_idx[i] or i], n pages in this engine's HBM."""
         di = None if dst_idx is None else np.ascontiguousarray(dst_idx, dtype=np.uint32)
@@ -607,6 +613,24 @@ def save_set(handles, path: str) -> int:
     arr, g = _handles(handles)
     n = C.c_uint64(0)
     _check(lib().cmb200_save_set(arr, g, path.encode(), C.byref(n)), "cmb200_save_set")
+    return n.value
+
+
+def snapshot_begin(handles, path: str) -> int:
+    """cmb200_snapshot_begin over engine handles -> snapshot handle.  The engines' live records are
+    listed now and written by a thread of the snapshot while the engines keep serving."""
+    arr, g = _handles(handles)
+    s = lib().cmb200_snapshot_begin(arr, g, path.encode())
+    if not s:
+        raise RuntimeError(f"cmb200_snapshot_begin failed: {last_error()}")
+    return int(s)
+
+
+def snapshot_finish(s: int) -> int:
+    """cmb200_snapshot_finish: waits for the writer and renames the file into place -> records written.
+    The handle is freed, whatever the outcome."""
+    n = C.c_uint64(0)
+    _check(lib().cmb200_snapshot_finish(s, C.byref(n)), "cmb200_snapshot_finish")
     return n.value
 
 

@@ -29,6 +29,7 @@
  * (set CMB200_SOFT_FAIL=1 to degrade to "every put dropped, every get a miss" instead).
  */
 #define _GNU_SOURCE
+#include <errno.h>
 #include <pthread.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -156,9 +157,14 @@ struct filemap {
 	uint64_t reserved;      /* (atomic) */
 	/* persistence: <destdir>/cachemap_b200.snap (cmb200_save_set / cmb200_load_set) */
 	int persist;
-	long checkpoint_sec;    /* > 0: the first engine's flusher saves a snapshot this often when puts have arrived */
-	uint64_t puts_seen, puts_saved;
+	long checkpoint_sec;    /* > 0: the checkpoint thread saves a snapshot this often when puts have landed */
+	uint64_t puts_seen, puts_saved; /* (atomic) */
 	pthread_mutex_t snap_mu;
+	/* the checkpoint thread (CMB200_CHECKPOINT_SEC): sleeps on ckpt_cv, so that filemap_free can wake it */
+	pthread_mutex_t ckpt_mu;
+	pthread_cond_t ckpt_cv;
+	pthread_t ckpt_thread;
+	int ckpt_started, ckpt_stop;
 };
 
 #define SNAPSHOT_NAME "cachemap_b200.snap"
@@ -222,6 +228,7 @@ filemap_device_list(int *out)
 }
 
 static void *filemap_flusher(void *arg);
+static void *filemap_checkpointer(void *arg);
 
 static void
 fm_dev_free(struct fm_dev *d)
@@ -377,6 +384,9 @@ filemap_engine_ready(struct filemap *m)
 				else
 					d->wb_n = 0;
 			}
+			if (m->persist && m->checkpoint_sec > 0 &&
+			    pthread_create(&m->ckpt_thread, NULL, filemap_checkpointer, m) == 0)
+				m->ckpt_started = 1;
 			__atomic_store_n(&m->init_state, 1, __ATOMIC_RELEASE);
 		}
 	}
@@ -404,6 +414,8 @@ filemap_create(char *destdir, uint64_t n, int compress_accel, int pshift)
 	pthread_mutex_init(&m->init_mu, NULL);
 	pthread_mutex_init(&m->evict_mu, NULL);
 	pthread_mutex_init(&m->snap_mu, NULL);
+	pthread_mutex_init(&m->ckpt_mu, NULL);
+	pthread_cond_init(&m->ckpt_cv, NULL);
 	return m;
 }
 
@@ -424,11 +436,36 @@ filemap_save(struct filemap *m)
 	uint64_t seen = __atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED);
 	int rc = cmb200_save_set(m->engs, m->g, snap, NULL);
 	if (rc == 0)
-		m->puts_saved = seen;
+		__atomic_store_n(&m->puts_saved, seen, __ATOMIC_RELAXED);
 	else
 		fprintf(stderr, "cachemap_b200: snapshot not written: %s\n", cmb200_last_error());
 	pthread_mutex_unlock(&m->snap_mu);
 	return rc;
+}
+
+/* CMB200_CHECKPOINT_SEC: every checkpoint_sec seconds, a snapshot if puts have landed since the last
+ * one.  The engines list their records under their locks and write them outside, so neither the
+ * flushers nor the callers of the map wait for the file. */
+static void *
+filemap_checkpointer(void *arg)
+{
+	struct filemap *m = arg;
+	pthread_mutex_lock(&m->ckpt_mu);
+	while (!m->ckpt_stop) {
+		struct timespec until;
+		clock_gettime(CLOCK_REALTIME, &until);
+		until.tv_sec += m->checkpoint_sec;
+		while (!m->ckpt_stop && pthread_cond_timedwait(&m->ckpt_cv, &m->ckpt_mu, &until) != ETIMEDOUT)
+			;
+		if (m->ckpt_stop)
+			break;
+		pthread_mutex_unlock(&m->ckpt_mu);
+		if (__atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED) != __atomic_load_n(&m->puts_saved, __ATOMIC_RELAXED))
+			filemap_save(m);
+		pthread_mutex_lock(&m->ckpt_mu);
+	}
+	pthread_mutex_unlock(&m->ckpt_mu);
+	return NULL;
 }
 
 /* Waits until every page accepted by this engine's ring so far is in its store. */
@@ -469,6 +506,13 @@ filemap_free(struct filemap *m)
 {
 	if (!m)
 		return;
+	if (m->ckpt_started) {
+		pthread_mutex_lock(&m->ckpt_mu);
+		m->ckpt_stop = 1;
+		pthread_cond_broadcast(&m->ckpt_cv);
+		pthread_mutex_unlock(&m->ckpt_mu);
+		pthread_join(m->ckpt_thread, NULL);     /* a save in progress ends first */
+	}
 	for (int i = 0; i < m->g; i++) {
 		struct fm_dev *d = m->dev[i];
 		if (!d->wb_started)
@@ -493,6 +537,8 @@ filemap_free(struct filemap *m)
 	for (int i = 0; i < m->g; i++)
 		fm_dev_free(m->dev[i]);
 	pthread_mutex_destroy(&m->snap_mu);
+	pthread_cond_destroy(&m->ckpt_cv);
+	pthread_mutex_destroy(&m->ckpt_mu);
 	pthread_mutex_destroy(&m->evict_mu);
 	pthread_mutex_destroy(&m->init_mu);
 	free(m);
@@ -910,8 +956,7 @@ timespec_add_ms(struct timespec *t, long ms)
 }
 
 /* The flusher of one engine: takes the longest run of finished slots from the tail of its ring and
- * puts it into the engine as one batch (two calls when the run wraps around the ring).  The first
- * engine's flusher also writes the CMB200_CHECKPOINT_SEC snapshots of the whole map. */
+ * puts it into the engine as one batch (two calls when the run wraps around the ring). */
 static void *
 filemap_flusher(void *arg)
 {
@@ -919,8 +964,6 @@ filemap_flusher(void *arg)
 	struct filemap *m = d->m;
 	cmb200_addr *addr = malloc(FLUSH_MAX * sizeof(cmb200_addr));
 	uint64_t *ts = malloc(FLUSH_MAX * sizeof(uint64_t));
-	time_t last_save = time(NULL);
-	const int checkpoints = m->checkpoint_sec > 0 && m->persist && d->index == 0;
 	pthread_mutex_lock(&d->wb_mu);
 	for (;;) {
 		uint64_t count = 0;
@@ -942,26 +985,7 @@ filemap_flusher(void *arg)
 				pthread_mutex_lock(&d->wb_mu);
 				continue;
 			}
-			if (checkpoints) {
-				struct timespec now, until;
-				clock_gettime(CLOCK_REALTIME, &now);
-				if (__atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED) != m->puts_saved &&
-				    now.tv_sec - last_save >= m->checkpoint_sec) {
-					pthread_mutex_unlock(&d->wb_mu);
-					filemap_save(m);
-					pthread_mutex_lock(&d->wb_mu);
-					last_save = now.tv_sec;
-					continue;
-				}
-				until = now;
-				if (d->tier_promote)
-					timespec_add_ms(&until, PROMOTE_EVERY_MS);
-				else
-					until.tv_sec += 1;
-				d->wb_flusher_asleep = 1;
-				pthread_cond_timedwait(&d->wb_work, &d->wb_mu, &until);
-				d->wb_flusher_asleep = 0;
-			} else if (d->tier_promote) {
+			if (d->tier_promote) {
 				/* woken for the next promotion round at the latest */
 				struct timespec until;
 				clock_gettime(CLOCK_REALTIME, &until);

@@ -12,6 +12,7 @@
 // A get batch is: k_lookup -> k_decode -> D2H copy.
 #include <algorithm>
 #include <atomic>
+#include <condition_variable>
 #include <deque>
 #include <mutex>
 #include <set>
@@ -19,6 +20,7 @@
 #include <sched.h>
 #include <string>
 #include <new>
+#include <thread>
 #include <unordered_set>
 #include <stdio.h>
 #include <stdlib.h>
@@ -158,6 +160,16 @@ struct cmb200_engine {
 	unsigned long long *d_vstat = nullptr;
 	uint32_t *d_vidx = nullptr;          // slot of each request of a verified get batch (max_batch)
 	uint64_t scanned = 0, scan_corrupt = 0;
+	// snapshots (cmb200_snapshot_begin): SNAP_FREE, SNAP_CLAIMED by a snapshot that has not listed this
+	// engine's records yet, or SNAP_PENDING: listed, section not written yet.  snap_state changes under
+	// snap_mu and every change is broadcast on snap_cv.  Lock order: mu before snap_mu.  The snapshot's
+	// writer takes snap_mu only, never mu, so a holder of mu may wait on snap_cv for the writer.
+	enum { SNAP_FREE = 0, SNAP_CLAIMED, SNAP_PENDING };
+	int snap_state = SNAP_FREE;
+	std::mutex snap_mu;
+	std::condition_variable snap_cv;
+	uint8_t *snap_win = nullptr;         // page-locked window of the writer, kept from the first snapshot on
+	cudaStream_t snap_st = nullptr;      // the writer's copies: they do not queue behind encodes on st
 };
 
 #define ENG_CHECK(expr)                                                 \
@@ -228,6 +240,8 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	for (int i = 0; i < cmb200_engine::TICKETS; i++) if (e->ticket_ev[i]) cudaEventDestroy(e->ticket_ev[i]);
 	if (e->meta_done) cudaEventDestroy(e->meta_done);
 	for (int i = 0; i < 2; i++) if (e->meta_free[i]) cudaEventDestroy(e->meta_free[i]);
+	if (e->snap_win) cudaFreeHost(e->snap_win);
+	if (e->snap_st) cudaStreamDestroy(e->snap_st);
 	if (e->st) cudaStreamDestroy(e->st);
 	if (e->copy) cudaStreamDestroy(e->copy);
 	delete e;
@@ -1094,15 +1108,31 @@ struct SnapRecord { uint64_t ts, fp_hi, fp_lo; uint32_t len, zero; };
 static_assert(sizeof(SnapRecord) == 32, "snapshot record header");
 static const size_t SNAP_WINDOW = 64u << 20;
 
-// Writes every live record of e to f through the page-locked window `win` and adds to *records /
-// *bytes.  (e->mu held)  0 = written, -1 = a CUDA call failed (error set), -2 = a write failed.
-static int save_engine(cmb200_engine *e, FILE *f, uint8_t *win, uint64_t *records, uint64_t *bytes) {
-	unsigned long long c[8];
-	std::vector<ExportEntry> list;
-	if (live_records(e, false, list, c) < 0) return -1;
-	*records += list.size();
-	for (const ExportEntry &x : list) *bytes += x.len;
+// A snapshot lists each engine's live records under its lock and writes them from a thread of its own
+// while the engines keep serving.  That is sound because records are immutable (DESIGN.md §2): only
+// compaction (which slides records down) and a host-tier lap (which overwrites the tier's oldest
+// records) reuse the bytes of a record, and both wait in snap_wait_written until the engine's section
+// is written.  Every other writer of arena or tier bytes writes bytes no listed record occupies.
 
+// Waits until no snapshot holds a list of e's records that it has not written yet.  (e->mu held; the
+// writer never takes it, see cmb200_engine::snap_state)
+static void snap_wait_written(cmb200_engine *e) {
+	std::unique_lock<std::mutex> lk(e->snap_mu);
+	e->snap_cv.wait(lk, [e] { return e->snap_state != cmb200_engine::SNAP_PENDING; });
+}
+
+static void snap_set_state(cmb200_engine *e, int state) {
+	std::lock_guard<std::mutex> lk(e->snap_mu);
+	e->snap_state = state;
+	e->snap_cv.notify_all();
+}
+
+// Writes the listed records of e to f through the engine's page-locked window, copying arena windows on
+// the writer's stream.  A window may also hold garbage or records put after the list was taken; only
+// listed records are written, and their bytes do not change until the section is released.  (runs
+// without e->mu)  0 = written, -1 = a CUDA call failed (error set), -2 = a write failed.
+static int write_section(cmb200_engine *e, FILE *f, const std::vector<ExportEntry> &list) {
+	uint8_t *win = e->snap_win;
 	bool ok = true;
 	static const uint8_t zeros[16] = {0};
 	size_t k = 0;
@@ -1120,8 +1150,8 @@ static int save_engine(cmb200_engine *e, FILE *f, uint8_t *win, uint64_t *record
 		const unsigned long long w0 = list[k].rec_off;
 		unsigned long long w1 = w0 + SNAP_WINDOW;
 		if (w1 > e->arena.size + 256) w1 = e->arena.size + 256;
-		if (cudaMemcpyAsync(win, e->arena.base + w0, (size_t)(w1 - w0), cudaMemcpyDeviceToHost, e->st) != cudaSuccess ||
-		    cudaStreamSynchronize(e->st) != cudaSuccess) { ok = false; break; }
+		CMB_CHECK(cudaMemcpyAsync(win, e->arena.base + w0, (size_t)(w1 - w0), cudaMemcpyDeviceToHost, e->snap_st));
+		CMB_CHECK(cudaStreamSynchronize(e->snap_st));
 		for (; k < list.size() && list[k].rec_off + list[k].len <= w1; k++) {
 			const ExportEntry &x = list[k];
 			SnapRecord r{x.ts, x.fp_hi, x.fp_lo, x.len, 0};
@@ -1133,36 +1163,122 @@ static int save_engine(cmb200_engine *e, FILE *f, uint8_t *win, uint64_t *record
 	return ok ? 0 : -2;
 }
 
-extern "C" int cmb200_save_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out) {
-	if (g < 1 || !engines) { set_error_msg("cmb200_save_set: no engines"); return -1; }
-	for (int i = 1; i < g; i++)
-		if (engines[i]->pshift != engines[0]->pshift) { set_error_msg("cmb200_save_set: engines of different page sizes"); return -1; }
-	std::string tmp = std::string(path) + ".tmp";
-	FILE *f = fopen(tmp.c_str(), "wb");
-	if (!f) { set_error_msg("cmb200_save: cannot create the snapshot file"); return -1; }
-	uint8_t *win = nullptr;
-	if (cudaMallocHost(&win, SNAP_WINDOW) != cudaSuccess) { fclose(f); remove(tmp.c_str()); set_error_msg("cmb200_save: no page-locked window"); return -1; }
-	// the header goes first with the counts zero and is written again once every section is out
+struct cmb200_snapshot {
+	std::vector<cmb200_engine *> engines;                 // in file order
+	std::vector<std::vector<ExportEntry>> lists;          // each engine's live records at begin, by offset
+	std::string tmp;
+	FILE *f = nullptr;
 	SnapHeader h{};
-	memcpy(h.magic, "CMB200S1", 8);
-	h.version = 1; h.pshift = (uint32_t)engines[0]->pshift; h.flags = engines[0]->table.fp ? 1u : 0u;
-	bool ok = fwrite(&h, sizeof(h), 1, f) == 1;
+	std::thread writer;
+	int rc = 0;                                           // the writer's: 0, -1 CUDA, -2 file
+	std::string err;                                      // the writer's error text (g_err is per thread)
+};
+
+// The writer thread: header, then each engine's section; an engine is released as soon as its section
+// is written (or the write has failed), so that its compactions and tier laps go ahead.
+static void snapshot_write(cmb200_snapshot *s) {
+	bool ok = fwrite(&s->h, sizeof(s->h), 1, s->f) == 1;
+	int rc = ok ? 0 : -2;
+	for (size_t i = 0; i < s->engines.size(); i++) {
+		cmb200_engine *e = s->engines[i];
+		if (rc == 0) {
+			if (cudaSetDevice(e->device) != cudaSuccess) { cmb_set_error("cudaSetDevice", cudaGetLastError(), __FILE__, __LINE__); rc = -1; }
+			else rc = write_section(e, s->f, s->lists[i]);
+		}
+		std::vector<ExportEntry>().swap(s->lists[i]);
+		snap_set_state(e, cmb200_engine::SNAP_FREE);
+	}
+	if (rc == 0 && fflush(s->f) != 0) rc = -2;
+	if (fclose(s->f) != 0 && rc == 0) rc = -2;
+	s->f = nullptr;
+	if (rc == -2) set_error_msg("cmb200_save: write failed");
+	if (rc) s->err = g_err;
+	s->rc = rc;
+}
+
+extern "C" cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines, int g, const char *path) {
+	if (g < 1 || !engines || !path) { set_error_msg("cmb200_snapshot_begin: no engines"); return nullptr; }
+	for (int i = 1; i < g; i++)
+		if (engines[i]->pshift != engines[0]->pshift) { set_error_msg("cmb200_save_set: engines of different page sizes"); return nullptr; }
+	// engines are claimed in address order, so that two snapshots of overlapping sets never each hold
+	// an engine the other one waits for
+	std::vector<cmb200_engine *> order(engines, engines + g);
+	std::sort(order.begin(), order.end());
+	if (std::adjacent_find(order.begin(), order.end()) != order.end()) { set_error_msg("cmb200_snapshot_begin: an engine is listed twice"); return nullptr; }
+	cmb200_snapshot *s = new (std::nothrow) cmb200_snapshot();
+	if (!s) { set_error_msg("cmb200_snapshot_begin: out of memory"); return nullptr; }
+	s->engines.assign(engines, engines + g);
+	s->lists.resize(g);
+	s->tmp = std::string(path) + ".tmp";
+	s->f = fopen(s->tmp.c_str(), "wb");
+	if (!s->f) { set_error_msg("cmb200_save: cannot create the snapshot file"); delete s; return nullptr; }
+	for (cmb200_engine *e : order) {
+		std::unique_lock<std::mutex> lk(e->snap_mu);
+		e->snap_cv.wait(lk, [e] { return e->snap_state == cmb200_engine::SNAP_FREE; });
+		e->snap_state = cmb200_engine::SNAP_CLAIMED;
+	}
 	int rc = 0;
-	for (int i = 0; i < g && ok && rc == 0; i++) {
-		std::lock_guard<std::mutex> lk(engines[i]->mu);
-		rc = save_engine(engines[i], f, win, &h.records, &h.bytes);
+	for (cmb200_engine *e : order) {
+		// allocated once: cudaFreeHost may synchronise the device
+		if (cudaSetDevice(e->device) != cudaSuccess ||
+		    (!e->snap_win && cudaMallocHost(&e->snap_win, SNAP_WINDOW) != cudaSuccess) ||
+		    (!e->snap_st && cudaStreamCreateWithFlags(&e->snap_st, cudaStreamNonBlocking) != cudaSuccess)) {
+			cmb_set_error("cmb200_snapshot_begin: no page-locked window or stream", cudaGetLastError(), __FILE__, __LINE__);
+			rc = -1;
+			break;
+		}
 	}
-	cudaFreeHost(win);
-	ok = ok && rc != -2 && fseek(f, 0, SEEK_SET) == 0 && fwrite(&h, sizeof(h), 1, f) == 1;
-	ok = ok && fflush(f) == 0;
-	ok = (fclose(f) == 0) && ok;
-	if (rc == -1 || !ok || rename(tmp.c_str(), path) != 0) {
-		remove(tmp.c_str());
-		if (rc != -1) set_error_msg("cmb200_save: write failed");
-		return -1;
+	s->h = SnapHeader{};
+	memcpy(s->h.magic, "CMB200S1", 8);
+	s->h.version = 1; s->h.pshift = (uint32_t)engines[0]->pshift;
+	for (int i = 0; i < g && rc == 0; i++) {
+		cmb200_engine *e = engines[i];
+		std::lock_guard<std::mutex> lk(e->mu);
+		if (i == 0) s->h.flags = e->table.fp ? 1u : 0u;
+		unsigned long long c[8];
+		// live_records synchronises the stream first: every put enqueued before now is listed
+		if (live_records(e, false, s->lists[i], c) < 0) { rc = -1; break; }
+		snap_set_state(e, cmb200_engine::SNAP_PENDING);
+		s->h.records += s->lists[i].size();
+		for (const ExportEntry &x : s->lists[i]) s->h.bytes += x.len;
 	}
-	if (records_out) *records_out = h.records;
-	return 0;
+	if (rc == 0) {
+		try {
+			s->writer = std::thread(snapshot_write, s);
+		} catch (...) {
+			set_error_msg("cmb200_snapshot_begin: cannot start the writer thread");
+			rc = -1;
+		}
+	}
+	if (rc == 0) return s;
+	for (cmb200_engine *e : order) snap_set_state(e, cmb200_engine::SNAP_FREE);
+	fclose(s->f);
+	remove(s->tmp.c_str());
+	delete s;
+	return nullptr;
+}
+
+extern "C" int cmb200_snapshot_finish(cmb200_snapshot *s, uint64_t *records_out) {
+	if (!s) { set_error_msg("cmb200_snapshot_finish: no snapshot"); return -1; }
+	s->writer.join();
+	const std::string path = s->tmp.substr(0, s->tmp.size() - 4);
+	int rc = 0;
+	if (s->rc != 0) {
+		set_error_msg(s->err.c_str());
+		rc = -1;
+	} else if (rename(s->tmp.c_str(), path.c_str()) != 0) {
+		set_error_msg("cmb200_save: write failed");
+		rc = -1;
+	}
+	if (rc) remove(s->tmp.c_str());
+	else if (records_out) *records_out = s->h.records;
+	delete s;
+	return rc;
+}
+
+extern "C" int cmb200_save_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out) {
+	cmb200_snapshot *s = cmb200_snapshot_begin(engines, g, path);
+	return s ? cmb200_snapshot_finish(s, records_out) : -1;
 }
 
 extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records_out) {
@@ -1345,6 +1461,7 @@ extern "C" int cmb200_copy_peer(cmb200_engine *dst_e, void *dst_dev, cmb200_engi
 // to overflow although a good part of it is garbage (filemap_make_room, cmb200_compact).
 // (e->mu held)
 static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
+	snap_wait_written(e);                                // records move over listed ones; small gets go on meanwhile
 	cmb200_engine::GateClosed gg(e->get_gate);          // records move: no small get may be reading the arena
 	harvest_pending(e, true);
 	unsigned long long c[8];
@@ -1541,7 +1658,10 @@ static int demote_group(cmb200_engine *e, const std::vector<DemoteEntry> &grp,
 		t.log.pop_front();
 	}
 	const bool overwrite = end > t.size;        // the region holds bytes of an earlier lap
-	if (overwrite) e->get_gate.close();          // no small get may be reading what is overwritten
+	if (overwrite) {
+		snap_wait_written(e);                    // nor a snapshot that has listed them
+		e->get_gate.close();                     // no small get may be reading what is overwritten
+	}
 	int rc = 0;
 	const size_t nr = ret.size() / 4;
 	if (nr > t.retire_cap) {

@@ -158,7 +158,9 @@ int cmb200_import_records_dev(cmb200_engine *e, size_t n_total, const void *reco
 /* Slides the live records to the start of the arena so that the space of deleted and outgrown
  * records (stats.arena_garbage, and the unused remainders of per-warp segments) can be allocated
  * again; *reclaimed_out = bytes by which stats.arena_used went down.  Blocks the engine while it
- * runs (HBM speed).  The cachemap layer calls it by itself when the arena is about to overflow. */
+ * runs (HBM speed).  The cachemap layer calls it by itself when the arena is about to overflow.
+ * While a snapshot's section of this engine is not written yet, it first waits for the writer
+ * (cmb200_snapshot_begin). */
 int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out);
 
 /* ---- snapshot: what makes the cache directory persistent (SURVEY.md §8 f3) --------------------
@@ -185,12 +187,29 @@ inline int cmb200_owner(uint64_t key, int g) { return (int)(((key >> 32) * (uint
 
 /* cmb200_save / cmb200_load over g engines that split the keys by cmb200_owner.  The file is the one
  * cmb200_save writes: one header, then the records of engine 0, 1, ...  Each engine's section is a
- * point-in-time copy of that engine (the engine is locked while it is written, the others are not);
- * the engines hold disjoint keys, so the union is a valid store.  cmb200_load_set reads the file once
- * and puts each record into engine cmb200_owner(key, g), whatever g the file was written with.
- * cmb200_save and cmb200_load are these calls with g = 1. */
+ * point-in-time copy of that engine (its records as they were when its list was taken, see
+ * cmb200_snapshot_begin); the engines hold disjoint keys, so the union is a valid store.
+ * cmb200_load_set reads the file once and puts each record into engine cmb200_owner(key, g), whatever g
+ * the file was written with.  cmb200_save_set is cmb200_snapshot_begin followed by
+ * cmb200_snapshot_finish; cmb200_save and cmb200_load are these calls with g = 1. */
 int cmb200_save_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out);
 int cmb200_load_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out);
+
+typedef struct cmb200_snapshot cmb200_snapshot;
+/* Starts a snapshot of g engines (the cmb200_save_set file, written to path.tmp).  Each engine is
+ * locked only while its live records (both tiers) are listed, after its stream has been synchronised,
+ * so every put enqueued before the call (asynchronous ones included) is in the list.  The listed
+ * records are then written by a thread of the snapshot while the engines keep serving.  The file holds
+ * exactly the records that were live when each engine's list was taken: puts, unsets, demotions and
+ * promotions after that do not change it.  Until an engine's section is written, the two operations
+ * that reuse record bytes (compaction, and a host-tier lap that overwrites records) wait for the
+ * writer.  Nothing else waits.  A begin on an engine whose previous snapshot is still writing waits for
+ * it.  Destroying an engine while a snapshot of it is open is a caller error, as destroying an engine
+ * whose peers are mapped is.  An engine may appear once per call.
+ * NULL on failure (cmb200_last_error); a failed begin leaves no file behind. */
+cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines, int g, const char *path);
+/* Waits for the writer, renames path.tmp to path (on failure removes it), frees s.  0 / -1. */
+int cmb200_snapshot_finish(cmb200_snapshot *s, uint64_t *records_out);
 
 /* Moves n pages of the engine's page size within the engine's device memory:
  * dst[dst_idx ? dst_idx[i] : i] = src[src_idx ? src_idx[i] : i] (one warp per page, 16-byte loads and
