@@ -22,6 +22,7 @@
 #include <new>
 #include <thread>
 #include <unordered_set>
+#include <utility>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -41,6 +42,106 @@ static void set_error_msg(const char *msg) { snprintf(g_err, sizeof(g_err), "%s"
 
 using namespace cmb;
 
+// ---- owners of CUDA resources ------------------------------------------------------------------
+// Each owner frees its resource in its destructor on the device it was made on, and leaves the
+// calling thread's current device as it found it: a load or a snapshot of several engines releases
+// one engine's buffers on a thread that often has another engine's device current.
+template <class H, cudaError_t (*Release)(H)>
+class Owned {
+public:
+	Owned() = default;
+	Owned(Owned &&o) noexcept { *this = std::move(o); }
+	Owned &operator=(Owned &&o) noexcept {
+		if (this != &o) { reset(); std::swap(h_, o.h_); std::swap(dev_, o.dev_); std::swap(bytes_, o.bytes_); }
+		return *this;
+	}
+	~Owned() { reset(); }
+	void reset() {
+		if (!h_) return;
+		int cur = dev_;
+		cudaGetDevice(&cur);
+		if (cur != dev_) cudaSetDevice(dev_);
+		Release(h_);
+		if (cur != dev_) cudaSetDevice(cur);
+		h_ = nullptr; bytes_ = 0;
+	}
+	H get() const { return h_; }
+protected:
+	int adopt(H h, size_t bytes = 0) {                   // h was just made on the current device
+		reset();
+		h_ = h; bytes_ = bytes;
+		cudaGetDevice(&dev_);
+		return 0;
+	}
+	H h_ = nullptr;
+	int dev_ = 0;
+	size_t bytes_ = 0;
+};
+
+template <class T = uint8_t>
+struct DevMem : Owned<void *, cudaFree> {
+	operator T *() const { return (T *)h_; }
+	int alloc(size_t bytes) {
+		reset();                                         // first: the old and the new never coexist
+		void *p;
+		CMB_CHECK(cudaMalloc(&p, bytes));
+		return adopt(p, bytes);
+	}
+	// Scratch kept across calls: grown to the largest request, never shrunk (a cudaFree per call would
+	// synchronise the whole device); the work on `st` that may still read it is waited for first.
+	int grow(size_t bytes, cudaStream_t st) {
+		if (bytes <= bytes_) return 0;
+		CMB_CHECK(cudaStreamSynchronize(st));
+		return alloc(bytes);
+	}
+};
+
+template <class T = uint8_t>
+struct HostMem : Owned<void *, cudaFreeHost> {            // page-locked
+	operator T *() const { return (T *)h_; }
+	int alloc(size_t bytes, bool mapped = false) {
+		void *p;
+		CMB_CHECK(cudaHostAlloc(&p, bytes, mapped ? cudaHostAllocMapped : cudaHostAllocDefault));
+		return adopt(p);
+	}
+};
+
+struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
+	operator cudaStream_t() const { return h_; }
+	int create() { cudaStream_t s; CMB_CHECK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); return adopt(s); }
+};
+
+struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
+	operator cudaEvent_t() const { return h_; }
+	int create(unsigned flags) { cudaEvent_t ev; CMB_CHECK(cudaEventCreateWithFlags(&ev, flags)); return adopt(ev); }
+};
+
+// The key table's memory: cap + 2 slots and the side tables the engine's flags call for.  The kernels
+// get it as a TableView, refreshed by view() whenever the table is replaced.
+struct TableMem {
+	DevMem<Slot> slots;
+	DevMem<uint64_t> fp;
+	DevMem<uint32_t> fp_tag, ckpt;
+	void view(TableView &t) const { t.slots = slots; t.fp = fp; t.fp_tag = fp_tag; t.ckpt = ckpt; }
+};
+
+// Allocates the slots and each side table asked for, zeroed on st.  0 = done; 1 = a table found no
+// room (error set, CUDA's cleared; m is left empty); -1 = another CUDA call failed (error set).
+static int table_alloc(TableMem &m, uint64_t cap, bool fp, bool fp_tag, bool ckpt, cudaStream_t st) {
+	const size_t n = cap + 2;
+	if (m.slots.alloc(n * sizeof(Slot)) || (fp && m.fp.alloc(n * 16)) || (fp_tag && m.fp_tag.alloc(n * 4)) ||
+	    (ckpt && m.ckpt.alloc(n * CKPT_WORDS * 4))) {
+		(void)cudaGetLastError();
+		m = TableMem{};
+		return 1;
+	}
+	CMB_CHECK(cudaMemsetAsync(m.slots, 0, n * sizeof(Slot), st));
+	if (fp) CMB_CHECK(cudaMemsetAsync(m.fp, 0, n * 16, st));
+	if (fp_tag) CMB_CHECK(cudaMemsetAsync(m.fp_tag, 0, n * 4, st));
+	if (ckpt) CMB_CHECK(cudaMemsetAsync(m.ckpt, 0, n * CKPT_WORDS * 4, st));
+	return 0;
+}
+
 struct cmb200_engine {
 	int device = 0;
 	int pshift = 16;
@@ -50,7 +151,7 @@ struct cmb200_engine {
 	uint32_t max_batch = 4096;   // chunks per kernel launch (stage buffer size)
 	uint32_t host_batch = 4096;  // chunks per H2D/D2H pipeline step (page ring size), <= max_batch
 	uint32_t flags = 0;
-	cudaStream_t st = nullptr, copy = nullptr;
+	Stream st, copy;
 	// small gets (cmb200_get_small) have their own stream, lock and buffers: they neither queue behind
 	// a put batch on `st` nor take `mu`
 	// Several small gets may be in flight at once (two leader threads of the combining queue, or any
@@ -58,7 +159,7 @@ struct cmb200_engine {
 	// words — and the open side of get_gate; what moves records or peer mappings (compaction, peers,
 	// destroy) closes get_gate.
 	static constexpr int GET_LANES = 32;
-	struct GetLane { std::atomic<int> busy{0}; cudaStream_t st = nullptr; int32_t *h_status = nullptr; cmb200_addr *h_addr = nullptr; };
+	struct GetLane { std::atomic<int> busy{0}; Stream st; HostMem<int32_t> h_status; HostMem<cmb200_addr> h_addr; };
 	GetLane lane[GET_LANES];
 	// A small get may be begun by one thread and ended by another (cmb200_get_small_begin / _end), so
 	// the "no small get in flight" condition is a counter and a closing flag, not a lock a thread owns.
@@ -90,46 +191,47 @@ struct cmb200_engine {
 	const uint8_t *peer_base[GET_MAX_PEERS] = {};
 	uint64_t peer_size[GET_MAX_PEERS] = {};
 	std::atomic<uint64_t> small_get_requests{0}, small_get_hits{0}, small_get_launches{0};
-	unsigned long long *d_recoff_out = nullptr;  // arena offset per chunk of the current put slice (exchange records)
+	DevMem<unsigned long long> d_recoff_out;     // arena offset per chunk of the current put slice (exchange records)
 	// k_get_small's sequence descriptors: one scratch region per CTA that can be resident (kernels.cu:gs_region_take)
-	uint4 *d_scratch = nullptr;
-	uint32_t *d_pool_bits = nullptr;
+	DevMem<uint4> d_scratch;
+	DevMem<uint32_t> d_pool_bits;
 	uint32_t pool_n = 0, region_entries = 0;
-	cudaEvent_t landed[2] = {nullptr, nullptr}, consumed[2] = {nullptr, nullptr};
+	Event landed[2], consumed[2];
+	TableMem table_mem;
 	TableView table{};
+	DevMem<uint8_t> arena_base;
+	DevMem<unsigned long long> arena_seg;
 	ArenaView arena{};
-	unsigned long long *d_counters = nullptr;   // entries, tombs, head, garbage, dropped
-	uint8_t *d_pages[2] = {nullptr, nullptr};
-	uint8_t *d_stage = nullptr;
+	DevMem<unsigned long long> d_counters;      // entries, tombs, head, garbage, dropped
+	DevMem<uint8_t> d_pages[2];
+	DevMem<uint8_t> d_stage;
 	uint64_t stage_stride = 0;
-	unsigned long long *d_addr = nullptr, *d_ts = nullptr;
-	uint8_t *d_valid = nullptr;
-	uint32_t *d_slot = nullptr, *d_vlen = nullptr;
-	int32_t *d_lens = nullptr, *d_status = nullptr;
-	uint64_t *d_fps = nullptr, *d_recoff = nullptr;
-	unsigned int *d_work = nullptr;
-	uint32_t *d_order = nullptr;         // the encoder's longest-first chunk lists (encode_order_words(max_batch))
-	uint32_t *d_import_slot = nullptr;   // slot scratch of cmb200_import_records_dev
-	size_t import_slot_cap = 0;
-	uint32_t *d_move_idx = nullptr;      // index scratch of cmb200_move_pages (2 x move_idx_cap), grown, never shrunk
-	size_t move_idx_cap = 0;
+	DevMem<unsigned long long> d_addr, d_ts;
+	DevMem<uint8_t> d_valid;
+	DevMem<uint32_t> d_slot, d_vlen;
+	DevMem<int32_t> d_lens, d_status;
+	DevMem<uint64_t> d_fps, d_recoff;
+	DevMem<unsigned int> d_work;
+	DevMem<uint32_t> d_order;            // the encoder's longest-first chunk lists (encode_order_words(max_batch))
+	DevMem<uint32_t> d_import_slot;      // slot scratch of cmb200_import_records_dev, grown, never shrunk
+	DevMem<uint32_t> d_move_idx;         // index scratch of cmb200_move_pages (destination, then source), grown, never shrunk
 	// page-locked staging for the small per-chunk arrays, so that no copy ever blocks the host
 	// thread that is feeding the pipeline (a pageable cudaMemcpyAsync waits for the stream)
 	static constexpr size_t META_CAP = 1u << 18;   // chunks per outer slice of a call
-	uint8_t *h_meta = nullptr;                     // META_CAP x (16 addr + 8 ts + 4 lens + 4 status + 1 valid)
+	HostMem<uint8_t> h_meta;                       // META_CAP x (16 addr + 8 ts + 4 lens + 4 status + 1 valid)
 	unsigned long long seq = 1;          // sequence of the next chunk
 	unsigned long long seq_stride = 1;   // > 1 when the global stream is sharded round-robin over ranks
 	// per-launch device timing of the dominant kernels (roofline evidence for bench.py)
 	static constexpr int RING = 64;
-	cudaEvent_t t0[RING] = {}, t1[RING] = {};
+	Event t0[RING], t1[RING];
 	// asynchronous puts (cmb200_put_batch_async): kernel timing events not harvested yet are
 	// p0/p1[pend_tail .. pend_head), completion tickets are events on the compute stream
-	cudaEvent_t p0[RING] = {}, p1[RING] = {};
+	Event p0[RING], p1[RING];
 	uint64_t pend_head = 0, pend_tail = 0;
 	static constexpr int TICKETS = 8;
-	cudaEvent_t ticket_ev[TICKETS] = {};
+	Event ticket_ev[TICKETS];
 	uint64_t tickets = 0;
-	cudaEvent_t meta_done = nullptr, meta_free[2] = {nullptr, nullptr};
+	Event meta_done, meta_free[2];
 	uint64_t ring_pos = 0;               // page ring buffer in turn, kept across calls
 	uint64_t meta_pos = 0;               // same for the two copies of d_addr / d_ts / d_valid (host puts)
 	size_t meta_cap = 0;                 // entries per copy
@@ -138,27 +240,26 @@ struct cmb200_engine {
 	// host tier: a ring of records in demotion order.  Log position p lies at tier offset p % size; a
 	// record never straddles the end of the ring (the rest of the lap is skipped).
 	struct HostTier {
-		uint8_t *host = nullptr;             // cudaHostAlloc(mapped); null = no tier
+		HostMem<uint8_t> host;               // mapped; null = no tier
 		uint8_t *dev = nullptr;              // its device address
 		uint64_t size = 0;
 		uint64_t head = 0;                   // log position of the next record
 		std::deque<std::pair<uint64_t, uint32_t>> log;   // {position, bytes} of each record not yet overwritten, oldest first
 		uint64_t demoted_records = 0, demoted_bytes = 0;
 		uint64_t promoted_records = 0, promoted_bytes = 0;
-		unsigned long long *d_ctr = nullptr; // device: [0] records retired by wrap-around, [1] host-tier hits,
+		DevMem<unsigned long long> d_ctr;    // device: [0] records retired by wrap-around, [1] host-tier hits,
 		                                     // [2] head of the hot log
-		ulonglong2 *d_hot = nullptr;         // the hot log: HOT_LOG_N addresses of tier hits
+		DevMem<ulonglong2> d_hot;            // the hot log: HOT_LOG_N addresses of tier hits
 		uint64_t hot_drained = 0;            // hot-log head at the last cmb200_host_tier_hot
-		unsigned long long *d_retire = nullptr;   // {u, l, location, bytes} per record a wrap overwrites
-		size_t retire_cap = 0;
-		DemoteEntry *d_moves = nullptr;      // max_batch entries
-		PromoteEntry *d_promote = nullptr;   // max_batch entries
+		DevMem<unsigned long long> d_retire; // {u, l, location, bytes} per record a wrap overwrites, grown, never shrunk
+		DevMem<DemoteEntry> d_moves;         // max_batch entries
+		DevMem<PromoteEntry> d_promote;      // max_batch entries
 		HotLog hot() const { return HotLog{d_ctr ? d_ctr + 2 : nullptr, d_hot}; }
 	} tier;
 	std::atomic<bool> multi_gpu{false};  // a multi-GPU call was made: no host tier from then on
 	// CMB200_VERIFY: device counters, VS_WORDS of the gets, then VS_WORDS of the running store scan
-	unsigned long long *d_vstat = nullptr;
-	uint32_t *d_vidx = nullptr;          // slot of each request of a verified get batch (max_batch)
+	DevMem<unsigned long long> d_vstat;
+	DevMem<uint32_t> d_vidx;             // slot of each request of a verified get batch (max_batch)
 	uint64_t scanned = 0, scan_corrupt = 0;
 	// snapshots (cmb200_snapshot_begin): SNAP_FREE, SNAP_CLAIMED by a snapshot that has not listed this
 	// engine's records yet, or SNAP_PENDING: listed, section not written yet.  snap_state changes under
@@ -168,18 +269,9 @@ struct cmb200_engine {
 	int snap_state = SNAP_FREE;
 	std::mutex snap_mu;
 	std::condition_variable snap_cv;
-	uint8_t *snap_win = nullptr;         // page-locked window of the writer, kept from the first snapshot on
-	cudaStream_t snap_st = nullptr;      // the writer's copies: they do not queue behind encodes on st
+	HostMem<uint8_t> snap_win;           // page-locked window of the writer, kept from the first snapshot on
+	Stream snap_st;                      // the writer's copies: they do not queue behind encodes on st
 };
-
-#define ENG_CHECK(expr)                                                 \
-	do {                                                            \
-		cudaError_t e_ = (expr);                                \
-		if (e_ != cudaSuccess) {                                \
-			cmb_set_error(#expr, e_, __FILE__, __LINE__);   \
-			goto fail;                                      \
-		}                                                       \
-	} while (0)
 
 static uint64_t next_pow2(uint64_t v) {
 	uint64_t p = 1;
@@ -209,49 +301,12 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	cudaSetDevice(e->device);
 	if (e->st) cudaStreamSynchronize(e->st);
 	if (e->copy) cudaStreamSynchronize(e->copy);
-	cudaFree(e->d_scratch); cudaFree(e->d_pool_bits); cudaFree(e->table.ckpt); cudaFree(e->table.fp_tag);
-	cudaFree(e->d_vstat); cudaFree(e->d_vidx);
-	cudaFree(e->table.slots); cudaFree(e->table.fp); cudaFree(e->arena.base); cudaFree(e->arena.seg); cudaFree(e->d_counters);
-	cudaFree(e->d_pages[0]); cudaFree(e->d_pages[1]); cudaFree(e->d_stage);
-	cudaFree(e->d_addr); cudaFree(e->d_ts); cudaFree(e->d_valid); cudaFree(e->d_slot); cudaFree(e->d_vlen);
-	cudaFree(e->d_move_idx);
-	if (e->h_meta) cudaFreeHost(e->h_meta);
-	for (auto &ln : e->lane) {
-		if (ln.st) { cudaStreamSynchronize(ln.st); cudaStreamDestroy(ln.st); }
-		if (ln.h_status) cudaFreeHost(ln.h_status);
-		if (ln.h_addr) cudaFreeHost(ln.h_addr);
-	}
-	cudaFree(e->d_recoff_out);
+	for (auto &ln : e->lane) if (ln.st) cudaStreamSynchronize(ln.st);
 	for (int r = 0; r < GET_MAX_PEERS; r++) if (e->peer_base[r]) cudaIpcCloseMemHandle((void *)e->peer_base[r]);
-	if (e->tier.host) cudaFreeHost(e->tier.host);
-	cudaFree(e->tier.d_ctr); cudaFree(e->tier.d_retire); cudaFree(e->tier.d_moves);
-	cudaFree(e->tier.d_promote); cudaFree(e->tier.d_hot);
-	cudaFree(e->d_lens); cudaFree(e->d_status); cudaFree(e->d_fps); cudaFree(e->d_recoff); cudaFree(e->d_work); cudaFree(e->d_order); cudaFree(e->d_import_slot);
-	for (int i = 0; i < 2; i++) {
-		if (e->landed[i]) cudaEventDestroy(e->landed[i]);
-		if (e->consumed[i]) cudaEventDestroy(e->consumed[i]);
-	}
-	for (int i = 0; i < cmb200_engine::RING; i++) {
-		if (e->t0[i]) cudaEventDestroy(e->t0[i]);
-		if (e->t1[i]) cudaEventDestroy(e->t1[i]);
-		if (e->p0[i]) cudaEventDestroy(e->p0[i]);
-		if (e->p1[i]) cudaEventDestroy(e->p1[i]);
-	}
-	for (int i = 0; i < cmb200_engine::TICKETS; i++) if (e->ticket_ev[i]) cudaEventDestroy(e->ticket_ev[i]);
-	if (e->meta_done) cudaEventDestroy(e->meta_done);
-	for (int i = 0; i < 2; i++) if (e->meta_free[i]) cudaEventDestroy(e->meta_free[i]);
-	if (e->snap_win) cudaFreeHost(e->snap_win);
-	if (e->snap_st) cudaStreamDestroy(e->snap_st);
-	if (e->st) cudaStreamDestroy(e->st);
-	if (e->copy) cudaStreamDestroy(e->copy);
 	delete e;
 }
 
-extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
-	if (!cfg || cfg->pshift < 6 || cfg->pshift > 20) { set_error_msg("bad config: pshift must be 6..20"); return nullptr; }
-	if (select_device(cfg->device) != 0) return nullptr;
-	cmb200_engine *e = new (std::nothrow) cmb200_engine();
-	if (!e) return nullptr;
+static int engine_init(cmb200_engine *e, const cmb200_config *cfg) {
 	cudaGetDevice(&e->device);
 	e->pshift = cfg->pshift;
 	e->bsize = 1u << cfg->pshift;
@@ -264,137 +319,117 @@ extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
 	e->flags = cfg->flags;
 	if (e->flags & CMB200_VERIFY) e->flags |= CMB200_FINGERPRINT;
 	const uint64_t B = e->max_batch;
-	{
-		uint64_t slots = cfg->table_slots ? next_pow2(cfg->table_slots) : next_pow2(4 * (cfg->capacity ? cfg->capacity : 1024));
-		if (slots < 1024) slots = 1024;
-		if (slots > (1ull << 27)) slots = 1ull << 27;
-		e->table.cap = slots;
-		ENG_CHECK(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
-		ENG_CHECK(cudaStreamCreateWithFlags(&e->copy, cudaStreamNonBlocking));
-		for (auto &ln : e->lane) ENG_CHECK(cudaStreamCreateWithFlags(&ln.st, cudaStreamNonBlocking));
-		for (int i = 0; i < 2; i++) {
-			ENG_CHECK(cudaEventCreateWithFlags(&e->landed[i], cudaEventDisableTiming));
-			ENG_CHECK(cudaEventCreateWithFlags(&e->consumed[i], cudaEventDisableTiming));
-		}
-		for (int i = 0; i < cmb200_engine::RING; i++) {
-			ENG_CHECK(cudaEventCreate(&e->t0[i]));
-			ENG_CHECK(cudaEventCreate(&e->t1[i]));
-			ENG_CHECK(cudaEventCreate(&e->p0[i]));
-			ENG_CHECK(cudaEventCreate(&e->p1[i]));
-		}
-		for (int i = 0; i < cmb200_engine::TICKETS; i++)
-			ENG_CHECK(cudaEventCreateWithFlags(&e->ticket_ev[i], cudaEventDisableTiming));
-		ENG_CHECK(cudaEventCreateWithFlags(&e->meta_done, cudaEventDisableTiming));
-		ENG_CHECK(cudaEventCreateWithFlags(&e->meta_free[0], cudaEventDisableTiming));
-		ENG_CHECK(cudaEventCreateWithFlags(&e->meta_free[1], cudaEventDisableTiming));
-		ENG_CHECK(cudaMalloc(&e->table.slots, (slots + 2) * sizeof(Slot)));
-		ENG_CHECK(cudaMemsetAsync(e->table.slots, 0, (slots + 2) * sizeof(Slot), e->st));
-		if (e->flags & CMB200_FINGERPRINT) {
-			ENG_CHECK(cudaMalloc(&e->table.fp, (slots + 2) * 16));
-			ENG_CHECK(cudaMemsetAsync(e->table.fp, 0, (slots + 2) * 16, e->st));
-		}
-		if (e->flags & CMB200_VERIFY) {
-			ENG_CHECK(cudaMalloc(&e->table.fp_tag, (slots + 2) * 4));
-			ENG_CHECK(cudaMemsetAsync(e->table.fp_tag, 0, (slots + 2) * 4, e->st));
-			ENG_CHECK(cudaMalloc(&e->d_vstat, 2 * VS_WORDS * sizeof(unsigned long long)));
-			ENG_CHECK(cudaMemsetAsync(e->d_vstat, 0, 2 * VS_WORDS * sizeof(unsigned long long), e->st));
-			ENG_CHECK(cudaMalloc(&e->d_vidx, B * 4));
-		}
-		if (get_small_supports(e->bsize)) {
-			// parse checkpoints per slot (64 bytes) and the descriptor scratch of the fused single-page get
-			const char *ck = getenv("CMB200_CKPT");
-			if (!ck || atoi(ck) != 0) {
-				ENG_CHECK(cudaMalloc(&e->table.ckpt, (slots + 2) * CKPT_WORDS * 4));
-				ENG_CHECK(cudaMemsetAsync(e->table.ckpt, 0, (slots + 2) * CKPT_WORDS * 4, e->st));
-			}
-			const int resident = get_small_residency(e->bsize, e->table.fp_tag != nullptr);
-			if (resident <= 0) { set_error_msg("k_get_small does not fit this device"); goto fail; }
-			e->pool_n = (uint32_t)resident;
-			e->region_entries = get_small_region_entries(e->bsize);
-			ENG_CHECK(cudaMalloc(&e->d_scratch, (size_t)e->pool_n * e->region_entries * sizeof(uint4)));
-			ENG_CHECK(cudaMalloc(&e->d_pool_bits, ((size_t)e->pool_n + 31) / 32 * 4));
-			ENG_CHECK(cudaMemsetAsync(e->d_pool_bits, 0, ((size_t)e->pool_n + 31) / 32 * 4, e->st));
-		}
-		ENG_CHECK(cudaMalloc(&e->d_counters, 8 * sizeof(unsigned long long)));
-		ENG_CHECK(cudaMemsetAsync(e->d_counters, 0, 8 * sizeof(unsigned long long), e->st));
-		e->table.entries = e->d_counters + 0;
-		e->table.tombs = e->d_counters + 1;
-		e->arena.head = e->d_counters + 2;
-		e->arena.garbage = e->d_counters + 3;
-		e->arena.dropped = e->d_counters + 4;
-		e->table.remote = e->d_counters + 5;
-		e->arena.tier = e->d_counters + 6;
-
-		// filemap.c:120 dest[bsize+1024], but never below LZ4_compressBound: the encoder has no output
-		// limit, and above 128 KiB pages an incompressible block is longer than bsize + 1024 (k_encode
-		// then stores the page raw, as LZ4_compress_fast's 0 would make filemap_set do)
-		{
-			const uint64_t bound = (uint64_t)e->bsize + e->bsize / 255 + 16;
-			const uint64_t row = (uint64_t)e->bsize + 1024 > bound ? (uint64_t)e->bsize + 1024 : bound;
-			e->stage_stride = (row + 15) & ~15ull;
-		}
-		ENG_CHECK(cudaMalloc(&e->d_pages[0], (uint64_t)e->host_batch * e->bsize + 256));
-		ENG_CHECK(cudaMalloc(&e->d_pages[1], (uint64_t)e->host_batch * e->bsize + 256));
-		// one stage row per resident warp / group of the encode kernels (store mode), not per chunk
-		ENG_CHECK(cudaMalloc(&e->d_stage, (uint64_t)16384 * e->stage_stride + 256));
-		// small per-chunk arrays are sized for a whole slice of a call (META_CAP chunks) so that
-		// they cross PCIe once, outside the page pipeline
-		const uint64_t M = cmb200_engine::META_CAP > B ? cmb200_engine::META_CAP : B;
-		// two copies: a host put stages the next call's arrays while the kernels of the previous
-		// one still read theirs (cmb200_put_batch_async)
-		e->meta_cap = M;
-		ENG_CHECK(cudaMalloc(&e->d_addr, 2 * M * 16));
-		ENG_CHECK(cudaMalloc(&e->d_ts, 2 * M * 8));
-		ENG_CHECK(cudaMalloc(&e->d_valid, 2 * M));
-		ENG_CHECK(cudaMalloc(&e->d_slot, B * 4));
-		ENG_CHECK(cudaMalloc(&e->d_vlen, B * 4));
-		ENG_CHECK(cudaMalloc(&e->d_lens, M * 4));
-		ENG_CHECK(cudaMalloc(&e->d_status, M * 4));
-		ENG_CHECK(cudaMalloc(&e->d_fps, B * 16));
-		ENG_CHECK(cudaMalloc(&e->d_recoff, B * 8));
-		ENG_CHECK(cudaMalloc(&e->d_work, 64));
-		ENG_CHECK(cudaMalloc(&e->d_order, encode_order_words((uint32_t)B) * 4));
-		ENG_CHECK(cudaMallocHost(&e->h_meta, cmb200_engine::META_CAP * 33));
-		for (auto &ln : e->lane) {
-			ENG_CHECK(cudaMallocHost(&ln.h_status, cmb200_engine::GET_SMALL_MAX * 4));
-			ENG_CHECK(cudaMallocHost(&ln.h_addr, cmb200_engine::GET_SMALL_MAX * 16));
-		}
-		ENG_CHECK(cudaMalloc(&e->d_recoff_out, M * 8));
-
-		uint64_t arena = cfg->arena_bytes;
-		if (!arena) {
-			size_t free_b = 0, total_b = 0;
-			ENG_CHECK(cudaMemGetInfo(&free_b, &total_b));
-			// capacity worst-case records (24 + a stage row: a stored record is never longer, since a
-			// block longer than bsize + 1024 is stored as the raw page) plus 1/8 headroom, so that a
-			// store at capacity still has garbage worth compacting
-			uint64_t want = (cfg->capacity ? cfg->capacity : 1024) * (e->stage_stride + 32);
-			want += want / 8;
-			uint64_t lim = (uint64_t)(free_b * 0.8);
-			arena = want < lim ? want : lim;
-		}
-		arena = (arena + 255) & ~255ull;
-		ENG_CHECK(cudaMalloc(&e->arena.base, arena + 256));
-		e->arena.size = arena;
-		{
-			// direct encode into per-warp arena segments when the arena is large enough that
-			// 4096 segments of >= 4 worst-case records stay a small part of it
-			// (CMB200_SEG_KB overrides: 0 = always through the stage buffer)
-			const uint64_t worst = (24 + e->stage_stride + 15) & ~15ull;
-			uint64_t seg = arena / (8ull * 2072ull);
-			if (seg > (2ull << 20)) seg = 2ull << 20;
-			if (seg < 4 * worst) seg = 0;
-			const char *kb = getenv("CMB200_SEG_KB");
-			if (kb && *kb) { seg = strtoull(kb, nullptr, 10) << 10; if (seg && seg < worst) seg = worst; }
-			seg = (seg + 255) & ~255ull;
-			e->arena.seg_bytes = (uint32_t)seg;
-			ENG_CHECK(cudaMalloc(&e->arena.seg, ARENA_SEG_SLOTS * 2 * sizeof(unsigned long long)));
-			ENG_CHECK(cudaMemsetAsync(e->arena.seg, 0, ARENA_SEG_SLOTS * 2 * sizeof(unsigned long long), e->st));
-		}
-		ENG_CHECK(cudaStreamSynchronize(e->st));
+	uint64_t slots = cfg->table_slots ? next_pow2(cfg->table_slots) : next_pow2(4 * (cfg->capacity ? cfg->capacity : 1024));
+	if (slots < 1024) slots = 1024;
+	if (slots > (1ull << 27)) slots = 1ull << 27;
+	e->table.cap = slots;
+	if (e->st.create() || e->copy.create()) return -1;
+	for (auto &ln : e->lane) if (ln.st.create()) return -1;
+	for (int i = 0; i < 2; i++)
+		if (e->landed[i].create(cudaEventDisableTiming) || e->consumed[i].create(cudaEventDisableTiming)) return -1;
+	for (int i = 0; i < cmb200_engine::RING; i++)
+		if (e->t0[i].create(cudaEventDefault) || e->t1[i].create(cudaEventDefault) ||
+		    e->p0[i].create(cudaEventDefault) || e->p1[i].create(cudaEventDefault)) return -1;
+	for (Event &ev : e->ticket_ev) if (ev.create(cudaEventDisableTiming)) return -1;
+	if (e->meta_done.create(cudaEventDisableTiming) || e->meta_free[0].create(cudaEventDisableTiming) ||
+	    e->meta_free[1].create(cudaEventDisableTiming)) return -1;
+	// parse checkpoints per slot (64 bytes) when the fused single-page get serves this page size
+	const char *ck = getenv("CMB200_CKPT");
+	const bool ckpt = get_small_supports(e->bsize) && (!ck || atoi(ck) != 0);
+	if (table_alloc(e->table_mem, slots, e->flags & CMB200_FINGERPRINT, e->flags & CMB200_VERIFY, ckpt, e->st)) return -1;
+	e->table_mem.view(e->table);
+	if (e->flags & CMB200_VERIFY) {
+		if (e->d_vstat.alloc(2 * VS_WORDS * sizeof(unsigned long long)) || e->d_vidx.alloc(B * 4)) return -1;
+		CMB_CHECK(cudaMemsetAsync(e->d_vstat, 0, 2 * VS_WORDS * sizeof(unsigned long long), e->st));
 	}
-	return e;
-fail:
+	if (get_small_supports(e->bsize)) {
+		// the descriptor scratch of the fused single-page get
+		const int resident = get_small_residency(e->bsize, e->table.fp_tag != nullptr);
+		if (resident <= 0) { set_error_msg("k_get_small does not fit this device"); return -1; }
+		e->pool_n = (uint32_t)resident;
+		e->region_entries = get_small_region_entries(e->bsize);
+		if (e->d_scratch.alloc((size_t)e->pool_n * e->region_entries * sizeof(uint4)) ||
+		    e->d_pool_bits.alloc(((size_t)e->pool_n + 31) / 32 * 4)) return -1;
+		CMB_CHECK(cudaMemsetAsync(e->d_pool_bits, 0, ((size_t)e->pool_n + 31) / 32 * 4, e->st));
+	}
+	if (e->d_counters.alloc(8 * sizeof(unsigned long long))) return -1;
+	CMB_CHECK(cudaMemsetAsync(e->d_counters, 0, 8 * sizeof(unsigned long long), e->st));
+	e->table.entries = e->d_counters + 0;
+	e->table.tombs = e->d_counters + 1;
+	e->arena.head = e->d_counters + 2;
+	e->arena.garbage = e->d_counters + 3;
+	e->arena.dropped = e->d_counters + 4;
+	e->table.remote = e->d_counters + 5;
+	e->arena.tier = e->d_counters + 6;
+
+	// filemap.c:120 dest[bsize+1024], but never below LZ4_compressBound: the encoder has no output
+	// limit, and above 128 KiB pages an incompressible block is longer than bsize + 1024 (k_encode
+	// then stores the page raw, as LZ4_compress_fast's 0 would make filemap_set do)
+	{
+		const uint64_t bound = (uint64_t)e->bsize + e->bsize / 255 + 16;
+		const uint64_t row = (uint64_t)e->bsize + 1024 > bound ? (uint64_t)e->bsize + 1024 : bound;
+		e->stage_stride = (row + 15) & ~15ull;
+	}
+	if (e->d_pages[0].alloc((uint64_t)e->host_batch * e->bsize + 256) ||
+	    e->d_pages[1].alloc((uint64_t)e->host_batch * e->bsize + 256)) return -1;
+	// one stage row per resident warp / group of the encode kernels (store mode), not per chunk
+	if (e->d_stage.alloc((uint64_t)16384 * e->stage_stride + 256)) return -1;
+	// small per-chunk arrays are sized for a whole slice of a call (META_CAP chunks) so that
+	// they cross PCIe once, outside the page pipeline
+	const uint64_t M = cmb200_engine::META_CAP > B ? cmb200_engine::META_CAP : B;
+	// two copies: a host put stages the next call's arrays while the kernels of the previous
+	// one still read theirs (cmb200_put_batch_async)
+	e->meta_cap = M;
+	if (e->d_addr.alloc(2 * M * 16) || e->d_ts.alloc(2 * M * 8) || e->d_valid.alloc(2 * M) ||
+	    e->d_slot.alloc(B * 4) || e->d_vlen.alloc(B * 4) || e->d_lens.alloc(M * 4) || e->d_status.alloc(M * 4) ||
+	    e->d_fps.alloc(B * 16) || e->d_recoff.alloc(B * 8) || e->d_work.alloc(64) ||
+	    e->d_order.alloc(encode_order_words((uint32_t)B) * 4) || e->h_meta.alloc(cmb200_engine::META_CAP * 33)) return -1;
+	for (auto &ln : e->lane)
+		if (ln.h_status.alloc(cmb200_engine::GET_SMALL_MAX * 4) || ln.h_addr.alloc(cmb200_engine::GET_SMALL_MAX * 16)) return -1;
+	if (e->d_recoff_out.alloc(M * 8)) return -1;
+
+	uint64_t arena = cfg->arena_bytes;
+	if (!arena) {
+		size_t free_b = 0, total_b = 0;
+		CMB_CHECK(cudaMemGetInfo(&free_b, &total_b));
+		// capacity worst-case records (24 + a stage row: a stored record is never longer, since a
+		// block longer than bsize + 1024 is stored as the raw page) plus 1/8 headroom, so that a
+		// store at capacity still has garbage worth compacting
+		uint64_t want = (cfg->capacity ? cfg->capacity : 1024) * (e->stage_stride + 32);
+		want += want / 8;
+		uint64_t lim = (uint64_t)(free_b * 0.8);
+		arena = want < lim ? want : lim;
+	}
+	arena = (arena + 255) & ~255ull;
+	if (e->arena_base.alloc(arena + 256)) return -1;
+	e->arena.base = e->arena_base;
+	e->arena.size = arena;
+	{
+		// direct encode into per-warp arena segments when the arena is large enough that
+		// 4096 segments of >= 4 worst-case records stay a small part of it
+		// (CMB200_SEG_KB overrides: 0 = always through the stage buffer)
+		const uint64_t worst = (24 + e->stage_stride + 15) & ~15ull;
+		uint64_t seg = arena / (8ull * 2072ull);
+		if (seg > (2ull << 20)) seg = 2ull << 20;
+		if (seg < 4 * worst) seg = 0;
+		const char *kb = getenv("CMB200_SEG_KB");
+		if (kb && *kb) { seg = strtoull(kb, nullptr, 10) << 10; if (seg && seg < worst) seg = worst; }
+		seg = (seg + 255) & ~255ull;
+		e->arena.seg_bytes = (uint32_t)seg;
+		if (e->arena_seg.alloc(ARENA_SEG_SLOTS * 2 * sizeof(unsigned long long))) return -1;
+		CMB_CHECK(cudaMemsetAsync(e->arena_seg, 0, ARENA_SEG_SLOTS * 2 * sizeof(unsigned long long), e->st));
+		e->arena.seg = e->arena_seg;
+	}
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	return 0;
+}
+
+extern "C" cmb200_engine *cmb200_engine_create(const cmb200_config *cfg) {
+	if (!cfg || cfg->pshift < 6 || cfg->pshift > 20) { set_error_msg("bad config: pshift must be 6..20"); return nullptr; }
+	if (select_device(cfg->device) != 0) return nullptr;
+	cmb200_engine *e = new (std::nothrow) cmb200_engine();
+	if (!e) return nullptr;
+	if (engine_init(e, cfg) == 0) return e;
 	cmb200_engine_destroy(e);
 	return nullptr;
 }
@@ -468,7 +503,7 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 	const bool copy_meta = !pages_on_dev || deferred;      // small arrays travel on the copy stream
 	const unsigned long long seq_first = e->seq;
 	// stage the small arrays in page-locked memory once; every copy below is then truly async
-	cmb200_addr *h_addr = (cmb200_addr *)e->h_meta;
+	cmb200_addr *h_addr = (cmb200_addr *)e->h_meta.get();
 	uint64_t *h_ts = (uint64_t *)(e->h_meta + cmb200_engine::META_CAP * 16);
 	int32_t *h_lens = (int32_t *)(e->h_meta + cmb200_engine::META_CAP * 24);
 	uint8_t *h_valid = e->h_meta + cmb200_engine::META_CAP * 32;
@@ -523,7 +558,7 @@ static int put_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		job.stage = e->d_stage; job.stage_stride = e->stage_stride;
 		job.lens = e->d_lens + at;
 		job.rec_out = e->d_recoff_out + at;
-		job.fps = (e->flags & CMB200_FINGERPRINT) ? e->d_fps : nullptr;
+		job.fps = (e->flags & CMB200_FINGERPRINT) ? (uint64_t *)e->d_fps : nullptr;
 		job.work = e->d_work;
 		job.order = e->d_order;
 		job.slot_idx = e->d_slot;
@@ -643,13 +678,7 @@ extern "C" int cmb200_import_records_dev(cmb200_engine *e, size_t n_total, const
 	if (n_total == 0) return 0;
 	if (n_total > 0xffffffffull) { set_error_msg("cmb200_import_records_dev: too many records"); return -1; }
 	// the whole gathered buffer in one claim + one apply launch (the slot scratch grows on demand)
-	if (n_total > e->import_slot_cap) {
-		CMB_CHECK(cudaStreamSynchronize(e->st));
-		if (e->d_import_slot) cudaFree(e->d_import_slot);
-		e->d_import_slot = nullptr; e->import_slot_cap = 0;
-		CMB_CHECK(cudaMalloc(&e->d_import_slot, n_total * sizeof(uint32_t)));
-		e->import_slot_cap = n_total;
-	}
+	if (e->d_import_slot.grow(n_total * sizeof(uint32_t), e->st)) return -1;
 	if (launch_import_records(e->table, e->arena, (const unsigned long long *)records_dev, (uint32_t)n_total, my_rank,
 		e->d_import_slot, e->st)) return -1;
 	e->stats.kernel_launches += 2;
@@ -679,7 +708,7 @@ extern "C" int cmb200_put_batch_dev(cmb200_engine *e, size_t n, const cmb200_add
 static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     uint8_t *pages_out, bool out_on_dev, int32_t *status_out) {
 	const size_t B = out_on_dev ? e->max_batch : e->host_batch;
-	cmb200_addr *h_addr = (cmb200_addr *)e->h_meta;
+	cmb200_addr *h_addr = (cmb200_addr *)e->h_meta.get();
 	int32_t *h_status = (int32_t *)(e->h_meta + cmb200_engine::META_CAP * 28);
 	uint8_t *h_valid = e->h_meta + cmb200_engine::META_CAP * 32;
 	memcpy(h_addr, addr, n * 16);
@@ -825,7 +854,7 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	GetJob job{};
 	job.table = e->table; job.arena = e->arena.base; job.arena_size = e->arena.size;
 	job.host = e->tier.dev; job.host_size = e->tier.size; job.host_hits = e->tier.d_ctr + 1;
-	job.addr = (const unsigned long long *)ln->h_addr; job.valid = nullptr; job.n = (uint32_t)n; job.nbytes = e->bsize;
+	job.addr = (const unsigned long long *)ln->h_addr.get(); job.valid = nullptr; job.n = (uint32_t)n; job.nbytes = e->bsize;
 	job.out = (uint8_t *)pages_out;                          // device memory or page-locked host memory (UVA)
 	job.status = ln->h_status;
 	for (int r = 0; r < GET_MAX_PEERS; r++) { job.peer[r] = e->peer_base[r]; job.peer_size[r] = e->peer_size[r]; }
@@ -982,7 +1011,7 @@ extern "C" int cmb200_sample(cmb200_engine *e, size_t n, const uint64_t *r, cmb2
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
 		CMB_CHECK(cudaMemcpyAsync(e->d_recoff, r + at, (size_t)m * 8, cudaMemcpyHostToDevice, e->st));
-		if (launch_sample(e->table, (const unsigned long long *)e->d_recoff, m, e->d_addr, e->d_ts, e->d_status, e->st)) return -1;
+		if (launch_sample(e->table, (const unsigned long long *)e->d_recoff.get(), m, e->d_addr, e->d_ts, e->d_status, e->st)) return -1;
 		CMB_CHECK(cudaMemcpyAsync(addr_out + at, e->d_addr, (size_t)m * 16, cudaMemcpyDeviceToHost, e->st));
 		CMB_CHECK(cudaMemcpyAsync(ts_out + at, e->d_ts, (size_t)m * 8, cudaMemcpyDeviceToHost, e->st));
 		CMB_CHECK(cudaMemcpyAsync(ok_out + at, e->d_status, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
@@ -1033,13 +1062,6 @@ extern "C" int cmb200_read_fingerprints(cmb200_engine *e, size_t n, const cmb200
 	return 0;
 }
 
-struct DevBuf {
-	void *p = nullptr;
-	~DevBuf() { if (p) cudaFree(p); }
-	int alloc(size_t bytes) { CMB_CHECK(cudaMalloc(&p, bytes + 256)); return 0; }
-	template <class T> T *as() { return (T *)p; }
-};
-
 extern "C" int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint32_t *words_out,
     int32_t *ok_out) {
 	std::lock_guard<std::mutex> g(e->mu);
@@ -1049,13 +1071,13 @@ extern "C" int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_
 		for (size_t i = 0; i < n; i++) ok_out[i] = -1;
 		return 0;
 	}
-	DevBuf d_words;
-	if (n && d_words.alloc((size_t)e->max_batch * CKPT_WORDS * 4)) return -1;
+	DevMem<uint32_t> d_words;
+	if (n && d_words.alloc((size_t)e->max_batch * CKPT_WORDS * 4 + 256)) return -1;
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
 		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
-		if (launch_read_ckpt(e->table, e->d_addr, m, d_words.as<uint32_t>(), e->d_status, e->st)) return -1;
-		CMB_CHECK(cudaMemcpyAsync(words_out + at * CKPT_WORDS, d_words.p, (size_t)m * CKPT_WORDS * 4, cudaMemcpyDeviceToHost, e->st));
+		if (launch_read_ckpt(e->table, e->d_addr, m, d_words, e->d_status, e->st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(words_out + at * CKPT_WORDS, d_words, (size_t)m * CKPT_WORDS * 4, cudaMemcpyDeviceToHost, e->st));
 		CMB_CHECK(cudaMemcpyAsync(ok_out + at, e->d_status, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
 		CMB_CHECK(cudaStreamSynchronize(e->st));
 	}
@@ -1069,18 +1091,18 @@ extern "C" int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_
 static int live_records(cmb200_engine *e, bool arena_only, std::vector<ExportEntry> &list, unsigned long long c[8]) {
 	if (read_counters(e, c)) return -1;
 	const unsigned long long cap_out = c[0] + 16;
-	DevBuf d_list, d_count;
-	if (d_list.alloc(cap_out * sizeof(ExportEntry)) || d_count.alloc(8)) return -1;
-	CMB_CHECK(cudaMemsetAsync(d_count.p, 0, 8, e->st));
-	if (launch_export_list(e->table, e->bsize, d_list.as<ExportEntry>(), d_count.as<unsigned long long>(), cap_out,
-		arena_only, e->st)) return -1;
+	DevMem<ExportEntry> d_list;
+	DevMem<unsigned long long> d_count;
+	if (d_list.alloc(cap_out * sizeof(ExportEntry) + 256) || d_count.alloc(8 + 256)) return -1;
+	CMB_CHECK(cudaMemsetAsync(d_count, 0, 8, e->st));
+	if (launch_export_list(e->table, e->bsize, d_list, d_count, cap_out, arena_only, e->st)) return -1;
 	unsigned long long count = 0;
-	CMB_CHECK(cudaMemcpyAsync(&count, d_count.p, 8, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaMemcpyAsync(&count, d_count, 8, cudaMemcpyDeviceToHost, e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
 	const int over = count > cap_out;
 	if (over) count = cap_out;
 	list.resize(count);
-	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list.p, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
+	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
 	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
 	return over;
 }
@@ -1221,8 +1243,7 @@ extern "C" cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines,
 	for (cmb200_engine *e : order) {
 		// allocated once: cudaFreeHost may synchronise the device
 		if (cudaSetDevice(e->device) != cudaSuccess ||
-		    (!e->snap_win && cudaMallocHost(&e->snap_win, SNAP_WINDOW) != cudaSuccess) ||
-		    (!e->snap_st && cudaStreamCreateWithFlags(&e->snap_st, cudaStreamNonBlocking) != cudaSuccess)) {
+		    (!e->snap_win && e->snap_win.alloc(SNAP_WINDOW)) || (!e->snap_st && e->snap_st.create())) {
 			cmb_set_error("cmb200_snapshot_begin: no page-locked window or stream", cudaGetLastError(), __FILE__, __LINE__);
 			rc = -1;
 			break;
@@ -1291,29 +1312,19 @@ static int demote_arena_all(cmb200_engine *e);
 // (<= max_batch records and <= one page-ring buffer of bytes), then put in as one upsert + k_restore.
 struct LoadBatch {
 	cmb200_engine *e = nullptr;
-	uint8_t *blob = nullptr;
+	HostMem<uint8_t> blob;
 	size_t cap = 0, B = 0, used = 0, m = 0;
 	std::vector<unsigned long long> off, ts, fps;
 	std::vector<cmb200_addr> addr;
-	unsigned long long *d_off = nullptr;
-	uint64_t *d_fp = nullptr;
+	DevMem<unsigned long long> d_off;
+	DevMem<uint64_t> d_fp;
 	int setup(cmb200_engine *eng) {
 		e = eng;
 		CMB_CHECK(cudaSetDevice(e->device));
 		cap = (size_t)e->host_batch * e->bsize;
 		B = e->max_batch < cmb200_engine::META_CAP ? e->max_batch : cmb200_engine::META_CAP;
 		off.resize(B); ts.resize(B); fps.resize(2 * B); addr.resize(B);
-		CMB_CHECK(cudaMallocHost(&blob, cap));
-		CMB_CHECK(cudaMalloc(&d_off, B * 8));
-		CMB_CHECK(cudaMalloc(&d_fp, B * 16));
-		return 0;
-	}
-	void release() {
-		if (!e) return;
-		cudaSetDevice(e->device);
-		if (blob) cudaFreeHost(blob);
-		if (d_off) cudaFree(d_off);
-		if (d_fp) cudaFree(d_fp);
+		return blob.alloc(cap) || d_off.alloc(B * 8) || d_fp.alloc(B * 16) ? -1 : 0;
 	}
 };
 
@@ -1341,7 +1352,7 @@ static long long load_flush(LoadBatch &b, bool with_fp) {
 	job.slot_idx = e->d_slot; job.addr = e->d_addr; job.ts = e->d_ts;
 	job.seq0 = e->seq; job.seq_stride = e->seq_stride;
 	job.table = e->table; job.arena = e->arena;
-	if (launch_restore(job, e->d_pages[0], b.d_off, with_fp ? b.d_fp : nullptr, e->bsize, e->st)) return -1;
+	if (launch_restore(job, e->d_pages[0], b.d_off, with_fp ? (uint64_t *)b.d_fp : nullptr, e->bsize, e->st)) return -1;
 	CMB_CHECK(cudaStreamSynchronize(e->st));
 	e->seq += (unsigned long long)m * e->seq_stride;
 	e->stats.kernel_launches += 2;
@@ -1405,7 +1416,6 @@ extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char 
 		if (got < 0) rc = -1;
 		else loaded += (uint64_t)got;
 	}
-	for (LoadBatch &b : bs) b.release();
 	fclose(f);
 	if (records_out) *records_out = loaded;
 	return rc;
@@ -1424,17 +1434,9 @@ extern "C" int cmb200_move_pages(cmb200_engine *e, size_t n, void *dst_dev, cons
 	if (n > 0xffffffffu) { set_error_msg("cmb200_move_pages: too many pages"); return -1; }
 	std::lock_guard<std::mutex> g(e->mu);
 	CMB_CHECK(cudaSetDevice(e->device));
-	if ((dst_idx || src_idx) && n > e->move_idx_cap) {
-		// grown to the largest call so far: a cudaFree per call would synchronise the whole device
-		CMB_CHECK(cudaStreamSynchronize(e->st));
-		cudaFree(e->d_move_idx);
-		e->d_move_idx = nullptr;
-		e->move_idx_cap = 0;
-		CMB_CHECK(cudaMalloc(&e->d_move_idx, n * 8));
-		e->move_idx_cap = n;
-	}
-	uint32_t *d_dst_idx = dst_idx ? e->d_move_idx : nullptr;
-	uint32_t *d_src_idx = src_idx ? e->d_move_idx + e->move_idx_cap : nullptr;
+	if ((dst_idx || src_idx) && e->d_move_idx.grow(n * 8, e->st)) return -1;
+	uint32_t *d_dst_idx = dst_idx ? (uint32_t *)e->d_move_idx : nullptr;
+	uint32_t *d_src_idx = src_idx ? e->d_move_idx + n : nullptr;
 	if (dst_idx) CMB_CHECK(cudaMemcpyAsync(d_dst_idx, dst_idx, n * 4, cudaMemcpyHostToDevice, e->st));
 	if (src_idx) CMB_CHECK(cudaMemcpyAsync(d_src_idx, src_idx, n * 4, cudaMemcpyHostToDevice, e->st));
 	if (launch_move_pages(dst_dev, d_dst_idx, src_dev, d_src_idx, (uint32_t)n, e->bsize, e->st)) return -1;
@@ -1472,15 +1474,15 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 	if (listed > 0) { set_error_msg("cmb200_compact: the store changed under the compaction"); return -1; }
 	const unsigned long long head_before = c[2];
 	const size_t count = list.size();
-	DevBuf d_moves;
+	DevMem<MoveEntry> d_moves;
 	std::vector<MoveEntry> moves(count);
 	unsigned long long at = 0;
 	for (size_t i = 0; i < count; i++) {
 		moves[i] = MoveEntry{list[i].rec_off, at, list[i].len, list[i].slot};
 		at += ((unsigned long long)list[i].len + 15ull) & ~15ull;
 	}
-	if (count && d_moves.alloc(count * sizeof(MoveEntry))) return -1;
-	if (count) CMB_CHECK(cudaMemcpyAsync(d_moves.p, moves.data(), count * sizeof(MoveEntry), cudaMemcpyHostToDevice, e->st));
+	if (count && d_moves.alloc(count * sizeof(MoveEntry) + 256)) return -1;
+	if (count) CMB_CHECK(cudaMemcpyAsync(d_moves, moves.data(), count * sizeof(MoveEntry), cudaMemcpyHostToDevice, e->st));
 	// windows: as many records as fit the bounce buffer (one page-ring buffer)
 	const unsigned long long bounce_cap = (unsigned long long)e->host_batch * e->bsize;
 	size_t k = 0;
@@ -1488,7 +1490,7 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 		size_t j = k;
 		while (j < count && moves[j].new_off + (((unsigned long long)moves[j].len + 15ull) & ~15ull) - moves[k].new_off <= bounce_cap) j++;
 		if (j == k) { set_error_msg("cmb200_compact: record larger than the bounce buffer"); return -1; }
-		if (launch_compact_window(e->table, e->arena, d_moves.as<MoveEntry>() + k, (uint32_t)(j - k), e->d_pages[0], e->st)) return -1;
+		if (launch_compact_window(e->table, e->arena, d_moves + k, (uint32_t)(j - k), e->d_pages[0], e->st)) return -1;
 		e->stats.kernel_launches += 2;
 		k = j;
 	}
@@ -1502,34 +1504,24 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 	// slots (tombstones; slots of dropped puts go with them): miss probes end at an EMPTY slot, and
 	// linear probing never frees one by itself.
 	if (c[1] > e->table.cap / 8) {
+		// parse checkpoints move with their slots (k_rehash); without room for a second side table
+		// they are dropped instead, and those records are walked by one warp until rewritten
+		const bool ckpt = e->table.ckpt != nullptr;
+		TableMem mem;
+		int got = table_alloc(mem, e->table.cap, e->table.fp != nullptr, e->table.fp_tag != nullptr, ckpt, e->st);
+		if (got > 0 && ckpt) got = table_alloc(mem, e->table.cap, e->table.fp != nullptr, e->table.fp_tag != nullptr, false, e->st);
+		if (got < 0) return -1;
+		if (got > 0) return 0;                           // no room for a second table: keep the old one
 		TableView fresh = e->table;
-		fresh.slots = nullptr; fresh.fp = nullptr; fresh.ckpt = nullptr; fresh.fp_tag = nullptr;
-		if (cudaMalloc(&fresh.slots, (e->table.cap + 2) * sizeof(Slot)) == cudaSuccess &&
-		    (!e->table.fp || cudaMalloc(&fresh.fp, (e->table.cap + 2) * 16) == cudaSuccess) &&
-		    (!e->table.fp_tag || cudaMalloc(&fresh.fp_tag, (e->table.cap + 2) * 4) == cudaSuccess)) {
-			CMB_CHECK(cudaMemsetAsync(fresh.slots, 0, (e->table.cap + 2) * sizeof(Slot), e->st));
-			if (fresh.fp) CMB_CHECK(cudaMemsetAsync(fresh.fp, 0, (e->table.cap + 2) * 16, e->st));
-			if (fresh.fp_tag) CMB_CHECK(cudaMemsetAsync(fresh.fp_tag, 0, (e->table.cap + 2) * 4, e->st));
-			// parse checkpoints move with their slots (k_rehash); without room for a second side table
-			// they are dropped instead, and those records are walked by one warp until rewritten
-			const size_t ck_bytes = (e->table.cap + 2) * CKPT_WORDS * 4;
-			if (e->table.ckpt && cudaMalloc(&fresh.ckpt, ck_bytes) != cudaSuccess) {
-				(void)cudaGetLastError();
-				fresh.ckpt = nullptr;
-			}
-			if (fresh.ckpt) CMB_CHECK(cudaMemsetAsync(fresh.ckpt, 0, ck_bytes, e->st));
-			if (launch_rehash(e->table, fresh, e->st)) return -1;
-			if (e->table.ckpt && !fresh.ckpt) CMB_CHECK(cudaMemsetAsync(e->table.ckpt, 0, ck_bytes, e->st));
-			CMB_CHECK(cudaMemsetAsync(e->d_counters + 1, 0, sizeof(unsigned long long), e->st));   // tombstones
-			CMB_CHECK(cudaStreamSynchronize(e->st));
-			cudaFree(e->table.slots); cudaFree(e->table.fp); cudaFree(e->table.fp_tag);
-			e->table.slots = fresh.slots; e->table.fp = fresh.fp; e->table.fp_tag = fresh.fp_tag;
-			if (fresh.ckpt) { cudaFree(e->table.ckpt); e->table.ckpt = fresh.ckpt; }
-			e->stats.kernel_launches++;
-		} else {
-			(void)cudaGetLastError();                    // no room for a second table: keep the old one
-			cudaFree(fresh.slots); cudaFree(fresh.fp); cudaFree(fresh.fp_tag);
-		}
+		mem.view(fresh);
+		if (launch_rehash(e->table, fresh, e->st)) return -1;
+		if (ckpt && !fresh.ckpt) CMB_CHECK(cudaMemsetAsync(e->table.ckpt, 0, (e->table.cap + 2) * CKPT_WORDS * 4, e->st));
+		CMB_CHECK(cudaMemsetAsync(e->d_counters + 1, 0, sizeof(unsigned long long), e->st));   // tombstones
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		if (!mem.ckpt) mem.ckpt = std::move(e->table_mem.ckpt);
+		e->table_mem = std::move(mem);
+		e->table_mem.view(e->table);
+		e->stats.kernel_launches++;
 	}
 	return 0;
 }
@@ -1573,15 +1565,15 @@ extern "C" int cmb200_verify_store(cmb200_engine *e, size_t max, cmb200_addr *ba
 	unsigned long long *scan = e->d_vstat + VS_WORDS;
 	CMB_CHECK(cudaMemsetAsync(scan, 0, VS_WORDS * sizeof(unsigned long long), e->st));
 	const size_t B = e->host_batch;
-	DevBuf d_list;
-	if (!list.empty() && d_list.alloc(B * sizeof(ExportEntry))) return -1;
+	DevMem<ExportEntry> d_list;
+	if (!list.empty() && d_list.alloc(B * sizeof(ExportEntry) + 256)) return -1;
 	std::vector<int32_t> st(B);
 	std::vector<cmb200_addr> addr(B);
 	size_t bad = 0;
 	for (size_t at = 0; at < list.size(); at += B) {
 		const uint32_t m = (uint32_t)(list.size() - at < B ? list.size() - at : B);
-		CMB_CHECK(cudaMemcpyAsync(d_list.p, list.data() + at, m * sizeof(ExportEntry), cudaMemcpyHostToDevice, e->st));
-		if (launch_scan_prep(e->table, d_list.as<ExportEntry>(), m, e->d_status, e->d_recoff, e->d_vlen, e->d_vidx,
+		CMB_CHECK(cudaMemcpyAsync(d_list, list.data() + at, m * sizeof(ExportEntry), cudaMemcpyHostToDevice, e->st));
+		if (launch_scan_prep(e->table, d_list, m, e->d_status, e->d_recoff, e->d_vlen, e->d_vidx,
 			e->d_addr, e->st)) return -1;
 		DecodeJob job{};
 		job.n = m; job.nbytes = e->bsize; job.pages = e->d_pages[0]; job.status = e->d_status;
@@ -1621,22 +1613,18 @@ extern "C" int cmb200_host_tier_enable(cmb200_engine *e, uint64_t bytes) {
 	bytes = (bytes + 4095) & ~4095ull;
 	if (bytes < 4ull * e->stage_stride) { set_error_msg("cmb200_host_tier_enable: fewer bytes than four worst-case records"); return -1; }
 	CMB_CHECK(cudaSetDevice(e->device));
-	cmb200_engine::HostTier &t = e->tier;
-	if (cudaMalloc(&t.d_ctr, 3 * sizeof(unsigned long long)) != cudaSuccess ||
-	    cudaMalloc(&t.d_moves, (size_t)e->max_batch * sizeof(DemoteEntry)) != cudaSuccess ||
-	    cudaMalloc(&t.d_promote, (size_t)e->max_batch * sizeof(PromoteEntry)) != cudaSuccess ||
-	    cudaMalloc(&t.d_hot, HOT_LOG_N * sizeof(ulonglong2)) != cudaSuccess ||
-	    cudaMemset(t.d_ctr, 0, 3 * sizeof(unsigned long long)) != cudaSuccess ||
-	    cudaMemset(t.d_hot, 0, HOT_LOG_N * sizeof(ulonglong2)) != cudaSuccess ||
-	    cudaHostAlloc(&t.host, bytes, cudaHostAllocMapped) != cudaSuccess ||
-	    cudaHostGetDevicePointer(&t.dev, t.host, 0) != cudaSuccess) {
+	cmb200_engine::HostTier t;                          // built aside: the engine gets all of it or nothing
+	if (t.d_ctr.alloc(3 * sizeof(unsigned long long)) || t.d_moves.alloc((size_t)e->max_batch * sizeof(DemoteEntry)) ||
+	    t.d_promote.alloc((size_t)e->max_batch * sizeof(PromoteEntry)) || t.d_hot.alloc(HOT_LOG_N * sizeof(ulonglong2)) ||
+	    cudaMemsetAsync(t.d_ctr, 0, 3 * sizeof(unsigned long long), e->st) != cudaSuccess ||
+	    cudaMemsetAsync(t.d_hot, 0, HOT_LOG_N * sizeof(ulonglong2), e->st) != cudaSuccess ||
+	    cudaStreamSynchronize(e->st) != cudaSuccess ||
+	    t.host.alloc(bytes, true) || cudaHostGetDevicePointer(&t.dev, t.host, 0) != cudaSuccess) {
 		cmb_set_error("cmb200_host_tier_enable", cudaGetLastError(), __FILE__, __LINE__);
-		if (t.host) cudaFreeHost(t.host);
-		cudaFree(t.d_ctr); cudaFree(t.d_moves); cudaFree(t.d_promote); cudaFree(t.d_hot);
-		t = cmb200_engine::HostTier{};
 		return -1;
 	}
 	t.size = bytes;
+	e->tier = std::move(t);
 	return 0;
 }
 
@@ -1664,13 +1652,7 @@ static int demote_group(cmb200_engine *e, const std::vector<DemoteEntry> &grp,
 	}
 	int rc = 0;
 	const size_t nr = ret.size() / 4;
-	if (nr > t.retire_cap) {
-		if (cudaStreamSynchronize(e->st) != cudaSuccess) rc = -1;
-		cudaFree(t.d_retire);
-		t.d_retire = nullptr; t.retire_cap = 0;
-		if (rc == 0 && cudaMalloc(&t.d_retire, nr * 32) == cudaSuccess) t.retire_cap = nr;
-		else rc = -1;
-	}
+	if (t.d_retire.grow(nr * 32, e->st)) rc = -1;
 	const uint64_t a0 = start % t.size, bytes = end - start, first = std::min(bytes, t.size - a0);
 	if (rc == 0 && nr) {
 		rc = cudaMemcpyAsync(t.d_retire, ret.data(), nr * 32, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
@@ -1860,20 +1842,24 @@ extern "C" int cmb200_host_tier_stats(cmb200_engine *e, struct cmb200_host_tier_
 }
 
 // ---- kernel-level entry points -------------------------------------------------------------
+// Their device buffers, like the engine's page and stage buffers, end in 256 bytes of slack.
 
 extern "C" int cmb200_compose_keys(int device, size_t n, const uint64_t *offset, const uint64_t *nhid,
     const uint32_t *genid, int pshift, cmb200_addr *addr_out, uint8_t *valid_out, uint64_t *key_out) {
 	if (select_device(device)) return -1;
-	DevBuf d_off, d_nh, d_g, d_addr, d_valid, d_key;
-	if (d_off.alloc(n * 8) || d_nh.alloc(n * 8) || d_g.alloc(n * 4) || d_addr.alloc(n * 16) || d_valid.alloc(n) || d_key.alloc(n * 8)) return -1;
-	CMB_CHECK(cudaMemcpy(d_off.p, offset, n * 8, cudaMemcpyHostToDevice));
-	CMB_CHECK(cudaMemcpy(d_nh.p, nhid, n * 8, cudaMemcpyHostToDevice));
-	CMB_CHECK(cudaMemcpy(d_g.p, genid, n * 4, cudaMemcpyHostToDevice));
-	if (launch_compose(d_off.as<uint64_t>(), d_nh.as<uint64_t>(), d_g.as<uint32_t>(), pshift, (uint32_t)n,
-		d_addr.as<unsigned long long>(), d_valid.as<uint8_t>(), d_key.as<unsigned long long>(), 0)) return -1;
-	CMB_CHECK(cudaMemcpy(addr_out, d_addr.p, n * 16, cudaMemcpyDeviceToHost));
-	CMB_CHECK(cudaMemcpy(valid_out, d_valid.p, n, cudaMemcpyDeviceToHost));
-	CMB_CHECK(cudaMemcpy(key_out, d_key.p, n * 8, cudaMemcpyDeviceToHost));
+	DevMem<uint64_t> d_off, d_nh;
+	DevMem<uint32_t> d_g;
+	DevMem<unsigned long long> d_addr, d_key;
+	DevMem<uint8_t> d_valid;
+	if (d_off.alloc(n * 8 + 256) || d_nh.alloc(n * 8 + 256) || d_g.alloc(n * 4 + 256) || d_addr.alloc(n * 16 + 256) ||
+	    d_valid.alloc(n + 256) || d_key.alloc(n * 8 + 256)) return -1;
+	CMB_CHECK(cudaMemcpy(d_off, offset, n * 8, cudaMemcpyHostToDevice));
+	CMB_CHECK(cudaMemcpy(d_nh, nhid, n * 8, cudaMemcpyHostToDevice));
+	CMB_CHECK(cudaMemcpy(d_g, genid, n * 4, cudaMemcpyHostToDevice));
+	if (launch_compose(d_off, d_nh, d_g, pshift, (uint32_t)n, d_addr, d_valid, d_key, 0)) return -1;
+	CMB_CHECK(cudaMemcpy(addr_out, d_addr, n * 16, cudaMemcpyDeviceToHost));
+	CMB_CHECK(cudaMemcpy(valid_out, d_valid, n, cudaMemcpyDeviceToHost));
+	CMB_CHECK(cudaMemcpy(key_out, d_key, n * 8, cudaMemcpyDeviceToHost));
 	return 0;
 }
 
@@ -1884,23 +1870,27 @@ extern "C" int cmb200_lz4_encode_batch(int device, const void *pages_host, size_
 	size_t bound = (size_t)nbytes + nbytes / 255 + 16;
 	size_t sstride = (bound + 15) & ~(size_t)15;
 	if (out_stride < bound) { set_error_msg("encode_batch: out_stride below LZ4_compressBound"); return -1; }
-	DevBuf d_in, d_stage, d_lens, d_fps, d_work, d_order;
-	if (d_in.alloc(n * stride) || d_stage.alloc(n * sstride) || d_lens.alloc(n * 4) || d_fps.alloc(n * 16) || d_work.alloc(64) ||
-	    d_order.alloc(encode_order_words((uint32_t)n) * 4)) return -1;
-	CMB_CHECK(cudaMemcpy(d_in.p, pages_host, n * stride, cudaMemcpyHostToDevice));
+	DevMem<uint8_t> d_in, d_stage;
+	DevMem<int32_t> d_lens;
+	DevMem<uint64_t> d_fps;
+	DevMem<unsigned int> d_work;
+	DevMem<uint32_t> d_order;
+	if (d_in.alloc(n * stride + 256) || d_stage.alloc(n * sstride + 256) || d_lens.alloc(n * 4 + 256) ||
+	    d_fps.alloc(n * 16 + 256) || d_work.alloc(64 + 256) || d_order.alloc(encode_order_words((uint32_t)n) * 4 + 256)) return -1;
+	CMB_CHECK(cudaMemcpy(d_in, pages_host, n * stride, cudaMemcpyHostToDevice));
 	EncodeJob job{};
-	job.pages = d_in.as<uint8_t>(); job.page_stride = stride; job.nbytes = nbytes; job.n = (uint32_t)n;
+	job.pages = d_in; job.page_stride = stride; job.nbytes = nbytes; job.n = (uint32_t)n;
 	job.accel = accel < 0 ? 1u : (uint32_t)(accel > (1 << 20) ? (1 << 20) : accel);
 	if (accel == 0) job.accel = 1;   // LZ4_compress_fast(accel<1) -> 1 (lz4.c:740); raw mode is a store-level notion
-	job.stage = d_stage.as<uint8_t>(); job.stage_stride = sstride;
-	job.lens = d_lens.as<int32_t>();
-	job.fps = fp_out ? d_fps.as<uint64_t>() : nullptr;
-	job.work = d_work.as<unsigned int>();
-	job.order = d_order.as<uint32_t>();
+	job.stage = d_stage; job.stage_stride = sstride;
+	job.lens = d_lens;
+	job.fps = fp_out ? (uint64_t *)d_fps : nullptr;
+	job.work = d_work;
+	job.order = d_order;
 	if (launch_encode(job, 0) < 0) return -1;
-	CMB_CHECK(cudaMemcpy(lens_out, d_lens.p, n * 4, cudaMemcpyDeviceToHost));
-	if (fp_out) CMB_CHECK(cudaMemcpy(fp_out, d_fps.p, n * 16, cudaMemcpyDeviceToHost));
-	CMB_CHECK(cudaMemcpy2D(blocks_out_host, out_stride, d_stage.p, sstride, bound < out_stride ? bound : out_stride, n,
+	CMB_CHECK(cudaMemcpy(lens_out, d_lens, n * 4, cudaMemcpyDeviceToHost));
+	if (fp_out) CMB_CHECK(cudaMemcpy(fp_out, d_fps, n * 16, cudaMemcpyDeviceToHost));
+	CMB_CHECK(cudaMemcpy2D(blocks_out_host, out_stride, d_stage, sstride, bound < out_stride ? bound : out_stride, n,
 	    cudaMemcpyDeviceToHost));
 	return 0;
 }
@@ -1908,17 +1898,19 @@ extern "C" int cmb200_lz4_encode_batch(int device, const void *pages_host, size_
 extern "C" int cmb200_lz4_decode_batch(int device, const void *blocks_host, size_t in_stride, const int32_t *lens,
     size_t n, uint32_t nbytes, void *pages_out_host, int32_t *consumed_out) {
 	if (select_device(device)) return -1;
-	DevBuf d_blk, d_lens, d_out, d_used;
-	if (d_blk.alloc(n * in_stride) || d_lens.alloc(n * 4) || d_out.alloc(n * (size_t)nbytes) || d_used.alloc(n * 4)) return -1;
-	CMB_CHECK(cudaMemcpy(d_blk.p, blocks_host, n * in_stride, cudaMemcpyHostToDevice));
-	CMB_CHECK(cudaMemcpy(d_lens.p, lens, n * 4, cudaMemcpyHostToDevice));
-	CMB_CHECK(cudaMemset(d_out.p, 0, n * (size_t)nbytes));
+	DevMem<uint8_t> d_blk, d_out;
+	DevMem<int32_t> d_lens, d_used;
+	if (d_blk.alloc(n * in_stride + 256) || d_lens.alloc(n * 4 + 256) || d_out.alloc(n * (size_t)nbytes + 256) ||
+	    d_used.alloc(n * 4 + 256)) return -1;
+	CMB_CHECK(cudaMemcpy(d_blk, blocks_host, n * in_stride, cudaMemcpyHostToDevice));
+	CMB_CHECK(cudaMemcpy(d_lens, lens, n * 4, cudaMemcpyHostToDevice));
+	CMB_CHECK(cudaMemset(d_out, 0, n * (size_t)nbytes));
 	DecodeJob job{};
-	job.n = (uint32_t)n; job.nbytes = nbytes; job.pages = d_out.as<uint8_t>(); job.status = d_used.as<int32_t>();
-	job.blocks = d_blk.as<uint8_t>(); job.block_stride = in_stride; job.lens = d_lens.as<int32_t>();
+	job.n = (uint32_t)n; job.nbytes = nbytes; job.pages = d_out; job.status = d_used;
+	job.blocks = d_blk; job.block_stride = in_stride; job.lens = d_lens;
 	if (launch_decode(job, 0)) return -1;
-	CMB_CHECK(cudaMemcpy(consumed_out, d_used.p, n * 4, cudaMemcpyDeviceToHost));
-	CMB_CHECK(cudaMemcpy(pages_out_host, d_out.p, n * (size_t)nbytes, cudaMemcpyDeviceToHost));
+	CMB_CHECK(cudaMemcpy(consumed_out, d_used, n * 4, cudaMemcpyDeviceToHost));
+	CMB_CHECK(cudaMemcpy(pages_out_host, d_out, n * (size_t)nbytes, cudaMemcpyDeviceToHost));
 	return 0;
 }
 
@@ -1926,11 +1918,12 @@ extern "C" int cmb200_fingerprint_batch(int device, const void *pages_host, size
     size_t stride, uint64_t *fp_out) {
 	if (select_device(device)) return -1;
 	if (stride % 16) { set_error_msg("fingerprint_batch: stride must be a multiple of 16"); return -1; }
-	DevBuf d_in, d_fps;
-	if (d_in.alloc(n * stride) || d_fps.alloc(n * 16)) return -1;
-	CMB_CHECK(cudaMemcpy(d_in.p, pages_host, n * stride, cudaMemcpyHostToDevice));
-	if (launch_fingerprint(d_in.as<uint8_t>(), stride, nbytes, (uint32_t)n, d_fps.as<uint64_t>(), 0)) return -1;
-	CMB_CHECK(cudaMemcpy(fp_out, d_fps.p, n * 16, cudaMemcpyDeviceToHost));
+	DevMem<uint8_t> d_in;
+	DevMem<uint64_t> d_fps;
+	if (d_in.alloc(n * stride + 256) || d_fps.alloc(n * 16 + 256)) return -1;
+	CMB_CHECK(cudaMemcpy(d_in, pages_host, n * stride, cudaMemcpyHostToDevice));
+	if (launch_fingerprint(d_in, stride, nbytes, (uint32_t)n, d_fps, 0)) return -1;
+	CMB_CHECK(cudaMemcpy(fp_out, d_fps, n * 16, cudaMemcpyDeviceToHost));
 	return 0;
 }
 
@@ -1939,12 +1932,12 @@ extern "C" int cmb200_fingerprint_batch(int device, const void *pages_host, size
 extern "C" int cmb200_fingerprint_dev(cmb200_engine *e, size_t n, const void *pages_dev, uint64_t *fp_out_host) {
 	std::lock_guard<std::mutex> g(e->mu);
 	CMB_CHECK(cudaSetDevice(e->device));
-	DevBuf d_fps;
-	if (d_fps.alloc(n * 16)) return -1;
+	DevMem<uint64_t> d_fps;
+	if (d_fps.alloc(n * 16 + 256)) return -1;
 	CMB_CHECK(cudaEventRecord(e->t0[0], e->st));
-	if (launch_fingerprint((const uint8_t *)pages_dev, e->bsize, e->bsize, (uint32_t)n, d_fps.as<uint64_t>(), e->st)) return -1;
+	if (launch_fingerprint((const uint8_t *)pages_dev, e->bsize, e->bsize, (uint32_t)n, d_fps, e->st)) return -1;
 	CMB_CHECK(cudaEventRecord(e->t1[0], e->st));
-	CMB_CHECK(cudaMemcpyAsync(fp_out_host, d_fps.p, n * 16, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaMemcpyAsync(fp_out_host, d_fps, n * 16, cudaMemcpyDeviceToHost, e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
 	float ms = 0;
 	CMB_CHECK(cudaEventElapsedTime(&ms, e->t0[0], e->t1[0]));
@@ -1963,10 +1956,10 @@ extern "C" void cmb200_gen_chunk_host(uint64_t seed, uint64_t cid, uint32_t bsiz
 extern "C" int cmb200_gen_chunks_dev(cmb200_engine *e, uint64_t seed, const uint64_t *cids_host, size_t n, void *out_dev) {
 	std::lock_guard<std::mutex> g(e->mu);
 	CMB_CHECK(cudaSetDevice(e->device));
-	DevBuf d_c;
-	if (d_c.alloc(n * 8)) return -1;
-	CMB_CHECK(cudaMemcpyAsync(d_c.p, cids_host, n * 8, cudaMemcpyHostToDevice, e->st));
-	if (launch_streamgen(d_c.as<uint64_t>(), (uint32_t)n, seed, e->bsize, (uint8_t *)out_dev, e->st)) return -1;
+	DevMem<uint64_t> d_c;
+	if (d_c.alloc(n * 8 + 256)) return -1;
+	CMB_CHECK(cudaMemcpyAsync(d_c, cids_host, n * 8, cudaMemcpyHostToDevice, e->st));
+	if (launch_streamgen(d_c, (uint32_t)n, seed, e->bsize, (uint8_t *)out_dev, e->st)) return -1;
 	CMB_CHECK(cudaStreamSynchronize(e->st));
 	return 0;
 }
