@@ -923,6 +923,25 @@ __device__ bool gs_sections_fit(const DecodeCta *dc, uint32_t clen, uint32_t n) 
 	return dc->ip1[prev] == clen && dc->op1[prev] == n;          // filemap.c:244-248: consumed == compressed_length
 }
 
+// The request's answer, by thread 0 of the CTA that answers (k_get_small; the page CTA of
+// k_get_small_pair), after a barrier that follows the page's last store.  The status may live in
+// page-locked host memory that the caller polls: the page first, then the status (every thread's
+// stores happen before the barrier, this thread's system-wide fence after it is cumulative).
+template <bool VERIFY>
+__device__ __forceinline__ void gs_answer(const GetJob &job, uint32_t i, int32_t result, uint32_t region, bool from_host,
+    uint32_t fp_ok) {
+	if (region != 0xffffffffu) gs_region_give(job, region);
+	if (result == ST_HIT && from_host) {
+		atomicAdd(job.host_hits, 1ull);
+		// loaded again rather than kept from the top: u and l live past the loop would cost registers
+		hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
+	}
+	if (VERIFY && (result == ST_HIT || result == ST_CORRUPT))
+		atomicAdd(&job.vstat[result == ST_CORRUPT ? VS_CORRUPT : fp_ok ? VS_VERIFIED : VS_UNVERIFIED], 1ull);
+	__threadfence_system();
+	*reinterpret_cast<volatile int32_t *>(&job.status[i]) = result;
+}
+
 // VERIFY (CMB200_VERIFY): the page, decoded or raw, is compared with the record's stored EF128 while it
 // is still in shared memory (gs_page_matches), so a page that does not match is never written out and
 // is answered ST_CORRUPT.
@@ -1046,21 +1065,8 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 		result = ST_HIT;
 		break;
 	}
-	// status may live in page-locked host memory that the caller polls: the page first, then the status
-	// (every thread's stores happen before the barrier, thread 0's system-wide fence after it is cumulative)
 	__syncthreads();
-	if (tid == 0) {
-		if (sh->region != 0xffffffffu) gs_region_give(job, sh->region);
-		if (result == ST_HIT && from_host) {
-			atomicAdd(job.host_hits, 1ull);
-			// loaded again rather than kept from the top: u and l live past the loop would cost registers
-			hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
-		}
-		if (VERIFY && (result == ST_HIT || result == ST_CORRUPT))
-			atomicAdd(&job.vstat[result == ST_CORRUPT ? VS_CORRUPT : sh->fp_ok ? VS_VERIFIED : VS_UNVERIFIED], 1ull);
-		__threadfence_system();
-		*reinterpret_cast<volatile int32_t *>(&job.status[i]) = result;
-	}
+	if (tid == 0) gs_answer<VERIFY>(job, i, result, sh->region, from_host, sh->fp_ok);
 }
 
 // ---- pages above 64 KiB: one request per cluster of two CTAs ----------------------------------------
@@ -1071,7 +1077,7 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 //           the page CTA over DSMEM.  Raw pages go straight to `out`.  Every decision is taken here.
 //   rank 1, the PAGE CTA: holds the page at the record buffer's offset.  Given the record CTA's
 //           verdict it runs the match phase on its own shared memory, writes the page out, then the
-//           status.  It is the one CTA that answers: region release, host-tier hit, status word.
+//           status.  It is the one CTA that answers (gs_answer): region release, host-tier hit, status word.
 // Two cluster barrier phases.  A: both CTAs arrive at entry, and the record CTA waits for A before
 // its first remote store, so the page CTA has started.  B: the record CTA arrives with release after
 // its last remote store and global write, the page CTA waits with acquire: literals, descriptors,
@@ -1142,21 +1148,10 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 				for (uint32_t k = tid; k < job.nbytes / 16u; k += GS_THREADS)
 					reinterpret_cast<uint4 *>(out)[k] = reinterpret_cast<const uint4 *>(buf)[k];
 		}
-		// the page first, then the status (as k_get_small; a raw page was written by the record CTA
-		// before it arrived at B, and this thread acquired B)
+		// the page first, then the status (a raw page was written by the record CTA before it arrived
+		// at B, and this thread acquired B)
 		__syncthreads();
-		if (tid == 0) {
-			if (v->region != 0xffffffffu) gs_region_give(job, v->region);
-			if (v->result == ST_HIT && v->from_host) {
-				atomicAdd(job.host_hits, 1ull);
-				hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
-			}
-			if constexpr (VERIFY)
-				if (v->result == ST_HIT || v->result == ST_CORRUPT)
-					atomicAdd(&job.vstat[v->result == ST_CORRUPT ? VS_CORRUPT : v->fp_ok ? VS_VERIFIED : VS_UNVERIFIED], 1ull);
-			__threadfence_system();
-			*reinterpret_cast<volatile int32_t *>(&job.status[i]) = v->result;
-		}
+		if (tid == 0) gs_answer<VERIFY>(job, i, v->result, v->region, v->from_host, v->fp_ok);
 		return;
 	}
 	GetShared *sh = reinterpret_cast<GetShared *>(smem);
