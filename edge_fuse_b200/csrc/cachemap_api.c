@@ -88,6 +88,7 @@ struct fm_req {
 
 struct wb_slot {
 	cmb200_addr addr;
+	uint64_t key;           /* store key of addr (addr_key): ring lookups go by key, as the store does */
 	uint64_t ts;
 	int state;
 };
@@ -182,13 +183,20 @@ env_long(const char *name, long dflt)
 	return (v && *v) ? strtol(v, NULL, 0) : dflt;
 }
 
+/* The store key of `a`: the store keeps one record per key, not per address. */
+static uint64_t
+addr_key(const cmb200_addr *a)
+{
+	uint64_t key;
+	FNV_hash(a, (int)sizeof(*a), &key);                     /* filemap.c:18-24 */
+	return key;
+}
+
 /* The engine that owns `a`. */
 static struct fm_dev *
 filemap_owner(struct filemap *m, const cmb200_addr *a)
 {
-	uint64_t key;
-	FNV_hash(a, (int)sizeof(*a), &key);                     /* filemap.c:18-24 */
-	return m->dev[cmb200_owner(key, m->g)];
+	return m->dev[cmb200_owner(addr_key(a), m->g)];
 }
 
 /* CMB200_DEVICES: "all", or a comma-separated list of CUDA ordinals (one may repeat: two engines on
@@ -1038,26 +1046,35 @@ filemap_flusher(void *arg)
 	return NULL;
 }
 
-/* Newest copy of `addr` still in its engine's ring -> malloc()ed page (or dst), else NULL. */
-static void *
-filemap_ring_lookup(struct fm_dev *d, const cmb200_addr *addr, void *dst)
+/* The newest page of `key` (the store key of `addr`) still in its engine's ring decides, as it will
+ * once it has landed: CMB200_HIT when it is of `addr` (*page = a malloc()ed copy, or dst; NULL if malloc fails),
+ * CMB200_BAD_ENTRY when it is of another address with the same key (that put replaces the record of
+ * `addr`, filemap.c:236-240), CMB200_MISS when the ring holds no page of the key: ask the engine. */
+static int32_t
+filemap_ring_lookup(struct fm_dev *d, const cmb200_addr *addr, uint64_t key, void *dst, void **page)
 {
-	void *page = NULL;
+	int32_t st = CMB200_MISS;
+	*page = NULL;
 	if (!d->wb_n)
-		return NULL;
+		return st;
 	const size_t bsize = (size_t)d->m->bsize;
 	pthread_mutex_lock(&d->wb_mu);
 	for (uint64_t s = d->wb_head; s > d->wb_tail; s--) {
 		struct wb_slot *w = &d->wb_slot[(s - 1) % d->wb_n];
-		if (w->state >= WB_READY && w->addr.u == addr->u && w->addr.l == addr->l) {
-			page = dst ? dst : malloc(bsize);
-			if (page)
-				memcpy(page, d->wb_pages + ((s - 1) % d->wb_n) * bsize, bsize);
+		if (w->state < WB_READY || w->key != key)
+			continue;
+		if (w->addr.u != addr->u || w->addr.l != addr->l) {
+			st = CMB200_BAD_ENTRY;
 			break;
 		}
+		st = CMB200_HIT;
+		*page = dst ? dst : malloc(bsize);
+		if (*page)
+			memcpy(*page, d->wb_pages + ((s - 1) % d->wb_n) * bsize, bsize);
+		break;
 	}
 	pthread_mutex_unlock(&d->wb_mu);
-	return page;
+	return st;
 }
 
 /* Combining queue of the single-page calls (cachemap_get / filemap_unset from FUSE worker threads),
@@ -1255,7 +1272,8 @@ filemap_set(struct filemap *m, uint128_t *key, void *value, uint64_t attr)
 	if (!filemap_engine_ready(m))
 		return;
 	cmb200_addr a = { key->u, key->l };
-	struct fm_dev *d = filemap_owner(m, &a);
+	const uint64_t k = addr_key(&a);
+	struct fm_dev *d = m->dev[cmb200_owner(k, m->g)];
 	if (!d->wb_n) {                         /* write-behind disabled: one synchronous GPU put */
 		filemap_make_room(d, 1);
 		filemap_land_begin(d);
@@ -1270,6 +1288,7 @@ filemap_set(struct filemap *m, uint128_t *key, void *value, uint64_t attr)
 	const uint64_t s = d->wb_head++;
 	struct wb_slot *w = &d->wb_slot[s % d->wb_n];
 	w->addr = a;
+	w->key = k;
 	w->ts = attr;
 	w->state = WB_FILLING;
 	pthread_mutex_unlock(&d->wb_mu);
@@ -1306,12 +1325,18 @@ filemap_get(struct filemap *m, uint128_t *key)
 	r.kind = REQ_GET;
 	r.addr.u = key->u;
 	r.addr.l = key->l;
-	struct fm_dev *d = filemap_owner(m, &r.addr);
+	const uint64_t k = addr_key(&r.addr);
+	struct fm_dev *d = m->dev[cmb200_owner(k, m->g)];
 	/* a page accepted by filemap_set but not flushed yet is served from the ring; a slot leaves
 	 * the ring only after the GPU put of its batch has completed, so nothing falls between */
-	void *page = filemap_ring_lookup(d, &r.addr, NULL);
-	if (page)
+	void *page;
+	const int32_t st = filemap_ring_lookup(d, &r.addr, k, NULL, &page);
+	if (st == CMB200_HIT)
 		return page;
+	if (st == CMB200_BAD_ENTRY) {
+		printf("bad entry\n");          /* filemap.c:237 */
+		return NULL;
+	}
 	filemap_submit(d, &r);
 	if (r.bad_entry)
 		printf("bad entry\n");          /* filemap.c:237 */
@@ -1888,7 +1913,8 @@ cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 	cmb200_addr *addr = malloc((size_t)n * sizeof(cmb200_addr));
 	int *own = malloc((size_t)n * sizeof(int));
 	size_t *order = malloc((size_t)n * sizeof(size_t));
-	uint8_t *state = calloc((size_t)n, 1);          /* 0 miss, 1 hit, 2 invalid address, 3 asked of an engine */
+	uint8_t *state = calloc((size_t)n, 1);          /* 0 miss, 1 hit, 2 invalid address, 3 asked of an engine,
+	                                                 * 4 bad entry in a ring */
 	if (!reqs || !addr || !own || !order || !state) {
 		free(reqs); free(addr); free(own); free(order); free(state);
 		return 0;
@@ -1902,9 +1928,12 @@ cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 			state[i] = 2;
 			continue;
 		}
-		struct fm_dev *d = filemap_owner(fm, &addr[ask]);
-		if (filemap_ring_lookup(d, &addr[ask], dst)) {
-			state[i] = 1;
+		const uint64_t k = addr_key(&addr[ask]);
+		struct fm_dev *d = fm->dev[cmb200_owner(k, fm->g)];
+		void *page;
+		const int32_t rs = filemap_ring_lookup(d, &addr[ask], k, dst, &page);
+		if (rs != CMB200_MISS) {
+			state[i] = rs == CMB200_HIT ? 1 : 4;
 			continue;
 		}
 		state[i] = 3;
@@ -1949,6 +1978,8 @@ cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 	for (size_t j = 0; j < ask; j++)
 		if (reqs[j].bad_entry && (uint64_t)page_of[order[j]] <= i)
 			printf("bad entry\n");                  /* filemap.c:237 */
+	if (i < n && state[i] == 4)
+		printf("bad entry\n");
 	__atomic_fetch_add(&cm->requests, rq, __ATOMIC_RELAXED);
 	__atomic_fetch_add(&cm->hits, ht, __ATOMIC_RELAXED);
 	free(reqs); free(addr); free(own); free(order); free(state); free(page_of);

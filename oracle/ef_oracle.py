@@ -244,6 +244,7 @@ class StoreModel:
         self.rec: dict[int, tuple[tuple[int, int], int, bytes]] = {}
         self.requests = 0
         self.hits = 0
+        self.bad_entries = 0
 
     def put(self, offset: int, nhid: int, genid: int, page) -> None:
         a = addr_compose(offset, nhid, genid, self.pshift)
@@ -259,21 +260,29 @@ class StoreModel:
             self.rec[key] = (a, 0, bytes(_u8(page)))
 
     def get(self, offset: int, nhid: int, genid: int):
+        return self.get_status(offset, nhid, genid)[1]
+
+    def get_status(self, offset: int, nhid: int, genid: int):
+        """-> (status, page or None); status "hit", "miss", or "bad entry" when the key holds a record
+        of another address (the reference prints `bad entry` then, filemap.c:236-240)."""
         a = addr_compose(offset, nhid, genid, self.pshift)
         if a is None:
-            return None
+            return "miss", None
         self.requests += 1
         r = self.rec.get(addr_key(*a))
-        if r is None or r[0] != a:
-            return None
+        if r is None:
+            return "miss", None
+        if r[0] != a:
+            self.bad_entries += 1
+            return "bad entry", None
         if r[1]:
             page, used = lz4_decode(r[2], self.bsize)
             if used != r[1]:
-                return None
+                return "miss", None
         else:
             page = r[2]
         self.hits += 1
-        return page
+        return "hit", page
 
     def unset(self, u: int, l: int) -> None:
         self.rec.pop(addr_key(u, l), None)

@@ -6,6 +6,10 @@
  * engine promises the host layer, including the asynchronous part: cmb200_get_small_begin returns at
  * once and worker threads answer the requests one by one, in shuffled order, after short random
  * delays — page first, then the status word (release) — exactly the order the kernel keeps.
+ * Like the engine it keeps one record per store key (FNV-1a-64 of the 16 address bytes, filemap.c:18-24):
+ * a put replaces the key's record whatever address it held, a get of a key that holds another address
+ * answers CMB200_BAD_ENTRY, and an unset deletes the key's record.  mock_hold_puts(1) makes every put
+ * wait until mock_hold_puts(0), so that a test can keep pages in the drop-in's write-behind ring.
  * Nothing of the product links against this file. */
 #include <pthread.h>
 #include <sched.h>
@@ -16,13 +20,14 @@
 #include <unistd.h>
 
 #include "../../include/cachemap_b200.h"
+#include "../../include/uint128.h"
 
 #define SLOTS (1u << 17)
 #define LANES 32
 #define LANE_MAX 1024
 #define WORKERS 6
 
-struct entry { int used; cmb200_addr a; uint64_t ts; uint8_t *page; };
+struct entry { int used; uint64_t key; cmb200_addr a; uint64_t ts; uint8_t *page; };
 
 struct job { int lane; uint32_t n; uint8_t *out; };
 
@@ -48,22 +53,44 @@ int cmb200_device_count(void) { return 1; }
 void *cmb200_host_alloc(size_t bytes) { return malloc(bytes ? bytes : 1); }
 void cmb200_host_free(void *p) { free(p); }
 
-static uint64_t mix(uint64_t u, uint64_t l) {
-	uint64_t h = u * 0x9E3779B97F4A7C15ull ^ (l + 0x7F4A7C15ull) * 0xC2B2AE3D27D4EB4Full;
-	return h ^ (h >> 29);
+static uint64_t addr_key(const cmb200_addr *a) {
+	uint64_t key;
+	FNV_hash(a, (int)sizeof(*a), &key);
+	return key;
 }
-/* slot of `a`, or the free slot where it would go (mu held) */
+/* slot of the key of `a` (whatever address its record holds), or the free slot where it would go (mu held) */
 static struct entry *find(cmb200_engine *e, const cmb200_addr *a, int *present) {
-	uint64_t i = mix(a->u, a->l) & (SLOTS - 1);
+	const uint64_t key = addr_key(a);
+	uint64_t i = (key ^ (key >> 29)) & (SLOTS - 1);
 	struct entry *hole = NULL;
 	for (uint32_t n = 0; n < SLOTS; n++, i = (i + 1) & (SLOTS - 1)) {
 		struct entry *s = &e->tab[i];
-		if (s->used == 1 && s->a.u == a->u && s->a.l == a->l) { *present = 1; return s; }
+		if (s->used == 1 && s->key == key) { *present = 1; return s; }
 		if (s->used == 2 && !hole) hole = s;                 /* deleted */
 		if (s->used == 0) { *present = 0; return hole ? hole : s; }
 	}
 	*present = 0;
 	return hole;
+}
+/* HIT, BAD_ENTRY (the key holds another address) or MISS for `a`, and its entry on a hit (mu held) */
+static int32_t lookup(cmb200_engine *e, const cmb200_addr *a, struct entry **hit) {
+	int present;
+	struct entry *s = find(e, a, &present);
+	*hit = NULL;
+	if (!present) return CMB200_MISS;
+	if (s->a.u != a->u || s->a.l != a->l) return CMB200_BAD_ENTRY;
+	*hit = s;
+	return CMB200_HIT;
+}
+
+static pthread_mutex_t hold_mu = PTHREAD_MUTEX_INITIALIZER;
+static pthread_cond_t hold_cv = PTHREAD_COND_INITIALIZER;
+static int hold_puts;
+void mock_hold_puts(int on) {
+	pthread_mutex_lock(&hold_mu);
+	hold_puts = on;
+	pthread_cond_broadcast(&hold_cv);
+	pthread_mutex_unlock(&hold_mu);
 }
 
 static void *worker(void *arg) {
@@ -82,11 +109,10 @@ static void *worker(void *arg) {
 		for (uint32_t q = 0; q < j.n; q++) {
 			const uint32_t i = order[q];
 			if ((rand_r(&seed) & 3) == 0) usleep(rand_r(&seed) % 40);
-			int32_t st = CMB200_MISS;
 			pthread_mutex_lock(&e->mu);
-			int present;
-			struct entry *s = find(e, &e->lane_addr[j.lane][i], &present);
-			if (present) { memcpy(j.out + (size_t)i * e->bsize, s->page, e->bsize); st = CMB200_HIT; }
+			struct entry *s;
+			const int32_t st = lookup(e, &e->lane_addr[j.lane][i], &s);
+			if (s) memcpy(j.out + (size_t)i * e->bsize, s->page, e->bsize);
 			pthread_mutex_unlock(&e->mu);
 			__atomic_store_n(&e->lane_status[j.lane][i], st, __ATOMIC_RELEASE);    /* the page first, then its status */
 		}
@@ -123,6 +149,9 @@ void cmb200_engine_destroy(cmb200_engine *e) {
 
 int cmb200_put_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid, const void *pages,
     const uint64_t *ts, int32_t *lens_out) {
+	pthread_mutex_lock(&hold_mu);
+	while (hold_puts) pthread_cond_wait(&hold_cv, &hold_mu);
+	pthread_mutex_unlock(&hold_mu);
 	usleep(30 + n / 8);                                           /* a launch and a copy take a while */
 	pthread_mutex_lock(&e->mu);
 	for (size_t i = 0; i < n; i++) {
@@ -130,7 +159,8 @@ int cmb200_put_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		int present;
 		struct entry *s = find(e, &addr[i], &present);
 		if (!s) continue;                                         /* map full: dropped */
-		if (!present) { s->used = 1; s->a = addr[i]; if (!s->page) s->page = malloc(e->bsize); e->entries++; }
+		if (!present) { s->used = 1; s->key = addr_key(&addr[i]); if (!s->page) s->page = malloc(e->bsize); e->entries++; }
+		s->a = addr[i];                                           /* the key's record, whatever address it held */
 		memcpy(s->page, (const uint8_t *)pages + i * e->bsize, e->bsize);
 		s->ts = ts ? ts[i] : 0;
 		if (lens_out) lens_out[i] = (int32_t)e->bsize;
@@ -157,11 +187,10 @@ int cmb200_get_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 	pthread_mutex_lock(&e->mu);
 	for (size_t i = 0; i < n; i++) {
 		if (valid && !valid[i]) { status_out[i] = CMB200_INVALID; continue; }
-		int present;
-		struct entry *s = find(e, &addr[i], &present);
-		status_out[i] = present ? CMB200_HIT : CMB200_MISS;
-		if (present) memcpy((uint8_t *)pages_out + i * e->bsize, s->page, e->bsize);
-		e->gets++; e->hits += present;
+		struct entry *s;
+		status_out[i] = lookup(e, &addr[i], &s);
+		if (s) memcpy((uint8_t *)pages_out + i * e->bsize, s->page, e->bsize);
+		e->gets++; e->hits += s != NULL;
 	}
 	pthread_mutex_unlock(&e->mu);
 	return 0;

@@ -4,7 +4,7 @@
 own uint128.h).  Run in the authoring container only; the fixtures it writes are committed and
 are what pins the oracle (and, on the GPU box, the CUDA path) where /root/reference is absent.
 
-    python tools/gen_golden.py [lz4 keys ref_blocks limit exerciser store]
+    python tools/gen_golden.py [lz4 keys ref_blocks limit exerciser key_edges store]
 """
 from __future__ import annotations
 
@@ -211,10 +211,161 @@ def gen_store():
     os._exit(0)
 
 
+KEY_EDGE_PSHIFTS = (12, 16, 17)         # the page sizes of the GPU replay: k_get_small 4 KiB, 64 KiB, pair 128 KiB
+
+
+def key_edge_groups():
+    """Addresses that share a store key (FNV-1a-64 of the 16 address bytes), found by tools/fnv_preimage.py
+    from fixed seeds: a group of four, three pairs, three addresses each for the table's empty (0) and
+    tombstone (~0) keys, and ordinary addresses whose keys are all different."""
+    import random
+    import fnv_preimage as F
+    base = (0x1234, 0x100000000007)
+    groups = {"quad": [base] + F.preimages(F.addr_key(*base), 3, seed=1, avoid=[base])}
+    rng = random.Random(7)
+    for i in range(3):
+        a = (rng.getrandbits(64), rng.getrandbits(64))
+        groups[f"pair{i}"] = [a] + F.preimages(F.addr_key(*a), 1, seed=10 + i, avoid=[a])
+    groups["key0"] = F.preimages(0, 3, seed=20)
+    groups["key_ones"] = F.preimages(F.MASK, 3, seed=21)
+    ordinary = [(rng.getrandbits(64), rng.getrandbits(64)) for _ in range(6)]
+    keys = [F.addr_key(*a) for a in ordinary] + [F.addr_key(*g[0]) for g in groups.values()]
+    assert len(set(keys)) == len(keys)
+    for g in groups.values():
+        assert len(set(g)) == len(g) and len({F.addr_key(*a) for a in g}) == 1
+    return groups, ordinary
+
+
+def key_edge_script(groups, ordinary):
+    """Ops [kind, u, l, content]: per group (members A, B, C...) put A, get A, put B, get A, get B; put A
+    again, get B, get A; unset through C (B for a pair), get every member; put B again, get B, get A —
+    with an ordinary address put and read around each group."""
+    kinds = "TMRXZ"
+    ops, seed = [], [0]
+
+    def put(a):
+        seed[0] += 1
+        ops.append(["put", a[0], a[1], [kinds[seed[0] % len(kinds)], seed[0]]])
+
+    def get(a):
+        ops.append(["get", a[0], a[1], None])
+
+    for gi, g in enumerate(groups.values()):
+        A, B = g[0], g[1]
+        C = g[2] if len(g) > 2 else B
+        o = ordinary[gi % len(ordinary)]
+        put(o)
+        put(A); get(A); put(B); get(A); get(B)
+        get(o)
+        put(A); get(B); get(A)
+        ops.append(["unset", C[0], C[1], None])
+        for a in g:
+            get(a)
+        get(o)
+        put(B); get(B); get(A)
+    for o in ordinary:
+        get(o)
+    return ops
+
+
+def _key_edges_ref(pshift: str, ops_path: str, destdir: str):
+    """Child process of gen_key_edges: replays the ops against the reference, writing after each op
+    (and after the reference's own stdout has been flushed) `op <i> <answer>`, then one JSON line."""
+    pshift = int(pshift)
+    R = O.ref()
+    R.filemap_unset.restype = None
+    R.filemap_unset.argtypes = [C.c_void_p, C.c_void_p]
+    libc = C.CDLL(None)
+    libc.free.argtypes = [C.c_void_p]
+    libc.fflush.argtypes = [C.c_void_p]
+    with open(ops_path) as f:
+        ops = json.load(f)
+    cm = R.cachemap_create(destdir.encode(), 1024, 12, pshift)
+    assert cm
+    pages_ptr = C.cast(cm, C.POINTER(C.c_void_p))[0]                          # cm->pages
+    for i, (kind, u, l, content) in enumerate(ops):
+        off, gen = (l & ((1 << 44) - 1)) << pshift, l >> 44
+        ans = "-"
+        if kind == "put":
+            page = datagen.make_page(content[0], 1 << pshift, content[1])
+            R.cachemap_put(cm, off, u, gen, page.ctypes.data)
+        elif kind == "unset":
+            R.filemap_unset(pages_ptr, (C.c_uint64 * 2)(u, l))
+        else:
+            p = R.cachemap_get(cm, off, u, gen)
+            ans = sha(C.string_at(p, 1 << pshift)) if p else "miss"
+            if p:
+                libc.free(p)
+        libc.fflush(None)
+        os.write(1, f"op {i} {ans}\n".encode())
+    entries = int(R.filemap_entries(pages_ptr))
+    sz = 8 + 8 + 8 + 4 * 8 + 48 + 40 + 8 + 3 * 8                               # as in gen_store
+    _, req, hits = np.frombuffer(C.string_at(cm, sz)[-24:], dtype=np.uint64)
+    libc.fflush(None)
+    os.write(1, (json.dumps({"entries": entries, "requests": int(req), "hits": int(hits)}) + "\n").encode())
+    os._exit(0)                             # no cachemap_free(): it can hang in the reference (SURVEY.md §5)
+
+
+def gen_key_edges():
+    """tests/golden/key_edges.json: colliding and sentinel-key addresses and the reference's answers to a
+    trace over them at every page size of KEY_EDGE_PSHIFTS.  Each get's answer is the SHA-256 of the page,
+    "miss", or "bad entry" when the reference printed `bad entry` for it (filemap.c:237)."""
+    import re
+    import shutil
+    groups, ordinary = key_edge_groups()
+    ops = key_edge_script(groups, ordinary)
+    runs = {}
+    with tempfile.TemporaryDirectory() as tmp:
+        ops_path = os.path.join(tmp, "ops.json")
+        with open(ops_path, "w") as f:
+            json.dump(ops, f)
+        for pshift in KEY_EDGE_PSHIFTS:
+            for attempt in range(8):                    # the reference can hang at start-up (SURVEY.md §5)
+                d = tempfile.mkdtemp(dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
+                try:
+                    out = subprocess.run([sys.executable, os.path.abspath(__file__), "_key_edges_ref", str(pshift),
+                                          ops_path, d], capture_output=True, text=True, timeout=120).stdout
+                    break
+                except subprocess.TimeoutExpired:
+                    continue
+                finally:
+                    shutil.rmtree(d, ignore_errors=True)
+            else:
+                raise RuntimeError("the reference hung in every attempt")
+            lines = out.splitlines()
+            tail = json.loads(lines[-1])
+            gets, bad_since = [], 0
+            for line in lines[:-1]:
+                if line == "bad entry":
+                    bad_since += 1
+                    continue
+                m = re.fullmatch(r"op (\d+) (\S+)", line)
+                assert m, line
+                i, ans = int(m.group(1)), m.group(2)
+                assert bad_since <= (ops[i][0] == "get" and ans == "miss"), (i, ans, bad_since)
+                if ops[i][0] == "get":
+                    gets.append("bad entry" if bad_since else ans)
+                bad_since = 0
+            assert len(gets) == sum(op[0] == "get" for op in ops)
+            runs[str(pshift)] = {"gets": gets, "bad_entries": gets.count("bad entry"), **tail}
+    with open(os.path.join(GOLD, "key_edges.json"), "w") as f:
+        json.dump({"generator": "tools/gen_golden.py key_edges (addresses: tools/fnv_preimage.py) against "
+                   "libcachemap_ref.so (LMDB on tmpfs): cachemap_put, cachemap_get, filemap_unset",
+                   "capacity": 1024, "accel": 12,
+                   "op": "[kind, u, l, content]: offset = (l & (2^44 - 1)) << pshift, nhid = u, genid = l >> 44; "
+                         "content = datagen.make_page(content[0], 1 << pshift, content[1])",
+                   "groups": {k: [list(a) for a in v] for k, v in groups.items()},
+                   "ordinary": [list(a) for a in ordinary], "ops": ops, "runs": runs}, f, indent=0)
+    print("key edges ops:", len(ops), {p: {k: v for k, v in r.items() if k != "gets"} for p, r in runs.items()})
+
+
 if __name__ == "__main__":
+    if sys.argv[1:2] == ["_key_edges_ref"]:
+        _key_edges_ref(*sys.argv[2:])
     assert O.ref() is not None, "oracle/_ref/libcachemap_ref.so missing: run make -C oracle"
     os.makedirs(GOLD, exist_ok=True)
+    sys.path.insert(0, os.path.join(ROOT, "tools"))
     steps = {"lz4": gen_lz4, "keys": gen_keys, "ref_blocks": gen_ref_blocks, "limit": gen_limit, "exerciser": gen_exerciser,
-             "store": gen_store}                   # gen_store ends the process: keep it last
+             "key_edges": gen_key_edges, "store": gen_store}   # gen_store ends the process: keep it last
     for name in sys.argv[1:] or steps:
         steps[name]()
