@@ -40,6 +40,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_promote_batch", "cmb200_host_tier_hot", "cmb200_read_checkpoints",
     "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
     "cmb200_verify_stats", "cmb200_verify_store", "cmb200_snapshot_begin", "cmb200_snapshot_finish",
+    "cmb200_chain_begin", "cmb200_load_chain",
 ]
 
 
@@ -169,6 +170,8 @@ def lib() -> C.CDLL:
         "cmb200_verify_store": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_snapshot_begin": (vp, [vp, i32, C.c_char_p]),
         "cmb200_snapshot_finish": (i32, [vp, vp]),
+        "cmb200_chain_begin": (vp, [vp, i32, C.c_char_p, i32]),
+        "cmb200_load_chain": (i32, [vp, i32, C.c_char_p, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -640,6 +643,25 @@ def load_set(handles, path: str) -> int:
     n = C.c_uint64(0)
     _check(lib().cmb200_load_set(arr, g, path.encode(), C.byref(n)), "cmb200_load_set")
     return n.value
+
+
+def chain_begin(handles, base_path: str, delta: bool) -> int:
+    """cmb200_chain_begin over engine handles -> snapshot handle for snapshot_finish.  delta=False
+    writes a base at base_path with a fresh chain id, delta=True the chain's next base_path.d<k>."""
+    arr, g = _handles(handles)
+    s = lib().cmb200_chain_begin(arr, g, base_path.encode(), int(bool(delta)))
+    if not s:
+        raise RuntimeError(f"cmb200_chain_begin failed: {last_error()}")
+    return int(s)
+
+
+def load_chain(handles, base_path: str):
+    """cmb200_load_chain over engine handles -> (records loaded, deltas applied)."""
+    arr, g = _handles(handles)
+    n = C.c_uint64(0)
+    k = C.c_uint32(0)
+    _check(lib().cmb200_load_chain(arr, g, base_path.encode(), C.byref(n), C.byref(k)), "cmb200_load_chain")
+    return n.value, k.value
 
 
 class Cachemap:

@@ -29,6 +29,7 @@
  * (set CMB200_SOFT_FAIL=1 to degrade to "every put dropped, every get a miss" instead).
  */
 #define _GNU_SOURCE
+#include <dirent.h>
 #include <errno.h>
 #include <pthread.h>
 #include <stdio.h>
@@ -58,6 +59,9 @@ extern int cmb200_owner(uint64_t key, int g);
 #pragma weak cmb200_host_tier_hot
 #pragma weak cmb200_save_set
 #pragma weak cmb200_load_set
+#pragma weak cmb200_chain_begin
+#pragma weak cmb200_snapshot_finish
+#pragma weak cmb200_load_chain
 #pragma weak cmb200_move_pages
 #pragma weak cmb200_copy_peer
 #pragma weak cmb200_dev_alloc
@@ -159,6 +163,8 @@ struct filemap {
 	/* persistence: <destdir>/cachemap_b200.snap (cmb200_save_set / cmb200_load_set) */
 	int persist;
 	long checkpoint_sec;    /* > 0: the checkpoint thread saves a snapshot this often when puts have landed */
+	long checkpoint_deltas; /* CMB200_CHECKPOINT_DELTAS: > 0 = its ticks write deltas of a chain, at most this many per base */
+	int chain_deltas;       /* deltas of the chain at the snapshot path, -1 = no chain open (under snap_mu) */
 	uint64_t puts_seen, puts_saved; /* (atomic) */
 	pthread_mutex_t snap_mu;
 	/* the checkpoint thread (CMB200_CHECKPOINT_SEC): sleeps on ckpt_cv, so that filemap_free can wake it */
@@ -376,10 +382,21 @@ filemap_engine_ready(struct filemap *m)
 			 * any number of engines loads into this one's. */
 			m->persist = (int)env_long("CMB200_PERSIST", 1);
 			m->checkpoint_sec = env_long("CMB200_CHECKPOINT_SEC", 0);
-			char snap[2200];
+			m->checkpoint_deltas = env_long("CMB200_CHECKPOINT_DELTAS", 0);
+			m->chain_deltas = -1;
+			char snap[2200], d1[2300];
 			if (m->persist && filemap_snapshot_path(m, snap, sizeof(snap)) && access(snap, R_OK) == 0) {
 				uint64_t got = 0;
-				if (!cmb200_load_set)
+				uint32_t k = 0;
+				snprintf(d1, sizeof(d1), "%s.d1", snap);
+				/* a chain next to the base is never ignored, whatever CMB200_CHECKPOINT_DELTAS says now;
+				 * a base whose deltas do not match it loads alone */
+				if (cmb200_load_chain && (m->checkpoint_deltas > 0 || access(d1, R_OK) == 0)) {
+					if (cmb200_load_chain(m->engs, g, snap, &got, &k) != 0)
+						fprintf(stderr, "cachemap_b200: %s ignored: %s\n", snap, cmb200_last_error());
+					else
+						m->chain_deltas = (int)k;
+				} else if (!cmb200_load_set)
 					fprintf(stderr, "cachemap_b200: %s ignored: the engine cannot load snapshots\n", snap);
 				else if (cmb200_load_set(m->engs, g, snap, &got) != 0)
 					fprintf(stderr, "cachemap_b200: %s ignored: %s\n", snap, cmb200_last_error());
@@ -427,22 +444,89 @@ filemap_create(char *destdir, uint64_t n, int compress_accel, int pshift)
 	return m;
 }
 
-/* Saves the store to <destdir>/cachemap_b200.snap.  0 = saved, -1 = not (disabled, engine never
- * started, or I/O error). */
+/* Removes the deltas (and half-written deltas) of any chain next to the base at `snap`: a base that
+ * was just renamed into place has a chain id of its own, or none. */
+static void
+filemap_remove_deltas(struct filemap *m)
+{
+	DIR *dir = opendir(m->destdir);
+	if (!dir)
+		return;
+	const char *stem = SNAPSHOT_NAME ".d";
+	struct dirent *ent;
+	char path[2600];
+	while ((ent = readdir(dir)) != NULL)
+		if (strncmp(ent->d_name, stem, strlen(stem)) == 0 &&
+		    snprintf(path, sizeof(path), "%s/%s", m->destdir, ent->d_name) < (int)sizeof(path))
+			unlink(path);
+	closedir(dir);
+}
+
+static long long
+file_bytes(const char *path)
+{
+	struct stat st;
+	return stat(path, &st) == 0 ? (long long)st.st_size : -1;
+}
+
+/* CMB200_CHECKPOINT_DELTAS: one tick of the chain at `snap` (under snap_mu).  A tick of the checkpoint
+ * thread writes the chain's next delta; it writes a base instead when no chain is open (none yet, or a
+ * load left the engines without chain state), when the chain already has checkpoint_deltas deltas, or
+ * when its deltas together are as large as its base, so that a chain stays within about twice the store.
+ * cachemap_checkpoint and cachemap_free always write a base. */
 static int
-filemap_save(struct filemap *m)
+filemap_save_chain(struct filemap *m, const char *snap, int tick)
+{
+	int delta = tick && m->chain_deltas >= 0 && m->chain_deltas < m->checkpoint_deltas;
+	if (delta) {
+		long long sum = 0;
+		char path[2300];
+		for (int k = 1; k <= m->chain_deltas; k++) {
+			snprintf(path, sizeof(path), "%s.d%d", snap, k);
+			const long long b = file_bytes(path);
+			sum += b > 0 ? b : 0;
+		}
+		delta = sum < file_bytes(snap);
+	}
+	cmb200_snapshot *s = delta ? cmb200_chain_begin(m->engs, m->g, snap, 1) : NULL;
+	if (!s) {
+		delta = 0;
+		s = cmb200_chain_begin(m->engs, m->g, snap, 0);
+	}
+	const int rc = s ? cmb200_snapshot_finish(s, NULL) : -1;
+	if (rc == 0 && delta)
+		m->chain_deltas++;
+	else if (rc == 0) {
+		m->chain_deltas = 0;
+		filemap_remove_deltas(m);
+	}
+	return rc;
+}
+
+/* Saves the store to <destdir>/cachemap_b200.snap (tick: a save of the checkpoint thread, which may
+ * write a delta instead).  0 = saved, -1 = not (disabled, engine never started, or I/O error). */
+static int
+filemap_save(struct filemap *m, int tick)
 {
 	char snap[2200];
 	if (__atomic_load_n(&m->init_state, __ATOMIC_ACQUIRE) != 1 || !m->persist ||
 	    !filemap_snapshot_path(m, snap, sizeof(snap)))
 		return -1;
-	if (!cmb200_save_set) {
+	const int chain = m->checkpoint_deltas > 0 && cmb200_chain_begin && cmb200_snapshot_finish;
+	if (!chain && !cmb200_save_set) {
 		fprintf(stderr, "cachemap_b200: snapshot not written: the engine cannot save snapshots\n");
 		return -1;
 	}
 	pthread_mutex_lock(&m->snap_mu);
 	uint64_t seen = __atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED);
-	int rc = cmb200_save_set(m->engs, m->g, snap, NULL);
+	int rc;
+	if (chain)
+		rc = filemap_save_chain(m, snap, tick);
+	else if ((rc = cmb200_save_set(m->engs, m->g, snap, NULL)) == 0 && m->chain_deltas >= 0) {
+		/* a chain loaded at start is folded into this base */
+		m->chain_deltas = -1;
+		filemap_remove_deltas(m);
+	}
 	if (rc == 0)
 		__atomic_store_n(&m->puts_saved, seen, __ATOMIC_RELAXED);
 	else
@@ -469,7 +553,7 @@ filemap_checkpointer(void *arg)
 			break;
 		pthread_mutex_unlock(&m->ckpt_mu);
 		if (__atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED) != __atomic_load_n(&m->puts_saved, __ATOMIC_RELAXED))
-			filemap_save(m);
+			filemap_save(m, 1);
 		pthread_mutex_lock(&m->ckpt_mu);
 	}
 	pthread_mutex_unlock(&m->ckpt_mu);
@@ -531,7 +615,7 @@ filemap_free(struct filemap *m)
 		pthread_mutex_unlock(&d->wb_mu);
 		pthread_join(d->wb_thread, NULL);      /* drains the ring first */
 	}
-	filemap_save(m);                                /* the cache directory outlives the process */
+	filemap_save(m, 0);                             /* the cache directory outlives the process */
 	for (int i = 0; i < m->g; i++) {
 		/* staging first, while every engine that allocated it is alive */
 		struct fm_dev *d = m->dev[i];
@@ -2006,7 +2090,7 @@ cachemap_checkpoint(struct cachemap *cm)
 	if (!filemap_engine_ready(cm->pages))
 		return -1;
 	filemap_drain(cm->pages);
-	return filemap_save(cm->pages);
+	return filemap_save(cm->pages, 0);
 }
 
 void

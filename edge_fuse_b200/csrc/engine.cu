@@ -14,6 +14,7 @@
 #include <atomic>
 #include <condition_variable>
 #include <deque>
+#include <dirent.h>
 #include <mutex>
 #include <set>
 #include <shared_mutex>
@@ -26,6 +27,8 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <time.h>
+#include <unistd.h>
 #include <vector>
 #include "../../include/cachemap_b200.h"
 #include "../../include/uint128.h"
@@ -271,6 +274,25 @@ struct cmb200_engine {
 	std::condition_variable snap_cv;
 	HostMem<uint8_t> snap_win;           // page-locked window of the writer, kept from the first snapshot on
 	Stream snap_st;                      // the writer's copies: they do not queue behind encodes on st
+	// snapshot chains (cmb200_chain_begin): the file `id` and its `k` deltas describe this engine's
+	// records as of the last tick, whose watermark was w (every record version put since has seq >= w)
+	// and whose live addresses are the baseline base[cur][0 .. n).  The baseline is page-locked,
+	// device-mapped host memory, double-buffered: a tick's export writes the next one into the other
+	// half.  A tick that is listed and not finished keeps its results in the *_next fields until
+	// cmb200_snapshot_finish commits them (the file is in place) or drops them.  Under mu.
+	struct Chain {
+		uint64_t id = 0;                 // 0 = no chain state: the next tick must write a base
+		uint32_t k = 0;
+		unsigned long long w = 0;
+		HostMem<ulonglong2> base[2];
+		ulonglong2 *base_dev[2] = {};
+		uint64_t cap[2] = {}, n = 0;
+		int cur = 0;
+		bool pending = false;
+		uint64_t id_next = 0, n_next = 0;
+		uint32_t k_next = 0;
+		unsigned long long w_next = 0;
+	} chain;
 };
 
 static uint64_t next_pow2(uint64_t v) {
@@ -1087,20 +1109,24 @@ extern "C" int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_
 // Every live local record (arena_only: leave out the host tier's), sorted by offset, and the counters
 // read just before the export.  (e->mu held)  0 = listed, -1 = a CUDA call failed (error set), 1 = more
 // than c[0] + 16 records were found (the store changed since the counters were read): the list holds
-// c[0] + 16 of them.
-static int live_records(cmb200_engine *e, bool arena_only, std::vector<ExportEntry> &list, unsigned long long c[8]) {
+// c[0] + 16 of them.  seq_min and addr_out as for launch_export_list; addr_out (device address, room for
+// c[0] + 16) then gets every live local address and *n_addr their number.
+static int live_records(cmb200_engine *e, bool arena_only, std::vector<ExportEntry> &list, unsigned long long c[8],
+    unsigned long long seq_min = 0, ulonglong2 *addr_out = nullptr, uint64_t *n_addr = nullptr) {
 	if (read_counters(e, c)) return -1;
 	const unsigned long long cap_out = c[0] + 16;
 	DevMem<ExportEntry> d_list;
 	DevMem<unsigned long long> d_count;
-	if (d_list.alloc(cap_out * sizeof(ExportEntry) + 256) || d_count.alloc(8 + 256)) return -1;
-	CMB_CHECK(cudaMemsetAsync(d_count, 0, 8, e->st));
-	if (launch_export_list(e->table, e->bsize, d_list, d_count, cap_out, arena_only, e->st)) return -1;
-	unsigned long long count = 0;
-	CMB_CHECK(cudaMemcpyAsync(&count, d_count, 8, cudaMemcpyDeviceToHost, e->st));
+	if (d_list.alloc(cap_out * sizeof(ExportEntry) + 256) || d_count.alloc(16 + 256)) return -1;
+	CMB_CHECK(cudaMemsetAsync(d_count, 0, 16, e->st));
+	if (launch_export_list(e->table, e->bsize, d_list, d_count, cap_out, arena_only, e->st, seq_min, addr_out)) return -1;
+	unsigned long long counts[2] = {0, 0};
+	CMB_CHECK(cudaMemcpyAsync(counts, d_count, 16, cudaMemcpyDeviceToHost, e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
-	const int over = count > cap_out;
-	if (over) count = cap_out;
+	unsigned long long count = counts[0];
+	int over = count > cap_out || counts[1] > cap_out;
+	if (count > cap_out) count = cap_out;
+	if (n_addr) *n_addr = counts[1] < cap_out ? counts[1] : cap_out;
 	list.resize(count);
 	if (count) CMB_CHECK(cudaMemcpy(list.data(), d_list, count * sizeof(ExportEntry), cudaMemcpyDeviceToHost));
 	std::sort(list.begin(), list.end(), [](const ExportEntry &a, const ExportEntry &b) { return a.rec_off < b.rec_off; });
@@ -1185,6 +1211,37 @@ static int write_section(cmb200_engine *e, FILE *f, const std::vector<ExportEntr
 	return ok ? 0 : -2;
 }
 
+// ---- snapshot chains (cmb200_chain_begin / cmb200_load_chain) ----
+// A base is the file above with a nonzero 64-bit chain id in bytes 40..47 (pad[1..2], zero in a file
+// written by cmb200_save_set).  Delta k of that chain, <base>.d<k>, holds what changed between tick k-1
+// (tick 0 = the base) and tick k:
+//
+//   header      "CMB200D1" | u32 version=1 | u32 pshift | u64 chain id | u32 k | u32 flags |
+//               u64 tombstones | u64 records | u64 record bytes | pad to 64
+//   tombstones  16-byte addresses that were live at tick k-1 and are not at tick k
+//   records     every live local record put since tick k-1, in the base's record format
+//
+// The store of a chain is the base, then for each delta in order its tombstones removed and its records
+// put.  "Put since tick k-1" is Slot::seq >= the engine's seq at tick k-1: every put raises the slot's
+// seq (k_upsert), a table rebuild copies it, and compaction, demotion and promotion leave it alone, so
+// a record that only moved is not in the delta.
+struct DeltaHeader {
+	char magic[8];
+	uint32_t version, pshift;
+	uint64_t chain;
+	uint32_t index, flags;
+	uint64_t tombstones, records, bytes, pad;
+};
+static_assert(sizeof(DeltaHeader) == 64, "delta header");
+
+static uint64_t snap_chain_id(const SnapHeader &h) {
+	uint64_t id;
+	memcpy(&id, &h.pad[1], 8);
+	return id;
+}
+
+enum { CHAIN_NONE = 0, CHAIN_BASE, CHAIN_DELTA };
+
 struct cmb200_snapshot {
 	std::vector<cmb200_engine *> engines;                 // in file order
 	std::vector<std::vector<ExportEntry>> lists;          // each engine's live records at begin, by offset
@@ -1194,12 +1251,18 @@ struct cmb200_snapshot {
 	std::thread writer;
 	int rc = 0;                                           // the writer's: 0, -1 CUDA, -2 file
 	std::string err;                                      // the writer's error text (g_err is per thread)
+	int chain = CHAIN_NONE;
+	DeltaHeader dh{};                                     // CHAIN_DELTA: the header written instead of h
+	std::vector<ulonglong2> tombs;                        // CHAIN_DELTA: every engine's tombstones
 };
 
 // The writer thread: header, then each engine's section; an engine is released as soon as its section
 // is written (or the write has failed), so that its compactions and tier laps go ahead.
 static void snapshot_write(cmb200_snapshot *s) {
-	bool ok = fwrite(&s->h, sizeof(s->h), 1, s->f) == 1;
+	bool ok = s->chain == CHAIN_DELTA
+	    ? fwrite(&s->dh, sizeof(s->dh), 1, s->f) == 1 &&
+	      (s->tombs.empty() || fwrite(s->tombs.data(), 16, s->tombs.size(), s->f) == s->tombs.size())
+	    : fwrite(&s->h, sizeof(s->h), 1, s->f) == 1;
 	int rc = ok ? 0 : -2;
 	for (size_t i = 0; i < s->engines.size(); i++) {
 		cmb200_engine *e = s->engines[i];
@@ -1218,7 +1281,58 @@ static void snapshot_write(cmb200_snapshot *s) {
 	s->rc = rc;
 }
 
-extern "C" cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines, int g, const char *path) {
+// Makes room for c0 + 16 addresses in the half of e's baseline that the next tick writes.  (e->mu held)
+static int chain_room(cmb200_engine *e, unsigned long long c0) {
+	cmb200_engine::Chain &ch = e->chain;
+	const int nx = ch.cur ^ 1;
+	const uint64_t need = c0 + 16;
+	if (ch.cap[nx] >= need) return 0;
+	const uint64_t cap = need + need / 4 + 1024;
+	ch.cap[nx] = 0; ch.base_dev[nx] = nullptr;
+	if (ch.base[nx].alloc(cap * 16, true)) return -1;
+	void *dev = nullptr;
+	CMB_CHECK(cudaHostGetDevicePointer(&dev, (void *)ch.base[nx], 0));
+	ch.base_dev[nx] = (ulonglong2 *)dev;
+	ch.cap[nx] = cap;
+	return 0;
+}
+
+// Lists engine i of a chain tick (e->mu held): the tombstones against the previous baseline (a delta),
+// then the records put since the previous watermark (a delta) or all of them (a base), with the next
+// baseline exported by the same pass.  The results wait in the *_next fields for cmb200_snapshot_finish.
+static int chain_list(cmb200_engine *e, cmb200_snapshot *s, int i) {
+	cmb200_engine::Chain &ch = e->chain;
+	const bool delta = s->chain == CHAIN_DELTA;
+	if (ch.pending) { set_error_msg("cmb200_chain_begin: a chain tick of this engine is not finished"); return -1; }
+	if (delta && (ch.id != s->dh.chain || ch.k + 1 != s->dh.index)) {
+		set_error_msg("cmb200_chain_begin: an engine holds no chain state for this base: write a base first");
+		return -1;
+	}
+	unsigned long long c[8];
+	if (read_counters(e, c) || chain_room(e, c[0])) return -1;
+	if (delta && ch.n) {
+		DevMem<ulonglong2> d_out;
+		DevMem<unsigned long long> d_cnt;
+		if (d_out.alloc(ch.n * 16 + 256) || d_cnt.alloc(8 + 256)) return -1;
+		CMB_CHECK(cudaMemsetAsync(d_cnt, 0, 8, e->st));
+		if (launch_delta_gone(e->table, ch.base_dev[ch.cur], ch.n, d_out, d_cnt, e->st)) return -1;
+		unsigned long long nt = 0;
+		CMB_CHECK(cudaMemcpyAsync(&nt, d_cnt, 8, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		const size_t at = s->tombs.size();
+		s->tombs.resize(at + nt);
+		if (nt) CMB_CHECK(cudaMemcpy(s->tombs.data() + at, d_out, nt * 16, cudaMemcpyDeviceToHost));
+	}
+	uint64_t n_next = 0;
+	if (live_records(e, false, s->lists[i], c, delta ? ch.w : 0, ch.base_dev[ch.cur ^ 1], &n_next) < 0) return -1;
+	// the stream is synchronised and mu held: every record version put so far has seq < e->seq, every later one >=
+	ch.w_next = e->seq; ch.n_next = n_next; ch.id_next = s->dh.chain; ch.k_next = s->dh.index;
+	ch.pending = true;
+	return 0;
+}
+
+static cmb200_snapshot *snapshot_start(cmb200_engine *const *engines, int g, const char *path, int chain,
+    uint64_t chain_id, uint32_t k) {
 	if (g < 1 || !engines || !path) { set_error_msg("cmb200_snapshot_begin: no engines"); return nullptr; }
 	for (int i = 1; i < g; i++)
 		if (engines[i]->pshift != engines[0]->pshift) { set_error_msg("cmb200_save_set: engines of different page sizes"); return nullptr; }
@@ -1252,16 +1366,26 @@ extern "C" cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines,
 	s->h = SnapHeader{};
 	memcpy(s->h.magic, "CMB200S1", 8);
 	s->h.version = 1; s->h.pshift = (uint32_t)engines[0]->pshift;
+	s->chain = chain;
+	s->dh.chain = chain_id; s->dh.index = k;
+	if (chain == CHAIN_BASE) memcpy(&s->h.pad[1], &chain_id, 8);
+	int listed = 0;                                       // engines whose chain tick is pending
 	for (int i = 0; i < g && rc == 0; i++) {
 		cmb200_engine *e = engines[i];
 		std::lock_guard<std::mutex> lk(e->mu);
 		if (i == 0) s->h.flags = e->table.fp ? 1u : 0u;
 		unsigned long long c[8];
 		// live_records synchronises the stream first: every put enqueued before now is listed
-		if (live_records(e, false, s->lists[i], c) < 0) { rc = -1; break; }
+		if (chain != CHAIN_NONE ? chain_list(e, s, i) : live_records(e, false, s->lists[i], c) < 0) { rc = -1; break; }
+		listed++;
 		snap_set_state(e, cmb200_engine::SNAP_PENDING);
 		s->h.records += s->lists[i].size();
 		for (const ExportEntry &x : s->lists[i]) s->h.bytes += x.len;
+	}
+	if (chain == CHAIN_DELTA) {
+		memcpy(s->dh.magic, "CMB200D1", 8);
+		s->dh.version = 1; s->dh.pshift = s->h.pshift; s->dh.flags = s->h.flags;
+		s->dh.tombstones = s->tombs.size(); s->dh.records = s->h.records; s->dh.bytes = s->h.bytes;
 	}
 	if (rc == 0) {
 		try {
@@ -1273,10 +1397,48 @@ extern "C" cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines,
 	}
 	if (rc == 0) return s;
 	for (cmb200_engine *e : order) snap_set_state(e, cmb200_engine::SNAP_FREE);
+	for (int i = 0; i < listed && chain != CHAIN_NONE; i++) {
+		std::lock_guard<std::mutex> lk(engines[i]->mu);
+		engines[i]->chain.pending = false;
+	}
 	fclose(s->f);
 	remove(s->tmp.c_str());
 	delete s;
 	return nullptr;
+}
+
+extern "C" cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines, int g, const char *path) {
+	return snapshot_start(engines, g, path, CHAIN_NONE, 0, 0);
+}
+
+extern "C" cmb200_snapshot *cmb200_chain_begin(cmb200_engine *const *engines, int g, const char *base_path, int delta) {
+	if (g < 1 || !engines || !base_path) { set_error_msg("cmb200_chain_begin: no engines"); return nullptr; }
+	if (!delta) {
+		// a fresh id: the deltas of any earlier chain next to this base stop matching it
+		uint64_t id = 0;
+		while (id == 0) {
+			struct timespec ts;
+			clock_gettime(CLOCK_REALTIME, &ts);
+			static std::atomic<uint64_t> calls{0};
+			const uint64_t seed[2] = {(uint64_t)ts.tv_sec * 1000000000ull + (uint64_t)ts.tv_nsec,
+			    ((uint64_t)getpid() << 32) ^ (uint64_t)(uintptr_t)engines[0] ^ calls.fetch_add(1)};
+			FNV_hash(seed, 16, &id);
+		}
+		return snapshot_start(engines, g, base_path, CHAIN_BASE, id, 0);
+	}
+	SnapHeader h{};
+	FILE *f = fopen(base_path, "rb");
+	const bool ok = f && fread(&h, sizeof(h), 1, f) == 1 && memcmp(h.magic, "CMB200S1", 8) == 0 && h.version == 1;
+	if (f) fclose(f);
+	if (!ok || snap_chain_id(h) == 0) { set_error_msg("cmb200_chain_begin: no chain base at this path"); return nullptr; }
+	uint32_t k;
+	{
+		// checked against every engine under its lock when the tick lists it
+		std::lock_guard<std::mutex> lk(engines[0]->mu);
+		k = engines[0]->chain.k + 1;
+	}
+	const std::string path = std::string(base_path) + ".d" + std::to_string(k);
+	return snapshot_start(engines, g, path.c_str(), CHAIN_DELTA, snap_chain_id(h), k);
 }
 
 extern "C" int cmb200_snapshot_finish(cmb200_snapshot *s, uint64_t *records_out) {
@@ -1293,6 +1455,16 @@ extern "C" int cmb200_snapshot_finish(cmb200_snapshot *s, uint64_t *records_out)
 	}
 	if (rc) remove(s->tmp.c_str());
 	else if (records_out) *records_out = s->h.records;
+	// a chain tick becomes the engines' chain state only once its file is in place
+	for (size_t i = 0; i < s->engines.size() && s->chain != CHAIN_NONE; i++) {
+		cmb200_engine *e = s->engines[i];
+		std::lock_guard<std::mutex> lk(e->mu);
+		cmb200_engine::Chain &ch = e->chain;
+		if (rc == 0) {
+			ch.cur ^= 1; ch.n = ch.n_next; ch.w = ch.w_next; ch.id = ch.id_next; ch.k = ch.k_next;
+		}
+		ch.pending = false;
+	}
 	delete s;
 	return rc;
 }
@@ -1360,39 +1532,59 @@ static long long load_flush(LoadBatch &b, bool with_fp) {
 	return (long long)m;
 }
 
-extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out) {
-	if (records_out) *records_out = 0;
-	if (g < 1 || !engines) { set_error_msg("cmb200_load_set: no engines"); return -1; }
+struct AddrHash {
+	size_t operator()(const std::pair<uint64_t, uint64_t> &a) const { return (size_t)(a.first * 0x9E3779B97F4A7C15ull ^ a.second); }
+};
+typedef std::unordered_set<std::pair<uint64_t, uint64_t>, AddrHash> AddrSet;
+
+// Opens a snapshot file (a base) for a load into g engines and reads its header.  nullptr on failure
+// (error set).
+static FILE *open_snapshot(cmb200_engine *const *engines, int g, const char *path, SnapHeader &h) {
 	FILE *f = fopen(path, "rb");
-	if (!f) { set_error_msg("cmb200_load: no snapshot file"); return -1; }
-	SnapHeader h{};
+	if (!f) { set_error_msg("cmb200_load: no snapshot file"); return nullptr; }
 	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "CMB200S1", 8) != 0 || h.version != 1) {
-		fclose(f); set_error_msg("cmb200_load: not a snapshot of this library"); return -1;
+		fclose(f); set_error_msg("cmb200_load: not a snapshot of this library"); return nullptr;
 	}
 	for (int i = 0; i < g; i++)
-		if ((int)h.pshift != engines[i]->pshift) { fclose(f); set_error_msg("cmb200_load: snapshot has another page size"); return -1; }
-	const uint32_t bsize = engines[0]->bsize;
-	std::vector<LoadBatch> bs(g);
+		if ((int)h.pshift != engines[i]->pshift) { fclose(f); set_error_msg("cmb200_load: snapshot has another page size"); return nullptr; }
+	return f;
+}
+
+// Stages the next n records of f into the load batches of their engines (cmb200_owner), flushing a batch
+// when it is full; *loaded += records put.  skip (nullable): addresses a newer file of a chain has
+// decided, whose records are passed over unread; decide (nullable) gets every address read.  The
+// batches are not flushed at the end.  0 / -1 (error set).
+static int load_records(FILE *f, uint64_t n, std::vector<LoadBatch> &bs, int g, bool with_fp, const AddrSet *skip,
+    AddrSet *decide, uint64_t *loaded) {
+	const uint32_t bsize = bs[0].e->bsize;
 	int rc = 0;
-	for (int i = 0; i < g && rc == 0; i++)
-		if (bs[i].setup(engines[i])) { rc = -1; set_error_msg("cmb200_load: no staging buffers"); }
-	uint64_t done = 0, loaded = 0;
-	while (rc == 0 && done < h.records) {
+	uint64_t done = 0;
+	while (rc == 0 && done < n) {
 		// record header and address first: the address names the engine whose batch takes the bytes
 		SnapRecord r;
 		cmb200_addr a;
 		if (fread(&r, sizeof(r), 1, f) != 1 || r.len < 24 || r.len > 24u + bsize + 1024u || fread(&a, 16, 1, f) != 1) {
 			rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
 		}
+		const size_t padded = ((size_t)r.len + 15) & ~(size_t)15;
+		if (skip || decide) {
+			const std::pair<uint64_t, uint64_t> ul(a.u, a.l);
+			const bool decided = skip && skip->count(ul);
+			if (decide && !decided) decide->insert(ul);
+			if (decided) {
+				if (fseeko(f, (off_t)(padded - 16), SEEK_CUR) != 0) { rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); }
+				done++;
+				continue;
+			}
+		}
 		uint64_t key;
 		FNV_hash(&a, 16, &key);
 		LoadBatch &b = bs[cmb200_owner(key, g)];
-		const size_t padded = ((size_t)r.len + 15) & ~(size_t)15;
 		if (padded > b.cap) { rc = -1; set_error_msg("cmb200_load: record larger than the staging buffer"); break; }
 		if (b.m == b.B || b.used + padded > b.cap) {
-			const long long got = load_flush(b, h.flags & 1u);
+			const long long got = load_flush(b, with_fp);
 			if (got < 0) { rc = -1; break; }
-			loaded += (uint64_t)got;
+			*loaded += (uint64_t)got;
 		}
 		uint8_t *rec = b.blob + b.used;
 		memcpy(rec, &a, 16);
@@ -1411,13 +1603,156 @@ extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char 
 		b.used += padded; b.m++;
 		done++;
 	}
-	for (int i = 0; i < g && rc == 0; i++) {
-		const long long got = load_flush(bs[i], h.flags & 1u);
-		if (got < 0) rc = -1;
-		else loaded += (uint64_t)got;
+	return rc;
+}
+
+static int load_flush_all(std::vector<LoadBatch> &bs, bool with_fp, uint64_t *loaded) {
+	for (LoadBatch &b : bs) {
+		const long long got = load_flush(b, with_fp);
+		if (got < 0) return -1;
+		*loaded += (uint64_t)got;
 	}
+	return 0;
+}
+
+static int load_setup(std::vector<LoadBatch> &bs, cmb200_engine *const *engines, int g) {
+	bs.resize(g);
+	for (int i = 0; i < g; i++)
+		if (bs[i].setup(engines[i])) { set_error_msg("cmb200_load: no staging buffers"); return -1; }
+	return 0;
+}
+
+extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out) {
+	if (records_out) *records_out = 0;
+	if (g < 1 || !engines) { set_error_msg("cmb200_load_set: no engines"); return -1; }
+	SnapHeader h{};
+	FILE *f = open_snapshot(engines, g, path, h);
+	if (!f) return -1;
+	std::vector<LoadBatch> bs;
+	uint64_t loaded = 0;
+	int rc = load_setup(bs, engines, g);
+	if (rc == 0) rc = load_records(f, h.records, bs, g, h.flags & 1u, nullptr, nullptr, &loaded);
+	if (rc == 0) rc = load_flush_all(bs, h.flags & 1u, &loaded);
 	fclose(f);
 	if (records_out) *records_out = loaded;
+	return rc;
+}
+
+// Opens delta k of chain `id` and checks it whole before anything of it is applied: header, then the
+// bounds of every record header and the file's exact length (the record bytes are not read).  Leaves
+// the file at its first tombstone.  nullptr when the delta is missing, from another chain, out of
+// sequence, truncated or corrupt: the chain's valid run ends before it.
+static FILE *open_delta(const std::string &path, uint64_t id, uint32_t k, uint32_t pshift, uint32_t bsize, DeltaHeader &dh) {
+	FILE *f = fopen(path.c_str(), "rb");
+	if (!f) return nullptr;
+	bool ok = fread(&dh, sizeof(dh), 1, f) == 1 && memcmp(dh.magic, "CMB200D1", 8) == 0 && dh.version == 1 &&
+	    dh.pshift == pshift && dh.chain == id && dh.index == k && fseeko(f, 0, SEEK_END) == 0;
+	const uint64_t size = ok ? (uint64_t)ftello(f) : 0;
+	uint64_t pos = sizeof(dh) + 16 * dh.tombstones, bytes = 0;
+	ok = ok && dh.tombstones <= size / 16 && pos <= size;
+	for (uint64_t i = 0; ok && i < dh.records; i++) {
+		SnapRecord r;
+		ok = pos + sizeof(r) <= size && fseeko(f, (off_t)pos, SEEK_SET) == 0 && fread(&r, sizeof(r), 1, f) == 1 &&
+		    r.len >= 24 && r.len <= 24u + bsize + 1024u;
+		pos += sizeof(r) + (((uint64_t)r.len + 15) & ~15ull);
+		bytes += r.len;
+	}
+	ok = ok && pos == size && bytes == dh.bytes && fseeko(f, sizeof(dh), SEEK_SET) == 0;
+	if (!ok) { fclose(f); return nullptr; }
+	return f;
+}
+
+// Whether a file <base_path>.d<j> with j > k exists.
+static bool delta_beyond(const char *base_path, uint32_t k) {
+	const std::string path(base_path);
+	const size_t slash = path.rfind('/');
+	const std::string dir = slash == std::string::npos ? "." : path.substr(0, slash + 1);
+	const std::string stem = (slash == std::string::npos ? path : path.substr(slash + 1)) + ".d";
+	DIR *d = opendir(dir.c_str());
+	if (!d) return true;
+	bool found = false;
+	while (struct dirent *ent = readdir(d)) {
+		const char *name = ent->d_name;
+		if (strncmp(name, stem.c_str(), stem.size()) != 0) continue;
+		const char *num = name + stem.size();
+		char *end = nullptr;
+		const unsigned long long j = strtoull(num, &end, 10);
+		if (*num >= '0' && *num <= '9' && *end == '\0' && j > k) found = true;
+	}
+	closedir(d);
+	return found;
+}
+
+extern "C" int cmb200_load_chain(cmb200_engine *const *engines, int g, const char *base_path, uint64_t *records_out,
+    uint32_t *deltas_out) {
+	if (records_out) *records_out = 0;
+	if (deltas_out) *deltas_out = 0;
+	if (g < 1 || !engines || !base_path) { set_error_msg("cmb200_load_chain: no engines"); return -1; }
+	SnapHeader h{};
+	FILE *base = open_snapshot(engines, g, base_path, h);
+	if (!base) return -1;
+	const uint64_t id = snap_chain_id(h);
+	std::vector<FILE *> ds;
+	std::vector<DeltaHeader> dhs;
+	for (uint32_t k = 1; id != 0; k++) {
+		DeltaHeader dh{};
+		FILE *f = open_delta(std::string(base_path) + ".d" + std::to_string(k), id, k, h.pshift, engines[0]->bsize, dh);
+		if (!f) break;
+		ds.push_back(f); dhs.push_back(dh);
+	}
+	uint64_t before = 0;
+	for (int i = 0; i < g; i++) before += cmb200_entries(engines[i]);
+	std::vector<LoadBatch> bs;
+	uint64_t loaded = 0;
+	int rc = load_setup(bs, engines, g);
+	// newest first: an address a newer file names (a record or a tombstone) is decided there, so every
+	// record is put once, and none an older file names in vain takes arena space
+	AddrSet decided;
+	std::vector<ulonglong2> tombs;
+	for (size_t j = ds.size(); j-- > 0 && rc == 0;) {
+		FILE *f = ds[j];
+		const DeltaHeader &dh = dhs[j];
+		tombs.resize(dh.tombstones);
+		if (dh.tombstones && fread(tombs.data(), 16, tombs.size(), f) != tombs.size()) { rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break; }
+		rc = load_records(f, dh.records, bs, g, dh.flags & 1u, &decided, &decided, &loaded);
+		if (rc == 0) rc = load_flush_all(bs, dh.flags & 1u, &loaded);
+		// the records of a delta apply after its tombstones, so its records decide first
+		for (const ulonglong2 &a : tombs) decided.insert(std::make_pair((uint64_t)a.x, (uint64_t)a.y));
+	}
+	if (rc == 0) rc = load_records(base, h.records, bs, g, h.flags & 1u, &decided, nullptr, &loaded);
+	if (rc == 0) rc = load_flush_all(bs, h.flags & 1u, &loaded);
+	for (FILE *f : ds) fclose(f);
+	fclose(base);
+	if (rc) return -1;
+	// The engines continue the chain only if they hold exactly the store it describes: they were empty
+	// and every record put is live (none dropped for lack of space, none retired by a host-tier lap),
+	// and no delta file lies beyond the run (a tick that continued it would leave that file in a valid
+	// position).  Otherwise they hold no chain state, and the next tick writes a base.
+	bool whole = id != 0 && before == 0 && !delta_beyond(base_path, (uint32_t)ds.size());
+	uint64_t live = 0;
+	for (int i = 0; i < g && rc == 0; i++) {
+		cmb200_engine *e = engines[i];
+		std::lock_guard<std::mutex> lk(e->mu);
+		cmb200_engine::Chain &ch = e->chain;
+		if (ch.pending) { whole = false; continue; }
+		unsigned long long c[8];
+		std::vector<ExportEntry> none;
+		if (read_counters(e, c) || chain_room(e, c[0]) ||
+		    live_records(e, false, none, c, ~0ull, ch.base_dev[ch.cur ^ 1], &ch.n_next) < 0) { rc = -1; break; }
+		ch.w_next = e->seq;
+		live += ch.n_next;
+	}
+	whole = whole && rc == 0 && live == loaded;
+	for (int i = 0; i < g; i++) {
+		cmb200_engine *e = engines[i];
+		std::lock_guard<std::mutex> lk(e->mu);
+		cmb200_engine::Chain &ch = e->chain;
+		if (ch.pending) continue;
+		if (whole) { ch.cur ^= 1; ch.n = ch.n_next; ch.w = ch.w_next; ch.id = id; ch.k = (uint32_t)ds.size(); }
+		else ch.id = 0;
+	}
+	if (records_out) *records_out = loaded;
+	if (deltas_out) *deltas_out = (uint32_t)ds.size();
 	return rc;
 }
 

@@ -1512,13 +1512,18 @@ int launch_read_ckpt(TableView t, const unsigned long long *addr, uint32_t n, ui
 }
 // ---- snapshot -----------------------------------------------------------------------------
 __global__ void k_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
-    unsigned long long max_out, bool arena_only) {
+    unsigned long long max_out, bool arena_only, unsigned long long seq_min, ulonglong2 *addr_out) {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= t.cap + 2) return;
 	const Slot &s = t.slots[i];
 	if (s.vlen == 0 || s.owner != 0) return;        // empty / deleted / the record lives on another GPU
 	if (arena_only && (s.rec_off & REC_HOST)) return;
 	if (i < t.cap && (s.key == KEY_EMPTY || s.key == KEY_TOMB)) return;
+	if (addr_out) {
+		const unsigned long long k = atomicAdd(count + 1, 1ull);
+		if (k < max_out) addr_out[k] = make_ulonglong2(s.addr_u, s.addr_l);
+	}
+	if (s.seq < seq_min) return;                    // put before the watermark: in an earlier file of the chain
 	const unsigned long long j = atomicAdd(count, 1ull);
 	if (j >= max_out) return;
 	ExportEntry e;
@@ -1532,9 +1537,29 @@ __global__ void k_export_list(TableView t, uint32_t bsize, ExportEntry *out, uns
 	out[j] = e;
 }
 int launch_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
-    unsigned long long max_out, bool arena_only, cudaStream_t st) {
+    unsigned long long max_out, bool arena_only, cudaStream_t st, unsigned long long seq_min, ulonglong2 *addr_out) {
 	const uint64_t n = t.cap + 2;
-	k_export_list<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, bsize, out, count, max_out, arena_only);
+	k_export_list<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, bsize, out, count, max_out, arena_only, seq_min, addr_out);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+// One thread per address of the previous tick's baseline (page-locked host memory read over PCIe, so
+// 16-byte loads that bypass L1): a tombstone for each address that no longer holds a live local record.
+__global__ void k_delta_gone(TableView t, const ulonglong2 *base, uint64_t n, ulonglong2 *out, unsigned long long *count) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const ulonglong2 a = __ldcg(base + i);
+	const uint32_t idx = table_find(t, fnv_addr(a.x, a.y));
+	if (idx != 0xffffffffu) {
+		const Slot &s = t.slots[idx];
+		if (s.vlen != 0 && s.owner == 0 && s.addr_u == a.x && s.addr_l == a.y) return;
+	}
+	out[atomicAdd(count, 1ull)] = a;
+}
+int launch_delta_gone(TableView t, const ulonglong2 *base, uint64_t n, ulonglong2 *out, unsigned long long *count,
+    cudaStream_t st) {
+	if (n == 0) return 0;
+	k_delta_gone<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, base, n, out, count);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

@@ -250,9 +250,17 @@ struct ExportEntry {
 	uint32_t slot;
 };
 static_assert(sizeof(ExportEntry) == 40, "export entry layout");
-// arena_only: leave out the records of the host tier (compaction moves arena records only)
+// arena_only: leave out the records of the host tier (compaction moves arena records only).
+// seq_min: list only records whose slot's seq is at least this (a delta of a snapshot chain).
+// addr_out (nullable): also receives the address {u, l} of every live local record, whatever its seq,
+// counted in count[1] (then count has two words); at most max_out of either are written.
 int launch_export_list(TableView t, uint32_t bsize, ExportEntry *out, unsigned long long *count,
-    unsigned long long max_out, bool arena_only, cudaStream_t st);
+    unsigned long long max_out, bool arena_only, cudaStream_t st, unsigned long long seq_min = 0,
+    ulonglong2 *addr_out = nullptr);
+// Snapshot chains: the addresses among base[0 .. n) that no longer hold a live local record (absent,
+// no record, owned by another GPU, or the key holds another address) go to out, counted in *count.
+int launch_delta_gone(TableView t, const ulonglong2 *base, uint64_t n, ulonglong2 *out, unsigned long long *count,
+    cudaStream_t st);
 // cmb200_verify_store: turns n export entries into the lookup results of their keys (status ST_HIT,
 // location, vlen, slot, address), the input k_decode's verified store mode reads.
 int launch_scan_prep(TableView t, const ExportEntry *list, uint32_t n, int32_t *status, uint64_t *rec_off,

@@ -211,6 +211,36 @@ cmb200_snapshot *cmb200_snapshot_begin(cmb200_engine *const *engines, int g, con
 /* Waits for the writer, renames path.tmp to path (on failure removes it), frees s.  0 / -1. */
 int cmb200_snapshot_finish(cmb200_snapshot *s, uint64_t *records_out);
 
+/* ---- snapshot chains: checkpoints whose cost follows how much the store changed -------------------
+ * A chain is a base, the cmb200_save_set file with a nonzero 64-bit chain id in header bytes 40..47
+ * (zero in files written by cmb200_save_set), and deltas base_path.d1, .d2, ...  Delta k holds the
+ * addresses that were live at tick k-1 and are not at tick k (tombstones), then every live local record
+ * put between the two ticks, in the base's record format.  A record that only moved (compaction,
+ * demotion, promotion, a table rebuild) is not in a delta.  The store a chain describes is the base,
+ * then for each delta in order its tombstones removed and its records put.
+ *
+ * cmb200_chain_begin starts one tick over g engines, finished by cmb200_snapshot_finish, with the
+ * contract of cmb200_snapshot_begin (engines locked only while listed, file written to .tmp and renamed,
+ * the file holds the records as of begin).  delta = 0 writes a base at base_path with a fresh chain id.
+ * delta = 1 writes the next delta of the chain whose base lies at base_path; it fails (NULL, error set)
+ * unless every engine holds chain state for that base's id.  An engine holds chain state once a tick of
+ * it has been finished successfully, or after a complete cmb200_load_chain; the state is that tick's
+ * watermark (records put since have a higher sequence) and its live addresses, kept in page-locked host
+ * memory.  Only one chain tick of an engine may be open at a time.
+ *
+ * cmb200_load_chain loads the base plus the longest run of deltas 1, 2, ... that are present, complete,
+ * of the base's chain id and in sequence; the first that is not ends the run without failing the load,
+ * and nothing after it is applied (*deltas_out = deltas applied, *records_out = records put).  Files are
+ * read newest first and each address is decided by the newest file that names it, so each record is put
+ * once.  Records route by cmb200_owner, so a chain written by any number of engines loads into g.  When
+ * the engines were empty, every record the chain names is live afterwards and no base_path.d<j> lies
+ * beyond the run (a missing or damaged delta ended it early), each engine takes chain
+ * state from the load, so that the next delta tick continues the chain; otherwise none holds any and
+ * the next tick must write a base.  Load before the engines serve.  0 / -1. */
+cmb200_snapshot *cmb200_chain_begin(cmb200_engine *const *engines, int g, const char *base_path, int delta);
+int cmb200_load_chain(cmb200_engine *const *engines, int g, const char *base_path, uint64_t *records_out,
+    uint32_t *deltas_out);
+
 /* Moves n pages of the engine's page size within the engine's device memory:
  * dst[dst_idx ? dst_idx[i] : i] = src[src_idx ? src_idx[i] : i] (one warp per page, 16-byte loads and
  * stores; dst and src 16-byte aligned and not overlapping; the index arrays are host memory).  Returns

@@ -22,6 +22,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <unistd.h>
 
 /* ---- the reference's public API (include/filemap.h mirrors cachemap/filemap.h) ---- */
 #include "filemap.h"
@@ -63,6 +64,16 @@ to_lmdb(const char *snap, char *dir, uint64_t capacity, int pshift)
 	struct snap_header h;
 	if (!f || fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "CMB200S1", 8) != 0 || (int)h.pshift != pshift) {
 		fprintf(stderr, "snap2lmdb: %s is not a snapshot with pshift %d\n", snap, pshift);
+		return 1;
+	}
+	/* a base whose chain has deltas next to it is not the whole store (bytes 40..47: the chain id) */
+	uint64_t chain;
+	char d1[4096];
+	memcpy(&chain, &h.pad[1], 8);
+	snprintf(d1, sizeof(d1), "%s.d1", snap);
+	if (chain != 0 && access(d1, R_OK) == 0) {
+		fprintf(stderr, "snap2lmdb: %s has deltas next to it (%s ...): fold the chain first: open the cache "
+		    "directory with the library, which loads base and deltas, and call cachemap_checkpoint\n", snap, d1);
 		return 1;
 	}
 	const size_t bsize = (size_t)1 << pshift;
