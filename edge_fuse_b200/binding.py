@@ -20,7 +20,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_create", "cachemap_free", "cachemap_get", "cachemap_put", "cachemap_put_async",
     "cachemap_print_stats", "cachemap_put_batch", "cachemap_get_batch", "cachemap_put_batch_dev",
     "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
-    "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint",
+    "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -40,7 +40,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_promote_batch", "cmb200_host_tier_hot", "cmb200_read_checkpoints",
     "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
     "cmb200_verify_stats", "cmb200_verify_store", "cmb200_snapshot_begin", "cmb200_snapshot_finish",
-    "cmb200_chain_begin", "cmb200_load_chain",
+    "cmb200_chain_begin", "cmb200_load_chain", "cmb200_invalidate",
 ]
 
 
@@ -100,6 +100,7 @@ def lib() -> C.CDLL:
         "cachemap_engine": (vp, [vp]),
         "cachemap_engines": (i32, [vp, vp, i32]),
         "cachemap_checkpoint": (i32, [vp]),
+        "cachemap_invalidate": (u64, [vp, u64, u32, u64, u64]),
         "cachemap_read_range": (i32, [vp, u64, u32, u64, sz, vp]),
         "cachemap_write_range": (None, [vp, u64, u32, u64, sz, vp]),
         "filemap_create": (vp, [C.c_char_p, u64, i32, i32]),
@@ -133,6 +134,7 @@ def lib() -> C.CDLL:
         "cmb200_get_batch": (i32, [vp, sz, vp, vp, vp, vp]),
         "cmb200_get_batch_dev": (i32, [vp, sz, vp, vp, vp, vp]),
         "cmb200_unset_batch": (i32, [vp, sz, vp]),
+        "cmb200_invalidate": (i32, [vp, u64, u64, u64, vp]),
         "cmb200_entries": (u64, [vp]),
         "cmb200_sample": (i32, [vp, sz, vp, vp, vp, vp]),
         "cmb200_read_records": (i32, [vp, sz, vp, vp, sz, vp]),
@@ -490,6 +492,12 @@ class Engine:
         addr = _addr_array(u, l)
         _check(lib().cmb200_unset_batch(self.h, len(addr), _ptr(addr)), "cmb200_unset_batch")
 
+    def invalidate(self, u: int, l_first: int, l_last: int) -> int:
+        """Removes every live record stored at {u, l} with l_first <= l <= l_last -> records removed."""
+        removed = C.c_uint64()
+        _check(lib().cmb200_invalidate(self.h, u, l_first, l_last, C.byref(removed)), "cmb200_invalidate")
+        return removed.value
+
     def entries(self) -> int:
         return int(lib().cmb200_entries(self.h))
 
@@ -729,6 +737,13 @@ class Cachemap:
 
     def checkpoint(self) -> int:
         return int(lib().cachemap_checkpoint(self.h))
+
+    TO_END = (1 << 64) - 1
+
+    def invalidate(self, nhid: int, genid: int, off: int, size: int) -> int:
+        """Drops the cached pages of (nhid, genid) overlapping bytes [off, off + size) -> pages removed;
+        size = Cachemap.TO_END drops every page from off on."""
+        return int(lib().cachemap_invalidate(self.h, nhid, genid, off, size))
 
     def counters(self):
         rq, ht = C.c_uint64(), C.c_uint64()

@@ -66,6 +66,7 @@ extern int cmb200_owner(uint64_t key, int g);
 #pragma weak cmb200_copy_peer
 #pragma weak cmb200_dev_alloc
 #pragma weak cmb200_dev_free
+#pragma weak cmb200_invalidate
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -2082,6 +2083,36 @@ cachemap_write_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, u
 	 * edgefs.c:1186-1190 / 1219-1223 already hands the GPU one batch */
 	for (uint64_t i = 0; i < ((uint64_t)size >> pshift); i++)
 		cachemap_put(cm, off + (i << pshift), nhid_small, genid, (const uint8_t *)data + (i << pshift));
+}
+
+uint64_t
+cachemap_invalidate(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size)
+{
+	struct filemap *fm = cm->pages;
+	if (size == 0 || !cmb200_invalidate)
+		return 0;
+	/* a call before the first get applies to the loaded snapshot, not before it */
+	if (!filemap_engine_ready(fm))
+		return 0;
+	filemap_drain(fm);                      /* every page accepted before the call is in a store */
+	cmb200_addr first, last;
+	if (compose_addr(cm, off, nhid_small, genid, &first) != 0)
+		return 0;                       /* put ignores such a page: none is cached */
+	/* the last byte, off + size - 1, saturating: TO_END and an overflowing end both mean "to the end" */
+	const uint64_t end = size - 1 > UINT64_MAX - off ? UINT64_MAX : off + (size - 1);
+	if (compose_addr(cm, end, nhid_small, genid, &last) != 0)
+		last.l = ((1ULL << PNUM_SHIFT) - 1) | ((uint64_t)genid << PNUM_SHIFT);
+	uint64_t removed = 0;
+	for (int i = 0; i < fm->g; i++) {       /* the object's pages are spread over the engines by key */
+		uint64_t r = 0;
+		if (cmb200_invalidate(fm->dev[i]->eng, nhid_small, first.l, last.l, &r) == 0)
+			removed += r;
+		else
+			fprintf(stderr, "cachemap_b200: cachemap_invalidate: %s\n", cmb200_last_error());
+	}
+	/* a removal is a change of the store: the next checkpoint must write it */
+	__atomic_fetch_add(&fm->puts_seen, removed, __ATOMIC_RELAXED);
+	return removed;
 }
 
 int

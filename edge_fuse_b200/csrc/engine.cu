@@ -218,6 +218,7 @@ struct cmb200_engine {
 	DevMem<uint32_t> d_order;            // the encoder's longest-first chunk lists (encode_order_words(max_batch))
 	DevMem<uint32_t> d_import_slot;      // slot scratch of cmb200_import_records_dev, grown, never shrunk
 	DevMem<uint32_t> d_move_idx;         // index scratch of cmb200_move_pages (destination, then source), grown, never shrunk
+	DevMem<unsigned long long> d_removed; // records removed by cmb200_invalidate, allocated by its first call
 	// page-locked staging for the small per-chunk arrays, so that no copy ever blocks the host
 	// thread that is feeding the pipeline (a pageable cudaMemcpyAsync waits for the stream)
 	static constexpr size_t META_CAP = 1u << 18;   // chunks per outer slice of a call
@@ -1789,6 +1790,67 @@ extern "C" int cmb200_copy_peer(cmb200_engine *dst_e, void *dst_dev, cmb200_engi
 	return 0;
 }
 
+// ---- table rebuild ----------------------------------------------------------------------------
+// The table is rebuilt when deleted keys (`tombs` tombstones; slots of dropped puts go with them) have
+// eaten a good part of its empty slots: miss probes end at an EMPTY slot, and linear probing never
+// frees one by itself.  Slots move, records do not, so a snapshot's writer need not be waited for.
+// (e->mu held, get_gate closed: small gets read slots)
+static int rebuild_table_locked(cmb200_engine *e, unsigned long long tombs) {
+	if (tombs <= e->table.cap / 8) return 0;
+	// parse checkpoints move with their slots (k_rehash); without room for a second side table
+	// they are dropped instead, and those records are walked by one warp until rewritten
+	const bool ckpt = e->table.ckpt != nullptr;
+	TableMem mem;
+	int got = table_alloc(mem, e->table.cap, e->table.fp != nullptr, e->table.fp_tag != nullptr, ckpt, e->st);
+	if (got > 0 && ckpt) got = table_alloc(mem, e->table.cap, e->table.fp != nullptr, e->table.fp_tag != nullptr, false, e->st);
+	if (got < 0) return -1;
+	if (got > 0) return 0;                           // no room for a second table: keep the old one
+	TableView fresh = e->table;
+	mem.view(fresh);
+	if (launch_rehash(e->table, fresh, e->st)) return -1;
+	if (ckpt && !fresh.ckpt) CMB_CHECK(cudaMemsetAsync(e->table.ckpt, 0, (e->table.cap + 2) * CKPT_WORDS * 4, e->st));
+	CMB_CHECK(cudaMemsetAsync(e->d_counters + 1, 0, sizeof(unsigned long long), e->st));   // tombstones
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	if (!mem.ckpt) mem.ckpt = std::move(e->table_mem.ckpt);
+	e->table_mem = std::move(mem);
+	e->table_mem.view(e->table);
+	e->stats.kernel_launches++;
+	return 0;
+}
+
+// ---- invalidation of an object's pages ----------------------------------------------------------
+// An interval of at most this many addresses is looked up key by key (k_invalidate_keys), a longer
+// one by a scan of the whole table (k_invalidate_scan).  On an H100 the two cost the same at 1/58 of
+// the slots of a 2^25-slot table and 1/38 of a 2^27-slot one (DESIGN.md §2, *Invalidation*): 1/64
+// keeps the keyed path where it was measured cheaper.
+static uint64_t invalidate_keyed_max(uint64_t cap) { return (cap + 2) / 64; }
+
+extern "C" int cmb200_invalidate(cmb200_engine *e, uint64_t u, uint64_t l_first, uint64_t l_last, uint64_t *removed_out) {
+	if (l_first > l_last) { set_error_msg("cmb200_invalidate: l_first > l_last"); return -1; }
+	std::lock_guard<std::mutex> g(e->mu);
+	if (e->multi_gpu) {
+		set_error_msg("cmb200_invalidate: not available after a multi-GPU call (the index holds other ranks' records)");
+		return -1;
+	}
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (!e->d_removed && e->d_removed.alloc(sizeof(unsigned long long))) return -1;
+	CMB_CHECK(cudaMemsetAsync(e->d_removed, 0, sizeof(unsigned long long), e->st));
+	// l_last - l_first + 1 overflows for the full interval: compare the difference instead
+	const bool scan = l_last - l_first >= invalidate_keyed_max(e->table.cap);
+	if (launch_invalidate(e->table, e->arena, u, l_first, l_last, scan, e->d_removed, e->st)) return -1;
+	e->stats.kernel_launches++;
+	unsigned long long removed = 0;
+	CMB_CHECK(cudaMemcpyAsync(&removed, e->d_removed, sizeof(removed), cudaMemcpyDeviceToHost, e->st));
+	unsigned long long c[8];
+	if (read_counters(e, c)) return -1;
+	if (removed_out) *removed_out = removed;
+	if (c[1] > e->table.cap / 8) {
+		cmb200_engine::GateClosed gg(e->get_gate);
+		return rebuild_table_locked(e, c[1]);
+	}
+	return 0;
+}
+
 // ---- arena compaction -------------------------------------------------------------------------
 // The arena is a bump allocator: a deleted record, or one that outgrew its place, leaves its bytes
 // behind as garbage.  Compaction slides the live records down to the start of the arena (sorted by
@@ -1835,30 +1897,8 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 	CMB_CHECK(cudaMemsetAsync(e->arena.seg, 0, ARENA_SEG_SLOTS * 2 * sizeof(unsigned long long), e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
 	if (reclaimed_out) *reclaimed_out = head_before > at ? head_before - at : 0;
-	// The table is rebuilt on the same occasion when deleted keys have eaten a good part of its empty
-	// slots (tombstones; slots of dropped puts go with them): miss probes end at an EMPTY slot, and
-	// linear probing never frees one by itself.
-	if (c[1] > e->table.cap / 8) {
-		// parse checkpoints move with their slots (k_rehash); without room for a second side table
-		// they are dropped instead, and those records are walked by one warp until rewritten
-		const bool ckpt = e->table.ckpt != nullptr;
-		TableMem mem;
-		int got = table_alloc(mem, e->table.cap, e->table.fp != nullptr, e->table.fp_tag != nullptr, ckpt, e->st);
-		if (got > 0 && ckpt) got = table_alloc(mem, e->table.cap, e->table.fp != nullptr, e->table.fp_tag != nullptr, false, e->st);
-		if (got < 0) return -1;
-		if (got > 0) return 0;                           // no room for a second table: keep the old one
-		TableView fresh = e->table;
-		mem.view(fresh);
-		if (launch_rehash(e->table, fresh, e->st)) return -1;
-		if (ckpt && !fresh.ckpt) CMB_CHECK(cudaMemsetAsync(e->table.ckpt, 0, (e->table.cap + 2) * CKPT_WORDS * 4, e->st));
-		CMB_CHECK(cudaMemsetAsync(e->d_counters + 1, 0, sizeof(unsigned long long), e->st));   // tombstones
-		CMB_CHECK(cudaStreamSynchronize(e->st));
-		if (!mem.ckpt) mem.ckpt = std::move(e->table_mem.ckpt);
-		e->table_mem = std::move(mem);
-		e->table_mem.view(e->table);
-		e->stats.kernel_launches++;
-	}
-	return 0;
+	// the table is rebuilt on the same occasion
+	return rebuild_table_locked(e, c[1]);
 }
 
 extern "C" int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out) {

@@ -3,7 +3,7 @@
 //   k_encode      fingerprint + LZ4 block encode + arena commit, one warp per chunk  (HBM: §4)
 //   k_decode      table record -> LZ4 decode -> page, one warp per request
 //   k_fingerprint EF128 alone
-//   k_compose / k_upsert / k_lookup / k_unset / k_sample   the HBM key table
+//   k_compose / k_upsert / k_lookup / k_unset / k_sample / k_invalidate_*   the HBM key table
 //   k_streamgen   synthetic benchmark input
 #include "kernels.h"
 #include "common.cuh"
@@ -179,16 +179,13 @@ __device__ __forceinline__ void hot_log(const HotLog &h, unsigned long long u, u
 	h.ring[k % HOT_LOG_N] = make_ulonglong2(u, l);
 }
 
-// filemap_unset (filemap.c:188-215): delete by key, whatever address the record holds.
-__global__ void k_unset(TableView t, ArenaView a, const unsigned long long *addr, uint32_t n) {
-	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	uint32_t idx = table_find(t, fnv_addr(addr[2 * i], addr[2 * i + 1]));
-	if (idx == 0xffffffffu) return;
+// Retires the record of slot idx: the slot becomes a tombstone (the side slots of keys 0 and ~0 stay
+// empty slots) and the record's bytes garbage.  Returns false when the slot held no record, so that
+// of two threads naming the same slot exactly one retires it.
+__device__ __forceinline__ bool slot_retire(const TableView &t, const ArenaView &a, uint32_t idx) {
 	Slot &s = t.slots[idx];
-	// Two requests of one batch may name the same key: let exactly one retire the record.
 	uint32_t old = atomicExch(&s.vlen, 0u);
-	if (old == 0) return;
+	if (old == 0) return false;
 	atomicAdd(t.entries, (unsigned long long)-1ll);
 	slot_release(a, s);
 	s.alloc = 0;
@@ -198,6 +195,62 @@ __global__ void k_unset(TableView t, ArenaView a, const unsigned long long *addr
 		s.key = KEY_TOMB;
 		atomicAdd(t.tombs, 1ull);
 	}
+	return true;
+}
+
+// filemap_unset (filemap.c:188-215): delete by key, whatever address the record holds.
+__global__ void k_unset(TableView t, ArenaView a, const unsigned long long *addr, uint32_t n) {
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	uint32_t idx = table_find(t, fnv_addr(addr[2 * i], addr[2 * i + 1]));
+	if (idx == 0xffffffffu) return;
+	// Two requests of one batch may name the same key: let exactly one retire the record.
+	slot_retire(t, a, idx);
+}
+
+// cmb200_invalidate: retire every live local record whose stored address is {u, l}, l in
+// [l_first, l_last].  Two paths that leave the same store, chosen by the engine from the interval's
+// length (DESIGN.md §2, *Invalidation*).  Removals are counted once per warp.
+__device__ __forceinline__ void count_warp(bool hit, unsigned long long *removed) {
+	const unsigned m = __ballot_sync(0xffffffffu, hit);
+	if (m && (threadIdx.x & 31) == 0) atomicAdd(removed, (unsigned long long)__popc(m));
+}
+
+// One thread per slot (cap + 2 of them).  Only the first 16 bytes {key, addr_u} are read for every
+// slot, by one streaming load, so that a scan of a large table does not push the encoder's and the
+// small gets' lines out of L2; the rest of the slot is read only where addr_u matches.  A dead slot
+// keeps its old address, hence the liveness test of k_export_list.
+__global__ void __launch_bounds__(256) k_invalidate_scan(TableView t, ArenaView a, unsigned long long u,
+    unsigned long long l_first, unsigned long long l_last, unsigned long long *removed) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	bool hit = false;
+	if (i < t.cap + 2) {
+		const ulonglong2 ku = __ldcs(reinterpret_cast<const ulonglong2 *>(t.slots + i));
+		if (ku.y == u && (i >= t.cap || (ku.x != KEY_EMPTY && ku.x != KEY_TOMB))) {
+			const Slot &s = t.slots[i];
+			const unsigned long long l = s.addr_l;
+			if (l >= l_first && l <= l_last && s.vlen != 0 && s.owner == 0) hit = slot_retire(t, a, (uint32_t)i);
+		}
+	}
+	count_warp(hit, removed);
+}
+
+// One thread per l of the interval: the thread builds its address, finds the key's slot and retires
+// it only when the slot holds exactly that address.  A key names one record, not one address: another
+// object's page may hold it, and that page stays.
+__global__ void __launch_bounds__(256) k_invalidate_keys(TableView t, ArenaView a, unsigned long long u,
+    unsigned long long l_first, uint64_t n, unsigned long long *removed) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	bool hit = false;
+	if (i < n) {
+		const unsigned long long l = l_first + i;
+		const uint32_t idx = table_find(t, fnv_addr(u, l));
+		if (idx != 0xffffffffu) {
+			const Slot &s = t.slots[idx];
+			if (s.addr_u == u && s.addr_l == l && s.owner == 0) hit = slot_retire(t, a, idx);
+		}
+	}
+	count_warp(hit, removed);
 }
 
 // filemap_get_rand (filemap.c:264-314) picks the first key at or after a random 64-bit draw; the
@@ -1464,6 +1517,18 @@ int launch_lookup(TableView t, const unsigned long long *addr, const uint8_t *va
 int launch_unset(TableView t, ArenaView a, const unsigned long long *addr, uint32_t n, cudaStream_t st) {
 	if (n == 0) return 0;
 	k_unset<<<GRID1D(n), 0, st>>>(t, a, addr, n);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_invalidate(TableView t, ArenaView a, unsigned long long u, unsigned long long l_first,
+    unsigned long long l_last, bool scan, unsigned long long *removed, cudaStream_t st) {
+	if (scan) {
+		const uint64_t n = t.cap + 2;
+		k_invalidate_scan<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, a, u, l_first, l_last, removed);
+	} else {
+		const uint64_t n = l_last - l_first + 1;
+		k_invalidate_keys<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, a, u, l_first, n, removed);
+	}
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

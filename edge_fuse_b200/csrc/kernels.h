@@ -225,6 +225,11 @@ int launch_lookup(TableView t, const unsigned long long *addr, const uint8_t *va
 // gets the key's slot of every ST_HIT.
 
 int launch_unset(TableView t, ArenaView a, const unsigned long long *addr, uint32_t n, cudaStream_t st);
+// cmb200_invalidate: retires every live local record whose stored address is {u, l} with
+// l_first <= l <= l_last, adding the count to *removed.  scan: k_invalidate_scan, one thread per slot;
+// otherwise k_invalidate_keys, one thread per l (the caller keeps l_last - l_first + 1 small).
+int launch_invalidate(TableView t, ArenaView a, unsigned long long u, unsigned long long l_first,
+    unsigned long long l_last, bool scan, unsigned long long *removed, cudaStream_t st);
 
 // Policy-equivalent of filemap_get_rand (filemap.c:264-314): first live slot at or after r.
 int launch_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,

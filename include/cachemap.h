@@ -89,6 +89,20 @@ void cachemap_write_range(struct cachemap *cm, uint64_t nhid_small, uint32_t gen
  */
 int cachemap_checkpoint(struct cachemap *cm);
 
+/*
+ * Invalidation.  The key of a page is its object's nhid_small and generation plus the page number,
+ * so a file that is replaced (rename over it), deleted and created again under the same name, or
+ * truncated, would be served its old pages; the file system calls this at those points
+ * (INTEGRATION.md, "Invalidation").
+ * Drops every cached page of object (nhid_small, genid) that overlaps bytes [off, off + size);
+ * size = CACHEMAP_TO_END (UINT64_MAX) drops every page from off on.  Partial pages at either end are
+ * dropped.  Pages accepted by cachemap_put before the call are dropped; pages put after it returns
+ * are kept.  Returns the pages removed.  A removal counts as a change for the next checkpoint, so a
+ * restart does not bring the pages back.
+ */
+#define CACHEMAP_TO_END UINT64_MAX
+uint64_t cachemap_invalidate(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size);
+
 /* requests / hits counters (cachemap.c:176,181) and the engine under the map. */
 void cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hits);
 struct cmb200_engine *cachemap_engine(struct cachemap *cm);

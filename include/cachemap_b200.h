@@ -112,6 +112,18 @@ int cmb200_get_batch_dev(cmb200_engine *e, size_t n, const cmb200_addr *addr, co
 /* filemap_unset (filemap.c:188-215), filemap_entries (filemap.c:316-330),
  * filemap_get_rand (filemap.c:264-314; policy-equivalent: first live record at or after r). */
 int cmb200_unset_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr);
+/* Removes every live local record whose stored address has u == u and l_first <= l <= l_last
+ * (one generation's pages p..q of one object: l = genid << 44 | page).  Unlike cmb200_unset_batch it
+ * goes by stored address, never by key alone: a record of another address that shares a key stays.
+ * Ordered after everything enqueued on the engine before the call, async puts included; runs under the
+ * engine lock on its stream, as cmb200_unset_batch does.  A short interval is looked up page by page,
+ * a long one by a scan of the table; both leave the same store.  Records of the host tier leave it as
+ * if unset.  The table only changes, so a snapshot begun before the call still holds the records, and
+ * the next delta of a chain names them as tombstones.  When the removals leave more than cap/8
+ * tombstones the table is rebuilt, as cmb200_compact does.  *removed_out = records removed.  -1 if
+ * l_first > l_last, or on an engine that has made a multi-GPU call (its index holds other ranks'
+ * records). */
+int cmb200_invalidate(cmb200_engine *e, uint64_t u, uint64_t l_first, uint64_t l_last, uint64_t *removed_out);
 uint64_t cmb200_entries(cmb200_engine *e);
 int cmb200_sample(cmb200_engine *e, size_t n, const uint64_t *r, cmb200_addr *addr_out,
     uint64_t *ts_out, int32_t *ok_out);
