@@ -13,6 +13,7 @@ _LIB = None
 MISS, HIT, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, CORRUPT = 0, 1, 2, 3, 4, 5, 6
 FINGERPRINT = 1
 VERIFY = 2
+TOUCH = 4       # a hit raises its record's timestamp: eviction by last access (CMB200_EVICT=access)
 
 # every symbol the headers in include/ declare (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [

@@ -271,6 +271,24 @@ fm_dev_free(struct fm_dev *d)
 	free(d);
 }
 
+/* CMB200_EVICT: what a record's timestamp means to eviction and demotion, which take the oldest of what
+ * they sample.  "put" (or unset): the put time, the reference's policy.  "access": the last hit as well
+ * (CMB200_TOUCH), so pages that are read stay.  Reads alone are not changes for a checkpoint (puts_seen):
+ * a full snapshot saves the touched timestamps, a chain delta carries only the records put since the last
+ * tick, each with the timestamp it had then.  Any other value warns (once, with `warn`) and keeps "put". */
+static uint32_t
+evict_flags(int warn)
+{
+	const char *v = getenv("CMB200_EVICT");
+	if (!v || !*v || strcmp(v, "put") == 0)
+		return 0;
+	if (strcmp(v, "access") == 0)
+		return CMB200_TOUCH;
+	if (warn)
+		fprintf(stderr, "cachemap_b200: CMB200_EVICT=%s is neither put nor access; evicting by put time\n", v);
+	return 0;
+}
+
 /* Engine `index` of the map on CUDA device `device`, with its buffers; NULL if it cannot start.
  * The knobs apply per engine; the table and the default arena are sized for its share of the
  * capacity, ceil(n / G). */
@@ -305,6 +323,7 @@ fm_dev_start(struct filemap *m, int index, int device, int g)
 	cfg.flags = env_long("CMB200_FINGERPRINT", 0) ? CMB200_FINGERPRINT : 0;
 	/* every get compared with its page's EF128 on the GPU; a page that differs is a miss */
 	if (env_long("CMB200_VERIFY", 0)) cfg.flags |= CMB200_VERIFY;
+	cfg.flags |= evict_flags(index == 0);
 	d->eng = cmb200_engine_create(&cfg);
 	const long tier_mb = env_long("CMB200_HOST_TIER_MB", 0);
 	if (d->eng && tier_mb > 0) {

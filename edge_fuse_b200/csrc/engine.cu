@@ -263,7 +263,7 @@ struct cmb200_engine {
 	std::atomic<bool> multi_gpu{false};  // a multi-GPU call was made: no host tier from then on
 	// CMB200_VERIFY: device counters, VS_WORDS of the gets, then VS_WORDS of the running store scan
 	DevMem<unsigned long long> d_vstat;
-	DevMem<uint32_t> d_vidx;             // slot of each request of a verified get batch (max_batch)
+	DevMem<uint32_t> d_vidx;             // slot of each request of a verified or touching get batch (max_batch)
 	uint64_t scanned = 0, scan_corrupt = 0;
 	// snapshots (cmb200_snapshot_begin): SNAP_FREE, SNAP_CLAIMED by a snapshot that has not listed this
 	// engine's records yet, or SNAP_PENDING: listed, section not written yet.  snap_state changes under
@@ -295,6 +295,15 @@ struct cmb200_engine {
 		unsigned long long w_next = 0;
 	} chain;
 };
+
+// CMB200_TOUCH: the stamp a get raises its hits' ts to, taken at launch from the clock the drop-in's puts
+// stamp with (cachemap_api.c:now_ns, the reference's cachemap.c:10-15).  Never 0 (GetJob::touch_ts).
+static unsigned long long touch_stamp() {
+	struct timespec tp;
+	clock_gettime(CLOCK_REALTIME_COARSE, &tp);
+	const unsigned long long ns = (unsigned long long)tp.tv_sec * 1000000000ull + (unsigned long long)tp.tv_nsec;
+	return ns ? ns : 1ull;
+}
 
 static uint64_t next_pow2(uint64_t v) {
 	uint64_t p = 1;
@@ -362,12 +371,13 @@ static int engine_init(cmb200_engine *e, const cmb200_config *cfg) {
 	if (table_alloc(e->table_mem, slots, e->flags & CMB200_FINGERPRINT, e->flags & CMB200_VERIFY, ckpt, e->st)) return -1;
 	e->table_mem.view(e->table);
 	if (e->flags & CMB200_VERIFY) {
-		if (e->d_vstat.alloc(2 * VS_WORDS * sizeof(unsigned long long)) || e->d_vidx.alloc(B * 4)) return -1;
+		if (e->d_vstat.alloc(2 * VS_WORDS * sizeof(unsigned long long))) return -1;
 		CMB_CHECK(cudaMemsetAsync(e->d_vstat, 0, 2 * VS_WORDS * sizeof(unsigned long long), e->st));
 	}
+	if ((e->flags & (CMB200_VERIFY | CMB200_TOUCH)) && e->d_vidx.alloc(B * 4)) return -1;
 	if (get_small_supports(e->bsize)) {
 		// the descriptor scratch of the fused single-page get
-		const int resident = get_small_residency(e->bsize, e->table.fp_tag != nullptr);
+		const int resident = get_small_residency(e->bsize, e->table.fp_tag != nullptr, e->flags & CMB200_TOUCH);
 		if (resident <= 0) { set_error_msg("k_get_small does not fit this device"); return -1; }
 		e->pool_n = (uint32_t)resident;
 		e->region_entries = get_small_region_entries(e->bsize);
@@ -752,8 +762,9 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		job.host = e->tier.dev; job.host_hits = e->tier.d_ctr + 1;
 		job.hot = e->tier.hot(); job.addr = e->d_addr + 2 * at;
 		const DecodeVerify ver{e->d_vidx, e->table.fp, e->table.fp_tag, e->d_vstat};
+		const DecodeTouch touch{e->d_vidx, e->table.slots, (e->flags & CMB200_TOUCH) ? touch_stamp() : 0ull};
 		CMB_CHECK(cudaEventRecord(e->t0[nb % e->RING], e->st));
-		if (launch_decode(job, e->st, e->table.fp_tag ? &ver : nullptr)) return -1;
+		if (launch_decode(job, e->st, e->table.fp_tag ? &ver : nullptr, touch.ts ? &touch : nullptr)) return -1;
 		CMB_CHECK(cudaEventRecord(e->t1[nb % e->RING], e->st));
 		if (!out_on_dev) {
 			CMB_CHECK(cudaEventRecord(e->landed[buf], e->st));
@@ -884,6 +895,7 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	job.scratch = e->d_scratch; job.region_entries = e->region_entries; job.pool_bits = e->d_pool_bits; job.pool_n = e->pool_n;
 	job.hot = e->tier.hot();
 	job.vstat = e->d_vstat;
+	job.touch_ts = (e->flags & CMB200_TOUCH) ? touch_stamp() : 0ull;
 	if (launch_get_small(job, e->device, ln->st)) { ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1; }
 	t->lane = li; t->n = (uint32_t)n; t->status = ln->h_status;
 	return 0;

@@ -179,6 +179,17 @@ __device__ __forceinline__ void hot_log(const HotLog &h, unsigned long long u, u
 	h.ring[k % HOT_LOG_N] = make_ulonglong2(u, l);
 }
 
+// CMB200_TOUCH: a hit on {u, l} raises the ts of its slot idx to `stamp` (one thread).  The slot is
+// re-checked for the key first, so a slot that a table rebuild or a tombstone reuse gave to another key
+// keeps its ts; the side slots of keys 0 and ~0 belong to their key alone.  atomicMax: a stamp never
+// lowers ts, whichever of two gets (or a put and a get) lands first.
+__device__ __forceinline__ void slot_touch(Slot *slots, uint32_t idx, unsigned long long u, unsigned long long l,
+    unsigned long long stamp) {
+	Slot &s = slots[idx];
+	const unsigned long long key = fnv_addr(u, l);
+	if (key == KEY_EMPTY || key == KEY_TOMB || ld_key(&s) == key) atomicMax(&s.ts, stamp);
+}
+
 // Retires the record of slot idx: the slot becomes a tombstone (the side slots of keys 0 and ~0 stay
 // empty slots) and the record's bytes garbage.  Returns false when the slot held no record, so that
 // of two threads naming the same slot exactly one retires it.
@@ -742,8 +753,17 @@ extern "C" int cmb200_enc_phases(void *buf, uint32_t *nphases) {   // n x 2 x EN
 // store (cmb200_verify_store), which is not a get and books no tier hit.
 // The verify state is a parameter of k_decode_verify alone, so that k_decode's parameter block (and with
 // it its register allocation) stays what it is without the flag.
-template <bool VERIFY>
-__device__ __forceinline__ void decode_request(const DecodeJob &job, const DecodeVerify &v) {
+// TOUCH (CMB200_TOUCH): lane 0 raises the slot's ts once the request's answer is ST_HIT (after the
+// fingerprint comparison under VERIFY); the state is, likewise, a parameter of the touching kernels alone.
+template <bool TOUCH>
+__device__ __forceinline__ void decode_touch(const DecodeJob &job, const DecodeTouch &t, uint32_t i, int lane) {
+	if constexpr (TOUCH) {
+		if (lane == 0) slot_touch(t.slots, t.idx[i], job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1], t.ts);
+	}
+}
+
+template <bool VERIFY, bool TOUCH>
+__device__ __forceinline__ void decode_request(const DecodeJob &job, const DecodeVerify &v, const DecodeTouch &t) {
 	const int lane = threadIdx.x & 31;
 	const uint32_t i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
 	if (i >= job.n) return;
@@ -761,10 +781,12 @@ __device__ __forceinline__ void decode_request(const DecodeJob &job, const Decod
 		if constexpr (!VERIFY) {
 			if (clen == 0) {                            // raw page (filemap.c:249-251)
 				warp_copy_ro(out, rec + 24, job.nbytes, lane);
+				decode_touch<TOUCH>(job, t, i, lane);
 				return;
 			}
 			int used = lz4_decode_warp(rec + 24, clen, out, job.nbytes, lane);
 			if (used != (int)clen && lane == 0) job.status[i] = ST_BAD_DECODE;   // filemap.c:244-248
+			if (used == (int)clen) decode_touch<TOUCH>(job, t, i, lane);
 		} else {
 			if (clen == 0) {
 				warp_copy_ro(out, rec + 24, job.nbytes, lane);
@@ -775,6 +797,7 @@ __device__ __forceinline__ void decode_request(const DecodeJob &job, const Decod
 			const uint32_t idx = v.idx[i];
 			if (v.fp_tag[idx] != ckpt_tag(off, clen)) {
 				if (lane == 0) atomicAdd(&v.vstat[VS_UNVERIFIED], 1ull);
+				decode_touch<TOUCH>(job, t, i, lane);
 				return;
 			}
 			__syncwarp();                           // every lane's stores of the page are visible to the warp
@@ -785,6 +808,7 @@ __device__ __forceinline__ void decode_request(const DecodeJob &job, const Decod
 				atomicAdd(&v.vstat[match ? VS_VERIFIED : VS_CORRUPT], 1ull);
 				if (!match) job.status[i] = ST_CORRUPT;
 			}
+			if (match) decode_touch<TOUCH>(job, t, i, lane);
 		}
 	} else {
 		int used = lz4_decode_warp(job.blocks + (size_t)i * job.block_stride, (uint32_t)job.lens[i], out,
@@ -793,16 +817,33 @@ __device__ __forceinline__ void decode_request(const DecodeJob &job, const Decod
 	}
 }
 
-__global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) { decode_request<false>(job, DecodeVerify{}); }
+__global__ void __launch_bounds__(256, 8) k_decode(DecodeJob job) {
+	decode_request<false, false>(job, DecodeVerify{}, DecodeTouch{});
+}
 // 4 CTAs per SM rather than 8: the fingerprint's 16 loads in flight per lane need the registers that 8
 // would leave to spills.
-__global__ void __launch_bounds__(256, 4) k_decode_verify(DecodeJob job, DecodeVerify v) { decode_request<true>(job, v); }
+__global__ void __launch_bounds__(256, 4) k_decode_verify(DecodeJob job, DecodeVerify v) {
+	decode_request<true, false>(job, v, DecodeTouch{});
+}
+__global__ void __launch_bounds__(256, 8) k_decode_touch(DecodeJob job, DecodeTouch t) {
+	decode_request<false, true>(job, DecodeVerify{}, t);
+}
+__global__ void __launch_bounds__(256, 4) k_decode_verify_touch(DecodeJob job, DecodeVerify v, DecodeTouch t) {
+	decode_request<true, true>(job, v, t);
+}
 
-int launch_decode(const DecodeJob &job, cudaStream_t st, const DecodeVerify *verify) {
+int launch_decode(const DecodeJob &job, cudaStream_t st, const DecodeVerify *verify, const DecodeTouch *touch) {
 	if (job.n == 0) return 0;
 	const int warps = 8;
-	if (job.rec_off && verify) k_decode_verify<<<(job.n + warps - 1) / warps, warps * 32, 0, st>>>(job, *verify);
-	else k_decode<<<(job.n + warps - 1) / warps, warps * 32, 0, st>>>(job);
+	const uint32_t grid = (job.n + warps - 1) / warps;
+	if (job.rec_off && touch) {
+		if (verify) k_decode_verify_touch<<<grid, warps * 32, 0, st>>>(job, *verify, *touch);
+		else k_decode_touch<<<grid, warps * 32, 0, st>>>(job, *touch);
+	} else if (job.rec_off && verify) {
+		k_decode_verify<<<grid, warps * 32, 0, st>>>(job, *verify);
+	} else {
+		k_decode<<<grid, warps * 32, 0, st>>>(job);
+	}
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
@@ -980,9 +1021,11 @@ __device__ bool gs_sections_fit(const DecodeCta *dc, uint32_t clen, uint32_t n) 
 // k_get_small_pair), after a barrier that follows the page's last store.  The status may live in
 // page-locked host memory that the caller polls: the page first, then the status (every thread's
 // stores happen before the barrier, this thread's system-wide fence after it is cumulative).
-template <bool VERIFY>
+// TOUCH (CMB200_TOUCH): a hit on a local record (touch_idx = its slot; ~0 for a peer's record) raises the
+// slot's ts to job.touch_ts before the status is stored, so a caller that has seen the status sees the ts.
+template <bool VERIFY, bool TOUCH>
 __device__ __forceinline__ void gs_answer(const GetJob &job, uint32_t i, int32_t result, uint32_t region, bool from_host,
-    uint32_t fp_ok) {
+    uint32_t fp_ok, uint32_t touch_idx) {
 	if (region != 0xffffffffu) gs_region_give(job, region);
 	if (result == ST_HIT && from_host) {
 		atomicAdd(job.host_hits, 1ull);
@@ -991,6 +1034,8 @@ __device__ __forceinline__ void gs_answer(const GetJob &job, uint32_t i, int32_t
 	}
 	if (VERIFY && (result == ST_HIT || result == ST_CORRUPT))
 		atomicAdd(&job.vstat[result == ST_CORRUPT ? VS_CORRUPT : fp_ok ? VS_VERIFIED : VS_UNVERIFIED], 1ull);
+	if (TOUCH && result == ST_HIT && touch_idx != 0xffffffffu)
+		slot_touch(job.table.slots, touch_idx, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1], job.touch_ts);
 	__threadfence_system();
 	*reinterpret_cast<volatile int32_t *>(&job.status[i]) = result;
 }
@@ -998,7 +1043,7 @@ __device__ __forceinline__ void gs_answer(const GetJob &job, uint32_t i, int32_t
 // VERIFY (CMB200_VERIFY): the page, decoded or raw, is compared with the record's stored EF128 while it
 // is still in shared memory (gs_page_matches), so a page that does not match is never written out and
 // is answered ST_CORRUPT.
-template <bool VERIFY>
+template <bool VERIFY, bool TOUCH>
 __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
 	GetShared *sh = reinterpret_cast<GetShared *>(smem);
@@ -1119,7 +1164,10 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 		break;
 	}
 	__syncthreads();
-	if (tid == 0) gs_answer<VERIFY>(job, i, result, sh->region, from_host, sh->fp_ok);
+	// the last lookup decided the answer: owner 0 is a local record, which a hit may touch
+	if (tid == 0)
+		gs_answer<VERIFY, TOUCH>(job, i, result, sh->region, from_host, sh->fp_ok,
+		    TOUCH && sh->owner == 0u ? sh->idx : 0xffffffffu);
 }
 
 // ---- pages above 64 KiB: one request per cluster of two CTAs ----------------------------------------
@@ -1144,6 +1192,7 @@ struct PairVerdict {                              // the page CTA's control bloc
 	uint32_t fp_ok;                           // VERIFY: fp holds the record's stored EF128 (GetShared::fp_ok)
 	uint32_t match;                           // the page CTA's gs_page_matches answer
 	uint32_t fp[4];                           // {hi, lo} as 32-bit halves (DSMEM stores are 32-bit)
+	uint32_t touch_idx;                       // TOUCH: slot of a local record, ~0 otherwise
 };
 static_assert(sizeof(PairVerdict) <= 128, "control block");
 
@@ -1166,7 +1215,7 @@ __device__ __forceinline__ void dsmem_st32(uint32_t a, uint32_t v) { asm volatil
 
 // VERIFY: the CTA that holds the page compares it with the record's stored EF128 before writing it out
 // (gs_page_matches): the page CTA for a decoded page, the record CTA for a raw one.
-template <bool VERIFY>
+template <bool VERIFY, bool TOUCH>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get_small_pair(GetJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
 	DecodeCta *dc = reinterpret_cast<DecodeCta *>(smem + 128);
@@ -1204,7 +1253,7 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 		// the page first, then the status (a raw page was written by the record CTA before it arrived
 		// at B, and this thread acquired B)
 		__syncthreads();
-		if (tid == 0) gs_answer<VERIFY>(job, i, v->result, v->region, v->from_host, v->fp_ok);
+		if (tid == 0) gs_answer<VERIFY, TOUCH>(job, i, v->result, v->region, v->from_host, v->fp_ok, TOUCH ? v->touch_idx : 0u);
 		return;
 	}
 	GetShared *sh = reinterpret_cast<GetShared *>(smem);
@@ -1319,12 +1368,13 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 			for (uint32_t k = 0; k < 4; k++)
 				dsmem_st32(v + offsetof(PairVerdict, fp) + 4u * k, (uint32_t)(sh->fp[k >> 1] >> (32u * (k & 1u))));
 		}
+		if (TOUCH) dsmem_st32(v + offsetof(PairVerdict, touch_idx), sh->owner == 0u ? sh->idx : 0xffffffffu);
 	}
 	cluster_arrive_release();                                   // B
 	cluster_wait();
 }
 
-template <bool VERIFY>
+template <bool VERIFY, bool TOUCH>
 static int launch_get_small_kernel(const GetJob &job, int device, cudaStream_t st) {
 	const size_t smem = get_small_smem(job.nbytes, VERIFY);
 	// the attribute belongs to the device: engines on several GPUs (CMB200_DEVICES) each set their own
@@ -1333,49 +1383,52 @@ static int launch_get_small_kernel(const GetJob &job, int device, cudaStream_t s
 	if (job.nbytes > GS_MAX_PAGE) {
 		static size_t configured_pair[MAX_DEV] = {};
 		if (smem > configured_pair[dev]) {
-			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 			configured_pair[dev] = smem;
 		}
-		k_get_small_pair<VERIFY><<<2u * job.n, GS_THREADS, smem, st>>>(job);
+		k_get_small_pair<VERIFY, TOUCH><<<2u * job.n, GS_THREADS, smem, st>>>(job);
 		CMB_CHECK(cudaGetLastError());
 		return 0;
 	}
 	static size_t configured[MAX_DEV] = {};
 	if (smem > configured[dev]) {
-		CMB_CHECK(cudaFuncSetAttribute(k_get_small<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+		CMB_CHECK(cudaFuncSetAttribute(k_get_small<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 		configured[dev] = smem;
 	}
-	k_get_small<VERIFY><<<job.n, GS_THREADS, smem, st>>>(job);
+	k_get_small<VERIFY, TOUCH><<<job.n, GS_THREADS, smem, st>>>(job);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
 int launch_get_small(const GetJob &job, int device, cudaStream_t st) {
 	if (job.n == 0) return 0;
-	return job.table.fp_tag ? launch_get_small_kernel<true>(job, device, st) : launch_get_small_kernel<false>(job, device, st);
+	if (job.touch_ts)
+		return job.table.fp_tag ? launch_get_small_kernel<true, true>(job, device, st) : launch_get_small_kernel<false, true>(job, device, st);
+	return job.table.fp_tag ? launch_get_small_kernel<true, false>(job, device, st) : launch_get_small_kernel<false, false>(job, device, st);
 }
 
 // Requests of k_get_small (CTAs) or k_get_small_pair (clusters) that can be resident on the device at
 // once (= scratch regions needed).  Clusters of two need two SMs of one GPC.
-template <bool VERIFY>
+template <bool VERIFY, bool TOUCH>
 static int get_small_residency_of(uint32_t nbytes) {
 	const size_t smem = get_small_smem(nbytes, VERIFY);
 	if (nbytes > GS_MAX_PAGE) {
-		if (cudaFuncSetAttribute(k_get_small_pair<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+		if (cudaFuncSetAttribute(k_get_small_pair<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
 		cudaLaunchConfig_t cfg = {};
 		cfg.gridDim = dim3(2u * (uint32_t)sm_count());
 		cfg.blockDim = dim3(GS_THREADS);
 		cfg.dynamicSmemBytes = smem;
 		int clusters = 0;
-		if (cudaOccupancyMaxActiveClusters(&clusters, k_get_small_pair<VERIFY>, &cfg) != cudaSuccess) return -1;
+		if (cudaOccupancyMaxActiveClusters(&clusters, k_get_small_pair<VERIFY, TOUCH>, &cfg) != cudaSuccess) return -1;
 		return clusters;
 	}
-	if (cudaFuncSetAttribute(k_get_small<VERIFY>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+	if (cudaFuncSetAttribute(k_get_small<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
 	int per_sm = 0;
-	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_get_small<VERIFY>, (int)GS_THREADS, smem) != cudaSuccess) return -1;
+	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_get_small<VERIFY, TOUCH>, (int)GS_THREADS, smem) != cudaSuccess) return -1;
 	return per_sm * sm_count();
 }
-int get_small_residency(uint32_t nbytes, bool verify) {
-	return verify ? get_small_residency_of<true>(nbytes) : get_small_residency_of<false>(nbytes);
+int get_small_residency(uint32_t nbytes, bool verify, bool touch) {
+	if (touch) return verify ? get_small_residency_of<true, true>(nbytes) : get_small_residency_of<false, true>(nbytes);
+	return verify ? get_small_residency_of<true, false>(nbytes) : get_small_residency_of<false, false>(nbytes);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -149,7 +149,15 @@ struct DecodeVerify {
 	const uint32_t *fp_tag;
 	unsigned long long *vstat;        // VS_WORDS counters
 };
-int launch_decode(const DecodeJob &job, cudaStream_t st, const DecodeVerify *verify = nullptr);
+// Store mode with CMB200_TOUCH: every request answered ST_HIT raises its slot's ts to `ts`
+// (k_decode_touch, k_decode_verify_touch).
+struct DecodeTouch {
+	const uint32_t *idx;              // per request, the key's slot (from lookup)
+	Slot *slots;
+	unsigned long long ts;
+};
+int launch_decode(const DecodeJob &job, cudaStream_t st, const DecodeVerify *verify = nullptr,
+    const DecodeTouch *touch = nullptr);
 
 // Fused small-batch get (one CTA per request): key lookup, record staged in shared memory by TMA,
 // LZ4 decode shared -> shared, page written out with 16-byte stores (device memory or page-locked
@@ -179,11 +187,13 @@ struct GetJob {
 	HotLog hot;                       // where tier hits are logged (null: no tier); last, so that the
 	                                  // other members keep their parameter offsets
 	unsigned long long *vstat;        // CMB200_VERIFY (table.fp_tag set): VS_WORDS counters
+	unsigned long long touch_ts;      // CMB200_TOUCH: a local hit raises its slot's ts to this; 0 = no touch
 };
 bool get_small_supports(uint32_t nbytes);
 size_t get_small_smem(uint32_t nbytes, bool verify);
 uint32_t get_small_region_entries(uint32_t nbytes);
-int get_small_residency(uint32_t nbytes, bool verify);   // requests resident on the device at once, < 0 on error
+// requests resident on the device at once, < 0 on error
+int get_small_residency(uint32_t nbytes, bool verify, bool touch);
 int launch_get_small(const GetJob &job, int device, cudaStream_t st);   // device: CUDA ordinal the launch runs on
 
 int launch_fingerprint(const uint8_t *pages, uint64_t stride, uint32_t nbytes, uint32_t n,

@@ -18,6 +18,9 @@
  * With CMB200_VERIFY=1 in the environment every engine checks each page it serves against the
  * page's stored EF128 fingerprint (cachemap_b200.h, CMB200_VERIFY): a page that differs is a miss,
  * counted in `requests` and not in `hits`, so the caller fetches and puts it again.
+ * With CMB200_EVICT=access, eviction (and demotion into a host tier) takes the pages read least
+ * recently instead of those put longest ago: every page a get serves has its timestamp raised to the time
+ * of the get (cachemap_b200.h, CMB200_TOUCH).  CMB200_EVICT=put, the default, is the reference's policy.
  * struct cachemap is opaque (edgefs.c never looks inside it).
  */
 #ifndef CACHEMAP_H

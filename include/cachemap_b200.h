@@ -38,6 +38,23 @@ typedef struct { uint64_t u; uint64_t l; } cmb200_addr;
  * rank, read from a peer's arena, or loaded from a snapshot written without fingerprints) is served
  * as CMB200_HIT and counted unverified.  See cmb200_verify_stats and cmb200_verify_store. */
 #define CMB200_VERIFY 2u
+/* Eviction by last access: every get of cmb200_get_small, cmb200_get_small_begin / _end, cmb200_get_batch
+ * and cmb200_get_batch_dev that answers CMB200_HIT for a LOCAL record (in the arena or the host tier)
+ * raises that record's timestamp attribute — the ts that cmb200_sample reports and eviction and demotion
+ * compare — to a stamp taken when the get is launched: CLOCK_REALTIME_COARSE in ns, the clock the
+ * reference's cachemap_put stamps with (cachemap.c:10-15).  The update is an atomic maximum, so ts never
+ * goes backwards whichever of two gets lands first.  Without the flag ts is the put time, as in the
+ * reference, and no get changes it.
+ * Nothing else touches: misses, CMB200_BAD_ENTRY, _BAD_DECODE, _CORRUPT, _INVALID and _REMOTE answers, hits
+ * served from a peer's arena (the slot is a replica; the owner's is in another process), and
+ * cmb200_locate_batch, cmb200_read_records, cmb200_verify_store, cmb200_sample, snapshots, compaction,
+ * demotion and promotion (which keep ts as it is).
+ * The stamps compare only with put timestamps of the same clock: the drop-in's puts use it; an engine
+ * level put with ts = NULL stores 0, older than any stamp.
+ * Two races are benign, because ts is eviction metadata and never decides which bytes a get returns: a
+ * touch that lands on a slot a put of the same key has just rewritten raises the new record's ts to about
+ * now, and a touch that races a table rebuild may be lost. */
+#define CMB200_TOUCH 4u
 
 typedef struct cmb200_config {
 	int device;             /* CUDA ordinal, -1 = current device */
@@ -278,7 +295,8 @@ int cmb200_copy_peer(cmb200_engine *dst_e, void *dst_dev, cmb200_engine *src_e, 
  * it overwrites are unset, an eviction like cmb200_unset_batch (retired_records).  A record leaves
  * the tier when it is unset, overwritten, retired or promoted back to the arena (cmb200_promote_batch).
  * A promoted record's tier bytes become tier garbage until the ring laps them; its key is not retired
- * then.  Promotion keeps the put timestamp, which the eviction policy reads. */
+ * then.  Promotion keeps the record's timestamp, which the eviction policy reads: the put time, or with
+ * CMB200_TOUCH the last hit, tier hits included. */
 struct cmb200_host_tier_stats {
 	uint64_t bytes, used, records, garbage;     /* tier size; bytes between oldest and newest record; live records; dead bytes */
 	uint64_t demoted_records, demoted_bytes;    /* moved from the arena so far (bytes = record lengths) */
