@@ -415,7 +415,12 @@ __device__ unsigned long long commit_record(const EncodeJob &job, uint32_t i, ui
 		}
 	}
 	ok = __shfl_sync(CMB_FULL, ok, 0);
-	if (!ok) { if (lane == 0 && job.rec_out) job.rec_out[i] = ~0ull; return ~0ull; }
+	if (!ok) {
+		// nothing was stored: lens_out says so (-1), as for a skipped chunk (cachemap_b200.h)
+		if (lane == 0 && job.rec_out) job.rec_out[i] = ~0ull;
+		if (lane == 0 && job.lens) job.lens[i] = -1;
+		return ~0ull;
+	}
 	off = __shfl_sync(CMB_FULL, off, 0);
 	uint8_t *rec = job.arena.base + off;
 	const unsigned long long au = job.addr[2 * i], al = job.addr[2 * i + 1];

@@ -78,9 +78,10 @@ def test_ordered_handout_with_duplicates_and_an_invalid_address(E, gpu, oracle, 
     eng.close()
 
 
-def test_ordered_handout_into_a_full_arena(E, gpu, oracle, monkeypatch):
+def test_ordered_handout_into_a_full_arena_reports_drops(E, gpu, oracle, monkeypatch):
     """Rewrite every key of a stored batch while the arena has room for about half of the new records:
-    a put that does not fit is dropped and counted, and its key still reads its old record."""
+    a put that does not fit is dropped and counted, its lens entry is -1 (it stored nothing), and its
+    key still reads its old record."""
     monkeypatch.setenv("CMB200_SEG_KB", "0")                    # records through the stage: exact arena accounting
     a_cids = np.arange(N, dtype=np.uint64)
     b_cids = a_cids + np.uint64(4 * N)
@@ -96,13 +97,14 @@ def test_ordered_handout_into_a_full_arena(E, gpu, oracle, monkeypatch):
     check_batch(E, oracle, eng, u, l, pa, lens_a, 12)
     assert eng.stats()["arena_garbage"] == 0
     lens_b = eng.put(u, l, pb)
-    assert (lens_b == lb).all()                                 # the block is made before the arena is asked
     out, status = eng.get(u, l)
     assert (status == E.HIT).all()
     new = np.array([(out[i] == pb[i]).all() for i in range(N)])
     old = np.array([(out[i] == pa[i]).all() for i in range(N)])
     assert (new ^ old).all(), "a key reads neither its old nor its new page"
     assert 0 < new.sum() < N
+    # lens: the stored block's length, -1 exactly for the puts the full arena dropped
+    assert (lens_b == np.where(new, lb, -1)).all()
     st = eng.stats()
     assert st["dropped_puts"] == int(old.sum())
     assert st["entries"] == N
