@@ -10,7 +10,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
-MISS, HIT, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, CORRUPT = 0, 1, 2, 3, 4, 5, 6
+MISS, HIT, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, CORRUPT, DROPPED = 0, 1, 2, 3, 4, 5, 6, 7
 FINGERPRINT = 1
 VERIFY = 2
 TOUCH = 4       # a hit raises its record's timestamp: eviction by last access (CMB200_EVICT=access)
@@ -22,6 +22,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_print_stats", "cachemap_put_batch", "cachemap_get_batch", "cachemap_put_batch_dev",
     "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
+    "cachemap_pread", "cachemap_pwrite",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -41,7 +42,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_promote_batch", "cmb200_host_tier_hot", "cmb200_read_checkpoints",
     "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
     "cmb200_verify_stats", "cmb200_verify_store", "cmb200_snapshot_begin", "cmb200_snapshot_finish",
-    "cmb200_chain_begin", "cmb200_load_chain", "cmb200_invalidate",
+    "cmb200_chain_begin", "cmb200_load_chain", "cmb200_invalidate", "cmb200_patch_batch",
 ]
 
 
@@ -104,6 +105,8 @@ def lib() -> C.CDLL:
         "cachemap_invalidate": (u64, [vp, u64, u32, u64, u64]),
         "cachemap_read_range": (i32, [vp, u64, u32, u64, sz, vp]),
         "cachemap_write_range": (None, [vp, u64, u32, u64, sz, vp]),
+        "cachemap_pread": (i32, [vp, u64, u32, u64, sz, vp]),
+        "cachemap_pwrite": (None, [vp, u64, u32, u64, sz, vp]),
         "filemap_create": (vp, [C.c_char_p, u64, i32, i32]),
         "filemap_free": (None, [vp]),
         "filemap_set": (None, [vp, vp, vp, u64]),
@@ -136,6 +139,7 @@ def lib() -> C.CDLL:
         "cmb200_get_batch_dev": (i32, [vp, sz, vp, vp, vp, vp]),
         "cmb200_unset_batch": (i32, [vp, sz, vp]),
         "cmb200_invalidate": (i32, [vp, u64, u64, u64, vp]),
+        "cmb200_patch_batch": (i32, [vp, sz, vp, vp, vp, vp, vp, vp]),
         "cmb200_entries": (u64, [vp]),
         "cmb200_sample": (i32, [vp, sz, vp, vp, vp, vp]),
         "cmb200_read_records": (i32, [vp, sz, vp, vp, sz, vp]),
@@ -499,6 +503,20 @@ class Engine:
         _check(lib().cmb200_invalidate(self.h, u, l_first, l_last, C.byref(removed)), "cmb200_invalidate")
         return removed.value
 
+    def patch(self, u, l, page_off, data, ts=None):
+        """cmb200_patch_batch: patch i writes data[i] (bytes) at byte page_off[i] of the page stored at
+        {u[i], l[i]}, in array order -> status per patch (HIT, MISS, BAD_ENTRY, BAD_DECODE, CORRUPT, DROPPED)."""
+        addr = _addr_array(u, l)
+        n = len(addr)
+        off = np.ascontiguousarray(page_off, dtype=np.uint32)
+        lens = np.array([len(d) for d in data], dtype=np.uint32)
+        blob = np.frombuffer(b"".join(bytes(d) for d in data) or b"\0", dtype=np.uint8)
+        ts = None if ts is None else np.ascontiguousarray(ts, dtype=np.uint64)
+        status = np.zeros(n, dtype=np.int32)
+        _check(lib().cmb200_patch_batch(self.h, n, _ptr(addr), _ptr(off), _ptr(lens), _ptr(blob), _ptr(ts),
+                                        _ptr(status)), "cmb200_patch_batch")
+        return status
+
     def entries(self) -> int:
         return int(lib().cmb200_entries(self.h))
 
@@ -735,6 +753,17 @@ class Cachemap:
         """The put loop of edgefs_read's miss path / edgefs_write (edgefs.c:1183-1195,1216-1228)."""
         data = np.ascontiguousarray(np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray)) else data)
         lib().cachemap_write_range(self.h, nhid, genid, off, data.size, _ptr(data))
+
+    def pread(self, nhid: int, genid: int, off: int, size: int):
+        """Any byte range [off, off + size) -> bytes when every page it overlaps hits, else None."""
+        out = np.zeros(max(size, 1), dtype=np.uint8)
+        ok = lib().cachemap_pread(self.h, nhid, genid, off, size, _ptr(out))
+        return out[:size].tobytes() if ok else None
+
+    def pwrite(self, nhid: int, genid: int, off: int, data):
+        """Any byte range: whole pages put, cached pages covered in part patched, the rest left uncached."""
+        data = np.ascontiguousarray(np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray)) else data)
+        lib().cachemap_pwrite(self.h, nhid, genid, off, data.size, _ptr(data))
 
     def checkpoint(self) -> int:
         return int(lib().cachemap_checkpoint(self.h))

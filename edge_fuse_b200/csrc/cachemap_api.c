@@ -67,6 +67,7 @@ extern int cmb200_owner(uint64_t key, int g);
 #pragma weak cmb200_dev_alloc
 #pragma weak cmb200_dev_free
 #pragma weak cmb200_invalidate
+#pragma weak cmb200_patch_batch
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -1999,18 +2000,26 @@ cachemap_get_batch_dev(struct cachemap *cm, uint64_t n, const uint64_t *offset, 
 
 /* ---- request ranges (edgefs.c:1159-1195, 1216-1228) ------------------------------------------ */
 
-int
-cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size,
-    void *out_buf)
+/* Where page i of n goes in a read of the pages from a page-aligned offset: into first (i == 0) or last
+ * (i == n - 1) when those are given, else into out, which holds the read from `skew` bytes into page 0. */
+static uint8_t *
+page_dst(uint64_t i, uint64_t n, int pshift, uint8_t *out, size_t skew, uint8_t *first, uint8_t *last)
+{
+	if (i == 0 && first)
+		return first;
+	if (i == n - 1 && last)
+		return last;
+	return out + ((i << pshift) - skew);
+}
+
+/* The page loop of edgefs_read over n >= 1 pages from the page-aligned offset off, each page to its
+ * page_dst.  1 when every page hits; requests / hits advance as the reference's loop advances them. */
+static int
+read_pages(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t n, uint8_t *out,
+    size_t skew, uint8_t *first, uint8_t *last)
 {
 	struct filemap *fm = cm->pages;
 	const int pshift = fm->pshift;
-	const uint64_t page_size = 1ULL << pshift;
-	if ((off & (page_size - 1)) || ((off + (uint64_t)size) & (page_size - 1)))     /* edgefs.c:192-203 */
-		return 0;
-	const uint64_t n = (uint64_t)size >> pshift;
-	if (n == 0)
-		return 1;
 	if (!filemap_engine_ready(fm))
 		return 0;
 	struct fm_req *reqs = calloc((size_t)n, sizeof(*reqs));
@@ -2027,7 +2036,7 @@ cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 	 * of requests per engine (one batch unless the chain is longer than COMBINE_MAX) */
 	size_t ask = 0;
 	for (uint64_t i = 0; i < n; i++) {
-		uint8_t *dst = (uint8_t *)out_buf + (i << pshift);
+		uint8_t *dst = page_dst(i, n, pshift, out, skew, first, last);
 		if (compose_addr(cm, off + (i << pshift), nhid_small, genid, &addr[ask]) != 0) {
 			state[i] = 2;
 			continue;
@@ -2055,7 +2064,7 @@ cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 	for (size_t j = 0; j < ask; j++) {
 		reqs[j].kind = REQ_GET;
 		reqs[j].addr = addr[order[j]];
-		reqs[j].dst = (uint8_t *)out_buf + ((uint64_t)page_of[order[j]] << pshift);
+		reqs[j].dst = page_dst(page_of[order[j]], n, pshift, out, skew, first, last);
 	}
 	/* every engine's chain is queued before any is waited for, in engine order (so that two callers
 	 * never hold the door of one engine while they wait for the other's) */
@@ -2090,6 +2099,20 @@ cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 	return i == n;
 }
 
+int
+cachemap_read_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size,
+    void *out_buf)
+{
+	const int pshift = cm->pages->pshift;
+	const uint64_t page_size = 1ULL << pshift;
+	if ((off & (page_size - 1)) || ((off + (uint64_t)size) & (page_size - 1)))     /* edgefs.c:192-203 */
+		return 0;
+	const uint64_t n = (uint64_t)size >> pshift;
+	if (n == 0)
+		return 1;
+	return read_pages(cm, nhid_small, genid, off, n, out_buf, 0, NULL, NULL);
+}
+
 void
 cachemap_write_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size,
     const void *data)
@@ -2102,6 +2125,132 @@ cachemap_write_range(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, u
 	 * edgefs.c:1186-1190 / 1219-1223 already hands the GPU one batch */
 	for (uint64_t i = 0; i < ((uint64_t)size >> pshift); i++)
 		cachemap_put(cm, off + (i << pshift), nhid_small, genid, (const uint8_t *)data + (i << pshift));
+}
+
+int
+cachemap_pread(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size, void *out_buf)
+{
+	const int pshift = cm->pages->pshift;
+	const uint64_t page_size = 1ULL << pshift;
+	if (size == 0)
+		return 1;
+	if ((uint64_t)size - 1 > UINT64_MAX - off)
+		return 0;
+	const uint64_t end = off + size;
+	const size_t skew = off & (page_size - 1), tail = end & (page_size - 1);
+	if (!skew && !tail)
+		return cachemap_read_range(cm, nhid_small, genid, off, size, out_buf);
+	/* the pages in between go straight to out_buf, the partial ones at the ends through whole pages */
+	const uint64_t n = ((end - 1) >> pshift) - (off >> pshift) + 1;
+	uint8_t *edge = malloc(2 * page_size);
+	if (!edge)
+		return 0;
+	uint8_t *first = skew || n == 1 ? edge : NULL;
+	uint8_t *last = tail && n > 1 ? edge + page_size : NULL;
+	const int ok = read_pages(cm, nhid_small, genid, off - skew, n, out_buf, skew, first, last);
+	if (ok) {
+		if (first)
+			memcpy(out_buf, first + skew, n == 1 ? size : page_size - skew);
+		if (last)
+			memcpy((uint8_t *)out_buf + (((n - 1) << pshift) - skew), last, tail);
+	}
+	free(edge);
+	return ok;
+}
+
+/* Writes len bytes at byte page_off of the cached page of `a` (filemap level, ts = the put time the
+ * patched page takes).  The newest page of the key in the engine's write-behind ring decides, as it
+ * decides a get: a page of `a` is copied into a new slot with the bytes applied, all under wb_mu, so that
+ * concurrent writers of one page each patch the other's result; a page of another address replaces the
+ * key's record anyway.  Without a ring page the engine patches its stored page (cmb200_patch_batch), or,
+ * if it cannot, drops it: no get returns the page's old bytes afterwards. */
+static void
+filemap_patch(struct filemap *m, const cmb200_addr *a, uint32_t page_off, uint32_t len, const void *bytes, uint64_t ts)
+{
+	const uint64_t k = addr_key(a);
+	struct fm_dev *d = m->dev[cmb200_owner(k, m->g)];
+	const size_t bsize = (size_t)m->bsize;
+	if (d->wb_n) {
+		pthread_mutex_lock(&d->wb_mu);
+		for (;;) {
+			uint64_t s = d->wb_head;
+			while (s > d->wb_tail && d->wb_slot[(s - 1) % d->wb_n].key != k)
+				s--;
+			if (s == d->wb_tail)
+				break;
+			struct wb_slot *w = &d->wb_slot[(s - 1) % d->wb_n];
+			if (w->state == WB_FILLING) {           /* a put of the key is copying its page in: take that one */
+				pthread_mutex_unlock(&d->wb_mu);
+				sched_yield();
+				pthread_mutex_lock(&d->wb_mu);
+				continue;
+			}
+			if (w->addr.u != a->u || w->addr.l != a->l) {
+				pthread_mutex_unlock(&d->wb_mu);
+				return;
+			}
+			if (d->wb_head - d->wb_tail == d->wb_n) {
+				pthread_cond_wait(&d->wb_space, &d->wb_mu);     /* the ring may have moved on: look again */
+				continue;
+			}
+			const uint64_t t = d->wb_head++;
+			struct wb_slot *nw = &d->wb_slot[t % d->wb_n];
+			uint8_t *page = d->wb_pages + (t % d->wb_n) * bsize;
+			memcpy(page, d->wb_pages + ((s - 1) % d->wb_n) * bsize, bsize);
+			memcpy(page + page_off, bytes, len);
+			nw->addr = *a;
+			nw->key = k;
+			nw->ts = ts;
+			nw->state = WB_READY;
+			if (d->wb_flusher_asleep)
+				pthread_cond_signal(&d->wb_work);
+			pthread_mutex_unlock(&d->wb_mu);
+			return;
+		}
+		pthread_mutex_unlock(&d->wb_mu);
+	}
+	/* a patch adds no entry, so only the arena needs room: no eviction by count */
+	filemap_check_arena(d, 1);
+	int32_t st = CMB200_MISS;
+	if (!cmb200_patch_batch || cmb200_patch_batch(d->eng, 1, a, &page_off, &len, bytes, &ts, &st) != 0) {
+		if (cmb200_patch_batch)
+			fprintf(stderr, "cachemap_b200: a page could not be patched, it is dropped: %s\n", cmb200_last_error());
+		cmb200_unset_batch(d->eng, 1, a);
+		st = CMB200_DROPPED;
+	}
+	/* a patched page and a removed one are changes of the store: the next checkpoint must write them */
+	if (st != CMB200_MISS && st != CMB200_BAD_ENTRY)
+		__atomic_fetch_add(&m->puts_seen, 1, __ATOMIC_RELAXED);
+}
+
+void
+cachemap_pwrite(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size, const void *data)
+{
+	struct filemap *fm = cm->pages;
+	const int pshift = fm->pshift;
+	const uint64_t page_size = 1ULL << pshift;
+	if (size == 0 || (uint64_t)size - 1 > UINT64_MAX - off)
+		return;
+	const uint64_t end = off + size;
+	const size_t skew = off & (page_size - 1), tail = end & (page_size - 1);
+	if (!skew && !tail) {
+		cachemap_write_range(cm, nhid_small, genid, off, size, data);
+		return;
+	}
+	const uint8_t *src = data;
+	const uint64_t p0 = off >> pshift, p1 = (end - 1) >> pshift;
+	/* pages the range covers whole are put */
+	for (uint64_t p = skew ? p0 + 1 : p0; p < (tail ? p1 : p1 + 1); p++)
+		cachemap_put(cm, p << pshift, nhid_small, genid, src + ((p << pshift) - off));
+	if (!filemap_engine_ready(fm))
+		return;
+	/* the one or two pages it covers in part are patched where cached */
+	const uint64_t ts = now_ns();
+	cmb200_addr a;
+	if (skew && compose_addr(cm, off, nhid_small, genid, &a) == 0)
+		filemap_patch(fm, &a, (uint32_t)skew, (uint32_t)(p1 == p0 ? size : page_size - skew), src, ts);
+	if (tail && (p1 != p0 || !skew) && compose_addr(cm, p1 << pshift, nhid_small, genid, &a) == 0)
+		filemap_patch(fm, &a, 0, (uint32_t)tail, src + ((p1 << pshift) - off), ts);
 }
 
 uint64_t

@@ -22,6 +22,7 @@
 #include <string>
 #include <new>
 #include <thread>
+#include <unordered_map>
 #include <unordered_set>
 #include <utility>
 #include <stdio.h>
@@ -219,6 +220,12 @@ struct cmb200_engine {
 	DevMem<uint32_t> d_import_slot;      // slot scratch of cmb200_import_records_dev, grown, never shrunk
 	DevMem<uint32_t> d_move_idx;         // index scratch of cmb200_move_pages (destination, then source), grown, never shrunk
 	DevMem<unsigned long long> d_removed; // records removed by cmb200_invalidate, allocated by its first call
+	// cmb200_patch_batch: the call's rows, spans and bytes, staged page-locked and copied over in one piece,
+	// grown, never shrunk; and the tier-hit counter and hot log its decode books into instead of the gets'
+	HostMem<uint8_t> h_patch;
+	size_t h_patch_bytes = 0;
+	DevMem<uint8_t> d_patch;
+	DevMem<unsigned long long> d_patch_hot;
 	// page-locked staging for the small per-chunk arrays, so that no copy ever blocks the host
 	// thread that is feeding the pipeline (a pageable cudaMemcpyAsync waits for the stream)
 	static constexpr size_t META_CAP = 1u << 18;   // chunks per outer slice of a call
@@ -1860,6 +1867,146 @@ extern "C" int cmb200_invalidate(cmb200_engine *e, uint64_t u, uint64_t l_first,
 		cmb200_engine::GateClosed gg(e->get_gate);
 		return rebuild_table_locked(e, c[1]);
 	}
+	return 0;
+}
+
+// ---- read-modify-write of stored pages ----------------------------------------------------------
+// The patches are grouped by address into rows of the page ring.  Rows, spans and bytes cross to the
+// device in one copy; then each slice of host_batch rows runs a get's lookup and decode into the ring,
+// k_patch, and a put's upsert and encode from the ring, so that only the written bytes cross PCIe.
+// The decode is a put's read, not a get: verified, it books into the store scan's counters (which
+// cmb200_verify_store zeroes before it reads them); otherwise its tier hits and hot-log entries go to
+// scratch words.  It never touches.
+static size_t align16(size_t v) { return (v + 15) & ~(size_t)15; }
+
+extern "C" int cmb200_patch_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint32_t *page_off,
+    const uint32_t *len, const void *bytes_host, const uint64_t *ts, int32_t *status_out) {
+	for (size_t i = 0; i < n; i++)
+		if (len[i] == 0 || (uint64_t)page_off[i] + len[i] > e->bsize) {
+			set_error_msg("cmb200_patch_batch: a patch is empty or reaches past the page");
+			return -1;
+		}
+	if (n >= 0xffffffffull) { set_error_msg("cmb200_patch_batch: too many patches"); return -1; }
+	std::lock_guard<std::mutex> g(e->mu);
+	if (e->multi_gpu) {
+		set_error_msg("cmb200_patch_batch: not available after a multi-GPU call (the index holds other ranks' records)");
+		return -1;
+	}
+	if (n == 0) return 0;
+	CMB_CHECK(cudaSetDevice(e->device));
+	// rows in order of first appearance; each patch's span goes to its row, in array order
+	std::unordered_map<std::pair<uint64_t, uint64_t>, uint32_t, AddrHash> row_of;
+	std::vector<uint32_t> row(n);
+	for (size_t i = 0; i < n; i++)
+		row[i] = row_of.emplace(std::make_pair(addr[i].u, addr[i].l), (uint32_t)row_of.size()).first->second;
+	const size_t R = row_of.size();
+	std::vector<uint32_t> first(R + 1, 0);                  // first span of each row
+	for (size_t i = 0; i < n; i++) first[row[i] + 1]++;
+	for (size_t r = 0; r < R; r++) first[r + 1] += first[r];
+	// staging: addr (16 / row), ts (8 / row), first (4 / row + 4), spans (16 / patch), bytes (each span
+	// placed congruent to its page offset modulo 16, so that k_patch moves it in 16-byte words), then the
+	// device-only valid flags (1 / row)
+	const size_t o_ts = R * 16, o_first = align16(o_ts + R * 8), o_spans = align16(o_first + (R + 1) * 4);
+	const size_t o_bytes = align16(o_spans + n * sizeof(PatchSpan));
+	size_t nbytes = 0;
+	for (size_t i = 0; i < n; i++) nbytes += len[i] + 15;
+	const size_t o_valid = align16(o_bytes + nbytes), total = o_valid + align16(R);
+	if (e->h_patch_bytes < o_valid) {
+		e->h_patch_bytes = 0;
+		if (e->h_patch.alloc(o_valid)) return -1;
+		e->h_patch_bytes = o_valid;
+	}
+	if (e->d_patch.grow(total, e->st)) return -1;
+	uint8_t *h = e->h_patch;
+	unsigned long long *h_addr = (unsigned long long *)h, *h_ts = (unsigned long long *)(h + o_ts);
+	PatchSpan *h_spans = (PatchSpan *)(h + o_spans);
+	std::vector<uint32_t> fill(first.begin(), first.end() - 1);
+	const uint8_t *src = (const uint8_t *)bytes_host;
+	size_t at = 0;                                          // next free byte of the bytes region
+	for (size_t i = 0; i < n; i++) {
+		const uint32_t r = row[i];
+		h_addr[2 * r] = addr[i].u; h_addr[2 * r + 1] = addr[i].l;
+		h_ts[r] = ts ? ts[i] : 0;                           // the last patch of the row wins
+		at += (page_off[i] - at) & 15u;
+		h_spans[fill[r]++] = PatchSpan{page_off[i], len[i], (unsigned long long)at};
+		memcpy(h + o_bytes + at, src, len[i]);
+		src += len[i];
+		at += len[i];
+	}
+	memcpy(h + o_first, first.data(), (R + 1) * 4);
+	uint8_t *d = e->d_patch;
+	CMB_CHECK(cudaMemcpyAsync(d, h, o_valid, cudaMemcpyHostToDevice, e->st));
+	const bool verify = e->table.fp_tag != nullptr;
+	if (!verify && e->tier.dev && !e->d_patch_hot) {
+		if (e->d_patch_hot.alloc((2 + 2 * (size_t)HOT_LOG_N) * sizeof(unsigned long long))) return -1;
+		CMB_CHECK(cudaMemsetAsync(e->d_patch_hot, 0, 2 * sizeof(unsigned long long), e->st));
+	}
+	std::vector<int32_t> st(R), lens(R);
+	std::vector<cmb200_addr> drop;
+	uint64_t stored = 0;
+	for (size_t r0 = 0; r0 < R; r0 += e->host_batch) {
+		const uint32_t m = (uint32_t)(R - r0 < e->host_batch ? R - r0 : e->host_batch);
+		const unsigned long long *d_addr = (const unsigned long long *)d + 2 * r0;
+		uint8_t *d_valid = d + o_valid + r0;
+		uint8_t *ring = e->d_pages[(r0 / e->host_batch) & 1];
+		if (launch_lookup(e->table, d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st,
+			verify ? (uint32_t *)e->d_vidx : nullptr)) return -1;
+		DecodeJob job{};
+		job.n = m; job.nbytes = e->bsize; job.pages = ring; job.status = e->d_status;
+		job.rec_off = e->d_recoff; job.vlen = e->d_vlen; job.arena = e->arena.base; job.host = e->tier.dev;
+		job.addr = d_addr;
+		if (verify) {
+			const DecodeVerify ver{e->d_vidx, e->table.fp, e->table.fp_tag, e->d_vstat + VS_WORDS};
+			if (launch_decode(job, e->st, &ver)) return -1;
+		} else {
+			if (e->d_patch_hot) {
+				job.host_hits = e->d_patch_hot;
+				job.hot = HotLog{e->d_patch_hot + 1, (ulonglong2 *)(e->d_patch_hot + 2)};
+			}
+			if (launch_decode(job, e->st)) return -1;
+		}
+		if (launch_patch(ring, e->bsize, m, e->d_status, (const uint32_t *)(d + o_first) + r0,
+			(const PatchSpan *)(d + o_spans), d + o_bytes, d_valid, e->st)) return -1;
+		if (launch_upsert(e->table, d_addr, d_valid, m, e->seq, e->seq_stride, e->d_slot, e->st)) return -1;
+		EncodeJob enc{};
+		enc.pages = ring; enc.page_stride = e->bsize; enc.nbytes = e->bsize; enc.n = m;
+		enc.accel = (uint32_t)e->accel;
+		enc.stage = e->d_stage; enc.stage_stride = e->stage_stride;
+		enc.lens = e->d_lens;
+		enc.rec_out = e->d_recoff_out;
+		enc.fps = (e->flags & CMB200_FINGERPRINT) ? (uint64_t *)e->d_fps : nullptr;
+		enc.work = e->d_work;
+		enc.order = e->d_order;
+		enc.slot_idx = e->d_slot;
+		enc.addr = d_addr;
+		enc.ts = ts ? (const unsigned long long *)(d + o_ts) + r0 : nullptr;
+		enc.seq0 = e->seq; enc.seq_stride = e->seq_stride;
+		enc.table = e->table; enc.arena = e->arena;
+		const int encode_kernels = launch_encode(enc, e->st);
+		if (encode_kernels < 0) return -1;
+		e->seq += (unsigned long long)m * e->seq_stride;
+		e->stats.kernel_launches += 4 + encode_kernels;
+		CMB_CHECK(cudaMemcpyAsync(st.data() + r0, e->d_status, m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemcpyAsync(lens.data() + r0, e->d_lens, m * 4, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		for (size_t r = r0; r < r0 + m; r++) {
+			// a hit that stored nothing was dropped for lack of arena space (the encoder leaves the slot as it was)
+			if (st[r] == CMB200_HIT && lens[r] < 0) st[r] = CMB200_DROPPED;
+			if (st[r] == CMB200_HIT) stored++;
+			if (st[r] == CMB200_DROPPED || st[r] == CMB200_BAD_DECODE || st[r] == CMB200_CORRUPT)
+				drop.push_back(cmb200_addr{h_addr[2 * r], h_addr[2 * r + 1]});
+		}
+	}
+	// records that cannot be trusted, and old pages whose patched version found no room, leave the store
+	for (size_t k = 0; k < drop.size(); k += e->max_batch) {
+		const uint32_t m = (uint32_t)(drop.size() - k < e->max_batch ? drop.size() - k : e->max_batch);
+		CMB_CHECK(cudaMemcpyAsync(e->d_addr, drop.data() + k, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
+		if (launch_unset(e->table, e->arena, e->d_addr, m, e->st)) return -1;
+		e->stats.kernel_launches++;
+	}
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	e->stats.put_chunks += stored;
+	for (size_t i = 0; i < n; i++) status_out[i] = st[row[i]];
 	return 0;
 }
 

@@ -2005,4 +2005,40 @@ int launch_move_pages(void *dst, const uint32_t *dst_idx, const void *src, const
 	return 0;
 }
 
+// ---- read-modify-write of stored pages (cmb200_patch_batch) ------------------------------------
+// One CTA per page-ring row.  A row that lookup and decode did not answer ST_HIT is left out of the
+// upsert (valid = 0); the spans of every other row are copied over its decoded page in array order,
+// with a barrier after each, since a later span may overwrite bytes of an earlier one.  The part of a
+// span between the 16-byte boundaries of source and destination moves in 16-byte words when the two are
+// congruent modulo 16 (the engine lays the bytes out so that they are), the ragged ends byte by byte.
+__global__ void __launch_bounds__(256) k_patch(uint8_t *pages, uint32_t nbytes, const int32_t *status,
+    const uint32_t *first, const PatchSpan *spans, const uint8_t *bytes, uint8_t *valid) {
+	const uint32_t row = blockIdx.x;
+	const bool hit = status[row] == ST_HIT;
+	if (threadIdx.x == 0) valid[row] = hit;
+	if (!hit) return;
+	uint8_t *page = pages + (size_t)row * nbytes;
+	for (uint32_t k = first[row]; k < first[row + 1]; k++) {
+		const PatchSpan s = spans[k];
+		uint8_t *dst = page + s.page_off;
+		const uint8_t *src = bytes + s.src_off;
+		const bool wide = ((s.page_off ^ s.src_off) & 15u) == 0;
+		const uint32_t lead = wide ? min((0u - s.page_off) & 15u, s.len) : s.len;
+		const uint32_t words = (s.len - lead) >> 4;
+		const uint32_t tail = lead + (words << 4);
+		for (uint32_t j = threadIdx.x; j < lead; j += blockDim.x) dst[j] = src[j];
+		for (uint32_t j = threadIdx.x; j < words; j += blockDim.x)
+			reinterpret_cast<uint4 *>(dst + lead)[j] = reinterpret_cast<const uint4 *>(src + lead)[j];
+		for (uint32_t j = tail + threadIdx.x; j < s.len; j += blockDim.x) dst[j] = src[j];
+		__syncthreads();
+	}
+}
+int launch_patch(uint8_t *pages, uint32_t nbytes, uint32_t rows, const int32_t *status, const uint32_t *first,
+    const PatchSpan *spans, const uint8_t *bytes, uint8_t *valid, cudaStream_t st) {
+	if (rows == 0) return 0;
+	k_patch<<<rows, 256, 0, st>>>(pages, nbytes, status, first, spans, bytes, valid);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
 }  // namespace cmb

@@ -325,6 +325,15 @@ int launch_rehash(TableView from, TableView to, cudaStream_t st);
 int launch_move_pages(void *dst, const uint32_t *dst_idx, const void *src, const uint32_t *src_idx, uint32_t n,
     uint32_t nbytes, cudaStream_t st);
 
+// ---- read-modify-write of stored pages (cmb200_patch_batch) ----
+// Span k of a row: len bytes at bytes + src_off go to byte page_off of the row's decoded page.
+struct PatchSpan { uint32_t page_off, len; unsigned long long src_off; };
+static_assert(sizeof(PatchSpan) == 16, "patch span layout");
+// For each of `rows` pages (nbytes apart, 16-byte aligned): valid[r] = status[r] == ST_HIT, and on a hit
+// spans first[r] .. first[r + 1] - 1 are applied in order.  bytes is 16-byte aligned.
+int launch_patch(uint8_t *pages, uint32_t nbytes, uint32_t rows, const int32_t *status, const uint32_t *first,
+    const PatchSpan *spans, const uint8_t *bytes, uint8_t *valid, cudaStream_t st);
+
 int sm_count();
 
 }  // namespace cmb

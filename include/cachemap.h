@@ -83,6 +83,22 @@ void cachemap_write_range(struct cachemap *cm, uint64_t nhid_small, uint32_t gen
     size_t size, const void *data);
 
 /*
+ * Any byte range [off, off + size) of object (nhid_small, genid), for requests whose ends are not
+ * page-aligned (INTEGRATION.md).
+ * cachemap_pread: 1 and out_buf[0..size) filled when every page overlapping the range hits (ring or
+ * store), else 0.  requests / hits advance over those pages as cachemap_read_range's do (page order,
+ * stop at the first miss).  An aligned range behaves exactly as cachemap_read_range; size 0 returns 1.
+ * cachemap_pwrite: pages the range covers whole are put (cachemap_put).  A page it covers in part is
+ * patched if it is cached (on the GPU, cmb200_patch_batch: only the written bytes cross PCIe), and left
+ * uncached otherwise.  Afterwards no get returns the page's old bytes.  Concurrent writes of disjoint
+ * bytes of one page all land.  An aligned range behaves exactly as cachemap_write_range.
+ */
+int cachemap_pread(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size,
+    void *out_buf);
+void cachemap_pwrite(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, size_t size,
+    const void *data);
+
+/*
  * Persistence.  The reference's cache survives a restart because its store is a set of LMDB files
  * in destdir (cachemap/filemap.c:57,71-72).  Here the store is in HBM: it is written to
  * destdir/cachemap_b200.snap by cachemap_free, by cachemap_checkpoint, and every

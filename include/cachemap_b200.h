@@ -76,9 +76,10 @@ enum {
 	CMB200_BAD_ENTRY = 3,   /* key present under another address: a miss (filemap.c:236-240) */
 	CMB200_BAD_DECODE = 4,  /* decoded length != stored length: a miss (filemap.c:244-248) */
 	CMB200_REMOTE = 5,      /* multi-GPU: the newest record of this key lives on another rank */
-	CMB200_CORRUPT = 6      /* CMB200_VERIFY: the decoded page differs from the stored EF128: a miss.
+	CMB200_CORRUPT = 6,     /* CMB200_VERIFY: the decoded page differs from the stored EF128: a miss.
 	                         * The page is not written by cmb200_get_small; cmb200_get_batch(_dev) may
 	                         * have written it, as for CMB200_BAD_DECODE. */
+	CMB200_DROPPED = 7      /* cmb200_patch_batch: the patched page did not fit the arena */
 };
 
 const char *cmb200_last_error(void);
@@ -141,6 +142,27 @@ int cmb200_unset_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr);
  * l_first > l_last, or on an engine that has made a multi-GPU call (its index holds other ranks'
  * records). */
 int cmb200_invalidate(cmb200_engine *e, uint64_t u, uint64_t l_first, uint64_t l_last, uint64_t *removed_out);
+/* Read-modify-write of stored pages.  Patch i writes len[i] >= 1 bytes at byte page_off[i] of the page
+ * stored at addr[i] (page_off[i] + len[i] <= 1 << pshift).  bytes_host holds the patches' bytes back to
+ * back in array order.  ts (nullable) as for cmb200_put_batch; a page patched more than once in the call
+ * takes the ts of its last patch.  status_out[i]:
+ *   CMB200_HIT        the new page (old page, patches applied) is stored, exactly as a put of it would
+ *                     store it: same record bytes, fingerprint, parse checkpoints, ts, sequence
+ *   CMB200_MISS       no record of addr[i]: nothing is stored (the rest of the page is unknown)
+ *   CMB200_BAD_ENTRY  the key holds another address: nothing changes
+ *   CMB200_BAD_DECODE / CMB200_CORRUPT   the stored record cannot be trusted: it is removed
+ *   CMB200_DROPPED    the new record did not fit the arena: the old record is removed
+ * After the call, a get of addr[i] returns the patched page or misses.  It never returns the old page.
+ * Patches of one address in one call are applied in array order to one page and stored once; they all
+ * get the same status.  Ordered after everything enqueued on the engine before the call, async puts
+ * included; runs under the engine lock on its stream, as cmb200_invalidate does.  A concurrent
+ * cmb200_get_small returns the old or the new page, never a mix.  A patch is a put, not a get: the get
+ * counters, the verified-read counters, tier hits, the tier's hot log and CMB200_TOUCH stamps do not move;
+ * put_chunks counts the pages stored.  A patched host-tier record is stored again in the arena and its
+ * tier bytes become tier garbage.  -1 before anything is applied if an extent is out of the page or len
+ * is 0, and on an engine that has made a multi-GPU call. */
+int cmb200_patch_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint32_t *page_off,
+    const uint32_t *len, const void *bytes_host, const uint64_t *ts, int32_t *status_out);
 uint64_t cmb200_entries(cmb200_engine *e);
 int cmb200_sample(cmb200_engine *e, size_t n, const uint64_t *r, cmb200_addr *addr_out,
     uint64_t *ts_out, int32_t *ok_out);
