@@ -136,6 +136,9 @@ struct fm_dev {
 	int wb_started, wb_stop;
 	int wb_flusher_asleep;  /* the flusher waits on wb_work (under wb_mu) */
 	pthread_mutex_t land_mu;        /* held while a put batch lands in this engine (filemap_land_begin) */
+	/* held from making arena room until the call that uses it is done (a put batch, a patch, a promotion
+	 * round), so that no other call on this engine takes the room in between and the put drops pages */
+	pthread_mutex_t room_mu;
 	/* staging of this engine's share of batch calls that span engines (stage_mu): page-locked host
 	 * pages, and device buffers on the first engine's GPU and on this engine's, grown as needed */
 	pthread_mutex_t stage_mu;
@@ -262,6 +265,7 @@ fm_dev_free(struct fm_dev *d)
 	free(d->promo_guard);
 	pthread_mutex_destroy(&d->promo_mu);
 	pthread_mutex_destroy(&d->land_mu);
+	pthread_mutex_destroy(&d->room_mu);
 	pthread_mutex_destroy(&d->stage_mu);
 	pthread_mutex_destroy(&d->q_mu);
 	sem_destroy(&d->q_door);
@@ -310,6 +314,7 @@ fm_dev_start(struct filemap *m, int index, int device, int g)
 	pthread_cond_init(&d->wb_idle, NULL);
 	pthread_mutex_init(&d->promo_mu, NULL);
 	pthread_mutex_init(&d->land_mu, NULL);
+	pthread_mutex_init(&d->room_mu, NULL);
 	pthread_mutex_init(&d->stage_mu, NULL);
 
 	cmb200_config cfg;
@@ -1025,9 +1030,12 @@ filemap_promote_round(struct fm_dev *d)
 	}
 	if (n == 0)
 		return;
+	pthread_mutex_lock(&d->room_mu);
 	filemap_arena_room(d, n, 0);
 	uint64_t got = 0;
-	if (cmb200_promote_batch(d->eng, n, d->promo_hot, &got) != 0) {
+	const int rc = cmb200_promote_batch(d->eng, n, d->promo_hot, &got);
+	pthread_mutex_unlock(&d->room_mu);
+	if (rc != 0) {
 		fprintf(stderr, "cachemap_b200: promotion from the host tier failed: %s\n", cmb200_last_error());
 		return;
 	}
@@ -1060,6 +1068,32 @@ filemap_make_room(struct fm_dev *d, uint64_t incoming)
 	filemap_check_arena(d, incoming);
 }
 
+/* After a put of n pages whose stored lengths are lens (-1: nothing stored): the keys whose newest page
+ * in the batch found no arena room are unset.  The engine leaves such a key's record as it was, and
+ * that record holds bytes older than the page just written; served, it would be stale. */
+static void
+filemap_unset_dropped(struct fm_dev *d, size_t n, const cmb200_addr *addr, const int32_t *lens)
+{
+	cmb200_addr *v = NULL;
+	size_t nv = 0;
+	for (size_t i = 0; i < n; i++) {
+		if (lens[i] >= 0)
+			continue;
+		size_t j = i + 1;       /* a later row of the same key supersedes this one (its lens is -1 too) */
+		const uint64_t k = addr_key(&addr[i]);
+		while (j < n && addr_key(&addr[j]) != k)
+			j++;
+		if (j < n)
+			continue;
+		if (!v && !(v = malloc(n * sizeof(*v))))
+			return;
+		v[nv++] = addr[i];
+	}
+	if (nv)
+		cmb200_unset_batch(d->eng, nv, v);
+	free(v);
+}
+
 static void
 timespec_add_ms(struct timespec *t, long ms)
 {
@@ -1077,6 +1111,7 @@ filemap_flusher(void *arg)
 	struct filemap *m = d->m;
 	cmb200_addr *addr = malloc(FLUSH_MAX * sizeof(cmb200_addr));
 	uint64_t *ts = malloc(FLUSH_MAX * sizeof(uint64_t));
+	int32_t *lens = malloc(FLUSH_MAX * sizeof(int32_t));
 	pthread_mutex_lock(&d->wb_mu);
 	for (;;) {
 		uint64_t count = 0;
@@ -1122,14 +1157,20 @@ filemap_flusher(void *arg)
 		const uint64_t first = d->wb_tail % d->wb_n;
 		pthread_mutex_unlock(&d->wb_mu);
 
-		if (addr && ts) {
+		if (addr && ts && lens) {
+			pthread_mutex_lock(&d->room_mu);
 			filemap_make_room(d, count);
 			filemap_land_begin(d);
 			uint64_t run1 = count < d->wb_n - first ? count : d->wb_n - first;
-			cmb200_put_batch(d->eng, (size_t)run1, addr, NULL, d->wb_pages + first * (size_t)m->bsize, ts, NULL);
+			for (uint64_t i = 0; i < count; i++)
+				lens[i] = 0;
+			cmb200_put_batch(d->eng, (size_t)run1, addr, NULL, d->wb_pages + first * (size_t)m->bsize, ts, lens);
 			if (run1 < count)
-				cmb200_put_batch(d->eng, (size_t)(count - run1), addr + run1, NULL, d->wb_pages, ts + run1, NULL);
+				cmb200_put_batch(d->eng, (size_t)(count - run1), addr + run1, NULL, d->wb_pages, ts + run1, lens + run1);
+			/* while the slots are still in the ring, which answers gets of their keys */
+			filemap_unset_dropped(d, (size_t)count, addr, lens);
 			filemap_land_end(d, count);
+			pthread_mutex_unlock(&d->room_mu);
 		}
 
 		pthread_mutex_lock(&d->wb_mu);
@@ -1148,6 +1189,7 @@ filemap_flusher(void *arg)
 	pthread_mutex_unlock(&d->wb_mu);
 	free(addr);
 	free(ts);
+	free(lens);
 	return NULL;
 }
 
@@ -1380,10 +1422,14 @@ filemap_set(struct filemap *m, uint128_t *key, void *value, uint64_t attr)
 	const uint64_t k = addr_key(&a);
 	struct fm_dev *d = m->dev[cmb200_owner(k, m->g)];
 	if (!d->wb_n) {                         /* write-behind disabled: one synchronous GPU put */
+		pthread_mutex_lock(&d->room_mu);
 		filemap_make_room(d, 1);
 		filemap_land_begin(d);
-		cmb200_put_batch(d->eng, 1, &a, NULL, value, &attr, NULL);
+		int32_t len = 0;
+		cmb200_put_batch(d->eng, 1, &a, NULL, value, &attr, &len);
+		filemap_unset_dropped(d, 1, &a, &len);
 		filemap_land_end(d, 1);
+		pthread_mutex_unlock(&d->room_mu);
 		__atomic_fetch_add(&m->puts_seen, 1, __ATOMIC_RELAXED);
 		return;
 	}
@@ -1716,6 +1762,7 @@ put_part(void *arg)
 	const size_t bsize = (size_t)m->bsize, bytes = p->c * bsize;
 	int rc = -1;
 	pthread_mutex_lock(&d->stage_mu);
+	pthread_mutex_lock(&d->room_mu);
 	filemap_check_arena(d, p->c);
 	filemap_land_begin(d);
 	if (!p->on_dev) {
@@ -1741,6 +1788,7 @@ put_part(void *arg)
 			rc = cmb200_put_batch_dev(d->eng, p->c, p->addr, p->valid, buf, p->ts, NULL);
 	}
 	filemap_land_end(d, p->c);
+	pthread_mutex_unlock(&d->room_mu);
 	pthread_mutex_unlock(&d->stage_mu);
 	if (rc != 0)
 		fprintf(stderr, "cachemap_b200: %zu pages not stored on engine %d: %s\n", p->c, d->index, cmb200_last_error());
@@ -1862,6 +1910,7 @@ put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 			struct fm_dev *d = fm->dev[k];
 			if (c == m && (k == 0 || !on_dev)) {
 				/* the whole slice is this engine's (always so with one engine): the caller's arrays as they are */
+				pthread_mutex_lock(&d->room_mu);
 				filemap_check_arena(d, c);
 				filemap_land_begin(d);
 				if (on_dev)
@@ -1873,6 +1922,7 @@ put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 					cmb200_put_batch_async(d->eng, (size_t)m, bk.addr + at, bk.valid + at, pg, bk.ts + at, NULL, &ticket);
 				}
 				filemap_land_end(d, m);
+				pthread_mutex_unlock(&d->room_mu);
 				continue;
 			}
 			struct batch_part *p = &parts[np];
@@ -2210,6 +2260,7 @@ filemap_patch(struct filemap *m, const cmb200_addr *a, uint32_t page_off, uint32
 		pthread_mutex_unlock(&d->wb_mu);
 	}
 	/* a patch adds no entry, so only the arena needs room: no eviction by count */
+	pthread_mutex_lock(&d->room_mu);
 	filemap_check_arena(d, 1);
 	int32_t st = CMB200_MISS;
 	if (!cmb200_patch_batch || cmb200_patch_batch(d->eng, 1, a, &page_off, &len, bytes, &ts, &st) != 0) {
@@ -2218,6 +2269,7 @@ filemap_patch(struct filemap *m, const cmb200_addr *a, uint32_t page_off, uint32
 		cmb200_unset_batch(d->eng, 1, a);
 		st = CMB200_DROPPED;
 	}
+	pthread_mutex_unlock(&d->room_mu);
 	/* a patched page and a removed one are changes of the store: the next checkpoint must write them */
 	if (st != CMB200_MISS && st != CMB200_BAD_ENTRY)
 		__atomic_fetch_add(&m->puts_seen, 1, __ATOMIC_RELAXED);

@@ -10,6 +10,8 @@
  * a put replaces the key's record whatever address it held, a get of a key that holds another address
  * answers CMB200_BAD_ENTRY, and an unset deletes the key's record.  mock_hold_puts(1) makes every put
  * wait until mock_hold_puts(0), so that a test can keep pages in the drop-in's write-behind ring.
+ * A put of a page that begins with the 8 bytes MOCK_DROP finds no room, as a put into a full arena:
+ * lens_out is -1 and the key keeps the record it had.
  * Nothing of the product links against this file. */
 #include <pthread.h>
 #include <sched.h>
@@ -26,6 +28,7 @@
 #define LANES 32
 #define LANE_MAX 1024
 #define WORKERS 6
+#define MOCK_DROP "MOCKDROP"
 
 struct entry { int used; uint64_t key; cmb200_addr a; uint64_t ts; uint8_t *page; };
 
@@ -156,6 +159,7 @@ int cmb200_put_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 	pthread_mutex_lock(&e->mu);
 	for (size_t i = 0; i < n; i++) {
 		if (valid && !valid[i]) { if (lens_out) lens_out[i] = -1; continue; }
+		if (memcmp((const uint8_t *)pages + i * e->bsize, MOCK_DROP, 8) == 0) { if (lens_out) lens_out[i] = -1; continue; }
 		int present;
 		struct entry *s = find(e, &addr[i], &present);
 		if (!s) continue;                                         /* map full: dropped */

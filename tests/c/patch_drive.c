@@ -9,6 +9,8 @@
  *   patch_drive multi <dir>     patches reach the engine that owns the page's key (CMB200_DEVICES)
  *   patch_drive ckpt <dir>      checkpoint ticks (CMB200_CHECKPOINT_SEC=1) before and after a patch-only change
  *   patch_drive fallback <dir>  without cmb200_patch_batch a page covered in part is dropped
+ *   patch_drive dropped <dir>   puts the store drops (pages beginning with MOCKDROP, mock_engine.c) leave
+ *                               no old page behind; with the ring on, also within one flush batch
  *   patch_drive stress <dir> <threads> <seconds>
  *                               threads pwrite disjoint bytes of one page while its puts are held back
  *                               for a while and others read it; every thread's last bytes must land
@@ -190,6 +192,43 @@ int main(int argc, char **argv) {
 			for (const char *q = log; (q = strstr(q, "save\n")) != NULL; q++) saves[k]++;
 		}
 		printf("saves %d %d %d\n", saves[0], saves[1], saves[2]);
+	} else if (strcmp(mode, "dropped") == 0) {
+		put_all(5, 1);
+		struct cmb200_engine *e;
+		cachemap_engines(cm, &e, 1);
+		for (uint64_t p = 2; p <= 3; p++) {                                 /* rewritten, and dropped */
+			memset(model + p * P, (int)(0xd0 + p), P);
+			memcpy(model + p * P, "MOCKDROP", 8);
+			cachemap_put(cm, p * P, 5, 0, model + p * P);
+		}
+		cachemap_engines(cm, &e, 1);
+		int cached, wrong;
+		check_pages(&cached, &wrong);
+		printf("dropped %d %d\n", cached, wrong);
+		const char *wb = getenv("CMB200_WB_SLOTS");
+		if (!wb || atoi(wb) != 0) {
+			/* one flush batch: page 4 dropped, then put again; page 5 put again, then dropped */
+			mock_hold_puts(1);
+			cachemap_put(cm, 0, 5, 0, model);                               /* the flusher takes it and waits */
+			usleep(50000);
+			for (uint64_t p = 4; p <= 5; p++) {
+				uint8_t *pg = model + p * P;
+				memset(pg, (int)(0xe0 + p), P);
+				if (p == 4) memcpy(pg, "MOCKDROP", 8);
+				cachemap_put(cm, p * P, 5, 0, pg);
+				memset(pg, (int)(0xf0 + p), P);
+				if (p == 5) memcpy(pg, "MOCKDROP", 8);
+				cachemap_put(cm, p * P, 5, 0, pg);
+			}
+			pthread_t t;
+			pthread_create(&t, NULL, release_puts, NULL);
+			pthread_join(t, NULL);
+			cachemap_engines(cm, &e, 1);
+			void *p4 = cachemap_get(cm, 4 * P, 5, 0);
+			check_pages(&cached, &wrong);
+			printf("batch %d %d %d\n", p4 != NULL, cached, wrong);
+			free(p4);
+		}
 	} else if (strcmp(mode, "fallback") == 0) {
 		put_all(5, 1);
 		struct cmb200_engine *e;

@@ -3,7 +3,8 @@
 The model (`Model`) wraps oracle StoreModel, which decides hit, miss and bad entry and holds each key's
 exact record bytes, and adds what the engine's bookkeeping must agree with: each record's page, tier
 (arena or host), ring position in the host tier, fingerprint, parse checkpoints and timestamp, the arena's
-bump pointer and the host tier's ring.  `gen_ops` turns a seed into a replayable list of operations over
+bump pointer and the host tier's ring.  A patch is restated as cmb200_patch_batch stores it: a put of
+each named page with its spans applied.  `gen_ops` turns a seed into a replayable list of operations over
 every engine call; `census` runs a log through the model alone and reports which rare events it reaches.
 CPU only: the GPU test (test_gpu_store_machine.py) drives an engine and this model side by side.
 """
@@ -20,6 +21,7 @@ from ckpt_def import ckpt_words
 
 FINGERPRINT, VERIFY, TOUCH = 1, 2, 4
 MISS, HIT, INVALID, BAD_ENTRY = 0, 1, 2, 3
+DROPPED = 7
 KEY_SENTINELS = (0, (1 << 64) - 1)
 
 
@@ -57,20 +59,29 @@ class MachineConfig:
 
 
 ALL_EVENTS = ("drop", "compact", "rebuild", "wrap", "inval_keyed", "inval_scan", "load", "promote_after_demote_after_compact")
+# patch_drop needs exact_head, patch_host a host tier, patch_slices a call with more rows than max_batch
+PATCH_EVENTS = ("patch_hit", "patch_miss", "patch_bad_entry", "patch_sentinel", "patch_after_load")
 
 CONFIGS = {
     "A": MachineConfig("A", 12, 12, VERIFY, 96 << 10, 1024, 512 << 10, 2048, 2 << 20,
-                       (("CMB200_SEG_KB", "0"),), (3, 5, 7), 80, 48, 70, (11, 12), True, ALL_EVENTS),
+                       (("CMB200_SEG_KB", "0"),), (3, 5, 7), 80, 48, 70, (11, 12), True,
+                       ALL_EVENTS + PATCH_EVENTS + ("patch_drop", "patch_host")),
     "B": MachineConfig("B", 16, 12, FINGERPRINT | TOUCH, 0, 1024, 512 << 20, 4096, 384 << 20,
                        (("CMB200_SEG_KB", "512"),), (3, 5), 24, 12, 30, (21, 22), False,
-                       ("compact", "rebuild", "inval_keyed", "inval_scan", "load")),
+                       ("compact", "rebuild", "inval_keyed", "inval_scan", "load") + PATCH_EVENTS),
     "C": MachineConfig("C", 17, 12, VERIFY, 1 << 20, 1024, 3 << 20, 2048, 12 << 20,
                        (), (3, 5), 16, 8, 30, (31, 32), True,
-                       ("drop", "compact", "rebuild", "wrap", "inval_keyed", "inval_scan", "load",
-                        "promote_after_demote_after_compact")),
+                       ALL_EVENTS + PATCH_EVENTS + ("patch_drop", "patch_host")),
     "D": MachineConfig("D", 12, 0, 0, 0, 1024, 1536 << 10, 2048, 4 << 20,
                        (("CMB200_CKPT", "0"),), (3, 5, 7), 80, 48, 60, (41, 42), True,
-                       ("drop", "compact", "rebuild", "inval_keyed", "inval_scan", "load")),
+                       ("drop", "compact", "rebuild", "inval_keyed", "inval_scan", "load") + PATCH_EVENTS
+                       + ("patch_drop",)),
+    # verified and touching gets together, 16 KiB pages, and a page ring of 32 rows, so that an
+    # ordinary patch call spans ring slices
+    "E": MachineConfig("E", 14, 12, VERIFY | TOUCH, 192 << 10, 1024, 1 << 20, 2048, 4 << 20,
+                       (("CMB200_SEG_KB", "0"),), (3, 5), 32, 24, 60, (51, 52), True,
+                       ALL_EVENTS + PATCH_EVENTS + ("patch_drop", "patch_host", "patch_slices"),
+                       max_batch=32),
 }
 
 
@@ -94,6 +105,12 @@ def universe(cfg: MachineConfig) -> list:
 
 def alloc(payload: int) -> int:
     return (24 + payload + 15) & ~15
+
+
+def span_bytes(span) -> bytes:
+    """A patch span (page offset, length, fill, seed) -> its bytes: fill "R" random, "0" zeros."""
+    _off, n, fill, seed = span
+    return bytes(n) if fill == "0" else datagen.rand_bytes(seed, n).tobytes()
 
 
 # ---- model ----------------------------------------------------------------------------------------
@@ -213,6 +230,62 @@ class Model:
 
     def certain_drop(self, addrs, pages, valid) -> bool:
         return bool(self.stand_in_drops(addrs, pages, valid))
+
+    # patch (engine.cu cmb200_patch_batch): a read-modify-write put of each stored page it names
+    @staticmethod
+    def patch_rows(addrs) -> list:
+        """Distinct addresses, in order of first appearance: the rows of the call."""
+        return list(dict.fromkeys(tuple(a) for a in addrs))
+
+    def patch_status(self, a) -> int:
+        r = self.rec.get(self.key(a))
+        if r is None:
+            return MISS
+        return HIT if r.addr == tuple(a) else BAD_ENTRY
+
+    def patched_pages(self, addrs, spans) -> dict:
+        """{row: patched page} of the rows that hit; each row's spans apply in array order."""
+        rows = self.patch_rows(addrs)
+        out = {i: np.frombuffer(self.live(a).page, dtype=np.uint8).copy()
+               for i, a in enumerate(rows) if self.patch_status(a) == HIT}
+        row_of = {a: i for i, a in enumerate(rows)}
+        for a, s in zip(addrs, spans):
+            pg = out.get(row_of[tuple(a)])
+            if pg is not None:
+                pg[s[0]:s[0] + s[1]] = np.frombuffer(span_bytes(s), dtype=np.uint8)
+        return out
+
+    def patch_stand_in_drops(self, addrs, spans) -> set:
+        """Rows whose patched record a sequential bump allocator drops (see stand_in_drops)."""
+        pages = self.patched_pages(addrs, spans)
+        rows = sorted(pages)
+        rows_of = self.patch_rows(addrs)
+        got = self.stand_in_drops([rows_of[i] for i in rows], [pages[i] for i in rows], None)
+        return {rows[j] for j in got}
+
+    def patch(self, addrs, spans, ts, dropped_rows) -> list:
+        """Applies a patch whose rows `dropped_rows` (row indices) found no arena room -> status per patch.
+        A hit row is stored as a put of its patched page with the ts of the row's last patch (0 without
+        ts); a dropped one is counted as a dropped put and its key removed, as the engine unsets it."""
+        rows = self.patch_rows(addrs)
+        status = [self.patch_status(a) for a in rows]
+        pages = self.patched_pages(addrs, spans)
+        row_ts = {}
+        for a, t in zip(addrs, ts if ts is not None else [0] * len(addrs)):
+            row_ts[tuple(a)] = int(t)
+        for i in sorted(pages):
+            r = self.make(rows[i], pages[i], row_ts[rows[i]])
+            self.head += r.need
+            if i in dropped_rows:
+                status[i] = DROPPED
+                self.ctr.dropped += 1
+                self._remove(self.key(rows[i]))
+            else:
+                self._install(r)                     # an old host-tier record stays in tier_log as garbage
+        if dropped_rows:
+            self.saturated = True
+        row_of = {a: i for i, a in enumerate(rows)}
+        return [status[row_of[tuple(a)]] for a in addrs]
 
     def get(self, addrs, valid, t0=None, t1=None):
         """-> list of (status, page bytes or None); books requests, hits, verification and touches."""
@@ -436,6 +509,70 @@ def gen_ops(cfg: MachineConfig, seed: int) -> list:
         lf = R.below(cfg.nl)
         ops.append(("invalidate", cfg.us[R.below(len(cfg.us))], lf, lf + w))
 
+    bs = cfg.bsize
+    absent = [(u, cfg.nl + l) for u in cfg.us for l in range(4)]     # never put
+
+    def span(shape=None, fill=None):
+        """(page offset, length, fill, seed): the ends of the page, the whole page, all but a byte, a
+        short span at any offset, or a long one."""
+        pseq[0] += 1
+        fill = fill or ("0" if R.chance(0.1) else "R")
+        shape = R.below(8) if shape is None else shape
+        if shape == 0:
+            o, n = 0, 1 + R.below(17)
+        elif shape == 1:
+            n = 1 + R.below(17)
+            o = bs - n
+        elif shape == 2:
+            o, n = 0, bs
+        elif shape == 3:
+            o, n = R.below(2), bs - 1
+        elif shape in (4, 5):
+            n = 1 + R.below(17)
+            o = R.below(bs - n + 1)
+        else:
+            n = 1 + R.below(bs // 3)
+            o = R.below(bs - n + 1)
+        return (o, n, fill, pseq[0])
+
+    def patch(rows=None, spans_per=3, shapes=None, fill=None, ts=None):
+        """One call: each row gets 1..spans_per spans, rows interleaved, and a few rows named again
+        after other rows."""
+        rows = list(rows or pick(1 + R.below(2 * cfg.batch), main + edges + absent))
+        addrs, spans = [], []
+        for a in rows:
+            for _ in range(1 + R.below(spans_per)):
+                addrs.append(a)
+                spans.append(span(None if shapes is None else shapes[R.below(len(shapes))], fill))
+        for _ in range(R.below(4)):                                  # an address again, after others
+            addrs.append(rows[R.below(len(rows))])
+            spans.append(span(4))
+        ts = (None if R.chance(0.3) else True) if ts is None else ts
+        tsv = [1 + R.below(1 << 40) for _ in addrs] if ts else None
+        ops.append(("patch", addrs, spans, tsv))
+
+    def patch_shapes():
+        """Lengths 1..17 at every page offset modulo 16, overlapping spans of one page, and the page's
+        ends, spread over hot addresses and the key-edge addresses."""
+        rows = pick(8) + edges
+        addrs, spans = [], []
+        for k in range(16):
+            for n in range(1, 18):
+                pseq[0] += 1
+                addrs.append(rows[(17 * k + n) % len(rows)])
+                spans.append((16 * R.below(bs // 16 - 2) + k, n, "R", pseq[0]))
+        a = rows[0]
+        for o, n in ((3, bs // 2), (bs // 4, bs // 2), (1, 7), (bs // 3, bs - bs // 3), (0, 1), (bs - 1, 1)):
+            pseq[0] += 1
+            addrs.append(a)
+            spans.append((o, n, "R", pseq[0]))
+        for sh in (2, 3):
+            addrs.append(rows[1])
+            spans.append(span(sh))
+        addrs += [rows[2], a]                                         # named again after other rows
+        spans += [span(4), span(4)]
+        ops.append(("patch", addrs, spans, [1 + R.below(1 << 40) for _ in addrs]))
+
     def demote(n=None):
         if cfg.tier_bytes:
             ops.append(("demote", pick(n or 1 + R.below(cfg.batch))))
@@ -447,9 +584,11 @@ def gen_ops(cfg: MachineConfig, seed: int) -> list:
     def mix(k):
         for _ in range(k):
             x = R.below(100)
-            if x < 38:
+            if x < 32:
                 put()
-            elif x < 60:
+            elif x < 42:
+                patch()
+            elif x < 61:
                 get()
             elif x < 68:
                 unset()
@@ -468,22 +607,34 @@ def gen_ops(cfg: MachineConfig, seed: int) -> list:
             else:
                 get()
 
-    # fill, then overflow the arena with incompressible pages
+    # fill; the key-edge addresses, then patches of every span shape over them and hot pages
     for at in range(0, len(main), cfg.batch):
         put(rows=main[at:at + cfg.batch])
+    put(rows=edges)
+    patch_shapes()
+    ops.append(("compact",))
     mix(cfg.steps // 6)
+    # overflow the arena with incompressible pages, and patch into the full arena
     if cfg.exact_head:
         for _ in range(3):
             put(n=cfg.batch, heavy="R")
+        patch(rows=ops[-1][1][:4] + main[:4])
     mix(cfg.steps // 6)
-    # compaction, then demotion (enough to wrap the ring), promotion
+    # compaction; random bytes over zero pages, so that their records outgrow their places; demotion of
+    # those (enough to wrap the ring), promotion, patches of host-tier records, zeros over the
+    # incompressible pages
     ops.append(("compact",))
+    zrows = main[-cfg.batch:]
+    put(rows=zrows, heavy="Z")
+    patch(rows=zrows, spans_per=1, shapes=(2,), fill="R")
     if cfg.tier_bytes:
-        demote(cfg.batch)
+        ops.append(("demote", list(zrows)))
         demote(cfg.batch)
         promote()
         ops.append(("promote", list(main)))
         demote(cfg.batch)
+        patch(rows=ops[-1][1])
+    patch(rows=zrows, spans_per=2, shapes=(2, 3), fill="0")
     mix(cfg.steps // 6)
     # purge: more tombstones than cap / 8, then an invalidation (rebuild), both invalidation paths
     purge = purge_addrs(cfg)
@@ -494,8 +645,13 @@ def gen_ops(cfg: MachineConfig, seed: int) -> list:
     ops.append(("unset", purge))
     invalidate(scan=False)
     invalidate(scan=True)
+    patch(rows=main)
     mix(cfg.steps // 6)
+    # a load into another geometry; every page patched (more rows than max_batch in config E), with
+    # its last patch's ts, then sampled
     ops.append(("load",))
+    patch(rows=main, spans_per=2, ts=True)
+    ops.append(("sample", [R.next() for _ in range(64)]))
     mix(cfg.steps // 6)
     ops.append(("compact",))
     mix(cfg.steps - 5 * (cfg.steps // 6))
@@ -515,6 +671,9 @@ def describe(op) -> str:
         return f"{k} n={len(op[1])} addrs={op[1][:4]}... invalid={op[2] and op[2].count(0)}"
     if k in ("unset", "demote", "promote"):
         return f"{k} n={len(op[1])} addrs={op[1][:6]}..."
+    if k == "patch":
+        return (f"patch n={len(op[1])} rows={len(Model.patch_rows(op[1]))} addrs={op[1][:4]}... "
+                f"spans={[s[:3] for s in op[2][:4]]}... ts={'set' if op[3] else None}")
     if k == "invalidate":
         return f"invalidate u={op[1]} l=[{op[2]}, {op[3]}]"
     if k == "sample":
@@ -538,9 +697,32 @@ def census(cfg: MachineConfig, seed: int, oracle) -> dict:
     a rebuild whose tombstones certainly pass cap / 8, a demotion that certainly retires records."""
     m = Model(cfg, oracle)
     c = Census()
-    compacted = demoted_after = False
+    compacted = demoted_after = loaded = False
     for op in gen_ops(cfg, seed):
         k = op[0]
+        if k == "patch":
+            rows = m.patch_rows(op[1])
+            st = [m.patch_status(a) for a in rows]
+            for a, s in zip(rows, st):
+                if s == HIT:
+                    c.hit("patch_host" if m.live(a).host_pos is not None else "patch_arena")
+                    if m.key(a) in KEY_SENTINELS:
+                        c.hit("patch_sentinel")
+            drops = m.patch_stand_in_drops(op[1], op[2])
+            if drops:
+                c.hit("patch_drop")
+            if len(rows) > cfg.max_batch:
+                c.hit("patch_slices")
+            if HIT in st:
+                c.hit("patch_hit" if len(drops) < st.count(HIT) else "patch_all_dropped")
+                if loaded:
+                    c.hit("patch_after_load")
+            for s, name in ((MISS, "patch_miss"), (BAD_ENTRY, "patch_bad_entry")):
+                if s in st:
+                    c.hit(name)
+            m.patch(op[1], op[2], op[3], drops)
+            continue
+        loaded = False
         if k in ("put", "put_async"):
             pages = pages_of(cfg, op[2])
             drops = m.stand_in_drops(op[1], pages, op[4])
@@ -575,4 +757,5 @@ def census(cfg: MachineConfig, seed: int, oracle) -> dict:
         elif k == "load":
             c.hit("load")
             m.load(cfg.load_slots, cfg.load_arena)
+            loaded = True
     return c.events

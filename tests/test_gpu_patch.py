@@ -303,17 +303,41 @@ print("no mixed pages")
 
 
 DROP_IN = textwrap.dedent("""
-    import os, sys, threading
+    import os, pickle, shutil, sys, threading, time
     sys.path.insert(0, sys.argv[1])
     import numpy as np
     import edge_fuse_b200 as E
-    d = sys.argv[2]
-    ps = 12
-    P = 1 << ps
-    N = 48                                                # pages per object
-    cm = E.Cachemap(d, 1 << 16, 12, ps)
-    rng = np.random.default_rng(int(sys.argv[3]))
+    d, seed, ps, N, mode, phase = sys.argv[2], int(sys.argv[3]), int(sys.argv[4]), int(sys.argv[5]), sys.argv[6], sys.argv[7]
+    P = 1 << ps                                           # N pages per object
     objs = (3, 4, 5)
+    fails = []
+
+    def check(what, cond):
+        if not cond:
+            fails.append(what)
+
+    if phase == "read":                                   # a second process opens what the first one left
+        with open(d + ".model", "rb") as f:
+            model, cached = pickle.load(f)
+        cm = E.Cachemap(d, 1 << 16, 12, ps)
+        assert cm.ok
+        for o in objs:
+            for p in range(N):
+                g = cm.get(p * P, o, 0)
+                check(("restart get", o, p), (g is not None) == (p in cached[o]))
+                check(("restart stale", o, p), g is None or g == bytes(model[o][p * P:(p + 1) * P]))
+        cm.free()
+        print("fails", len(fails), fails[:5])
+        sys.exit(0)
+
+    # exact: every page the model caches hits and no other does; evict: the capacity is below the
+    # working set, so only "never stale" holds, and pread returns bytes exactly when every page of its
+    # range hits; stale: the flusher drops pages in the background, so only "never stale" holds;
+    # restart: exact, then the directory is copied as a crash leaves it for the read phase
+    exact = mode in ("exact", "restart")
+    cm = E.Cachemap(d, 1024 if mode == "evict" else 1 << 16, 12, ps)
+    assert cm.ok
+    rng = np.random.default_rng(seed)
     model = {o: bytearray(rng.integers(0, 256, N * P, dtype=np.uint8).tobytes()) for o in objs}
     cached = {o: set() for o in objs}
     for o in objs:                                        # most pages cached whole, a few not
@@ -321,11 +345,6 @@ DROP_IN = textwrap.dedent("""
             if rng.random() < 0.8:
                 cm.write_range(o, 0, p * P, bytes(model[o][p * P:(p + 1) * P]))
                 cached[o].add(p)
-    fails = []
-
-    def check(what, cond):
-        if not cond:
-            fails.append(what)
 
     def want_read(o, off, size):
         pages = range(off // P, (off + size - 1) // P + 1) if size else []
@@ -348,36 +367,74 @@ DROP_IN = textwrap.dedent("""
             p = int(rng.integers(0, N - 4)); return p * P, int(rng.integers(1, 5)) * P
         a = int(rng.integers(1, N * P - 3)); return a, int(rng.integers(1, min(3 * P, N * P - a)))
 
+    def pwrite(o, off, size):
+        data = rng.integers(0, 256, size, dtype=np.uint8).tobytes()
+        cm.pwrite(o, 0, off, data)
+        model[o][off:off + size] = data
+        first, last = off // P, (off + size - 1) // P
+        for p in range(first, last + 1):
+            if p * P >= off and (p + 1) * P <= off + size:
+                cached[o].add(p)                          # covered whole: put
+
+    def sweep():                                          # every page: hit with the model's bytes, or miss
+        for oo in objs:
+            for p in range(N):
+                g = cm.get(p * P, oo, 0)
+                check(("get", oo, p, g is not None), not exact or (g is not None) == (p in cached[oo]))
+                check(("stale", oo, p), g is None or g == bytes(model[oo][p * P:(p + 1) * P]))
+
     for step in range(400):
         o = objs[int(rng.integers(0, len(objs)))]
         off, size = rand_range()
         if rng.random() < 0.5:
-            data = rng.integers(0, 256, size, dtype=np.uint8).tobytes()
-            cm.pwrite(o, 0, off, data)
-            model[o][off:off + size] = data
-            first, last = off // P, (off + size - 1) // P
-            for p in range(first, last + 1):
-                if p * P >= off and (p + 1) * P <= off + size:
-                    cached[o].add(p)                      # covered whole: put
+            pwrite(o, off, size)
         else:
             r0 = cm.counters()
             got = cm.pread(o, 0, off, size)
             r1 = cm.counters()
-            ok, rq, ht = want_read(o, off, size)
-            check(("pread", o, off, size, ok, got is not None), (got is not None) == ok)
             check(("bytes", o, off, size), got is None or got == bytes(model[o][off:off + size]))
-            check(("counters", o, off, size), (r1[0] - r0[0], r1[1] - r0[1]) == (rq, ht))
-            if off % P == 0 and size % P == 0:            # aligned: exactly read_range
+            if exact:
+                ok, rq, ht = want_read(o, off, size)
+                check(("pread", o, off, size, ok, got is not None), (got is not None) == ok)
+                check(("counters", o, off, size), (r1[0] - r0[0], r1[1] - r0[1]) == (rq, ht))
+            elif mode == "evict":                         # bytes exactly when every page of the range hits now
+                every = all(cm.get(p * P, o, 0) is not None for p in range(off // P, (off + size - 1) // P + 1))
+                check(("pread", o, off, size, every, got is not None), (got is not None) == every)
+            if off % P == 0 and size % P == 0 and exact:  # aligned: exactly read_range
                 r2 = cm.counters()
                 alt = cm.read_range(o, 0, off, size)
                 r3 = cm.counters()
                 check(("aligned", o, off, size), alt == got and (r3[0] - r2[0], r3[1] - r2[1]) == (rq, ht))
-        if step % 50 == 49:                               # every page: hit with the model's bytes, or miss
-            for oo in objs:
-                for p in range(N):
-                    g = cm.get(p * P, oo, 0)
-                    check(("get", oo, p), (g is not None) == (p in cached[oo]))
-                    check(("stale", oo, p), g is None or g == bytes(model[oo][p * P:(p + 1) * P]))
+        if step % 50 == 49:
+            sweep()
+
+    if mode == "restart":
+        # the write-behind ring drains (engine_handles waits for it) and a base is written, so that the
+        # next tick writes a delta; then unaligned writes over cached pages, whose edge pages are patched
+        # by the engine, and the store left until that tick has written them
+        cm.engine_handles()
+        check("a base written", cm.checkpoint() == 0)
+        for k in range(12):
+            o = objs[k % 3]
+            p = sorted(cached[o])[(7 * k) % len(cached[o])]
+            pwrite(o, p * P + 1 + k, P - 2 - k)
+            if p + 1 < N:
+                pwrite(o, p * P + P // 2, P)              # the end of p and the start of p + 1
+        sweep()
+        names = lambda: sorted((f, os.stat(os.path.join(d, f)).st_mtime_ns) for f in os.listdir(d))
+        seen, quiet, t0 = names(), time.time(), time.time()
+        while time.time() - quiet < 3.5 and time.time() - t0 < 60:      # no tick for more than 3 ticks
+            time.sleep(0.1)
+            now = names()
+            if now != seen:
+                seen, quiet = now, time.time()
+        copy = d + ".copy"
+        shutil.copytree(d, copy)                          # the directory as a crash leaves it
+        with open(copy + ".model", "wb") as f:
+            pickle.dump((model, cached), f)
+        print("files", " ".join(f for f, _ in seen), flush=True)
+        print("fails", len(fails), fails[:5], flush=True)
+        os._exit(0)
 
     # 16 threads write disjoint bytes of one cached page: every write lands
     cm.write_range(9, 0, 0, bytes(P))
@@ -393,17 +450,43 @@ DROP_IN = textwrap.dedent("""
     [t.start() for t in th]
     [t.join() for t in th]
     page = cm.pread(9, 0, 0, P)
-    check("threads page", page is not None)
+    check("threads page", page is not None or not exact)
     for t in range(16):
-        check(("thread", t), page is not None and page[7 + 40 * t:47 + 40 * t] == last[t])
+        check(("thread", t), page is None or page[7 + 40 * t:47 + 40 * t] == last[t])
     cm.free()
     print("fails", len(fails), fails[:5])
 """)
 
+# (environment, page shift, pages per object, mode); every case drives the byte model above
+DROP_IN_CASES = {
+    "ring": ({}, 12, 48, "exact"),
+    "no_ring": ({"CMB200_WB_SLOTS": "0"}, 12, 48, "exact"),
+    "two_engines": ({"CMB200_DEVICES": "0,0"}, 12, 48, "exact"),
+    # 128 KiB pages: pread's edge pages decode in the fused pair kernel
+    "pshift17": ({}, 17, 48, "exact"),
+    # 1 MiB pages: no fused get, and records that leave the arena check no margin
+    "pshift20": ({}, 20, 12, "exact"),
+    # 3 MiB of incompressible pages over a 1 MiB arena: writes demote, reads promote, and pwrite
+    # patches host-tier records after filemap_check_arena has made room.  A ring of 64 slots flushes
+    # batches that demotion always makes room for
+    "host_tier": ({"CMB200_ARENA_MB": "1", "CMB200_HOST_TIER_MB": "64", "CMB200_TIER_PROMOTE": "1",
+                   "CMB200_WB_SLOTS": "64"}, 12, 256, "exact"),
+    # the default ring flushes batches larger than the whole arena: pages are dropped, never stale
+    "host_tier_full_batches": ({"CMB200_ARENA_MB": "1", "CMB200_HOST_TIER_MB": "64", "CMB200_TIER_PROMOTE": "1"},
+                               12, 256, "stale"),
+    "verify_evict_access": ({"CMB200_VERIFY": "1", "CMB200_EVICT": "access"}, 12, 48, "exact"),
+    # 1 024 pages (the least capacity a map accepts) for 3 x 512: eviction runs; synchronous puts, so
+    # that nothing evicts between a pread and the gets that check it
+    "evict": ({"CMB200_WB_SLOTS": "0"}, 12, 512, "evict"),
+    "evict_access": ({"CMB200_WB_SLOTS": "0", "CMB200_EVICT": "access"}, 14, 512, "evict"),
+    "restart": ({"CMB200_PERSIST": "1", "CMB200_CHECKPOINT_SEC": "1", "CMB200_CHECKPOINT_DELTAS": "64"}, 12, 48,
+                "restart"),
+}
 
-@pytest.mark.parametrize("env", [{}, {"CMB200_WB_SLOTS": "0"}, {"CMB200_DEVICES": "0,0"}],
-                         ids=["ring", "no_ring", "two_engines"])
-def test_drop_in_pread_pwrite_match_a_model(E, gpu, tmp_path, env):
+
+@pytest.mark.parametrize("case", list(DROP_IN_CASES))
+def test_drop_in_pread_pwrite_match_a_model(E, gpu, tmp_path, case):
+    env, ps, n, mode = DROP_IN_CASES[case]
     script = tmp_path / "drive.py"
     script.write_text(DROP_IN)
     base = dict(os.environ, CMB200_PERSIST="0", CMB200_ARENA_MB="256")
@@ -413,6 +496,11 @@ def test_drop_in_pread_pwrite_match_a_model(E, gpu, tmp_path, env):
     base.update(env)
     d = tmp_path / "cache"
     d.mkdir()
-    r = subprocess.run([sys.executable, str(script), ROOT, str(d), "17"], capture_output=True, text=True,
-                       timeout=600, env=base)
+    args = [sys.executable, str(script), ROOT, str(d), "17", str(ps), str(n), mode]
+    r = subprocess.run(args + ["run"], capture_output=True, text=True, timeout=600, env=base)
     assert r.returncode == 0 and "fails 0 []" in r.stdout, r.stdout + r.stderr[-3000:]
+    if mode == "restart":
+        assert ".d1" in r.stdout.split("files", 1)[1], r.stdout      # the tick wrote a delta
+        args[3] = str(d) + ".copy"
+        r = subprocess.run(args + ["read"], capture_output=True, text=True, timeout=600, env=base)
+        assert r.returncode == 0 and "fails 0 []" in r.stdout, r.stdout + r.stderr[-3000:]

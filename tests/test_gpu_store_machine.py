@@ -1,8 +1,9 @@
-"""One engine driven through long seeded interleavings of every engine operation, compared after every
-step with the model of tests/store_machine.py: entries, every record byte, fingerprints, parse
-checkpoints, get answers on both get paths, arena and host-tier accounting, verification counters,
-sampled addresses and timestamps, and the request counters.  A failure names its configuration, seed
-and step and prints the log of the operations that led there."""
+"""One engine driven through long seeded interleavings of every engine operation, patches included,
+compared after every step with the model of tests/store_machine.py: entries, every record byte,
+fingerprints, parse checkpoints, get answers on both get paths, patch statuses and drops, arena and
+host-tier accounting, verification counters, sampled addresses and timestamps, and the request
+counters.  A failure names its configuration, seed and step and prints the log of the operations that
+led there."""
 import ctypes as C
 import time
 
@@ -108,6 +109,35 @@ class Machine:
         out, status = self.eng.get_small(u, l)
         t1 = time.clock_gettime_ns(time.CLOCK_REALTIME)
         self._get(addrs, out, status, None, t0, t1)
+
+    def op_patch(self, op, step):
+        _, addrs, spans, ts = op
+        m, eng = self.m, self.eng
+        u, l = _addr(addrs)
+        must_drop = self.cfg.exact_head and bool(m.patch_stand_in_drops(addrs, spans))
+        chunks = eng.stats()["put_chunks"]
+        if self.cfg.tier_bytes:
+            eng.tier_hot()                                   # drained: the patch must add nothing
+            hits = eng.host_tier_stats()["hits"]
+        status = eng.patch(u, l, [s[0] for s in spans], [SM.span_bytes(s) for s in spans],
+                           ts=None if ts is None else np.array(ts, dtype=np.uint64))
+        rows = m.patch_rows(addrs)
+        first = {}
+        for i, a in enumerate(addrs):
+            first.setdefault(tuple(a), i)
+        dropped = {r for r, a in enumerate(rows) if status[first[a]] == SM.DROPPED}
+        want = m.patch(addrs, spans, ts, dropped)
+        for i, a in enumerate(addrs):
+            assert status[i] == want[i], f"patch {i} {a}: status {status[i]}, model {want[i]}"
+        if self.cfg.exact_head:
+            assert bool(dropped) == must_drop, f"dropped rows {sorted(dropped)}; the arena certainly overflows: {must_drop}"
+        stored = sum(1 for a in rows if status[first[a]] == SM.HIT)
+        got = eng.stats()["put_chunks"] - chunks
+        assert got == stored, f"put_chunks grew by {got}, stored rows {stored}"
+        if self.cfg.tier_bytes:
+            assert eng.host_tier_stats()["hits"] == hits, "a patch counted host-tier hits"
+            hu, _, lost = eng.tier_hot()
+            assert len(hu) == 0 and lost == 0, f"a patch logged {len(hu)} host-tier reads ({lost} lost)"
 
     def op_unset(self, op, step):
         self.eng.unset(*_addr(op[1]))

@@ -31,7 +31,8 @@ def exe(tmp_path_factory):
 
 def _drive(exe, d, *args, **env_extra):
     env = dict(os.environ, CMB200_PERSIST="1", CMB200_WB_SLOTS="64",
-               TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0", **env_extra)
+               TSAN_OPTIONS="halt_on_error=0 report_signal_unsafe=0")
+    env.update(env_extra)
     for k in ("CMB200_DEVICES", "CMB200_DEVICE", "CMB200_HOST_TIER_MB", "CMB200_TIER_PROMOTE",
               "CMB200_CHECKPOINT_SEC", "CMB200_CHECKPOINT_DELTAS"):
         if k not in env_extra:
@@ -144,6 +145,17 @@ def test_without_the_engine_call_partial_pages_are_dropped(tmp_path):
     head, _patches, _log, out = _drive(exe, tmp_path / "c", "fallback")
     # pages 2 and 4 are written in part: dropped, never served stale; page 3 is put whole
     assert "fallback 0 1 0 cached 14 wrong 0" in head, out.stdout
+
+
+@pytest.mark.parametrize("wb_slots", ["64", "0"])
+def test_a_dropped_put_leaves_no_old_page(exe, tmp_path, wb_slots):
+    """A put the store drops for lack of arena room (the engine keeps the key's old record) removes the
+    key: the old page would be stale.  In one flush batch only a key's newest page decides: a drop
+    followed by a stored put of the key keeps it."""
+    head, _patches, _log, out = _drive(exe, tmp_path / "c", "dropped", CMB200_WB_SLOTS=wb_slots)
+    assert "dropped 14 0" in head, out.stdout             # pages 2 and 3 miss, no page is stale
+    if wb_slots != "0":
+        assert "batch 1 13 0" in head, out.stdout         # page 4 holds its last put, page 5 misses
 
 
 @pytest.mark.parametrize("threads", [4, 16])
