@@ -22,7 +22,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_print_stats", "cachemap_put_batch", "cachemap_get_batch", "cachemap_put_batch_dev",
     "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
-    "cachemap_pread", "cachemap_pwrite",
+    "cachemap_pread", "cachemap_pwrite", "cachemap_rename",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -43,6 +43,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
     "cmb200_verify_stats", "cmb200_verify_store", "cmb200_snapshot_begin", "cmb200_snapshot_finish",
     "cmb200_chain_begin", "cmb200_load_chain", "cmb200_invalidate", "cmb200_patch_batch",
+    "cmb200_rename", "cmb200_rename_set",
 ]
 
 
@@ -103,6 +104,7 @@ def lib() -> C.CDLL:
         "cachemap_engines": (i32, [vp, vp, i32]),
         "cachemap_checkpoint": (i32, [vp]),
         "cachemap_invalidate": (u64, [vp, u64, u32, u64, u64]),
+        "cachemap_rename": (u64, [vp, u64, u64, u32]),
         "cachemap_read_range": (i32, [vp, u64, u32, u64, sz, vp]),
         "cachemap_write_range": (None, [vp, u64, u32, u64, sz, vp]),
         "cachemap_pread": (i32, [vp, u64, u32, u64, sz, vp]),
@@ -139,6 +141,8 @@ def lib() -> C.CDLL:
         "cmb200_get_batch_dev": (i32, [vp, sz, vp, vp, vp, vp]),
         "cmb200_unset_batch": (i32, [vp, sz, vp]),
         "cmb200_invalidate": (i32, [vp, u64, u64, u64, vp]),
+        "cmb200_rename": (i32, [vp, u64, u64, u64, u64, vp, vp]),
+        "cmb200_rename_set": (i32, [vp, i32, u64, u64, u64, u64, vp, vp]),
         "cmb200_patch_batch": (i32, [vp, sz, vp, vp, vp, vp, vp, vp]),
         "cmb200_entries": (u64, [vp]),
         "cmb200_sample": (i32, [vp, sz, vp, vp, vp, vp]),
@@ -503,6 +507,14 @@ class Engine:
         _check(lib().cmb200_invalidate(self.h, u, l_first, l_last, C.byref(removed)), "cmb200_invalidate")
         return removed.value
 
+    def rename(self, u_from: int, u_to: int, l_first: int, l_last: int):
+        """Moves every live record stored at {u_from, l}, l_first <= l <= l_last, to {u_to, l}
+        -> (records moved, records dropped for lack of arena room)."""
+        moved, dropped = C.c_uint64(), C.c_uint64()
+        _check(lib().cmb200_rename(self.h, u_from, u_to, l_first, l_last, C.byref(moved), C.byref(dropped)),
+               "cmb200_rename")
+        return moved.value, dropped.value
+
     def patch(self, u, l, page_off, data, ts=None):
         """cmb200_patch_batch: patch i writes data[i] (bytes) at byte page_off[i] of the page stored at
         {u[i], l[i]}, in array order -> status per patch (HIT, MISS, BAD_ENTRY, BAD_DECODE, CORRUPT, DROPPED)."""
@@ -646,6 +658,15 @@ def save_set(handles, path: str) -> int:
     return n.value
 
 
+def rename_set(handles, u_from: int, u_to: int, l_first: int, l_last: int):
+    """cmb200_rename_set over engine handles that split the keys by cmb200_owner -> (moved, dropped)."""
+    arr, g = _handles(handles)
+    moved, dropped = C.c_uint64(), C.c_uint64()
+    _check(lib().cmb200_rename_set(arr, g, u_from, u_to, l_first, l_last, C.byref(moved), C.byref(dropped)),
+           "cmb200_rename_set")
+    return moved.value, dropped.value
+
+
 def snapshot_begin(handles, path: str) -> int:
     """cmb200_snapshot_begin over engine handles -> snapshot handle.  The engines' live records are
     listed now and written by a thread of the snapshot while the engines keep serving."""
@@ -774,6 +795,11 @@ class Cachemap:
         """Drops the cached pages of (nhid, genid) overlapping bytes [off, off + size) -> pages removed;
         size = Cachemap.TO_END drops every page from off on."""
         return int(lib().cachemap_invalidate(self.h, nhid, genid, off, size))
+
+    def rename(self, nhid_from: int, nhid_to: int, genid: int) -> int:
+        """edgefs_rename: the cached pages of (nhid_to, genid) are dropped and those of (nhid_from, genid)
+        move to nhid_to -> pages moved."""
+        return int(lib().cachemap_rename(self.h, nhid_from, nhid_to, genid))
 
     def counters(self):
         rq, ht = C.c_uint64(), C.c_uint64()

@@ -67,6 +67,7 @@ extern int cmb200_owner(uint64_t key, int g);
 #pragma weak cmb200_dev_alloc
 #pragma weak cmb200_dev_free
 #pragma weak cmb200_invalidate
+#pragma weak cmb200_rename_set
 #pragma weak cmb200_patch_batch
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
@@ -2333,6 +2334,57 @@ cachemap_invalidate(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 	/* a removal is a change of the store: the next checkpoint must write it */
 	__atomic_fetch_add(&fm->puts_seen, removed, __ATOMIC_RELAXED);
 	return removed;
+}
+
+/* Every page of (nhid_small, genid) leaves every engine.  Returns the pages removed. */
+static uint64_t
+filemap_invalidate_all(struct filemap *fm, uint64_t nhid_small, uint32_t genid)
+{
+	const uint64_t first = (uint64_t)genid << PNUM_SHIFT, last = first | ((1ULL << PNUM_SHIFT) - 1);
+	uint64_t removed = 0;
+	for (int i = 0; i < fm->g; i++) {
+		uint64_t r = 0;
+		if (cmb200_invalidate && cmb200_invalidate(fm->dev[i]->eng, nhid_small, first, last, &r) == 0)
+			removed += r;
+		else
+			fprintf(stderr, "cachemap_b200: cachemap_rename: %s\n",
+			    cmb200_invalidate ? cmb200_last_error() : "the engine cannot invalidate");
+	}
+	return removed;
+}
+
+uint64_t
+cachemap_rename(struct cachemap *cm, uint64_t nhid_from, uint64_t nhid_to, uint32_t genid)
+{
+	struct filemap *fm = cm->pages;
+	if (nhid_from == nhid_to)
+		return 0;
+	/* a call before the first get applies to the loaded snapshot, not before it */
+	if (!filemap_engine_ready(fm))
+		return 0;
+	filemap_drain(fm);                      /* every page accepted before the call is in a store */
+	/* the old pages of `to` go first: the move replaces only the pages `from` has */
+	uint64_t removed = filemap_invalidate_all(fm, nhid_to, genid);
+	const uint64_t first = (uint64_t)genid << PNUM_SHIFT, last = first | ((1ULL << PNUM_SHIFT) - 1);
+	uint64_t moved = 0, dropped = 0;
+	int rc = -1;
+	if (cmb200_rename_set) {
+		/* every engine's room lock, in index order, so that no flusher's room-making is eaten by the
+		 * moved records; the engine call takes each engine's own lock in turn */
+		for (int i = 0; i < fm->g; i++)
+			pthread_mutex_lock(&fm->dev[i]->room_mu);
+		rc = cmb200_rename_set(fm->engs, fm->g, nhid_from, nhid_to, first, last, &moved, &dropped);
+		for (int i = fm->g - 1; i >= 0; i--)
+			pthread_mutex_unlock(&fm->dev[i]->room_mu);
+		if (rc != 0)
+			fprintf(stderr, "cachemap_b200: cachemap_rename: %s\n", cmb200_last_error());
+	}
+	/* without the move, what is left of `from` must not be served under its old name either */
+	if (rc != 0)
+		removed += filemap_invalidate_all(fm, nhid_from, genid);
+	/* moves and removals are changes of the store: the next checkpoint must write them */
+	__atomic_fetch_add(&fm->puts_seen, moved + dropped + removed, __ATOMIC_RELAXED);
+	return moved;
 }
 
 int

@@ -220,6 +220,9 @@ struct cmb200_engine {
 	DevMem<uint32_t> d_import_slot;      // slot scratch of cmb200_import_records_dev, grown, never shrunk
 	DevMem<uint32_t> d_move_idx;         // index scratch of cmb200_move_pages (destination, then source), grown, never shrunk
 	DevMem<unsigned long long> d_removed; // records removed by cmb200_invalidate, allocated by its first call
+	// cmb200_rename: a slice's list and staged records, on the engine they leave and on the one they enter,
+	// grown, never shrunk (rename_mu: one rename call at a time uses them)
+	DevMem<uint8_t> d_ren_list, d_ren_bytes;
 	// cmb200_patch_batch: the call's rows, spans and bytes, staged page-locked and copied over in one piece,
 	// grown, never shrunk; and the tier-hit counter and hot log its decode books into instead of the gets'
 	HostMem<uint8_t> h_patch;
@@ -1520,6 +1523,25 @@ struct LoadBatch {
 	}
 };
 
+// The device half of a load and of a rename: m records {24-byte prefix, payload} at blob + off[i] (device
+// memory of e, 16-byte aligned) are stored at addr[i] with ts[i] and fingerprint fps[i] ({0, 0} or
+// fps = nullptr: none), as if put in this order: k_upsert claims the keys and raises seq, k_restore writes
+// each record under its new prefix and rebuilds its parse checkpoints.  A record the arena has no room
+// for is dropped, as a put is.  Enqueued on e->st.  (e->mu held; m <= max_batch)
+static int restore_records(cmb200_engine *e, const uint8_t *blob, const unsigned long long *addr,
+    const unsigned long long *ts, const unsigned long long *off, const uint64_t *fps, size_t m) {
+	if (launch_upsert(e->table, addr, nullptr, (uint32_t)m, e->seq, e->seq_stride, e->d_slot, e->st)) return -1;
+	EncodeJob job{};
+	job.n = (uint32_t)m; job.nbytes = e->bsize;
+	job.slot_idx = e->d_slot; job.addr = addr; job.ts = ts;
+	job.seq0 = e->seq; job.seq_stride = e->seq_stride;
+	job.table = e->table; job.arena = e->arena;
+	if (launch_restore(job, blob, off, fps, e->bsize, e->st)) return -1;
+	e->seq += (unsigned long long)m * e->seq_stride;
+	e->stats.kernel_launches += 2;
+	return 0;
+}
+
 // Puts the staged records into their engine as if they had been put in file order.  Returns how many
 // (>= 0) or -1.
 static long long load_flush(LoadBatch &b, bool with_fp) {
@@ -1538,16 +1560,8 @@ static long long load_flush(LoadBatch &b, bool with_fp) {
 	CMB_CHECK(cudaMemcpyAsync(e->d_ts, b.ts.data(), m * 8, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(b.d_off, b.off.data(), m * 8, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(b.d_fp, b.fps.data(), m * 16, cudaMemcpyHostToDevice, e->st));
-	if (launch_upsert(e->table, e->d_addr, nullptr, (uint32_t)m, e->seq, e->seq_stride, e->d_slot, e->st)) return -1;
-	EncodeJob job{};
-	job.n = (uint32_t)m; job.nbytes = e->bsize;
-	job.slot_idx = e->d_slot; job.addr = e->d_addr; job.ts = e->d_ts;
-	job.seq0 = e->seq; job.seq_stride = e->seq_stride;
-	job.table = e->table; job.arena = e->arena;
-	if (launch_restore(job, e->d_pages[0], b.d_off, with_fp ? (uint64_t *)b.d_fp : nullptr, e->bsize, e->st)) return -1;
+	if (restore_records(e, e->d_pages[0], e->d_addr, e->d_ts, b.d_off, with_fp ? (uint64_t *)b.d_fp : nullptr, m)) return -1;
 	CMB_CHECK(cudaStreamSynchronize(e->st));
-	e->seq += (unsigned long long)m * e->seq_stride;
-	e->stats.kernel_launches += 2;
 	b.m = 0; b.used = 0;
 	return (long long)m;
 }
@@ -2063,6 +2077,171 @@ static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out) {
 extern "C" int cmb200_compact(cmb200_engine *e, uint64_t *reclaimed_out) {
 	std::lock_guard<std::mutex> g(e->mu);
 	return compact_locked(e, reclaimed_out);
+}
+
+// ---- rename: an object's records move to another object's addresses ----------------------------
+// A record's prefix names its address and k_get_small trusts that prefix, so a record cannot be aliased
+// under a new key: it is copied under the new prefix and the old one is retired.  The LZ4 block does not
+// depend on the address, so nothing is encoded again.  The work goes in slices that are bounded as a
+// load's batches are (<= min(max_batch, META_CAP) records, one page-ring buffer of bytes plus one
+// record), per pair (source engine, destination engine):
+//   1. under the source's lock: k_rename_select lists the records whose new key the destination owns,
+//      k_rename_gather copies them to the source's staging buffer and retires their slots;
+//   2. the slice crosses to the destination (a peer copy, or none when both are one engine);
+//   3. under the destination's lock: a compaction if the slice does not fit above the bump pointer and
+//      garbage covers the shortfall, then restore_records, as a load stores its records.
+// No list of arena offsets outlives step 1, so a compaction in step 3 moves nothing a later step reads.
+// One call at a time uses the staging buffers; the call never holds two engine locks at once.
+static std::mutex rename_mu;
+
+// The list of a slice inside an engine's d_ren_list, for n entries: cursor (4 words), addr, ts, off, fp
+// (the part a destination reads, contiguous), then loc, slot, len.
+static size_t rename_list_bytes(size_t n) { return 32 + n * 64; }
+static size_t rename_list_head(size_t n) { return 32 + n * 48; }
+static RenameList rename_list_view(uint8_t *base, size_t n, unsigned long long max_bytes) {
+	RenameList r{};
+	r.cursor = (unsigned long long *)base;
+	r.addr = (unsigned long long *)(base + 32);
+	r.ts = r.addr + 2 * n;
+	r.off = r.ts + n;
+	r.fp = (uint64_t *)(r.off + n);
+	r.loc = (unsigned long long *)(r.fp + 2 * n);
+	r.slot = (uint32_t *)(r.loc + n);
+	r.len = r.slot + n;
+	r.max_n = (uint32_t)n;
+	r.max_bytes = max_bytes;
+	return r;
+}
+
+// Step 3 on engine e, whose d_ren_list / d_ren_bytes hold the slice (m records, `bytes` staged).
+// (e->mu held)
+static int rename_store(cmb200_engine *e, size_t n, size_t m, unsigned long long bytes, uint64_t *moved,
+    uint64_t *dropped) {
+	unsigned long long c[8];
+	if (read_counters(e, c)) return -1;
+	// room: compact once if the garbage covers what the slice needs beyond the bump pointer (with per-warp
+	// arena segments the unused ends of segments come back too, and are not counted as garbage); never
+	// evict or demote here, so whatever still does not fit is dropped by k_restore
+	if (c[2] + bytes > e->arena.size && (c[3] >= c[2] + bytes - e->arena.size || e->arena.seg_bytes != 0)) {
+		if (compact_locked(e, nullptr)) return -1;
+		if (read_counters(e, c)) return -1;
+	}
+	const unsigned long long dropped_before = c[4];
+	const RenameList r = rename_list_view(e->d_ren_list, n, 0);
+	if (restore_records(e, e->d_ren_bytes, r.addr, r.ts, r.off, r.fp, m)) return -1;
+	if (read_counters(e, c)) return -1;
+	const uint64_t lost = c[4] - dropped_before;
+	*moved += m - lost;
+	*dropped += lost;
+	return 0;
+}
+
+// One slice from engine s to engine d (index di of g).  Returns the records taken (0: none left), -1.
+// An engine that has made a multi-GPU call holds other ranks' records in its index.  (e->mu held)
+static bool rename_refused(cmb200_engine *e) {
+	if (!e->multi_gpu) return false;
+	set_error_msg("cmb200_rename: not available after a multi-GPU call (the index holds other ranks' records)");
+	return true;
+}
+
+static long long rename_slice(cmb200_engine *s, cmb200_engine *d, int g, int di, uint64_t u_from, uint64_t u_to,
+    uint64_t l_first, uint64_t l_last, size_t n, unsigned long long max_bytes, uint64_t *moved, uint64_t *dropped) {
+	size_t m;
+	unsigned long long bytes;
+	{
+		std::unique_lock<std::mutex> lk(s->mu);
+		if (rename_refused(s)) return -1;
+		CMB_CHECK(cudaSetDevice(s->device));
+		if (s->d_ren_list.grow(rename_list_bytes(n), s->st)) return -1;
+		const RenameList r = rename_list_view(s->d_ren_list, n, max_bytes);
+		CMB_CHECK(cudaMemsetAsync(r.cursor, 0, 8, s->st));
+		// l_last - l_first + 1 overflows for the full interval: compare the difference instead
+		const bool scan = l_last - l_first >= invalidate_keyed_max(s->table.cap);
+		if (launch_rename_select(s->table, r, u_from, u_to, l_first, l_last, scan, g, di, s->bsize, s->st)) return -1;
+		unsigned long long cur[3] = {};
+		CMB_CHECK(cudaMemcpyAsync(cur, r.cursor, sizeof(cur), cudaMemcpyDeviceToHost, s->st));
+		CMB_CHECK(cudaStreamSynchronize(s->st));
+		s->stats.kernel_launches += 2;
+		if (cur[0] == 0) return 0;                           // nothing left to move to engine di
+		m = (size_t)cur[1];
+		bytes = cur[2];
+		// grown to the largest slice so far, never past one page-ring buffer plus one record
+		if (s->d_ren_bytes.grow(bytes, s->st)) return -1;
+		if (launch_rename_gather(s->table, s->arena, s->tier.dev, r, (uint32_t)m, s->d_ren_bytes, s->st)) return -1;
+		s->stats.kernel_launches++;
+		if (s == d) {
+			if (rename_store(s, n, m, bytes, moved, dropped)) return -1;
+		} else {
+			CMB_CHECK(cudaStreamSynchronize(s->st));
+		}
+		// the retired slots are tombstones: rebuild the table when they have eaten its empty slots
+		unsigned long long c[8];
+		if (read_counters(s, c)) return -1;
+		if (c[1] > s->table.cap / 8) {
+			cmb200_engine::GateClosed gg(s->get_gate);
+			if (rebuild_table_locked(s, c[1])) return -1;
+		}
+		if (s == d) return (long long)m;
+	}
+	std::lock_guard<std::mutex> lk(d->mu);
+	// the slice is out of the source already: a refusal here loses it, as a drop would, and never serves it stale
+	if (rename_refused(d)) return -1;
+	CMB_CHECK(cudaSetDevice(d->device));
+	if (d->d_ren_list.grow(rename_list_bytes(n), d->st) || d->d_ren_bytes.grow(bytes, d->st)) return -1;
+	// the list's cursor, addr, ts, off and fp, then the staged records
+	const size_t head = rename_list_head(n);
+	if (s->device == d->device) {
+		CMB_CHECK(cudaMemcpyAsync(d->d_ren_list, s->d_ren_list, head, cudaMemcpyDeviceToDevice, d->st));
+		CMB_CHECK(cudaMemcpyAsync(d->d_ren_bytes, s->d_ren_bytes, bytes, cudaMemcpyDeviceToDevice, d->st));
+	} else {
+		CMB_CHECK(cudaMemcpyPeerAsync(d->d_ren_list, d->device, s->d_ren_list, s->device, head, d->st));
+		CMB_CHECK(cudaMemcpyPeerAsync(d->d_ren_bytes, d->device, s->d_ren_bytes, s->device, bytes, d->st));
+	}
+	if (rename_store(d, n, m, bytes, moved, dropped)) return -1;
+	return (long long)m;
+}
+
+extern "C" int cmb200_rename_set(cmb200_engine *const *engines, int g, uint64_t u_from, uint64_t u_to,
+    uint64_t l_first, uint64_t l_last, uint64_t *moved_out, uint64_t *dropped_out) {
+	if (moved_out) *moved_out = 0;
+	if (dropped_out) *dropped_out = 0;
+	if (!engines || g < 1) { set_error_msg("cmb200_rename_set: no engines"); return -1; }
+	if (l_first > l_last) { set_error_msg("cmb200_rename: l_first > l_last"); return -1; }
+	for (int i = 0; i < g; i++) {
+		if (engines[i]->pshift != engines[0]->pshift) { set_error_msg("cmb200_rename_set: engines of different page sizes"); return -1; }
+		// under each engine's lock in turn, as cmb200_invalidate reads the flag; rename_slice reads it
+		// again under the lock it works under
+		std::lock_guard<std::mutex> lk(engines[i]->mu);
+		if (rename_refused(engines[i])) return -1;
+	}
+	if (u_from == u_to) return 0;
+	std::lock_guard<std::mutex> call(rename_mu);
+	// slice bounds common to every engine of the call, as a load's batches are bounded
+	size_t n = cmb200_engine::META_CAP;
+	unsigned long long max_bytes = ~0ull;
+	for (int i = 0; i < g; i++) {
+		if (engines[i]->max_batch < n) n = engines[i]->max_batch;
+		const unsigned long long ring = (unsigned long long)engines[i]->host_batch * engines[i]->bsize;
+		if (ring < max_bytes) max_bytes = ring;
+	}
+	uint64_t moved = 0, dropped = 0;
+	int rc = 0;
+	for (int si = 0; si < g && rc == 0; si++)
+		for (int di = 0; di < g && rc == 0; di++)
+			for (;;) {
+				const long long took = rename_slice(engines[si], engines[di], g, di, u_from, u_to, l_first, l_last, n,
+				    max_bytes, &moved, &dropped);
+				if (took < 0) rc = -1;
+				if (took <= 0) break;
+			}
+	if (moved_out) *moved_out = moved;
+	if (dropped_out) *dropped_out = dropped;
+	return rc;
+}
+
+extern "C" int cmb200_rename(cmb200_engine *e, uint64_t u_from, uint64_t u_to, uint64_t l_first, uint64_t l_last,
+    uint64_t *moved_out, uint64_t *dropped_out) {
+	return cmb200_rename_set(&e, 1, u_from, u_to, l_first, l_last, moved_out, dropped_out);
 }
 
 // ---- verified reads (CMB200_VERIFY) ------------------------------------------------------------

@@ -14,6 +14,7 @@
 #include "lz4_decode.cuh"
 #include "lz4_decode_cta.cuh"
 #include "streamgen.cuh"
+#include <cub/block/block_scan.cuh>
 
 namespace cmb {
 
@@ -227,28 +228,40 @@ __device__ __forceinline__ void count_warp(bool hit, unsigned long long *removed
 	if (m && (threadIdx.x & 31) == 0) atomicAdd(removed, (unsigned long long)__popc(m));
 }
 
-// One thread per slot (cap + 2 of them).  Only the first 16 bytes {key, addr_u} are read for every
-// slot, by one streaming load, so that a scan of a large table does not push the encoder's and the
-// small gets' lines out of L2; the rest of the slot is read only where addr_u matches.  A dead slot
-// keeps its old address, hence the liveness test of k_export_list.
+// The selection of one object's records, shared by cmb200_invalidate and cmb200_rename.
+// Scan: slot i (of cap + 2) holds a live local record of object u with l_first <= l <= l_last.  Only
+// the first 16 bytes {key, addr_u} are read for every slot, by one streaming load, so that a scan of a
+// large table does not push the encoder's and the small gets' lines out of L2; the rest of the slot is
+// read only where addr_u matches.  A dead slot keeps its old address, hence the liveness test of
+// k_export_list.
+__device__ __forceinline__ bool slot_in_scan(const TableView &t, uint64_t i, unsigned long long u,
+    unsigned long long l_first, unsigned long long l_last) {
+	const ulonglong2 ku = __ldcs(reinterpret_cast<const ulonglong2 *>(t.slots + i));
+	if (ku.y == u && (i >= t.cap || (ku.x != KEY_EMPTY && ku.x != KEY_TOMB))) {
+		const Slot &s = t.slots[i];
+		const unsigned long long l = s.addr_l;
+		return l >= l_first && l <= l_last && s.vlen != 0 && s.owner == 0;
+	}
+	return false;
+}
+// Keyed: slot s, found by the key of {u, l}, stores exactly that address, locally (its vlen is not
+// tested).  A key names one record, not one address: another object's page may hold it, and that
+// page is not selected.
+__device__ __forceinline__ bool slot_holds(const Slot &s, unsigned long long u, unsigned long long l) {
+	return s.addr_u == u && s.addr_l == l && s.owner == 0;
+}
+
+// One thread per slot (cap + 2 of them).
 __global__ void __launch_bounds__(256) k_invalidate_scan(TableView t, ArenaView a, unsigned long long u,
     unsigned long long l_first, unsigned long long l_last, unsigned long long *removed) {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
 	bool hit = false;
-	if (i < t.cap + 2) {
-		const ulonglong2 ku = __ldcs(reinterpret_cast<const ulonglong2 *>(t.slots + i));
-		if (ku.y == u && (i >= t.cap || (ku.x != KEY_EMPTY && ku.x != KEY_TOMB))) {
-			const Slot &s = t.slots[i];
-			const unsigned long long l = s.addr_l;
-			if (l >= l_first && l <= l_last && s.vlen != 0 && s.owner == 0) hit = slot_retire(t, a, (uint32_t)i);
-		}
-	}
+	if (i < t.cap + 2 && slot_in_scan(t, i, u, l_first, l_last)) hit = slot_retire(t, a, (uint32_t)i);
 	count_warp(hit, removed);
 }
 
 // One thread per l of the interval: the thread builds its address, finds the key's slot and retires
-// it only when the slot holds exactly that address.  A key names one record, not one address: another
-// object's page may hold it, and that page stays.
+// it only when the slot holds exactly that address.
 __global__ void __launch_bounds__(256) k_invalidate_keys(TableView t, ArenaView a, unsigned long long u,
     unsigned long long l_first, uint64_t n, unsigned long long *removed) {
 	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -256,12 +269,109 @@ __global__ void __launch_bounds__(256) k_invalidate_keys(TableView t, ArenaView 
 	if (i < n) {
 		const unsigned long long l = l_first + i;
 		const uint32_t idx = table_find(t, fnv_addr(u, l));
-		if (idx != 0xffffffffu) {
-			const Slot &s = t.slots[idx];
-			if (s.addr_u == u && s.addr_l == l && s.owner == 0) hit = slot_retire(t, a, idx);
-		}
+		if (idx != 0xffffffffu && slot_holds(t.slots[idx], u, l)) hit = slot_retire(t, a, idx);
 	}
 	count_warp(hit, removed);
+}
+
+// cmb200_rename, one slice.  Selection: every live local record of {u_from, l}, l in [l_first, l_last],
+// whose new address {u_to, l} belongs to engine `dst` of g, is a candidate.  Each warp reserves list
+// entries for its candidates with one atomicAdd on the count cursor r.cursor[0] (an add never fails, so
+// no warp waits on another); a candidate whose entry falls at or past r.max_n is not listed and stays
+// for the next slice.  Staging offsets are placed afterwards by k_rename_place.  Nothing in the table
+// changes here.
+__global__ void __launch_bounds__(256) k_rename_select(TableView t, RenameList r, unsigned long long u_from,
+    unsigned long long u_to, unsigned long long l_first, unsigned long long l_last, bool scan, int g, int dst,
+    uint32_t bsize) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	const int lane = threadIdx.x & 31;
+	uint32_t idx = 0xffffffffu;
+	if (scan) {
+		if (i < t.cap + 2 && slot_in_scan(t, i, u_from, l_first, l_last)) idx = (uint32_t)i;
+	} else if (i <= l_last - l_first) {
+		const unsigned long long l = l_first + i;
+		idx = table_find(t, fnv_addr(u_from, l));
+		if (idx != 0xffffffffu && (!slot_holds(t.slots[idx], u_from, l) || t.slots[idx].vlen == 0)) idx = 0xffffffffu;
+	}
+	if (idx != 0xffffffffu) {
+		const unsigned long long key = fnv_addr(u_to, t.slots[idx].addr_l);
+		if ((int)(((key >> 32) * (unsigned long long)g) >> 32) != dst) idx = 0xffffffffu;   // cmb200_owner
+	}
+	const bool want = idx != 0xffffffffu;
+	const unsigned m = __ballot_sync(0xffffffffu, want);
+	if (!m) return;
+	const int leader = __ffs(m) - 1;
+	unsigned long long c = 0;
+	if (lane == leader) c = atomicAdd(r.cursor, (unsigned long long)__popc(m));
+	c = __shfl_sync(0xffffffffu, c, leader);
+	const unsigned long long k = c + __popc(m & ((1u << lane) - 1u));
+	if (!want || k >= r.max_n) return;
+	const Slot &s = t.slots[idx];
+	const uint32_t vlen = s.vlen;
+	r.addr[2 * k] = u_to; r.addr[2 * k + 1] = s.addr_l;
+	r.ts[k] = s.ts;
+	r.loc[k] = s.rec_off;
+	r.slot[k] = idx;
+	r.len[k] = (24u + (vlen > 1u ? vlen - 1u : bsize) + 15u) & ~15u;
+	// the fingerprint goes along only when it belongs to this record version (k_export_list)
+	const bool has_fp = t.fp && (!t.fp_tag || t.fp_tag[idx] == ckpt_tag(s.rec_off, vlen - 1u));
+	r.fp[2 * k] = has_fp ? t.fp[2 * (size_t)idx] : 0ull;
+	r.fp[2 * k + 1] = has_fp ? t.fp[2 * (size_t)idx + 1] : 0ull;
+}
+
+// One CTA: the listed entries (min(cursor[0], max_n) of them) get their staging offsets, the exclusive
+// prefix sum of their lengths in list order.  The entries that start below r.max_bytes are the slice:
+// a prefix of the list, never empty when anything was listed (entry 0 starts at 0).  cursor[1] = its
+// records, cursor[2] = its bytes.  The rest stays in the table for the next slice.
+constexpr int RENAME_PLACE_THREADS = 256;
+__global__ void __launch_bounds__(RENAME_PLACE_THREADS) k_rename_place(RenameList r) {
+	typedef cub::BlockScan<unsigned long long, RENAME_PLACE_THREADS> Scan;
+	__shared__ typename Scan::TempStorage tmp;
+	__shared__ unsigned long long carry, end;
+	__shared__ uint32_t taken;
+	const unsigned long long listed = r.cursor[0] < r.max_n ? r.cursor[0] : r.max_n;
+	if (threadIdx.x == 0) { carry = 0; end = 0; taken = 0; }
+	__syncthreads();
+	for (unsigned long long base = 0; base < listed; base += RENAME_PLACE_THREADS) {
+		const unsigned long long k = base + threadIdx.x;
+		const unsigned long long need = k < listed ? r.len[k] : 0ull;
+		unsigned long long excl, total;
+		Scan(tmp).ExclusiveSum(need, excl, total);
+		const unsigned long long off = carry + excl;
+		if (k < listed) {
+			r.off[k] = off;
+			if (off < r.max_bytes) { atomicMax(&taken, (uint32_t)(k + 1)); atomicMax(&end, off + need); }
+		}
+		__syncthreads();
+		if (threadIdx.x == 0) carry += total;
+		__syncthreads();
+	}
+	if (threadIdx.x == 0) { r.cursor[1] = taken; r.cursor[2] = end; }
+}
+
+// One warp per taken record: its bytes, prefix and padding included, go to stage + off[k] with 16-byte
+// loads (from the mapped host tier past the L1, as k_promote reads it); then lane 0 retires the slot if
+// it still holds that location.  The retired record's bytes become garbage of their tier and are never
+// reused before a compaction or a lap of the tier, so small gets that staged it still read it whole.
+__global__ void __launch_bounds__(256) k_rename_gather(TableView t, ArenaView a, const uint8_t *host, RenameList r,
+    uint32_t n, uint8_t *stage) {
+	const int lane = threadIdx.x & 31;
+	const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	if (k >= n) return;
+	const unsigned long long loc = r.loc[k];
+	const uint32_t words = r.len[k] / 16u;
+	uint4 *dst = reinterpret_cast<uint4 *>(stage + r.off[k]);
+	if (loc & REC_HOST) {
+		const uint4 *src = reinterpret_cast<const uint4 *>(host + (loc & ~REC_HOST));
+		for (uint32_t w = lane; w < words; w += 32) dst[w] = __ldcg(src + w);
+	} else {
+		const uint4 *src = reinterpret_cast<const uint4 *>(a.base + loc);
+		for (uint32_t w = lane; w < words; w += 32) dst[w] = src[w];
+	}
+	__syncwarp();
+	if (lane != 0) return;
+	const uint32_t idx = r.slot[k];
+	if (t.slots[idx].vlen != 0 && t.slots[idx].rec_off == loc) slot_retire(t, a, idx);
 }
 
 // filemap_get_rand (filemap.c:264-314) picks the first key at or after a random 64-bit draw; the
@@ -1587,6 +1697,22 @@ int launch_invalidate(TableView t, ArenaView a, unsigned long long u, unsigned l
 		const uint64_t n = l_last - l_first + 1;
 		k_invalidate_keys<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, a, u, l_first, n, removed);
 	}
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_rename_select(TableView t, const RenameList &r, unsigned long long u_from, unsigned long long u_to,
+    unsigned long long l_first, unsigned long long l_last, bool scan, int g, int dst, uint32_t bsize, cudaStream_t st) {
+	const uint64_t n = scan ? t.cap + 2 : l_last - l_first + 1;
+	k_rename_select<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, r, u_from, u_to, l_first, l_last, scan, g, dst, bsize);
+	CMB_CHECK(cudaGetLastError());
+	k_rename_place<<<1, RENAME_PLACE_THREADS, 0, st>>>(r);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_rename_gather(TableView t, ArenaView a, const uint8_t *host, const RenameList &r, uint32_t n, uint8_t *stage,
+    cudaStream_t st) {
+	if (n == 0) return 0;
+	k_rename_gather<<<(n * 32 + 255) / 256, 256, 0, st>>>(t, a, host, r, n, stage);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

@@ -241,6 +241,29 @@ int launch_unset(TableView t, ArenaView a, const unsigned long long *addr, uint3
 int launch_invalidate(TableView t, ArenaView a, unsigned long long u, unsigned long long l_first,
     unsigned long long l_last, bool scan, unsigned long long *removed, cudaStream_t st);
 
+// cmb200_rename: the records of one slice, in the order they were taken.  Record k lies at loc[k] (slot
+// slot[k], len[k] bytes with the 16-byte padding) and is staged at off[k]; it is stored again at addr[k]
+// with ts[k] and fingerprint fp[k] ({0, 0} = none).  addr, ts, off and fp are what launch_restore reads.
+struct RenameList {
+	unsigned long long *cursor;       // [0] candidates counted by the select (zeroed before it), [1] records
+	                                  // of the slice, [2] its staged bytes (both written by the placement)
+	unsigned long long *addr, *ts, *off, *loc;
+	uint64_t *fp;
+	uint32_t *slot, *len;
+	uint32_t max_n;
+	unsigned long long max_bytes;
+};
+// k_rename_select: lists every live local record of {u_from, l}, l_first <= l <= l_last, whose {u_to, l}
+// belongs to engine dst of g, while the list has room (scan: one thread per slot, as k_invalidate_scan;
+// otherwise one thread per l, as k_invalidate_keys); then k_rename_place gives the listed records their
+// staging offsets and cuts the slice at max_bytes (cursor[1], cursor[2]).
+int launch_rename_select(TableView t, const RenameList &r, unsigned long long u_from, unsigned long long u_to,
+    unsigned long long l_first, unsigned long long l_last, bool scan, int g, int dst, uint32_t bsize, cudaStream_t st);
+// k_rename_gather: copies the n taken records to stage + off[k] (arena or mapped host tier `host`) and
+// retires each slot that still holds its record.
+int launch_rename_gather(TableView t, ArenaView a, const uint8_t *host, const RenameList &r, uint32_t n, uint8_t *stage,
+    cudaStream_t st);
+
 // Policy-equivalent of filemap_get_rand (filemap.c:264-314): first live slot at or after r.
 int launch_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,
     unsigned long long *ts_out, int32_t *ok, cudaStream_t st);

@@ -122,6 +122,18 @@ int cachemap_checkpoint(struct cachemap *cm);
 #define CACHEMAP_TO_END UINT64_MAX
 uint64_t cachemap_invalidate(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size);
 
+/*
+ * Rename.  edgefs_rename has the server copy `from` to `to` and delete `from`, after which `to` holds
+ * exactly the bytes `from` held; the file system calls this at that point (INTEGRATION.md, "Invalidation")
+ * with the nhid_small of each name.  Every cached page of `to` for genid is dropped, then every cached
+ * page of `from` moves to `to` on the GPU, without a decode or an encode; afterwards no page of `from` is
+ * cached.  Pages accepted by cachemap_put before the call are part of it.  A page the store has no room
+ * for is dropped; if the engine cannot move pages at all, the pages of `from` are dropped instead, so that
+ * nothing is served stale under either name.  Returns the pages moved.  The change counts for the next
+ * checkpoint.
+ */
+uint64_t cachemap_rename(struct cachemap *cm, uint64_t nhid_from, uint64_t nhid_to, uint32_t genid);
+
 /* requests / hits counters (cachemap.c:176,181) and the engine under the map. */
 void cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hits);
 struct cmb200_engine *cachemap_engine(struct cachemap *cm);

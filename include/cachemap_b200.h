@@ -142,6 +142,29 @@ int cmb200_unset_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr);
  * l_first > l_last, or on an engine that has made a multi-GPU call (its index holds other ranks'
  * records). */
 int cmb200_invalidate(cmb200_engine *e, uint64_t u, uint64_t l_first, uint64_t l_last, uint64_t *removed_out);
+/* Moves every live local record stored at {u_from, l}, l_first <= l <= l_last, to {u_to, l} on engine
+ * cmb200_owner(FNV(u_to, l), g), with the same block, ts and fingerprint (a fingerprint only where the
+ * record had one for that version).  After a 0 return no record is stored at {u_from, l} in the interval on
+ * any engine; each one that was is stored at {u_to, l}, byte for byte what a put of the same page there
+ * stores, its parse checkpoints rebuilt as a load rebuilds them, or was dropped for lack of arena room
+ * (counted in *dropped_out and in the `dropped` statistic, as a put is).  Only the moved pages' slots
+ * change: a {u_to, l} whose key another address holds replaces that record as a put would; a key of the
+ * interval that holds another object's address is left alone; the rest of u_to is not cleared (invalidate
+ * it first).  Selection goes key by key or by a scan of the table on cmb200_invalidate's threshold.
+ * The records move in slices (<= max_batch records, one page-ring buffer of bytes): under the source
+ * engine's lock they are copied out and retired, then under the destination's lock they are stored,
+ * after one compaction if the slice does not fit and garbage covers the shortfall; nothing is evicted or
+ * demoted.  Ordered after everything enqueued on each engine before the call, async puts included; never
+ * holds two engine locks at once, and one rename runs at a time.  Small gets on other streams may overlap
+ * and get the right page or a miss.  Records of the host tier move into the arena; retired bytes become
+ * garbage of their tier.  The next chain delta holds the moved records and tombstones for the old
+ * addresses.  u_from == u_to: 0, nothing changes.  -1 if l_first > l_last, g < 1, the engines' page sizes
+ * differ, or an engine has made a multi-GPU call (checked before anything changes). */
+int cmb200_rename_set(cmb200_engine *const *engines, int g, uint64_t u_from, uint64_t u_to,
+    uint64_t l_first, uint64_t l_last, uint64_t *moved_out, uint64_t *dropped_out);
+/* cmb200_rename_set with g = 1 */
+int cmb200_rename(cmb200_engine *e, uint64_t u_from, uint64_t u_to, uint64_t l_first, uint64_t l_last,
+    uint64_t *moved_out, uint64_t *dropped_out);
 /* Read-modify-write of stored pages.  Patch i writes len[i] >= 1 bytes at byte page_off[i] of the page
  * stored at addr[i] (page_off[i] + len[i] <= 1 << pshift).  bytes_host holds the patches' bytes back to
  * back in array order.  ts (nullable) as for cmb200_put_batch; a page patched more than once in the call
