@@ -10,5 +10,5 @@ from .binding import (  # noqa: F401
     fingerprint_batch, gen_chunk_host, gen_stream_ids, gen_addr, device_count, last_error,
     HIT, MISS, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, FINGERPRINT, EXPORTED_SYMBOLS, engine_stats,
     host_tier_stats, read_checkpoints, VERIFY, CORRUPT, verify_stats, owner, save_set, load_set,
-    snapshot_begin, snapshot_finish, chain_begin, load_chain, TOUCH, DROPPED, rename_set,
+    snapshot_begin, snapshot_finish, chain_begin, load_chain, TOUCH, DROPPED, rename_set, FREQ, freq_index,
 )

@@ -14,6 +14,7 @@ MISS, HIT, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, CORRUPT, DROPPED = 0, 1, 2, 3
 FINGERPRINT = 1
 VERIFY = 2
 TOUCH = 4       # a hit raises its record's timestamp: eviction by last access (CMB200_EVICT=access)
+FREQ = 8        # every get counts in a frequency sketch: admission by frequency (CMB200_ADMIT=freq)
 
 # every symbol the headers in include/ declare (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [
@@ -22,7 +23,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_print_stats", "cachemap_put_batch", "cachemap_get_batch", "cachemap_put_batch_dev",
     "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
-    "cachemap_pread", "cachemap_pwrite", "cachemap_rename",
+    "cachemap_pread", "cachemap_pwrite", "cachemap_rename", "cachemap_get_admission",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -43,7 +44,8 @@ EXPORTED_SYMBOLS = [
     "cmb200_owner", "cmb200_save_set", "cmb200_load_set", "cmb200_move_pages", "cmb200_copy_peer",
     "cmb200_verify_stats", "cmb200_verify_store", "cmb200_snapshot_begin", "cmb200_snapshot_finish",
     "cmb200_chain_begin", "cmb200_load_chain", "cmb200_invalidate", "cmb200_patch_batch",
-    "cmb200_rename", "cmb200_rename_set",
+    "cmb200_rename", "cmb200_rename_set", "cmb200_freq_index", "cmb200_freq_estimate", "cmb200_freq_read",
+    "cmb200_freq_stats",
 ]
 
 
@@ -65,6 +67,10 @@ class HostTierStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in (
         "bytes", "used", "records", "garbage", "demoted_records", "demoted_bytes", "retired_records", "hits",
         "promoted_records", "promoted_bytes")]
+
+
+class FreqStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in ("width", "period", "increments", "since_halving", "halvings")]
 
 
 class VerifyStats(C.Structure):
@@ -100,6 +106,7 @@ def lib() -> C.CDLL:
         "cachemap_put_batch_dev": (None, [vp, u64, vp, vp, vp, vp]),
         "cachemap_get_batch_dev": (None, [vp, u64, vp, vp, vp, vp, vp]),
         "cachemap_get_counters": (None, [vp, vp, vp]),
+        "cachemap_get_admission": (None, [vp, vp, vp]),
         "cachemap_engine": (vp, [vp]),
         "cachemap_engines": (i32, [vp, vp, i32]),
         "cachemap_checkpoint": (i32, [vp]),
@@ -173,6 +180,10 @@ def lib() -> C.CDLL:
         "cmb200_host_tier_hot": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_read_checkpoints": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_owner": (i32, [u64, i32]),
+        "cmb200_freq_index": (u32, [u64, i32, i32]),
+        "cmb200_freq_estimate": (i32, [vp, sz, vp, vp]),
+        "cmb200_freq_read": (i32, [vp, vp, sz]),
+        "cmb200_freq_stats": (i32, [vp, vp]),
         "cmb200_save_set": (i32, [vp, i32, C.c_char_p, vp]),
         "cmb200_load_set": (i32, [vp, i32, C.c_char_p, vp]),
         "cmb200_move_pages": (i32, [vp, sz, vp, vp, vp, vp]),
@@ -399,6 +410,25 @@ class Engine:
                "cmb200_verify_store")
         k = min(n.value, max_bad)
         return addr[:k, 0].copy(), addr[:k, 1].copy(), int(n.value), int(checked.value)
+
+    def freq_estimate(self, u, l) -> np.ndarray:
+        """cmb200_freq_estimate (engine created with FREQ) -> uint8 estimate (0..15) of each address's key."""
+        addr = _addr_array(u, l)
+        est = np.zeros(len(addr), dtype=np.uint8)
+        _check(lib().cmb200_freq_estimate(self.h, len(addr), _ptr(addr), _ptr(est)), "cmb200_freq_estimate")
+        return est
+
+    def freq_stats(self) -> dict:
+        """cmb200_freq_stats: width, period, increments, since_halving, halvings."""
+        st = FreqStats()
+        _check(lib().cmb200_freq_stats(self.h, C.byref(st)), "cmb200_freq_stats")
+        return {n: int(getattr(st, n)) for n, _ in FreqStats._fields_}
+
+    def freq_read(self) -> np.ndarray:
+        """cmb200_freq_read -> the sketch as uint64 words (4 rows of width / 16 words)."""
+        words = np.zeros(self.freq_stats()["width"] // 4, dtype=np.uint64)
+        _check(lib().cmb200_freq_read(self.h, _ptr(words), words.nbytes), "cmb200_freq_read")
+        return words
 
     def close(self):
         if self.h:
@@ -640,6 +670,11 @@ class Engine:
         _check(lib().cmb200_gen_chunks_dev(self.h, seed, _ptr(cids), len(cids), out_dev), "cmb200_gen_chunks_dev")
 
 
+def freq_index(key: int, row: int, log2_width: int) -> int:
+    """cmb200_freq_index: the counter of store key `key` in row `row` of a sketch of 2^log2_width per row."""
+    return int(lib().cmb200_freq_index(key, row, log2_width))
+
+
 def owner(key: int, g: int) -> int:
     """cmb200_owner: which of g engines holds the store key `key` (FNV-1a-64 of the address)."""
     return int(lib().cmb200_owner(key, g))
@@ -805,6 +840,12 @@ class Cachemap:
         rq, ht = C.c_uint64(), C.c_uint64()
         lib().cachemap_get_counters(self.h, C.byref(rq), C.byref(ht))
         return rq.value, ht.value
+
+    def admission(self):
+        """cachemap_get_admission -> (pages admitted over their victim, pages rejected) under CMB200_ADMIT=freq."""
+        a, r = C.c_uint64(), C.c_uint64()
+        lib().cachemap_get_admission(self.h, C.byref(a), C.byref(r))
+        return a.value, r.value
 
     def engine_handle(self) -> int:
         return int(lib().cachemap_engine(self.h) or 0)

@@ -46,6 +46,8 @@
 
 /* the library's external definition of the header's inline cmb200_owner */
 extern int cmb200_owner(uint64_t key, int g);
+/* ... and of cmb200_freq_index */
+extern uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width);
 
 /* The host tier is optional in the engine this layer links against: libcachemap's engine defines
  * these, an engine without a tier (such as the CPU stand-in the host-layer tests link) does not, and
@@ -69,6 +71,7 @@ extern int cmb200_owner(uint64_t key, int g);
 #pragma weak cmb200_invalidate
 #pragma weak cmb200_rename_set
 #pragma weak cmb200_patch_batch
+#pragma weak cmb200_freq_estimate
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -166,6 +169,10 @@ struct filemap {
 	 * flushers never evict for the same excess nor both fill the same room */
 	pthread_mutex_t evict_mu;
 	uint64_t reserved;      /* (atomic) */
+	/* CMB200_ADMIT=freq: count eviction admits a page only if it is asked for more often than its victim
+	 * (filemap_admit_n); set while the engines start, read after */
+	int admit;
+	uint64_t admitted, rejected;    /* (atomic) pages admitted over a victim / rejected */
 	/* persistence: <destdir>/cachemap_b200.snap (cmb200_save_set / cmb200_load_set) */
 	int persist;
 	long checkpoint_sec;    /* > 0: the checkpoint thread saves a snapshot this often when puts have landed */
@@ -295,6 +302,24 @@ evict_flags(int warn)
 	return 0;
 }
 
+/* CMB200_ADMIT: "freq" gives every engine a frequency sketch (CMB200_FREQ) that counts every get the GPU
+ * looks up, and eviction by count admits an incoming page only if its key has been asked for more often
+ * than the victim it would replace (filemap_admit_n).  It combines with CMB200_EVICT, which still chooses
+ * the victims.  "all" (or unset): every page is admitted, today's behaviour.  Any other value warns (once,
+ * with `warn`) and admits all. */
+static uint32_t
+admit_flags(int warn)
+{
+	const char *v = getenv("CMB200_ADMIT");
+	if (!v || !*v || strcmp(v, "all") == 0)
+		return 0;
+	if (strcmp(v, "freq") == 0)
+		return CMB200_FREQ;
+	if (warn)
+		fprintf(stderr, "cachemap_b200: CMB200_ADMIT=%s is neither freq nor all; admitting every page\n", v);
+	return 0;
+}
+
 /* Engine `index` of the map on CUDA device `device`, with its buffers; NULL if it cannot start.
  * The knobs apply per engine; the table and the default arena are sized for its share of the
  * capacity, ceil(n / G). */
@@ -331,6 +356,10 @@ fm_dev_start(struct filemap *m, int index, int device, int g)
 	/* every get compared with its page's EF128 on the GPU; a page that differs is a miss */
 	if (env_long("CMB200_VERIFY", 0)) cfg.flags |= CMB200_VERIFY;
 	cfg.flags |= evict_flags(index == 0);
+	const uint32_t admit = admit_flags(index == 0);
+	cfg.flags |= admit;
+	if (admit && cmb200_freq_estimate)
+		m->admit = 1;
 	d->eng = cmb200_engine_create(&cfg);
 	const long tier_mb = env_long("CMB200_HOST_TIER_MB", 0);
 	if (d->eng && tier_mb > 0) {
@@ -897,6 +926,131 @@ filemap_demote_n(struct fm_dev *d, uint64_t want)
 	return moved;
 }
 
+/* est_out[i] = the frequency estimate of addr[i]'s key, from the sketch of the engine that owns it.  -1 if
+ * an engine cannot give one. */
+static int
+filemap_estimate(struct filemap *m, size_t n, const cmb200_addr *addr, uint8_t *est_out)
+{
+	if (m->g == 1)
+		return cmb200_freq_estimate(m->dev[0]->eng, n, addr, est_out);
+	cmb200_addr *a = malloc(n * sizeof(*a));
+	size_t *at = malloc(n * sizeof(*at));
+	uint8_t *e = malloc(n);
+	int rc = (a && at && e) ? 0 : -1;
+	for (int k = 0; k < m->g && rc == 0; k++) {
+		size_t c = 0;
+		for (size_t i = 0; i < n; i++)
+			if (filemap_owner(m, &addr[i]) == m->dev[k]) {
+				at[c] = i;
+				a[c++] = addr[i];
+			}
+		if (c && cmb200_freq_estimate(m->dev[k]->eng, c, a, e) != 0)
+			rc = -1;
+		for (size_t i = 0; i < c && rc == 0; i++)
+			est_out[at[i]] = e[i];
+	}
+	free(a); free(at); free(e);
+	return rc;
+}
+
+struct drawn { cmb200_addr a; uint64_t i; };
+
+static int
+drawn_cmp(const void *x, const void *y)
+{
+	const struct drawn *p = x, *q = y;
+	const int c = addr_cmp(&p->a, &q->a);
+	return c ? c : (p->i < q->i ? -1 : p->i > q->i);
+}
+
+/* Admission by frequency (CMB200_ADMIT=freq) for the `want` pages that overflow the store, pages[0..want):
+ * victim k, drawn as filemap_evict_n draws it (the oldest of three), is paired with page k.  The page is
+ * admitted if its key's estimate is strictly greater than its victim's, and the victim is unset; otherwise
+ * reject[k] = 1 and the victim stays.  With want = 1 this is TinyLFU over the reference's sampler.  A
+ * victim drawn twice in a round is paired once, with the first page: the pages after it take the next
+ * victims, so every admitted page evicts a record of its own.  Pages left unpaired when the draws find
+ * nothing are admitted, as eviction that makes no progress admits them. */
+static void
+filemap_admit_n(struct filemap *m, uint64_t want, const cmb200_addr *pages, uint8_t *reject)
+{
+	static int warned;
+	uint64_t done = 0;
+	int idle = 0;
+	while (done < want && idle < 16) {
+		uint64_t need = want - done;
+		if (need > 4096)
+			need = 4096;
+		uint64_t *draws = malloc(3 * need * sizeof(uint64_t));
+		uint64_t *ts = malloc(3 * need * sizeof(uint64_t));
+		int32_t *ok = malloc(3 * need * sizeof(int32_t));
+		int *own = malloc(3 * need * sizeof(int));
+		cmb200_addr *cand = malloc(3 * need * sizeof(cmb200_addr));
+		struct drawn *dr = malloc(need * sizeof(struct drawn));
+		int *pk = malloc(need * sizeof(int));
+		cmb200_addr *victim = malloc(2 * need * sizeof(cmb200_addr));  /* then the pages, for one estimate */
+		int *vown = malloc(need * sizeof(int));
+		uint8_t *ev = malloc(2 * need);        /* estimates: the victims', then the pages' (ep) */
+		uint64_t nv = 0;
+		if (draws && ts && ok && own && cand && dr && pk && victim && vown && ev) {
+			for (uint64_t i = 0; i < 3 * need; i++)
+				draws[i] = rand64();
+			if (filemap_sample(m, NULL, (size_t)(3 * need), draws, cand, ts, ok, own) == 0) {
+				uint64_t nd = 0;
+				for (uint64_t i = 0; i < need; i++) {
+					uint64_t a = ts[3 * i], b = ts[3 * i + 1], c = ts[3 * i + 2];
+					int pick;
+					if (a < b)
+						pick = (a > c) ? 2 : 0;         /* cachemap.c:29-41 */
+					else
+						pick = (b > c) ? 2 : 1;
+					pk[i] = ok[3 * i + pick] > 0 ? pick : -1;
+					if (pk[i] >= 0)
+						dr[nd++] = (struct drawn){ cand[3 * i + pick], i };
+				}
+				qsort(dr, (size_t)nd, sizeof(*dr), drawn_cmp);
+				for (uint64_t k = 1; k < nd; k++)
+					if (addr_cmp(&dr[k].a, &dr[k - 1].a) == 0)
+						pk[dr[k].i] = -1;                 /* drawn before in this round */
+				for (uint64_t i = 0; i < need; i++)
+					if (pk[i] >= 0) {
+						victim[nv] = cand[3 * i + pk[i]];
+						vown[nv++] = own[3 * i + pk[i]];
+					}
+				/* victims and pages in one call per engine */
+				uint8_t *ep = ev + nv;
+				memcpy(victim + nv, pages + done, (size_t)nv * sizeof(cmb200_addr));
+				if (nv && filemap_estimate(m, (size_t)(2 * nv), victim, ev) != 0) {
+					if (!__atomic_exchange_n(&warned, 1, __ATOMIC_RELAXED))
+						fprintf(stderr, "cachemap_b200: admission has no estimates (%s); admitting every page\n",
+						    cmb200_last_error());
+					memset(ev, 0, (size_t)nv);
+					memset(ep, 1, (size_t)nv);
+				}
+				uint64_t ng = 0, nr = 0;
+				for (uint64_t k = 0; k < nv; k++) {
+					if (ep[k] > ev[k]) {
+						victim[ng] = victim[k];
+						vown[ng++] = vown[k];
+					} else {
+						reject[done + k] = 1;
+						nr++;
+					}
+				}
+				if (ng)
+					filemap_unset_victims(m, (size_t)ng, victim, vown);
+				__atomic_fetch_add(&m->admitted, ng, __ATOMIC_RELAXED);
+				__atomic_fetch_add(&m->rejected, nr, __ATOMIC_RELAXED);
+			} else {
+				fprintf(stderr, "cachemap_b200: eviction could not sample the store: %s\n", cmb200_last_error());
+			}
+		}
+		free(draws); free(ts); free(ok); free(own); free(cand); free(dr); free(pk); free(victim); free(vown);
+		free(ev);
+		done += nv;
+		idle = nv ? 0 : idle + 1;
+	}
+}
+
 /* Before a batch of `incoming` puts: while entries + incoming > capacity over all engines, evict
  * (cachemap.c:17-45); loops until the count fits or nothing more can be retired.  Then the batch's
  * pages are reserved until they have landed in their engine (filemap_land_end): a batch that has made
@@ -904,9 +1058,12 @@ filemap_demote_n(struct fm_dev *d, uint64_t want)
  * neither evict for the same excess nor fill the same room.  The estimate (entries + reserved) can
  * count a batch twice, after it has landed and before its reservation is released; so when the
  * estimate says evict, the decision takes every engine's land_mu and counts again: no batch is
- * between the two then, and no more is evicted than the count needs. */
+ * between the two then, and no more is evicted than the count needs.
+ * With CMB200_ADMIT=freq and the batch's addresses given (addr, nullable), the pages that overflow, the last
+ * `need` of the batch (the first ones fill the room that is free), go through filemap_admit_n instead:
+ * reject[i] = 1 marks a page that must not be stored (the caller zeroes reject). */
 static void
-filemap_evict(struct filemap *m, uint64_t incoming)
+filemap_evict(struct filemap *m, uint64_t incoming, const cmb200_addr *addr, uint8_t *reject)
 {
 	if (!m->capacity)
 		return;
@@ -922,6 +1079,14 @@ filemap_evict(struct filemap *m, uint64_t incoming)
 			uint64_t need = entries + incoming - m->capacity;
 			if (incoming == 1)
 				need = 1;       /* the reference evicts exactly one per put */
+			if (m->admit && addr) {
+				/* an excess beyond the batch (the store over capacity already) is evicted as before */
+				const uint64_t paired = need < incoming ? need : incoming;
+				if (need > paired)
+					filemap_evict_n(m, NULL, need - paired);
+				filemap_admit_n(m, paired, addr + incoming - paired, reject + incoming - paired);
+				break;
+			}
 			if (filemap_evict_n(m, NULL, need) == 0 || incoming == 1)
 				break;
 		}
@@ -1061,11 +1226,12 @@ filemap_promote_due(struct fm_dev *d)
 
 /* Before a batch of `incoming` puts into engine d: evict the map down to capacity (and reserve the
  * batch, see filemap_evict), then make sure d's arena has room (what eviction frees is garbage until
- * the arena is compacted).  The put follows between filemap_land_begin and filemap_land_end. */
+ * the arena is compacted).  The put follows between filemap_land_begin and filemap_land_end.  addr and
+ * reject: the batch's pages and the admission's verdicts (filemap_evict). */
 static void
-filemap_make_room(struct fm_dev *d, uint64_t incoming)
+filemap_make_room(struct fm_dev *d, uint64_t incoming, const cmb200_addr *addr, uint8_t *reject)
 {
-	filemap_evict(d->m, incoming);
+	filemap_evict(d->m, incoming, addr, reject);
 	filemap_check_arena(d, incoming);
 }
 
@@ -1113,6 +1279,7 @@ filemap_flusher(void *arg)
 	cmb200_addr *addr = malloc(FLUSH_MAX * sizeof(cmb200_addr));
 	uint64_t *ts = malloc(FLUSH_MAX * sizeof(uint64_t));
 	int32_t *lens = malloc(FLUSH_MAX * sizeof(int32_t));
+	uint8_t *reject = malloc(FLUSH_MAX);    /* admission's verdicts, then the put's valid flags */
 	pthread_mutex_lock(&d->wb_mu);
 	for (;;) {
 		uint64_t count = 0;
@@ -1158,16 +1325,24 @@ filemap_flusher(void *arg)
 		const uint64_t first = d->wb_tail % d->wb_n;
 		pthread_mutex_unlock(&d->wb_mu);
 
-		if (addr && ts && lens) {
+		if (addr && ts && lens && reject) {
 			pthread_mutex_lock(&d->room_mu);
-			filemap_make_room(d, count);
+			memset(reject, 0, (size_t)count);
+			filemap_make_room(d, count, addr, reject);
 			filemap_land_begin(d);
 			uint64_t run1 = count < d->wb_n - first ? count : d->wb_n - first;
+			uint8_t *valid = NULL;
+			if (m->admit) {                 /* a rejected page is not stored; its lens -1 unsets its key below */
+				for (uint64_t i = 0; i < count; i++)
+					reject[i] = !reject[i];
+				valid = reject;
+			}
 			for (uint64_t i = 0; i < count; i++)
 				lens[i] = 0;
-			cmb200_put_batch(d->eng, (size_t)run1, addr, NULL, d->wb_pages + first * (size_t)m->bsize, ts, lens);
+			cmb200_put_batch(d->eng, (size_t)run1, addr, valid, d->wb_pages + first * (size_t)m->bsize, ts, lens);
 			if (run1 < count)
-				cmb200_put_batch(d->eng, (size_t)(count - run1), addr + run1, NULL, d->wb_pages, ts + run1, lens + run1);
+				cmb200_put_batch(d->eng, (size_t)(count - run1), addr + run1, valid ? valid + run1 : NULL, d->wb_pages,
+				    ts + run1, lens + run1);
 			/* while the slots are still in the ring, which answers gets of their keys */
 			filemap_unset_dropped(d, (size_t)count, addr, lens);
 			filemap_land_end(d, count);
@@ -1191,6 +1366,7 @@ filemap_flusher(void *arg)
 	free(addr);
 	free(ts);
 	free(lens);
+	free(reject);
 	return NULL;
 }
 
@@ -1424,10 +1600,12 @@ filemap_set(struct filemap *m, uint128_t *key, void *value, uint64_t attr)
 	struct fm_dev *d = m->dev[cmb200_owner(k, m->g)];
 	if (!d->wb_n) {                         /* write-behind disabled: one synchronous GPU put */
 		pthread_mutex_lock(&d->room_mu);
-		filemap_make_room(d, 1);
+		uint8_t reject = 0;
+		filemap_make_room(d, 1, &a, &reject);
 		filemap_land_begin(d);
 		int32_t len = 0;
-		cmb200_put_batch(d->eng, 1, &a, NULL, value, &attr, &len);
+		const uint8_t valid = !reject;
+		cmb200_put_batch(d->eng, 1, &a, &valid, value, &attr, &len);
 		filemap_unset_dropped(d, 1, &a, &len);
 		filemap_land_end(d, 1);
 		pthread_mutex_unlock(&d->room_mu);
@@ -1867,6 +2045,39 @@ run_parts(struct batch_part *parts, int np, void *(*fn)(void *))
 	}
 }
 
+/* The admission's verdicts on a slice of a batch call (filemap_evict): a key whose newest page in the
+ * slice was rejected stores none of the slice's pages (valid = 0) and is unset now, before the put, so
+ * that no older page of it is served.  reject is zeroed again for the next slice. */
+static void
+filemap_reject_batch(struct filemap *m, size_t n, const cmb200_addr *addr, uint8_t *valid, uint8_t *reject)
+{
+	cmb200_addr *v = NULL;
+	int *own = NULL;
+	size_t nv = 0;
+	for (size_t i = 0; i < n; i++) {
+		if (!reject[i])
+			continue;
+		const uint64_t k = addr_key(&addr[i]);
+		size_t j = i + 1;
+		while (j < n && addr_key(&addr[j]) != k)
+			j++;
+		if (j < n)
+			continue;               /* a later page of the key decides */
+		for (j = 0; j <= i; j++)
+			if (addr_key(&addr[j]) == k)
+				valid[j] = 0;
+		if (!v && (!(v = malloc(n * sizeof(*v))) || !(own = malloc(n * sizeof(*own)))))
+			break;
+		own[nv] = cmb200_owner(k, m->g);
+		v[nv++] = addr[i];
+	}
+	if (nv)
+		filemap_unset_victims(m, nv, v, own);
+	free(v);
+	free(own);
+	memset(reject, 0, n);
+}
+
 static void
 put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const uint64_t *nhid,
     const uint32_t *genid, const void *pages, int on_dev)
@@ -1878,7 +2089,10 @@ put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 	if (batch_keys_build(cm, n, offset, nhid, genid, 1, &bk) != 0)
 		return;
 	size_t *order = malloc((size_t)n * sizeof(size_t));
-	if (!order) {
+	uint8_t *reject = calloc((size_t)n, 1);
+	if (!order || !reject) {
+		free(order);
+		free(reject);
 		batch_keys_free(&bk);
 		return;
 	}
@@ -1901,7 +2115,9 @@ put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 		const uint8_t *pg = (const uint8_t *)pages + at * bsize;
 		size_t start[MAX_DEVICES + 1];
 		group_by_owner(fm->g, (size_t)m, bk.own + at, order, start);
-		filemap_evict(fm, m);
+		filemap_evict(fm, m, bk.addr + at, reject);
+		if (fm->admit)
+			filemap_reject_batch(fm, (size_t)m, bk.addr + at, bk.valid + at, reject);
 		struct batch_part parts[MAX_DEVICES];
 		int np = 0;
 		for (int k = 0; k < fm->g; k++) {
@@ -1945,6 +2161,7 @@ put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 			batch_part_free(&parts[i]);
 	}
 	free(order);
+	free(reject);
 	batch_keys_free(&bk);
 }
 
@@ -2401,6 +2618,13 @@ cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hits)
 {
 	*requests = __atomic_load_n(&cm->requests, __ATOMIC_RELAXED);
 	*hits = __atomic_load_n(&cm->hits, __ATOMIC_RELAXED);
+}
+
+void
+cachemap_get_admission(struct cachemap *cm, uint64_t *admitted, uint64_t *rejected)
+{
+	*admitted = __atomic_load_n(&cm->pages->admitted, __ATOMIC_RELAXED);
+	*rejected = __atomic_load_n(&cm->pages->rejected, __ATOMIC_RELAXED);
 }
 
 struct cmb200_engine *

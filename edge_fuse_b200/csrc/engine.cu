@@ -163,7 +163,10 @@ struct cmb200_engine {
 	// words — and the open side of get_gate; what moves records or peer mappings (compaction, peers,
 	// destroy) closes get_gate.
 	static constexpr int GET_LANES = 32;
-	struct GetLane { std::atomic<int> busy{0}; Stream st; HostMem<int32_t> h_status; HostMem<cmb200_addr> h_addr; };
+	struct GetLane {
+		std::atomic<int> busy{0}; Stream st; HostMem<int32_t> h_status; HostMem<cmb200_addr> h_addr;
+		Event freq_done;                     // CMB200_FREQ: recorded after the lane's last counting get
+	};
 	GetLane lane[GET_LANES];
 	// A small get may be begun by one thread and ended by another (cmb200_get_small_begin / _end), so
 	// the "no small get in flight" condition is a counter and a closing flag, not a lock a thread owns.
@@ -275,6 +278,17 @@ struct cmb200_engine {
 	DevMem<unsigned long long> d_vstat;
 	DevMem<uint32_t> d_vidx;             // slot of each request of a verified or touching get batch (max_batch)
 	uint64_t scanned = 0, scan_corrupt = 0;
+	// CMB200_FREQ: the count-min sketch (4 rows of 2^freq_log2w 4-bit counters) and the host's count of the
+	// increments its launches made, kept in atomics so that a counting get takes no lock.  freq_streams has
+	// bit k set once lane k has counted (bit GET_LANES: the engine's stream st); freq_done of that lane
+	// (freq_st_done) follows its last counting launch, freq_halved the last halving.  freq_mu is taken by
+	// halvings and by the calls that read the sketch, never by a get that does not halve.
+	DevMem<unsigned long long> d_freq;
+	uint32_t freq_log2w = 0;
+	uint64_t freq_period = 0;
+	std::mutex freq_mu;
+	std::atomic<uint64_t> freq_incs{0}, freq_since{0}, freq_halvings{0}, freq_streams{0};
+	Event freq_st_done, freq_halved;
 	// snapshots (cmb200_snapshot_begin): SNAP_FREE, SNAP_CLAIMED by a snapshot that has not listed this
 	// engine's records yet, or SNAP_PENDING: listed, section not written yet.  snap_state changes under
 	// snap_mu and every change is broadcast on snap_cv.  Lock order: mu before snap_mu.  The snapshot's
@@ -385,9 +399,22 @@ static int engine_init(cmb200_engine *e, const cmb200_config *cfg) {
 		CMB_CHECK(cudaMemsetAsync(e->d_vstat, 0, 2 * VS_WORDS * sizeof(unsigned long long), e->st));
 	}
 	if ((e->flags & (CMB200_VERIFY | CMB200_TOUCH)) && e->d_vidx.alloc(B * 4)) return -1;
+	if (e->flags & CMB200_FREQ) {
+		// 2 x width bytes, before the arena takes its share of free memory
+		uint64_t w = next_pow2(cfg->capacity ? cfg->capacity : e->table.cap / 4);
+		if (w < 16) w = 16;
+		if (w > (1ull << 32)) w = 1ull << 32;
+		while ((1ull << e->freq_log2w) < w) e->freq_log2w++;
+		e->freq_period = 10 * (cfg->capacity ? cfg->capacity : w);
+		if (e->d_freq.alloc(2 * w)) return -1;
+		CMB_CHECK(cudaMemsetAsync(e->d_freq, 0, 2 * w, e->st));
+		if (e->freq_st_done.create(cudaEventDisableTiming) || e->freq_halved.create(cudaEventDisableTiming)) return -1;
+		for (auto &ln : e->lane) if (ln.freq_done.create(cudaEventDisableTiming)) return -1;
+	}
 	if (get_small_supports(e->bsize)) {
 		// the descriptor scratch of the fused single-page get
-		const int resident = get_small_residency(e->bsize, e->table.fp_tag != nullptr, e->flags & CMB200_TOUCH);
+		const int resident = get_small_residency(e->bsize, e->table.fp_tag != nullptr, e->flags & CMB200_TOUCH,
+		    e->flags & CMB200_FREQ);
 		if (resident <= 0) { set_error_msg("k_get_small does not fit this device"); return -1; }
 		e->pool_n = (uint32_t)resident;
 		e->region_entries = get_small_region_entries(e->bsize);
@@ -663,6 +690,13 @@ static int check_dev_pages(const void *pages, const char *what) {
 	return 0;
 }
 
+// The multi-GPU calls are refused with a sketch: it counts the gets of this engine's own keys.
+static int freq_refuses(cmb200_engine *e, const char *what) {
+	if (!e->d_freq) return 0;
+	snprintf(g_err, sizeof(g_err), "%s: not available on an engine with CMB200_FREQ", what);
+	return -1;
+}
+
 // The multi-GPU calls and the host tier exclude each other: the exchange records and peer reads know
 // arena locations only.
 static int multi_gpu_call(cmb200_engine *e, const char *what) {
@@ -702,7 +736,7 @@ extern "C" int cmb200_put_batch_async(cmb200_engine *e, size_t n, const cmb200_a
 extern "C" int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     const void *pages, int pages_on_dev, const uint64_t *ts, uint32_t rank, void *records_dev_out,
     int32_t *lens_out, uint64_t *ticket) {
-	if (multi_gpu_call(e, "cmb200_put_step")) return -1;
+	if (freq_refuses(e, "cmb200_put_step") || multi_gpu_call(e, "cmb200_put_step")) return -1;
 	if (n > cmb200_engine::META_CAP) { set_error_msg("cmb200_put_step: more than 262144 chunks in one step"); return -1; }
 	if (pages_on_dev == 1 && check_dev_pages(pages, "cmb200_put_step")) return -1;
 	std::lock_guard<std::mutex> g(e->mu);
@@ -716,7 +750,7 @@ extern "C" int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *ad
 
 extern "C" int cmb200_import_records_dev(cmb200_engine *e, size_t n_total, const void *records_dev, uint32_t my_rank) {
 	std::lock_guard<std::mutex> g(e->mu);
-	if (multi_gpu_call(e, "cmb200_import_records_dev")) return -1;
+	if (freq_refuses(e, "cmb200_import_records_dev") || multi_gpu_call(e, "cmb200_import_records_dev")) return -1;
 	CMB_CHECK(cudaSetDevice(e->device));
 	if (n_total == 0) return 0;
 	if (n_total > 0xffffffffull) { set_error_msg("cmb200_import_records_dev: too many records"); return -1; }
@@ -746,6 +780,100 @@ extern "C" int cmb200_put_batch_dev(cmb200_engine *e, size_t n, const cmb200_add
 	return put_impl(e, n, addr, valid, (const uint8_t *)pages_dev, true, ts, lens_out, nullptr);
 }
 
+// ---- CMB200_FREQ: ordering of the sketch's launches ---------------------------------------------
+// Increments commute, a halving does not: a halving waits for every counting launch enqueued before it on
+// any stream, and every counting launch waits for the last halving.  Launches of concurrent calls on
+// different streams are not ordered with each other's halvings (cachemap_b200.h: benign).
+
+// `st` (stream index k: a lane, or GET_LANES for the engine's stream) waits for every other stream's last
+// counting launch.  (freq_mu held)
+static int freq_fence(cmb200_engine *e, cudaStream_t st, int k) {
+	const uint64_t streams = e->freq_streams.load(std::memory_order_acquire);
+	for (int j = 0; j <= cmb200_engine::GET_LANES; j++) {
+		if (j == k || !((streams >> j) & 1u)) continue;
+		CMB_CHECK(cudaStreamWaitEvent(st, j == cmb200_engine::GET_LANES ? e->freq_st_done : e->lane[j].freq_done, 0));
+	}
+	return 0;
+}
+
+// Before a counting launch on `st`: after the last halving.  No lock: freq_halvings is raised only after
+// freq_halved has been recorded, and a wait takes the event's latest record.
+static int freq_before(cmb200_engine *e, cudaStream_t st) {
+	if (e->freq_halvings.load(std::memory_order_acquire)) CMB_CHECK(cudaStreamWaitEvent(st, e->freq_halved, 0));
+	return 0;
+}
+
+// After a counting launch of `valid` requests on stream index k (whose event only this call records: a lane
+// belongs to one get at a time, st to the holder of e->mu): books the increments.  The launch whose
+// increments take the count since the last halving across the period halves the sketch behind itself on its
+// stream, under freq_mu, and takes its share off the count; increments of concurrent calls stay counted.
+static int freq_after(cmb200_engine *e, cudaStream_t st, int k, uint64_t valid) {
+	CMB_CHECK(cudaEventRecord(k == cmb200_engine::GET_LANES ? e->freq_st_done : e->lane[k].freq_done, st));
+	e->freq_streams.fetch_or(1ull << k, std::memory_order_release);
+	e->freq_incs.fetch_add(valid, std::memory_order_relaxed);
+	const uint64_t before = e->freq_since.fetch_add(valid, std::memory_order_acq_rel);
+	if (before >= e->freq_period || before + valid < e->freq_period) return 0;
+	std::lock_guard<std::mutex> g(e->freq_mu);
+	if (freq_fence(e, st, k) || launch_freq_halve(e->d_freq, e->freq_log2w, st)) return -1;
+	CMB_CHECK(cudaEventRecord(e->freq_halved, st));
+	e->freq_since.fetch_sub(before + valid, std::memory_order_acq_rel);
+	e->freq_halvings.fetch_add(1, std::memory_order_release);
+	return 0;
+}
+
+static int freq_required(cmb200_engine *e, const char *what) {
+	if (e->d_freq) return 0;
+	snprintf(g_err, sizeof(g_err), "%s: the engine was created without CMB200_FREQ", what);
+	return -1;
+}
+
+// The engine's stream after every counting launch and halving enqueued so far.  (freq_mu not held)
+static int freq_settle(cmb200_engine *e) {
+	std::lock_guard<std::mutex> g(e->freq_mu);
+	if (freq_fence(e, e->st, cmb200_engine::GET_LANES)) return -1;
+	if (e->freq_halvings.load(std::memory_order_acquire)) CMB_CHECK(cudaStreamWaitEvent(e->st, e->freq_halved, 0));
+	return 0;
+}
+
+extern "C" int cmb200_freq_estimate(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint8_t *est_out) {
+	if (freq_required(e, "cmb200_freq_estimate")) return -1;
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (freq_settle(e)) return -1;
+	for (size_t at = 0; at < n; at += e->max_batch) {
+		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
+		uint8_t *d_est = reinterpret_cast<uint8_t *>((int32_t *)e->d_status);
+		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
+		if (launch_freq_estimate(e->d_freq, e->freq_log2w, e->d_addr, m, d_est, e->st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(est_out + at, d_est, m, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		e->stats.kernel_launches++;
+	}
+	return 0;
+}
+
+extern "C" int cmb200_freq_read(cmb200_engine *e, void *out, size_t bytes) {
+	if (freq_required(e, "cmb200_freq_read")) return -1;
+	if (bytes != ((size_t)2 << e->freq_log2w)) { set_error_msg("cmb200_freq_read: bytes is not the sketch's size"); return -1; }
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (freq_settle(e)) return -1;
+	CMB_CHECK(cudaMemcpyAsync(out, e->d_freq, bytes, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	return 0;
+}
+
+extern "C" int cmb200_freq_stats(cmb200_engine *e, struct cmb200_freq_stats *out) {
+	if (freq_required(e, "cmb200_freq_stats")) return -1;
+	std::lock_guard<std::mutex> g(e->freq_mu);
+	out->width = 1ull << e->freq_log2w;
+	out->period = e->freq_period;
+	out->increments = e->freq_incs.load();
+	out->since_halving = e->freq_since.load();
+	out->halvings = e->freq_halvings.load();
+	return 0;
+}
+
 // ---- get ---------------------------------------------------------------------------------
 
 static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
@@ -759,6 +887,7 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 	CMB_CHECK(cudaMemcpyAsync(e->d_addr, h_addr, n * 16, cudaMemcpyHostToDevice, e->st));
 	if (valid) CMB_CHECK(cudaMemcpyAsync(e->d_valid, h_valid, n, cudaMemcpyHostToDevice, e->st));
 	size_t nb = 0;
+	if (e->d_freq && freq_before(e, e->st)) return -1;
 	for (size_t at = 0; at < n; at += B, nb++) {
 		const uint32_t m = (uint32_t)((n - at < B) ? n - at : B);
 		const int buf = (int)(nb & 1);
@@ -766,6 +895,11 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		if (!out_on_dev) CMB_CHECK(cudaStreamWaitEvent(e->st, e->consumed[buf], 0));   // D2H of buf finished
 		if (launch_lookup(e->table, e->d_addr + 2 * at, valid ? e->d_valid + at : nullptr, m, e->d_status + at, e->d_recoff,
 			e->d_vlen, nullptr, e->st, e->d_vidx)) return -1;
+		if (e->d_freq) {
+			if (launch_freq_add(e->d_freq, e->freq_log2w, e->d_addr + 2 * at, valid ? e->d_valid + at : nullptr, m, e->st))
+				return -1;
+			e->stats.kernel_launches++;
+		}
 		DecodeJob job{};
 		job.n = m; job.nbytes = e->bsize; job.pages = d_out; job.status = e->d_status + at;
 		job.rec_off = e->d_recoff; job.vlen = e->d_vlen; job.arena = e->arena.base;
@@ -776,6 +910,11 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 		CMB_CHECK(cudaEventRecord(e->t0[nb % e->RING], e->st));
 		if (launch_decode(job, e->st, e->table.fp_tag ? &ver : nullptr, touch.ts ? &touch : nullptr)) return -1;
 		CMB_CHECK(cudaEventRecord(e->t1[nb % e->RING], e->st));
+		if (e->d_freq) {
+			uint64_t counted = m;
+			if (valid) { counted = 0; for (uint32_t k = 0; k < m; k++) counted += valid[at + k] != 0; }
+			if (freq_after(e, e->st, cmb200_engine::GET_LANES, counted)) return -1;
+		}
 		if (!out_on_dev) {
 			CMB_CHECK(cudaEventRecord(e->landed[buf], e->st));
 			CMB_CHECK(cudaStreamWaitEvent(e->copy, e->landed[buf], 0));
@@ -906,7 +1045,15 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	job.hot = e->tier.hot();
 	job.vstat = e->d_vstat;
 	job.touch_ts = (e->flags & CMB200_TOUCH) ? touch_stamp() : 0ull;
-	if (launch_get_small(job, e->device, ln->st)) { ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1; }
+	job.freq = e->d_freq; job.freq_log2w = e->freq_log2w;
+	if ((e->d_freq && freq_before(e, ln->st)) || launch_get_small(job, e->device, ln->st)) {
+		ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1;
+	}
+	if (e->d_freq && freq_after(e, ln->st, li, n)) {
+		// the kernel is in flight and writes the lane's status words: the lane is freed once it is done
+		cudaStreamSynchronize(ln->st);
+		ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1;
+	}
 	t->lane = li; t->n = (uint32_t)n; t->status = ln->h_status;
 	return 0;
 }
@@ -989,7 +1136,7 @@ extern "C" int cmb200_arena_ipc_handle(cmb200_engine *e, void *handle64, uint64_
 extern "C" int cmb200_open_peer(cmb200_engine *e, uint32_t rank, const void *handle64, uint64_t arena_bytes) {
 	{
 		std::lock_guard<std::mutex> g(e->mu);
-		if (multi_gpu_call(e, "cmb200_open_peer")) return -1;
+		if (freq_refuses(e, "cmb200_open_peer") || multi_gpu_call(e, "cmb200_open_peer")) return -1;
 	}
 	if (rank >= GET_MAX_PEERS) { set_error_msg("cmb200_open_peer: rank out of range"); return -1; }
 	cmb200_engine::GateClosed g(e->get_gate);

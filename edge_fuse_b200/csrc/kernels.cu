@@ -7,6 +7,7 @@
 //   k_streamgen   synthetic benchmark input
 #include "kernels.h"
 #include "common.cuh"
+#include "../../include/cachemap_b200.h"
 #include "fingerprint.cuh"
 #include "lz4_encode.cuh"
 #include "lz4_encode_ring.cuh"
@@ -189,6 +190,22 @@ __device__ __forceinline__ void slot_touch(Slot *slots, uint32_t idx, unsigned l
 	Slot &s = slots[idx];
 	const unsigned long long key = fnv_addr(u, l);
 	if (key == KEY_EMPTY || key == KEY_TOMB || ld_key(&s) == key) atomicMax(&s.ts, stamp);
+}
+
+// ---- CMB200_FREQ: the count-min sketch (cachemap_b200.h) ----
+// +1 on key's counter in row r, saturating at 15 (one thread).  A CAS loop on the counter's word: two
+// increments of one word from different requests both land, and a halving (k_freq_halve) that lands in
+// between makes the CAS fail and the loop retry on the halved word.
+__device__ __forceinline__ void freq_add_row(unsigned long long *f, uint32_t log2w, unsigned long long key, int r) {
+	const uint32_t j = cmb200_freq_index(key, r, (int)log2w);
+	const uint32_t sh = 4u * (j & 15u);
+	unsigned long long *w = f + ((size_t)r << (log2w - 4u)) + (j >> 4);
+	unsigned long long old = *reinterpret_cast<volatile unsigned long long *>(w);
+	while (((old >> sh) & 15ull) != 15ull) {
+		const unsigned long long seen = atomicCAS(w, old, old + (1ull << sh));
+		if (seen == old) break;
+		old = seen;
+	}
 }
 
 // Retires the record of slot idx: the slot becomes a tombstone (the side slots of keys 0 and ~0 stay
@@ -1158,7 +1175,11 @@ __device__ __forceinline__ void gs_answer(const GetJob &job, uint32_t i, int32_t
 // VERIFY (CMB200_VERIFY): the page, decoded or raw, is compared with the record's stored EF128 while it
 // is still in shared memory (gs_page_matches), so a page that does not match is never written out and
 // is answered ST_CORRUPT.
-template <bool VERIFY, bool TOUCH>
+// FREQ (CMB200_FREQ): every request with a valid address adds 1 to its key's four sketch counters, one
+// lane of warp 1 per row, once the answer is decided: off the path to the status word, which thread 0
+// of warp 0 stores.  The key is hashed from the address loaded at entry: the request arrays are not read
+// once the status may be visible.
+template <bool VERIFY, bool TOUCH, bool FREQ>
 __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
 	GetShared *sh = reinterpret_cast<GetShared *>(smem);
@@ -1169,6 +1190,9 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	const int lane = tid & 31;
 	const uint32_t warp = tid >> 5;
 	const unsigned long long u = job.addr[2 * (size_t)i], l = job.addr[2 * (size_t)i + 1];
+	// FREQ: the key is taken now.  Once the status is published the caller may hand the request arrays (a
+	// lane's page-locked words) to its next call, so nothing of them is read after that.
+	const unsigned long long fkey = FREQ ? fnv_addr(u, l) : 0ull;
 	uint8_t *out = job.out + (size_t)i * job.nbytes;
 	const uint32_t s_bar = smem_addr(&sh->bar);
 	if (job.valid && !job.valid[i]) { if (tid == 0) job.status[i] = ST_INVALID; return; }
@@ -1283,6 +1307,7 @@ __global__ void __launch_bounds__(GS_THREADS, 1) k_get_small(GetJob job) {
 	if (tid == 0)
 		gs_answer<VERIFY, TOUCH>(job, i, result, sh->region, from_host, sh->fp_ok,
 		    TOUCH && sh->owner == 0u ? sh->idx : 0xffffffffu);
+	if (FREQ && warp == 1u && lane < 4) freq_add_row(job.freq, job.freq_log2w, fkey, lane);
 }
 
 // ---- pages above 64 KiB: one request per cluster of two CTAs ----------------------------------------
@@ -1330,7 +1355,9 @@ __device__ __forceinline__ void dsmem_st32(uint32_t a, uint32_t v) { asm volatil
 
 // VERIFY: the CTA that holds the page compares it with the record's stored EF128 before writing it out
 // (gs_page_matches): the page CTA for a decoded page, the record CTA for a raw one.
-template <bool VERIFY, bool TOUCH>
+// FREQ: the record CTA counts the request in the sketch (warp 1, one lane per row) once it has handed
+// the verdict over, as k_get_small does.
+template <bool VERIFY, bool TOUCH, bool FREQ>
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get_small_pair(GetJob job) {
 	extern __shared__ __align__(128) uint8_t smem[];
 	DecodeCta *dc = reinterpret_cast<DecodeCta *>(smem + 128);
@@ -1374,6 +1401,7 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 	GetShared *sh = reinterpret_cast<GetShared *>(smem);
 	uint8_t *rec = buf;
 	const unsigned long long u = job.addr[2 * (size_t)i], l = job.addr[2 * (size_t)i + 1];
+	const unsigned long long fkey = FREQ ? fnv_addr(u, l) : 0ull;   // as in k_get_small: read before any answer
 	const uint32_t s_bar = smem_addr(&sh->bar);
 	if (tid == 0) {
 		sh->region = 0xffffffffu;
@@ -1487,9 +1515,10 @@ __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GS_THREADS, 1) k_get
 	}
 	cluster_arrive_release();                                   // B
 	cluster_wait();
+	if (FREQ && warp == 1u && lane < 4) freq_add_row(job.freq, job.freq_log2w, fkey, lane);
 }
 
-template <bool VERIFY, bool TOUCH>
+template <bool VERIFY, bool TOUCH, bool FREQ>
 static int launch_get_small_kernel(const GetJob &job, int device, cudaStream_t st) {
 	const size_t smem = get_small_smem(job.nbytes, VERIFY);
 	// the attribute belongs to the device: engines on several GPUs (CMB200_DEVICES) each set their own
@@ -1498,52 +1527,120 @@ static int launch_get_small_kernel(const GetJob &job, int device, cudaStream_t s
 	if (job.nbytes > GS_MAX_PAGE) {
 		static size_t configured_pair[MAX_DEV] = {};
 		if (smem > configured_pair[dev]) {
-			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+			CMB_CHECK(cudaFuncSetAttribute(k_get_small_pair<VERIFY, TOUCH, FREQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 			configured_pair[dev] = smem;
 		}
-		k_get_small_pair<VERIFY, TOUCH><<<2u * job.n, GS_THREADS, smem, st>>>(job);
+		k_get_small_pair<VERIFY, TOUCH, FREQ><<<2u * job.n, GS_THREADS, smem, st>>>(job);
 		CMB_CHECK(cudaGetLastError());
 		return 0;
 	}
 	static size_t configured[MAX_DEV] = {};
 	if (smem > configured[dev]) {
-		CMB_CHECK(cudaFuncSetAttribute(k_get_small<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+		CMB_CHECK(cudaFuncSetAttribute(k_get_small<VERIFY, TOUCH, FREQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 		configured[dev] = smem;
 	}
-	k_get_small<VERIFY, TOUCH><<<job.n, GS_THREADS, smem, st>>>(job);
+	k_get_small<VERIFY, TOUCH, FREQ><<<job.n, GS_THREADS, smem, st>>>(job);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
+}
+template <bool VERIFY, bool TOUCH>
+static int launch_get_small_vt(const GetJob &job, int device, cudaStream_t st) {
+	return job.freq ? launch_get_small_kernel<VERIFY, TOUCH, true>(job, device, st)
+	                : launch_get_small_kernel<VERIFY, TOUCH, false>(job, device, st);
 }
 int launch_get_small(const GetJob &job, int device, cudaStream_t st) {
 	if (job.n == 0) return 0;
 	if (job.touch_ts)
-		return job.table.fp_tag ? launch_get_small_kernel<true, true>(job, device, st) : launch_get_small_kernel<false, true>(job, device, st);
-	return job.table.fp_tag ? launch_get_small_kernel<true, false>(job, device, st) : launch_get_small_kernel<false, false>(job, device, st);
+		return job.table.fp_tag ? launch_get_small_vt<true, true>(job, device, st) : launch_get_small_vt<false, true>(job, device, st);
+	return job.table.fp_tag ? launch_get_small_vt<true, false>(job, device, st) : launch_get_small_vt<false, false>(job, device, st);
 }
 
 // Requests of k_get_small (CTAs) or k_get_small_pair (clusters) that can be resident on the device at
 // once (= scratch regions needed).  Clusters of two need two SMs of one GPC.
-template <bool VERIFY, bool TOUCH>
+template <bool VERIFY, bool TOUCH, bool FREQ>
 static int get_small_residency_of(uint32_t nbytes) {
 	const size_t smem = get_small_smem(nbytes, VERIFY);
 	if (nbytes > GS_MAX_PAGE) {
-		if (cudaFuncSetAttribute(k_get_small_pair<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+		if (cudaFuncSetAttribute(k_get_small_pair<VERIFY, TOUCH, FREQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
 		cudaLaunchConfig_t cfg = {};
 		cfg.gridDim = dim3(2u * (uint32_t)sm_count());
 		cfg.blockDim = dim3(GS_THREADS);
 		cfg.dynamicSmemBytes = smem;
 		int clusters = 0;
-		if (cudaOccupancyMaxActiveClusters(&clusters, k_get_small_pair<VERIFY, TOUCH>, &cfg) != cudaSuccess) return -1;
+		if (cudaOccupancyMaxActiveClusters(&clusters, k_get_small_pair<VERIFY, TOUCH, FREQ>, &cfg) != cudaSuccess) return -1;
 		return clusters;
 	}
-	if (cudaFuncSetAttribute(k_get_small<VERIFY, TOUCH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
+	if (cudaFuncSetAttribute(k_get_small<VERIFY, TOUCH, FREQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -1;
 	int per_sm = 0;
-	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_get_small<VERIFY, TOUCH>, (int)GS_THREADS, smem) != cudaSuccess) return -1;
+	if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_get_small<VERIFY, TOUCH, FREQ>, (int)GS_THREADS, smem) != cudaSuccess) return -1;
 	return per_sm * sm_count();
 }
-int get_small_residency(uint32_t nbytes, bool verify, bool touch) {
-	if (touch) return verify ? get_small_residency_of<true, true>(nbytes) : get_small_residency_of<false, true>(nbytes);
-	return verify ? get_small_residency_of<true, false>(nbytes) : get_small_residency_of<false, false>(nbytes);
+template <bool VERIFY, bool TOUCH>
+static int get_small_residency_vt(uint32_t nbytes, bool freq) {
+	return freq ? get_small_residency_of<VERIFY, TOUCH, true>(nbytes) : get_small_residency_of<VERIFY, TOUCH, false>(nbytes);
+}
+int get_small_residency(uint32_t nbytes, bool verify, bool touch, bool freq) {
+	if (touch) return verify ? get_small_residency_vt<true, true>(nbytes, freq) : get_small_residency_vt<false, true>(nbytes, freq);
+	return verify ? get_small_residency_vt<true, false>(nbytes, freq) : get_small_residency_vt<false, false>(nbytes, freq);
+}
+
+// ---- CMB200_FREQ: the sketch's batch kernels -----------------------------------------------------
+
+__global__ void __launch_bounds__(256) k_freq_add(unsigned long long *f, uint32_t log2w, const unsigned long long *addr,
+    const uint8_t *valid, uint32_t n) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n || (valid && !valid[i])) return;
+	const unsigned long long key = fnv_addr(addr[2 * (size_t)i], addr[2 * (size_t)i + 1]);
+	for (int r = 0; r < 4; r++) freq_add_row(f, log2w, key, r);
+}
+
+// Every counter halved: (w >> 1) & 0x7777... per word, by CAS, so that an increment that lands on the word
+// meanwhile is kept (before or after the halving) rather than overwritten.
+__global__ void __launch_bounds__(256) k_freq_halve(unsigned long long *f, size_t words) {
+	for (size_t k = blockIdx.x * (size_t)blockDim.x + threadIdx.x; k < words; k += (size_t)gridDim.x * blockDim.x) {
+		unsigned long long old = *reinterpret_cast<volatile unsigned long long *>(f + k);
+		for (;;) {
+			const unsigned long long seen = atomicCAS(f + k, old, (old >> 1) & 0x7777777777777777ull);
+			if (seen == old) break;
+			old = seen;
+		}
+	}
+}
+
+__global__ void __launch_bounds__(256) k_freq_estimate(const unsigned long long *f, uint32_t log2w,
+    const unsigned long long *addr, uint32_t n, uint8_t *est) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const unsigned long long key = fnv_addr(addr[2 * (size_t)i], addr[2 * (size_t)i + 1]);
+	uint32_t m = 15u;
+	for (int r = 0; r < 4; r++) {
+		const uint32_t j = cmb200_freq_index(key, r, (int)log2w);
+		const unsigned long long w = f[((size_t)r << (log2w - 4u)) + (j >> 4)];
+		m = min(m, (uint32_t)(w >> (4u * (j & 15u))) & 15u);
+	}
+	est[i] = (uint8_t)m;
+}
+
+int launch_freq_add(unsigned long long *freq, uint32_t log2w, const unsigned long long *addr, const uint8_t *valid,
+    uint32_t n, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_freq_add<<<(n + 255) / 256, 256, 0, st>>>(freq, log2w, addr, valid, n);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_freq_halve(unsigned long long *freq, uint32_t log2w, cudaStream_t st) {
+	const size_t words = (size_t)1 << (log2w - 2u);            // 4 rows of 2^log2w / 16 words
+	const size_t blocks = (words + 255) / 256 < 1024 ? (words + 255) / 256 : 1024;
+	k_freq_halve<<<(unsigned)blocks, 256, 0, st>>>(freq, words);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_freq_estimate(const unsigned long long *freq, uint32_t log2w, const unsigned long long *addr, uint32_t n,
+    uint8_t *est, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_freq_estimate<<<(n + 255) / 256, 256, 0, st>>>(freq, log2w, addr, n, est);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
 }
 
 // ------------------------------------------------------------------------------------------

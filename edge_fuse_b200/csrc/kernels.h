@@ -188,13 +188,24 @@ struct GetJob {
 	                                  // other members keep their parameter offsets
 	unsigned long long *vstat;        // CMB200_VERIFY (table.fp_tag set): VS_WORDS counters
 	unsigned long long touch_ts;      // CMB200_TOUCH: a local hit raises its slot's ts to this; 0 = no touch
+	unsigned long long *freq;         // CMB200_FREQ: the sketch every valid request counts in; null = no sketch
+	uint32_t freq_log2w;              // log2 of the sketch's counters per row
 };
 bool get_small_supports(uint32_t nbytes);
 size_t get_small_smem(uint32_t nbytes, bool verify);
 uint32_t get_small_region_entries(uint32_t nbytes);
 // requests resident on the device at once, < 0 on error
-int get_small_residency(uint32_t nbytes, bool verify, bool touch);
+int get_small_residency(uint32_t nbytes, bool verify, bool touch, bool freq);
 int launch_get_small(const GetJob &job, int device, cudaStream_t st);   // device: CUDA ordinal the launch runs on
+
+// CMB200_FREQ: the count-min sketch of cachemap_b200.h, 4 rows of 2^log2w 4-bit counters, 16 per word.
+// k_freq_add: one thread per request, +1 (saturating at 15) on the key's four counters of every request
+// with a valid address; k_freq_halve: every counter halved; k_freq_estimate: the least of a key's four.
+int launch_freq_add(unsigned long long *freq, uint32_t log2w, const unsigned long long *addr, const uint8_t *valid,
+    uint32_t n, cudaStream_t st);
+int launch_freq_halve(unsigned long long *freq, uint32_t log2w, cudaStream_t st);
+int launch_freq_estimate(const unsigned long long *freq, uint32_t log2w, const unsigned long long *addr, uint32_t n,
+    uint8_t *est, cudaStream_t st);
 
 int launch_fingerprint(const uint8_t *pages, uint64_t stride, uint32_t nbytes, uint32_t n,
     uint64_t *fps, cudaStream_t st);

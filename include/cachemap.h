@@ -21,6 +21,9 @@
  * With CMB200_EVICT=access, eviction (and demotion into a host tier) takes the pages read least
  * recently instead of those put longest ago: every page a get serves has its timestamp raised to the time
  * of the get (cachemap_b200.h, CMB200_TOUCH).  CMB200_EVICT=put, the default, is the reference's policy.
+ * With CMB200_ADMIT=freq, a page that would evict another is stored only if its key has been asked for
+ * more often than the victim's, counted by every get the GPU looks up (cachemap_b200.h, CMB200_FREQ), so a
+ * one-time scan of many pages does not flush the pages read often.  CMB200_ADMIT=all, the default, admits all.
  * struct cachemap is opaque (edgefs.c never looks inside it).
  */
 #ifndef CACHEMAP_H
@@ -136,6 +139,9 @@ uint64_t cachemap_rename(struct cachemap *cm, uint64_t nhid_from, uint64_t nhid_
 
 /* requests / hits counters (cachemap.c:176,181) and the engine under the map. */
 void cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hits);
+/* CMB200_ADMIT=freq: pages admitted over the victim they were paired with, and pages rejected (not stored,
+ * their key unset) since cachemap_create.  Both 0 without admission. */
+void cachemap_get_admission(struct cachemap *cm, uint64_t *admitted, uint64_t *rejected);
 struct cmb200_engine *cachemap_engine(struct cachemap *cm);
 /* Every engine under the map, in CMB200_DEVICES order (cachemap_engine is out[0]): stores up to max
  * of them in out and returns how many there are, 0 if none could be started.  Like cachemap_engine,

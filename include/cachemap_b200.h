@@ -55,6 +55,28 @@ typedef struct { uint64_t u; uint64_t l; } cmb200_addr;
  * touch that lands on a slot a put of the same key has just rewritten raises the new record's ts to about
  * now, and a touch that races a table rebuild may be lost. */
 #define CMB200_TOUCH 4u
+/* Frequency sketch for admission (the drop-in's CMB200_ADMIT=freq): the engine keeps a count-min sketch of
+ * how often each key is asked for, in HBM next to the key table.  4 rows of `width` 4-bit counters, 16 per
+ * 64-bit word, row r at words [r * width / 16, (r + 1) * width / 16); counter j of a row is bits
+ * 4 (j % 16) .. 4 (j % 16) + 3 of the row's word j / 16.  width = the power of two at or above capacity
+ * (table_slots / 4 when capacity is 0), at least 16: 2 x width bytes, allocated at engine creation before the
+ * arena is sized.  Key k's counter in row r is cmb200_freq_index(k, r, log2 width).
+ * Every get request with a valid address that cmb200_get_small, cmb200_get_small_begin / _end,
+ * cmb200_get_batch or cmb200_get_batch_dev looks up adds 1 to its key's four counters, saturating at 15:
+ * hits, misses, CMB200_BAD_ENTRY, _BAD_DECODE and _CORRUPT answers count, CMB200_INVALID ones do not.  Plain
+ * count-min, no conservative update, so the counters after n increments of a key are min(15, before + n) in
+ * any order.  Nothing else counts: lookups, cmb200_locate_batch, record reads, store scans, sampling,
+ * patches, renames, promotion, demotion, snapshots.
+ * Aging: the engine counts the valid requests of its launches on the host; the launch that takes the count
+ * to 10 x capacity (10 x width when capacity is 0) since the last halving halves every counter after its
+ * own get, on its own stream, and the count starts again from 0.  Every later get of the engine is ordered
+ * after that halving.  Two races are benign, because the sketch never decides which bytes a get returns:
+ * an increment of a get running concurrently on another stream can land on either side of a halving, and
+ * the lanes of concurrent gets increment the same words at once (each increment is one CAS on its word, so
+ * none is lost).  The sketch is not saved in snapshots or chain deltas: after a restart it starts empty.
+ * With the flag, cmb200_put_step, cmb200_import_records_dev and cmb200_open_peer fail (-1): the sketch counts
+ * the gets of one engine's own keys. */
+#define CMB200_FREQ 8u
 
 typedef struct cmb200_config {
 	int device;             /* CUDA ordinal, -1 = current device */
@@ -258,6 +280,35 @@ int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out);
  * (filemap.c:26-33).  This is the only definition; the drop-in and the snapshot code both call it.
  * (C99 inline: cachemap_api.c emits the external definition, so the library exports it as well.) */
 inline int cmb200_owner(uint64_t key, int g) { return (int)(((key >> 32) * (uint64_t)g) >> 32); }
+
+/* The counter of store key `key` in row `row` (0..3) of a CMB200_FREQ sketch of 2^log2_width counters per
+ * row (4 <= log2_width <= 32): multiply-shift of the key by one fixed odd constant per row, top bits of the
+ * product.  The only definition; the kernels, the drop-in and the tests' models use it.  (C99 inline, as
+ * cmb200_owner; host and device code under nvcc.) */
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+inline uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width) {
+	const uint64_t c = row == 0 ? 0x9E3779B97F4A7C15ull : row == 1 ? 0xC2B2AE3D27D4EB4Full
+	    : row == 2 ? 0x165667B19E3779F9ull : 0xD6E8FEB86659FD93ull;
+	return (uint32_t)((key * c) >> (64 - log2_width));
+}
+
+/* ---- frequency sketch (CMB200_FREQ) ----------------------------------------------------------------
+ * cmb200_freq_estimate: est_out[i] = the estimate of addr[i]'s key, the least of its four counters (0..15),
+ * computed in one kernel on the engine's stream after every halving enqueued so far.  Counts nothing.
+ * cmb200_freq_read: copies the sketch (2 x width bytes, the layout of CMB200_FREQ) to host memory `out`;
+ * `bytes` must be that size.  Waits for every get and halving enqueued before the call.
+ * cmb200_freq_stats: the sketch's width, its halving period (increments), the increments counted so far,
+ * those since the last halving, and the halvings.
+ * All three fail (-1) on an engine created without CMB200_FREQ. */
+struct cmb200_freq_stats {
+	uint64_t width, period;
+	uint64_t increments, since_halving, halvings;
+};
+int cmb200_freq_estimate(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint8_t *est_out);
+int cmb200_freq_read(cmb200_engine *e, void *out, size_t bytes);
+int cmb200_freq_stats(cmb200_engine *e, struct cmb200_freq_stats *out);
 
 /* cmb200_save / cmb200_load over g engines that split the keys by cmb200_owner.  The file is the one
  * cmb200_save writes: one header, then the records of engine 0, 1, ...  Each engine's section is a
