@@ -24,6 +24,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
     "cachemap_pread", "cachemap_pwrite", "cachemap_rename", "cachemap_get_admission",
+    "cachemap_load_progress",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -45,7 +46,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_verify_stats", "cmb200_verify_store", "cmb200_snapshot_begin", "cmb200_snapshot_finish",
     "cmb200_chain_begin", "cmb200_load_chain", "cmb200_invalidate", "cmb200_patch_batch",
     "cmb200_rename", "cmb200_rename_set", "cmb200_freq_index", "cmb200_freq_estimate", "cmb200_freq_read",
-    "cmb200_freq_stats",
+    "cmb200_freq_stats", "cmb200_load_open", "cmb200_load_step", "cmb200_load_total", "cmb200_load_close",
 ]
 
 
@@ -107,6 +108,7 @@ def lib() -> C.CDLL:
         "cachemap_get_batch_dev": (None, [vp, u64, vp, vp, vp, vp, vp]),
         "cachemap_get_counters": (None, [vp, vp, vp]),
         "cachemap_get_admission": (None, [vp, vp, vp]),
+        "cachemap_load_progress": (i32, [vp, vp, vp]),
         "cachemap_engine": (vp, [vp]),
         "cachemap_engines": (i32, [vp, vp, i32]),
         "cachemap_checkpoint": (i32, [vp]),
@@ -194,6 +196,10 @@ def lib() -> C.CDLL:
         "cmb200_snapshot_finish": (i32, [vp, vp]),
         "cmb200_chain_begin": (vp, [vp, i32, C.c_char_p, i32]),
         "cmb200_load_chain": (i32, [vp, i32, C.c_char_p, vp, vp]),
+        "cmb200_load_open": (vp, [vp, i32, C.c_char_p]),
+        "cmb200_load_step": (i32, [vp, sz, vp]),
+        "cmb200_load_total": (u64, [vp]),
+        "cmb200_load_close": (i32, [vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -747,6 +753,39 @@ def load_chain(handles, base_path: str):
     return n.value, k.value
 
 
+class Loader:
+    """cmb200_load_open over engine handles: the load of load_chain in steps, while the engines serve.
+    step() stores at most max_records more records (0: all that are left) and returns True while records
+    are left; close() frees the loader -> (records loaded, deltas applied)."""
+
+    def __init__(self, handles, base_path: str):
+        arr, g = _handles(handles)
+        self.h = lib().cmb200_load_open(arr, g, base_path.encode())
+        if not self.h:
+            raise RuntimeError(f"cmb200_load_open failed: {last_error()}")
+        self.loaded = 0
+
+    @property
+    def total(self) -> int:
+        """Records the files hold by their headers, an upper bound of what the load puts."""
+        return int(lib().cmb200_load_total(self.h))
+
+    def step(self, max_records: int = 0) -> bool:
+        n = C.c_uint64(0)
+        rc = lib().cmb200_load_step(self.h, max_records, C.byref(n))
+        self.loaded = n.value
+        if rc < 0:
+            raise RuntimeError(f"cmb200_load_step failed: {last_error()}")
+        return rc == 1
+
+    def close(self):
+        h, self.h = self.h, None
+        n = C.c_uint64(0)
+        k = C.c_uint32(0)
+        _check(lib().cmb200_load_close(h, C.byref(n), C.byref(k)), "cmb200_load_close")
+        return n.value, k.value
+
+
 class Cachemap:
     """The reference's cachemap API (cachemap/cachemap.h:33-47) plus the batch extension.  The engine
     starts on first use and reads its settings from the environment then, the host tier included
@@ -846,6 +885,13 @@ class Cachemap:
         a, r = C.c_uint64(), C.c_uint64()
         lib().cachemap_get_admission(self.h, C.byref(a), C.byref(r))
         return a.value, r.value
+
+    def load_progress(self):
+        """cachemap_load_progress -> (loading, records loaded, records the files hold): loading is True while
+        a background load (CMB200_LOAD=background) runs."""
+        a, t = C.c_uint64(), C.c_uint64()
+        r = lib().cachemap_load_progress(self.h, C.byref(a), C.byref(t))
+        return bool(r), a.value, t.value
 
     def engine_handle(self) -> int:
         return int(lib().cachemap_engine(self.h) or 0)

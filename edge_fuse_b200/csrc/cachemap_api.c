@@ -72,6 +72,10 @@ extern uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width);
 #pragma weak cmb200_rename_set
 #pragma weak cmb200_patch_batch
 #pragma weak cmb200_freq_estimate
+#pragma weak cmb200_load_open
+#pragma weak cmb200_load_step
+#pragma weak cmb200_load_total
+#pragma weak cmb200_load_close
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -81,6 +85,7 @@ extern uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width);
 #define PNUM_SHIFT 44           /* cachemap.c:155 */
 #define PROMOTE_EVERY_MS 100    /* CMB200_TIER_PROMOTE: at most one promotion round this often */
 #define MAX_DEVICES 64          /* engines one map may own (CMB200_DEVICES) */
+#define LOAD_STEP 4096          /* CMB200_LOAD=background: records per step of the loader thread */
 
 enum req_kind { REQ_GET, REQ_UNSET };
 enum wb_state { WB_FREE = 0, WB_FILLING, WB_READY, WB_FLUSHING };
@@ -185,6 +190,16 @@ struct filemap {
 	pthread_cond_t ckpt_cv;
 	pthread_t ckpt_thread;
 	int ckpt_started, ckpt_stop;
+	/* CMB200_LOAD=background: the loader thread runs the steps of `loader` while the map serves.  loading
+	 * is 1 from the load's open until its close (under load_mu, read atomically); load_cv is broadcast when
+	 * it ends.  load_chain: the load stands for cmb200_load_chain (chain_deltas follows it) rather than
+	 * cmb200_load_set. */
+	cmb200_loader *loader;
+	pthread_t load_thread;
+	int load_started, loading, load_chain;
+	uint64_t load_loaded, load_total;       /* (atomic) */
+	pthread_mutex_t load_mu;
+	pthread_cond_t load_cv;
 };
 
 #define SNAPSHOT_NAME "cachemap_b200.snap"
@@ -256,6 +271,7 @@ filemap_device_list(int *out)
 
 static void *filemap_flusher(void *arg);
 static void *filemap_checkpointer(void *arg);
+static void *filemap_loader(void *arg);
 
 static void
 fm_dev_free(struct fm_dev *d)
@@ -317,6 +333,21 @@ admit_flags(int warn)
 		return CMB200_FREQ;
 	if (warn)
 		fprintf(stderr, "cachemap_b200: CMB200_ADMIT=%s is neither freq nor all; admitting every page\n", v);
+	return 0;
+}
+
+/* CMB200_LOAD: how the first call after cachemap_create reads the cache directory back.  "wait" (or unset):
+ * the call returns once every record is in HBM.  "background": the engines serve at once while a thread
+ * loads the file in steps (filemap_loader).  Any other value warns and waits.  1 = background. */
+static int
+load_background(void)
+{
+	const char *v = getenv("CMB200_LOAD");
+	if (!v || !*v || strcmp(v, "wait") == 0)
+		return 0;
+	if (strcmp(v, "background") == 0)
+		return 1;
+	fprintf(stderr, "cachemap_b200: CMB200_LOAD=%s is neither wait nor background; loading before serving\n", v);
 	return 0;
 }
 
@@ -447,7 +478,19 @@ filemap_engine_ready(struct filemap *m)
 				snprintf(d1, sizeof(d1), "%s.d1", snap);
 				/* a chain next to the base is never ignored, whatever CMB200_CHECKPOINT_DELTAS says now;
 				 * a base whose deltas do not match it loads alone */
-				if (cmb200_load_chain && (m->checkpoint_deltas > 0 || access(d1, R_OK) == 0)) {
+				const int chain = cmb200_load_chain && (m->checkpoint_deltas > 0 || access(d1, R_OK) == 0);
+				if (load_background() && cmb200_load_open && cmb200_load_step && cmb200_load_total && cmb200_load_close) {
+					/* the loader thread starts with the flushers below */
+					m->loader = cmb200_load_open(m->engs, g, snap);
+					if (!m->loader)
+						fprintf(stderr, "cachemap_b200: %s: no background load (%s); loading before serving\n", snap,
+						    cmb200_last_error());
+				}
+				if (m->loader) {
+					m->load_chain = chain;
+					m->load_total = cmb200_load_total(m->loader);
+					m->loading = 1;
+				} else if (chain) {
 					if (cmb200_load_chain(m->engs, g, snap, &got, &k) != 0)
 						fprintf(stderr, "cachemap_b200: %s ignored: %s\n", snap, cmb200_last_error());
 					else
@@ -464,6 +507,12 @@ filemap_engine_ready(struct filemap *m)
 					d->wb_started = 1;
 				else
 					d->wb_n = 0;
+			}
+			if (m->loader) {
+				if (pthread_create(&m->load_thread, NULL, filemap_loader, m) == 0)
+					m->load_started = 1;
+				else
+					filemap_loader(m);      /* no thread: the load runs here, as a blocking one */
 			}
 			if (m->persist && m->checkpoint_sec > 0 &&
 			    pthread_create(&m->ckpt_thread, NULL, filemap_checkpointer, m) == 0)
@@ -497,6 +546,8 @@ filemap_create(char *destdir, uint64_t n, int compress_accel, int pshift)
 	pthread_mutex_init(&m->snap_mu, NULL);
 	pthread_mutex_init(&m->ckpt_mu, NULL);
 	pthread_cond_init(&m->ckpt_cv, NULL);
+	pthread_mutex_init(&m->load_mu, NULL);
+	pthread_cond_init(&m->load_cv, NULL);
 	return m;
 }
 
@@ -591,9 +642,49 @@ filemap_save(struct filemap *m, int tick)
 	return rc;
 }
 
+/* CMB200_LOAD=background: runs the load's steps to the end, then closes it.  The engines refuse
+ * snapshots while the load is open; chain_deltas takes the load's outcome under snap_mu, as a load before
+ * serving sets it. */
+static void *
+filemap_loader(void *arg)
+{
+	struct filemap *m = arg;
+	uint64_t loaded = 0, records = 0;
+	uint32_t k = 0;
+	int r;
+	char snap[2200];
+	filemap_snapshot_path(m, snap, sizeof(snap));
+	while ((r = cmb200_load_step(m->loader, LOAD_STEP, &loaded)) == 1)
+		__atomic_store_n(&m->load_loaded, loaded, __ATOMIC_RELAXED);
+	__atomic_store_n(&m->load_loaded, loaded, __ATOMIC_RELAXED);
+	if (r < 0)
+		fprintf(stderr, "cachemap_b200: %s: the load stopped: %s\n", snap, cmb200_last_error());
+	pthread_mutex_lock(&m->snap_mu);
+	if (cmb200_load_close(m->loader, &records, &k) == 0 && r == 0 && m->load_chain)
+		m->chain_deltas = (int)k;
+	pthread_mutex_unlock(&m->snap_mu);
+	m->loader = NULL;
+	pthread_mutex_lock(&m->load_mu);
+	__atomic_store_n(&m->loading, 0, __ATOMIC_RELEASE);
+	pthread_cond_broadcast(&m->load_cv);
+	pthread_mutex_unlock(&m->load_mu);
+	return NULL;
+}
+
+/* Waits until a background load has ended. */
+static void
+filemap_load_wait(struct filemap *m)
+{
+	pthread_mutex_lock(&m->load_mu);
+	while (m->loading)
+		pthread_cond_wait(&m->load_cv, &m->load_mu);
+	pthread_mutex_unlock(&m->load_mu);
+}
+
 /* CMB200_CHECKPOINT_SEC: every checkpoint_sec seconds, a snapshot if puts have landed since the last
  * one.  The engines list their records under their locks and write them outside, so neither the
- * flushers nor the callers of the map wait for the file. */
+ * flushers nor the callers of the map wait for the file.  No tick while a background load runs: a file
+ * of the half-loaded store would replace the one it is loaded from with less. */
 static void *
 filemap_checkpointer(void *arg)
 {
@@ -608,7 +699,8 @@ filemap_checkpointer(void *arg)
 		if (m->ckpt_stop)
 			break;
 		pthread_mutex_unlock(&m->ckpt_mu);
-		if (__atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED) != __atomic_load_n(&m->puts_saved, __ATOMIC_RELAXED))
+		if (!__atomic_load_n(&m->loading, __ATOMIC_ACQUIRE) &&
+		    __atomic_load_n(&m->puts_seen, __ATOMIC_RELAXED) != __atomic_load_n(&m->puts_saved, __ATOMIC_RELAXED))
 			filemap_save(m, 1);
 		pthread_mutex_lock(&m->ckpt_mu);
 	}
@@ -661,6 +753,10 @@ filemap_free(struct filemap *m)
 		pthread_mutex_unlock(&m->ckpt_mu);
 		pthread_join(m->ckpt_thread, NULL);     /* a save in progress ends first */
 	}
+	/* a background load runs to its end: the base written below must hold the pages not loaded yet, and
+	 * not those this session removed */
+	if (m->load_started)
+		pthread_join(m->load_thread, NULL);
 	for (int i = 0; i < m->g; i++) {
 		struct fm_dev *d = m->dev[i];
 		if (!d->wb_started)
@@ -685,6 +781,8 @@ filemap_free(struct filemap *m)
 	for (int i = 0; i < m->g; i++)
 		fm_dev_free(m->dev[i]);
 	pthread_mutex_destroy(&m->snap_mu);
+	pthread_cond_destroy(&m->load_cv);
+	pthread_mutex_destroy(&m->load_mu);
 	pthread_cond_destroy(&m->ckpt_cv);
 	pthread_mutex_destroy(&m->ckpt_mu);
 	pthread_mutex_destroy(&m->evict_mu);
@@ -2609,8 +2707,21 @@ cachemap_checkpoint(struct cachemap *cm)
 {
 	if (!filemap_engine_ready(cm->pages))
 		return -1;
+	filemap_load_wait(cm->pages);
 	filemap_drain(cm->pages);
 	return filemap_save(cm->pages, 0);
+}
+
+int
+cachemap_load_progress(struct cachemap *cm, uint64_t *loaded, uint64_t *total)
+{
+	struct filemap *m = cm->pages;
+	const int loading = __atomic_load_n(&m->loading, __ATOMIC_ACQUIRE);
+	if (loaded)
+		*loaded = __atomic_load_n(&m->load_loaded, __ATOMIC_RELAXED);
+	if (total)
+		*total = __atomic_load_n(&m->load_total, __ATOMIC_RELAXED);
+	return loading;
 }
 
 void

@@ -15,10 +15,12 @@
 #include <condition_variable>
 #include <deque>
 #include <dirent.h>
+#include <map>
 #include <mutex>
 #include <set>
 #include <shared_mutex>
 #include <sched.h>
+#include <sys/stat.h>
 #include <string>
 #include <new>
 #include <thread>
@@ -145,6 +147,48 @@ static int table_alloc(TableMem &m, uint64_t cap, bool fp, bool fp_tag, bool ckp
 	if (ckpt) CMB_CHECK(cudaMemsetAsync(m.ckpt, 0, n * CKPT_WORDS * 4, st));
 	return 0;
 }
+
+struct AddrHash {
+	size_t operator()(const std::pair<uint64_t, uint64_t> &a) const { return (size_t)(a.first * 0x9E3779B97F4A7C15ull ^ a.second); }
+};
+typedef std::unordered_set<std::pair<uint64_t, uint64_t>, AddrHash> AddrSet;
+
+// The removals made while a background load (cmb200_load_open) is open on an engine: a record of the
+// load whose key, address or interval is here was removed, moved or could not be patched since the load
+// opened, so the load passes it over.  Removals are the one change the load's sequence floor
+// (k_upsert_floor) cannot see.  Under the engine's mu.
+struct LoadFence {
+	std::atomic<bool> open{false};                        // changes under mu; cmb200_put_step reads it without
+	std::unordered_set<uint64_t> keys;                    // cmb200_unset_batch deletes by key; a host-tier lap retires
+	                                                      // the records it overwrites
+	AddrSet addrs;                                        // cmb200_patch_batch's unpatched addresses
+	std::map<std::pair<uint64_t, uint64_t>, uint64_t> spans;   // {u, l_first} -> l_last, disjoint
+	bool empty() const { return keys.empty() && addrs.empty() && spans.empty(); }
+	void clear() { open = false; keys.clear(); addrs.clear(); spans.clear(); }
+	LoadFence() = default;
+	LoadFence(const LoadFence &) = delete;
+	void add_span(uint64_t u, uint64_t lo, uint64_t hi) {
+		// merged with every span it overlaps or touches, so that one lookup answers a query
+		auto it = spans.lower_bound(std::make_pair(u, lo));
+		if (it != spans.begin()) {
+			auto p = std::prev(it);
+			if (p->first.first == u && (p->second >= lo || p->second + 1 == lo)) it = p;
+		}
+		while (it != spans.end() && it->first.first == u && (it->first.second <= hi || it->first.second == hi + 1)) {
+			lo = std::min(lo, it->first.second);
+			hi = std::max(hi, it->second);
+			it = spans.erase(it);
+		}
+		spans.emplace(std::make_pair(u, lo), hi);
+	}
+	bool holds(uint64_t u, uint64_t l, uint64_t key) const {
+		if (keys.count(key) || addrs.count(std::make_pair(u, l))) return true;
+		auto it = spans.upper_bound(std::make_pair(u, l));
+		if (it == spans.begin()) return false;
+		--it;
+		return it->first.first == u && it->second >= l;
+	}
+};
 
 struct cmb200_engine {
 	int device = 0;
@@ -318,6 +362,7 @@ struct cmb200_engine {
 		uint32_t k_next = 0;
 		unsigned long long w_next = 0;
 	} chain;
+	LoadFence fence;                     // an open cmb200_loader's removals (under mu)
 };
 
 // CMB200_TOUCH: the stamp a get raises its hits' ts to, taken at launch from the clock the drop-in's puts
@@ -700,6 +745,11 @@ static int freq_refuses(cmb200_engine *e, const char *what) {
 // The multi-GPU calls and the host tier exclude each other: the exchange records and peer reads know
 // arena locations only.
 static int multi_gpu_call(cmb200_engine *e, const char *what) {
+	if (e->fence.open) {
+		// a stream order would set seq below an open load's floor, and the file would win over later puts
+		snprintf(g_err, sizeof(g_err), "%s: not available while a load into the engine is open (cmb200_load_open)", what);
+		return -1;
+	}
 	if (e->tier.host) {
 		snprintf(g_err, sizeof(g_err), "%s: not available on an engine with a host tier", what);
 		return -1;
@@ -1156,6 +1206,12 @@ extern "C" int cmb200_open_peer(cmb200_engine *e, uint32_t rank, const void *han
 extern "C" int cmb200_unset_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr) {
 	std::lock_guard<std::mutex> g(e->mu);
 	CMB_CHECK(cudaSetDevice(e->device));
+	if (e->fence.open)
+		for (size_t i = 0; i < n; i++) {
+			uint64_t key;
+			FNV_hash(&addr[i], 16, &key);
+			e->fence.keys.insert(key);
+		}
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
 		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
@@ -1543,6 +1599,12 @@ static cmb200_snapshot *snapshot_start(cmb200_engine *const *engines, int g, con
 	for (int i = 0; i < g && rc == 0; i++) {
 		cmb200_engine *e = engines[i];
 		std::lock_guard<std::mutex> lk(e->mu);
+		if (e->fence.open) {
+			// a file of a half-loaded store would replace the one it is loaded from with less
+			set_error_msg("cmb200_snapshot_begin: a load into this engine is open (cmb200_load_open)");
+			rc = -1;
+			break;
+		}
 		if (i == 0) s->h.flags = e->table.fp ? 1u : 0u;
 		unsigned long long c[8];
 		// live_records synchronises the stream first: every put enqueued before now is listed
@@ -1649,6 +1711,7 @@ extern "C" int cmb200_save(cmb200_engine *e, const char *path, uint64_t *records
 }
 
 static int demote_arena_all(cmb200_engine *e);
+static int compact_locked(cmb200_engine *e, uint64_t *reclaimed_out);
 
 // One engine's share of a load: its records are staged in page-locked memory until the batch is full
 // (<= max_batch records and <= one page-ring buffer of bytes), then put in as one upsert + k_restore.
@@ -1660,6 +1723,8 @@ struct LoadBatch {
 	std::vector<cmb200_addr> addr;
 	DevMem<unsigned long long> d_off;
 	DevMem<uint64_t> d_fp;
+	// a background load's batch (floor != 0): the sequence of its next record, below the engine's floor
+	unsigned long long seq = 0, floor = 0;
 	int setup(cmb200_engine *eng) {
 		e = eng;
 		CMB_CHECK(cudaSetDevice(e->device));
@@ -1674,49 +1739,69 @@ struct LoadBatch {
 // memory of e, 16-byte aligned) are stored at addr[i] with ts[i] and fingerprint fps[i] ({0, 0} or
 // fps = nullptr: none), as if put in this order: k_upsert claims the keys and raises seq, k_restore writes
 // each record under its new prefix and rebuilds its parse checkpoints.  A record the arena has no room
-// for is dropped, as a put is.  Enqueued on e->st.  (e->mu held; m <= max_batch)
+// for is dropped, as a put is.  The records take sequences seq, seq + stride, ... and seq advances past
+// them: e->seq for a rename or a snapshot load.  floor != 0: a background load's records, claimed by
+// k_upsert_floor, which passes over the keys changed since the load opened.  Enqueued on e->st.
+// (e->mu held; m <= max_batch)
 static int restore_records(cmb200_engine *e, const uint8_t *blob, const unsigned long long *addr,
-    const unsigned long long *ts, const unsigned long long *off, const uint64_t *fps, size_t m) {
-	if (launch_upsert(e->table, addr, nullptr, (uint32_t)m, e->seq, e->seq_stride, e->d_slot, e->st)) return -1;
+    const unsigned long long *ts, const unsigned long long *off, const uint64_t *fps, size_t m,
+    unsigned long long &seq, unsigned long long floor = 0) {
+	if (floor ? launch_upsert_floor(e->table, addr, (uint32_t)m, seq, e->seq_stride, floor, e->d_slot, e->st)
+	          : launch_upsert(e->table, addr, nullptr, (uint32_t)m, seq, e->seq_stride, e->d_slot, e->st)) return -1;
 	EncodeJob job{};
 	job.n = (uint32_t)m; job.nbytes = e->bsize;
 	job.slot_idx = e->d_slot; job.addr = addr; job.ts = ts;
-	job.seq0 = e->seq; job.seq_stride = e->seq_stride;
+	job.seq0 = seq; job.seq_stride = e->seq_stride;
 	job.table = e->table; job.arena = e->arena;
 	if (launch_restore(job, blob, off, fps, e->bsize, e->st)) return -1;
-	e->seq += (unsigned long long)m * e->seq_stride;
+	seq += (unsigned long long)m * e->seq_stride;
 	e->stats.kernel_launches += 2;
 	return 0;
 }
 
 // Puts the staged records into their engine as if they had been put in file order.  Returns how many
-// (>= 0) or -1.
+// were handed to the engine (>= 0) or -1.  A background load's batch first leaves out the records its
+// engine's fence holds, and compacts when the garbage covers what the slice lacks.
 static long long load_flush(LoadBatch &b, bool with_fp) {
 	if (b.m == 0) return 0;
 	cmb200_engine *e = b.e;
 	std::lock_guard<std::mutex> g(e->mu);
 	CMB_CHECK(cudaSetDevice(e->device));
-	const size_t m = b.m;
+	size_t m = b.m;
+	if (b.floor && !e->fence.empty()) {
+		size_t k = 0;
+		for (size_t j = 0; j < m; j++) {
+			uint64_t key;
+			FNV_hash(&b.addr[j], 16, &key);
+			if (e->fence.holds(b.addr[j].u, b.addr[j].l, key)) continue;
+			b.addr[k] = b.addr[j]; b.off[k] = b.off[j]; b.ts[k] = b.ts[j];
+			b.fps[2 * k] = b.fps[2 * j]; b.fps[2 * k + 1] = b.fps[2 * j + 1];
+			k++;
+		}
+		m = k;
+	}
+	b.m = 0;
+	if (m == 0) { b.used = 0; return 0; }
 	if (e->tier.host) {
 		unsigned long long c[8];
 		if (read_counters(e, c)) return -1;
 		if (c[2] + b.used > e->arena.size && demote_arena_all(e)) return -1;
+	} else if (b.floor) {
+		unsigned long long c[8];
+		if (read_counters(e, c)) return -1;
+		if (c[2] + b.used > e->arena.size && c[3] >= c[2] + b.used - e->arena.size && compact_locked(e, nullptr)) return -1;
 	}
 	CMB_CHECK(cudaMemcpyAsync(e->d_pages[0], b.blob, b.used, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(e->d_addr, b.addr.data(), m * 16, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(e->d_ts, b.ts.data(), m * 8, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(b.d_off, b.off.data(), m * 8, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(b.d_fp, b.fps.data(), m * 16, cudaMemcpyHostToDevice, e->st));
-	if (restore_records(e, e->d_pages[0], e->d_addr, e->d_ts, b.d_off, with_fp ? (uint64_t *)b.d_fp : nullptr, m)) return -1;
+	if (restore_records(e, e->d_pages[0], e->d_addr, e->d_ts, b.d_off, with_fp ? (uint64_t *)b.d_fp : nullptr, m,
+	    b.floor ? b.seq : e->seq, b.floor)) return -1;
 	CMB_CHECK(cudaStreamSynchronize(e->st));
-	b.m = 0; b.used = 0;
+	b.used = 0;
 	return (long long)m;
 }
-
-struct AddrHash {
-	size_t operator()(const std::pair<uint64_t, uint64_t> &a) const { return (size_t)(a.first * 0x9E3779B97F4A7C15ull ^ a.second); }
-};
-typedef std::unordered_set<std::pair<uint64_t, uint64_t>, AddrHash> AddrSet;
 
 // Opens a snapshot file (a base) for a load into g engines and reads its header.  nullptr on failure
 // (error set).
@@ -1864,77 +1949,209 @@ static bool delta_beyond(const char *base_path, uint32_t k) {
 	return found;
 }
 
-extern "C" int cmb200_load_chain(cmb200_engine *const *engines, int g, const char *base_path, uint64_t *records_out,
-    uint32_t *deltas_out) {
-	if (records_out) *records_out = 0;
-	if (deltas_out) *deltas_out = 0;
-	if (g < 1 || !engines || !base_path) { set_error_msg("cmb200_load_chain: no engines"); return -1; }
+// ---- background loads (cmb200_load_open / _step / _close) ----
+// A load of a chain in steps, while the engines serve.  The files and their order are cmb200_load_chain's:
+// newest first, each address decided by the newest file that names it.  What the engines are asked to do
+// while the load is open wins over the files:
+//   - puts, patch hits and renamed records claim their slots with k_upsert at sequences >= the engine's
+//     floor, which open sets past every sequence the load's own records take; k_upsert_floor passes over a
+//     key whose slot was written at or above the floor;
+//   - removals leave no slot to compare, so they go to the engine's fence, which each slice consults
+//     under the engine's lock before it is staged.
+struct cmb200_loader {
+	std::vector<cmb200_engine *> engines;
+	std::string base_path;
 	SnapHeader h{};
-	FILE *base = open_snapshot(engines, g, base_path, h);
-	if (!base) return -1;
-	const uint64_t id = snap_chain_id(h);
-	std::vector<FILE *> ds;
+	FILE *base = nullptr;
+	uint64_t id = 0, total = 0, before = 0, loaded = 0;
+	std::vector<FILE *> ds;                              // the valid run of deltas, opened by the first step
 	std::vector<DeltaHeader> dhs;
-	for (uint32_t k = 1; id != 0; k++) {
-		DeltaHeader dh{};
-		FILE *f = open_delta(std::string(base_path) + ".d" + std::to_string(k), id, k, h.pshift, engines[0]->bsize, dh);
-		if (!f) break;
-		ds.push_back(f); dhs.push_back(dh);
-	}
-	uint64_t before = 0;
-	for (int i = 0; i < g; i++) before += cmb200_entries(engines[i]);
-	std::vector<LoadBatch> bs;
-	uint64_t loaded = 0;
-	int rc = load_setup(bs, engines, g);
-	// newest first: an address a newer file names (a record or a tombstone) is decided there, so every
-	// record is put once, and none an older file names in vain takes arena space
-	AddrSet decided;
+	bool checked = false, done = false;
+	int rc = 0;
+	size_t file = 0;                                     // files left, newest first: ds[file - 1], then the base
+	uint64_t left = 0;                                   // records left in the file being read
+	bool started = false;                                // its tombstones are read and `left` is set
 	std::vector<ulonglong2> tombs;
-	for (size_t j = ds.size(); j-- > 0 && rc == 0;) {
-		FILE *f = ds[j];
-		const DeltaHeader &dh = dhs[j];
-		tombs.resize(dh.tombstones);
-		if (dh.tombstones && fread(tombs.data(), 16, tombs.size(), f) != tombs.size()) { rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break; }
-		rc = load_records(f, dh.records, bs, g, dh.flags & 1u, &decided, &decided, &loaded);
-		if (rc == 0) rc = load_flush_all(bs, dh.flags & 1u, &loaded);
-		// the records of a delta apply after its tombstones, so its records decide first
-		for (const ulonglong2 &a : tombs) decided.insert(std::make_pair((uint64_t)a.x, (uint64_t)a.y));
+	AddrSet decided;
+	std::vector<LoadBatch> bs;
+	~cmb200_loader() {
+		for (FILE *f : ds) fclose(f);
+		if (base) fclose(base);
 	}
-	if (rc == 0) rc = load_records(base, h.records, bs, g, h.flags & 1u, &decided, nullptr, &loaded);
-	if (rc == 0) rc = load_flush_all(bs, h.flags & 1u, &loaded);
-	for (FILE *f : ds) fclose(f);
-	fclose(base);
-	if (rc) return -1;
-	// The engines continue the chain only if they hold exactly the store it describes: they were empty
-	// and every record put is live (none dropped for lack of space, none retired by a host-tier lap),
-	// and no delta file lies beyond the run (a tick that continued it would leave that file in a valid
-	// position).  Otherwise they hold no chain state, and the next tick writes a base.
-	bool whole = id != 0 && before == 0 && !delta_beyond(base_path, (uint32_t)ds.size());
-	uint64_t live = 0;
-	for (int i = 0; i < g && rc == 0; i++) {
+};
+
+// Closes the fences of engines[0 .. n).
+static void load_fences_close(cmb200_engine *const *engines, int n) {
+	for (int i = 0; i < n; i++) {
+		std::lock_guard<std::mutex> lk(engines[i]->mu);
+		engines[i]->fence.clear();
+	}
+}
+
+extern "C" cmb200_loader *cmb200_load_open(cmb200_engine *const *engines, int g, const char *base_path) {
+	if (g < 1 || !engines || !base_path) { set_error_msg("cmb200_load_open: no engines"); return nullptr; }
+	std::vector<cmb200_engine *> order(engines, engines + g);
+	std::sort(order.begin(), order.end());
+	if (std::adjacent_find(order.begin(), order.end()) != order.end()) { set_error_msg("cmb200_load_open: an engine is listed twice"); return nullptr; }
+	cmb200_loader *l = new (std::nothrow) cmb200_loader();
+	if (!l) { set_error_msg("cmb200_load_open: out of memory"); return nullptr; }
+	l->engines.assign(engines, engines + g);
+	l->base_path = base_path;
+	l->base = open_snapshot(engines, g, base_path, l->h);
+	if (!l->base) { delete l; return nullptr; }
+	l->id = snap_chain_id(l->h);
+	// an upper bound of the records the load puts, from the headers alone: the base's and those of the
+	// deltas whose headers name this chain in sequence (the first step checks the deltas whole)
+	// A header's count is bounded by its file's size (a record takes at least its header and a 24-byte
+	// prefix), so that a corrupt or foreign header cannot push the engines' sequence numbers arbitrarily far.
+	const auto bounded = [](uint64_t records, FILE *f, uint64_t header) {
+		struct stat st;
+		const uint64_t size = fstat(fileno(f), &st) == 0 ? (uint64_t)st.st_size : 0;
+		const uint64_t most = size > header ? (size - header) / (sizeof(SnapRecord) + 24) : 0;
+		return records < most ? records : most;
+	};
+	l->total = bounded(l->h.records, l->base, sizeof(SnapHeader));
+	for (uint32_t k = 1; l->id != 0; k++) {
+		DeltaHeader dh{};
+		FILE *f = fopen((l->base_path + ".d" + std::to_string(k)).c_str(), "rb");
+		const bool ok = f && fread(&dh, sizeof(dh), 1, f) == 1 && memcmp(dh.magic, "CMB200D1", 8) == 0 &&
+		    dh.version == 1 && dh.chain == l->id && dh.index == k;
+		if (ok) l->total += bounded(dh.records, f, sizeof(dh));
+		if (f) fclose(f);
+		if (!ok) break;
+	}
+	for (int i = 0; i < g; i++) l->before += cmb200_entries(engines[i]);
+	if (load_setup(l->bs, engines, g)) { delete l; return nullptr; }
+	for (int i = 0; i < g; i++) {
 		cmb200_engine *e = engines[i];
 		std::lock_guard<std::mutex> lk(e->mu);
+		const char *why = e->multi_gpu ? "cmb200_load_open: not available after a multi-GPU call (the index holds other ranks' records)"
+		    : e->fence.open ? "cmb200_load_open: a load into this engine is open already"
+		    : (l->total + 1) > (~0ull - e->seq) / e->seq_stride ? "cmb200_load_open: the files name more records than the engine has sequence numbers left"
+		    : nullptr;
+		if (why) {
+			set_error_msg(why);
+			load_fences_close(engines, i);
+			delete l;
+			return nullptr;
+		}
+		// the load's records take the sequences [seq, floor); every later write of a slot is above them
+		l->bs[i].seq = e->seq;
+		e->seq += (l->total + 1) * e->seq_stride;
+		l->bs[i].floor = e->seq;
+		e->fence.open = true;
+	}
+	return l;
+}
+
+extern "C" uint64_t cmb200_load_total(const cmb200_loader *l) { return l ? l->total : 0; }
+
+extern "C" int cmb200_load_step(cmb200_loader *l, size_t max_records, uint64_t *loaded_out) {
+	if (!l) { set_error_msg("cmb200_load_step: no loader"); return -1; }
+	if (l->rc == 0 && !l->done && !l->checked) {
+		// the whole check of each delta (every record header and the file's length) before any is applied
+		for (uint32_t k = 1; l->id != 0; k++) {
+			DeltaHeader dh{};
+			FILE *f = open_delta(l->base_path + ".d" + std::to_string(k), l->id, k, l->h.pshift, l->engines[0]->bsize, dh);
+			if (!f) break;
+			l->ds.push_back(f); l->dhs.push_back(dh);
+		}
+		l->file = l->ds.size() + 1;
+		l->checked = true;
+	}
+	const int g = (int)l->engines.size();
+	size_t budget = max_records ? max_records : SIZE_MAX;
+	while (l->rc == 0 && !l->done && budget > 0) {
+		const bool delta = l->file > 1;
+		FILE *f = delta ? l->ds[l->file - 2] : l->base;
+		const bool with_fp = (delta ? l->dhs[l->file - 2].flags : l->h.flags) & 1u;
+		if (!l->started) {
+			if (delta) {
+				const DeltaHeader &dh = l->dhs[l->file - 2];
+				l->tombs.resize(dh.tombstones);
+				if (dh.tombstones && fread(l->tombs.data(), 16, l->tombs.size(), f) != l->tombs.size()) {
+					l->rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
+				}
+				l->left = dh.records;
+			} else {
+				l->left = l->h.records;
+			}
+			l->started = true;
+		}
+		const uint64_t n = l->left < budget ? l->left : (uint64_t)budget;
+		l->rc = load_records(f, n, l->bs, g, with_fp, &l->decided, delta ? &l->decided : nullptr, &l->loaded);
+		l->left -= n;
+		budget -= (size_t)n;
+		if (l->rc == 0 && (l->left == 0 || budget == 0)) l->rc = load_flush_all(l->bs, with_fp, &l->loaded);
+		if (l->rc || l->left) break;
+		// the records of a delta apply after its tombstones, so its records decide first
+		for (const ulonglong2 &a : l->tombs) l->decided.insert(std::make_pair((uint64_t)a.x, (uint64_t)a.y));
+		l->tombs.clear();
+		l->started = false;
+		if (--l->file == 0) l->done = true;
+	}
+	if (loaded_out) *loaded_out = l->loaded;
+	if (l->rc) return -1;
+	return l->done ? 0 : 1;
+}
+
+extern "C" int cmb200_load_close(cmb200_loader *l, uint64_t *records_out, uint32_t *deltas_out) {
+	if (records_out) *records_out = 0;
+	if (deltas_out) *deltas_out = 0;
+	if (!l) { set_error_msg("cmb200_load_close: no loader"); return -1; }
+	const int g = (int)l->engines.size();
+	cmb200_engine *const *engines = l->engines.data();
+	int rc = l->rc;
+	if (rc) {
+		load_fences_close(engines, g);
+		delete l;
+		return -1;
+	}
+	// The engines continue the chain only if they hold exactly the store it describes: they were empty,
+	// the load ran to its end, no other call changed them since open (no slot written above the floor,
+	// nothing fenced), every record put is live (none dropped for lack of space, none retired by a
+	// host-tier lap), and no delta file lies beyond the run (a tick that continued it would leave that
+	// file in a valid position).  Otherwise they hold no chain state, and the next tick writes a base.
+	bool whole = l->done && l->id != 0 && l->before == 0 && !delta_beyond(l->base_path.c_str(), (uint32_t)l->ds.size());
+	uint64_t live = 0;
+	for (int i = 0; i < g; i++) {
+		cmb200_engine *e = engines[i];
+		std::lock_guard<std::mutex> lk(e->mu);
+		if (e->seq != l->bs[i].floor || !e->fence.empty()) whole = false;
+		e->fence.clear();
 		cmb200_engine::Chain &ch = e->chain;
-		if (ch.pending) { whole = false; continue; }
+		if (ch.pending || rc) { whole = false; continue; }
 		unsigned long long c[8];
 		std::vector<ExportEntry> none;
 		if (read_counters(e, c) || chain_room(e, c[0]) ||
-		    live_records(e, false, none, c, ~0ull, ch.base_dev[ch.cur ^ 1], &ch.n_next) < 0) { rc = -1; break; }
+		    live_records(e, false, none, c, ~0ull, ch.base_dev[ch.cur ^ 1], &ch.n_next) < 0) { rc = -1; continue; }
 		ch.w_next = e->seq;
 		live += ch.n_next;
 	}
-	whole = whole && rc == 0 && live == loaded;
+	whole = whole && rc == 0 && live == l->loaded;
 	for (int i = 0; i < g; i++) {
 		cmb200_engine *e = engines[i];
 		std::lock_guard<std::mutex> lk(e->mu);
 		cmb200_engine::Chain &ch = e->chain;
 		if (ch.pending) continue;
-		if (whole) { ch.cur ^= 1; ch.n = ch.n_next; ch.w = ch.w_next; ch.id = id; ch.k = (uint32_t)ds.size(); }
+		if (whole) { ch.cur ^= 1; ch.n = ch.n_next; ch.w = ch.w_next; ch.id = l->id; ch.k = (uint32_t)l->ds.size(); }
 		else ch.id = 0;
 	}
-	if (records_out) *records_out = loaded;
-	if (deltas_out) *deltas_out = (uint32_t)ds.size();
+	if (records_out) *records_out = l->loaded;
+	if (deltas_out) *deltas_out = (uint32_t)l->ds.size();
+	delete l;
 	return rc;
+}
+
+extern "C" int cmb200_load_chain(cmb200_engine *const *engines, int g, const char *base_path, uint64_t *records_out,
+    uint32_t *deltas_out) {
+	if (records_out) *records_out = 0;
+	if (deltas_out) *deltas_out = 0;
+	if (g < 1 || !engines || !base_path) { set_error_msg("cmb200_load_chain: no engines"); return -1; }
+	cmb200_loader *l = cmb200_load_open(engines, g, base_path);
+	if (!l) return -1;
+	while (cmb200_load_step(l, 0, nullptr) == 1) {}
+	return cmb200_load_close(l, records_out, deltas_out);
 }
 
 extern "C" int cmb200_load(cmb200_engine *e, const char *path, uint64_t *records_out) {
@@ -2013,6 +2230,7 @@ extern "C" int cmb200_invalidate(cmb200_engine *e, uint64_t u, uint64_t l_first,
 		return -1;
 	}
 	CMB_CHECK(cudaSetDevice(e->device));
+	if (e->fence.open) e->fence.add_span(u, l_first, l_last);
 	if (!e->d_removed && e->d_removed.alloc(sizeof(unsigned long long))) return -1;
 	CMB_CHECK(cudaMemsetAsync(e->d_removed, 0, sizeof(unsigned long long), e->st));
 	// l_last - l_first + 1 overflows for the full interval: compare the difference instead
@@ -2156,6 +2374,8 @@ extern "C" int cmb200_patch_batch(cmb200_engine *e, size_t n, const cmb200_addr 
 			if (st[r] == CMB200_HIT) stored++;
 			if (st[r] == CMB200_DROPPED || st[r] == CMB200_BAD_DECODE || st[r] == CMB200_CORRUPT)
 				drop.push_back(cmb200_addr{h_addr[2 * r], h_addr[2 * r + 1]});
+			// an open load must not bring back the unpatched page of an address it has not loaded yet
+			if (st[r] != CMB200_HIT && e->fence.open) e->fence.addrs.insert(std::make_pair(h_addr[2 * r], h_addr[2 * r + 1]));
 		}
 	}
 	// records that cannot be trusted, and old pages whose patched version found no room, leave the store
@@ -2275,7 +2495,7 @@ static int rename_store(cmb200_engine *e, size_t n, size_t m, unsigned long long
 	}
 	const unsigned long long dropped_before = c[4];
 	const RenameList r = rename_list_view(e->d_ren_list, n, 0);
-	if (restore_records(e, e->d_ren_bytes, r.addr, r.ts, r.off, r.fp, m)) return -1;
+	if (restore_records(e, e->d_ren_bytes, r.addr, r.ts, r.off, r.fp, m, e->seq)) return -1;
 	if (read_counters(e, c)) return -1;
 	const uint64_t lost = c[4] - dropped_before;
 	*moved += m - lost;
@@ -2362,6 +2582,19 @@ extern "C" int cmb200_rename_set(cmb200_engine *const *engines, int g, uint64_t 
 		if (rename_refused(engines[i])) return -1;
 	}
 	if (u_from == u_to) return 0;
+	// an open load passes over both intervals from now on: it must not bring back a source page the move
+	// leaves behind, nor put an older destination page over a moved one
+	for (int i = 0; i < g; i++) {
+		{
+			std::lock_guard<std::mutex> lk(engines[i]->mu);
+			if (!engines[i]->fence.open) continue;
+			engines[i]->fence.add_span(u_from, l_first, l_last);
+		}
+		// A source page the load has not reached cannot move, and a destination page already there would
+		// then stay in its place although the move replaces it: the destination interval goes first
+		// (cmb200_invalidate fences it), so such an address is a miss, never the page the move replaced.
+		if (cmb200_invalidate(engines[i], u_to, l_first, l_last, nullptr)) return -1;
+	}
 	std::lock_guard<std::mutex> call(rename_mu);
 	// slice bounds common to every engine of the call, as a load's batches are bounded
 	size_t n = cmb200_engine::META_CAP;
@@ -2503,6 +2736,13 @@ static int demote_group(cmb200_engine *e, const std::vector<DemoteEntry> &grp,
 		const uint64_t p = t.log.front().first, at = p % t.size;
 		const unsigned long long *pre = reinterpret_cast<const unsigned long long *>(t.host + at);
 		ret.insert(ret.end(), {pre[0], pre[1], REC_HOST | at, t.log.front().second});
+		// a page put during an open load and retired here must not come back from the file: its slot turns
+		// into a tombstone, which a table rebuild drops, and the file may still hold an older version
+		if (e->fence.open) {
+			uint64_t key;
+			FNV_hash(pre, 16, &key);
+			e->fence.keys.insert(key);
+		}
 		t.log.pop_front();
 	}
 	const bool overwrite = end > t.size;        // the region holds bytes of an earlier lap

@@ -129,6 +129,38 @@ __global__ void k_upsert(TableView t, const unsigned long long *addr, const uint
 	slot_idx[i] = idx;
 }
 
+// k_upsert for the records of a background load (cmb200_load_step).  Every call that writes a slot since
+// the load was opened gave it a sequence >= floor, and the load's own records take sequences below floor.
+// So a record is passed over (slot_idx 0xffffffff, which k_restore skips) when its key's slot, or a
+// tombstone on the key's probe chain before it, was written at or above floor: the key was put, moved or
+// removed since the load opened, and the file's page is older than that change.
+__global__ void k_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
+    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx) {
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	const unsigned long long key = fnv_addr(addr[2 * i], addr[2 * i + 1]);
+	bool newer = false;
+	if (key == KEY_EMPTY || key == KEY_TOMB) {
+		newer = t.slots[t.cap + (key == KEY_TOMB ? 1 : 0)].seq >= floor;
+	} else {
+		uint64_t j = home_slot(key, t.cap);
+		for (uint64_t s = 0; s < t.cap; s++, j = (j + 1) & (t.cap - 1)) {
+			const unsigned long long cur = ld_key(&t.slots[j]);
+			if (cur == KEY_EMPTY) break;
+			if (cur == key || cur == KEY_TOMB) {
+				if (t.slots[j].seq >= floor) { newer = true; break; }
+				if (cur == key) break;
+			}
+		}
+	}
+	uint32_t idx = 0xffffffffu;
+	if (!newer) {
+		idx = table_find_or_claim(t, key);
+		if (idx != 0xffffffffu) atomicMax(&t.slots[idx].seq, seq0 + seq_stride * i);
+	}
+	slot_idx[i] = idx;
+}
+
 __global__ void k_lookup(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
     int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out, uint32_t *idx_out) {
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1769,6 +1801,13 @@ int launch_upsert(TableView t, const unsigned long long *addr, const uint8_t *va
     unsigned long long seq0, unsigned long long seq_stride, uint32_t *slot_idx, cudaStream_t st) {
 	if (n == 0) return 0;
 	k_upsert<<<GRID1D(n), 0, st>>>(t, addr, valid, n, seq0, seq_stride, slot_idx);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
+    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_upsert_floor<<<GRID1D(n), 0, st>>>(t, addr, n, seq0, seq_stride, floor, slot_idx);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

@@ -216,6 +216,10 @@ int launch_compose(const uint64_t *offset, const uint64_t *nhid, const uint32_t 
 
 int launch_upsert(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
     unsigned long long seq0, unsigned long long seq_stride, uint32_t *slot_idx, cudaStream_t st);
+// launch_upsert for a background load's records: a key whose slot (or a tombstone on its probe chain) holds
+// a sequence >= floor was changed since the load opened; its record gets slot_idx 0xffffffff.
+int launch_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
+    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st);
 
 // Multi-GPU index replication, the records staying on the device: pack one 32-byte record per chunk
 // of a put step, import all-gathered records written on other GPUs (rows of my_rank / rows that stored

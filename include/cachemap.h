@@ -108,8 +108,20 @@ void cachemap_pwrite(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, u
  * CMB200_CHECKPOINT_SEC seconds if that variable is set (edgefs never calls cachemap_free), and
  * read back on the first put/get after cachemap_create on the same directory
  * (CMB200_PERSIST=0 turns all of it off).  Returns 0 when a snapshot was written.
+ *
+ * CMB200_LOAD says how that first call reads the file back.  "wait" (or unset): the call returns once
+ * the whole store is in HBM.  "background": it starts the engines and returns; a thread loads the file
+ * in steps while the map serves.  A page not loaded yet is a miss, and the file never overrides a change
+ * made since the restart: a get returns either the page that loading the whole file first and then
+ * making every later call would leave, or a miss (cmb200_load_open in cachemap_b200.h).  While the load
+ * runs, checkpoint ticks are skipped; cachemap_checkpoint and cachemap_free wait for the load to end and
+ * then write a base.  If the engine cannot load in steps, the call waits as with "wait".  Any other
+ * value warns and waits.
  */
 int cachemap_checkpoint(struct cachemap *cm);
+/* 1 while a background load runs (*loaded = records stored so far, *total = records the files hold by
+ * their headers, an upper bound), 0 otherwise. */
+int cachemap_load_progress(struct cachemap *cm, uint64_t *loaded, uint64_t *total);
 
 /*
  * Invalidation.  The key of a page is its object's nhid_small and generation plus the page number,

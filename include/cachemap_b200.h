@@ -361,10 +361,53 @@ int cmb200_snapshot_finish(cmb200_snapshot *s, uint64_t *records_out);
  * the engines were empty, every record the chain names is live afterwards and no base_path.d<j> lies
  * beyond the run (a missing or damaged delta ended it early), each engine takes chain
  * state from the load, so that the next delta tick continues the chain; otherwise none holds any and
- * the next tick must write a base.  Load before the engines serve.  0 / -1. */
+ * the next tick must write a base.  It is cmb200_load_open, steps to the end, then cmb200_load_close;
+ * load this way before the engines serve, or load in the background with those calls.  0 / -1. */
 cmb200_snapshot *cmb200_chain_begin(cmb200_engine *const *engines, int g, const char *base_path, int delta);
 int cmb200_load_chain(cmb200_engine *const *engines, int g, const char *base_path, uint64_t *records_out,
     uint32_t *deltas_out);
+
+/* ---- loading while serving: cmb200_load_chain in steps ------------------------------------------
+ * cmb200_load_open starts a load of the chain at base_path (a base alone when it has no chain id) into g
+ * engines.  It reads the headers, no records: the expensive check of the deltas is done by the first
+ * step.  It sets aside one sequence number per record the files may hold on each engine and records the
+ * engine's floor W0, the sequence after them (the count is bounded by the files' sizes).  It fails (NULL, error set) on an engine that has made a
+ * multi-GPU call, or that has a load open already: one loader per engine.
+ * cmb200_load_step stores at most max_records more records (0: all that are left), in file order.  Each
+ * engine's lock is held for one slice of <= max_batch records at a time: its copy to the device, the
+ * upsert and k_restore.  When a slice does not fit the free arena bytes and the garbage covers the
+ * shortfall, the step compacts first; with a host tier it demotes the arena, as cmb200_load_chain does.
+ * What still does not fit is dropped and counted in dropped_puts.  A step never evicts.  *loaded_out =
+ * records stored so far.  Returns 1 while records are left, 0 when the load is done, -1 on error.
+ * cmb200_load_total: the records the files hold by their headers, an upper bound of what the load puts.
+ * cmb200_load_close frees the loader, whether or not the load ran to its end (*records_out = records
+ * stored, *deltas_out = deltas of the run).  0 / -1 (a step failed, or the chain state could not be set).
+ *
+ * The file never overrides a change.  Take the "as-if store": the whole chain loaded at open, then every
+ * call made on the engines since, in order.  Every get, while the load is open and after close, returns
+ * the page the as-if store holds or a miss, never a page the as-if store does not hold:
+ *   - puts, patch hits and the records a rename stores take sequences >= W0; a record of the load whose
+ *     key's slot holds a sequence >= W0 (k_upsert_floor) is passed over;
+ *   - removals are fenced while the load is open: the keys of cmb200_unset_batch (it deletes by key),
+ *     the intervals of cmb200_invalidate, both intervals of cmb200_rename_set, every address
+ *     cmb200_patch_batch does not answer HIT, and the keys of the records a host-tier lap retires.  A
+ *     record of the load that a fence holds is passed over.
+ *   - a rename or a patch that meets a page not yet loaded cannot move or patch it, so that page is not
+ *     served at all; while a load is open cmb200_rename_set invalidates its destination interval first,
+ *     so that no destination page the move would have replaced stays.
+ * The one exception needs a 64-bit FNV collision: a page put during the load whose key equals a file
+ * address's, then invalidated or renamed away, leaves only a tombstone, which a table rebuild or a reuse
+ * loses (DESIGN.md §2, *Loading while serving*).  The multi-GPU calls are refused while a load is open.
+ * With no other call between open and close, the engines end as cmb200_load_chain leaves them: records,
+ * fingerprints, parse checkpoints, ts, entries and chain state.  Otherwise they hold no chain state, and
+ * the next tick writes a base.  While a loader is open on an engine, cmb200_snapshot_begin,
+ * cmb200_chain_begin and cmb200_save_set of it fail: a file of a half-loaded store would replace the one
+ * it is loaded from with less.  Destroying an engine with an open loader is a caller error. */
+typedef struct cmb200_loader cmb200_loader;
+cmb200_loader *cmb200_load_open(cmb200_engine *const *engines, int g, const char *base_path);
+int cmb200_load_step(cmb200_loader *l, size_t max_records, uint64_t *loaded_out);
+uint64_t cmb200_load_total(const cmb200_loader *l);
+int cmb200_load_close(cmb200_loader *l, uint64_t *records_out, uint32_t *deltas_out);
 
 /* Moves n pages of the engine's page size within the engine's device memory:
  * dst[dst_idx ? dst_idx[i] : i] = src[src_idx ? src_idx[i] : i] (one warp per page, 16-byte loads and
