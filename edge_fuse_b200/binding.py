@@ -47,6 +47,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_chain_begin", "cmb200_load_chain", "cmb200_invalidate", "cmb200_patch_batch",
     "cmb200_rename", "cmb200_rename_set", "cmb200_freq_index", "cmb200_freq_estimate", "cmb200_freq_read",
     "cmb200_freq_stats", "cmb200_load_open", "cmb200_load_step", "cmb200_load_total", "cmb200_load_close",
+    "cmb200_set_file_key", "cmb200_load_rejected", "cmb200_aead_seal_batch", "cmb200_aead_open_batch",
 ]
 
 
@@ -168,6 +169,10 @@ def lib() -> C.CDLL:
         "cmb200_locate_batch": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_compose_keys": (i32, [i32, sz, vp, vp, vp, i32, vp, vp, vp]),
         "cmb200_lz4_encode_batch": (i32, [i32, vp, sz, u32, sz, i32, vp, sz, vp, vp]),
+        "cmb200_aead_seal_batch": (i32, [i32, vp, sz, vp, vp, vp, vp, vp, vp]),
+        "cmb200_aead_open_batch": (i32, [i32, vp, sz, vp, vp, vp, vp, vp, vp, vp]),
+        "cmb200_set_file_key": (i32, [vp, vp]),
+        "cmb200_load_rejected": (u64, [vp]),
         "cmb200_lz4_decode_batch": (i32, [i32, vp, sz, vp, sz, u32, vp, vp]),
         "cmb200_fingerprint_batch": (i32, [i32, vp, sz, u32, sz, vp]),
         "cmb200_fingerprint_dev": (i32, [vp, sz, vp, vp]),
@@ -296,6 +301,38 @@ def fingerprint_batch(pages: np.ndarray, nbytes: int | None = None, device: int 
 
 
 # ---- synthetic streams --------------------------------------------------------------------------
+
+def _aead_args(key: bytes, nonces, aads, msgs, extra: int):
+    n = len(msgs)
+    if len(nonces) != n or len(aads) != n or any(len(x) != 12 for x in nonces) or len(key) != 32:
+        raise ValueError("one 12-byte nonce and one AAD per message, and a 32-byte key")
+    bufs = [C.create_string_buffer(bytes(m), len(m) + 1) for m in msgs]
+    abufs = [C.create_string_buffer(bytes(a), len(a) + 1) for a in aads]
+    outs = [C.create_string_buffer(len(m) + extra + 1) for m in msgs]
+    P = C.c_void_p * max(n, 1)
+    S = C.c_size_t * max(n, 1)
+    return (C.create_string_buffer(bytes(key), 32), b"".join(bytes(x) for x in nonces),
+            P(*[C.addressof(b) for b in abufs]), S(*[len(a) for a in aads]),
+            P(*[C.addressof(b) for b in bufs]), P(*[C.addressof(b) for b in outs]), outs, (bufs, abufs))
+
+
+def aead_seal_batch(key: bytes, nonces, aads, msgs, device: int = -1) -> list[bytes]:
+    """cmb200_aead_seal_batch: ChaCha20-Poly1305 of each message on the GPU -> [ciphertext || tag]."""
+    k, nb, ap, al, mp, op, outs, _keep = _aead_args(key, nonces, aads, msgs, 16)
+    ml = (C.c_size_t * max(len(msgs), 1))(*[len(m) for m in msgs])
+    _check(lib().cmb200_aead_seal_batch(device, k, len(msgs), nb, ap, al, mp, ml, op), "cmb200_aead_seal_batch")
+    return [o.raw[:len(m) + 16] for o, m in zip(outs, msgs)]
+
+
+def aead_open_batch(key: bytes, nonces, aads, sealed, device: int = -1):
+    """cmb200_aead_open_batch -> [plaintext, or None where the tag is wrong]."""
+    k, nb, ap, al, mp, op, outs, _keep = _aead_args(key, nonces, aads, sealed, -16)
+    tl = (C.c_size_t * max(len(sealed), 1))(*[len(m) - 16 for m in sealed])
+    ok = np.zeros(max(len(sealed), 1), np.uint8)
+    _check(lib().cmb200_aead_open_batch(device, k, len(sealed), nb, ap, al, mp, tl, op, _ptr(ok)),
+           "cmb200_aead_open_batch")
+    return [o.raw[:len(m) - 16] if ok[i] else None for i, (o, m) in enumerate(zip(outs, sealed))]
+
 
 def gen_chunk_host(seed: int, cid: int, bsize: int) -> np.ndarray:
     out = np.empty(bsize, dtype=np.uint8)
@@ -610,6 +647,17 @@ class Engine:
         n = C.c_uint64(0)
         _check(lib().cmb200_compact(self.h, C.byref(n)), "cmb200_compact")
         return n.value
+
+    def set_file_key(self, key: bytes | None):
+        """cmb200_set_file_key: the 32-byte key of the files this engine writes and reads (None: no key)."""
+        if key is not None and len(key) != 32:
+            raise ValueError("a file key is 32 bytes")
+        _check(lib().cmb200_set_file_key(self.h, None if key is None else C.create_string_buffer(bytes(key), 32)),
+               "cmb200_set_file_key")
+
+    def load_rejected(self) -> int:
+        """cmb200_load_rejected: records of sealed files whose tag or length failed, since create."""
+        return int(lib().cmb200_load_rejected(self.h))
 
     def save(self, path: str) -> int:
         n = C.c_uint64(0)

@@ -76,6 +76,7 @@ extern uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width);
 #pragma weak cmb200_load_step
 #pragma weak cmb200_load_total
 #pragma weak cmb200_load_close
+#pragma weak cmb200_set_file_key
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -208,6 +209,64 @@ static int
 filemap_snapshot_path(struct filemap *m, char *out, size_t cap)
 {
 	return snprintf(out, cap, "%s/%s", m->destdir, SNAPSHOT_NAME) < (int)cap;
+}
+
+/* CMB200_KEY_FILE: the 32-byte file key, as 32 raw bytes or 64 hex digits (surrounding white space
+ * allowed), into key[32].  1 = a key was read, 0 = the variable is unset, -1 = it is set and the file is
+ * missing, unreadable or malformed (warned). */
+static int
+read_key_file(uint8_t key[32])
+{
+	const char *path = getenv("CMB200_KEY_FILE");
+	if (!path || !*path)
+		return 0;
+	uint8_t buf[160];
+	size_t n = 0;
+	FILE *f = fopen(path, "rb");
+	if (f) {
+		n = fread(buf, 1, sizeof(buf), f);
+		fclose(f);
+	}
+	int ok = f && n == 32;
+	if (f && !ok) {
+		/* 64 hex digits */
+		size_t a = 0, b = n;
+		while (a < b && (buf[a] == ' ' || buf[a] == '\t' || buf[a] == '\n' || buf[a] == '\r'))
+			a++;
+		while (b > a && (buf[b - 1] == ' ' || buf[b - 1] == '\t' || buf[b - 1] == '\n' || buf[b - 1] == '\r'))
+			b--;
+		ok = b - a == 64 && n < sizeof(buf);
+		for (size_t i = 0; ok && i < 32; i++) {
+			unsigned v;
+			char hx[3] = {(char)buf[a + 2 * i], (char)buf[a + 2 * i + 1], 0};
+			char *end;
+			v = (unsigned)strtoul(hx, &end, 16);
+			ok = *end == 0 && hx[0] != '+' && hx[0] != '-' && hx[0] != ' ' && hx[1] != ' ';
+			key[i] = (uint8_t)v;
+		}
+	} else if (ok) {
+		memcpy(key, buf, 32);
+	}
+	explicit_bzero(buf, sizeof(buf));
+	if (ok)
+		return 1;
+	explicit_bzero(key, 32);
+	fprintf(stderr, "cachemap_b200: CMB200_KEY_FILE=%s is %s; the cache directory is neither read nor written\n",
+	    path, f ? "neither 32 raw bytes nor 64 hex digits" : "missing or unreadable");
+	return -1;
+}
+
+/* The first 8 bytes of the file at path are a sealed base's magic. */
+static int
+snapshot_sealed(const char *path)
+{
+	char magic[8] = {0};
+	FILE *f = fopen(path, "rb");
+	if (!f)
+		return 0;
+	const int ok = fread(magic, 8, 1, f) == 1 && memcmp(magic, "CMB200E1", 8) == 0;
+	fclose(f);
+	return ok;
 }
 
 static long
@@ -471,10 +530,30 @@ filemap_engine_ready(struct filemap *m)
 			m->checkpoint_sec = env_long("CMB200_CHECKPOINT_SEC", 0);
 			m->checkpoint_deltas = env_long("CMB200_CHECKPOINT_DELTAS", 0);
 			m->chain_deltas = -1;
+			if (m->persist) {
+				/* a misconfigured key must never replace an encrypted cache with a plaintext one */
+				uint8_t key[32];
+				const int have = read_key_file(key);
+				if (have < 0)
+					m->persist = 0;
+				else if (have && !cmb200_set_file_key) {
+					fprintf(stderr, "cachemap_b200: CMB200_KEY_FILE ignored: the engine cannot encrypt; the cache "
+					    "directory is neither read nor written\n");
+					m->persist = 0;
+				}
+				for (int i = 0; have > 0 && m->persist && i < g; i++)
+					if (cmb200_set_file_key(m->engs[i], key) != 0) {
+						fprintf(stderr, "cachemap_b200: no file key: %s; the cache directory is neither read nor "
+						    "written\n", cmb200_last_error());
+						m->persist = 0;
+					}
+				explicit_bzero(key, sizeof(key));
+			}
 			char snap[2200], d1[2300];
 			if (m->persist && filemap_snapshot_path(m, snap, sizeof(snap)) && access(snap, R_OK) == 0) {
 				uint64_t got = 0;
 				uint32_t k = 0;
+				int load_rc = 0;
 				snprintf(d1, sizeof(d1), "%s.d1", snap);
 				/* a chain next to the base is never ignored, whatever CMB200_CHECKPOINT_DELTAS says now;
 				 * a base whose deltas do not match it loads alone */
@@ -491,14 +570,21 @@ filemap_engine_ready(struct filemap *m)
 					m->load_total = cmb200_load_total(m->loader);
 					m->loading = 1;
 				} else if (chain) {
-					if (cmb200_load_chain(m->engs, g, snap, &got, &k) != 0)
+					if ((load_rc = cmb200_load_chain(m->engs, g, snap, &got, &k)) != 0)
 						fprintf(stderr, "cachemap_b200: %s ignored: %s\n", snap, cmb200_last_error());
 					else
 						m->chain_deltas = (int)k;
 				} else if (!cmb200_load_set)
 					fprintf(stderr, "cachemap_b200: %s ignored: the engine cannot load snapshots\n", snap);
-				else if (cmb200_load_set(m->engs, g, snap, &got) != 0)
+				else if ((load_rc = cmb200_load_set(m->engs, g, snap, &got)) != 0)
 					fprintf(stderr, "cachemap_b200: %s ignored: %s\n", snap, cmb200_last_error());
+				/* an encrypted base that does not load (no key, another key, a damaged file) is left as it is:
+				 * the map starts empty and never writes the directory, not even at cachemap_free */
+				if (load_rc != 0 && snapshot_sealed(snap)) {
+					fprintf(stderr, "cachemap_b200: %s is encrypted and did not load; the cache directory is left "
+					    "as it is and not written\n", snap);
+					m->persist = 0;
+				}
 			}
 			/* the flushers start here, i.e. in the process that actually caches (after any fork) */
 			for (int i = 0; i < g; i++) {

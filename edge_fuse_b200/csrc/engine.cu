@@ -20,6 +20,7 @@
 #include <set>
 #include <shared_mutex>
 #include <sched.h>
+#include <sys/random.h>
 #include <sys/stat.h>
 #include <string>
 #include <new>
@@ -363,6 +364,13 @@ struct cmb200_engine {
 		unsigned long long w_next = 0;
 	} chain;
 	LoadFence fence;                     // an open cmb200_loader's removals (under mu)
+	// encryption at rest (cmb200_set_file_key): the key of the files this engine writes and reads, under
+	// mu; snap_dev is the writer's device staging for sealed records, allocated by the first sealed
+	// snapshot (SEAL_STAGING bytes, grown only for a delta with more tombstones than it holds)
+	bool has_key = false;
+	AeadKey key{};
+	DevMem<uint8_t> snap_dev;
+	std::atomic<uint64_t> load_rejected{0};   // records whose tag or length failed, since create
 };
 
 // CMB200_TOUCH: the stamp a get raises its hits' ts to, taken at launch from the clock the drop-in's puts
@@ -404,6 +412,7 @@ extern "C" void cmb200_engine_destroy(cmb200_engine *e) {
 	if (e->copy) cudaStreamSynchronize(e->copy);
 	for (auto &ln : e->lane) if (ln.st) cudaStreamSynchronize(ln.st);
 	for (int r = 0; r < GET_MAX_PEERS; r++) if (e->peer_base[r]) cudaIpcCloseMemHandle((void *)e->peer_base[r]);
+	explicit_bzero(&e->key, sizeof(e->key));
 	delete e;
 }
 
@@ -1382,6 +1391,66 @@ struct SnapRecord { uint64_t ts, fp_hi, fp_lo; uint32_t len, zero; };
 static_assert(sizeof(SnapRecord) == 32, "snapshot record header");
 static const size_t SNAP_WINDOW = 64u << 20;
 
+// ---- encryption at rest (DESIGN.md §2 "Encryption at rest") ----
+// With a key, a base is "CMB200E1" and a delta "CMB200F1": the header above with a fresh 64-bit file
+// nonce (a base: header bytes 48..55; a delta: its last 8 bytes), then the tag of an AEAD seal with an
+// empty text and the header as AAD.  A delta's clear tombstones follow, then the tag of the i = 1 seal
+// with the tombstones as AAD.  Each record is {u32 len, u32 0, u64 u, u64 l} (AAD), the ciphertext of
+// {ts, fp_hi, fp_lo, compressed_length, pad, payload}, the tag, zeros to 16 (seal_record_bytes(len)).
+// The AEAD nonce is {file nonce, u32 i}: i = 0 the header, 1 the tombstones, 2 + ordinal the file's
+// ordinal-th record.  All of it is sealed and opened by k_seal / k_open; the host holds no cipher.
+static const size_t SEAL_MAX_RECS = 1u << 16;                // records per sealed window
+static const size_t SEAL_STAGING = SNAP_WINDOW + SEAL_MAX_RECS * sizeof(AeadMsg);
+static const uint32_t AEAD_TAG = 16;
+
+static uint64_t base_nonce(const SnapHeader &h) { uint64_t v; memcpy(&v, &h.pad[3], 8); return v; }
+
+// One header or tombstone seal (open = false: tag written) or check (open: 1 = the tag is right, 0 = not)
+// of aad_len bytes with an empty text, on st through `scratch` (device, >= aad_len + 256 bytes).
+static int aead_one(uint8_t *scratch, cudaStream_t st, bool open, const AeadKey &key, uint64_t nonce, uint32_t i,
+    const void *aad, size_t aad_len, uint8_t tag[16]) {
+	const size_t o_tag = (aad_len + 15) & ~(size_t)15, o_msg = o_tag + 16, o_ok = o_msg + sizeof(AeadMsg);
+	AeadMsg m{};
+	m.aad = scratch; m.aad_len = aad_len; m.src = scratch + o_tag; m.dst = scratch + o_tag; m.len = 0;
+	m.nonce[0] = (uint32_t)nonce; m.nonce[1] = (uint32_t)(nonce >> 32); m.nonce[2] = i;
+	if (aad_len) CMB_CHECK(cudaMemcpyAsync(scratch, aad, aad_len, cudaMemcpyHostToDevice, st));
+	CMB_CHECK(cudaMemcpyAsync(scratch + o_msg, &m, sizeof(m), cudaMemcpyHostToDevice, st));
+	if (open) CMB_CHECK(cudaMemcpyAsync(scratch + o_tag, tag, 16, cudaMemcpyHostToDevice, st));
+	if (open ? launch_open((const AeadMsg *)(scratch + o_msg), 1, key, 0, nullptr, nullptr, scratch + o_ok, nullptr, st)
+	         : launch_seal((const AeadMsg *)(scratch + o_msg), 1, key, st)) return -1;
+	uint8_t ok = 0;
+	if (open) CMB_CHECK(cudaMemcpyAsync(&ok, scratch + o_ok, 1, cudaMemcpyDeviceToHost, st));
+	else CMB_CHECK(cudaMemcpyAsync(tag, scratch + o_tag, 16, cudaMemcpyDeviceToHost, st));
+	CMB_CHECK(cudaStreamSynchronize(st));
+	return open ? (ok ? 1 : 0) : 0;
+}
+
+// aead_one on the device of engine e, through scratch of its own: a check made when a file is opened.
+static int aead_check(cmb200_engine *e, const AeadKey &key, uint64_t nonce, uint32_t i, const void *aad, size_t aad_len,
+    const uint8_t tag[16]) {
+	CMB_CHECK(cudaSetDevice(e->device));
+	DevMem<uint8_t> scratch;
+	Stream st;
+	if (scratch.alloc(aad_len + 256) || st.create()) return -1;
+	uint8_t t[16];
+	memcpy(t, tag, 16);
+	return aead_one(scratch, st, true, key, nonce, i, aad, aad_len, t);
+}
+
+// The key every engine of a call holds: *has = false when none does.  -1 (error set) when they differ.
+static int call_key(cmb200_engine *const *engines, int g, const char *what, AeadKey &key, bool &has) {
+	for (int i = 0; i < g; i++) {
+		std::lock_guard<std::mutex> lk(engines[i]->mu);
+		const cmb200_engine *e = engines[i];
+		if (i == 0) { has = e->has_key; key = e->key; continue; }
+		if (e->has_key != has || (has && memcmp(&e->key, &key, sizeof(key)) != 0)) {
+			set_error_msg((std::string(what) + ": the engines hold different file keys").c_str());
+			return -1;
+		}
+	}
+	return 0;
+}
+
 // A snapshot lists each engine's live records under its lock and writes them from a thread of its own
 // while the engines keep serving.  That is sound because records are immutable (DESIGN.md §2): only
 // compaction (which slides records down) and a host-tier lap (which overwrites the tier's oldest
@@ -1437,6 +1506,41 @@ static int write_section(cmb200_engine *e, FILE *f, const std::vector<ExportEntr
 	return ok ? 0 : -2;
 }
 
+// write_section for a sealed file: k_seal writes each window's records (arena records, and tier records
+// through the mapped tier) into snap_dev at their file offsets, and the window crosses PCIe and reaches
+// the file as ciphertext.  *ordinal numbers the file's records.  Returns as write_section.
+static int write_section_sealed(cmb200_engine *e, FILE *f, const std::vector<ExportEntry> &list, const AeadKey &key,
+    uint64_t nonce, uint64_t *ordinal) {
+	uint8_t *out = e->snap_dev;
+	AeadMsg *d_msg = (AeadMsg *)(out + SNAP_WINDOW);
+	std::vector<AeadMsg> msgs;
+	bool ok = true;
+	size_t k = 0;
+	while (ok && k < list.size()) {
+		msgs.clear();
+		size_t bytes = 0;
+		for (; k < list.size() && msgs.size() < SEAL_MAX_RECS; k++) {
+			const ExportEntry &x = list[k];
+			const size_t sb = seal_record_bytes(x.len);
+			if (bytes + sb > SNAP_WINDOW) break;
+			AeadMsg m{};
+			m.src = x.rec_off & REC_HOST ? e->tier.dev + (x.rec_off & ~REC_HOST) : e->arena.base + x.rec_off;
+			m.dst = out + bytes;
+			m.len = x.len; m.ts = x.ts; m.fp_hi = x.fp_hi; m.fp_lo = x.fp_lo;
+			const uint64_t i = 2 + (*ordinal)++;
+			m.nonce[0] = (uint32_t)nonce; m.nonce[1] = (uint32_t)(nonce >> 32); m.nonce[2] = (uint32_t)i;
+			msgs.push_back(m);
+			bytes += sb;
+		}
+		CMB_CHECK(cudaMemcpyAsync(d_msg, msgs.data(), msgs.size() * sizeof(AeadMsg), cudaMemcpyHostToDevice, e->snap_st));
+		if (launch_seal(d_msg, (uint32_t)msgs.size(), key, e->snap_st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(e->snap_win, out, bytes, cudaMemcpyDeviceToHost, e->snap_st));
+		CMB_CHECK(cudaStreamSynchronize(e->snap_st));
+		ok = fwrite(e->snap_win, bytes, 1, f) == 1;
+	}
+	return ok ? 0 : -2;
+}
+
 // ---- snapshot chains (cmb200_chain_begin / cmb200_load_chain) ----
 // A base is the file above with a nonzero 64-bit chain id in bytes 40..47 (pad[1..2], zero in a file
 // written by cmb200_save_set).  Delta k of that chain, <base>.d<k>, holds what changed between tick k-1
@@ -1480,21 +1584,48 @@ struct cmb200_snapshot {
 	int chain = CHAIN_NONE;
 	DeltaHeader dh{};                                     // CHAIN_DELTA: the header written instead of h
 	std::vector<ulonglong2> tombs;                        // CHAIN_DELTA: every engine's tombstones
+	bool sealed = false;                                  // the engines' key: the file is sealed
+	AeadKey key{};
+	uint64_t nonce = 0;
+	~cmb200_snapshot() { explicit_bzero(&key, sizeof(key)); }
 };
 
 // The writer thread: header, then each engine's section; an engine is released as soon as its section
 // is written (or the write has failed), so that its compactions and tier laps go ahead.
+// The sealed file's header tag and, for a delta, its tombstones and their tag: on engine 0's staging.
+static int write_sealed_head(cmb200_snapshot *s) {
+	cmb200_engine *e = s->engines[0];
+	CMB_CHECK(cudaSetDevice(e->device));
+	const bool delta = s->chain == CHAIN_DELTA;
+	uint8_t tag[16];
+	if (aead_one(e->snap_dev, e->snap_st, false, s->key, s->nonce, 0, delta ? (const void *)&s->dh : (const void *)&s->h, 64, tag)) return -1;
+	if (fwrite(delta ? (const void *)&s->dh : (const void *)&s->h, 64, 1, s->f) != 1 || fwrite(tag, 16, 1, s->f) != 1) return -2;
+	if (!delta) return 0;
+	const size_t tb = s->tombs.size() * 16;
+	if (e->snap_dev.grow(tb + 256, e->snap_st)) return -1;
+	if (aead_one(e->snap_dev, e->snap_st, false, s->key, s->nonce, 1, s->tombs.data(), tb, tag)) return -1;
+	if ((tb && fwrite(s->tombs.data(), 16, s->tombs.size(), s->f) != s->tombs.size()) || fwrite(tag, 16, 1, s->f) != 1) return -2;
+	return 0;
+}
+
 static void snapshot_write(cmb200_snapshot *s) {
-	bool ok = s->chain == CHAIN_DELTA
-	    ? fwrite(&s->dh, sizeof(s->dh), 1, s->f) == 1 &&
-	      (s->tombs.empty() || fwrite(s->tombs.data(), 16, s->tombs.size(), s->f) == s->tombs.size())
-	    : fwrite(&s->h, sizeof(s->h), 1, s->f) == 1;
-	int rc = ok ? 0 : -2;
+	int rc;
+	if (s->sealed) {
+		rc = write_sealed_head(s);
+	} else {
+		const bool ok = s->chain == CHAIN_DELTA
+		    ? fwrite(&s->dh, sizeof(s->dh), 1, s->f) == 1 &&
+		      (s->tombs.empty() || fwrite(s->tombs.data(), 16, s->tombs.size(), s->f) == s->tombs.size())
+		    : fwrite(&s->h, sizeof(s->h), 1, s->f) == 1;
+		rc = ok ? 0 : -2;
+	}
+	uint64_t ordinal = 0;
 	for (size_t i = 0; i < s->engines.size(); i++) {
 		cmb200_engine *e = s->engines[i];
 		if (rc == 0) {
 			if (cudaSetDevice(e->device) != cudaSuccess) { cmb_set_error("cudaSetDevice", cudaGetLastError(), __FILE__, __LINE__); rc = -1; }
-			else rc = write_section(e, s->f, s->lists[i]);
+			else rc = s->sealed ? write_section_sealed(e, s->f, s->lists[i], s->key, s->nonce, &ordinal)
+			                    : write_section(e, s->f, s->lists[i]);
 		}
 		std::vector<ExportEntry>().swap(s->lists[i]);
 		snap_set_state(e, cmb200_engine::SNAP_FREE);
@@ -1571,6 +1702,12 @@ static cmb200_snapshot *snapshot_start(cmb200_engine *const *engines, int g, con
 	if (!s) { set_error_msg("cmb200_snapshot_begin: out of memory"); return nullptr; }
 	s->engines.assign(engines, engines + g);
 	s->lists.resize(g);
+	if (call_key(engines, g, "cmb200_snapshot_begin", s->key, s->sealed)) { delete s; return nullptr; }
+	if (s->sealed && getrandom(&s->nonce, sizeof(s->nonce), 0) != (ssize_t)sizeof(s->nonce)) {
+		set_error_msg("cmb200_snapshot_begin: no random file nonce (getrandom failed)");
+		delete s;
+		return nullptr;
+	}
 	s->tmp = std::string(path) + ".tmp";
 	s->f = fopen(s->tmp.c_str(), "wb");
 	if (!s->f) { set_error_msg("cmb200_save: cannot create the snapshot file"); delete s; return nullptr; }
@@ -1583,15 +1720,17 @@ static cmb200_snapshot *snapshot_start(cmb200_engine *const *engines, int g, con
 	for (cmb200_engine *e : order) {
 		// allocated once: cudaFreeHost may synchronise the device
 		if (cudaSetDevice(e->device) != cudaSuccess ||
-		    (!e->snap_win && e->snap_win.alloc(SNAP_WINDOW)) || (!e->snap_st && e->snap_st.create())) {
+		    (!e->snap_win && e->snap_win.alloc(SNAP_WINDOW)) || (!e->snap_st && e->snap_st.create()) ||
+		    (s->sealed && !e->snap_dev && e->snap_dev.alloc(SEAL_STAGING))) {
 			cmb_set_error("cmb200_snapshot_begin: no page-locked window or stream", cudaGetLastError(), __FILE__, __LINE__);
 			rc = -1;
 			break;
 		}
 	}
 	s->h = SnapHeader{};
-	memcpy(s->h.magic, "CMB200S1", 8);
+	memcpy(s->h.magic, s->sealed ? "CMB200E1" : "CMB200S1", 8);
 	s->h.version = 1; s->h.pshift = (uint32_t)engines[0]->pshift;
+	if (s->sealed) memcpy(&s->h.pad[3], &s->nonce, 8);
 	s->chain = chain;
 	s->dh.chain = chain_id; s->dh.index = k;
 	if (chain == CHAIN_BASE) memcpy(&s->h.pad[1], &chain_id, 8);
@@ -1615,9 +1754,14 @@ static cmb200_snapshot *snapshot_start(cmb200_engine *const *engines, int g, con
 		for (const ExportEntry &x : s->lists[i]) s->h.bytes += x.len;
 	}
 	if (chain == CHAIN_DELTA) {
-		memcpy(s->dh.magic, "CMB200D1", 8);
+		memcpy(s->dh.magic, s->sealed ? "CMB200F1" : "CMB200D1", 8);
 		s->dh.version = 1; s->dh.pshift = s->h.pshift; s->dh.flags = s->h.flags;
 		s->dh.tombstones = s->tombs.size(); s->dh.records = s->h.records; s->dh.bytes = s->h.bytes;
+		if (s->sealed) s->dh.pad = s->nonce;
+	}
+	if (rc == 0 && s->sealed && s->h.records >= 0xfffffffeull) {
+		set_error_msg("cmb200_snapshot_begin: a sealed file holds fewer than 2^32 - 2 records");
+		rc = -1;
 	}
 	if (rc == 0) {
 		try {
@@ -1660,7 +1804,8 @@ extern "C" cmb200_snapshot *cmb200_chain_begin(cmb200_engine *const *engines, in
 	}
 	SnapHeader h{};
 	FILE *f = fopen(base_path, "rb");
-	const bool ok = f && fread(&h, sizeof(h), 1, f) == 1 && memcmp(h.magic, "CMB200S1", 8) == 0 && h.version == 1;
+	const bool ok = f && fread(&h, sizeof(h), 1, f) == 1 &&
+	    (memcmp(h.magic, "CMB200S1", 8) == 0 || memcmp(h.magic, "CMB200E1", 8) == 0) && h.version == 1;
 	if (f) fclose(f);
 	if (!ok || snap_chain_id(h) == 0) { set_error_msg("cmb200_chain_begin: no chain base at this path"); return nullptr; }
 	uint32_t k;
@@ -1723,6 +1868,12 @@ struct LoadBatch {
 	std::vector<cmb200_addr> addr;
 	DevMem<unsigned long long> d_off;
 	DevMem<uint64_t> d_fp;
+	// the records of a sealed file (sealed): k_open's messages, run in place on the slice in d_pages[0]
+	bool sealed = false;
+	AeadKey key{};                       // zeroed by load_teardown
+	std::vector<AeadMsg> msg;
+	DevMem<AeadMsg> d_msg;
+	DevMem<unsigned long long> d_rej;
 	// a background load's batch (floor != 0): the sequence of its next record, below the engine's floor
 	unsigned long long seq = 0, floor = 0;
 	int setup(cmb200_engine *eng) {
@@ -1730,8 +1881,10 @@ struct LoadBatch {
 		CMB_CHECK(cudaSetDevice(e->device));
 		cap = (size_t)e->host_batch * e->bsize;
 		B = e->max_batch < cmb200_engine::META_CAP ? e->max_batch : cmb200_engine::META_CAP;
-		off.resize(B); ts.resize(B); fps.resize(2 * B); addr.resize(B);
-		return blob.alloc(cap) || d_off.alloc(B * 8) || d_fp.alloc(B * 16) ? -1 : 0;
+		off.resize(B); ts.resize(B); fps.resize(2 * B); addr.resize(B); msg.resize(B);
+		if (blob.alloc(cap) || d_off.alloc(B * 8) || d_fp.alloc(B * 16) || d_msg.alloc(B * sizeof(AeadMsg)) || d_rej.alloc(8)) return -1;
+		CMB_CHECK(cudaMemset(d_rej, 0, 8));
+		return 0;
 	}
 };
 
@@ -1745,9 +1898,10 @@ struct LoadBatch {
 // (e->mu held; m <= max_batch)
 static int restore_records(cmb200_engine *e, const uint8_t *blob, const unsigned long long *addr,
     const unsigned long long *ts, const unsigned long long *off, const uint64_t *fps, size_t m,
-    unsigned long long &seq, unsigned long long floor = 0) {
-	if (floor ? launch_upsert_floor(e->table, addr, (uint32_t)m, seq, e->seq_stride, floor, e->d_slot, e->st)
-	          : launch_upsert(e->table, addr, nullptr, (uint32_t)m, seq, e->seq_stride, e->d_slot, e->st)) return -1;
+    unsigned long long &seq, unsigned long long floor = 0, const uint8_t *valid = nullptr) {
+	if (floor ? (valid ? launch_upsert_floor_valid(e->table, addr, valid, (uint32_t)m, seq, e->seq_stride, floor, e->d_slot, e->st)
+	                   : launch_upsert_floor(e->table, addr, (uint32_t)m, seq, e->seq_stride, floor, e->d_slot, e->st))
+	          : launch_upsert(e->table, addr, valid, (uint32_t)m, seq, e->seq_stride, e->d_slot, e->st)) return -1;
 	EncodeJob job{};
 	job.n = (uint32_t)m; job.nbytes = e->bsize;
 	job.slot_idx = e->d_slot; job.addr = addr; job.ts = ts;
@@ -1774,7 +1928,7 @@ static long long load_flush(LoadBatch &b, bool with_fp) {
 			uint64_t key;
 			FNV_hash(&b.addr[j], 16, &key);
 			if (e->fence.holds(b.addr[j].u, b.addr[j].l, key)) continue;
-			b.addr[k] = b.addr[j]; b.off[k] = b.off[j]; b.ts[k] = b.ts[j];
+			b.addr[k] = b.addr[j]; b.off[k] = b.off[j]; b.ts[k] = b.ts[j]; b.msg[k] = b.msg[j];
 			b.fps[2 * k] = b.fps[2 * j]; b.fps[2 * k + 1] = b.fps[2 * j + 1];
 			k++;
 		}
@@ -1793,26 +1947,56 @@ static long long load_flush(LoadBatch &b, bool with_fp) {
 	}
 	CMB_CHECK(cudaMemcpyAsync(e->d_pages[0], b.blob, b.used, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(e->d_addr, b.addr.data(), m * 16, cudaMemcpyHostToDevice, e->st));
-	CMB_CHECK(cudaMemcpyAsync(e->d_ts, b.ts.data(), m * 8, cudaMemcpyHostToDevice, e->st));
 	CMB_CHECK(cudaMemcpyAsync(b.d_off, b.off.data(), m * 8, cudaMemcpyHostToDevice, e->st));
-	CMB_CHECK(cudaMemcpyAsync(b.d_fp, b.fps.data(), m * 16, cudaMemcpyHostToDevice, e->st));
+	if (b.sealed) {
+		// k_open checks and decrypts the slice in place and writes ts and fingerprints; a record whose tag or
+		// length fails is not valid, claims no slot and is counted
+		for (size_t j = 0; j < m; j++) b.msg[j].src = b.msg[j].dst = e->d_pages[0] + (b.off[j] - 32);
+		CMB_CHECK(cudaMemcpyAsync(b.d_msg, b.msg.data(), m * sizeof(AeadMsg), cudaMemcpyHostToDevice, e->st));
+		if (launch_open(b.d_msg, (uint32_t)m, b.key, e->bsize, e->d_ts, b.d_fp, e->d_valid, b.d_rej, e->st)) return -1;
+	} else {
+		CMB_CHECK(cudaMemcpyAsync(e->d_ts, b.ts.data(), m * 8, cudaMemcpyHostToDevice, e->st));
+		CMB_CHECK(cudaMemcpyAsync(b.d_fp, b.fps.data(), m * 16, cudaMemcpyHostToDevice, e->st));
+	}
 	if (restore_records(e, e->d_pages[0], e->d_addr, e->d_ts, b.d_off, with_fp ? (uint64_t *)b.d_fp : nullptr, m,
-	    b.floor ? b.seq : e->seq, b.floor)) return -1;
+	    b.floor ? b.seq : e->seq, b.floor, b.sealed ? (const uint8_t *)e->d_valid : nullptr)) return -1;
+	unsigned long long rej = 0;
+	if (b.sealed) {
+		CMB_CHECK(cudaMemcpyAsync(&rej, b.d_rej, 8, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaMemsetAsync(b.d_rej, 0, 8, e->st));
+	}
 	CMB_CHECK(cudaStreamSynchronize(e->st));
+	e->load_rejected += rej;
 	b.used = 0;
-	return (long long)m;
+	return (long long)(m - rej);
 }
 
 // Opens a snapshot file (a base) for a load into g engines and reads its header.  nullptr on failure
 // (error set).
-static FILE *open_snapshot(cmb200_engine *const *engines, int g, const char *path, SnapHeader &h) {
+// A sealed base (*sealed) is opened with the engines' key (key, has_key from call_key): its header tag is
+// checked first, so that a wrong key or a damaged header fails here, before any record is read.
+static FILE *open_snapshot(cmb200_engine *const *engines, int g, const char *path, SnapHeader &h, const AeadKey &key,
+    bool has_key, bool *sealed) {
 	FILE *f = fopen(path, "rb");
 	if (!f) { set_error_msg("cmb200_load: no snapshot file"); return nullptr; }
-	if (fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "CMB200S1", 8) != 0 || h.version != 1) {
+	const bool ok = fread(&h, sizeof(h), 1, f) == 1 && h.version == 1;
+	*sealed = ok && memcmp(h.magic, "CMB200E1", 8) == 0;
+	if (!ok || (!*sealed && memcmp(h.magic, "CMB200S1", 8) != 0)) {
 		fclose(f); set_error_msg("cmb200_load: not a snapshot of this library"); return nullptr;
 	}
 	for (int i = 0; i < g; i++)
 		if ((int)h.pshift != engines[i]->pshift) { fclose(f); set_error_msg("cmb200_load: snapshot has another page size"); return nullptr; }
+	if (*sealed) {
+		uint8_t tag[16];
+		if (!has_key) { fclose(f); set_error_msg("cmb200_load: the snapshot is encrypted and the engines hold no file key"); return nullptr; }
+		if (fread(tag, 16, 1, f) != 1) { fclose(f); set_error_msg("cmb200_load: truncated or corrupt snapshot"); return nullptr; }
+		const int r = aead_check(engines[0], key, base_nonce(h), 0, &h, sizeof(h), tag);
+		if (r != 1) {
+			fclose(f);
+			if (r == 0) set_error_msg("cmb200_load: the snapshot header does not open with this key (wrong key or damaged header)");
+			return nullptr;
+		}
+	}
 	return f;
 }
 
@@ -1820,8 +2004,54 @@ static FILE *open_snapshot(cmb200_engine *const *engines, int g, const char *pat
 // when it is full; *loaded += records put.  skip (nullable): addresses a newer file of a chain has
 // decided, whose records are passed over unread; decide (nullable) gets every address read.  The
 // batches are not flushed at the end.  0 / -1 (error set).
+// sealed: the file's records are sealed under `nonce`; *ordinal is the file ordinal of the next one.
+static int load_records_sealed(FILE *f, uint64_t n, std::vector<LoadBatch> &bs, int g, bool with_fp,
+    const AddrSet *skip, AddrSet *decide, uint64_t *loaded, uint64_t nonce, uint64_t *ordinal) {
+	const uint32_t bsize = bs[0].e->bsize;
+	for (uint64_t done = 0; done < n; done++) {
+		// the clear part {u32 len, u32 0, u, l} routes the record, as a plain file's address does
+		struct { uint32_t len, zero; cmb200_addr a; } c;
+		if (fread(&c, sizeof(c), 1, f) != 1 || c.zero != 0 || c.len < 24 || c.len > 24u + bsize + 1024u) {
+			set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1;
+		}
+		const size_t padded = seal_record_bytes(c.len);
+		const uint64_t i = 2 + (*ordinal)++;
+		if (skip || decide) {
+			const std::pair<uint64_t, uint64_t> ul(c.a.u, c.a.l);
+			const bool decided = skip && skip->count(ul);
+			if (decide && !decided) decide->insert(ul);
+			if (decided) {
+				if (fseeko(f, (off_t)(padded - sizeof(c)), SEEK_CUR) != 0) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1; }
+				continue;
+			}
+		}
+		uint64_t key;
+		FNV_hash(&c.a, 16, &key);
+		LoadBatch &b = bs[cmb200_owner(key, g)];
+		if (padded > b.cap) { set_error_msg("cmb200_load: record larger than the staging buffer"); return -1; }
+		if (b.m == b.B || b.used + padded > b.cap) {
+			const long long got = load_flush(b, with_fp);
+			if (got < 0) return -1;
+			*loaded += (uint64_t)got;
+		}
+		uint8_t *rec = b.blob + b.used;
+		memcpy(rec, &c, sizeof(c));
+		if (fread(rec + sizeof(c), padded - sizeof(c), 1, f) != 1) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1; }
+		AeadMsg &m = b.msg[b.m];
+		m = AeadMsg{};
+		m.len = c.len;
+		m.nonce[0] = (uint32_t)nonce; m.nonce[1] = (uint32_t)(nonce >> 32); m.nonce[2] = (uint32_t)i;
+		b.addr[b.m] = c.a;
+		b.off[b.m] = b.used + 32;              // where k_open leaves the record {u, l, compressed_length, ...}
+		b.used += padded; b.m++;
+	}
+	return 0;
+}
+
 static int load_records(FILE *f, uint64_t n, std::vector<LoadBatch> &bs, int g, bool with_fp, const AddrSet *skip,
-    AddrSet *decide, uint64_t *loaded) {
+    AddrSet *decide, uint64_t *loaded, bool sealed = false, uint64_t nonce = 0, uint64_t *ordinal = nullptr) {
+	for (LoadBatch &b : bs) b.sealed = sealed;
+	if (sealed) return load_records_sealed(f, n, bs, g, with_fp, skip, decide, loaded, nonce, ordinal);
 	const uint32_t bsize = bs[0].e->bsize;
 	int rc = 0;
 	uint64_t done = 0;
@@ -1881,10 +2111,16 @@ static int load_flush_all(std::vector<LoadBatch> &bs, bool with_fp, uint64_t *lo
 	return 0;
 }
 
-static int load_setup(std::vector<LoadBatch> &bs, cmb200_engine *const *engines, int g) {
+static void load_teardown(std::vector<LoadBatch> &bs) {
+	for (LoadBatch &b : bs) explicit_bzero(&b.key, sizeof(b.key));
+}
+
+static int load_setup(std::vector<LoadBatch> &bs, cmb200_engine *const *engines, int g, const AeadKey &key) {
 	bs.resize(g);
-	for (int i = 0; i < g; i++)
+	for (int i = 0; i < g; i++) {
 		if (bs[i].setup(engines[i])) { set_error_msg("cmb200_load: no staging buffers"); return -1; }
+		bs[i].key = key;
+	}
 	return 0;
 }
 
@@ -1892,13 +2128,18 @@ extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char 
 	if (records_out) *records_out = 0;
 	if (g < 1 || !engines) { set_error_msg("cmb200_load_set: no engines"); return -1; }
 	SnapHeader h{};
-	FILE *f = open_snapshot(engines, g, path, h);
+	AeadKey key{};
+	bool has_key = false, sealed = false;
+	if (call_key(engines, g, "cmb200_load_set", key, has_key)) return -1;
+	FILE *f = open_snapshot(engines, g, path, h, key, has_key, &sealed);
 	if (!f) return -1;
 	std::vector<LoadBatch> bs;
-	uint64_t loaded = 0;
-	int rc = load_setup(bs, engines, g);
-	if (rc == 0) rc = load_records(f, h.records, bs, g, h.flags & 1u, nullptr, nullptr, &loaded);
+	uint64_t loaded = 0, ordinal = 0;
+	int rc = load_setup(bs, engines, g, key);
+	explicit_bzero(&key, sizeof(key));
+	if (rc == 0) rc = load_records(f, h.records, bs, g, h.flags & 1u, nullptr, nullptr, &loaded, sealed, base_nonce(h), &ordinal);
 	if (rc == 0) rc = load_flush_all(bs, h.flags & 1u, &loaded);
+	load_teardown(bs);
 	fclose(f);
 	if (records_out) *records_out = loaded;
 	return rc;
@@ -1908,22 +2149,40 @@ extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char 
 // bounds of every record header and the file's exact length (the record bytes are not read).  Leaves
 // the file at its first tombstone.  nullptr when the delta is missing, from another chain, out of
 // sequence, truncated or corrupt: the chain's valid run ends before it.
-static FILE *open_delta(const std::string &path, uint64_t id, uint32_t k, uint32_t pshift, uint32_t bsize, DeltaHeader &dh) {
+// A sealed delta (*sealed) also needs the engines' key (has_key): its header tag and its tombstones' tag
+// are checked here, and it is left at its first tombstone too.
+static FILE *open_delta(const std::string &path, uint64_t id, uint32_t k, uint32_t pshift, uint32_t bsize, DeltaHeader &dh,
+    cmb200_engine *e, const AeadKey &key, bool has_key, bool *sealed) {
 	FILE *f = fopen(path.c_str(), "rb");
 	if (!f) return nullptr;
-	bool ok = fread(&dh, sizeof(dh), 1, f) == 1 && memcmp(dh.magic, "CMB200D1", 8) == 0 && dh.version == 1 &&
+	bool ok = fread(&dh, sizeof(dh), 1, f) == 1;
+	*sealed = ok && memcmp(dh.magic, "CMB200F1", 8) == 0;
+	ok = ok && (*sealed ? has_key : memcmp(dh.magic, "CMB200D1", 8) == 0) && dh.version == 1 &&
 	    dh.pshift == pshift && dh.chain == id && dh.index == k && fseeko(f, 0, SEEK_END) == 0;
 	const uint64_t size = ok ? (uint64_t)ftello(f) : 0;
-	uint64_t pos = sizeof(dh) + 16 * dh.tombstones, bytes = 0;
+	const uint64_t head = sizeof(dh) + (*sealed ? AEAD_TAG : 0);
+	uint64_t pos = head + 16 * dh.tombstones + (*sealed ? AEAD_TAG : 0), bytes = 0;
 	ok = ok && dh.tombstones <= size / 16 && pos <= size;
 	for (uint64_t i = 0; ok && i < dh.records; i++) {
 		SnapRecord r;
-		ok = pos + sizeof(r) <= size && fseeko(f, (off_t)pos, SEEK_SET) == 0 && fread(&r, sizeof(r), 1, f) == 1 &&
-		    r.len >= 24 && r.len <= 24u + bsize + 1024u;
-		pos += sizeof(r) + (((uint64_t)r.len + 15) & ~15ull);
+		const size_t rh = *sealed ? 8 : sizeof(r);           // a sealed record's clear {u32 len, u32 0}
+		ok = pos + rh <= size && fseeko(f, (off_t)pos, SEEK_SET) == 0 && fread(&r, rh, 1, f) == 1;
+		if (*sealed) { r.len = (uint32_t)r.ts; r.zero = (uint32_t)(r.ts >> 32); ok = ok && r.zero == 0; }
+		ok = ok && r.len >= 24 && r.len <= 24u + bsize + 1024u;
+		pos += *sealed ? seal_record_bytes(r.len) : sizeof(r) + (((uint64_t)r.len + 15) & ~15ull);
 		bytes += r.len;
 	}
-	ok = ok && pos == size && bytes == dh.bytes && fseeko(f, sizeof(dh), SEEK_SET) == 0;
+	ok = ok && pos == size && bytes == dh.bytes;
+	if (ok && *sealed) {
+		// the header, then the tombstones, under the engines' key
+		uint8_t tag[16];
+		std::vector<uint8_t> tombs(16 * dh.tombstones);
+		ok = fseeko(f, sizeof(dh), SEEK_SET) == 0 && fread(tag, 16, 1, f) == 1 &&
+		    aead_check(e, key, dh.pad, 0, &dh, sizeof(dh), tag) == 1 &&
+		    (tombs.empty() || fread(tombs.data(), tombs.size(), 1, f) == 1) && fread(tag, 16, 1, f) == 1 &&
+		    aead_check(e, key, dh.pad, 1, tombs.data(), tombs.size(), tag) == 1;
+	}
+	ok = ok && fseeko(f, (off_t)head, SEEK_SET) == 0;
 	if (!ok) { fclose(f); return nullptr; }
 	return f;
 }
@@ -1966,6 +2225,10 @@ struct cmb200_loader {
 	uint64_t id = 0, total = 0, before = 0, loaded = 0;
 	std::vector<FILE *> ds;                              // the valid run of deltas, opened by the first step
 	std::vector<DeltaHeader> dhs;
+	std::vector<bool> dsealed;
+	bool sealed = false, has_key = false;                // the base is sealed; the engines hold a key
+	AeadKey key{};
+	uint64_t ordinal = 0;                                // the file ordinal of the next record of the file being read
 	bool checked = false, done = false;
 	int rc = 0;
 	size_t file = 0;                                     // files left, newest first: ds[file - 1], then the base
@@ -1975,6 +2238,8 @@ struct cmb200_loader {
 	AddrSet decided;
 	std::vector<LoadBatch> bs;
 	~cmb200_loader() {
+		explicit_bzero(&key, sizeof(key));
+		load_teardown(bs);
 		for (FILE *f : ds) fclose(f);
 		if (base) fclose(base);
 	}
@@ -1997,7 +2262,8 @@ extern "C" cmb200_loader *cmb200_load_open(cmb200_engine *const *engines, int g,
 	if (!l) { set_error_msg("cmb200_load_open: out of memory"); return nullptr; }
 	l->engines.assign(engines, engines + g);
 	l->base_path = base_path;
-	l->base = open_snapshot(engines, g, base_path, l->h);
+	if (call_key(engines, g, "cmb200_load_open", l->key, l->has_key)) { delete l; return nullptr; }
+	l->base = open_snapshot(engines, g, base_path, l->h, l->key, l->has_key, &l->sealed);
 	if (!l->base) { delete l; return nullptr; }
 	l->id = snap_chain_id(l->h);
 	// an upper bound of the records the load puts, from the headers alone: the base's and those of the
@@ -2014,14 +2280,15 @@ extern "C" cmb200_loader *cmb200_load_open(cmb200_engine *const *engines, int g,
 	for (uint32_t k = 1; l->id != 0; k++) {
 		DeltaHeader dh{};
 		FILE *f = fopen((l->base_path + ".d" + std::to_string(k)).c_str(), "rb");
-		const bool ok = f && fread(&dh, sizeof(dh), 1, f) == 1 && memcmp(dh.magic, "CMB200D1", 8) == 0 &&
+		const bool ok = f && fread(&dh, sizeof(dh), 1, f) == 1 &&
+		    (memcmp(dh.magic, "CMB200D1", 8) == 0 || memcmp(dh.magic, "CMB200F1", 8) == 0) &&
 		    dh.version == 1 && dh.chain == l->id && dh.index == k;
 		if (ok) l->total += bounded(dh.records, f, sizeof(dh));
 		if (f) fclose(f);
 		if (!ok) break;
 	}
 	for (int i = 0; i < g; i++) l->before += cmb200_entries(engines[i]);
-	if (load_setup(l->bs, engines, g)) { delete l; return nullptr; }
+	if (load_setup(l->bs, engines, g, l->key)) { delete l; return nullptr; }
 	for (int i = 0; i < g; i++) {
 		cmb200_engine *e = engines[i];
 		std::lock_guard<std::mutex> lk(e->mu);
@@ -2052,9 +2319,11 @@ extern "C" int cmb200_load_step(cmb200_loader *l, size_t max_records, uint64_t *
 		// the whole check of each delta (every record header and the file's length) before any is applied
 		for (uint32_t k = 1; l->id != 0; k++) {
 			DeltaHeader dh{};
-			FILE *f = open_delta(l->base_path + ".d" + std::to_string(k), l->id, k, l->h.pshift, l->engines[0]->bsize, dh);
+			bool sealed = false;
+			FILE *f = open_delta(l->base_path + ".d" + std::to_string(k), l->id, k, l->h.pshift, l->engines[0]->bsize, dh,
+			    l->engines[0], l->key, l->has_key, &sealed);
 			if (!f) break;
-			l->ds.push_back(f); l->dhs.push_back(dh);
+			l->ds.push_back(f); l->dhs.push_back(dh); l->dsealed.push_back(sealed);
 		}
 		l->file = l->ds.size() + 1;
 		l->checked = true;
@@ -2065,21 +2334,25 @@ extern "C" int cmb200_load_step(cmb200_loader *l, size_t max_records, uint64_t *
 		const bool delta = l->file > 1;
 		FILE *f = delta ? l->ds[l->file - 2] : l->base;
 		const bool with_fp = (delta ? l->dhs[l->file - 2].flags : l->h.flags) & 1u;
+		const bool sealed = delta ? l->dsealed[l->file - 2] : l->sealed;
 		if (!l->started) {
 			if (delta) {
 				const DeltaHeader &dh = l->dhs[l->file - 2];
 				l->tombs.resize(dh.tombstones);
-				if (dh.tombstones && fread(l->tombs.data(), 16, l->tombs.size(), f) != l->tombs.size()) {
+				if ((dh.tombstones && fread(l->tombs.data(), 16, l->tombs.size(), f) != l->tombs.size()) ||
+				    (sealed && fseeko(f, AEAD_TAG, SEEK_CUR) != 0)) {
 					l->rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
 				}
 				l->left = dh.records;
 			} else {
 				l->left = l->h.records;
 			}
+			l->ordinal = 0;
 			l->started = true;
 		}
 		const uint64_t n = l->left < budget ? l->left : (uint64_t)budget;
-		l->rc = load_records(f, n, l->bs, g, with_fp, &l->decided, delta ? &l->decided : nullptr, &l->loaded);
+		l->rc = load_records(f, n, l->bs, g, with_fp, &l->decided, delta ? &l->decided : nullptr, &l->loaded, sealed,
+		    delta ? l->dhs[l->file - 2].pad : base_nonce(l->h), &l->ordinal);
 		l->left -= n;
 		budget -= (size_t)n;
 		if (l->rc == 0 && (l->left == 0 || budget == 0)) l->rc = load_flush_all(l->bs, with_fp, &l->loaded);
@@ -3083,4 +3356,75 @@ extern "C" uint64_t cmb200_gen_stream_ids(uint64_t seed2, size_t n, double dup, 
 extern "C" void cmb200_gen_addr(uint64_t seed, uint64_t cid, int pshift, uint64_t *offset_out, uint64_t *nhid_out) {
 	*offset_out = sg_offset(cid, pshift);
 	*nhid_out = sg_nhid(seed, cid);
+}
+
+// ---- encryption at rest: the engine's file key and the kernel-level AEAD ----------------------
+
+extern "C" int cmb200_set_file_key(cmb200_engine *e, const uint8_t *key) {
+	if (!e) { set_error_msg("cmb200_set_file_key: no engine"); return -1; }
+	std::lock_guard<std::mutex> lk(e->mu);
+	if (key) { memcpy(e->key.w, key, 32); e->has_key = true; }
+	else { explicit_bzero(&e->key, sizeof(e->key)); e->has_key = false; }
+	return 0;
+}
+
+extern "C" uint64_t cmb200_load_rejected(cmb200_engine *e) { return e ? e->load_rejected.load() : 0; }
+
+// n messages through k_seal (open = false) or k_open (open = true), staged in one device buffer: each
+// message's AAD, text and tag 16-byte aligned.
+static int aead_batch(bool open, int device, const uint8_t *key, size_t n, const uint8_t *nonces,
+    const uint8_t *const *aad, const size_t *aad_len, const uint8_t *const *in, const size_t *len,
+    uint8_t *const *out, uint8_t *ok_out) {
+	if (n == 0) return 0;
+	if (!key || !nonces || !in || !len || !out || (open && !ok_out)) { set_error_msg("cmb200_aead_batch: missing argument"); return -1; }
+	if (n > 0xffffffffu) { set_error_msg("cmb200_aead_batch: too many messages"); return -1; }
+	if (select_device(device)) return -1;
+	std::vector<size_t> o_aad(n), o_txt(n);
+	size_t total = 0;
+	for (size_t i = 0; i < n; i++) {
+		o_aad[i] = total; total += align16(aad_len ? aad_len[i] : 0);
+		o_txt[i] = total; total += align16(len[i] + 16);
+	}
+	const size_t o_msg = total, o_ok = o_msg + n * sizeof(AeadMsg);
+	DevMem<uint8_t> d;
+	if (d.alloc(o_ok + n + 256)) return -1;
+	std::vector<uint8_t> host(o_msg, 0);
+	std::vector<AeadMsg> msgs(n);
+	for (size_t i = 0; i < n; i++) {
+		const size_t al = aad_len ? aad_len[i] : 0;
+		if (al) memcpy(host.data() + o_aad[i], aad[i], al);
+		if (len[i] || open) memcpy(host.data() + o_txt[i], in[i], len[i] + (open ? 16 : 0));
+		AeadMsg &m = msgs[i];
+		m = AeadMsg{};
+		m.aad = d + o_aad[i]; m.aad_len = al;             // never null: a plain message
+		m.src = m.dst = d + o_txt[i]; m.len = len[i];
+		memcpy(m.nonce, nonces + 12 * i, 12);
+	}
+	AeadKey k;
+	memcpy(k.w, key, 32);
+	CMB_CHECK(cudaMemcpy(d, host.data(), o_msg, cudaMemcpyHostToDevice));
+	CMB_CHECK(cudaMemcpy(d + o_msg, msgs.data(), n * sizeof(AeadMsg), cudaMemcpyHostToDevice));
+	const int rc = open ? launch_open((const AeadMsg *)(d + o_msg), (uint32_t)n, k, 0, nullptr, nullptr, d + o_ok, nullptr, 0)
+	                    : launch_seal((const AeadMsg *)(d + o_msg), (uint32_t)n, k, 0);
+	explicit_bzero(&k, sizeof(k));
+	if (rc) return -1;
+	CMB_CHECK(cudaMemcpy(host.data(), d, o_msg, cudaMemcpyDeviceToHost));
+	if (open) CMB_CHECK(cudaMemcpy(ok_out, d + o_ok, n, cudaMemcpyDeviceToHost));
+	for (size_t i = 0; i < n; i++) {
+		// a message that does not open releases no plaintext
+		if (open && !ok_out[i]) memset(out[i], 0, len[i]);
+		else memcpy(out[i], host.data() + o_txt[i], len[i] + (open ? 0 : 16));
+	}
+	return 0;
+}
+
+extern "C" int cmb200_aead_seal_batch(int device, const uint8_t *key, size_t n, const uint8_t *nonces,
+    const uint8_t *const *aad, const size_t *aad_len, const uint8_t *const *msg, const size_t *msg_len, uint8_t *const *out) {
+	return aead_batch(false, device, key, n, nonces, aad, aad_len, msg, msg_len, out, nullptr);
+}
+
+extern "C" int cmb200_aead_open_batch(int device, const uint8_t *key, size_t n, const uint8_t *nonces,
+    const uint8_t *const *aad, const size_t *aad_len, const uint8_t *const *sealed, const size_t *text_len,
+    uint8_t *const *out, uint8_t *ok_out) {
+	return aead_batch(true, device, key, n, nonces, aad, aad_len, sealed, text_len, out, ok_out);
 }

@@ -5,6 +5,7 @@
 //   k_fingerprint EF128 alone
 //   k_compose / k_upsert / k_lookup / k_unset / k_sample / k_invalidate_*   the HBM key table
 //   k_streamgen   synthetic benchmark input
+//   k_seal / k_open  ChaCha20-Poly1305 of snapshot records, headers and tombstone blocks (aead.cuh)
 #include "kernels.h"
 #include "common.cuh"
 #include "../../include/cachemap_b200.h"
@@ -15,6 +16,7 @@
 #include "lz4_decode.cuh"
 #include "lz4_decode_cta.cuh"
 #include "streamgen.cuh"
+#include "aead.cuh"
 #include <cub/block/block_scan.cuh>
 
 namespace cmb {
@@ -134,10 +136,8 @@ __global__ void k_upsert(TableView t, const unsigned long long *addr, const uint
 // So a record is passed over (slot_idx 0xffffffff, which k_restore skips) when its key's slot, or a
 // tombstone on the key's probe chain before it, was written at or above floor: the key was put, moved or
 // removed since the load opened, and the file's page is older than that change.
-__global__ void k_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
-    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx) {
-	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
+__device__ __forceinline__ uint32_t upsert_floor_one(const TableView &t, const unsigned long long *addr, uint32_t i,
+    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor) {
 	const unsigned long long key = fnv_addr(addr[2 * i], addr[2 * i + 1]);
 	bool newer = false;
 	if (key == KEY_EMPTY || key == KEY_TOMB) {
@@ -158,7 +158,20 @@ __global__ void k_upsert_floor(TableView t, const unsigned long long *addr, uint
 		idx = table_find_or_claim(t, key);
 		if (idx != 0xffffffffu) atomicMax(&t.slots[idx].seq, seq0 + seq_stride * i);
 	}
-	slot_idx[i] = idx;
+	return idx;
+}
+__global__ void k_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
+    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx) {
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	slot_idx[i] = upsert_floor_one(t, addr, i, seq0, seq_stride, floor);
+}
+// k_upsert_floor over the records k_open let through (an encrypted load): valid[i] == 0 claims nothing.
+__global__ void k_upsert_floor_valid(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
+    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx) {
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	slot_idx[i] = valid[i] ? upsert_floor_one(t, addr, i, seq0, seq_stride, floor) : 0xffffffffu;
 }
 
 __global__ void k_lookup(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
@@ -1811,6 +1824,13 @@ int launch_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n,
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
+int launch_upsert_floor_valid(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
+    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_upsert_floor_valid<<<GRID1D(n), 0, st>>>(t, addr, valid, n, seq0, seq_stride, floor, slot_idx);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
 int launch_lookup(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
     int32_t *status, uint64_t *rec_off, uint32_t *vlen, unsigned long long *ts_out, cudaStream_t st, uint32_t *idx_out) {
 	if (n == 0) return 0;
@@ -2299,6 +2319,84 @@ int launch_patch(uint8_t *pages, uint32_t nbytes, uint32_t rows, const int32_t *
     const PatchSpan *spans, const uint8_t *bytes, uint8_t *valid, cudaStream_t st) {
 	if (rows == 0) return 0;
 	k_patch<<<rows, 256, 0, st>>>(pages, nbytes, status, first, spans, bytes, valid);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+// ---- ChaCha20-Poly1305 of snapshot files ----------------------------------------------------
+constexpr int AEAD_WARPS = 8;
+
+__global__ void __launch_bounds__(AEAD_WARPS * 32) k_seal(const AeadMsg *msgs, uint32_t n, AeadKey key) {
+	const int lane = threadIdx.x & 31;
+	const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	if (i >= n) return;
+	const AeadMsg m = msgs[i];
+	AeadText t;
+	const uint8_t *aad = m.aad;
+	uint64_t aad_len = m.aad_len;
+	uint8_t *tag;
+	if (aad) {
+		t.src = m.src; t.dst = m.dst; t.len = m.len; t.head_words = 0;
+		tag = m.dst + m.len;
+	} else {
+		// the clear part {u32 len, u32 0, u, l}, then the text {ts, fp_hi, fp_lo} + the record after its address
+		const uint64_t *rec = reinterpret_cast<const uint64_t *>(m.src);
+		if (lane < 3) reinterpret_cast<uint64_t *>(m.dst)[lane] = lane == 0 ? (uint64_t)(uint32_t)m.len : rec[lane - 1];
+		const uint64_t end = 24 + m.len + 8 + 16, padded = seal_record_bytes(m.len);
+		for (uint64_t k = end + lane; k < padded; k += 32) m.dst[k] = 0;
+		__syncwarp();
+		aad = m.dst; aad_len = 24;
+		t.src = m.src + 16 - 24; t.dst = m.dst + 24; t.len = m.len + 8; t.head_words = 3;
+		t.head[0] = m.ts; t.head[1] = m.fp_hi; t.head[2] = m.fp_lo;
+		tag = m.dst + 24 + t.len;
+	}
+	aead_warp<false>(key.w, m.nonce, aad, aad_len, t, tag, lane);
+}
+
+__global__ void __launch_bounds__(AEAD_WARPS * 32) k_open(const AeadMsg *msgs, uint32_t n, AeadKey key, uint32_t bsize,
+    unsigned long long *ts, uint64_t *fp, uint8_t *ok, unsigned long long *rejected) {
+	const int lane = threadIdx.x & 31;
+	const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+	if (i >= n) return;
+	const AeadMsg m = msgs[i];
+	AeadText t;
+	t.head_words = 0;
+	if (m.aad) {
+		t.src = m.src; t.dst = m.dst; t.len = m.len;
+		bool good = aead_warp<true>(key.w, m.nonce, m.aad, m.aad_len, t, const_cast<uint8_t *>(m.src) + m.len, lane);
+		if (lane == 0) {
+			ok[i] = good;
+			if (!good && rejected) atomicAdd(rejected, 1ull);
+		}
+		return;
+	}
+	uint8_t *rec = m.dst;
+	const uint32_t len = *reinterpret_cast<const uint32_t *>(rec);
+	t.src = rec + 24; t.dst = rec + 24; t.len = (uint64_t)len + 8;
+	bool good = aead_warp<true>(key.w, m.nonce, rec, 24, t, rec + 24 + t.len, lane);
+	__syncwarp();
+	if (lane != 0) return;
+	// the record must be what filemap_set would have stored (filemap.c:124-147): k_restore trusts
+	// compressed_length
+	const int32_t clen = *reinterpret_cast<const int32_t *>(rec + 48);
+	good = good && clen >= 0 && (uint32_t)clen <= bsize + 1024u && len == 24u + (clen ? (uint32_t)clen : bsize);
+	uint64_t *w = reinterpret_cast<uint64_t *>(rec);
+	ts[i] = w[3]; fp[2 * i] = w[4]; fp[2 * i + 1] = w[5];
+	w[4] = w[1]; w[5] = w[2];
+	ok[i] = good;
+	if (!good && rejected) atomicAdd(rejected, 1ull);
+}
+
+int launch_seal(const AeadMsg *msgs, uint32_t n, const AeadKey &key, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_seal<<<(n + AEAD_WARPS - 1) / AEAD_WARPS, AEAD_WARPS * 32, 0, st>>>(msgs, n, key);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_open(const AeadMsg *msgs, uint32_t n, const AeadKey &key, uint32_t bsize, unsigned long long *ts,
+    uint64_t *fp, uint8_t *ok, unsigned long long *rejected, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_open<<<(n + AEAD_WARPS - 1) / AEAD_WARPS, AEAD_WARPS * 32, 0, st>>>(msgs, n, key, bsize, ts, fp, ok, rejected);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

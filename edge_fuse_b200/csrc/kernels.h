@@ -374,4 +374,37 @@ int launch_patch(uint8_t *pages, uint32_t nbytes, uint32_t rows, const int32_t *
 
 int sm_count();
 
+// ---- ChaCha20-Poly1305 (RFC 8439 §2.8) of snapshot files (aead.cuh; DESIGN.md §2 "Encryption at rest") ----
+struct AeadKey { uint32_t w[8]; };
+// One message of k_seal / k_open, with nonce {nonce[0], nonce[1], nonce[2]} (little-endian words).
+//   aad != null: a plain message.  Seal: len bytes at src -> ciphertext at dst, then the tag at dst + len.
+//     Open: ciphertext at src, its tag at src + len -> plaintext at dst (may equal src).
+//   aad == null: a snapshot record.  Seal: src is the record {u, l, compressed_length, pad, payload} of len
+//     bytes; dst gets {u32 len, u32 0, u, l} (the AAD), the ciphertext of {ts, fp_hi, fp_lo,
+//     compressed_length, pad, payload}, the tag, and zeros up to seal_record_bytes(len).  Open: src = dst
+//     is such a sealed record (len from its first word); in place it becomes, at dst + 32, the record
+//     {u, l, compressed_length, pad, payload} that launch_restore reads, and ts / fp go to the arrays.
+// src and dst are 8-byte aligned (sealed records 16-byte aligned).
+struct AeadMsg {
+	const uint8_t *src;
+	uint8_t *dst;
+	const uint8_t *aad;
+	unsigned long long len, aad_len;
+	unsigned long long ts, fp_hi, fp_lo;
+	uint32_t nonce[3], pad;
+};
+static_assert(sizeof(AeadMsg) == 80, "aead message layout");
+__host__ __device__ inline unsigned long long seal_record_bytes(unsigned long long len) { return (len + 48 + 15) & ~15ull; }
+// k_seal: one warp per message.
+int launch_seal(const AeadMsg *msgs, uint32_t n, const AeadKey &key, cudaStream_t st);
+// k_open: one warp per message.  ok[i] = tag right (and, for a record, compressed_length as filemap_set
+// stores it: <= bsize + 1024 and len == 24 + (clen ? clen : bsize)); *rejected (nullable) += the others.
+// Records: ts[i] and fp[2i], fp[2i + 1] get the record's values.
+int launch_open(const AeadMsg *msgs, uint32_t n, const AeadKey &key, uint32_t bsize, unsigned long long *ts,
+    uint64_t *fp, uint8_t *ok, unsigned long long *rejected, cudaStream_t st);
+// launch_upsert_floor for records only some of which are valid: valid[i] == 0 claims nothing (slot_idx
+// 0xffffffff, which k_restore skips).
+int launch_upsert_floor_valid(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
+    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st);
+
 }  // namespace cmb

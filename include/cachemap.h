@@ -117,6 +117,16 @@ void cachemap_pwrite(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, u
  * runs, checkpoint ticks are skipped; cachemap_checkpoint and cachemap_free wait for the load to end and
  * then write a base.  If the engine cannot load in steps, the call waits as with "wait".  Any other
  * value warns and waits.
+ *
+ * CMB200_KEY_FILE=<path> encrypts the directory at rest: a file of 32 raw bytes or 64 hex digits, read
+ * once when the engines start (after any fork) and set on every engine (cmb200_set_file_key).  Every
+ * file the map writes is then sealed with ChaCha20-Poly1305, and a plaintext directory still loads (the
+ * next file written is sealed).  If the variable is set and the file is missing, unreadable or
+ * malformed, the map warns on stderr and runs without persistence: it neither reads nor writes the
+ * directory.  If the directory's base is sealed and does not load (no key, another key, a damaged
+ * file), the map warns, starts empty and never writes the directory, not even at cachemap_free, so
+ * that the sealed file stays as it was for a restart with the right key.  Records whose tag fails are
+ * left out and counted (cmb200_load_rejected); the rest loads.
  */
 int cachemap_checkpoint(struct cachemap *cm);
 /* 1 while a background load runs (*loaded = records stored so far, *total = records the files hold by

@@ -320,6 +320,22 @@ int cmb200_freq_stats(cmb200_engine *e, struct cmb200_freq_stats *out);
 int cmb200_save_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out);
 int cmb200_load_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out);
 
+/* ---- encryption at rest (DESIGN.md §2 "Encryption at rest") ----
+ * cmb200_set_file_key sets the 32-byte ChaCha20-Poly1305 key of the files e writes and reads; NULL clears
+ * it.  The key is held in host memory and zeroed on clear and on destroy.  Every call that writes or
+ * reads files (cmb200_save_set, cmb200_snapshot_begin, cmb200_chain_begin, cmb200_load_set,
+ * cmb200_load_chain, cmb200_load_open) takes the key of its engines, and fails (-1 or NULL) when they hold
+ * different keys.  With a key, every file written is sealed: a base "CMB200E1", a delta "CMB200F1"
+ * (older builds refuse both as "not a snapshot").  With a key, sealed and plaintext files load alike (a
+ * plaintext file is the migration path: the next base is sealed).  A sealed file loaded without its key
+ * fails at the header and stores nothing; a sealed delta that does not open ends the chain's run before
+ * it, as a damaged delta does.  A record whose tag or length fails is not stored, and counted:
+ * cmb200_load_rejected returns the count since the engine was created.  The record addresses {u, l} and
+ * sizes stay in the clear (authenticated); page bytes, fingerprints, timestamps and compressed lengths
+ * are encrypted. */
+int cmb200_set_file_key(cmb200_engine *e, const uint8_t *key);
+uint64_t cmb200_load_rejected(cmb200_engine *e);
+
 typedef struct cmb200_snapshot cmb200_snapshot;
 /* Starts a snapshot of g engines (the cmb200_save_set file, written to path.tmp).  Each engine is
  * locked only while its live records (both tiers) are listed, after its stream has been synchronised,
@@ -556,6 +572,18 @@ int cmb200_fingerprint_dev(cmb200_engine *e, size_t n, const void *pages_dev, ui
  * ok_out[i] = 1: the key's record is local and word 0 names its location and length;
  * 0: the key has a record without valid checkpoints; -1: absent, remote, or no side table. */
 int cmb200_read_checkpoints(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint32_t *words_out, int32_t *ok_out);
+
+/* ChaCha20-Poly1305 (RFC 8439 §2.8) of n messages on the GPU, through the kernels that seal and open
+ * snapshot files (k_seal / k_open).  key: 32 bytes; nonces: n x 12 bytes; aad[i] / aad_len[i] (aad_len
+ * nullable: no AAD).  Seal: out[i] gets msg_len[i] bytes of ciphertext, then the 16-byte tag.  Open:
+ * sealed[i] is text_len[i] bytes of ciphertext then the tag; ok_out[i] = 1 and out[i] the plaintext when
+ * the tag is right, else ok_out[i] = 0 and out[i] zeros.  0 / -1 (error set). */
+int cmb200_aead_seal_batch(int device, const uint8_t *key, size_t n, const uint8_t *nonces,
+    const uint8_t *const *aad, const size_t *aad_len, const uint8_t *const *msg, const size_t *msg_len,
+    uint8_t *const *out);
+int cmb200_aead_open_batch(int device, const uint8_t *key, size_t n, const uint8_t *nonces,
+    const uint8_t *const *aad, const size_t *aad_len, const uint8_t *const *sealed, const size_t *text_len,
+    uint8_t *const *out, uint8_t *ok_out);
 
 /* ---- synthetic streams (SURVEY.md §8d), same definition on host and device ---- */
 void cmb200_gen_chunk_host(uint64_t seed, uint64_t cid, uint32_t bsize, void *out);

@@ -62,6 +62,14 @@ to_lmdb(const char *snap, char *dir, uint64_t capacity, int pshift)
 {
 	FILE *f = fopen(snap, "rb");
 	struct snap_header h;
+	if (f && fread(&h, sizeof(h), 1, f) == 1 && memcmp(h.magic, "CMB200E1", 8) == 0) {
+		/* a sealed base (cmb200_set_file_key): its records are ciphertext, and this tool holds no key */
+		fprintf(stderr, "snap2lmdb: %s is an encrypted snapshot (CMB200E1): this tool holds no key; open the "
+		    "cache directory with the library and its CMB200_KEY_FILE, and write it without a key first\n", snap);
+		fclose(f);
+		return 1;
+	}
+	if (f) rewind(f);
 	if (!f || fread(&h, sizeof(h), 1, f) != 1 || memcmp(h.magic, "CMB200S1", 8) != 0 || (int)h.pshift != pshift) {
 		fprintf(stderr, "snap2lmdb: %s is not a snapshot with pshift %d\n", snap, pshift);
 		return 1;
