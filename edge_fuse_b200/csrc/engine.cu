@@ -373,6 +373,14 @@ struct cmb200_engine {
 	std::atomic<uint64_t> load_rejected{0};   // records whose tag or length failed, since create
 };
 
+// Bytes of a page-ring buffer (d_pages[i]), which a load also stages its slices in: host_batch pages, and
+// never less than the largest record a file can hold, sealed ({len, 0, u, l}, the 24 + bsize + 1024 bytes
+// of the record, the tag, padding), so that an engine with a small max_batch still loads every file.
+static uint64_t load_stage_bytes(const cmb200_engine *e) {
+	const uint64_t ring = (uint64_t)e->host_batch * e->bsize, largest = seal_record_bytes(24ull + e->bsize + 1024u);
+	return ring > largest ? ring : largest;
+}
+
 // CMB200_TOUCH: the stamp a get raises its hits' ts to, taken at launch from the clock the drop-in's puts
 // stamp with (cachemap_api.c:now_ns, the reference's cachemap.c:10-15).  Never 0 (GetJob::touch_ts).
 static unsigned long long touch_stamp() {
@@ -494,8 +502,7 @@ static int engine_init(cmb200_engine *e, const cmb200_config *cfg) {
 		const uint64_t row = (uint64_t)e->bsize + 1024 > bound ? (uint64_t)e->bsize + 1024 : bound;
 		e->stage_stride = (row + 15) & ~15ull;
 	}
-	if (e->d_pages[0].alloc((uint64_t)e->host_batch * e->bsize + 256) ||
-	    e->d_pages[1].alloc((uint64_t)e->host_batch * e->bsize + 256)) return -1;
+	if (e->d_pages[0].alloc(load_stage_bytes(e) + 256) || e->d_pages[1].alloc(load_stage_bytes(e) + 256)) return -1;
 	// one stage row per resident warp / group of the encode kernels (store mode), not per chunk
 	if (e->d_stage.alloc((uint64_t)16384 * e->stage_stride + 256)) return -1;
 	// small per-chunk arrays are sized for a whole slice of a call (META_CAP chunks) so that
@@ -1879,7 +1886,7 @@ struct LoadBatch {
 	int setup(cmb200_engine *eng) {
 		e = eng;
 		CMB_CHECK(cudaSetDevice(e->device));
-		cap = (size_t)e->host_batch * e->bsize;
+		cap = (size_t)load_stage_bytes(e);
 		B = e->max_batch < cmb200_engine::META_CAP ? e->max_batch : cmb200_engine::META_CAP;
 		off.resize(B); ts.resize(B); fps.resize(2 * B); addr.resize(B); msg.resize(B);
 		if (blob.alloc(cap) || d_off.alloc(B * 8) || d_fp.alloc(B * 16) || d_msg.alloc(B * sizeof(AeadMsg)) || d_rej.alloc(8)) return -1;
