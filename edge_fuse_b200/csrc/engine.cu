@@ -25,10 +25,12 @@
 #include <string>
 #include <new>
 #include <thread>
+#include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
 #include <utility>
 #include <stdio.h>
+#include <stddef.h>
 #include <stdlib.h>
 #include <string.h>
 #include <time.h>
@@ -1380,37 +1382,74 @@ static int live_records(cmb200_engine *e, bool arena_only, std::vector<ExportEnt
 // The reference's store is persistent because it IS a set of LMDB files under <cachedir>
 // (filemap.c:57,71-72).  Here the store lives in HBM, so it is saved to / restored from one file of
 // records, each exactly the LMDB value of the reference (24-byte data_prefix + payload,
-// filemap.c:140-147) preceded by {ts (the LMDB attribute), length, fingerprint}:
+// filemap.c:140-147) preceded by {ts (the LMDB attribute), length, fingerprint}.  It does not depend on
+// the table geometry or the arena layout, so a snapshot loads into an engine of any capacity (records
+// that do not fit are dropped like puts into a full store).  The format, every file of it:
 //
-//   header   "CMB200S1" | u32 version=1 | u32 pshift | u64 records | u64 payload bytes | u32 flags | pad to 64
-//   record   u64 ts | u64 fp_hi | u64 fp_lo | u32 len | u32 0 | len bytes {u, l, compressed_length, pad, payload} | pad to 16
+//   base header   "CMB200S1" | u32 version=1 | u32 pshift | u64 records | u64 payload bytes | u32 flags |
+//                 u32 0 | u64 chain id | u64 file nonce | u64 0
+//   delta header  "CMB200D1" | u32 version=1 | u32 pshift | u64 chain id | u32 k | u32 flags |
+//                 u64 tombstones | u64 records | u64 record bytes | u64 file nonce
+//   record        u64 ts | u64 fp_hi | u64 fp_lo | u32 len | u32 0 | len bytes {u, l, compressed_length, pad,
+//                 payload} | zeros to 16
 //
-// It does not depend on the table geometry or the arena layout, so a snapshot loads into an engine
-// of any capacity (records that do not fit are dropped like puts into a full store).
+// A base is the header, then its records.  The chain id is 0 outside a chain (cmb200_save_set); a delta
+// (below) is its header, its tombstones (16-byte addresses), then its records.  flags bit 0: the records'
+// fingerprints are set.  A record's len is at least 24 and at most 24 + bsize + 1024 (record_len_ok).
+//
+// Sealed (encryption at rest, DESIGN.md §2): a base is "CMB200E1" and a delta "CMB200F1", with a fresh
+// 64-bit file nonce in the header (0 in a plain file).  The header is followed by the tag of an AEAD seal
+// with an empty text and the header as AAD; a delta's tombstones are clear and followed by the tag of the
+// i = 1 seal with the tombstones as AAD.  Each record is {u32 len, u32 0, u64 u, u64 l} (AAD), the
+// ciphertext of {ts, fp_hi, fp_lo, compressed_length, pad, payload}, the tag, zeros to 16
+// (seal_record_bytes(len)).  The AEAD nonce is {file nonce, u32 i}: i = 0 the header, 1 the tombstones,
+// 2 + ordinal the file's ordinal-th record.  All of it is sealed and opened by k_seal / k_open; the host
+// holds no cipher.
 struct SnapHeader {
 	char magic[8];
 	uint32_t version, pshift;
 	uint64_t records, bytes;
-	uint32_t flags, pad[7];
+	uint32_t flags, zero;
+	uint64_t chain, nonce, reserved[1];
 };
+static_assert(offsetof(SnapHeader, chain) == 40, "snapshot header: chain id");
+static_assert(offsetof(SnapHeader, nonce) == 48, "snapshot header: file nonce");
 static_assert(sizeof(SnapHeader) == 64, "snapshot header");
+struct DeltaHeader {
+	char magic[8];
+	uint32_t version, pshift;
+	uint64_t chain;
+	uint32_t index, flags;
+	uint64_t tombstones, records, bytes, nonce;
+};
+static_assert(sizeof(DeltaHeader) == 64, "delta header");
 struct SnapRecord { uint64_t ts, fp_hi, fp_lo; uint32_t len, zero; };
 static_assert(sizeof(SnapRecord) == 32, "snapshot record header");
-static const size_t SNAP_WINDOW = 64u << 20;
 
-// ---- encryption at rest (DESIGN.md §2 "Encryption at rest") ----
-// With a key, a base is "CMB200E1" and a delta "CMB200F1": the header above with a fresh 64-bit file
-// nonce (a base: header bytes 48..55; a delta: its last 8 bytes), then the tag of an AEAD seal with an
-// empty text and the header as AAD.  A delta's clear tombstones follow, then the tag of the i = 1 seal
-// with the tombstones as AAD.  Each record is {u32 len, u32 0, u64 u, u64 l} (AAD), the ciphertext of
-// {ts, fp_hi, fp_lo, compressed_length, pad, payload}, the tag, zeros to 16 (seal_record_bytes(len)).
-// The AEAD nonce is {file nonce, u32 i}: i = 0 the header, 1 the tombstones, 2 + ordinal the file's
-// ordinal-th record.  All of it is sealed and opened by k_seal / k_open; the host holds no cipher.
+// The magic of each kind of file, [delta][sealed].
+static const char SNAP_MAGIC[2][2][9] = {{"CMB200S1", "CMB200E1"}, {"CMB200D1", "CMB200F1"}};
+
+// Reads the header at the start of f (nullable: no file) and checks what every reader checks: a magic of
+// this library for a base (SnapHeader) or a delta (DeltaHeader), and version 1.  *sealed: a sealed file.
+template <class Header>
+static bool read_header(FILE *f, Header &h, bool *sealed) {
+	const bool delta = std::is_same<Header, DeltaHeader>::value;
+	if (!f || fread(&h, sizeof(h), 1, f) != 1 || h.version != 1) return false;
+	for (int s = 0; s < 2; s++)
+		if (memcmp(h.magic, SNAP_MAGIC[delta][s], 8) == 0) { *sealed = s; return true; }
+	return false;
+}
+
+// A record's bytes in a plain or a sealed file.
+static uint64_t record_bytes(bool sealed, uint64_t len) {
+	return sealed ? seal_record_bytes(len) : sizeof(SnapRecord) + ((len + 15) & ~15ull);
+}
+static bool record_len_ok(uint32_t len, uint32_t bsize) { return len >= 24 && len <= 24u + bsize + 1024u; }
+
+static const size_t SNAP_WINDOW = 64u << 20;
 static const size_t SEAL_MAX_RECS = 1u << 16;                // records per sealed window
 static const size_t SEAL_STAGING = SNAP_WINDOW + SEAL_MAX_RECS * sizeof(AeadMsg);
 static const uint32_t AEAD_TAG = 16;
-
-static uint64_t base_nonce(const SnapHeader &h) { uint64_t v; memcpy(&v, &h.pad[3], 8); return v; }
 
 // One header or tombstone seal (open = false: tag written) or check (open: 1 = the tag is right, 0 = not)
 // of aad_len bytes with an empty text, on st through `scratch` (device, >= aad_len + 256 bytes).
@@ -1483,17 +1522,20 @@ static void snap_set_state(cmb200_engine *e, int state) {
 // without e->mu)  0 = written, -1 = a CUDA call failed (error set), -2 = a write failed.
 static int write_section(cmb200_engine *e, FILE *f, const std::vector<ExportEntry> &list) {
 	uint8_t *win = e->snap_win;
-	bool ok = true;
 	static const uint8_t zeros[16] = {0};
+	// one record, its bytes at src
+	const auto emit = [f](const ExportEntry &x, const uint8_t *src) {
+		const SnapRecord r{x.ts, x.fp_hi, x.fp_lo, x.len, 0};
+		const size_t padn = record_bytes(false, x.len) - sizeof(r) - x.len;
+		return fwrite(&r, sizeof(r), 1, f) == 1 && fwrite(src, x.len, 1, f) == 1 && (padn == 0 || fwrite(zeros, padn, 1, f) == 1);
+	};
+	bool ok = true;
 	size_t k = 0;
 	while (ok && k < list.size()) {
 		if (list[k].rec_off & REC_HOST) {
 			// host-tier records sort last and are written straight from the tier
-			const ExportEntry &x = list[k++];
-			SnapRecord r{x.ts, x.fp_hi, x.fp_lo, x.len, 0};
-			const size_t padn = (16 - (x.len & 15)) & 15;
-			ok = fwrite(&r, sizeof(r), 1, f) == 1 && fwrite(e->tier.host + (x.rec_off & ~REC_HOST), x.len, 1, f) == 1 &&
-			    (padn == 0 || fwrite(zeros, padn, 1, f) == 1);
+			ok = emit(list[k], e->tier.host + (list[k].rec_off & ~REC_HOST));
+			k++;
 			continue;
 		}
 		// one window of the arena starting at record k; the records wholly inside it are written out
@@ -1502,13 +1544,7 @@ static int write_section(cmb200_engine *e, FILE *f, const std::vector<ExportEntr
 		if (w1 > e->arena.size + 256) w1 = e->arena.size + 256;
 		CMB_CHECK(cudaMemcpyAsync(win, e->arena.base + w0, (size_t)(w1 - w0), cudaMemcpyDeviceToHost, e->snap_st));
 		CMB_CHECK(cudaStreamSynchronize(e->snap_st));
-		for (; k < list.size() && list[k].rec_off + list[k].len <= w1; k++) {
-			const ExportEntry &x = list[k];
-			SnapRecord r{x.ts, x.fp_hi, x.fp_lo, x.len, 0};
-			const size_t padn = (16 - (x.len & 15)) & 15;
-			ok = ok && fwrite(&r, sizeof(r), 1, f) == 1 && fwrite(win + (x.rec_off - w0), x.len, 1, f) == 1 &&
-			    (padn == 0 || fwrite(zeros, padn, 1, f) == 1);
-		}
+		for (; ok && k < list.size() && list[k].rec_off + list[k].len <= w1; k++) ok = emit(list[k], win + (list[k].rec_off - w0));
 	}
 	return ok ? 0 : -2;
 }
@@ -1528,7 +1564,7 @@ static int write_section_sealed(cmb200_engine *e, FILE *f, const std::vector<Exp
 		size_t bytes = 0;
 		for (; k < list.size() && msgs.size() < SEAL_MAX_RECS; k++) {
 			const ExportEntry &x = list[k];
-			const size_t sb = seal_record_bytes(x.len);
+			const size_t sb = record_bytes(true, x.len);
 			if (bytes + sb > SNAP_WINDOW) break;
 			AeadMsg m{};
 			m.src = x.rec_off & REC_HOST ? e->tier.dev + (x.rec_off & ~REC_HOST) : e->arena.base + x.rec_off;
@@ -1549,34 +1585,14 @@ static int write_section_sealed(cmb200_engine *e, FILE *f, const std::vector<Exp
 }
 
 // ---- snapshot chains (cmb200_chain_begin / cmb200_load_chain) ----
-// A base is the file above with a nonzero 64-bit chain id in bytes 40..47 (pad[1..2], zero in a file
-// written by cmb200_save_set).  Delta k of that chain, <base>.d<k>, holds what changed between tick k-1
-// (tick 0 = the base) and tick k:
-//
-//   header      "CMB200D1" | u32 version=1 | u32 pshift | u64 chain id | u32 k | u32 flags |
-//               u64 tombstones | u64 records | u64 record bytes | pad to 64
-//   tombstones  16-byte addresses that were live at tick k-1 and are not at tick k
-//   records     every live local record put since tick k-1, in the base's record format
+// A chain's base has a nonzero chain id.  Delta k of that chain, <base>.d<k>, holds what changed between
+// tick k-1 (tick 0 = the base) and tick k: its tombstones are the addresses that were live at tick k-1 and
+// are not at tick k, its records every live local record put since tick k-1.
 //
 // The store of a chain is the base, then for each delta in order its tombstones removed and its records
 // put.  "Put since tick k-1" is Slot::seq >= the engine's seq at tick k-1: every put raises the slot's
 // seq (k_upsert), a table rebuild copies it, and compaction, demotion and promotion leave it alone, so
 // a record that only moved is not in the delta.
-struct DeltaHeader {
-	char magic[8];
-	uint32_t version, pshift;
-	uint64_t chain;
-	uint32_t index, flags;
-	uint64_t tombstones, records, bytes, pad;
-};
-static_assert(sizeof(DeltaHeader) == 64, "delta header");
-
-static uint64_t snap_chain_id(const SnapHeader &h) {
-	uint64_t id;
-	memcpy(&id, &h.pad[1], 8);
-	return id;
-}
-
 enum { CHAIN_NONE = 0, CHAIN_BASE, CHAIN_DELTA };
 
 struct cmb200_snapshot {
@@ -1595,6 +1611,7 @@ struct cmb200_snapshot {
 	AeadKey key{};
 	uint64_t nonce = 0;
 	~cmb200_snapshot() { explicit_bzero(&key, sizeof(key)); }
+	const void *head() const { return chain == CHAIN_DELTA ? (const void *)&dh : (const void *)&h; }   // the file's header
 };
 
 // The writer thread: header, then each engine's section; an engine is released as soon as its section
@@ -1603,11 +1620,10 @@ struct cmb200_snapshot {
 static int write_sealed_head(cmb200_snapshot *s) {
 	cmb200_engine *e = s->engines[0];
 	CMB_CHECK(cudaSetDevice(e->device));
-	const bool delta = s->chain == CHAIN_DELTA;
 	uint8_t tag[16];
-	if (aead_one(e->snap_dev, e->snap_st, false, s->key, s->nonce, 0, delta ? (const void *)&s->dh : (const void *)&s->h, 64, tag)) return -1;
-	if (fwrite(delta ? (const void *)&s->dh : (const void *)&s->h, 64, 1, s->f) != 1 || fwrite(tag, 16, 1, s->f) != 1) return -2;
-	if (!delta) return 0;
+	if (aead_one(e->snap_dev, e->snap_st, false, s->key, s->nonce, 0, s->head(), 64, tag)) return -1;
+	if (fwrite(s->head(), 64, 1, s->f) != 1 || fwrite(tag, 16, 1, s->f) != 1) return -2;
+	if (s->chain != CHAIN_DELTA) return 0;
 	const size_t tb = s->tombs.size() * 16;
 	if (e->snap_dev.grow(tb + 256, e->snap_st)) return -1;
 	if (aead_one(e->snap_dev, e->snap_st, false, s->key, s->nonce, 1, s->tombs.data(), tb, tag)) return -1;
@@ -1620,10 +1636,9 @@ static void snapshot_write(cmb200_snapshot *s) {
 	if (s->sealed) {
 		rc = write_sealed_head(s);
 	} else {
-		const bool ok = s->chain == CHAIN_DELTA
-		    ? fwrite(&s->dh, sizeof(s->dh), 1, s->f) == 1 &&
-		      (s->tombs.empty() || fwrite(s->tombs.data(), 16, s->tombs.size(), s->f) == s->tombs.size())
-		    : fwrite(&s->h, sizeof(s->h), 1, s->f) == 1;
+		// a base has no tombstones
+		const bool ok = fwrite(s->head(), 64, 1, s->f) == 1 &&
+		    (s->tombs.empty() || fwrite(s->tombs.data(), 16, s->tombs.size(), s->f) == s->tombs.size());
 		rc = ok ? 0 : -2;
 	}
 	uint64_t ordinal = 0;
@@ -1735,12 +1750,12 @@ static cmb200_snapshot *snapshot_start(cmb200_engine *const *engines, int g, con
 		}
 	}
 	s->h = SnapHeader{};
-	memcpy(s->h.magic, s->sealed ? "CMB200E1" : "CMB200S1", 8);
+	memcpy(s->h.magic, SNAP_MAGIC[0][s->sealed], 8);
 	s->h.version = 1; s->h.pshift = (uint32_t)engines[0]->pshift;
-	if (s->sealed) memcpy(&s->h.pad[3], &s->nonce, 8);
+	s->h.nonce = s->nonce;                                // 0 unless sealed
 	s->chain = chain;
 	s->dh.chain = chain_id; s->dh.index = k;
-	if (chain == CHAIN_BASE) memcpy(&s->h.pad[1], &chain_id, 8);
+	if (chain == CHAIN_BASE) s->h.chain = chain_id;
 	int listed = 0;                                       // engines whose chain tick is pending
 	for (int i = 0; i < g && rc == 0; i++) {
 		cmb200_engine *e = engines[i];
@@ -1761,10 +1776,10 @@ static cmb200_snapshot *snapshot_start(cmb200_engine *const *engines, int g, con
 		for (const ExportEntry &x : s->lists[i]) s->h.bytes += x.len;
 	}
 	if (chain == CHAIN_DELTA) {
-		memcpy(s->dh.magic, s->sealed ? "CMB200F1" : "CMB200D1", 8);
+		memcpy(s->dh.magic, SNAP_MAGIC[1][s->sealed], 8);
 		s->dh.version = 1; s->dh.pshift = s->h.pshift; s->dh.flags = s->h.flags;
 		s->dh.tombstones = s->tombs.size(); s->dh.records = s->h.records; s->dh.bytes = s->h.bytes;
-		if (s->sealed) s->dh.pad = s->nonce;
+		s->dh.nonce = s->nonce;
 	}
 	if (rc == 0 && s->sealed && s->h.records >= 0xfffffffeull) {
 		set_error_msg("cmb200_snapshot_begin: a sealed file holds fewer than 2^32 - 2 records");
@@ -1810,11 +1825,11 @@ extern "C" cmb200_snapshot *cmb200_chain_begin(cmb200_engine *const *engines, in
 		return snapshot_start(engines, g, base_path, CHAIN_BASE, id, 0);
 	}
 	SnapHeader h{};
+	bool sealed = false;
 	FILE *f = fopen(base_path, "rb");
-	const bool ok = f && fread(&h, sizeof(h), 1, f) == 1 &&
-	    (memcmp(h.magic, "CMB200S1", 8) == 0 || memcmp(h.magic, "CMB200E1", 8) == 0) && h.version == 1;
+	const bool ok = read_header(f, h, &sealed);
 	if (f) fclose(f);
-	if (!ok || snap_chain_id(h) == 0) { set_error_msg("cmb200_chain_begin: no chain base at this path"); return nullptr; }
+	if (!ok || h.chain == 0) { set_error_msg("cmb200_chain_begin: no chain base at this path"); return nullptr; }
 	uint32_t k;
 	{
 		// checked against every engine under its lock when the tick lists it
@@ -1822,7 +1837,7 @@ extern "C" cmb200_snapshot *cmb200_chain_begin(cmb200_engine *const *engines, in
 		k = engines[0]->chain.k + 1;
 	}
 	const std::string path = std::string(base_path) + ".d" + std::to_string(k);
-	return snapshot_start(engines, g, path.c_str(), CHAIN_DELTA, snap_chain_id(h), k);
+	return snapshot_start(engines, g, path.c_str(), CHAIN_DELTA, h.chain, k);
 }
 
 extern "C" int cmb200_snapshot_finish(cmb200_snapshot *s, uint64_t *records_out) {
@@ -1906,8 +1921,7 @@ struct LoadBatch {
 static int restore_records(cmb200_engine *e, const uint8_t *blob, const unsigned long long *addr,
     const unsigned long long *ts, const unsigned long long *off, const uint64_t *fps, size_t m,
     unsigned long long &seq, unsigned long long floor = 0, const uint8_t *valid = nullptr) {
-	if (floor ? (valid ? launch_upsert_floor_valid(e->table, addr, valid, (uint32_t)m, seq, e->seq_stride, floor, e->d_slot, e->st)
-	                   : launch_upsert_floor(e->table, addr, (uint32_t)m, seq, e->seq_stride, floor, e->d_slot, e->st))
+	if (floor ? launch_upsert_floor(e->table, addr, valid, (uint32_t)m, seq, e->seq_stride, floor, e->d_slot, e->st)
 	          : launch_upsert(e->table, addr, valid, (uint32_t)m, seq, e->seq_stride, e->d_slot, e->st)) return -1;
 	EncodeJob job{};
 	job.n = (uint32_t)m; job.nbytes = e->bsize;
@@ -1978,135 +1992,112 @@ static long long load_flush(LoadBatch &b, bool with_fp) {
 	return (long long)(m - rej);
 }
 
-// Opens a snapshot file (a base) for a load into g engines and reads its header.  nullptr on failure
-// (error set).
-// A sealed base (*sealed) is opened with the engines' key (key, has_key from call_key): its header tag is
-// checked first, so that a wrong key or a damaged header fails here, before any record is read.
-static FILE *open_snapshot(cmb200_engine *const *engines, int g, const char *path, SnapHeader &h, const AeadKey &key,
-    bool has_key, bool *sealed) {
-	FILE *f = fopen(path, "rb");
-	if (!f) { set_error_msg("cmb200_load: no snapshot file"); return nullptr; }
-	const bool ok = fread(&h, sizeof(h), 1, f) == 1 && h.version == 1;
-	*sealed = ok && memcmp(h.magic, "CMB200E1", 8) == 0;
-	if (!ok || (!*sealed && memcmp(h.magic, "CMB200S1", 8) != 0)) {
-		fclose(f); set_error_msg("cmb200_load: not a snapshot of this library"); return nullptr;
-	}
+// A base or a delta opened for a load, its header checked, positioned at its first record (a base) or
+// tombstone (a delta).
+struct SnapFile {
+	FILE *f = nullptr;                                   // nullptr: the file did not open or failed a check
+	bool sealed = false;
+	uint64_t chain = 0, nonce = 0, records = 0, tombstones = 0;   // tombstones: 0 for a base
+	uint32_t flags = 0;
+	SnapFile() = default;
+	SnapFile(SnapFile &&o) noexcept : f(std::exchange(o.f, nullptr)), sealed(o.sealed), chain(o.chain), nonce(o.nonce),
+	    records(o.records), tombstones(o.tombstones), flags(o.flags) {}
+	~SnapFile() { if (f) fclose(f); }
+};
+
+// Opens a base for a load into g engines.  A sealed base is opened with the engines' key (key, has_key
+// from call_key): its header tag is checked first, so that a wrong key or a damaged header fails here,
+// before any record is read.  On failure the result holds no file (error set).
+static SnapFile open_snapshot(cmb200_engine *const *engines, int g, const char *path, const AeadKey &key, bool has_key) {
+	SnapFile sf;
+	SnapHeader h{};
+	sf.f = fopen(path, "rb");
+	if (!sf.f) { set_error_msg("cmb200_load: no snapshot file"); return sf; }
+	if (!read_header(sf.f, h, &sf.sealed)) { set_error_msg("cmb200_load: not a snapshot of this library"); return SnapFile(); }
 	for (int i = 0; i < g; i++)
-		if ((int)h.pshift != engines[i]->pshift) { fclose(f); set_error_msg("cmb200_load: snapshot has another page size"); return nullptr; }
-	if (*sealed) {
+		if ((int)h.pshift != engines[i]->pshift) { set_error_msg("cmb200_load: snapshot has another page size"); return SnapFile(); }
+	if (sf.sealed) {
 		uint8_t tag[16];
-		if (!has_key) { fclose(f); set_error_msg("cmb200_load: the snapshot is encrypted and the engines hold no file key"); return nullptr; }
-		if (fread(tag, 16, 1, f) != 1) { fclose(f); set_error_msg("cmb200_load: truncated or corrupt snapshot"); return nullptr; }
-		const int r = aead_check(engines[0], key, base_nonce(h), 0, &h, sizeof(h), tag);
+		if (!has_key) { set_error_msg("cmb200_load: the snapshot is encrypted and the engines hold no file key"); return SnapFile(); }
+		if (fread(tag, 16, 1, sf.f) != 1) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); return SnapFile(); }
+		const int r = aead_check(engines[0], key, h.nonce, 0, &h, sizeof(h), tag);
 		if (r != 1) {
-			fclose(f);
 			if (r == 0) set_error_msg("cmb200_load: the snapshot header does not open with this key (wrong key or damaged header)");
-			return nullptr;
+			return SnapFile();
 		}
 	}
-	return f;
+	sf.chain = h.chain; sf.nonce = h.nonce; sf.records = h.records; sf.flags = h.flags;
+	return sf;
 }
 
-// Stages the next n records of f into the load batches of their engines (cmb200_owner), flushing a batch
+// Stages the next n records of sf into the load batches of their engines (cmb200_owner), flushing a batch
 // when it is full; *loaded += records put.  skip (nullable): addresses a newer file of a chain has
-// decided, whose records are passed over unread; decide (nullable) gets every address read.  The
-// batches are not flushed at the end.  0 / -1 (error set).
-// sealed: the file's records are sealed under `nonce`; *ordinal is the file ordinal of the next one.
-static int load_records_sealed(FILE *f, uint64_t n, std::vector<LoadBatch> &bs, int g, bool with_fp,
-    const AddrSet *skip, AddrSet *decide, uint64_t *loaded, uint64_t nonce, uint64_t *ordinal) {
+// decided, whose records are passed over unread; decide (nullable) gets every address read.  *ordinal is
+// the file ordinal of the next record (a sealed record's nonce).  The batches are not flushed at the end.
+// 0 / -1 (error set).
+static int load_records(const SnapFile &sf, uint64_t n, std::vector<LoadBatch> &bs, int g, const AddrSet *skip,
+    AddrSet *decide, uint64_t *loaded, uint64_t *ordinal) {
+	for (LoadBatch &b : bs) b.sealed = sf.sealed;
+	const bool with_fp = sf.flags & 1u;
 	const uint32_t bsize = bs[0].e->bsize;
+	// A record's clear part, read first: its address names the engine whose batch takes the bytes.  A plain
+	// record's SnapRecord is not staged (lead); the rest of the record is, from its address on.  A sealed
+	// record is staged whole, its clear part {u32 len, u32 0, u, l} being k_open's AAD.
+	union {
+		struct { SnapRecord r; cmb200_addr a; } p;
+		struct { uint32_t len, zero; cmb200_addr a; } s;
+	} c;
+	static_assert(sizeof(c.p) == 48 && sizeof(c.s) == 24, "record clear parts");
+	const size_t clear = sf.sealed ? sizeof(c.s) : sizeof(c.p), lead = sf.sealed ? 0 : sizeof(SnapRecord);
 	for (uint64_t done = 0; done < n; done++) {
-		// the clear part {u32 len, u32 0, u, l} routes the record, as a plain file's address does
-		struct { uint32_t len, zero; cmb200_addr a; } c;
-		if (fread(&c, sizeof(c), 1, f) != 1 || c.zero != 0 || c.len < 24 || c.len > 24u + bsize + 1024u) {
+		if (fread(&c, clear, 1, sf.f) != 1 || (sf.sealed && c.s.zero != 0) || !record_len_ok(sf.sealed ? c.s.len : c.p.r.len, bsize)) {
 			set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1;
 		}
-		const size_t padded = seal_record_bytes(c.len);
+		const uint32_t len = sf.sealed ? c.s.len : c.p.r.len;
+		const cmb200_addr a = sf.sealed ? c.s.a : c.p.a;
+		const size_t bytes = record_bytes(sf.sealed, len), staged = bytes - lead;
 		const uint64_t i = 2 + (*ordinal)++;
-		if (skip || decide) {
-			const std::pair<uint64_t, uint64_t> ul(c.a.u, c.a.l);
-			const bool decided = skip && skip->count(ul);
-			if (decide && !decided) decide->insert(ul);
-			if (decided) {
-				if (fseeko(f, (off_t)(padded - sizeof(c)), SEEK_CUR) != 0) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1; }
-				continue;
-			}
-		}
-		uint64_t key;
-		FNV_hash(&c.a, 16, &key);
-		LoadBatch &b = bs[cmb200_owner(key, g)];
-		if (padded > b.cap) { set_error_msg("cmb200_load: record larger than the staging buffer"); return -1; }
-		if (b.m == b.B || b.used + padded > b.cap) {
-			const long long got = load_flush(b, with_fp);
-			if (got < 0) return -1;
-			*loaded += (uint64_t)got;
-		}
-		uint8_t *rec = b.blob + b.used;
-		memcpy(rec, &c, sizeof(c));
-		if (fread(rec + sizeof(c), padded - sizeof(c), 1, f) != 1) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1; }
-		AeadMsg &m = b.msg[b.m];
-		m = AeadMsg{};
-		m.len = c.len;
-		m.nonce[0] = (uint32_t)nonce; m.nonce[1] = (uint32_t)(nonce >> 32); m.nonce[2] = (uint32_t)i;
-		b.addr[b.m] = c.a;
-		b.off[b.m] = b.used + 32;              // where k_open leaves the record {u, l, compressed_length, ...}
-		b.used += padded; b.m++;
-	}
-	return 0;
-}
-
-static int load_records(FILE *f, uint64_t n, std::vector<LoadBatch> &bs, int g, bool with_fp, const AddrSet *skip,
-    AddrSet *decide, uint64_t *loaded, bool sealed = false, uint64_t nonce = 0, uint64_t *ordinal = nullptr) {
-	for (LoadBatch &b : bs) b.sealed = sealed;
-	if (sealed) return load_records_sealed(f, n, bs, g, with_fp, skip, decide, loaded, nonce, ordinal);
-	const uint32_t bsize = bs[0].e->bsize;
-	int rc = 0;
-	uint64_t done = 0;
-	while (rc == 0 && done < n) {
-		// record header and address first: the address names the engine whose batch takes the bytes
-		SnapRecord r;
-		cmb200_addr a;
-		if (fread(&r, sizeof(r), 1, f) != 1 || r.len < 24 || r.len > 24u + bsize + 1024u || fread(&a, 16, 1, f) != 1) {
-			rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
-		}
-		const size_t padded = ((size_t)r.len + 15) & ~(size_t)15;
 		if (skip || decide) {
 			const std::pair<uint64_t, uint64_t> ul(a.u, a.l);
 			const bool decided = skip && skip->count(ul);
 			if (decide && !decided) decide->insert(ul);
 			if (decided) {
-				if (fseeko(f, (off_t)(padded - 16), SEEK_CUR) != 0) { rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); }
-				done++;
+				if (fseeko(sf.f, (off_t)(bytes - clear), SEEK_CUR) != 0) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1; }
 				continue;
 			}
 		}
 		uint64_t key;
 		FNV_hash(&a, 16, &key);
 		LoadBatch &b = bs[cmb200_owner(key, g)];
-		if (padded > b.cap) { rc = -1; set_error_msg("cmb200_load: record larger than the staging buffer"); break; }
-		if (b.m == b.B || b.used + padded > b.cap) {
+		if (staged > b.cap) { set_error_msg("cmb200_load: record larger than the staging buffer"); return -1; }
+		if (b.m == b.B || b.used + staged > b.cap) {
 			const long long got = load_flush(b, with_fp);
-			if (got < 0) { rc = -1; break; }
+			if (got < 0) return -1;
 			*loaded += (uint64_t)got;
 		}
 		uint8_t *rec = b.blob + b.used;
-		memcpy(rec, &a, 16);
-		if (fread(rec + 16, padded - 16, 1, f) != 1) { rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break; }
-		{
+		memcpy(rec, (const uint8_t *)&c + lead, clear - lead);
+		if (fread(rec + clear - lead, bytes - clear, 1, sf.f) != 1) { set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1; }
+		b.addr[b.m] = a;
+		if (sf.sealed) {
+			AeadMsg &m = b.msg[b.m];
+			m = AeadMsg{};
+			m.len = len;
+			m.nonce[0] = (uint32_t)sf.nonce; m.nonce[1] = (uint32_t)(sf.nonce >> 32); m.nonce[2] = (uint32_t)i;
+			b.off[b.m] = b.used + 32;          // where k_open leaves the record {u, l, compressed_length, ...}
+		} else {
 			// the record must be what filemap_set would have stored (filemap.c:124-147): a foreign or
-			// corrupt file must not reach k_restore, which trusts compressed_length
+			// corrupt file must not reach k_restore, which trusts compressed_length (k_open checks a sealed one)
 			int32_t clen;
 			memcpy(&clen, rec + 16, 4);
-			if (clen < 0 || (uint32_t)clen > bsize + 1024u || r.len != 24u + (clen ? (uint32_t)clen : bsize)) {
-				rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
+			if (clen < 0 || (uint32_t)clen > bsize + 1024u || len != 24u + (clen ? (uint32_t)clen : bsize)) {
+				set_error_msg("cmb200_load: truncated or corrupt snapshot"); return -1;
 			}
+			b.off[b.m] = b.used; b.ts[b.m] = c.p.r.ts; b.fps[2 * b.m] = c.p.r.fp_hi; b.fps[2 * b.m + 1] = c.p.r.fp_lo;
 		}
-		b.addr[b.m] = a;
-		b.off[b.m] = b.used; b.ts[b.m] = r.ts; b.fps[2 * b.m] = r.fp_hi; b.fps[2 * b.m + 1] = r.fp_lo;
-		b.used += padded; b.m++;
-		done++;
+		b.used += staged; b.m++;
 	}
-	return rc;
+	return 0;
 }
 
 static int load_flush_all(std::vector<LoadBatch> &bs, bool with_fp, uint64_t *loaded) {
@@ -2134,64 +2125,62 @@ static int load_setup(std::vector<LoadBatch> &bs, cmb200_engine *const *engines,
 extern "C" int cmb200_load_set(cmb200_engine *const *engines, int g, const char *path, uint64_t *records_out) {
 	if (records_out) *records_out = 0;
 	if (g < 1 || !engines) { set_error_msg("cmb200_load_set: no engines"); return -1; }
-	SnapHeader h{};
 	AeadKey key{};
-	bool has_key = false, sealed = false;
+	bool has_key = false;
 	if (call_key(engines, g, "cmb200_load_set", key, has_key)) return -1;
-	FILE *f = open_snapshot(engines, g, path, h, key, has_key, &sealed);
-	if (!f) return -1;
+	const SnapFile sf = open_snapshot(engines, g, path, key, has_key);
+	if (!sf.f) return -1;
 	std::vector<LoadBatch> bs;
 	uint64_t loaded = 0, ordinal = 0;
 	int rc = load_setup(bs, engines, g, key);
 	explicit_bzero(&key, sizeof(key));
-	if (rc == 0) rc = load_records(f, h.records, bs, g, h.flags & 1u, nullptr, nullptr, &loaded, sealed, base_nonce(h), &ordinal);
-	if (rc == 0) rc = load_flush_all(bs, h.flags & 1u, &loaded);
+	if (rc == 0) rc = load_records(sf, sf.records, bs, g, nullptr, nullptr, &loaded, &ordinal);
+	if (rc == 0) rc = load_flush_all(bs, sf.flags & 1u, &loaded);
 	load_teardown(bs);
-	fclose(f);
 	if (records_out) *records_out = loaded;
 	return rc;
 }
 
 // Opens delta k of chain `id` and checks it whole before anything of it is applied: header, then the
 // bounds of every record header and the file's exact length (the record bytes are not read).  Leaves
-// the file at its first tombstone.  nullptr when the delta is missing, from another chain, out of
+// the file at its first tombstone.  No file when the delta is missing, from another chain, out of
 // sequence, truncated or corrupt: the chain's valid run ends before it.
-// A sealed delta (*sealed) also needs the engines' key (has_key): its header tag and its tombstones' tag
-// are checked here, and it is left at its first tombstone too.
-static FILE *open_delta(const std::string &path, uint64_t id, uint32_t k, uint32_t pshift, uint32_t bsize, DeltaHeader &dh,
-    cmb200_engine *e, const AeadKey &key, bool has_key, bool *sealed) {
-	FILE *f = fopen(path.c_str(), "rb");
-	if (!f) return nullptr;
-	bool ok = fread(&dh, sizeof(dh), 1, f) == 1;
-	*sealed = ok && memcmp(dh.magic, "CMB200F1", 8) == 0;
-	ok = ok && (*sealed ? has_key : memcmp(dh.magic, "CMB200D1", 8) == 0) && dh.version == 1 &&
-	    dh.pshift == pshift && dh.chain == id && dh.index == k && fseeko(f, 0, SEEK_END) == 0;
-	const uint64_t size = ok ? (uint64_t)ftello(f) : 0;
-	const uint64_t head = sizeof(dh) + (*sealed ? AEAD_TAG : 0);
-	uint64_t pos = head + 16 * dh.tombstones + (*sealed ? AEAD_TAG : 0), bytes = 0;
+// A sealed delta also needs the engines' key (has_key): its header tag and its tombstones' tag are
+// checked here too.
+static SnapFile open_delta(const std::string &path, uint64_t id, uint32_t k, uint32_t pshift, uint32_t bsize,
+    cmb200_engine *e, const AeadKey &key, bool has_key) {
+	SnapFile sf;
+	DeltaHeader dh{};
+	sf.f = fopen(path.c_str(), "rb");
+	bool ok = read_header(sf.f, dh, &sf.sealed) && (!sf.sealed || has_key) &&
+	    dh.pshift == pshift && dh.chain == id && dh.index == k && fseeko(sf.f, 0, SEEK_END) == 0;
+	const uint64_t size = ok ? (uint64_t)ftello(sf.f) : 0;
+	const uint64_t head = sizeof(dh) + (sf.sealed ? AEAD_TAG : 0);
+	uint64_t pos = head + 16 * dh.tombstones + (sf.sealed ? AEAD_TAG : 0), bytes = 0;
 	ok = ok && dh.tombstones <= size / 16 && pos <= size;
 	for (uint64_t i = 0; ok && i < dh.records; i++) {
 		SnapRecord r;
-		const size_t rh = *sealed ? 8 : sizeof(r);           // a sealed record's clear {u32 len, u32 0}
-		ok = pos + rh <= size && fseeko(f, (off_t)pos, SEEK_SET) == 0 && fread(&r, rh, 1, f) == 1;
-		if (*sealed) { r.len = (uint32_t)r.ts; r.zero = (uint32_t)(r.ts >> 32); ok = ok && r.zero == 0; }
-		ok = ok && r.len >= 24 && r.len <= 24u + bsize + 1024u;
-		pos += *sealed ? seal_record_bytes(r.len) : sizeof(r) + (((uint64_t)r.len + 15) & ~15ull);
+		const size_t rh = sf.sealed ? 8 : sizeof(r);         // a sealed record's clear {u32 len, u32 0}
+		ok = pos + rh <= size && fseeko(sf.f, (off_t)pos, SEEK_SET) == 0 && fread(&r, rh, 1, sf.f) == 1;
+		if (sf.sealed) { r.len = (uint32_t)r.ts; r.zero = (uint32_t)(r.ts >> 32); ok = ok && r.zero == 0; }
+		ok = ok && record_len_ok(r.len, bsize);
+		pos += record_bytes(sf.sealed, r.len);
 		bytes += r.len;
 	}
 	ok = ok && pos == size && bytes == dh.bytes;
-	if (ok && *sealed) {
+	if (ok && sf.sealed) {
 		// the header, then the tombstones, under the engines' key
 		uint8_t tag[16];
 		std::vector<uint8_t> tombs(16 * dh.tombstones);
-		ok = fseeko(f, sizeof(dh), SEEK_SET) == 0 && fread(tag, 16, 1, f) == 1 &&
-		    aead_check(e, key, dh.pad, 0, &dh, sizeof(dh), tag) == 1 &&
-		    (tombs.empty() || fread(tombs.data(), tombs.size(), 1, f) == 1) && fread(tag, 16, 1, f) == 1 &&
-		    aead_check(e, key, dh.pad, 1, tombs.data(), tombs.size(), tag) == 1;
+		ok = fseeko(sf.f, sizeof(dh), SEEK_SET) == 0 && fread(tag, 16, 1, sf.f) == 1 &&
+		    aead_check(e, key, dh.nonce, 0, &dh, sizeof(dh), tag) == 1 &&
+		    (tombs.empty() || fread(tombs.data(), tombs.size(), 1, sf.f) == 1) && fread(tag, 16, 1, sf.f) == 1 &&
+		    aead_check(e, key, dh.nonce, 1, tombs.data(), tombs.size(), tag) == 1;
 	}
-	ok = ok && fseeko(f, (off_t)head, SEEK_SET) == 0;
-	if (!ok) { fclose(f); return nullptr; }
-	return f;
+	ok = ok && fseeko(sf.f, (off_t)head, SEEK_SET) == 0;
+	if (!ok) return SnapFile();
+	sf.chain = dh.chain; sf.nonce = dh.nonce; sf.records = dh.records; sf.tombstones = dh.tombstones; sf.flags = dh.flags;
+	return sf;
 }
 
 // Whether a file <base_path>.d<j> with j > k exists.
@@ -2227,18 +2216,14 @@ static bool delta_beyond(const char *base_path, uint32_t k) {
 struct cmb200_loader {
 	std::vector<cmb200_engine *> engines;
 	std::string base_path;
-	SnapHeader h{};
-	FILE *base = nullptr;
+	std::vector<SnapFile> files;                         // the base, then the valid run of deltas (opened by the first step)
 	uint64_t id = 0, total = 0, before = 0, loaded = 0;
-	std::vector<FILE *> ds;                              // the valid run of deltas, opened by the first step
-	std::vector<DeltaHeader> dhs;
-	std::vector<bool> dsealed;
-	bool sealed = false, has_key = false;                // the base is sealed; the engines hold a key
+	bool has_key = false;                                // the engines hold a key
 	AeadKey key{};
 	uint64_t ordinal = 0;                                // the file ordinal of the next record of the file being read
 	bool checked = false, done = false;
 	int rc = 0;
-	size_t file = 0;                                     // files left, newest first: ds[file - 1], then the base
+	size_t file = 0;                                     // files left, newest first: the one being read is files[file - 1]
 	uint64_t left = 0;                                   // records left in the file being read
 	bool started = false;                                // its tombstones are read and `left` is set
 	std::vector<ulonglong2> tombs;
@@ -2247,9 +2232,8 @@ struct cmb200_loader {
 	~cmb200_loader() {
 		explicit_bzero(&key, sizeof(key));
 		load_teardown(bs);
-		for (FILE *f : ds) fclose(f);
-		if (base) fclose(base);
 	}
+	uint32_t deltas() const { return (uint32_t)(files.size() - 1); }
 };
 
 // Closes the fences of engines[0 .. n).
@@ -2270,9 +2254,10 @@ extern "C" cmb200_loader *cmb200_load_open(cmb200_engine *const *engines, int g,
 	l->engines.assign(engines, engines + g);
 	l->base_path = base_path;
 	if (call_key(engines, g, "cmb200_load_open", l->key, l->has_key)) { delete l; return nullptr; }
-	l->base = open_snapshot(engines, g, base_path, l->h, l->key, l->has_key, &l->sealed);
-	if (!l->base) { delete l; return nullptr; }
-	l->id = snap_chain_id(l->h);
+	l->files.push_back(open_snapshot(engines, g, base_path, l->key, l->has_key));
+	const SnapFile &base = l->files[0];
+	if (!base.f) { delete l; return nullptr; }
+	l->id = base.chain;
 	// an upper bound of the records the load puts, from the headers alone: the base's and those of the
 	// deltas whose headers name this chain in sequence (the first step checks the deltas whole)
 	// A header's count is bounded by its file's size (a record takes at least its header and a 24-byte
@@ -2283,13 +2268,12 @@ extern "C" cmb200_loader *cmb200_load_open(cmb200_engine *const *engines, int g,
 		const uint64_t most = size > header ? (size - header) / (sizeof(SnapRecord) + 24) : 0;
 		return records < most ? records : most;
 	};
-	l->total = bounded(l->h.records, l->base, sizeof(SnapHeader));
+	l->total = bounded(base.records, base.f, sizeof(SnapHeader));
 	for (uint32_t k = 1; l->id != 0; k++) {
 		DeltaHeader dh{};
+		bool sealed = false;
 		FILE *f = fopen((l->base_path + ".d" + std::to_string(k)).c_str(), "rb");
-		const bool ok = f && fread(&dh, sizeof(dh), 1, f) == 1 &&
-		    (memcmp(dh.magic, "CMB200D1", 8) == 0 || memcmp(dh.magic, "CMB200F1", 8) == 0) &&
-		    dh.version == 1 && dh.chain == l->id && dh.index == k;
+		const bool ok = read_header(f, dh, &sealed) && dh.chain == l->id && dh.index == k;
 		if (ok) l->total += bounded(dh.records, f, sizeof(dh));
 		if (f) fclose(f);
 		if (!ok) break;
@@ -2325,44 +2309,35 @@ extern "C" int cmb200_load_step(cmb200_loader *l, size_t max_records, uint64_t *
 	if (l->rc == 0 && !l->done && !l->checked) {
 		// the whole check of each delta (every record header and the file's length) before any is applied
 		for (uint32_t k = 1; l->id != 0; k++) {
-			DeltaHeader dh{};
-			bool sealed = false;
-			FILE *f = open_delta(l->base_path + ".d" + std::to_string(k), l->id, k, l->h.pshift, l->engines[0]->bsize, dh,
-			    l->engines[0], l->key, l->has_key, &sealed);
-			if (!f) break;
-			l->ds.push_back(f); l->dhs.push_back(dh); l->dsealed.push_back(sealed);
+			SnapFile d = open_delta(l->base_path + ".d" + std::to_string(k), l->id, k, (uint32_t)l->engines[0]->pshift,
+			    l->engines[0]->bsize, l->engines[0], l->key, l->has_key);
+			if (!d.f) break;
+			l->files.push_back(std::move(d));
 		}
-		l->file = l->ds.size() + 1;
+		l->file = l->files.size();
 		l->checked = true;
 	}
 	const int g = (int)l->engines.size();
 	size_t budget = max_records ? max_records : SIZE_MAX;
 	while (l->rc == 0 && !l->done && budget > 0) {
 		const bool delta = l->file > 1;
-		FILE *f = delta ? l->ds[l->file - 2] : l->base;
-		const bool with_fp = (delta ? l->dhs[l->file - 2].flags : l->h.flags) & 1u;
-		const bool sealed = delta ? l->dsealed[l->file - 2] : l->sealed;
+		const SnapFile &sf = l->files[l->file - 1];
 		if (!l->started) {
-			if (delta) {
-				const DeltaHeader &dh = l->dhs[l->file - 2];
-				l->tombs.resize(dh.tombstones);
-				if ((dh.tombstones && fread(l->tombs.data(), 16, l->tombs.size(), f) != l->tombs.size()) ||
-				    (sealed && fseeko(f, AEAD_TAG, SEEK_CUR) != 0)) {
-					l->rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
-				}
-				l->left = dh.records;
-			} else {
-				l->left = l->h.records;
+			// a delta's tombstones (and, sealed, their tag) lie between its header and its records
+			l->tombs.resize(sf.tombstones);
+			if ((sf.tombstones && fread(l->tombs.data(), 16, l->tombs.size(), sf.f) != l->tombs.size()) ||
+			    (delta && sf.sealed && fseeko(sf.f, AEAD_TAG, SEEK_CUR) != 0)) {
+				l->rc = -1; set_error_msg("cmb200_load: truncated or corrupt snapshot"); break;
 			}
+			l->left = sf.records;
 			l->ordinal = 0;
 			l->started = true;
 		}
 		const uint64_t n = l->left < budget ? l->left : (uint64_t)budget;
-		l->rc = load_records(f, n, l->bs, g, with_fp, &l->decided, delta ? &l->decided : nullptr, &l->loaded, sealed,
-		    delta ? l->dhs[l->file - 2].pad : base_nonce(l->h), &l->ordinal);
+		l->rc = load_records(sf, n, l->bs, g, &l->decided, delta ? &l->decided : nullptr, &l->loaded, &l->ordinal);
 		l->left -= n;
 		budget -= (size_t)n;
-		if (l->rc == 0 && (l->left == 0 || budget == 0)) l->rc = load_flush_all(l->bs, with_fp, &l->loaded);
+		if (l->rc == 0 && (l->left == 0 || budget == 0)) l->rc = load_flush_all(l->bs, sf.flags & 1u, &l->loaded);
 		if (l->rc || l->left) break;
 		// the records of a delta apply after its tombstones, so its records decide first
 		for (const ulonglong2 &a : l->tombs) l->decided.insert(std::make_pair((uint64_t)a.x, (uint64_t)a.y));
@@ -2392,7 +2367,7 @@ extern "C" int cmb200_load_close(cmb200_loader *l, uint64_t *records_out, uint32
 	// nothing fenced), every record put is live (none dropped for lack of space, none retired by a
 	// host-tier lap), and no delta file lies beyond the run (a tick that continued it would leave that
 	// file in a valid position).  Otherwise they hold no chain state, and the next tick writes a base.
-	bool whole = l->done && l->id != 0 && l->before == 0 && !delta_beyond(l->base_path.c_str(), (uint32_t)l->ds.size());
+	bool whole = l->done && l->id != 0 && l->before == 0 && !delta_beyond(l->base_path.c_str(), l->deltas());
 	uint64_t live = 0;
 	for (int i = 0; i < g; i++) {
 		cmb200_engine *e = engines[i];
@@ -2414,11 +2389,11 @@ extern "C" int cmb200_load_close(cmb200_loader *l, uint64_t *records_out, uint32
 		std::lock_guard<std::mutex> lk(e->mu);
 		cmb200_engine::Chain &ch = e->chain;
 		if (ch.pending) continue;
-		if (whole) { ch.cur ^= 1; ch.n = ch.n_next; ch.w = ch.w_next; ch.id = l->id; ch.k = (uint32_t)l->ds.size(); }
+		if (whole) { ch.cur ^= 1; ch.n = ch.n_next; ch.w = ch.w_next; ch.id = l->id; ch.k = l->deltas(); }
 		else ch.id = 0;
 	}
 	if (records_out) *records_out = l->loaded;
-	if (deltas_out) *deltas_out = (uint32_t)l->ds.size();
+	if (deltas_out) *deltas_out = l->deltas();
 	delete l;
 	return rc;
 }

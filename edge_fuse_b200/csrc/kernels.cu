@@ -135,9 +135,14 @@ __global__ void k_upsert(TableView t, const unsigned long long *addr, const uint
 // the load was opened gave it a sequence >= floor, and the load's own records take sequences below floor.
 // So a record is passed over (slot_idx 0xffffffff, which k_restore skips) when its key's slot, or a
 // tombstone on the key's probe chain before it, was written at or above floor: the key was put, moved or
-// removed since the load opened, and the file's page is older than that change.
-__device__ __forceinline__ uint32_t upsert_floor_one(const TableView &t, const unsigned long long *addr, uint32_t i,
-    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor) {
+// removed since the load opened, and the file's page is older than that change.  valid (nullable): the
+// records k_open let through (an encrypted load); valid[i] == 0 claims nothing.
+__global__ void k_upsert_floor(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
+    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx) {
+	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	uint32_t idx = 0xffffffffu;
+	if (valid && !valid[i]) { slot_idx[i] = idx; return; }
 	const unsigned long long key = fnv_addr(addr[2 * i], addr[2 * i + 1]);
 	bool newer = false;
 	if (key == KEY_EMPTY || key == KEY_TOMB) {
@@ -153,25 +158,11 @@ __device__ __forceinline__ uint32_t upsert_floor_one(const TableView &t, const u
 			}
 		}
 	}
-	uint32_t idx = 0xffffffffu;
 	if (!newer) {
 		idx = table_find_or_claim(t, key);
 		if (idx != 0xffffffffu) atomicMax(&t.slots[idx].seq, seq0 + seq_stride * i);
 	}
-	return idx;
-}
-__global__ void k_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
-    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx) {
-	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	slot_idx[i] = upsert_floor_one(t, addr, i, seq0, seq_stride, floor);
-}
-// k_upsert_floor over the records k_open let through (an encrypted load): valid[i] == 0 claims nothing.
-__global__ void k_upsert_floor_valid(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
-    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx) {
-	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
-	slot_idx[i] = valid[i] ? upsert_floor_one(t, addr, i, seq0, seq_stride, floor) : 0xffffffffu;
+	slot_idx[i] = idx;
 }
 
 __global__ void k_lookup(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
@@ -1817,17 +1808,10 @@ int launch_upsert(TableView t, const unsigned long long *addr, const uint8_t *va
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }
-int launch_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
-    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st) {
-	if (n == 0) return 0;
-	k_upsert_floor<<<GRID1D(n), 0, st>>>(t, addr, n, seq0, seq_stride, floor, slot_idx);
-	CMB_CHECK(cudaGetLastError());
-	return 0;
-}
-int launch_upsert_floor_valid(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
+int launch_upsert_floor(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
     unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st) {
 	if (n == 0) return 0;
-	k_upsert_floor_valid<<<GRID1D(n), 0, st>>>(t, addr, valid, n, seq0, seq_stride, floor, slot_idx);
+	k_upsert_floor<<<GRID1D(n), 0, st>>>(t, addr, valid, n, seq0, seq_stride, floor, slot_idx);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

@@ -217,9 +217,10 @@ int launch_compose(const uint64_t *offset, const uint64_t *nhid, const uint32_t 
 int launch_upsert(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
     unsigned long long seq0, unsigned long long seq_stride, uint32_t *slot_idx, cudaStream_t st);
 // launch_upsert for a background load's records: a key whose slot (or a tombstone on its probe chain) holds
-// a sequence >= floor was changed since the load opened; its record gets slot_idx 0xffffffff.
-int launch_upsert_floor(TableView t, const unsigned long long *addr, uint32_t n, unsigned long long seq0,
-    unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st);
+// a sequence >= floor was changed since the load opened; its record gets slot_idx 0xffffffff, as does a
+// record with valid[i] == 0 (valid nullable: all valid).
+int launch_upsert_floor(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
+    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st);
 
 // Multi-GPU index replication, the records staying on the device: pack one 32-byte record per chunk
 // of a put step, import all-gathered records written on other GPUs (rows of my_rank / rows that stored
@@ -402,9 +403,5 @@ int launch_seal(const AeadMsg *msgs, uint32_t n, const AeadKey &key, cudaStream_
 // Records: ts[i] and fp[2i], fp[2i + 1] get the record's values.
 int launch_open(const AeadMsg *msgs, uint32_t n, const AeadKey &key, uint32_t bsize, unsigned long long *ts,
     uint64_t *fp, uint8_t *ok, unsigned long long *rejected, cudaStream_t st);
-// launch_upsert_floor for records only some of which are valid: valid[i] == 0 claims nothing (slot_idx
-// 0xffffffff, which k_restore skips).
-int launch_upsert_floor_valid(TableView t, const unsigned long long *addr, const uint8_t *valid, uint32_t n,
-    unsigned long long seq0, unsigned long long seq_stride, unsigned long long floor, uint32_t *slot_idx, cudaStream_t st);
 
 }  // namespace cmb

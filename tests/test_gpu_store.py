@@ -893,7 +893,8 @@ def test_large_batches_at_capacity_stay_at_capacity(E, gpu, tmp_path, monkeypatc
 def test_sampling_a_nearly_empty_table_and_corrupt_snapshots(E, gpu, oracle, tmp_path):
     """(1) filemap_get_rand's policy equivalent on a table with 3 live slots out of 2^20: the bounded
     walk gives up and the cooperative scan finds them (k_sample / k_sample_scan).
-    (2) cmb200_load refuses records whose compressed_length disagrees with their length."""
+    (2) cmb200_load refuses records whose compressed_length disagrees with their length, and records
+    whose length is below 24 or above 24 + bsize + 1024."""
     eng = E.Engine(pshift=12, accel=12, capacity=1 << 18, arena_bytes=16 << 20, max_batch=256)
     assert eng.stats()["table_slots"] >= 1 << 20
     r = datagen.words(77, 64)
@@ -910,14 +911,15 @@ def test_sampling_a_nearly_empty_table_and_corrupt_snapshots(E, gpu, oracle, tmp
     snap = str(tmp_path / "s.snap")
     assert eng.save(snap) == 3
     raw = bytearray(open(snap, "rb").read())
-    # record 0: header 64 B, record header 32 B, then data_prefix {u, l, compressed_length, pad}
-    clen_at = 64 + 32 + 16
+    # record 0: header 64 B, record header 32 B {ts, fp, len, 0}, then data_prefix {u, l, compressed_length, pad}
+    len_at, clen_at = 64 + 24, 64 + 32 + 16
     good = int.from_bytes(raw[clen_at:clen_at + 4], "little", signed=True)
     assert 0 < good < 4096 + 1024
-    for bad in (-5, good + 7, 0x7fffffff):
+    cases = [(clen_at, bad) for bad in (-5, good + 7, 0x7fffffff)] + [(len_at, 23), (len_at, 24 + 4096 + 1025)]
+    for at, bad in cases:
         broken = bytearray(raw)
-        broken[clen_at:clen_at + 4] = int(bad).to_bytes(4, "little", signed=True)
-        p = str(tmp_path / f"bad{bad & 0xffff}.snap")
+        broken[at:at + 4] = int(bad).to_bytes(4, "little", signed=True)
+        p = str(tmp_path / f"bad{at}_{bad & 0xffff}.snap")
         open(p, "wb").write(broken)
         e2 = E.Engine(pshift=12, accel=12, capacity=4096, arena_bytes=16 << 20, max_batch=256)
         with pytest.raises(RuntimeError):
