@@ -15,6 +15,7 @@ FINGERPRINT = 1
 VERIFY = 2
 TOUCH = 4       # a hit raises its record's timestamp: eviction by last access (CMB200_EVICT=access)
 FREQ = 8        # every get counts in a frequency sketch: admission by frequency (CMB200_ADMIT=freq)
+GHOST = 16      # evicted addresses are remembered and misses measured against them (CMB200_GHOST=1)
 
 # every symbol the headers in include/ declare (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [
@@ -24,7 +25,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
     "cachemap_pread", "cachemap_pwrite", "cachemap_rename", "cachemap_get_admission",
-    "cachemap_load_progress",
+    "cachemap_load_progress", "cachemap_hit_curve",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -48,6 +49,7 @@ EXPORTED_SYMBOLS = [
     "cmb200_rename", "cmb200_rename_set", "cmb200_freq_index", "cmb200_freq_estimate", "cmb200_freq_read",
     "cmb200_freq_stats", "cmb200_load_open", "cmb200_load_step", "cmb200_load_total", "cmb200_load_close",
     "cmb200_set_file_key", "cmb200_load_rejected", "cmb200_aead_seal_batch", "cmb200_aead_open_batch",
+    "cmb200_ghost_set", "cmb200_evict_batch", "cmb200_ghost_stats", "cmb200_ghost_read",
 ]
 
 
@@ -73,6 +75,12 @@ class HostTierStats(C.Structure):
 
 class FreqStats(C.Structure):
     _fields_ = [(n, C.c_uint64) for n in ("width", "period", "increments", "since_halving", "halvings")]
+
+
+class GhostStats(C.Structure):
+    _fields_ = [(n, C.c_uint64) for n in (
+        "entries", "bucket_width", "clock", "inserted", "replaced", "removed", "probes", "refaults", "beyond")] + [
+        ("hist", C.c_uint64 * 64), ("lane_waits", C.c_uint64), ("lane_wait_ns", C.c_uint64)]
 
 
 class VerifyStats(C.Structure):
@@ -191,6 +199,11 @@ def lib() -> C.CDLL:
         "cmb200_freq_estimate": (i32, [vp, sz, vp, vp]),
         "cmb200_freq_read": (i32, [vp, vp, sz]),
         "cmb200_freq_stats": (i32, [vp, vp]),
+        "cmb200_ghost_set": (u32, [u64, i32]),
+        "cmb200_evict_batch": (i32, [vp, sz, vp, vp]),
+        "cmb200_ghost_stats": (i32, [vp, vp]),
+        "cmb200_ghost_read": (i32, [vp, vp, sz]),
+        "cachemap_hit_curve": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_save_set": (i32, [vp, i32, C.c_char_p, vp]),
         "cmb200_load_set": (i32, [vp, i32, C.c_char_p, vp]),
         "cmb200_move_pages": (i32, [vp, sz, vp, vp, vp, vp]),
@@ -467,6 +480,28 @@ class Engine:
         _check(lib().cmb200_freq_stats(self.h, C.byref(st)), "cmb200_freq_stats")
         return {n: int(getattr(st, n)) for n, _ in FreqStats._fields_}
 
+    def evict(self, u, l) -> int:
+        """cmb200_evict_batch (engine created with GHOST): unset as unset() does, a ghost per record removed
+        -> ghosts inserted."""
+        addr = _addr_array(u, l)
+        n = C.c_uint64()
+        _check(lib().cmb200_evict_batch(self.h, len(addr), _ptr(addr), C.byref(n)), "cmb200_evict_batch")
+        return n.value
+
+    def ghost_stats(self) -> dict:
+        """cmb200_ghost_stats: the GhostStats fields, hist as a list of 64 counts."""
+        st = GhostStats()
+        _check(lib().cmb200_ghost_stats(self.h, C.byref(st)), "cmb200_ghost_stats")
+        out = {n: int(getattr(st, n)) for n, _ in GhostStats._fields_ if n != "hist"}
+        out["hist"] = [int(x) for x in st.hist]
+        return out
+
+    def ghost_read(self) -> np.ndarray:
+        """cmb200_ghost_read -> the table as an (entries, 4) uint64 array of {u, l, stamp, 0}."""
+        tab = np.zeros((self.ghost_stats()["entries"], 4), dtype=np.uint64)
+        _check(lib().cmb200_ghost_read(self.h, _ptr(tab), tab.nbytes), "cmb200_ghost_read")
+        return tab
+
     def freq_read(self) -> np.ndarray:
         """cmb200_freq_read -> the sketch as uint64 words (4 rows of width / 16 words)."""
         words = np.zeros(self.freq_stats()["width"] // 4, dtype=np.uint64)
@@ -724,6 +759,11 @@ class Engine:
         _check(lib().cmb200_gen_chunks_dev(self.h, seed, _ptr(cids), len(cids), out_dev), "cmb200_gen_chunks_dev")
 
 
+def ghost_set(key: int, log2_sets: int) -> int:
+    """cmb200_ghost_set: the set of store key `key` in a ghost table of 2^log2_sets 4-way sets."""
+    return int(lib().cmb200_ghost_set(key, log2_sets))
+
+
 def freq_index(key: int, row: int, log2_width: int) -> int:
     """cmb200_freq_index: the counter of store key `key` in row `row` of a sketch of 2^log2_width per row."""
     return int(lib().cmb200_freq_index(key, row, log2_width))
@@ -933,6 +973,15 @@ class Cachemap:
         a, r = C.c_uint64(), C.c_uint64()
         lib().cachemap_get_admission(self.h, C.byref(a), C.byref(r))
         return a.value, r.value
+
+    def hit_curve(self, extra_pages):
+        """cachemap_hit_curve under CMB200_GHOST=1 -> (would_hit per extra_pages entry, GPU misses looked up)."""
+        extra = np.ascontiguousarray(extra_pages, dtype=np.uint64)
+        hit = np.zeros(len(extra), dtype=np.uint64)
+        misses = C.c_uint64()
+        _check(lib().cachemap_hit_curve(self.h, len(extra), _ptr(extra), _ptr(hit), C.byref(misses)),
+               "cachemap_hit_curve")
+        return hit, misses.value
 
     def load_progress(self):
         """cachemap_load_progress -> (loading, records loaded, records the files hold): loading is True while

@@ -48,6 +48,8 @@
 extern int cmb200_owner(uint64_t key, int g);
 /* ... and of cmb200_freq_index */
 extern uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width);
+/* ... and of cmb200_ghost_set */
+extern uint32_t cmb200_ghost_set(uint64_t key, int log2_sets);
 
 /* The host tier is optional in the engine this layer links against: libcachemap's engine defines
  * these, an engine without a tier (such as the CPU stand-in the host-layer tests link) does not, and
@@ -77,6 +79,8 @@ extern uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width);
 #pragma weak cmb200_load_total
 #pragma weak cmb200_load_close
 #pragma weak cmb200_set_file_key
+#pragma weak cmb200_evict_batch
+#pragma weak cmb200_ghost_stats
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -179,6 +183,10 @@ struct filemap {
 	 * (filemap_admit_n); set while the engines start, read after */
 	int admit;
 	uint64_t admitted, rejected;    /* (atomic) pages admitted over a victim / rejected */
+	/* CMB200_GHOST=1: every engine keeps ghosts of what it evicts (CMB200_GHOST), and the victims of eviction
+	 * by count and by arena pressure, and of admission, go through cmb200_evict_batch; set while the engines
+	 * start, read after */
+	int ghost;
 	/* persistence: <destdir>/cachemap_b200.snap (cmb200_save_set / cmb200_load_set) */
 	int persist;
 	long checkpoint_sec;    /* > 0: the checkpoint thread saves a snapshot this often when puts have landed */
@@ -450,6 +458,15 @@ fm_dev_start(struct filemap *m, int index, int device, int g)
 	cfg.flags |= admit;
 	if (admit && cmb200_freq_estimate)
 		m->admit = 1;
+	if (env_long("CMB200_GHOST", 0)) {
+		if (!cmb200_evict_batch || !cmb200_ghost_stats) {
+			if (index == 0)
+				fprintf(stderr, "cachemap_b200: CMB200_GHOST ignored: the engine keeps no ghosts\n");
+		} else {
+			cfg.flags |= CMB200_GHOST;
+			m->ghost = 1;
+		}
+	}
 	d->eng = cmb200_engine_create(&cfg);
 	const long tier_mb = env_long("CMB200_HOST_TIER_MB", 0);
 	if (d->eng && tier_mb > 0) {
@@ -940,9 +957,10 @@ filemap_sample(struct filemap *m, struct fm_dev *only, size_t n, const uint64_t 
 	return rc;
 }
 
-/* Unsets n victims, each on its engine own[i]. */
+/* Unsets n victims, each on its engine own[i].  evict: they are evictions, which leave ghosts under
+ * CMB200_GHOST (cmb200_evict_batch); other removals do not. */
 static void
-filemap_unset_victims(struct filemap *m, size_t n, const cmb200_addr *victim, const int *own)
+filemap_unset_victims(struct filemap *m, size_t n, const cmb200_addr *victim, const int *own, int evict)
 {
 	cmb200_addr *v = malloc(n * sizeof(cmb200_addr));
 	if (!v)
@@ -952,7 +970,9 @@ filemap_unset_victims(struct filemap *m, size_t n, const cmb200_addr *victim, co
 		for (size_t i = 0; i < n; i++)
 			if (own[i] == k)
 				v[c++] = victim[i];
-		if (c)
+		if (c && evict && m->ghost)
+			cmb200_evict_batch(m->dev[k]->eng, c, v, NULL);
+		else if (c)
 			cmb200_unset_batch(m->dev[k]->eng, c, v);
 	}
 	free(v);
@@ -997,7 +1017,7 @@ filemap_evict_n(struct filemap *m, struct fm_dev *only, uint64_t want)
 					}
 				}
 				if (nv)
-					filemap_unset_victims(m, (size_t)nv, victim, vown);
+					filemap_unset_victims(m, (size_t)nv, victim, vown, 1);
 			} else {
 				fprintf(stderr, "cachemap_b200: eviction could not sample the store: %s\n", cmb200_last_error());
 			}
@@ -1221,7 +1241,7 @@ filemap_admit_n(struct filemap *m, uint64_t want, const cmb200_addr *pages, uint
 					}
 				}
 				if (ng)
-					filemap_unset_victims(m, (size_t)ng, victim, vown);
+					filemap_unset_victims(m, (size_t)ng, victim, vown, 1);
 				__atomic_fetch_add(&m->admitted, ng, __ATOMIC_RELAXED);
 				__atomic_fetch_add(&m->rejected, nr, __ATOMIC_RELAXED);
 			} else {
@@ -2256,7 +2276,7 @@ filemap_reject_batch(struct filemap *m, size_t n, const cmb200_addr *addr, uint8
 		v[nv++] = addr[i];
 	}
 	if (nv)
-		filemap_unset_victims(m, nv, v, own);
+		filemap_unset_victims(m, nv, v, own, 0);
 	free(v);
 	free(own);
 	memset(reject, 0, n);
@@ -2822,6 +2842,37 @@ cachemap_get_admission(struct cachemap *cm, uint64_t *admitted, uint64_t *reject
 {
 	*admitted = __atomic_load_n(&cm->pages->admitted, __ATOMIC_RELAXED);
 	*rejected = __atomic_load_n(&cm->pages->rejected, __ATOMIC_RELAXED);
+}
+
+/* With G engines each engine's clock counts its own evictions, and keys split evenly over the engines
+ * (cmb200_owner), so Δ more pages for the map are Δ / G more for each engine.  A refault at distance d
+ * would have hit when d < Δ / G; Δ / G is rounded down to a bucket boundary, so that no refault at or beyond
+ * it is counted. */
+int
+cachemap_hit_curve(struct cachemap *cm, size_t n, const uint64_t *extra_pages, uint64_t *would_hit, uint64_t *misses)
+{
+	struct filemap *m = cm->pages;
+	if (!filemap_engine_ready(m) || !m->ghost)
+		return -1;
+	for (size_t i = 0; i < n; i++)
+		would_hit[i] = 0;
+	uint64_t probes = 0;
+	for (int k = 0; k < m->g; k++) {
+		struct cmb200_ghost_stats st;
+		if (cmb200_ghost_stats(m->dev[k]->eng, &st) != 0)
+			return -1;
+		probes += st.probes;
+		for (size_t i = 0; i < n; i++) {
+			uint64_t b = extra_pages[i] / (uint64_t)m->g / st.bucket_width;
+			if (b > 64)
+				b = 64;
+			for (uint64_t j = 0; j < b; j++)
+				would_hit[i] += st.hist[j];
+		}
+	}
+	if (misses)
+		*misses = probes;
+	return 0;
 }
 
 struct cmb200_engine *

@@ -12,6 +12,7 @@
 // A get batch is: k_lookup -> k_decode -> D2H copy.
 #include <algorithm>
 #include <atomic>
+#include <chrono>
 #include <condition_variable>
 #include <deque>
 #include <dirent.h>
@@ -213,6 +214,8 @@ struct cmb200_engine {
 	struct GetLane {
 		std::atomic<int> busy{0}; Stream st; HostMem<int32_t> h_status; HostMem<cmb200_addr> h_addr;
 		Event freq_done;                     // CMB200_FREQ: recorded after the lane's last counting get
+		Event ghost_done;                    // CMB200_GHOST: recorded after the lane's last probe
+		std::atomic<bool> ghost_pending{false};   // ghost_done has been recorded (by the lane's holder)
 	};
 	GetLane lane[GET_LANES];
 	// A small get may be begun by one thread and ended by another (cmb200_get_small_begin / _end), so
@@ -336,6 +339,19 @@ struct cmb200_engine {
 	std::mutex freq_mu;
 	std::atomic<uint64_t> freq_incs{0}, freq_since{0}, freq_halvings{0}, freq_streams{0};
 	Event freq_st_done, freq_halved;
+	// CMB200_GHOST: the ghost table and its device counters (GC_WORDS); the clock (evictions so far) and the
+	// inserts change under mu, the clock is read without it by small gets.  d_ghost_ins / d_ghost_seg: an
+	// insert call's entries grouped by set, and the groups' starts; d_ghost_flags: a tier lap's retired flags.
+	DevMem<GhostEntry> d_ghost;
+	DevMem<unsigned long long> d_ghost_ctr;
+	uint32_t ghost_log2_sets = 0;
+	std::atomic<uint64_t> ghost_clock{0};
+	uint64_t ghost_inserted = 0;
+	std::atomic<uint64_t> ghost_lane_waits{0}, ghost_lane_wait_ns{0};
+	DevMem<GhostEntry> d_ghost_ins;
+	DevMem<uint32_t> d_ghost_seg;
+	DevMem<uint8_t> d_ghost_flags;
+	GhostView ghost() const { return GhostView{d_ghost, ghost_log2_sets, d_ghost_ctr}; }
 	// snapshots (cmb200_snapshot_begin): SNAP_FREE, SNAP_CLAIMED by a snapshot that has not listed this
 	// engine's records yet, or SNAP_PENDING: listed, section not written yet.  snap_state changes under
 	// snap_mu and every change is broadcast on snap_cv.  Lock order: mu before snap_mu.  The snapshot's
@@ -474,6 +490,17 @@ static int engine_init(cmb200_engine *e, const cmb200_config *cfg) {
 		CMB_CHECK(cudaMemsetAsync(e->d_freq, 0, 2 * w, e->st));
 		if (e->freq_st_done.create(cudaEventDisableTiming) || e->freq_halved.create(cudaEventDisableTiming)) return -1;
 		for (auto &ln : e->lane) if (ln.freq_done.create(cudaEventDisableTiming)) return -1;
+	}
+	if (e->flags & CMB200_GHOST) {
+		// 32 bytes per entry, before the arena takes its share of free memory
+		uint64_t n = next_pow2(cfg->capacity ? cfg->capacity : e->table.cap / 4);
+		if (n < 256) n = 256;
+		if (n > (1ull << 32)) n = 1ull << 32;
+		while ((4ull << e->ghost_log2_sets) < n) e->ghost_log2_sets++;
+		if (e->d_ghost.alloc(n * sizeof(GhostEntry)) || e->d_ghost_ctr.alloc(GC_WORDS * sizeof(unsigned long long))) return -1;
+		CMB_CHECK(cudaMemsetAsync(e->d_ghost, 0, n * sizeof(GhostEntry), e->st));
+		CMB_CHECK(cudaMemsetAsync(e->d_ghost_ctr, 0, GC_WORDS * sizeof(unsigned long long), e->st));
+		for (auto &ln : e->lane) if (ln.ghost_done.create(cudaEventDisableTiming)) return -1;
 	}
 	if (get_small_supports(e->bsize)) {
 		// the descriptor scratch of the fused single-page get
@@ -753,10 +780,11 @@ static int check_dev_pages(const void *pages, const char *what) {
 	return 0;
 }
 
-// The multi-GPU calls are refused with a sketch: it counts the gets of this engine's own keys.
-static int freq_refuses(cmb200_engine *e, const char *what) {
-	if (!e->d_freq) return 0;
-	snprintf(g_err, sizeof(g_err), "%s: not available on an engine with CMB200_FREQ", what);
+// The multi-GPU calls are refused with a sketch or a ghost table: they count the gets and evictions of this
+// engine's own keys.
+static int local_only_refuses(cmb200_engine *e, const char *what) {
+	if (!e->d_freq && !e->d_ghost) return 0;
+	snprintf(g_err, sizeof(g_err), "%s: not available on an engine with %s", what, e->d_freq ? "CMB200_FREQ" : "CMB200_GHOST");
 	return -1;
 }
 
@@ -804,7 +832,7 @@ extern "C" int cmb200_put_batch_async(cmb200_engine *e, size_t n, const cmb200_a
 extern "C" int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
     const void *pages, int pages_on_dev, const uint64_t *ts, uint32_t rank, void *records_dev_out,
     int32_t *lens_out, uint64_t *ticket) {
-	if (freq_refuses(e, "cmb200_put_step") || multi_gpu_call(e, "cmb200_put_step")) return -1;
+	if (local_only_refuses(e, "cmb200_put_step") || multi_gpu_call(e, "cmb200_put_step")) return -1;
 	if (n > cmb200_engine::META_CAP) { set_error_msg("cmb200_put_step: more than 262144 chunks in one step"); return -1; }
 	if (pages_on_dev == 1 && check_dev_pages(pages, "cmb200_put_step")) return -1;
 	std::lock_guard<std::mutex> g(e->mu);
@@ -818,7 +846,7 @@ extern "C" int cmb200_put_step(cmb200_engine *e, size_t n, const cmb200_addr *ad
 
 extern "C" int cmb200_import_records_dev(cmb200_engine *e, size_t n_total, const void *records_dev, uint32_t my_rank) {
 	std::lock_guard<std::mutex> g(e->mu);
-	if (freq_refuses(e, "cmb200_import_records_dev") || multi_gpu_call(e, "cmb200_import_records_dev")) return -1;
+	if (local_only_refuses(e, "cmb200_import_records_dev") || multi_gpu_call(e, "cmb200_import_records_dev")) return -1;
 	CMB_CHECK(cudaSetDevice(e->device));
 	if (n_total == 0) return 0;
 	if (n_total > 0xffffffffull) { set_error_msg("cmb200_import_records_dev: too many records"); return -1; }
@@ -942,6 +970,126 @@ extern "C" int cmb200_freq_stats(cmb200_engine *e, struct cmb200_freq_stats *out
 	return 0;
 }
 
+// ---- CMB200_GHOST: evictions remembered, misses measured -----------------------------------------
+
+static int ghost_required(cmb200_engine *e, const char *what) {
+	if (e->d_ghost) return 0;
+	snprintf(g_err, sizeof(g_err), "%s: the engine was created without CMB200_GHOST", what);
+	return -1;
+}
+
+// The engine's stream after every lane's last probe.  A small get returns before its probe has run, so every
+// launch on st that reads or writes the ghost table waits for the probes of the small gets before it: calls
+// made one after another then leave the table the sequential rules give.  (mu held)
+static int ghost_settle(cmb200_engine *e) {
+	for (auto &ln : e->lane)
+		if (ln.ghost_pending.load(std::memory_order_acquire)) CMB_CHECK(cudaStreamWaitEvent(e->st, ln.ghost_done, 0));
+	return 0;
+}
+
+// Inserts a ghost for each address of `ev`, stamped clock + 1, clock + 2, ... in order, on the engine's
+// stream.  The inserts are grouped by set, stably, so that one thread of k_ghost_insert applies each set's
+// inserts in the call's order.  (mu held)
+static int ghost_insert(cmb200_engine *e, const std::vector<cmb200_addr> &ev) {
+	const size_t n = ev.size();
+	if (n == 0) return 0;
+	std::vector<uint32_t> set(n), order(n);
+	for (size_t i = 0; i < n; i++) {
+		uint64_t key;
+		FNV_hash(&ev[i], 16, &key);
+		set[i] = cmb200_ghost_set(key, (int)e->ghost_log2_sets);
+		order[i] = (uint32_t)i;
+	}
+	std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return set[a] < set[b]; });
+	if (ghost_settle(e)) return -1;
+	const uint64_t clock = e->ghost_clock.load(std::memory_order_relaxed);
+	std::vector<GhostEntry> ins(n);
+	std::vector<uint32_t> seg;
+	for (size_t k = 0; k < n; k++) {
+		const uint32_t i = order[k];
+		ins[k] = GhostEntry{ev[i].u, ev[i].l, clock + 1 + i, 0};
+		if (k == 0 || set[i] != set[order[k - 1]]) seg.push_back((uint32_t)k);
+	}
+	seg.push_back((uint32_t)n);
+	if (e->d_ghost_ins.grow(n * sizeof(GhostEntry), e->st) || e->d_ghost_seg.grow(seg.size() * 4, e->st)) return -1;
+	CMB_CHECK(cudaMemcpyAsync(e->d_ghost_ins, ins.data(), n * sizeof(GhostEntry), cudaMemcpyHostToDevice, e->st));
+	CMB_CHECK(cudaMemcpyAsync(e->d_ghost_seg, seg.data(), seg.size() * 4, cudaMemcpyHostToDevice, e->st));
+	if (launch_ghost_insert(e->ghost(), e->d_ghost_ins, e->d_ghost_seg, (uint32_t)(seg.size() - 1), e->st)) return -1;
+	e->stats.kernel_launches++;
+	e->ghost_clock.store(clock + n, std::memory_order_release);
+	e->ghost_inserted += n;
+	return 0;
+}
+
+extern "C" int cmb200_evict_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *evicted_out) {
+	if (evicted_out) *evicted_out = 0;
+	if (ghost_required(e, "cmb200_evict_batch")) return -1;
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (e->fence.open)
+		for (size_t i = 0; i < n; i++) {
+			uint64_t key;
+			FNV_hash(&addr[i], 16, &key);
+			e->fence.keys.insert(key);
+		}
+	int32_t *h_status = (int32_t *)(e->h_meta + cmb200_engine::META_CAP * 28);
+	uint64_t evicted = 0;
+	for (size_t at = 0; at < n; at += e->max_batch) {
+		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
+		// the lookup tells which requests name the record their key holds; k_unset then removes by key
+		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
+		if (launch_lookup(e->table, e->d_addr, nullptr, m, e->d_status, e->d_recoff, e->d_vlen, nullptr, e->st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(h_status, e->d_status, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
+		if (launch_unset(e->table, e->arena, e->d_addr, m, e->st)) return -1;
+		e->stats.kernel_launches += 2;
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		std::vector<cmb200_addr> ev;
+		AddrSet seen;
+		for (uint32_t i = 0; i < m; i++)
+			if (h_status[i] == CMB200_HIT && seen.insert(std::make_pair(addr[at + i].u, addr[at + i].l)).second)
+				ev.push_back(addr[at + i]);
+		if (ghost_insert(e, ev)) return -1;
+		evicted += ev.size();
+	}
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	if (evicted_out) *evicted_out = evicted;
+	return 0;
+}
+
+extern "C" int cmb200_ghost_stats(cmb200_engine *e, struct cmb200_ghost_stats *out) {
+	if (ghost_required(e, "cmb200_ghost_stats")) return -1;
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (ghost_settle(e)) return -1;
+	unsigned long long c[GC_WORDS];
+	CMB_CHECK(cudaMemcpyAsync(c, e->d_ghost_ctr, sizeof(c), cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	memset(out, 0, sizeof(*out));
+	out->entries = 4ull << e->ghost_log2_sets;
+	out->bucket_width = out->entries / 64;
+	out->clock = e->ghost_clock.load();
+	out->inserted = e->ghost_inserted;
+	out->replaced = c[GC_REPLACED]; out->removed = c[GC_REMOVED];
+	out->probes = c[GC_PROBES]; out->refaults = c[GC_REFAULTS]; out->beyond = c[GC_BEYOND];
+	for (int k = 0; k < 64; k++) out->hist[k] = c[GC_HIST + k];
+	out->lane_waits = e->ghost_lane_waits.load(); out->lane_wait_ns = e->ghost_lane_wait_ns.load();
+	return 0;
+}
+
+extern "C" int cmb200_ghost_read(cmb200_engine *e, void *out, size_t bytes) {
+	if (ghost_required(e, "cmb200_ghost_read")) return -1;
+	if (bytes != (size_t)(4ull << e->ghost_log2_sets) * sizeof(GhostEntry)) {
+		set_error_msg("cmb200_ghost_read: bytes is not the table's size");
+		return -1;
+	}
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (ghost_settle(e)) return -1;
+	CMB_CHECK(cudaMemcpyAsync(out, e->d_ghost, bytes, cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	return 0;
+}
+
 // ---- get ---------------------------------------------------------------------------------
 
 static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint8_t *valid,
@@ -956,6 +1104,7 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 	if (valid) CMB_CHECK(cudaMemcpyAsync(e->d_valid, h_valid, n, cudaMemcpyHostToDevice, e->st));
 	size_t nb = 0;
 	if (e->d_freq && freq_before(e, e->st)) return -1;
+	if (e->d_ghost && ghost_settle(e)) return -1;
 	for (size_t at = 0; at < n; at += B, nb++) {
 		const uint32_t m = (uint32_t)((n - at < B) ? n - at : B);
 		const int buf = (int)(nb & 1);
@@ -991,6 +1140,11 @@ static int get_slice(cmb200_engine *e, size_t n, const cmb200_addr *addr, const 
 			CMB_CHECK(cudaEventRecord(e->consumed[buf], e->copy));
 		}
 		e->stats.kernel_launches += 2;
+		if (e->d_ghost) {
+			if (launch_ghost_probe(e->ghost(), e->d_addr + 2 * at, e->d_status + at, valid ? e->d_valid + at : nullptr, m,
+				e->ghost_clock.load(std::memory_order_acquire), e->st)) return -1;
+			e->stats.kernel_launches++;
+		}
 	}
 	CMB_CHECK(cudaMemcpyAsync(h_status, e->d_status, n * 4, cudaMemcpyDeviceToHost, e->st));
 	CMB_CHECK(cudaStreamSynchronize(e->st));
@@ -1096,6 +1250,18 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 		if (!ln) sched_yield();
 	}
 	if (cudaSetDevice(e->device) != cudaSuccess) { ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1; }
+	// CMB200_GHOST: the lane's last probe reads its address and status words, which are rewritten below
+	if (ln->ghost_pending.load(std::memory_order_acquire) && cudaEventQuery(ln->ghost_done) != cudaSuccess) {
+		(void)cudaGetLastError();
+		const auto t0 = std::chrono::steady_clock::now();
+		if (cudaEventSynchronize(ln->ghost_done) != cudaSuccess) {
+			cmb_set_error("cudaEventSynchronize(ghost probe)", cudaGetLastError(), __FILE__, __LINE__);
+			ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1;
+		}
+		e->ghost_lane_waits.fetch_add(1, std::memory_order_relaxed);
+		e->ghost_lane_wait_ns.fetch_add((uint64_t)std::chrono::duration_cast<std::chrono::nanoseconds>(
+		    std::chrono::steady_clock::now() - t0).count(), std::memory_order_relaxed);
+	}
 	// Requests and answers travel through page-locked host memory that the kernel reads and writes
 	// directly: no copy is queued before or after the launch, and the end is seen by watching the
 	// status words flip, which costs a few microseconds where a stream synchronisation costs tens.
@@ -1117,7 +1283,15 @@ extern "C" int cmb200_get_small_begin(cmb200_engine *e, size_t n, const cmb200_a
 	if ((e->d_freq && freq_before(e, ln->st)) || launch_get_small(job, e->device, ln->st)) {
 		ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1;
 	}
-	if (e->d_freq && freq_after(e, ln->st, li, n)) {
+	bool failed = e->d_freq && freq_after(e, ln->st, li, n);
+	if (!failed && e->d_ghost) {
+		// the probe reads the statuses k_get_small wrote, after it on the lane's stream
+		failed = launch_ghost_probe(e->ghost(), (const unsigned long long *)ln->h_addr.get(), ln->h_status, nullptr,
+		    (uint32_t)n, e->ghost_clock.load(std::memory_order_acquire), ln->st) != 0 ||
+		    cudaEventRecord(ln->ghost_done, ln->st) != cudaSuccess;
+		if (!failed) ln->ghost_pending.store(true, std::memory_order_release);
+	}
+	if (failed) {
 		// the kernel is in flight and writes the lane's status words: the lane is freed once it is done
 		cudaStreamSynchronize(ln->st);
 		ln->busy.store(0, std::memory_order_release); e->get_gate.leave(); return -1;
@@ -1204,7 +1378,7 @@ extern "C" int cmb200_arena_ipc_handle(cmb200_engine *e, void *handle64, uint64_
 extern "C" int cmb200_open_peer(cmb200_engine *e, uint32_t rank, const void *handle64, uint64_t arena_bytes) {
 	{
 		std::lock_guard<std::mutex> g(e->mu);
-		if (freq_refuses(e, "cmb200_open_peer") || multi_gpu_call(e, "cmb200_open_peer")) return -1;
+		if (local_only_refuses(e, "cmb200_open_peer") || multi_gpu_call(e, "cmb200_open_peer")) return -1;
 	}
 	if (rank >= GET_MAX_PEERS) { set_error_msg("cmb200_open_peer: rank out of range"); return -1; }
 	cmb200_engine::GateClosed g(e->get_gate);
@@ -1230,11 +1404,16 @@ extern "C" int cmb200_unset_batch(cmb200_engine *e, size_t n, const cmb200_addr 
 			FNV_hash(&addr[i], 16, &key);
 			e->fence.keys.insert(key);
 		}
+	if (e->d_ghost && ghost_settle(e)) return -1;
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
 		CMB_CHECK(cudaMemcpyAsync(e->d_addr, addr + at, (size_t)m * 16, cudaMemcpyHostToDevice, e->st));
 		if (launch_unset(e->table, e->arena, e->d_addr, m, e->st)) return -1;
 		e->stats.kernel_launches++;
+		if (e->d_ghost) {
+			if (launch_ghost_remove(e->ghost(), e->d_addr, m, e->st)) return -1;
+			e->stats.kernel_launches++;
+		}
 	}
 	CMB_CHECK(cudaStreamSynchronize(e->st));
 	return 0;
@@ -2492,6 +2671,10 @@ extern "C" int cmb200_invalidate(cmb200_engine *e, uint64_t u, uint64_t l_first,
 	const bool scan = l_last - l_first >= invalidate_keyed_max(e->table.cap);
 	if (launch_invalidate(e->table, e->arena, u, l_first, l_last, scan, e->d_removed, e->st)) return -1;
 	e->stats.kernel_launches++;
+	if (e->d_ghost) {
+		if (ghost_settle(e) || launch_ghost_remove_span(e->ghost(), u, l_first, l_last, scan, e->st)) return -1;
+		e->stats.kernel_launches++;
+	}
 	unsigned long long removed = 0;
 	CMB_CHECK(cudaMemcpyAsync(&removed, e->d_removed, sizeof(removed), cudaMemcpyDeviceToHost, e->st));
 	unsigned long long c[8];
@@ -2837,6 +3020,18 @@ extern "C" int cmb200_rename_set(cmb200_engine *const *engines, int g, uint64_t 
 		if (rename_refused(engines[i])) return -1;
 	}
 	if (u_from == u_to) return 0;
+	// ghosts of both intervals are dropped, not moved (cachemap_b200.h, CMB200_GHOST)
+	for (int i = 0; i < g; i++) {
+		cmb200_engine *e = engines[i];
+		if (!e->d_ghost) continue;
+		std::lock_guard<std::mutex> lk(e->mu);
+		CMB_CHECK(cudaSetDevice(e->device));
+		const bool scan = l_last - l_first >= invalidate_keyed_max(e->table.cap);
+		if (ghost_settle(e) || launch_ghost_remove_span(e->ghost(), u_from, l_first, l_last, scan, e->st) ||
+		    launch_ghost_remove_span(e->ghost(), u_to, l_first, l_last, scan, e->st)) return -1;
+		e->stats.kernel_launches += 2;
+		CMB_CHECK(cudaStreamSynchronize(e->st));      // before the small gets that follow the call
+	}
 	// an open load passes over both intervals from now on: it must not bring back a source page the move
 	// leaves behind, nor put an older destination page over a moved one
 	for (int i = 0; i < g; i++) {
@@ -3009,15 +3204,22 @@ static int demote_group(cmb200_engine *e, const std::vector<DemoteEntry> &grp,
 	const size_t nr = ret.size() / 4;
 	if (t.d_retire.grow(nr * 32, e->st)) rc = -1;
 	const uint64_t a0 = start % t.size, bytes = end - start, first = std::min(bytes, t.size - a0);
+	// CMB200_GHOST: the records the lap unsets are evictions, and get ghosts in tier order
+	const bool ghosts = e->d_ghost && nr;
+	if (ghosts && e->d_ghost_flags.grow(nr, e->st)) rc = -1;
 	if (rc == 0 && nr) {
 		rc = cudaMemcpyAsync(t.d_retire, ret.data(), nr * 32, cudaMemcpyHostToDevice, e->st) != cudaSuccess ||
-		    launch_tier_retire(e->table, e->arena, t.d_retire, (uint32_t)nr, t.d_ctr, e->st) ? -1 : 0;
+		    (ghosts ? launch_tier_retire_list(e->table, e->arena, t.d_retire, (uint32_t)nr, t.d_ctr, e->d_ghost_flags, e->st)
+		            : launch_tier_retire(e->table, e->arena, t.d_retire, (uint32_t)nr, t.d_ctr, e->st)) ? -1 : 0;
 		e->stats.kernel_launches++;
 	}
 	if (rc == 0 && (cudaMemcpyAsync(t.host + a0, bounce, first, cudaMemcpyDeviceToHost, e->st) != cudaSuccess ||
 	    (bytes > first && cudaMemcpyAsync(t.host, bounce + first, bytes - first, cudaMemcpyDeviceToHost, e->st) != cudaSuccess)))
 		rc = -1;
 	if (rc == 0 && launch_demote_publish(e->table, e->arena, t.d_moves, n, e->st)) rc = -1;
+	std::vector<uint8_t> retired(ghosts ? nr : 0);
+	if (rc == 0 && ghosts && cudaMemcpyAsync(retired.data(), e->d_ghost_flags, nr, cudaMemcpyDeviceToHost, e->st) != cudaSuccess)
+		rc = -1;
 	if (cudaStreamSynchronize(e->st) != cudaSuccess) rc = -1;
 	if (overwrite) e->get_gate.reopen();
 	if (rc) { cmb_set_error("host tier demotion", cudaGetLastError(), __FILE__, __LINE__); return -1; }
@@ -3026,6 +3228,14 @@ static int demote_group(cmb200_engine *e, const std::vector<DemoteEntry> &grp,
 	t.demoted_records += n;
 	for (const DemoteEntry &d : grp) t.demoted_bytes += d.len;
 	e->stats.kernel_launches += 2;
+	if (ghosts) {
+		// after the ring's bookkeeping, which the published records need whether or not their ghosts land
+		std::vector<cmb200_addr> ev;
+		for (size_t i = 0; i < nr; i++)
+			if (retired[i]) ev.push_back(cmb200_addr{ret[4 * i], ret[4 * i + 1]});
+		if (ghost_insert(e, ev)) return -1;
+		CMB_CHECK(cudaStreamSynchronize(e->st));  // before the small gets that follow the call
+	}
 	return 0;
 }
 

@@ -1679,6 +1679,132 @@ int launch_freq_estimate(const unsigned long long *freq, uint32_t log2w, const u
 	return 0;
 }
 
+// ---- CMB200_GHOST: the ghost table (cachemap_b200.h) ----------------------------------------------
+// An entry is claimed or cleared through its stamp word: a probe or a removal takes a ghost with one
+// atomicExch of the stamp to 0, so of two takers exactly one gets it.  Inserts and probes on different
+// streams may meet in one entry; the worst they do is a lost or misattributed ghost (a statistic), never a
+// fault, since every index stays inside the set.
+
+__device__ __forceinline__ GhostEntry *ghost_ways(const GhostView &g, unsigned long long u, unsigned long long l) {
+	return g.tab + 4 * (size_t)cmb200_ghost_set(fnv_addr(u, l), (int)g.log2_sets);
+}
+
+// Clears the live ghost of {u, l} in its set; its stamp, or 0 when there is none.
+__device__ __forceinline__ unsigned long long ghost_take(GhostEntry *w, unsigned long long u, unsigned long long l) {
+	for (int k = 0; k < 4; k++) {
+		if (w[k].u != u || w[k].l != l) continue;
+		const unsigned long long s = atomicExch(&w[k].stamp, 0ull);
+		if (s) return s;
+	}
+	return 0ull;
+}
+
+// One thread per set of the call: its inserts in order.  The way: the live ghost of the same address, else
+// the first empty way, else the oldest stamp.
+__global__ void __launch_bounds__(256) k_ghost_insert(GhostView g, const GhostEntry *ins, const uint32_t *seg,
+    uint32_t nseg) {
+	const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+	if (k >= nseg) return;
+	unsigned long long replaced = 0;
+	for (uint32_t j = seg[k]; j < seg[k + 1]; j++) {
+		const GhostEntry x = ins[j];
+		GhostEntry *w = ghost_ways(g, x.u, x.l);
+		int pick = -1, empty = -1, oldest = 0;
+		for (int q = 0; q < 4; q++) {
+			const unsigned long long s = *reinterpret_cast<volatile unsigned long long *>(&w[q].stamp);
+			if (s && w[q].u == x.u && w[q].l == x.l) { pick = q; break; }
+			if (!s && empty < 0) empty = q;
+			if (s < w[oldest].stamp) oldest = q;
+		}
+		if (pick < 0) {
+			pick = empty >= 0 ? empty : oldest;
+			if (empty < 0) replaced++;
+		}
+		w[pick].stamp = 0ull;
+		w[pick].u = x.u;
+		w[pick].l = x.l;
+		__threadfence();
+		w[pick].stamp = x.stamp;
+	}
+	if (replaced) atomicAdd(g.ctr + GC_REPLACED, replaced);
+}
+
+__global__ void __launch_bounds__(256) k_ghost_probe(GhostView g, const unsigned long long *addr, const int32_t *status,
+    const uint8_t *valid, uint32_t n, unsigned long long clock) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	const bool probe = i < n && status[i] == ST_MISS && (!valid || valid[i]);
+	unsigned long long s = 0;
+	if (probe) {
+		const unsigned long long u = addr[2 * (size_t)i], l = addr[2 * (size_t)i + 1];
+		s = ghost_take(ghost_ways(g, u, l), u, l);
+	}
+	const unsigned m = __ballot_sync(0xffffffffu, probe), r = __ballot_sync(0xffffffffu, s != 0);
+	if ((threadIdx.x & 31) == 0) {
+		if (m) atomicAdd(g.ctr + GC_PROBES, (unsigned long long)__popc(m));
+		if (r) atomicAdd(g.ctr + GC_REFAULTS, (unsigned long long)__popc(r));
+	}
+	if (!s) return;
+	// d = the evictions made after the ghost's; one stamped after the clock this probe was given (an eviction
+	// racing a small get) counts as d = 0
+	const unsigned long long d = clock > s ? clock - s : 0ull, entries = 4ull << g.log2_sets;
+	if (d >= entries) atomicAdd(g.ctr + GC_BEYOND, 1ull);
+	else atomicAdd(g.ctr + GC_HIST + (d >> (g.log2_sets - 4u)), 1ull);     // bucket width = entries / 64
+}
+
+__global__ void __launch_bounds__(256) k_ghost_remove(GhostView g, const unsigned long long *addr, uint32_t n) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	bool hit = false;
+	if (i < n) {
+		const unsigned long long u = addr[2 * (size_t)i], l = addr[2 * (size_t)i + 1];
+		hit = ghost_take(ghost_ways(g, u, l), u, l) != 0;
+	}
+	count_warp(hit, g.ctr + GC_REMOVED);
+}
+
+// scan: one thread per entry; otherwise one thread per l of the interval (n of them).
+__global__ void __launch_bounds__(256) k_ghost_remove_span(GhostView g, unsigned long long u, unsigned long long l_first,
+    unsigned long long l_last, uint64_t n, bool scan) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	bool hit = false;
+	if (i < n) {
+		if (scan) {
+			GhostEntry &x = g.tab[i];
+			if (x.u == u && x.l >= l_first && x.l <= l_last && x.stamp) hit = atomicExch(&x.stamp, 0ull) != 0;
+		} else {
+			const unsigned long long l = l_first + i;
+			hit = ghost_take(ghost_ways(g, u, l), u, l) != 0;
+		}
+	}
+	count_warp(hit, g.ctr + GC_REMOVED);
+}
+
+int launch_ghost_insert(GhostView g, const GhostEntry *ins, const uint32_t *seg, uint32_t nseg, cudaStream_t st) {
+	if (nseg == 0) return 0;
+	k_ghost_insert<<<(nseg + 255) / 256, 256, 0, st>>>(g, ins, seg, nseg);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_ghost_probe(GhostView g, const unsigned long long *addr, const int32_t *status, const uint8_t *valid,
+    uint32_t n, unsigned long long clock, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_ghost_probe<<<(n + 255) / 256, 256, 0, st>>>(g, addr, status, valid, n, clock);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_ghost_remove(GhostView g, const unsigned long long *addr, uint32_t n, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_ghost_remove<<<(n + 255) / 256, 256, 0, st>>>(g, addr, n);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+int launch_ghost_remove_span(GhostView g, unsigned long long u, unsigned long long l_first, unsigned long long l_last,
+    bool scan, cudaStream_t st) {
+	const uint64_t n = scan ? 4ull << g.log2_sets : l_last - l_first + 1;
+	k_ghost_remove_span<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(g, u, l_first, l_last, n, scan);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
 // ------------------------------------------------------------------------------------------
 // fingerprint alone, stream generator, small launchers
 // ------------------------------------------------------------------------------------------
@@ -2172,10 +2298,9 @@ int launch_promote(TableView t, ArenaView a, const PromoteEntry *p, uint32_t n, 
 }
 
 // Conditional unset of the records a wrap of the tier overwrites: rec[4i..4i+3] = {u, l, location, bytes}.
-__global__ void k_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
-    unsigned long long *retired) {
-	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= n) return;
+// Returns whether record i was unset.
+__device__ __forceinline__ bool tier_retire_one(const TableView &t, const ArenaView &a, const unsigned long long *rec,
+    uint32_t i, unsigned long long *retired) {
 	const unsigned long long loc = rec[4 * (size_t)i + 2], bytes = rec[4 * (size_t)i + 3];
 	const uint32_t idx = table_find(t, fnv_addr(rec[4 * (size_t)i], rec[4 * (size_t)i + 1]));
 	if (idx != 0xffffffffu) {
@@ -2193,10 +2318,29 @@ __global__ void k_tier_retire(TableView t, ArenaView a, const unsigned long long
 				atomicAdd(t.tombs, 1ull);
 			}
 			atomicAdd(retired, 1ull);
-			return;
+			return true;
 		}
 	}
 	atomicAdd(a.tier, 0ull - bytes);                         // a dead record: its bytes leave the tier's garbage
+	return false;
+}
+__global__ void k_tier_retire_list(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
+    unsigned long long *retired, uint8_t *out) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) out[i] = tier_retire_one(t, a, rec, i, retired);
+}
+int launch_tier_retire_list(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
+    unsigned long long *retired, uint8_t *out, cudaStream_t st) {
+	if (n == 0) return 0;
+	k_tier_retire_list<<<GRID1D(n), 0, st>>>(t, a, rec, n, retired, out);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+__global__ void k_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
+    unsigned long long *retired) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) tier_retire_one(t, a, rec, i, retired);
 }
 int launch_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
     unsigned long long *retired, cudaStream_t st) {

@@ -355,6 +355,32 @@ int launch_promote(TableView t, ArenaView a, const PromoteEntry *p, uint32_t n, 
 // tier's garbage.  *retired counts the unset keys.
 int launch_tier_retire(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
     unsigned long long *retired, cudaStream_t st);
+// launch_tier_retire that also sets out[i] = 1 for each record it unset, 0 for the others (CMB200_GHOST).
+int launch_tier_retire_list(TableView t, ArenaView a, const unsigned long long *rec, uint32_t n,
+    unsigned long long *retired, uint8_t *out, cudaStream_t st);
+
+// ---- CMB200_GHOST: the ghost table of cachemap_b200.h ----
+struct GhostEntry { unsigned long long u, l, stamp, pad; };   // stamp 0 = empty
+static_assert(sizeof(GhostEntry) == 32, "ghost entry layout");
+// Device counters of the ghost table: live ghosts displaced by inserts, removed, requests probed, refaults,
+// refaults beyond the table, then the 64 histogram buckets.
+enum : uint32_t { GC_REPLACED = 0, GC_REMOVED, GC_PROBES, GC_REFAULTS, GC_BEYOND, GC_HIST, GC_WORDS = GC_HIST + 64 };
+struct GhostView {
+	GhostEntry *tab;              // 4 << log2_sets entries, set s at [4 s, 4 s + 4)
+	uint32_t log2_sets;
+	unsigned long long *ctr;      // GC_WORDS
+};
+// k_ghost_insert: ins[seg[k] .. seg[k + 1]) all fall in one set and are applied in order by thread k.
+int launch_ghost_insert(GhostView g, const GhostEntry *ins, const uint32_t *seg, uint32_t nseg, cudaStream_t st);
+// k_ghost_probe: every request with status[i] == ST_MISS (and valid[i], valid nullable) consumes the ghost of
+// its address, if any, and books its distance from `clock` (the evictions made so far).
+int launch_ghost_probe(GhostView g, const unsigned long long *addr, const int32_t *status, const uint8_t *valid,
+    uint32_t n, unsigned long long clock, cudaStream_t st);
+// k_ghost_remove: the ghosts of n addresses.  k_ghost_remove_span: the ghosts of {u, l}, l_first <= l <= l_last,
+// by a scan of the table (scan) or one thread per l (the caller keeps the interval short).
+int launch_ghost_remove(GhostView g, const unsigned long long *addr, uint32_t n, cudaStream_t st);
+int launch_ghost_remove_span(GhostView g, unsigned long long u, unsigned long long l_first, unsigned long long l_last,
+    bool scan, cudaStream_t st);
 
 // Re-inserts every live slot of `from` into the (zeroed) table `to` of the same geometry.
 int launch_rehash(TableView from, TableView to, cudaStream_t st);

@@ -164,6 +164,16 @@ void cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hi
 /* CMB200_ADMIT=freq: pages admitted over the victim they were paired with, and pages rejected (not stored,
  * their key unset) since cachemap_create.  Both 0 without admission. */
 void cachemap_get_admission(struct cachemap *cm, uint64_t *admitted, uint64_t *rejected);
+/* CMB200_GHOST=1: for each extra_pages[i], would_hit[i] = the GPU misses since cachemap_create that a map of
+ * capacity + extra_pages[i] pages would have served, estimated from the refault distances of evicted pages
+ * (cmb200_ghost_stats); *misses (nullable) = the GPU misses looked up.  It counts only the refaults whose
+ * distance lies below extra_pages[i] / G (G engines) rounded down to a bucket of the ghost table; that
+ * rounding, ghosts displaced from a full set, and renames make it low.  The eviction policy can make it high:
+ * under random oldest-of-three eviction a page read in a cycle that refaulted at distance d often would not
+ * have lasted d more evictions in the larger map either, and on such a workload the curve overestimates the
+ * hit ratio by up to 0.24 (DESIGN.md §2, *Ghost entries*).  -1 without CMB200_GHOST. */
+int cachemap_hit_curve(struct cachemap *cm, size_t n, const uint64_t *extra_pages, uint64_t *would_hit,
+    uint64_t *misses);
 struct cmb200_engine *cachemap_engine(struct cachemap *cm);
 /* Every engine under the map, in CMB200_DEVICES order (cachemap_engine is out[0]): stores up to max
  * of them in out and returns how many there are, 0 if none could be started.  Like cachemap_engine,

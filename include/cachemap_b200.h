@@ -77,6 +77,35 @@ typedef struct { uint64_t u; uint64_t l; } cmb200_addr;
  * With the flag, cmb200_put_step, cmb200_import_records_dev and cmb200_open_peer fail (-1): the sketch counts
  * the gets of one engine's own keys. */
 #define CMB200_FREQ 8u
+/* Ghost entries for sizing (the drop-in's CMB200_GHOST=1): the engine remembers the addresses it evicted,
+ * in a table in HBM, and measures each later miss's refault distance, the evictions made between the page's
+ * eviction and the miss.  A miss at distance d would have hit in a store larger by more than d pages.
+ * Table: `entries` = the power of two at or above capacity (table_slots / 4 when capacity is 0), at least
+ * 256, 32 bytes each ({u, l, stamp, 0}; stamp 0 = empty), allocated at engine creation before the arena is
+ * sized.  Entries form 4-way sets of one 128-byte line; the address {u, l} of store key k lies in set
+ * cmb200_ghost_set(k, log2(entries / 4)).
+ * Clock: the engine counts the records it evicts; the k-th gets stamp k, and the records one call evicts
+ * take consecutive stamps in array order (cmb200_evict_batch) or in tier order (a host-tier lap).
+ * Insert: into the entry of the same address, else an empty way, else the way with the oldest stamp; a live
+ * ghost of another address so displaced counts as `replaced`.  Inserts of one call land as if applied one by
+ * one in their order.
+ * Probe: every request that cmb200_get_small, cmb200_get_small_begin / _end, cmb200_get_batch or
+ * cmb200_get_batch_dev answers exactly CMB200_MISS (with a valid address) looks its address up; a match
+ * is consumed (cleared) and its distance d = clock - stamp, the evictions made after the ghost's as of the
+ * get's launch (clock = evictions so far), goes to bucket d / (entries / 64) of a 64-bucket histogram, or
+ * to `beyond` when d >= entries.  A second miss of the same address in one call finds nothing.
+ * Removal: cmb200_unset_batch (by address), cmb200_invalidate and both intervals of cmb200_rename_set remove
+ * the ghosts of what they name, since a larger store would have lost those pages too.  A rename drops its
+ * ghosts rather than moving them, so a page renamed while evicted is not counted when it refaults under its
+ * new name: the estimate errs low.  Puts, patches, demotion, promotion, compaction, table rebuilds and loads
+ * do not move ghosts, and ghosts are not saved in snapshots or chain deltas.
+ * Calls made one after another leave exactly the table the definition above gives: a small get returns
+ * before its probe has run, and every later call that reads or writes the table on the engine's stream waits
+ * for it.  Small gets run on lanes of their own, so the probe of a get made concurrently with an eviction or a
+ * removal depends on timing (it may miss a ghost inserted at the same moment, or see the clock of before it),
+ * as the sketch's increments do around a halving.  Never which bytes a get returns.
+ * With the flag, cmb200_put_step, cmb200_import_records_dev and cmb200_open_peer fail (-1). */
+#define CMB200_GHOST 16u
 
 typedef struct cmb200_config {
 	int device;             /* CUDA ordinal, -1 = current device */
@@ -293,6 +322,36 @@ inline uint32_t cmb200_freq_index(uint64_t key, int row, int log2_width) {
 	    : row == 2 ? 0x165667B19E3779F9ull : 0xD6E8FEB86659FD93ull;
 	return (uint32_t)((key * c) >> (64 - log2_width));
 }
+
+/* The set of store key `key` in a CMB200_GHOST table of 2^log2_sets 4-way sets (6 <= log2_sets <= 30):
+ * multiply-shift by one fixed odd constant, top bits.  The only definition, as cmb200_freq_index. */
+#if defined(__CUDACC__)
+__host__ __device__
+#endif
+inline uint32_t cmb200_ghost_set(uint64_t key, int log2_sets) {
+	return (uint32_t)((key * 0x9FB21C651E98DF25ull) >> (64 - log2_sets));
+}
+
+/* ---- ghost entries (CMB200_GHOST) ------------------------------------------------------------------
+ * cmb200_evict_batch: removes records exactly as cmb200_unset_batch does (by key), then inserts a ghost for
+ * each addr[i] whose own record it removed (the key held that address; the first of repeats), in array
+ * order.  *evicted_out (nullable) = ghosts inserted.  Without the flag: -1.
+ * cmb200_ghost_stats: the table's size, the bucket width (entries / 64) and clock; ghosts inserted, live
+ * ones displaced by inserts, removed by unsets, invalidations and renames; requests probed, those that found
+ * their ghost (refaults = sum(hist) + beyond); and how often cmb200_get_small_begin found a lane's previous
+ * probe still running and waited for it, and how long that took in all (ns).
+ * cmb200_ghost_read: copies the table (entries x 32 bytes, the layout of CMB200_GHOST) to host memory; bytes
+ * must be that size.  Both wait for the probes and inserts enqueued before the call.  -1 without the flag. */
+struct cmb200_ghost_stats {
+	uint64_t entries, bucket_width, clock;
+	uint64_t inserted, replaced, removed;
+	uint64_t probes, refaults, beyond;
+	uint64_t hist[64];
+	uint64_t lane_waits, lane_wait_ns;
+};
+int cmb200_evict_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *evicted_out);
+int cmb200_ghost_stats(cmb200_engine *e, struct cmb200_ghost_stats *out);
+int cmb200_ghost_read(cmb200_engine *e, void *out, size_t bytes);
 
 /* ---- frequency sketch (CMB200_FREQ) ----------------------------------------------------------------
  * cmb200_freq_estimate: est_out[i] = the estimate of addr[i]'s key, the least of its four counters (0..15),
