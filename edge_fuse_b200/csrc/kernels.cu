@@ -923,8 +923,15 @@ extern "C" int cmb200_enc_phases(void *buf, uint32_t *nphases) {   // n x 2 x EN
 // it its register allocation) stays what it is without the flag.
 // TOUCH (CMB200_TOUCH): lane 0 raises the slot's ts once the request's answer is ST_HIT (after the
 // fingerprint comparison under VERIFY); the state is, likewise, a parameter of the touching kernels alone.
-template <bool TOUCH>
-__device__ __forceinline__ void decode_touch(const DecodeJob &job, const DecodeTouch &t, uint32_t i, int lane) {
+// decode_hit books what only an ST_HIT answer books, as gs_answer does: a tier hit and its hot-log entry
+// (a record answered ST_BAD_DECODE or ST_CORRUPT is a miss, and is not queued for promotion), and the touch.
+template <bool VERIFY, bool TOUCH>
+__device__ __forceinline__ void decode_hit(const DecodeJob &job, const DecodeTouch &t, uint32_t i, int lane,
+    bool from_host) {
+	if (from_host && lane == 0 && (!VERIFY || job.host_hits)) {
+		atomicAdd(job.host_hits, 1ull);
+		hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
+	}
 	if constexpr (TOUCH) {
 		if (lane == 0) slot_touch(t.slots, t.idx[i], job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1], t.ts);
 	}
@@ -940,21 +947,18 @@ __device__ __forceinline__ void decode_request(const DecodeJob &job, const Decod
 		if (job.status[i] != ST_HIT) return;
 		const unsigned long long off = job.rec_off[i];
 		// host tier: mapped host memory, read over PCIe
-		const uint8_t *rec = (off & REC_HOST) ? job.host + (off & ~REC_HOST) : job.arena + off;
-		if ((off & REC_HOST) && lane == 0 && (!VERIFY || job.host_hits)) {
-			atomicAdd(job.host_hits, 1ull);
-			hot_log(job.hot, job.addr[2 * (size_t)i], job.addr[2 * (size_t)i + 1]);
-		}
+		const bool from_host = (off & REC_HOST) != 0;
+		const uint8_t *rec = from_host ? job.host + (off & ~REC_HOST) : job.arena + off;
 		uint32_t clen = job.vlen[i] - 1u;
 		if constexpr (!VERIFY) {
 			if (clen == 0) {                            // raw page (filemap.c:249-251)
 				warp_copy_ro(out, rec + 24, job.nbytes, lane);
-				decode_touch<TOUCH>(job, t, i, lane);
+				decode_hit<VERIFY, TOUCH>(job, t, i, lane, from_host);
 				return;
 			}
 			int used = lz4_decode_warp(rec + 24, clen, out, job.nbytes, lane);
 			if (used != (int)clen && lane == 0) job.status[i] = ST_BAD_DECODE;   // filemap.c:244-248
-			if (used == (int)clen) decode_touch<TOUCH>(job, t, i, lane);
+			if (used == (int)clen) decode_hit<VERIFY, TOUCH>(job, t, i, lane, from_host);
 		} else {
 			if (clen == 0) {
 				warp_copy_ro(out, rec + 24, job.nbytes, lane);
@@ -965,7 +969,7 @@ __device__ __forceinline__ void decode_request(const DecodeJob &job, const Decod
 			const uint32_t idx = v.idx[i];
 			if (v.fp_tag[idx] != ckpt_tag(off, clen)) {
 				if (lane == 0) atomicAdd(&v.vstat[VS_UNVERIFIED], 1ull);
-				decode_touch<TOUCH>(job, t, i, lane);
+				decode_hit<VERIFY, TOUCH>(job, t, i, lane, from_host);
 				return;
 			}
 			__syncwarp();                           // every lane's stores of the page are visible to the warp
@@ -976,7 +980,7 @@ __device__ __forceinline__ void decode_request(const DecodeJob &job, const Decod
 				atomicAdd(&v.vstat[match ? VS_VERIFIED : VS_CORRUPT], 1ull);
 				if (!match) job.status[i] = ST_CORRUPT;
 			}
-			if (match) decode_touch<TOUCH>(job, t, i, lane);
+			if (match) decode_hit<VERIFY, TOUCH>(job, t, i, lane, from_host);
 		}
 	} else {
 		int used = lz4_decode_warp(job.blocks + (size_t)i * job.block_stride, (uint32_t)job.lens[i], out,
