@@ -911,6 +911,53 @@ group_by_owner(int g, size_t n, const int *own, size_t *order, size_t *start)
 		order[fill[own[i]]++] = i;
 }
 
+/* One array of a fan-out: `elem` bytes per item; out = the engines write it, else they read it. */
+struct fan { void *p; size_t elem; int out; };
+
+/* What a fan-out calls on one engine: its n items, element j of each in p[j]. */
+typedef int (*fan_call)(struct fm_dev *d, size_t n, void *const *p);
+
+/* Calls `call` on each engine that has items, in engine order, with that engine's items in array order:
+ * item i of n is on engine own[i], and its values are element i of each of the na (<= 4) arrays a[].
+ * With one engine the caller's arrays go through as they are (own is not read).  Otherwise each engine's
+ * items are gathered by group_by_owner and, once every call has returned 0, the outputs scattered back.
+ * 0 = every call returned 0; -1 = no memory, or a call failed (the engines after it are not called). */
+static int
+filemap_fan_out(struct filemap *m, size_t n, const int *own, int na, const struct fan *a, fan_call call)
+{
+	void *p[4], *q[4];
+	for (int j = 0; j < na; j++)
+		p[j] = a[j].p;
+	if (n == 0 || m->g == 1)
+		return n ? call(m->dev[0], n, p) : 0;
+	size_t bytes = n * sizeof(size_t), start[MAX_DEVICES + 1];
+	for (int j = 0; j < na; j++)
+		bytes += (n * a[j].elem + 7) & ~(size_t)7;      /* each gathered array 8-byte aligned */
+	size_t *order = malloc(bytes);
+	if (!order)
+		return -1;
+	group_by_owner(m->g, n, own, order, start);
+	uint8_t *at = (uint8_t *)(order + n);
+	for (int j = 0; j < na; j++) {
+		p[j] = at;
+		at += (n * a[j].elem + 7) & ~(size_t)7;
+		for (size_t i = 0; !a[j].out && i < n; i++)
+			memcpy((uint8_t *)p[j] + i * a[j].elem, (const uint8_t *)a[j].p + order[i] * a[j].elem, a[j].elem);
+	}
+	int rc = 0;
+	for (int k = 0; k < m->g && rc == 0; k++) {
+		for (int j = 0; j < na; j++)
+			q[j] = (uint8_t *)p[j] + start[k] * a[j].elem;
+		if (start[k + 1] > start[k])
+			rc = call(m->dev[k], start[k + 1] - start[k], q);
+	}
+	for (int j = 0; rc == 0 && j < na; j++)
+		for (size_t i = 0; a[j].out && i < n; i++)
+			memcpy((uint8_t *)a[j].p + order[i] * a[j].elem, (const uint8_t *)p[j] + i * a[j].elem, a[j].elem);
+	free(order);
+	return rc;
+}
+
 static uint64_t
 rand64(void)
 {
@@ -920,41 +967,88 @@ rand64(void)
 	return r;
 }
 
-/* cmb200_sample of n draws: on engine `only`, or (only = NULL) each draw on engine cmb200_owner(r, G).
- * own_out[i] = the engine that answered draw i.  0 = sampled, -1 = an engine failed. */
+#define ROUND_MAX 4096          /* records one round of eviction, admission or demotion goes for, 3 draws each */
+
+/* One round of candidate draws: draw i from rand64(), and what engine own[i] answered for it
+ * (cmb200_sample: cand[i], ts[i], ok[i]).  One allocation, at cand. */
+struct round {
+	cmb200_addr *cand;
+	uint64_t *draw, *ts;
+	int32_t *ok;
+	int *own;
+};
+
 static int
-filemap_sample(struct filemap *m, struct fm_dev *only, size_t n, const uint64_t *draws, cmb200_addr *cand,
-    uint64_t *ts, int32_t *ok, int *own_out)
+sample_call(struct fm_dev *d, size_t n, void *const *p)
 {
-	if (only) {
-		for (size_t i = 0; i < n; i++)
-			own_out[i] = only->index;
-		return cmb200_sample(only->eng, n, draws, cand, ts, ok);
+	return cmb200_sample(d->eng, n, p[0], p[1], p[2], p[3]);
+}
+
+/* Takes n draws from rand64() and samples each on engine `only`, or (only = NULL) on engine
+ * cmb200_owner(r, G); r holds them in draw order.  0 = sampled; -1 = nothing was drawn (no memory) or an
+ * engine failed (said on stderr for `who`).  The caller frees r->cand either way. */
+static int
+round_draw(struct filemap *m, struct fm_dev *only, size_t n, const char *who, struct round *r)
+{
+	r->cand = malloc(n * (sizeof(cmb200_addr) + 2 * sizeof(uint64_t) + sizeof(int32_t) + sizeof(int)));
+	if (!r->cand)
+		return -1;
+	r->draw = (uint64_t *)(r->cand + n);
+	r->ts = r->draw + n;
+	r->ok = (int32_t *)(r->ts + n);
+	r->own = (int *)(r->ok + n);
+	for (size_t i = 0; i < n; i++) {
+		r->draw[i] = rand64();
+		r->own[i] = only ? only->index : cmb200_owner(r->draw[i], m->g);
 	}
-	size_t *order = malloc(n * sizeof(size_t));
-	uint64_t *r = malloc(n * sizeof(uint64_t)), *t = malloc(n * sizeof(uint64_t));
-	cmb200_addr *a = malloc(n * sizeof(cmb200_addr));
-	int32_t *o = malloc(n * sizeof(int32_t));
-	size_t start[MAX_DEVICES + 1];
-	int rc = (order && r && t && a && o) ? 0 : -1;
-	if (rc == 0) {
-		for (size_t i = 0; i < n; i++)
-			own_out[i] = cmb200_owner(draws[i], m->g);
-		group_by_owner(m->g, n, own_out, order, start);
-		for (size_t j = 0; j < n; j++)
-			r[j] = draws[order[j]];
-		for (int k = 0; k < m->g && rc == 0; k++)
-			if (start[k + 1] > start[k])
-				rc = cmb200_sample(m->dev[k]->eng, start[k + 1] - start[k], r + start[k], a + start[k], t + start[k],
-				    o + start[k]);
-		for (size_t j = 0; rc == 0 && j < n; j++) {
-			cand[order[j]] = a[j];
-			ts[order[j]] = t[j];
-			ok[order[j]] = o[j];
+	const struct fan a[] = { { r->draw, sizeof(uint64_t), 0 }, { r->cand, sizeof(cmb200_addr), 1 },
+	                         { r->ts, sizeof(uint64_t), 1 }, { r->ok, sizeof(int32_t), 1 } };
+	const int rc = only ? cmb200_sample(only->eng, n, r->draw, r->cand, r->ts, r->ok)
+	                    : filemap_fan_out(m, n, r->own, 4, a, sample_call);
+	if (rc != 0)
+		fprintf(stderr, "cachemap_b200: %s could not sample the store: %s\n", who, cmb200_last_error());
+	return rc;
+}
+
+/* The oldest of draws 3i .. 3i+2 by the reference's rule (cachemap.c:29-41), as its index in the round;
+ * -1 when that draw found no record. */
+static long
+oldest_of_three(const struct round *r, size_t i)
+{
+	const uint64_t a = r->ts[3 * i], b = r->ts[3 * i + 1], c = r->ts[3 * i + 2];
+	const size_t k = 3 * i + (a < b ? (a > c ? 2 : 0) : (b > c ? 2 : 1));
+	return r->ok[k] > 0 ? (long)k : -1;
+}
+
+/* Moves the oldest of each of the first `need` triples of draws to the front of the round, in order, and
+ * returns how many there are: victim v comes from draw 3i or later, i >= v, so none is overwritten unread. */
+static size_t
+round_victims(struct round *r, size_t need)
+{
+	size_t nv = 0;
+	for (size_t i = 0; i < need; i++) {
+		const long k = oldest_of_three(r, i);
+		if (k >= 0) {
+			r->cand[nv] = r->cand[k];
+			r->own[nv++] = r->own[k];
 		}
 	}
-	free(order); free(r); free(t); free(a); free(o);
-	return rc;
+	return nv;
+}
+
+/* Removals ignore what each engine answers: one engine's failure does not keep the others' victims. */
+static int
+evict_call(struct fm_dev *d, size_t n, void *const *p)
+{
+	cmb200_evict_batch(d->eng, n, p[0], NULL);
+	return 0;
+}
+
+static int
+unset_call(struct fm_dev *d, size_t n, void *const *p)
+{
+	cmb200_unset_batch(d->eng, n, p[0]);
+	return 0;
 }
 
 /* Unsets n victims, each on its engine own[i].  evict: they are evictions, which leave ghosts under
@@ -962,20 +1056,8 @@ filemap_sample(struct filemap *m, struct fm_dev *only, size_t n, const uint64_t 
 static void
 filemap_unset_victims(struct filemap *m, size_t n, const cmb200_addr *victim, const int *own, int evict)
 {
-	cmb200_addr *v = malloc(n * sizeof(cmb200_addr));
-	if (!v)
-		return;
-	for (int k = 0; k < m->g; k++) {
-		size_t c = 0;
-		for (size_t i = 0; i < n; i++)
-			if (own[i] == k)
-				v[c++] = victim[i];
-		if (c && evict && m->ghost)
-			cmb200_evict_batch(m->dev[k]->eng, c, v, NULL);
-		else if (c)
-			cmb200_unset_batch(m->dev[k]->eng, c, v);
-	}
-	free(v);
+	const struct fan a[] = { { (void *)victim, sizeof(cmb200_addr), 0 } };
+	filemap_fan_out(m, n, own, 1, a, evict && m->ghost ? evict_call : unset_call);
 }
 
 /* Retires up to `want` records, each the oldest of three random live ones (cachemap.c:17-45): on
@@ -990,39 +1072,15 @@ filemap_evict_n(struct filemap *m, struct fm_dev *only, uint64_t want)
 		uint64_t need = want - gone;
 		if (need > before)
 			need = before;
-		if (need > 4096)
-			need = 4096;    /* per round; the loop continues */
-		uint64_t *draws = malloc(3 * need * sizeof(uint64_t));
-		uint64_t *ts = malloc(3 * need * sizeof(uint64_t));
-		int32_t *ok = malloc(3 * need * sizeof(int32_t));
-		int *own = malloc(3 * need * sizeof(int));
-		cmb200_addr *cand = malloc(3 * need * sizeof(cmb200_addr));
-		cmb200_addr *victim = malloc(need * sizeof(cmb200_addr));
-		int *vown = malloc(need * sizeof(int));
-		uint64_t nv = 0;
-		if (draws && ts && ok && own && cand && victim && vown) {
-			for (uint64_t i = 0; i < 3 * need; i++)
-				draws[i] = rand64();
-			if (filemap_sample(m, only, (size_t)(3 * need), draws, cand, ts, ok, own) == 0) {
-				for (uint64_t i = 0; i < need; i++) {
-					uint64_t a = ts[3 * i], b = ts[3 * i + 1], c = ts[3 * i + 2];
-					int pick;
-					if (a < b)
-						pick = (a > c) ? 2 : 0;         /* cachemap.c:29-41 */
-					else
-						pick = (b > c) ? 2 : 1;
-					if (ok[3 * i + pick] > 0) {
-						victim[nv] = cand[3 * i + pick];
-						vown[nv++] = own[3 * i + pick];
-					}
-				}
-				if (nv)
-					filemap_unset_victims(m, (size_t)nv, victim, vown, 1);
-			} else {
-				fprintf(stderr, "cachemap_b200: eviction could not sample the store: %s\n", cmb200_last_error());
-			}
+		if (need > ROUND_MAX)
+			need = ROUND_MAX;       /* per round; the loop continues */
+		struct round r;
+		size_t nv = 0;
+		if (round_draw(m, only, (size_t)(3 * need), "eviction", &r) == 0) {
+			nv = round_victims(&r, (size_t)need);
+			filemap_unset_victims(m, nv, r.cand, r.own, 1);
 		}
-		free(draws); free(ts); free(ok); free(own); free(cand); free(victim); free(vown);
+		free(r.cand);
 		/* two draws may have picked the same victim: count what really left the table */
 		uint64_t after = only ? cmb200_entries(only->eng) : filemap_count(m);
 		if (nv == 0 || after >= before)
@@ -1088,46 +1146,43 @@ filemap_demote_n(struct fm_dev *d, uint64_t want)
 	cmb200_addr *guard = filemap_promo_guard(d, &ng);
 	while (moved < want && idle < 16) {
 		uint64_t need = want - moved;
-		if (need > 4096)
-			need = 4096;
-		const uint64_t nd = 3 * need;
-		uint64_t *draws = malloc(nd * sizeof(uint64_t));
-		uint64_t *ts = malloc(nd * sizeof(uint64_t));
-		int32_t *ok = malloc(nd * sizeof(int32_t));
-		cmb200_addr *cand = malloc(nd * sizeof(cmb200_addr));
+		if (need > ROUND_MAX)
+			need = ROUND_MAX;
+		const size_t nd = (size_t)(3 * need);
 		struct aged *old = malloc(nd * sizeof(struct aged));
-		cmb200_addr *victim = malloc(nd * sizeof(cmb200_addr));
+		struct round r = { NULL };
 		uint64_t round = 0;
-		if (draws && ts && ok && cand && old && victim) {
-			for (uint64_t i = 0; i < nd; i++)
-				draws[i] = rand64();
-			if (cmb200_sample(d->eng, (size_t)nd, draws, cand, ts, ok) == 0) {
-				uint64_t nv = 0;
-				for (uint64_t i = 0; i < nd; i++)
-					if (ok[i] > 0 && !(guard && bsearch(&cand[i], guard, ng, sizeof(cmb200_addr), addr_cmp)))
-						old[nv++] = (struct aged){ ts[i], cand[i] };
-				qsort(old, (size_t)nv, sizeof(struct aged), aged_cmp);
-				for (uint64_t k = 0; k < nv && moved < want;) {
-					uint64_t take = want - moved < nv - k ? want - moved : nv - k, got = 0;
-					for (uint64_t j = 0; j < take; j++)
-						victim[j] = old[k + j].a;
-					if (cmb200_demote_batch(d->eng, (size_t)take, victim, &got) != 0) {
-						fprintf(stderr, "cachemap_b200: demotion to the host tier failed: %s\n", cmb200_last_error());
-						break;
-					}
-					moved += got;
-					round += got;
-					k += take;
+		if (old && round_draw(d->m, d, nd, "demotion", &r) == 0) {
+			size_t nv = 0;
+			for (size_t i = 0; i < nd; i++)
+				if (r.ok[i] > 0 && !(guard && bsearch(&r.cand[i], guard, ng, sizeof(cmb200_addr), addr_cmp)))
+					old[nv++] = (struct aged){ r.ts[i], r.cand[i] };
+			qsort(old, nv, sizeof(struct aged), aged_cmp);
+			for (size_t k = 0; k < nv; k++)
+				r.cand[k] = old[k].a;           /* oldest first */
+			for (size_t k = 0; k < nv && moved < want;) {
+				uint64_t take = want - moved < nv - k ? want - moved : nv - k, got = 0;
+				if (cmb200_demote_batch(d->eng, (size_t)take, r.cand + k, &got) != 0) {
+					fprintf(stderr, "cachemap_b200: demotion to the host tier failed: %s\n", cmb200_last_error());
+					break;
 				}
-			} else {
-				fprintf(stderr, "cachemap_b200: demotion could not sample the store: %s\n", cmb200_last_error());
+				moved += got;
+				round += got;
+				k += take;
 			}
 		}
-		free(draws); free(ts); free(ok); free(cand); free(old); free(victim);
+		free(old);
+		free(r.cand);
 		idle = round ? 0 : idle + 1;
 	}
 	free(guard);
 	return moved;
+}
+
+static int
+estimate_call(struct fm_dev *d, size_t n, void *const *p)
+{
+	return cmb200_freq_estimate(d->eng, n, p[0], p[1]);
 }
 
 /* est_out[i] = the frequency estimate of addr[i]'s key, from the sketch of the engine that owns it.  -1 if
@@ -1135,36 +1190,27 @@ filemap_demote_n(struct fm_dev *d, uint64_t want)
 static int
 filemap_estimate(struct filemap *m, size_t n, const cmb200_addr *addr, uint8_t *est_out)
 {
-	if (m->g == 1)
-		return cmb200_freq_estimate(m->dev[0]->eng, n, addr, est_out);
-	cmb200_addr *a = malloc(n * sizeof(*a));
-	size_t *at = malloc(n * sizeof(*at));
-	uint8_t *e = malloc(n);
-	int rc = (a && at && e) ? 0 : -1;
-	for (int k = 0; k < m->g && rc == 0; k++) {
-		size_t c = 0;
+	int *own = NULL;
+	if (m->g > 1) {
+		if (!(own = malloc(n * sizeof(*own))))
+			return -1;
 		for (size_t i = 0; i < n; i++)
-			if (filemap_owner(m, &addr[i]) == m->dev[k]) {
-				at[c] = i;
-				a[c++] = addr[i];
-			}
-		if (c && cmb200_freq_estimate(m->dev[k]->eng, c, a, e) != 0)
-			rc = -1;
-		for (size_t i = 0; i < c && rc == 0; i++)
-			est_out[at[i]] = e[i];
+			own[i] = cmb200_owner(addr_key(&addr[i]), m->g);
 	}
-	free(a); free(at); free(e);
+	const struct fan a[] = { { (void *)addr, sizeof(cmb200_addr), 0 }, { est_out, 1, 1 } };
+	const int rc = filemap_fan_out(m, n, own, 2, a, estimate_call);
+	free(own);
 	return rc;
 }
 
-struct drawn { cmb200_addr a; uint64_t i; };
+struct drawn { cmb200_addr a; size_t k; };
 
 static int
 drawn_cmp(const void *x, const void *y)
 {
 	const struct drawn *p = x, *q = y;
 	const int c = addr_cmp(&p->a, &q->a);
-	return c ? c : (p->i < q->i ? -1 : p->i > q->i);
+	return c ? c : (p->k < q->k ? -1 : p->k > q->k);
 }
 
 /* Admission by frequency (CMB200_ADMIT=freq) for the `want` pages that overflow the store, pages[0..want):
@@ -1182,74 +1228,51 @@ filemap_admit_n(struct filemap *m, uint64_t want, const cmb200_addr *pages, uint
 	int idle = 0;
 	while (done < want && idle < 16) {
 		uint64_t need = want - done;
-		if (need > 4096)
-			need = 4096;
-		uint64_t *draws = malloc(3 * need * sizeof(uint64_t));
-		uint64_t *ts = malloc(3 * need * sizeof(uint64_t));
-		int32_t *ok = malloc(3 * need * sizeof(int32_t));
-		int *own = malloc(3 * need * sizeof(int));
-		cmb200_addr *cand = malloc(3 * need * sizeof(cmb200_addr));
+		if (need > ROUND_MAX)
+			need = ROUND_MAX;
 		struct drawn *dr = malloc(need * sizeof(struct drawn));
-		int *pk = malloc(need * sizeof(int));
-		cmb200_addr *victim = malloc(2 * need * sizeof(cmb200_addr));  /* then the pages, for one estimate */
-		int *vown = malloc(need * sizeof(int));
 		uint8_t *ev = malloc(2 * need);        /* estimates: the victims', then the pages' (ep) */
-		uint64_t nv = 0;
-		if (draws && ts && ok && own && cand && dr && pk && victim && vown && ev) {
-			for (uint64_t i = 0; i < 3 * need; i++)
-				draws[i] = rand64();
-			if (filemap_sample(m, NULL, (size_t)(3 * need), draws, cand, ts, ok, own) == 0) {
-				uint64_t nd = 0;
-				for (uint64_t i = 0; i < need; i++) {
-					uint64_t a = ts[3 * i], b = ts[3 * i + 1], c = ts[3 * i + 2];
-					int pick;
-					if (a < b)
-						pick = (a > c) ? 2 : 0;         /* cachemap.c:29-41 */
-					else
-						pick = (b > c) ? 2 : 1;
-					pk[i] = ok[3 * i + pick] > 0 ? pick : -1;
-					if (pk[i] >= 0)
-						dr[nd++] = (struct drawn){ cand[3 * i + pick], i };
-				}
-				qsort(dr, (size_t)nd, sizeof(*dr), drawn_cmp);
-				for (uint64_t k = 1; k < nd; k++)
-					if (addr_cmp(&dr[k].a, &dr[k - 1].a) == 0)
-						pk[dr[k].i] = -1;                 /* drawn before in this round */
-				for (uint64_t i = 0; i < need; i++)
-					if (pk[i] >= 0) {
-						victim[nv] = cand[3 * i + pk[i]];
-						vown[nv++] = own[3 * i + pk[i]];
-					}
-				/* victims and pages in one call per engine */
-				uint8_t *ep = ev + nv;
-				memcpy(victim + nv, pages + done, (size_t)nv * sizeof(cmb200_addr));
-				if (nv && filemap_estimate(m, (size_t)(2 * nv), victim, ev) != 0) {
-					if (!__atomic_exchange_n(&warned, 1, __ATOMIC_RELAXED))
-						fprintf(stderr, "cachemap_b200: admission has no estimates (%s); admitting every page\n",
-						    cmb200_last_error());
-					memset(ev, 0, (size_t)nv);
-					memset(ep, 1, (size_t)nv);
-				}
-				uint64_t ng = 0, nr = 0;
-				for (uint64_t k = 0; k < nv; k++) {
-					if (ep[k] > ev[k]) {
-						victim[ng] = victim[k];
-						vown[ng++] = vown[k];
-					} else {
-						reject[done + k] = 1;
-						nr++;
-					}
-				}
-				if (ng)
-					filemap_unset_victims(m, (size_t)ng, victim, vown, 1);
-				__atomic_fetch_add(&m->admitted, ng, __ATOMIC_RELAXED);
-				__atomic_fetch_add(&m->rejected, nr, __ATOMIC_RELAXED);
-			} else {
-				fprintf(stderr, "cachemap_b200: eviction could not sample the store: %s\n", cmb200_last_error());
+		struct round r = { NULL };
+		size_t nv = 0;
+		if (dr && ev && round_draw(m, NULL, (size_t)(3 * need), "eviction", &r) == 0) {
+			size_t nd = 0;
+			for (size_t i = 0; i < need; i++) {
+				const long k = oldest_of_three(&r, i);
+				if (k >= 0)
+					dr[nd++] = (struct drawn){ r.cand[k], (size_t)k };
 			}
+			qsort(dr, nd, sizeof(*dr), drawn_cmp);
+			for (size_t j = 1; j < nd; j++)
+				if (addr_cmp(&dr[j].a, &dr[j - 1].a) == 0)
+					r.ok[dr[j].k] = 0;              /* drawn before in this round: no victim */
+			nv = round_victims(&r, (size_t)need);
+			/* victims and pages in one call per engine */
+			uint8_t *ep = ev + nv;
+			memcpy(r.cand + nv, pages + done, nv * sizeof(cmb200_addr));
+			if (nv && filemap_estimate(m, 2 * nv, r.cand, ev) != 0) {
+				if (!__atomic_exchange_n(&warned, 1, __ATOMIC_RELAXED))
+					fprintf(stderr, "cachemap_b200: admission has no estimates (%s); admitting every page\n",
+					    cmb200_last_error());
+				memset(ev, 0, nv);
+				memset(ep, 1, nv);
+			}
+			uint64_t ng = 0, nr = 0;
+			for (size_t k = 0; k < nv; k++) {
+				if (ep[k] > ev[k]) {
+					r.cand[ng] = r.cand[k];
+					r.own[ng++] = r.own[k];
+				} else {
+					reject[done + k] = 1;
+					nr++;
+				}
+			}
+			filemap_unset_victims(m, (size_t)ng, r.cand, r.own, 1);
+			__atomic_fetch_add(&m->admitted, ng, __ATOMIC_RELAXED);
+			__atomic_fetch_add(&m->rejected, nr, __ATOMIC_RELAXED);
 		}
-		free(draws); free(ts); free(ok); free(own); free(cand); free(dr); free(pk); free(victim); free(vown);
+		free(dr);
 		free(ev);
+		free(r.cand);
 		done += nv;
 		idle = nv ? 0 : idle + 1;
 	}
@@ -1379,12 +1402,6 @@ filemap_arena_room(struct fm_dev *d, uint64_t incoming, int may_evict)
 	}
 }
 
-static void
-filemap_check_arena(struct fm_dev *d, uint64_t incoming)
-{
-	filemap_arena_room(d, incoming, 1);
-}
-
 /* One promotion round (CMB200_TIER_PROMOTE = N): up to N addresses that gets answered from the host
  * tier since the last round, newest first, go back to the arena.  Room is made only by demoting the
  * oldest arena records and compacting, never by evicting; when that frees too little, the round
@@ -1436,7 +1453,18 @@ static void
 filemap_make_room(struct fm_dev *d, uint64_t incoming, const cmb200_addr *addr, uint8_t *reject)
 {
 	filemap_evict(d->m, incoming, addr, reject);
-	filemap_check_arena(d, incoming);
+	filemap_arena_room(d, incoming, 1);
+}
+
+/* Row i is the last of its key in addr[0..n): a batch's newest page of a key decides for the key. */
+static int
+last_of_key(size_t n, const cmb200_addr *addr, size_t i)
+{
+	const uint64_t k = addr_key(&addr[i]);
+	for (size_t j = i + 1; j < n; j++)
+		if (addr_key(&addr[j]) == k)
+			return 0;
+	return 1;
 }
 
 /* After a put of n pages whose stored lengths are lens (-1: nothing stored): the keys whose newest page
@@ -1448,14 +1476,8 @@ filemap_unset_dropped(struct fm_dev *d, size_t n, const cmb200_addr *addr, const
 	cmb200_addr *v = NULL;
 	size_t nv = 0;
 	for (size_t i = 0; i < n; i++) {
-		if (lens[i] >= 0)
-			continue;
-		size_t j = i + 1;       /* a later row of the same key supersedes this one (its lens is -1 too) */
-		const uint64_t k = addr_key(&addr[i]);
-		while (j < n && addr_key(&addr[j]) != k)
-			j++;
-		if (j < n)
-			continue;
+		if (lens[i] >= 0 || !last_of_key(n, addr, i))
+			continue;       /* a later row of the same key supersedes this one (its lens is -1 too) */
 		if (!v && !(v = malloc(n * sizeof(*v))))
 			return;
 		v[nv++] = addr[i];
@@ -2146,7 +2168,7 @@ put_part(void *arg)
 	int rc = -1;
 	pthread_mutex_lock(&d->stage_mu);
 	pthread_mutex_lock(&d->room_mu);
-	filemap_check_arena(d, p->c);
+	filemap_arena_room(d, p->c, 1);
 	filemap_land_begin(d);
 	if (!p->on_dev) {
 		uint8_t *h = stage_host(d);
@@ -2259,15 +2281,10 @@ filemap_reject_batch(struct filemap *m, size_t n, const cmb200_addr *addr, uint8
 	int *own = NULL;
 	size_t nv = 0;
 	for (size_t i = 0; i < n; i++) {
-		if (!reject[i])
-			continue;
-		const uint64_t k = addr_key(&addr[i]);
-		size_t j = i + 1;
-		while (j < n && addr_key(&addr[j]) != k)
-			j++;
-		if (j < n)
+		if (!reject[i] || !last_of_key(n, addr, i))
 			continue;               /* a later page of the key decides */
-		for (j = 0; j <= i; j++)
+		const uint64_t k = addr_key(&addr[i]);
+		for (size_t j = 0; j <= i; j++)
 			if (addr_key(&addr[j]) == k)
 				valid[j] = 0;
 		if (!v && (!(v = malloc(n * sizeof(*v))) || !(own = malloc(n * sizeof(*own)))))
@@ -2275,8 +2292,7 @@ filemap_reject_batch(struct filemap *m, size_t n, const cmb200_addr *addr, uint8
 		own[nv] = cmb200_owner(k, m->g);
 		v[nv++] = addr[i];
 	}
-	if (nv)
-		filemap_unset_victims(m, nv, v, own, 0);
+	filemap_unset_victims(m, nv, v, own, 0);
 	free(v);
 	free(own);
 	memset(reject, 0, n);
@@ -2332,7 +2348,7 @@ put_batch_common(struct cachemap *cm, uint64_t n, const uint64_t *offset, const 
 			if (c == m && (k == 0 || !on_dev)) {
 				/* the whole slice is this engine's (always so with one engine): the caller's arrays as they are */
 				pthread_mutex_lock(&d->room_mu);
-				filemap_check_arena(d, c);
+				filemap_arena_room(d, c, 1);
 				filemap_land_begin(d);
 				if (on_dev)
 					cmb200_put_batch_dev(d->eng, (size_t)m, bk.addr + at, bk.valid + at, pg, bk.ts + at, NULL);
@@ -2683,7 +2699,7 @@ filemap_patch(struct filemap *m, const cmb200_addr *a, uint32_t page_off, uint32
 	}
 	/* a patch adds no entry, so only the arena needs room: no eviction by count */
 	pthread_mutex_lock(&d->room_mu);
-	filemap_check_arena(d, 1);
+	filemap_arena_room(d, 1, 1);
 	int32_t st = CMB200_MISS;
 	if (!cmb200_patch_batch || cmb200_patch_batch(d->eng, 1, a, &page_off, &len, bytes, &ts, &st) != 0) {
 		if (cmb200_patch_batch)

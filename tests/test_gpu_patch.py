@@ -467,7 +467,7 @@ DROP_IN_CASES = {
     # 1 MiB pages: no fused get, and records that leave the arena check no margin
     "pshift20": ({}, 20, 12, "exact"),
     # 3 MiB of incompressible pages over a 1 MiB arena: writes demote, reads promote, and pwrite
-    # patches host-tier records after filemap_check_arena has made room.  A ring of 64 slots flushes
+    # patches host-tier records after filemap_arena_room has made room.  A ring of 64 slots flushes
     # batches that demotion always makes room for
     "host_tier": ({"CMB200_ARENA_MB": "1", "CMB200_HOST_TIER_MB": "64", "CMB200_TIER_PROMOTE": "1",
                    "CMB200_WB_SLOTS": "64"}, 12, 256, "exact"),
