@@ -25,7 +25,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_get_batch_dev", "cachemap_get_counters", "cachemap_engine", "cachemap_engines",
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
     "cachemap_pread", "cachemap_pwrite", "cachemap_rename", "cachemap_get_admission",
-    "cachemap_load_progress", "cachemap_hit_curve",
+    "cachemap_load_progress", "cachemap_hit_curve", "cachemap_pin", "cachemap_unpin", "cachemap_pin_stats",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -34,7 +34,8 @@ EXPORTED_SYMBOLS = [
     "cmb200_host_alloc", "cmb200_host_free", "cmb200_dev_alloc", "cmb200_dev_free",
     "cmb200_memcpy_h2d", "cmb200_memcpy_d2h", "cmb200_stream", "cmb200_sync",
     "cmb200_put_batch", "cmb200_put_batch_dev", "cmb200_put_batch_async", "cmb200_wait", "cmb200_get_batch", "cmb200_get_batch_dev",
-    "cmb200_unset_batch", "cmb200_entries", "cmb200_sample", "cmb200_read_records",
+    "cmb200_unset_batch", "cmb200_entries", "cmb200_sample", "cmb200_pin_set", "cmb200_pin_count",
+    "cmb200_pin_promote", "cmb200_read_records",
     "cmb200_read_fingerprints", "cmb200_get_stats", "cmb200_compose_keys",
     "cmb200_set_stream_order", "cmb200_locate_batch", "cmb200_save", "cmb200_load",
     "cmb200_put_step", "cmb200_import_records_dev", "cmb200_compact",
@@ -123,6 +124,9 @@ def lib() -> C.CDLL:
         "cachemap_checkpoint": (i32, [vp]),
         "cachemap_invalidate": (u64, [vp, u64, u32, u64, u64]),
         "cachemap_rename": (u64, [vp, u64, u64, u32]),
+        "cachemap_pin": (C.c_int64, [vp, u64, u32, u64, u64]),
+        "cachemap_unpin": (u64, [vp, u64, u32, u64, u64]),
+        "cachemap_pin_stats": (None, [vp, vp, vp, vp]),
         "cachemap_read_range": (i32, [vp, u64, u32, u64, sz, vp]),
         "cachemap_write_range": (None, [vp, u64, u32, u64, sz, vp]),
         "cachemap_pread": (i32, [vp, u64, u32, u64, sz, vp]),
@@ -164,6 +168,9 @@ def lib() -> C.CDLL:
         "cmb200_patch_batch": (i32, [vp, sz, vp, vp, vp, vp, vp, vp]),
         "cmb200_entries": (u64, [vp]),
         "cmb200_sample": (i32, [vp, sz, vp, vp, vp, vp]),
+        "cmb200_pin_set": (i32, [vp, sz, vp]),
+        "cmb200_pin_count": (i32, [vp, vp, vp]),
+        "cmb200_pin_promote": (i32, [vp, vp]),
         "cmb200_read_records": (i32, [vp, sz, vp, vp, sz, vp]),
         "cmb200_read_fingerprints": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_get_stats": (i32, [vp, vp]),
@@ -649,6 +656,23 @@ class Engine:
         _check(lib().cmb200_sample(self.h, n, _ptr(r), _ptr(addr), _ptr(ts), _ptr(ok)), "cmb200_sample")
         return addr, ts, ok
 
+    def pin_set(self, ranges):
+        """cmb200_pin_set: ranges = [(u, l_first, l_last), ...], sorted by (u, l_first) and disjoint; [] clears."""
+        r = np.ascontiguousarray(np.array(ranges, dtype=np.uint64).reshape(-1, 3))
+        _check(lib().cmb200_pin_set(self.h, len(r), _ptr(r)), "cmb200_pin_set")
+
+    def pin_count(self):
+        """cmb200_pin_count -> (live pinned records in the arena, in the host tier)."""
+        a, t = C.c_uint64(), C.c_uint64()
+        _check(lib().cmb200_pin_count(self.h, C.byref(a), C.byref(t)), "cmb200_pin_count")
+        return a.value, t.value
+
+    def pin_promote(self) -> int:
+        """cmb200_pin_promote -> pinned host-tier records moved back to the arena."""
+        n = C.c_uint64()
+        _check(lib().cmb200_pin_promote(self.h, C.byref(n)), "cmb200_pin_promote")
+        return n.value
+
     def read_records_raw(self, u, l):
         """-> (records [n, 24 + bsize + 1024] uint8, lens [n] int32; -1 = no record): the stored
         filemap records {data_prefix, payload} as they lie in the arena."""
@@ -962,6 +986,21 @@ class Cachemap:
         """edgefs_rename: the cached pages of (nhid_to, genid) are dropped and those of (nhid_from, genid)
         move to nhid_to -> pages moved."""
         return int(lib().cachemap_rename(self.h, nhid_from, nhid_to, genid))
+
+    def pin(self, nhid: int, genid: int, off: int, size: int) -> int:
+        """cachemap_pin: pins the pages of (nhid, genid) overlapping bytes [off, off + size) -> pages newly
+        pinned, or -1 when refused (nothing pinned)."""
+        return int(lib().cachemap_pin(self.h, nhid, genid, off, size))
+
+    def unpin(self, nhid: int, genid: int, off: int, size: int) -> int:
+        """cachemap_unpin -> pages unpinned; size = Cachemap.TO_END unpins every page from off on."""
+        return int(lib().cachemap_unpin(self.h, nhid, genid, off, size))
+
+    def pin_stats(self):
+        """cachemap_pin_stats -> (pages named by pins, pinned pages cached in HBM, in the host tier)."""
+        p, a, t = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        lib().cachemap_pin_stats(self.h, C.byref(p), C.byref(a), C.byref(t))
+        return p.value, a.value, t.value
 
     def counters(self):
         rq, ht = C.c_uint64(), C.c_uint64()

@@ -35,6 +35,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <sys/random.h>
 #include <sys/stat.h>
 #include <time.h>
 #include <sched.h>
@@ -81,6 +82,10 @@ extern uint32_t cmb200_ghost_set(uint64_t key, int log2_sets);
 #pragma weak cmb200_set_file_key
 #pragma weak cmb200_evict_batch
 #pragma weak cmb200_ghost_stats
+#pragma weak cmb200_pin_set
+#pragma weak cmb200_pin_count
+#pragma weak cmb200_pin_promote
+#pragma weak cmb200_aead_seal_batch
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
 #define LEADERS 32              /* batches of gets that may be in flight at once, each on its own engine lane
@@ -209,9 +214,20 @@ struct filemap {
 	uint64_t load_loaded, load_total;       /* (atomic) */
 	pthread_mutex_t load_mu;
 	pthread_cond_t load_cv;
+	/* pins (cachemap_pin): pin_n ranges sorted by (u, l_first), disjoint and not touching, the same list on
+	 * every engine (cmb200_pin_set), naming pin_pages pages, at most pin_max (CMB200_PIN_MAX, set while the
+	 * engines start).  Under pin_mu, which also orders the writes of <destdir>/cachemap_b200.pins.  pin_sealed:
+	 * CMB200_KEY_FILE's key is in pin_key and seals the file. */
+	pthread_mutex_t pin_mu;
+	cmb200_pin_range *pins;
+	size_t pin_n;
+	uint64_t pin_pages, pin_max;
+	int pin_sealed;
+	uint8_t pin_key[32];
 };
 
 #define SNAPSHOT_NAME "cachemap_b200.snap"
+#define PINS_NAME "cachemap_b200.pins"
 
 static int
 filemap_snapshot_path(struct filemap *m, char *out, size_t cap)
@@ -418,6 +434,261 @@ load_background(void)
 	return 0;
 }
 
+/* ---- pin list ------------------------------------------------------------------------------------ */
+
+static int
+pin_cmp(const void *x, const void *y)
+{
+	const cmb200_pin_range *a = x, *b = y;
+	if (a->u != b->u)
+		return a->u < b->u ? -1 : 1;
+	return a->l_first < b->l_first ? -1 : a->l_first > b->l_first;
+}
+
+/* Sorts the n ranges of r and merges those of one u that overlap or touch.  Returns how many are left. */
+static size_t
+pin_normalize(cmb200_pin_range *r, size_t n)
+{
+	if (n == 0)
+		return 0;
+	qsort(r, n, sizeof(*r), pin_cmp);
+	size_t k = 0;
+	for (size_t i = 1; i < n; i++) {
+		cmb200_pin_range *p = &r[k];
+		if (r[i].u == p->u && (r[i].l_first <= p->l_last || r[i].l_first - 1 == p->l_last)) {
+			if (r[i].l_last > p->l_last)
+				p->l_last = r[i].l_last;
+		} else {
+			r[++k] = r[i];
+		}
+	}
+	return k + 1;
+}
+
+/* Copies the n ranges of cur to out (room for n + 1) without the pages {u, l}, lf <= l <= ll: a range
+ * that holds some of them keeps the rest, split in two when they lie inside it.  The pages taken go to
+ * cut (room for n, nullable) as ranges, *n_cut of them.  Returns the length of out. */
+static size_t
+pin_cut(const cmb200_pin_range *cur, size_t n, uint64_t u, uint64_t lf, uint64_t ll, cmb200_pin_range *out,
+    cmb200_pin_range *cut, size_t *n_cut)
+{
+	size_t k = 0, c = 0;
+	for (size_t i = 0; i < n; i++) {
+		const cmb200_pin_range r = cur[i];
+		if (r.u != u || r.l_last < lf || r.l_first > ll) {
+			out[k++] = r;
+			continue;
+		}
+		if (r.l_first < lf)
+			out[k++] = (cmb200_pin_range){ r.u, r.l_first, lf - 1 };
+		if (r.l_last > ll)
+			out[k++] = (cmb200_pin_range){ r.u, ll + 1, r.l_last };
+		if (cut)
+			cut[c++] = (cmb200_pin_range){ r.u, r.l_first > lf ? r.l_first : lf, r.l_last < ll ? r.l_last : ll };
+	}
+	if (n_cut)
+		*n_cut = c;
+	return k;
+}
+
+static uint64_t
+pin_total(const cmb200_pin_range *r, size_t n)
+{
+	uint64_t pages = 0;
+	for (size_t i = 0; i < n; i++)
+		pages += r[i].l_last - r[i].l_first + 1;
+	return pages;
+}
+
+/* {u, l} is pinned (pin_mu held). */
+static int
+pin_has(const struct filemap *m, const cmb200_addr *a)
+{
+	size_t lo = 0, hi = m->pin_n;                   /* the first range that starts after a */
+	while (lo < hi) {
+		const size_t mid = (lo + hi) / 2;
+		const cmb200_pin_range *r = &m->pins[mid];
+		if (r->u < a->u || (r->u == a->u && r->l_first <= a->l))
+			lo = mid + 1;
+		else
+			hi = mid;
+	}
+	return lo > 0 && m->pins[lo - 1].u == a->u && a->l <= m->pins[lo - 1].l_last;
+}
+
+/* The tag of a sealed pins file: one ChaCha20-Poly1305 seal of an empty text with the file before the tag
+ * as AAD, nonce {file nonce, 0}. */
+static int
+pins_tag(struct filemap *m, const uint8_t *aad, size_t aad_len, uint64_t nonce, uint8_t tag[16])
+{
+	if (!cmb200_aead_seal_batch)
+		return -1;
+	uint8_t nc[12] = {0};
+	memcpy(nc, &nonce, 8);
+	const uint8_t *a[1] = { aad }, *msg[1] = { aad };
+	const size_t al[1] = { aad_len }, ml[1] = { 0 };
+	uint8_t *out[1] = { tag };
+	return cmb200_aead_seal_batch(m->dev[0]->device, m->pin_key, 1, nc, a, al, msg, ml, out);
+}
+
+/* Rewrites <destdir>/cachemap_b200.pins with the list (pin_mu held): "CMB200P1" (sealed: "CMB200Q1") |
+ * u32 version 1 | u32 pshift | u64 ranges | u64 file nonce | ranges x {u64 u, l_first, l_last} (| the
+ * 16-byte tag), little-endian, written to a temporary file and renamed over the old one. */
+static void
+filemap_pins_write(struct filemap *m)
+{
+	char path[2200], tmp[2300];
+	if (!m->persist || snprintf(path, sizeof(path), "%s/%s", m->destdir, PINS_NAME) >= (int)sizeof(path))
+		return;
+	snprintf(tmp, sizeof(tmp), "%s.tmp", path);
+	const size_t body = 32 + 24 * m->pin_n, len = body + (m->pin_sealed ? 16 : 0);
+	uint8_t *buf = malloc(len);
+	if (!buf)
+		return;
+	const uint32_t head[2] = { 1, (uint32_t)m->pshift };
+	const uint64_t nr = m->pin_n;
+	uint64_t nonce = 0;
+	memcpy(buf, m->pin_sealed ? "CMB200Q1" : "CMB200P1", 8);
+	memcpy(buf + 8, head, 8);
+	memcpy(buf + 16, &nr, 8);
+	const char *why = NULL;
+	if (m->pin_sealed && getrandom(&nonce, sizeof(nonce), 0) != (ssize_t)sizeof(nonce))
+		why = "no random file nonce";
+	memcpy(buf + 24, &nonce, 8);
+	for (size_t k = 0; k < m->pin_n; k++)
+		memcpy(buf + 32 + 24 * k, &m->pins[k], 24);
+	if (!why && m->pin_sealed && pins_tag(m, buf, body, nonce, buf + body) != 0)
+		why = cmb200_aead_seal_batch ? cmb200_last_error() : "the engine cannot seal";
+	FILE *f = why ? NULL : fopen(tmp, "wb");
+	if (!why && !f)
+		why = strerror(errno);
+	if (f) {
+		const int ok = fwrite(buf, 1, len, f) == len;
+		if (fclose(f) != 0 || !ok || rename(tmp, path) != 0) {
+			why = "cannot write it";
+			unlink(tmp);
+		}
+	}
+	if (why)
+		fprintf(stderr, "cachemap_b200: %s not written: %s\n", path, why);
+	free(buf);
+}
+
+/* Reads <destdir>/cachemap_b200.pins into the list, which is empty (as the engines start).  A file that is
+ * not a pins file of this version and page size, whose tag fails, or that is sealed while no key is set is
+ * ignored with a warning.  Otherwise its ranges are taken in file order up to the first one that is
+ * malformed, out of order, missing from a short file, or would take the list past CMB200_PIN_MAX pages or
+ * CMB200_PIN_RANGES ranges; a file not taken whole is warned about. */
+static void
+filemap_pins_read(struct filemap *m)
+{
+	char path[2200];
+	if (snprintf(path, sizeof(path), "%s/%s", m->destdir, PINS_NAME) >= (int)sizeof(path))
+		return;
+	FILE *f = fopen(path, "rb");
+	if (!f)
+		return;
+	const size_t cap = 32 + 24 * (size_t)CMB200_PIN_RANGES + 16 + 1;
+	uint8_t *buf = malloc(cap);
+	const size_t len = buf ? fread(buf, 1, cap, f) : 0;
+	fclose(f);
+	const char *why = NULL;
+	uint32_t head[2] = {0};
+	uint64_t nr = 0, nonce = 0;
+	int sealed = 0;
+	if (len < 32 || (memcmp(buf, "CMB200P1", 8) != 0 && !(sealed = memcmp(buf, "CMB200Q1", 8) == 0)))
+		why = "not a pins file";
+	if (!why) {
+		memcpy(head, buf + 8, 8);
+		memcpy(&nr, buf + 16, 8);
+		memcpy(&nonce, buf + 24, 8);
+		if (head[0] != 1)
+			why = "of another version";
+		else if (head[1] != (uint32_t)m->pshift)
+			why = "of another page size";
+	}
+	if (!why && sealed) {
+		uint8_t tag[16];
+		if (!m->pin_sealed)
+			why = "sealed, and no CMB200_KEY_FILE is set";
+		else if (nr > CMB200_PIN_RANGES || len != 32 + 24 * nr + 16)
+			why = "damaged";
+		else if (pins_tag(m, buf, len - 16, nonce, tag) != 0)
+			why = "not checked: the engine cannot open it";
+		else {
+			uint8_t diff = 0;
+			for (int i = 0; i < 16; i++)
+				diff |= tag[i] ^ buf[len - 16 + i];
+			if (diff)
+				why = "damaged or sealed with another key (its tag fails)";
+		}
+	}
+	if (why) {
+		fprintf(stderr, "cachemap_b200: %s ignored: the file is %s\n", path, why);
+		free(buf);
+		return;
+	}
+	const size_t avail = (len - 32 - (sealed ? 16 : 0)) / 24;
+	const size_t want = nr < avail ? (size_t)nr : avail;
+	m->pins = malloc((want ? want : 1) * sizeof(cmb200_pin_range));
+	size_t k = 0;
+	uint64_t pages = 0;
+	for (; m->pins && k < want && k < CMB200_PIN_RANGES; k++) {
+		cmb200_pin_range r;
+		memcpy(&r, buf + 32 + 24 * k, 24);
+		const cmb200_pin_range *p = k ? &m->pins[k - 1] : NULL;
+		if (r.l_first > r.l_last || (p && (r.u < p->u || (r.u == p->u && r.l_first <= p->l_last))) ||
+		    r.l_last - r.l_first >= m->pin_max - pages)
+			break;
+		m->pins[k] = r;
+		pages += r.l_last - r.l_first + 1;
+	}
+	m->pin_n = k;
+	m->pin_pages = pages;
+	if (k < nr)
+		fprintf(stderr, "cachemap_b200: %s: %zu of its %llu ranges kept (%s)\n", path, k, (unsigned long long)nr,
+		    k == want && want < nr ? "the file is short" : "the next one is malformed or over CMB200_PIN_MAX");
+	free(buf);
+}
+
+/* Sends the list to every engine (pin_mu held, or the engines starting). */
+static void
+filemap_pins_send(struct filemap *m)
+{
+	for (int i = 0; i < m->g; i++)
+		if (cmb200_pin_set(m->engs[i], m->pin_n, m->pins) != 0)
+			fprintf(stderr, "cachemap_b200: pins not set on engine %d: %s\n", i, cmb200_last_error());
+}
+
+/* Makes `next` (n ranges, normalized) the list: on every engine, then in the file (pin_mu held).  The old
+ * list is freed. */
+static void
+filemap_pins_install(struct filemap *m, cmb200_pin_range *next, size_t n)
+{
+	free(m->pins);
+	m->pins = next;
+	m->pin_n = n;
+	m->pin_pages = pin_total(next, n);
+	filemap_pins_send(m);
+	filemap_pins_write(m);
+}
+
+/* The pinned records of each engine's host tier go back to its arena while free bytes hold them; under the
+ * engine's room lock, so that no put's room is taken. */
+static void
+filemap_pins_promote(struct filemap *m)
+{
+	for (int i = 0; i < m->g && cmb200_pin_promote; i++) {
+		struct fm_dev *d = m->dev[i];
+		if (!d->host_tier)
+			continue;
+		pthread_mutex_lock(&d->room_mu);
+		if (cmb200_pin_promote(d->eng, NULL) != 0)
+			fprintf(stderr, "cachemap_b200: pinned records not promoted: %s\n", cmb200_last_error());
+		pthread_mutex_unlock(&d->room_mu);
+	}
+}
+
 /* Engine `index` of the map on CUDA device `device`, with its buffers; NULL if it cannot start.
  * The knobs apply per engine; the table and the default arena are sized for its share of the
  * capacity, ceil(n / G). */
@@ -564,7 +835,26 @@ filemap_engine_ready(struct filemap *m)
 						    "written\n", cmb200_last_error());
 						m->persist = 0;
 					}
+				if (have > 0 && m->persist) {
+					memcpy(m->pin_key, key, sizeof(key));
+					m->pin_sealed = 1;
+				}
 				explicit_bzero(key, sizeof(key));
+			}
+			/* CMB200_PIN_MAX: pages the pins may name, capacity / 4 by default, at most half the capacity so
+			 * that at capacity at least half the entries stay evictable; 0 = no pins */
+			const long pin_max = env_long("CMB200_PIN_MAX", -1);
+			m->pin_max = pin_max < 0 ? m->n / 4 : (uint64_t)pin_max;
+			if (m->pin_max > m->n / 2) {
+				fprintf(stderr, "cachemap_b200: CMB200_PIN_MAX=%ld is above half the capacity; pinning at most "
+				    "%llu pages\n", pin_max, (unsigned long long)(m->n / 2));
+				m->pin_max = m->n / 2;
+			}
+			/* the pins are in force before any record is loaded */
+			if (m->persist && cmb200_pin_set) {
+				filemap_pins_read(m);
+				if (m->pin_n)
+					filemap_pins_send(m);
 			}
 			char snap[2200], d1[2300];
 			if (m->persist && filemap_snapshot_path(m, snap, sizeof(snap)) && access(snap, R_OK) == 0) {
@@ -602,6 +892,8 @@ filemap_engine_ready(struct filemap *m)
 					    "as it is and not written\n", snap);
 					m->persist = 0;
 				}
+				if (!m->loader && m->pin_n)
+					filemap_pins_promote(m);
 			}
 			/* the flushers start here, i.e. in the process that actually caches (after any fork) */
 			for (int i = 0; i < g; i++) {
@@ -651,6 +943,7 @@ filemap_create(char *destdir, uint64_t n, int compress_accel, int pshift)
 	pthread_cond_init(&m->ckpt_cv, NULL);
 	pthread_mutex_init(&m->load_mu, NULL);
 	pthread_cond_init(&m->load_cv, NULL);
+	pthread_mutex_init(&m->pin_mu, NULL);
 	return m;
 }
 
@@ -767,6 +1060,12 @@ filemap_loader(void *arg)
 		m->chain_deltas = (int)k;
 	pthread_mutex_unlock(&m->snap_mu);
 	m->loader = NULL;
+	/* the pinned records the load put in a host tier */
+	pthread_mutex_lock(&m->pin_mu);
+	const size_t pinned = m->pin_n;
+	pthread_mutex_unlock(&m->pin_mu);
+	if (pinned)
+		filemap_pins_promote(m);
 	pthread_mutex_lock(&m->load_mu);
 	__atomic_store_n(&m->loading, 0, __ATOMIC_RELEASE);
 	pthread_cond_broadcast(&m->load_cv);
@@ -884,6 +1183,9 @@ filemap_free(struct filemap *m)
 	for (int i = 0; i < m->g; i++)
 		fm_dev_free(m->dev[i]);
 	pthread_mutex_destroy(&m->snap_mu);
+	pthread_mutex_destroy(&m->pin_mu);
+	free(m->pins);
+	explicit_bzero(m->pin_key, sizeof(m->pin_key));
 	pthread_cond_destroy(&m->load_cv);
 	pthread_mutex_destroy(&m->load_mu);
 	pthread_cond_destroy(&m->ckpt_cv);
@@ -1256,6 +1558,12 @@ filemap_admit_n(struct filemap *m, uint64_t want, const cmb200_addr *pages, uint
 				memset(ev, 0, nv);
 				memset(ep, 1, nv);
 			}
+			/* a pinned page is always admitted: 16 is above every 4-bit counter */
+			pthread_mutex_lock(&m->pin_mu);
+			for (size_t k = 0; k < nv && m->pin_n; k++)
+				if (pin_has(m, &r.cand[nv + k]))
+					ep[k] = 16;
+			pthread_mutex_unlock(&m->pin_mu);
 			uint64_t ng = 0, nr = 0;
 			for (size_t k = 0; k < nv; k++) {
 				if (ep[k] > ev[k]) {
@@ -2743,6 +3051,21 @@ cachemap_pwrite(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64
 		filemap_patch(fm, &a, 0, (uint32_t)tail, src + ((p1 << pshift) - off), ts);
 }
 
+/* The addresses of the first and the last page of object (nhid_small, genid) that bytes [off, off + size)
+ * overlap, size >= 1.  The last byte, off + size - 1, saturates: TO_END and an overflowing end both mean
+ * "to the end", the page 2^44 - 1.  -1 when the first page does not fit 44 bits. */
+static int
+compose_span(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size,
+    cmb200_addr *first, cmb200_addr *last)
+{
+	if (compose_addr(cm, off, nhid_small, genid, first) != 0)
+		return -1;
+	const uint64_t end = size - 1 > UINT64_MAX - off ? UINT64_MAX : off + (size - 1);
+	if (compose_addr(cm, end, nhid_small, genid, last) != 0)
+		last->l = ((1ULL << PNUM_SHIFT) - 1) | ((uint64_t)genid << PNUM_SHIFT);
+	return 0;
+}
+
 uint64_t
 cachemap_invalidate(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size)
 {
@@ -2754,12 +3077,8 @@ cachemap_invalidate(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, ui
 		return 0;
 	filemap_drain(fm);                      /* every page accepted before the call is in a store */
 	cmb200_addr first, last;
-	if (compose_addr(cm, off, nhid_small, genid, &first) != 0)
+	if (compose_span(cm, nhid_small, genid, off, size, &first, &last) != 0)
 		return 0;                       /* put ignores such a page: none is cached */
-	/* the last byte, off + size - 1, saturating: TO_END and an overflowing end both mean "to the end" */
-	const uint64_t end = size - 1 > UINT64_MAX - off ? UINT64_MAX : off + (size - 1);
-	if (compose_addr(cm, end, nhid_small, genid, &last) != 0)
-		last.l = ((1ULL << PNUM_SHIFT) - 1) | ((uint64_t)genid << PNUM_SHIFT);
 	uint64_t removed = 0;
 	for (int i = 0; i < fm->g; i++) {       /* the object's pages are spread over the engines by key */
 		uint64_t r = 0;
@@ -2790,6 +3109,37 @@ filemap_invalidate_all(struct filemap *fm, uint64_t nhid_small, uint32_t genid)
 	return removed;
 }
 
+/* cachemap_rename's pins: those of `to` for genid are dropped and those of `from` become pins of `to`. */
+static void
+filemap_pins_rename(struct filemap *m, uint64_t from, uint64_t to, uint32_t genid)
+{
+	const uint64_t first = (uint64_t)genid << PNUM_SHIFT, last = first | ((1ULL << PNUM_SHIFT) - 1);
+	pthread_mutex_lock(&m->pin_mu);
+	const size_t n = m->pin_n;
+	/* room: each cut splits at most one range in two; the moved ranges come back at the end */
+	cmb200_pin_range *a = n ? malloc((2 * n + 2) * sizeof(*a)) : NULL, *b = n ? malloc((2 * n + 2) * sizeof(*b)) : NULL;
+	if (a && b) {
+		size_t moved = 0;
+		const size_t k = pin_cut(m->pins, n, to, first, last, a, NULL, NULL);
+		size_t j = pin_cut(a, k, from, first, last, b, a, &moved);
+		for (size_t i = 0; i < moved; i++)
+			b[j++] = (cmb200_pin_range){ to, a[i].l_first, a[i].l_last };
+		j = pin_normalize(b, j);
+		if (j != n || memcmp(b, m->pins, n * sizeof(*b)) != 0) {
+			if (j <= CMB200_PIN_RANGES) {
+				filemap_pins_install(m, b, j);
+				b = NULL;
+			} else {
+				fprintf(stderr, "cachemap_b200: cachemap_rename: the pins would need more than %d ranges; they "
+				    "stay as they are\n", CMB200_PIN_RANGES);
+			}
+		}
+	}
+	free(a);
+	free(b);
+	pthread_mutex_unlock(&m->pin_mu);
+}
+
 uint64_t
 cachemap_rename(struct cachemap *cm, uint64_t nhid_from, uint64_t nhid_to, uint32_t genid)
 {
@@ -2800,6 +3150,8 @@ cachemap_rename(struct cachemap *cm, uint64_t nhid_from, uint64_t nhid_to, uint3
 	if (!filemap_engine_ready(fm))
 		return 0;
 	filemap_drain(fm);                      /* every page accepted before the call is in a store */
+	/* the pins first, so that the moved pages are pinned on the engines before they arrive */
+	filemap_pins_rename(fm, nhid_from, nhid_to, genid);
 	/* the old pages of `to` go first: the move replaces only the pages `from` has */
 	uint64_t removed = filemap_invalidate_all(fm, nhid_to, genid);
 	const uint64_t first = (uint64_t)genid << PNUM_SHIFT, last = first | ((1ULL << PNUM_SHIFT) - 1);
@@ -2822,6 +3174,94 @@ cachemap_rename(struct cachemap *cm, uint64_t nhid_from, uint64_t nhid_to, uint3
 	/* moves and removals are changes of the store: the next checkpoint must write them */
 	__atomic_fetch_add(&fm->puts_seen, moved + dropped + removed, __ATOMIC_RELAXED);
 	return moved;
+}
+
+int64_t
+cachemap_pin(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size)
+{
+	struct filemap *m = cm->pages;
+	cmb200_addr first, last;
+	if (size == 0 || size == CACHEMAP_TO_END || compose_span(cm, nhid_small, genid, off, size, &first, &last) != 0)
+		return -1;
+	if (!cmb200_pin_set || !filemap_engine_ready(m))
+		return -1;
+	int64_t added = -1;
+	pthread_mutex_lock(&m->pin_mu);
+	cmb200_pin_range *next = malloc((m->pin_n + 1) * sizeof(*next));
+	if (next && m->pin_max) {
+		memcpy(next, m->pins, m->pin_n * sizeof(*next));
+		next[m->pin_n] = (cmb200_pin_range){ nhid_small, first.l, last.l };
+		const size_t n = pin_normalize(next, m->pin_n + 1);
+		const uint64_t pages = pin_total(next, n);
+		if (n <= CMB200_PIN_RANGES && pages <= m->pin_max) {
+			added = (int64_t)(pages - m->pin_pages);
+			if (added > 0)
+				filemap_pins_install(m, next, n);
+			else
+				free(next);
+			next = NULL;
+		}
+	}
+	free(next);
+	pthread_mutex_unlock(&m->pin_mu);
+	if (added > 0)
+		filemap_pins_promote(m);
+	return added;
+}
+
+uint64_t
+cachemap_unpin(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size)
+{
+	struct filemap *m = cm->pages;
+	cmb200_addr first, last;
+	if (size == 0 || compose_span(cm, nhid_small, genid, off, size, &first, &last) != 0)
+		return 0;
+	if (!cmb200_pin_set || !filemap_engine_ready(m))
+		return 0;
+	uint64_t removed = 0;
+	pthread_mutex_lock(&m->pin_mu);
+	cmb200_pin_range *next = malloc((m->pin_n + 1) * sizeof(*next));
+	if (next) {
+		const size_t n = pin_cut(m->pins, m->pin_n, nhid_small, first.l, last.l, next, NULL, NULL);
+		removed = m->pin_pages - pin_total(next, n);
+		if (n > CMB200_PIN_RANGES) {
+			fprintf(stderr, "cachemap_b200: cachemap_unpin: the pins would need more than %d ranges; nothing "
+			    "is unpinned\n", CMB200_PIN_RANGES);
+			removed = 0;
+		} else if (removed) {
+			filemap_pins_install(m, next, n);
+			next = NULL;
+		}
+	}
+	free(next);
+	pthread_mutex_unlock(&m->pin_mu);
+	return removed;
+}
+
+void
+cachemap_pin_stats(struct cachemap *cm, uint64_t *pinned, uint64_t *in_hbm, uint64_t *in_tier)
+{
+	struct filemap *m = cm->pages;
+	uint64_t p = 0, a = 0, t = 0;
+	if (filemap_engine_ready(m)) {
+		filemap_drain(m);               /* every page accepted before the call is counted */
+		pthread_mutex_lock(&m->pin_mu);
+		p = m->pin_pages;
+		pthread_mutex_unlock(&m->pin_mu);
+		for (int i = 0; i < m->g && cmb200_pin_count && p; i++) {
+			uint64_t x = 0, y = 0;
+			if (cmb200_pin_count(m->dev[i]->eng, &x, &y) == 0) {
+				a += x;
+				t += y;
+			}
+		}
+	}
+	if (pinned)
+		*pinned = p;
+	if (in_hbm)
+		*in_hbm = a;
+	if (in_tier)
+		*in_tier = t;
 }
 
 int

@@ -273,6 +273,13 @@ struct cmb200_engine {
 	DevMem<uint32_t> d_import_slot;      // slot scratch of cmb200_import_records_dev, grown, never shrunk
 	DevMem<uint32_t> d_move_idx;         // index scratch of cmb200_move_pages (destination, then source), grown, never shrunk
 	DevMem<unsigned long long> d_removed; // records removed by cmb200_invalidate, allocated by its first call
+	// cmb200_pin_set: the pin list, 3 words per range then the CMB200_PIN_RANGES + 1 page prefix sums,
+	// allocated by the first call; and cmb200_pin_count's counters {arena, tier, cursor, unused} then a
+	// list of max_batch tier addresses (16-byte aligned), allocated by its first call
+	DevMem<unsigned long long> d_pins, d_pin_work;
+	uint32_t pin_n = 0;
+	uint64_t pin_pages = 0;
+	PinView pins() const { return PinView{d_pins, d_pins + 3 * CMB200_PIN_RANGES, pin_n}; }
 	// cmb200_rename: a slice's list and staged records, on the engine they leave and on the one they enter,
 	// grown, never shrunk (rename_mu: one rename call at a time uses them)
 	DevMem<uint8_t> d_ren_list, d_ren_bytes;
@@ -1456,7 +1463,9 @@ extern "C" int cmb200_sample(cmb200_engine *e, size_t n, const uint64_t *r, cmb2
 	for (size_t at = 0; at < n; at += e->max_batch) {
 		const uint32_t m = (uint32_t)((n - at < e->max_batch) ? n - at : e->max_batch);
 		CMB_CHECK(cudaMemcpyAsync(e->d_recoff, r + at, (size_t)m * 8, cudaMemcpyHostToDevice, e->st));
-		if (launch_sample(e->table, (const unsigned long long *)e->d_recoff.get(), m, e->d_addr, e->d_ts, e->d_status, e->st)) return -1;
+		if (launch_sample(e->table, e->pins(), (const unsigned long long *)e->d_recoff.get(), m, e->d_addr, e->d_ts,
+		        e->d_status, e->st))
+			return -1;
 		CMB_CHECK(cudaMemcpyAsync(addr_out + at, e->d_addr, (size_t)m * 16, cudaMemcpyDeviceToHost, e->st));
 		CMB_CHECK(cudaMemcpyAsync(ts_out + at, e->d_ts, (size_t)m * 8, cudaMemcpyDeviceToHost, e->st));
 		CMB_CHECK(cudaMemcpyAsync(ok_out + at, e->d_status, (size_t)m * 4, cudaMemcpyDeviceToHost, e->st));
@@ -3312,8 +3321,13 @@ static int demote_arena_all(cmb200_engine *e) {
 // array order while they fit.  Nothing is evicted, demoted or compacted to make room; the caller does
 // that first if it wants to (the drop-in's CMB200_TIER_PROMOTE).  See slot_publish in kernels.cu for
 // why readers on other streams need no get_gate.
+static int promote_locked(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *promoted_out);
 extern "C" int cmb200_promote_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *promoted_out) {
 	std::lock_guard<std::mutex> g(e->mu);
+	return promote_locked(e, n, addr, promoted_out);
+}
+// (e->mu held)
+static int promote_locked(cmb200_engine *e, size_t n, const cmb200_addr *addr, uint64_t *promoted_out) {
 	if (promoted_out) *promoted_out = 0;
 	cmb200_engine::HostTier &t = e->tier;
 	if (!t.host) { set_error_msg("cmb200_promote_batch: the engine has no host tier"); return -1; }
@@ -3355,6 +3369,95 @@ extern "C" int cmb200_promote_batch(cmb200_engine *e, size_t n, const cmb200_add
 		for (const PromoteEntry &p : plan) t.promoted_bytes += p.len;
 	}
 	if (promoted_out) *promoted_out = done;
+	return 0;
+}
+
+// ---- pinned pages ------------------------------------------------------------------------------
+// The list goes to the device under the engine lock on its stream, so every sample launched after the
+// call sees it and none launched before does.
+extern "C" int cmb200_pin_set(cmb200_engine *e, size_t n, const cmb200_pin_range *r) {
+	if (n > CMB200_PIN_RANGES) { set_error_msg("cmb200_pin_set: more than CMB200_PIN_RANGES ranges"); return -1; }
+	std::vector<unsigned long long> w(3 * n + n + 1);
+	uint64_t pages = 0;
+	for (size_t k = 0; k < n; k++) {
+		const bool after = k == 0 || r[k].u > r[k - 1].u || (r[k].u == r[k - 1].u && r[k].l_first > r[k - 1].l_last);
+		if (r[k].l_first > r[k].l_last || !after) {
+			set_error_msg("cmb200_pin_set: the ranges are not sorted and disjoint");
+			return -1;
+		}
+		w[3 * k] = r[k].u; w[3 * k + 1] = r[k].l_first; w[3 * k + 2] = r[k].l_last;
+		w[3 * n + k] = pages;
+		pages += r[k].l_last - r[k].l_first + 1;         // a range of all 2^64 values of l wraps to 0 here
+	}
+	w[4 * n] = pages;
+	std::lock_guard<std::mutex> g(e->mu);
+	if (e->multi_gpu) {
+		set_error_msg("cmb200_pin_set: not available after a multi-GPU call (the index holds other ranks' records)");
+		return -1;
+	}
+	CMB_CHECK(cudaSetDevice(e->device));
+	if (!e->d_pins && e->d_pins.alloc((4 * (size_t)CMB200_PIN_RANGES + 1) * 8)) return -1;
+	// the samples launched before read the old list: the stream orders the copies after them
+	CMB_CHECK(cudaMemcpyAsync(e->d_pins, w.data(), 3 * n * 8, cudaMemcpyHostToDevice, e->st));
+	CMB_CHECK(cudaMemcpyAsync(e->d_pins + 3 * CMB200_PIN_RANGES, w.data() + 3 * n, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	e->pin_n = (uint32_t)n;
+	e->pin_pages = pages;
+	return 0;
+}
+
+// The live local records at pinned addresses: counts {arena, tier}, and up to max_batch tier addresses
+// in list (nullable).  Keyed while the list's pages stay within cmb200_invalidate's threshold.  (e->mu held)
+static int pin_select_locked(cmb200_engine *e, uint64_t counts[2], std::vector<cmb200_addr> *list) {
+	counts[0] = counts[1] = 0;
+	if (e->pin_n == 0) return 0;
+	if (!e->d_pin_work && e->d_pin_work.alloc((4 + 2 * (size_t)e->max_batch) * 8)) return -1;
+	CMB_CHECK(cudaMemsetAsync(e->d_pin_work, 0, 3 * 8, e->st));
+	const bool keyed = e->pin_pages != 0 && e->pin_pages - 1 < invalidate_keyed_max(e->table.cap);
+	if (launch_pin_select(e->table, e->pins(), keyed ? e->pin_pages : 0, e->d_pin_work,
+	        list ? (ulonglong2 *)(e->d_pin_work + 4) : nullptr, e->d_pin_work + 2, e->max_batch, e->st))
+		return -1;
+	e->stats.kernel_launches++;
+	unsigned long long c[3];
+	CMB_CHECK(cudaMemcpyAsync(c, e->d_pin_work, sizeof(c), cudaMemcpyDeviceToHost, e->st));
+	CMB_CHECK(cudaStreamSynchronize(e->st));
+	counts[0] = c[0]; counts[1] = c[1];
+	if (list) {
+		list->resize(c[2] < e->max_batch ? c[2] : e->max_batch);
+		CMB_CHECK(cudaMemcpyAsync(list->data(), e->d_pin_work + 4, list->size() * 16, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+	}
+	return 0;
+}
+
+extern "C" int cmb200_pin_count(cmb200_engine *e, uint64_t *in_arena, uint64_t *in_tier) {
+	std::lock_guard<std::mutex> g(e->mu);
+	CMB_CHECK(cudaSetDevice(e->device));
+	uint64_t c[2];
+	if (pin_select_locked(e, c, nullptr)) return -1;
+	if (in_arena) *in_arena = c[0];
+	if (in_tier) *in_tier = c[1];
+	return 0;
+}
+
+// Each round lists up to max_batch pinned tier records and promotes them while free arena bytes hold
+// them; a round that cannot promote all it listed is the last.
+extern "C" int cmb200_pin_promote(cmb200_engine *e, uint64_t *promoted_out) {
+	std::lock_guard<std::mutex> g(e->mu);
+	if (promoted_out) *promoted_out = 0;
+	if (!e->tier.host) return 0;
+	CMB_CHECK(cudaSetDevice(e->device));
+	std::vector<cmb200_addr> list;
+	uint64_t total = 0;
+	for (;;) {
+		uint64_t c[2], got = 0;
+		if (pin_select_locked(e, c, &list)) return -1;
+		if (list.empty()) break;
+		if (promote_locked(e, list.size(), list.data(), &got)) return -1;
+		total += got;
+		if (got < list.size()) break;
+	}
+	if (promoted_out) *promoted_out = total;
 	return 0;
 }
 

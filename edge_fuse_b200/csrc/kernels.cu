@@ -434,8 +434,33 @@ __global__ void __launch_bounds__(256) k_rename_gather(TableView t, ArenaView a,
 // (a nearly empty table) is finished by k_sample_scan, one CTA per draw, 256 slots per step.
 constexpr uint32_t SAMPLE_WALK = 128, SAMPLE_REDRAWS = 8;
 __device__ __forceinline__ bool slot_live(const Slot &s) { return s.vlen != 0; }
-__global__ void k_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,
-    unsigned long long *ts_out, int32_t *ok) {
+
+// {u, l} lies in a range of the pin list: a binary search for the last range that starts at or before
+// it, through the read-only path (the list is small and every thread of a launch reads it).  -1 if none,
+// else that range's index.
+__device__ __forceinline__ int32_t pin_find(const PinView &p, unsigned long long u, unsigned long long l) {
+	uint32_t lo = 0, hi = p.n;                            // the first range that starts after {u, l}
+	while (lo < hi) {
+		const uint32_t mid = (lo + hi) >> 1;
+		const unsigned long long ru = __ldg(p.r + 3 * mid), rf = __ldg(p.r + 3 * mid + 1);
+		if (ru < u || (ru == u && rf <= l)) lo = mid + 1;
+		else hi = mid;
+	}
+	if (lo == 0) return -1;
+	const uint32_t k = lo - 1;
+	return __ldg(p.r + 3 * k) == u && l <= __ldg(p.r + 3 * k + 2) ? (int32_t)k : -1;
+}
+
+// A slot the sampler may answer: live, and (PIN) not stored at a pinned address.
+template <bool PIN>
+__device__ __forceinline__ bool slot_drawable(const Slot &s, const PinView &p) {
+	if (!slot_live(s)) return false;
+	return !PIN || pin_find(p, s.addr_u, s.addr_l) < 0;
+}
+
+template <bool PIN>
+__device__ __forceinline__ void sample_walk(const TableView &t, const PinView &p, const unsigned long long *r,
+    uint32_t n, unsigned long long *addr_out, unsigned long long *ts_out, int32_t *ok) {
 	uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
 	if (i >= n) return;
 	unsigned long long draw = r[i];
@@ -445,7 +470,7 @@ __global__ void k_sample(TableView t, const unsigned long long *r, uint32_t n, u
 		for (uint32_t k = 0; k < SAMPLE_WALK; k++) {
 			const uint64_t j = (start + k) % (t.cap + 2);
 			const Slot &s = t.slots[j];
-			if (slot_live(s)) {
+			if (slot_drawable<PIN>(s, p)) {
 				addr_out[2 * i] = s.addr_u; addr_out[2 * i + 1] = s.addr_l; ts_out[i] = s.ts;
 				found = 1;
 				break;
@@ -455,8 +480,10 @@ __global__ void k_sample(TableView t, const unsigned long long *r, uint32_t n, u
 	}
 	ok[i] = found;
 }
-__global__ void __launch_bounds__(256) k_sample_scan(TableView t, const unsigned long long *r, uint32_t n,
-    unsigned long long *addr_out, unsigned long long *ts_out, int32_t *ok) {
+
+template <bool PIN>
+__device__ __forceinline__ void sample_scan(const TableView &t, const PinView &p, const unsigned long long *r,
+    uint32_t n, unsigned long long *addr_out, unsigned long long *ts_out, int32_t *ok) {
 	__shared__ unsigned long long first;
 	for (uint32_t i = blockIdx.x; i < n; i += gridDim.x) {
 		if (ok[i] >= 0) continue;                         // uniform across the CTA
@@ -465,7 +492,7 @@ __global__ void __launch_bounds__(256) k_sample_scan(TableView t, const unsigned
 		__syncthreads();
 		for (uint64_t base = 0; base < total; base += blockDim.x) {
 			const uint64_t k = base + threadIdx.x;
-			if (k < total && slot_live(t.slots[(start + k) % total])) atomicMin(&first, (unsigned long long)k);
+			if (k < total && slot_drawable<PIN>(t.slots[(start + k) % total], p)) atomicMin(&first, (unsigned long long)k);
 			__syncthreads();
 			if (first != ~0ull) break;
 			__syncthreads();
@@ -480,6 +507,56 @@ __global__ void __launch_bounds__(256) k_sample_scan(TableView t, const unsigned
 			}
 		}
 		__syncthreads();
+	}
+}
+
+__global__ void k_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,
+    unsigned long long *ts_out, int32_t *ok) {
+	sample_walk<false>(t, PinView{}, r, n, addr_out, ts_out, ok);
+}
+__global__ void __launch_bounds__(256) k_sample_scan(TableView t, const unsigned long long *r, uint32_t n,
+    unsigned long long *addr_out, unsigned long long *ts_out, int32_t *ok) {
+	sample_scan<false>(t, PinView{}, r, n, addr_out, ts_out, ok);
+}
+__global__ void k_sample_pin(TableView t, PinView p, const unsigned long long *r, uint32_t n,
+    unsigned long long *addr_out, unsigned long long *ts_out, int32_t *ok) {
+	sample_walk<true>(t, p, r, n, addr_out, ts_out, ok);
+}
+__global__ void __launch_bounds__(256) k_sample_scan_pin(TableView t, PinView p, const unsigned long long *r,
+    uint32_t n, unsigned long long *addr_out, unsigned long long *ts_out, int32_t *ok) {
+	sample_scan<true>(t, p, r, n, addr_out, ts_out, ok);
+}
+
+// cmb200_pin_count / cmb200_pin_promote.  The selection is cmb200_invalidate's: keyed, the slot that
+// the key of {u, l} finds holds exactly that address (slot_holds) and a record; by scan, the pin range
+// that holds the slot's stored address, if any, is the interval that slot_in_scan tests.
+__global__ void __launch_bounds__(256) k_pin_select(TableView t, PinView p, bool keyed, unsigned long long *counts,
+    ulonglong2 *list, unsigned long long *cursor, uint32_t max_n) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	uint32_t idx = 0xffffffffu;
+	if (keyed) {
+		if (i < p.pre[p.n]) {
+			uint32_t lo = 0, hi = p.n;                    // the range of pinned page i: last k with pre[k] <= i
+			while (hi - lo > 1) {
+				const uint32_t mid = (lo + hi) >> 1;
+				if (__ldg(p.pre + mid) <= i) lo = mid;
+				else hi = mid;
+			}
+			const unsigned long long u = __ldg(p.r + 3 * lo), l = __ldg(p.r + 3 * lo + 1) + (i - __ldg(p.pre + lo));
+			idx = table_find(t, fnv_addr(u, l));
+			if (idx != 0xffffffffu && (!slot_holds(t.slots[idx], u, l) || t.slots[idx].vlen == 0)) idx = 0xffffffffu;
+		}
+	} else if (i < t.cap + 2) {
+		const Slot &s = t.slots[i];
+		const int32_t k = s.vlen != 0 ? pin_find(p, s.addr_u, s.addr_l) : -1;
+		if (k >= 0 && slot_in_scan(t, i, p.r[3 * k], p.r[3 * k + 1], p.r[3 * k + 2])) idx = (uint32_t)i;
+	}
+	const bool tier = idx != 0xffffffffu && (t.slots[idx].rec_off & REC_HOST);
+	count_warp(idx != 0xffffffffu && !tier, counts);
+	count_warp(tier, counts + 1);
+	if (tier && list) {
+		const unsigned long long k = atomicAdd(cursor, 1ull);
+		if (k < max_n) list[k] = make_ulonglong2(t.slots[idx].addr_u, t.slots[idx].addr_l);
 	}
 }
 
@@ -2387,12 +2464,23 @@ int launch_rehash(TableView from, TableView to, cudaStream_t st) {
 	return 0;
 }
 
-int launch_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,
+int launch_sample(TableView t, PinView p, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,
     unsigned long long *ts_out, int32_t *ok, cudaStream_t st) {
 	if (n == 0) return 0;
-	k_sample<<<GRID1D(n), 0, st>>>(t, r, n, addr_out, ts_out, ok);
+	if (p.n) k_sample_pin<<<GRID1D(n), 0, st>>>(t, p, r, n, addr_out, ts_out, ok);
+	else k_sample<<<GRID1D(n), 0, st>>>(t, r, n, addr_out, ts_out, ok);
 	CMB_CHECK(cudaGetLastError());
-	k_sample_scan<<<n < 1024u ? n : 1024u, 256, 0, st>>>(t, r, n, addr_out, ts_out, ok);
+	if (p.n) k_sample_scan_pin<<<n < 1024u ? n : 1024u, 256, 0, st>>>(t, p, r, n, addr_out, ts_out, ok);
+	else k_sample_scan<<<n < 1024u ? n : 1024u, 256, 0, st>>>(t, r, n, addr_out, ts_out, ok);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+int launch_pin_select(TableView t, PinView p, uint64_t keyed_pages, unsigned long long *counts, ulonglong2 *list,
+    unsigned long long *cursor, uint32_t max_n, cudaStream_t st) {
+	if (p.n == 0) return 0;
+	const uint64_t threads = keyed_pages ? keyed_pages : t.cap + 2;
+	k_pin_select<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(t, p, keyed_pages != 0, counts, list, cursor, max_n);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

@@ -280,9 +280,26 @@ int launch_rename_select(TableView t, const RenameList &r, unsigned long long u_
 int launch_rename_gather(TableView t, ArenaView a, const uint8_t *host, const RenameList &r, uint32_t n, uint8_t *stage,
     cudaStream_t st);
 
-// Policy-equivalent of filemap_get_rand (filemap.c:264-314): first live slot at or after r.
-int launch_sample(TableView t, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,
+// cmb200_pin_set's list on the device: range k is {u, l_first, l_last} = r[3k .. 3k+2], sorted by
+// (u, l_first) and disjoint; pre[k] = the pages of ranges 0 .. k-1, pre[n] = all of them.
+struct PinView {
+	const unsigned long long *r;
+	const unsigned long long *pre;
+	uint32_t n;
+};
+
+// Policy-equivalent of filemap_get_rand (filemap.c:264-314): first live slot at or after r.  With a
+// non-empty pin list, the first live slot whose stored address is not pinned (k_sample_pin /
+// k_sample_scan_pin); with an empty one, k_sample / k_sample_scan.
+int launch_sample(TableView t, PinView p, const unsigned long long *r, uint32_t n, unsigned long long *addr_out,
     unsigned long long *ts_out, int32_t *ok, cudaStream_t st);
+
+// cmb200_pin_count / cmb200_pin_promote: the live local records stored at a pinned address.  keyed_pages
+// = p.pre[p.n] > 0: one thread per pinned page, looked up as k_invalidate_keys looks up; 0: one thread
+// per slot, as k_invalidate_scan.  counts[0] += those in the arena, counts[1] += those in the host tier;
+// the addresses of the tier ones go to list[cursor[0]++] while cursor[0] < max_n (list nullable).
+int launch_pin_select(TableView t, PinView p, uint64_t keyed_pages, unsigned long long *counts, ulonglong2 *list,
+    unsigned long long *cursor, uint32_t max_n, cudaStream_t st);
 
 int launch_read_fp(TableView t, const unsigned long long *addr, uint32_t n, uint64_t *fp_out, int32_t *ok,
     cudaStream_t st);

@@ -159,6 +159,35 @@ uint64_t cachemap_invalidate(struct cachemap *cm, uint64_t nhid_small, uint32_t 
  */
 uint64_t cachemap_rename(struct cachemap *cm, uint64_t nhid_from, uint64_t nhid_to, uint32_t genid);
 
+/*
+ * Pins.  A pinned page is never evicted (by count or by arena bytes), never paired as a victim by
+ * admission and never demoted to the host tier: every victim the map draws comes from a sampler that
+ * passes over pinned pages (cmb200_sample).  Under CMB200_ADMIT=freq a put of a pinned page is always
+ * admitted.  A pin names stored addresses {nhid_small, genid << 44 | page}, as cachemap_invalidate does,
+ * not keys: another object's page that shares a page's key is not pinned.  It holds whether the page is
+ * cached now or put later.  A pinned page still leaves when it is unset, invalidated, renamed away or
+ * over, and when a put or a patch of it finds no arena room, which happens only when pinned pages fill
+ * the arena, or when a background load (which never evicts) finds no room for it.
+ * Pins the pages of object (nhid_small, genid) that overlap bytes [off, off + size), partial pages at
+ * both ends included.  Returns the pages newly pinned (already pinned ones are not counted again), or -1,
+ * pinning nothing, when size is 0 or CACHEMAP_TO_END, when the first page does not fit 44 bits, when the
+ * map's pinned pages would exceed CMB200_PIN_MAX, or when the pins would need more than CMB200_PIN_RANGES
+ * disjoint ranges.  CMB200_PIN_MAX counts pages over the whole map: capacity / 4 by default, at most
+ * capacity / 2 (a larger value warns and is clamped), 0 = no pins.  Pinned records already in the host
+ * tier go back to HBM as far as free arena bytes hold them; the rest stay in the tier, counted in
+ * *in_tier, where a lap of the tier's ring may retire them before a later pin call moves them.
+ * Pins survive a restart in destdir/cachemap_b200.pins (sealed under CMB200_KEY_FILE; nothing is read or
+ * written with CMB200_PERSIST=0), read before any snapshot record is loaded.  cachemap_invalidate leaves
+ * pins alone, so a truncated file that is written again stays pinned; cachemap_rename drops the pins of
+ * `to` and moves those of `from` to `to` before it moves the pages.
+ */
+int64_t cachemap_pin(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size);
+/* Unpins the pages overlapping [off, off + size); CACHEMAP_TO_END is allowed.  Returns the pages
+ * unpinned; 0, unpinning nothing, when the pins would need more than CMB200_PIN_RANGES ranges. */
+uint64_t cachemap_unpin(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size);
+/* pinned = pages named by pins; in_hbm / in_tier = pinned pages cached in the arena / the host tier. */
+void cachemap_pin_stats(struct cachemap *cm, uint64_t *pinned, uint64_t *in_hbm, uint64_t *in_tier);
+
 /* requests / hits counters (cachemap.c:176,181) and the engine under the map. */
 void cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hits);
 /* CMB200_ADMIT=freq: pages admitted over the victim they were paired with, and pages rejected (not stored,

@@ -238,8 +238,30 @@ int cmb200_rename(cmb200_engine *e, uint64_t u_from, uint64_t u_to, uint64_t l_f
 int cmb200_patch_batch(cmb200_engine *e, size_t n, const cmb200_addr *addr, const uint32_t *page_off,
     const uint32_t *len, const void *bytes_host, const uint64_t *ts, int32_t *status_out);
 uint64_t cmb200_entries(cmb200_engine *e);
+/* filemap_get_rand's sampler: for draw r[i], the first live record at or after slot r[i] whose stored
+ * address is not pinned (cmb200_pin_set), within a bounded walk and a few redraws, else by a scan of the
+ * whole table.  ok_out[i] = 1 with its address and ts, or 0 when every live record is pinned or there is
+ * none.  Eviction, admission and demotion in the drop-in all draw their victims here, so they inherit the
+ * filter.  With no pins the launch is the unfiltered sampler's. */
 int cmb200_sample(cmb200_engine *e, size_t n, const uint64_t *r, cmb200_addr *addr_out,
     uint64_t *ts_out, int32_t *ok_out);
+
+/* ---- pinned pages ------------------------------------------------------------------------------
+ * A pin names stored addresses {u, l}, l_first <= l <= l_last, whether a record is stored there or not.
+ * cmb200_pin_set replaces the engine's list with n ranges sorted by (u, l_first) and disjoint (else -1,
+ * as on an engine that has made a multi-GPU call, and for n > CMB200_PIN_RANGES); n = 0 clears it.
+ * cmb200_sample never answers a pinned record.
+ * cmb200_pin_count: the live local records at pinned addresses, in the arena and in the host tier.  The
+ * list is walked page by page while its pages stay within cmb200_invalidate's threshold, else the table
+ * is scanned once.
+ * cmb200_pin_promote: moves pinned records of the host tier back to free arena bytes, as
+ * cmb200_promote_batch does, until they are all in the arena or the next one does not fit; *promoted_out
+ * = records moved.  0 on an engine without a tier. */
+#define CMB200_PIN_RANGES 4096
+typedef struct cmb200_pin_range { uint64_t u, l_first, l_last; } cmb200_pin_range;
+int cmb200_pin_set(cmb200_engine *e, size_t n, const cmb200_pin_range *r);
+int cmb200_pin_count(cmb200_engine *e, uint64_t *in_arena, uint64_t *in_tier);
+int cmb200_pin_promote(cmb200_engine *e, uint64_t *promoted_out);
 
 /* Copies the stored record of each address — the bytes the reference keeps in LMDB:
  * 24-byte data_prefix + payload (filemap.c:9-12,140-147) — into out (stride bytes apart) and its
