@@ -11,5 +11,5 @@ from .binding import (  # noqa: F401
     HIT, MISS, INVALID, BAD_ENTRY, BAD_DECODE, REMOTE, FINGERPRINT, EXPORTED_SYMBOLS, engine_stats,
     host_tier_stats, read_checkpoints, VERIFY, CORRUPT, verify_stats, owner, save_set, load_set,
     snapshot_begin, snapshot_finish, chain_begin, load_chain, TOUCH, DROPPED, rename_set, FREQ, freq_index,
-    Loader, aead_seal_batch, aead_open_batch, GHOST, ghost_set,
+    Loader, aead_seal_batch, aead_open_batch, GHOST, ghost_set, usage_set, USAGE_DTYPE, IN_HBM, IN_TIER, PINNED,
 )

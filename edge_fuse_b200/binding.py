@@ -26,6 +26,7 @@ EXPORTED_SYMBOLS = [
     "cachemap_read_range", "cachemap_write_range", "cachemap_checkpoint", "cachemap_invalidate",
     "cachemap_pread", "cachemap_pwrite", "cachemap_rename", "cachemap_get_admission",
     "cachemap_load_progress", "cachemap_hit_curve", "cachemap_pin", "cachemap_unpin", "cachemap_pin_stats",
+    "cachemap_residency", "cachemap_usage",
     # filemap.h — reference cachemap/filemap.h:19-29
     "filemap_create", "filemap_free", "filemap_set", "filemap_unset", "filemap_get",
     "filemap_get_rand", "filemap_entries",
@@ -51,7 +52,18 @@ EXPORTED_SYMBOLS = [
     "cmb200_freq_stats", "cmb200_load_open", "cmb200_load_step", "cmb200_load_total", "cmb200_load_close",
     "cmb200_set_file_key", "cmb200_load_rejected", "cmb200_aead_seal_batch", "cmb200_aead_open_batch",
     "cmb200_ghost_set", "cmb200_evict_batch", "cmb200_ghost_stats", "cmb200_ghost_read",
+    "cmb200_residency", "cmb200_usage_set",
 ]
+
+
+# cmb200_object_usage / struct cachemap_object_usage, one row per object
+USAGE_DTYPE = np.dtype([("nhid", "<u8"), ("genid", "<u4"), ("reserved", "<u4"), ("pages", "<u8"),
+                        ("tier_pages", "<u8"), ("pinned_pages", "<u8"), ("stored_bytes", "<u8"),
+                        ("first_page", "<u8"), ("last_page", "<u8"), ("oldest_ts", "<u8"), ("newest_ts", "<u8")])
+assert USAGE_DTYPE.itemsize == 80
+
+# cachemap_residency's bits
+IN_HBM, IN_TIER, PINNED = 1, 2, 4
 
 
 class Config(C.Structure):
@@ -127,6 +139,8 @@ def lib() -> C.CDLL:
         "cachemap_pin": (C.c_int64, [vp, u64, u32, u64, u64]),
         "cachemap_unpin": (u64, [vp, u64, u32, u64, u64]),
         "cachemap_pin_stats": (None, [vp, vp, vp, vp]),
+        "cachemap_residency": (C.c_int64, [vp, u64, u32, u64, u64, vp]),
+        "cachemap_usage": (C.c_int64, [vp, sz, vp]),
         "cachemap_read_range": (i32, [vp, u64, u32, u64, sz, vp]),
         "cachemap_write_range": (None, [vp, u64, u32, u64, sz, vp]),
         "cachemap_pread": (i32, [vp, u64, u32, u64, sz, vp]),
@@ -171,6 +185,8 @@ def lib() -> C.CDLL:
         "cmb200_pin_set": (i32, [vp, sz, vp]),
         "cmb200_pin_count": (i32, [vp, vp, vp]),
         "cmb200_pin_promote": (i32, [vp, vp]),
+        "cmb200_residency": (i32, [vp, u64, u64, u64, vp]),
+        "cmb200_usage_set": (i32, [vp, i32, sz, vp, vp]),
         "cmb200_read_records": (i32, [vp, sz, vp, vp, sz, vp]),
         "cmb200_read_fingerprints": (i32, [vp, sz, vp, vp, vp]),
         "cmb200_get_stats": (i32, [vp, vp]),
@@ -673,6 +689,17 @@ class Engine:
         _check(lib().cmb200_pin_promote(self.h, C.byref(n)), "cmb200_pin_promote")
         return n.value
 
+    def residency(self, u: int, l_first: int, l_last: int) -> np.ndarray:
+        """cmb200_residency -> uint8 [l_last - l_first + 1]: 1 = the record of {u, l_first + i} is in the
+        arena, 2 = in the host tier, 0 = no live local record."""
+        out = np.zeros(l_last - l_first + 1, dtype=np.uint8)
+        _check(lib().cmb200_residency(self.h, u, l_first, l_last, _ptr(out)), "cmb200_residency")
+        return out
+
+    def usage(self, max_rows: int = 1 << 16) -> np.ndarray:
+        """cmb200_usage_set over this engine alone (usage_set)."""
+        return usage_set([self.h], max_rows)[1]
+
     def read_records_raw(self, u, l):
         """-> (records [n, 24 + bsize + 1024] uint8, lens [n] int32; -1 = no record): the stored
         filemap records {data_prefix, payload} as they lie in the arena."""
@@ -818,6 +845,16 @@ def rename_set(handles, u_from: int, u_to: int, l_first: int, l_last: int):
     _check(lib().cmb200_rename_set(arr, g, u_from, u_to, l_first, l_last, C.byref(moved), C.byref(dropped)),
            "cmb200_rename_set")
     return moved.value, dropped.value
+
+
+def usage_set(handles, max_rows: int):
+    """cmb200_usage_set over engine handles -> (objects, rows): rows is a USAGE_DTYPE array of the first
+    min(max_rows, objects) objects, stored_bytes descending, then nhid, then genid."""
+    arr, g = _handles(handles)
+    out = np.zeros(max(max_rows, 1), dtype=USAGE_DTYPE)
+    n = C.c_uint64(0)
+    _check(lib().cmb200_usage_set(arr, g, max_rows, _ptr(out), C.byref(n)), "cmb200_usage_set")
+    return n.value, out[:min(max_rows, n.value)]
 
 
 def snapshot_begin(handles, path: str) -> int:
@@ -1001,6 +1038,22 @@ class Cachemap:
         p, a, t = C.c_uint64(), C.c_uint64(), C.c_uint64()
         lib().cachemap_pin_stats(self.h, C.byref(p), C.byref(a), C.byref(t))
         return p.value, a.value, t.value
+
+    def residency(self, nhid: int, genid: int, off: int, size: int):
+        """cachemap_residency -> (pages cached, uint8 vector of IN_HBM / IN_TIER | PINNED per page), or
+        (-1, None) when refused."""
+        last = off + size - 1
+        ok = 0 < size < (1 << 64) - 1 and last < 1 << 64 and (last >> self.pshift) < 1 << 44
+        n = (last >> self.pshift) - (off >> self.pshift) + 1 if ok else 1      # a refusal writes nothing
+        vec = np.zeros(n, dtype=np.uint8)
+        rc = int(lib().cachemap_residency(self.h, nhid, genid, off, size, _ptr(vec)))
+        return (rc, vec) if rc >= 0 else (-1, None)
+
+    def usage(self, max_rows: int = 1 << 16):
+        """cachemap_usage -> (objects, USAGE_DTYPE rows of the first min(max_rows, objects)), or (-1, None)."""
+        out = np.zeros(max(max_rows, 1), dtype=USAGE_DTYPE)
+        rc = int(lib().cachemap_usage(self.h, max_rows, _ptr(out)))
+        return (rc, out[:min(max_rows, rc)]) if rc >= 0 else (-1, None)
 
     def counters(self):
         rq, ht = C.c_uint64(), C.c_uint64()

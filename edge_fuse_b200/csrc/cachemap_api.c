@@ -32,6 +32,7 @@
 #include <dirent.h>
 #include <errno.h>
 #include <pthread.h>
+#include <stddef.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -85,6 +86,8 @@ extern uint32_t cmb200_ghost_set(uint64_t key, int log2_sets);
 #pragma weak cmb200_pin_set
 #pragma weak cmb200_pin_count
 #pragma weak cmb200_pin_promote
+#pragma weak cmb200_residency
+#pragma weak cmb200_usage_set
 #pragma weak cmb200_aead_seal_batch
 
 #define COMBINE_MAX 32          /* get/unset requests one leader takes per GPU batch */
@@ -3262,6 +3265,72 @@ cachemap_pin_stats(struct cachemap *cm, uint64_t *pinned, uint64_t *in_hbm, uint
 		*in_hbm = a;
 	if (in_tier)
 		*in_tier = t;
+}
+
+_Static_assert(sizeof(struct cachemap_object_usage) == sizeof(cmb200_object_usage) &&
+    offsetof(struct cachemap_object_usage, genid) == offsetof(cmb200_object_usage, genid) &&
+    offsetof(struct cachemap_object_usage, pages) == offsetof(cmb200_object_usage, pages) &&
+    offsetof(struct cachemap_object_usage, stored_bytes) == offsetof(cmb200_object_usage, stored_bytes) &&
+    offsetof(struct cachemap_object_usage, newest_ts) == offsetof(cmb200_object_usage, newest_ts),
+    "struct cachemap_object_usage is cmb200_object_usage");
+
+int64_t
+cachemap_residency(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size,
+    uint8_t *vec)
+{
+	struct filemap *m = cm->pages;
+	cmb200_addr first, last;
+	if (size == 0 || size == CACHEMAP_TO_END || size - 1 > UINT64_MAX - off)
+		return -1;
+	if (compose_addr(cm, off, nhid_small, genid, &first) != 0 ||
+	    compose_addr(cm, off + (size - 1), nhid_small, genid, &last) != 0)
+		return -1;
+	/* a call before the first get answers for the loaded snapshot, not before it */
+	if (!cmb200_residency || !filemap_engine_ready(m))
+		return -1;
+	filemap_drain(m);                       /* every page accepted before the call is in a store */
+	const uint64_t n = last.l - first.l + 1;
+	uint8_t *v = calloc(n, 1);              /* vec stays untouched unless every engine answers */
+	if (!v)
+		return -1;
+	for (int i = 0; i < m->g; i++)          /* the object's pages are spread over the engines by key */
+		if (cmb200_residency(m->dev[i]->eng, nhid_small, first.l, last.l, v) != 0) {
+			fprintf(stderr, "cachemap_b200: cachemap_residency: %s\n", cmb200_last_error());
+			free(v);
+			return -1;
+		}
+	int64_t cached = 0;
+	for (uint64_t k = 0; k < n; k++)
+		cached += v[k] != 0;
+	pthread_mutex_lock(&m->pin_mu);
+	for (size_t k = 0; k < m->pin_n; k++) {
+		const cmb200_pin_range *r = &m->pins[k];
+		if (r->u != nhid_small || r->l_last < first.l || r->l_first > last.l)
+			continue;
+		const uint64_t a = r->l_first > first.l ? r->l_first : first.l, b = r->l_last < last.l ? r->l_last : last.l;
+		for (uint64_t l = a; l <= b; l++)
+			v[l - first.l] |= CACHEMAP_PINNED;
+	}
+	pthread_mutex_unlock(&m->pin_mu);
+	memcpy(vec, v, n);
+	free(v);
+	return cached;
+}
+
+int64_t
+cachemap_usage(struct cachemap *cm, size_t max, struct cachemap_object_usage *out)
+{
+	struct filemap *m = cm->pages;
+	/* a call before the first get answers for the loaded snapshot, not before it */
+	if (!cmb200_usage_set || !filemap_engine_ready(m))
+		return -1;
+	filemap_drain(m);                       /* every page accepted before the call is counted */
+	uint64_t objects = 0;
+	if (cmb200_usage_set(m->engs, m->g, max, (cmb200_object_usage *)out, &objects) != 0) {
+		fprintf(stderr, "cachemap_b200: cachemap_usage: %s\n", cmb200_last_error());
+		return -1;
+	}
+	return (int64_t)objects;
 }
 
 int

@@ -3461,6 +3461,178 @@ extern "C" int cmb200_pin_promote(cmb200_engine *e, uint64_t *promoted_out) {
 	return 0;
 }
 
+// ---- usage and residency ----------------------------------------------------------------------
+// Read-only scans of the table under the engine lock, on its stream (DESIGN.md §2, *Usage and
+// residency*).  Their scratch is allocated per call and freed before it returns, and they move no
+// counter, not even kernel_launches, so that cmb200_get_stats reads the same before and after.
+static_assert(sizeof(cmb200_object_usage) == sizeof(UsageRow), "cmb200_object_usage is UsageRow");
+static_assert(offsetof(cmb200_object_usage, genid) == offsetof(UsageRow, genid) &&
+    offsetof(cmb200_object_usage, stored_bytes) == offsetof(UsageRow, stored_bytes) &&
+    offsetof(cmb200_object_usage, newest_ts) == offsetof(UsageRow, newest_ts), "cmb200_object_usage is UsageRow");
+
+// Scratch of one cmb200_usage_set call from the device's stream-ordered pool.  cudaFree synchronises the
+// whole device, which would stall the small gets running on other streams for the length of a usage call;
+// cudaFreeAsync only returns the bytes on the stream, and the stream synchronise that ends the call gives
+// them back to the device (the pool keeps none).  Mapping the pool's memory costs about 0.3 ms a call
+// (DESIGN.md §2, *Usage and residency*), so cmb200_residency, whose list is small, allocates plainly.
+template <class T>
+struct StreamMem {
+	T *p = nullptr;
+	cudaStream_t st = nullptr;
+	StreamMem() = default;
+	StreamMem(StreamMem &&o) noexcept : p(o.p), st(o.st) { o.p = nullptr; }
+	StreamMem &operator=(StreamMem &&o) noexcept {
+		if (this != &o) { reset(); p = o.p; st = o.st; o.p = nullptr; }
+		return *this;
+	}
+	~StreamMem() { reset(); }
+	int alloc(size_t bytes, cudaStream_t s) {
+		reset();
+		st = s;
+		CMB_CHECK(cudaMallocAsync((void **)&p, bytes, s));
+		return 0;
+	}
+	void reset() {
+		if (p) cudaFreeAsync(p, st);
+		p = nullptr;
+	}
+	operator T *() const { return p; }
+};
+
+static bool usage_refused(cmb200_engine *e, const char *what) {
+	if (!e->multi_gpu) return false;
+	char msg[160];
+	snprintf(msg, sizeof(msg), "%s: not available after a multi-GPU call (the index holds other ranks' records)", what);
+	set_error_msg(msg);
+	return true;
+}
+
+constexpr uint64_t RESIDENCY_LIST = 4096;
+
+extern "C" int cmb200_residency(cmb200_engine *e, uint64_t u, uint64_t l_first, uint64_t l_last, uint8_t *out) {
+	if (l_first > l_last) { set_error_msg("cmb200_residency: l_first > l_last"); return -1; }
+	std::lock_guard<std::mutex> g(e->mu);
+	if (usage_refused(e, "cmb200_residency")) return -1;
+	CMB_CHECK(cudaSetDevice(e->device));
+	// l_last - l_first + 1 overflows for the full interval: compare the difference instead
+	const bool scan = l_last - l_first >= invalidate_keyed_max(e->table.cap);
+	// the list holds the records found: a first pass lists up to 4096 of them, and when it found more, a
+	// second pass lists them all into a list of exactly that size
+	uint64_t max_n = l_last - l_first < RESIDENCY_LIST ? l_last - l_first + 1 : RESIDENCY_LIST;
+	for (;;) {
+		// the hit list is small and the call short: a plain allocation costs less than the pool's mapping
+		DevMem<unsigned long long> d;
+		if (d.alloc(16 + 16 * max_n)) return -1;
+		CMB_CHECK(cudaMemsetAsync(d, 0, 8, e->st));
+		ulonglong2 *hits = (ulonglong2 *)(d + 2);
+		if (launch_residency(e->table, u, l_first, l_last, scan, hits, d, max_n, e->st)) return -1;
+		unsigned long long found = 0;
+		CMB_CHECK(cudaMemcpyAsync(&found, d, 8, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		if (found > max_n) { max_n = found; continue; }
+		std::vector<ulonglong2> h(found);
+		if (found) CMB_CHECK(cudaMemcpyAsync(h.data(), hits, found * 16, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		for (const ulonglong2 &x : h) out[x.x - l_first] = (uint8_t)x.y;
+		return 0;
+	}
+}
+
+// Engine e's rows, sorted by (u, genid), into rows (reallocated) and *n_rows.  (e->mu held)
+static int usage_rows_locked(cmb200_engine *e, StreamMem<UsageRow> &rows, uint64_t *n_rows) {
+	unsigned long long c[8];
+	if (read_counters(e, c)) return -1;
+	uint64_t max_n = c[0] + 16;
+	for (;;) {
+		StreamMem<UsageRec> recs;
+		StreamMem<unsigned long long> word;
+		if (recs.alloc(max_n * sizeof(UsageRec), e->st) || word.alloc(16, e->st)) return -1;
+		CMB_CHECK(cudaMemsetAsync(word, 0, 16, e->st));
+		if (launch_usage_list(e->table, e->pins(), e->bsize, recs, word, max_n, e->st)) return -1;
+		unsigned long long found = 0;
+		CMB_CHECK(cudaMemcpyAsync(&found, word, 8, cudaMemcpyDeviceToHost, e->st));
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		if (found > max_n) { max_n = found; continue; }
+		if (found >= 0x80000000ull) { set_error_msg("cmb200_usage_set: too many records"); return -1; }
+		StreamMem<uint8_t> scratch;
+		if (rows.alloc((found ? found : 1) * sizeof(UsageRow), e->st) || scratch.alloc(usage_group_bytes(found) + 256, e->st))
+			return -1;
+		if (launch_usage_group(recs, nullptr, (uint32_t)found, rows, word + 1, scratch, e->st)) return -1;
+		unsigned long long r = 0;
+		CMB_CHECK(cudaMemcpyAsync(&r, word + 1, 8, cudaMemcpyDeviceToHost, e->st));
+		scratch.reset();
+		recs.reset();
+		word.reset();
+		CMB_CHECK(cudaStreamSynchronize(e->st));
+		*n_rows = r;
+		return 0;
+	}
+}
+
+extern "C" int cmb200_usage_set(cmb200_engine *const *engines, int g, size_t max, cmb200_object_usage *out,
+    uint64_t *objects_out) {
+	if (objects_out) *objects_out = 0;
+	if (!engines || g < 1) { set_error_msg("cmb200_usage_set: no engines"); return -1; }
+	for (int i = 0; i < g; i++) {
+		std::lock_guard<std::mutex> lk(engines[i]->mu);
+		if (usage_refused(engines[i], "cmb200_usage_set")) return -1;
+	}
+	cmb200_engine *e0 = engines[0];
+	// each engine's rows, under its own lock; then they cross to the first engine and group again there
+	std::vector<StreamMem<UsageRow>> rows(g);
+	std::vector<uint64_t> n(g, 0);
+	uint64_t total = 0;
+	for (int i = 0; i < g; i++) {
+		std::lock_guard<std::mutex> lk(engines[i]->mu);
+		if (usage_refused(engines[i], "cmb200_usage_set")) return -1;
+		CMB_CHECK(cudaSetDevice(engines[i]->device));
+		if (usage_rows_locked(engines[i], rows[i], &n[i])) return -1;
+		total += n[i];
+	}
+	if (total >= 0x80000000ull) { set_error_msg("cmb200_usage_set: too many objects"); return -1; }
+	StreamMem<UsageRow> merged;
+	if (g > 1) {
+		CMB_CHECK(cudaSetDevice(e0->device));
+		if (merged.alloc((total ? total : 1) * sizeof(UsageRow), e0->st)) return -1;
+		CMB_CHECK(cudaStreamSynchronize(e0->st));       // the copies below run on the source engines' streams
+		uint64_t at = 0;
+		for (int i = 0; i < g; i++) {
+			if (cmb200_copy_peer(e0, merged + at, engines[i], rows[i], n[i] * sizeof(UsageRow))) return -1;
+			at += n[i];
+			CMB_CHECK(cudaSetDevice(engines[i]->device));
+			rows[i].reset();
+			CMB_CHECK(cudaStreamSynchronize(engines[i]->st));
+		}
+	}
+	std::lock_guard<std::mutex> lk(e0->mu);
+	CMB_CHECK(cudaSetDevice(e0->device));
+	uint64_t objects = n[0];
+	const UsageRow *final_rows = g > 1 ? (const UsageRow *)merged : (const UsageRow *)rows[0];
+	StreamMem<uint8_t> scratch;
+	StreamMem<UsageRow> grouped, d_out;
+	if (scratch.alloc(usage_group_bytes(total) + 256, e0->st)) return -1;
+	if (g > 1) {
+		StreamMem<unsigned long long> word;
+		if (grouped.alloc((total ? total : 1) * sizeof(UsageRow), e0->st) || word.alloc(8, e0->st)) return -1;
+		if (launch_usage_group(nullptr, merged, (uint32_t)total, grouped, word, scratch, e0->st)) return -1;
+		unsigned long long r = 0;
+		CMB_CHECK(cudaMemcpyAsync(&r, word, 8, cudaMemcpyDeviceToHost, e0->st));
+		CMB_CHECK(cudaStreamSynchronize(e0->st));
+		objects = r;
+		final_rows = grouped;
+	}
+	const uint32_t take = (uint32_t)(max < objects ? max : objects);
+	if (take) {
+		if (d_out.alloc(take * sizeof(UsageRow), e0->st)) return -1;
+		if (launch_usage_order(final_rows, (uint32_t)objects, d_out, take, scratch, e0->st)) return -1;
+		CMB_CHECK(cudaMemcpyAsync(out, d_out, take * sizeof(UsageRow), cudaMemcpyDeviceToHost, e0->st));
+	}
+	d_out.reset(); scratch.reset(); grouped.reset(); merged.reset(); rows[0].reset();
+	CMB_CHECK(cudaStreamSynchronize(e0->st));
+	if (objects_out) *objects_out = objects;
+	return 0;
+}
+
 // The hot log is read while gets go on appending to it, without the lock that puts take.  An entry
 // read half-written, or one overwritten by a later lap, yields an address that is wrong or stale;
 // that is harmless, since cmb200_promote_batch looks every address up again and checks its record.

@@ -18,6 +18,9 @@
 #include "streamgen.cuh"
 #include "aead.cuh"
 #include <cub/block/block_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
+#include <algorithm>
 
 namespace cmb {
 
@@ -2481,6 +2484,266 @@ int launch_pin_select(TableView t, PinView p, uint64_t keyed_pages, unsigned lon
 	if (p.n == 0) return 0;
 	const uint64_t threads = keyed_pages ? keyed_pages : t.cap + 2;
 	k_pin_select<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(t, p, keyed_pages != 0, counts, list, cursor, max_n);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+// ---- usage and residency ----------------------------------------------------------------------
+// Read-only: nothing here writes a slot, a counter, the sketch, a ghost or a stamp.
+
+// A warp's threads with `want` set take consecutive entries of a list with one atomicAdd on *cursor, as
+// k_rename_select reserves them.  Returns this thread's entry (meaningless without want).  Every thread
+// of the warp calls it.
+__device__ __forceinline__ unsigned long long warp_reserve(bool want, unsigned long long *cursor) {
+	const int lane = threadIdx.x & 31;
+	const unsigned m = __ballot_sync(0xffffffffu, want);
+	if (!m) return 0;
+	const int leader = __ffs(m) - 1;
+	unsigned long long c = 0;
+	if (lane == leader) c = atomicAdd(cursor, (unsigned long long)__popc(m));
+	c = __shfl_sync(0xffffffffu, c, leader);
+	return c + __popc(m & ((1u << lane) - 1u));
+}
+
+// Residency, keyed: one thread per l of the interval; the key's slot must store exactly {u, l}, locally,
+// with a record.
+__global__ void __launch_bounds__(256) k_residency_keys(TableView t, unsigned long long u, unsigned long long l_first,
+    uint64_t n, ulonglong2 *hits, unsigned long long *cursor, uint64_t max_n) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	uint32_t idx = 0xffffffffu;
+	const unsigned long long l = l_first + i;
+	if (i < n) {
+		idx = table_find(t, fnv_addr(u, l));
+		if (idx != 0xffffffffu && (!slot_holds(t.slots[idx], u, l) || t.slots[idx].vlen == 0)) idx = 0xffffffffu;
+	}
+	const bool want = idx != 0xffffffffu;
+	const unsigned long long k = warp_reserve(want, cursor);
+	if (want && k < max_n) hits[k] = make_ulonglong2(l, (t.slots[idx].rec_off & REC_HOST) ? 2ull : 1ull);
+}
+
+// Residency by scan: one thread per slot (cap + 2 of them), slot_in_scan's selection.
+__global__ void __launch_bounds__(256) k_residency_scan(TableView t, unsigned long long u, unsigned long long l_first,
+    unsigned long long l_last, ulonglong2 *hits, unsigned long long *cursor, uint64_t max_n) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	const bool want = i < t.cap + 2 && slot_in_scan(t, i, u, l_first, l_last);
+	const unsigned long long k = warp_reserve(want, cursor);
+	if (want && k < max_n) {
+		const Slot &s = t.slots[i];
+		hits[k] = make_ulonglong2(s.addr_l, (s.rec_off & REC_HOST) ? 2ull : 1ull);
+	}
+}
+
+// One thread per slot: every live local record, listed.  The slot is read in 16-byte streaming loads
+// ({key, addr_u} first, as slot_in_scan reads it; the rest only for a slot in use), so that a scan of a
+// large table does not push the encoder's and the small gets' lines out of L2.
+__global__ void __launch_bounds__(256) k_usage_list(TableView t, PinView p, uint32_t bsize, UsageRec *recs,
+    unsigned long long *cursor, uint64_t max_n) {
+	const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+	bool want = false;
+	UsageRec r{};
+	if (i < t.cap + 2) {
+		const ulonglong2 *w = reinterpret_cast<const ulonglong2 *>(t.slots + i);
+		const ulonglong2 ku = __ldcs(w);
+		if (i >= t.cap || (ku.x != KEY_EMPTY && ku.x != KEY_TOMB)) {
+			const ulonglong2 lo = __ldcs(w + 1), vt = __ldcs(w + 2), so = __ldcs(w + 3);
+			const uint32_t vlen = (uint32_t)vt.x;
+			if (vlen != 0 && so.y == 0) {
+				want = true;
+				r.u = ku.y; r.l = lo.x; r.ts = vt.y;
+				r.len = 24u + (vlen > 1u ? vlen - 1u : bsize);
+				r.flags = ((lo.y & REC_HOST) ? USAGE_TIER : 0u) | (p.n && pin_find(p, ku.y, lo.x) >= 0 ? USAGE_PINNED : 0u);
+			}
+		}
+	}
+	const unsigned long long k = warp_reserve(want, cursor);
+	if (want && k < max_n) recs[k] = r;
+}
+
+// Item i of a grouping: a record (one page) or a row.
+__device__ __forceinline__ unsigned long long usage_u(const UsageRec *recs, const UsageRow *rows, uint32_t i) {
+	return recs ? recs[i].u : rows[i].u;
+}
+__device__ __forceinline__ uint32_t usage_genid(const UsageRec *recs, const UsageRow *rows, uint32_t i) {
+	return recs ? (uint32_t)(recs[i].l >> 44) : rows[i].genid;
+}
+__device__ __forceinline__ UsageRow usage_item(const UsageRec *recs, const UsageRow *rows, uint32_t i) {
+	if (!recs) return rows[i];
+	const UsageRec r = recs[i];
+	UsageRow o;
+	o.u = r.u; o.genid = (uint32_t)(r.l >> 44); o.reserved = 0;
+	o.pages = 1; o.tier_pages = (r.flags & USAGE_TIER) ? 1 : 0; o.pinned_pages = (r.flags & USAGE_PINNED) ? 1 : 0;
+	o.stored_bytes = r.len;
+	o.first_page = o.last_page = r.l & ((1ull << 44) - 1);
+	o.oldest_ts = o.newest_ts = r.ts;
+	return o;
+}
+__device__ __forceinline__ void usage_fold_into(UsageRow &a, const UsageRow &b) {
+	a.pages += b.pages; a.tier_pages += b.tier_pages; a.pinned_pages += b.pinned_pages; a.stored_bytes += b.stored_bytes;
+	a.first_page = min(a.first_page, b.first_page); a.last_page = max(a.last_page, b.last_page);
+	a.oldest_ts = min(a.oldest_ts, b.oldest_ts); a.newest_ts = max(a.newest_ts, b.newest_ts);
+}
+
+__global__ void k_usage_gkeys(const UsageRec *recs, const UsageRow *rows, uint32_t n, uint32_t *gkey, uint32_t *idx) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	gkey[i] = usage_genid(recs, rows, i);
+	idx[i] = i;
+}
+__global__ void k_usage_ukeys(const UsageRec *recs, const UsageRow *rows, uint32_t n, const uint32_t *idx,
+    unsigned long long *ukey) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < n) ukey[i] = usage_u(recs, rows, idx[i]);
+}
+// head[i] = 1 where item idx[i] starts an object in the sorted order.
+__global__ void k_usage_heads(const UsageRec *recs, const UsageRow *rows, uint32_t n, const uint32_t *idx,
+    uint32_t *head) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	head[i] = i == 0 || usage_u(recs, rows, idx[i]) != usage_u(recs, rows, idx[i - 1]) ||
+	    usage_genid(recs, rows, idx[i]) != usage_genid(recs, rows, idx[i - 1]);
+}
+// rid[i] = 1 + the row of sorted item i.  The head of each row sets the row up; the last item gives the count.
+__global__ void k_usage_rows_init(const UsageRec *recs, const UsageRow *rows, uint32_t n, const uint32_t *idx,
+    const uint32_t *rid, UsageRow *out, unsigned long long *n_rows) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	if (i == n - 1) *n_rows = rid[i];
+	if (i > 0 && rid[i] == rid[i - 1]) return;
+	UsageRow o{};
+	o.u = usage_u(recs, rows, idx[i]); o.genid = usage_genid(recs, rows, idx[i]);
+	o.first_page = o.oldest_ts = ~0ull;
+	out[rid[i] - 1] = o;
+}
+// Each warp folds its run of each row by a segmented shuffle scan (a row's items are contiguous), then
+// the last lane of the run adds it into the row: at most two atomic updates per row per warp.
+__global__ void __launch_bounds__(256) k_usage_fold(const UsageRec *recs, const UsageRow *rows, uint32_t n,
+    const uint32_t *idx, const uint32_t *rid, UsageRow *out) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	const int lane = threadIdx.x & 31;
+	const uint32_t me = i < n ? rid[i] : 0u;
+	UsageRow v{};
+	if (i < n) v = usage_item(recs, rows, idx[i]);
+	for (int d = 1; d < 32; d <<= 1) {
+		UsageRow o;
+		const uint32_t orid = __shfl_up_sync(0xffffffffu, me, d);
+		o.pages = __shfl_up_sync(0xffffffffu, v.pages, d);
+		o.tier_pages = __shfl_up_sync(0xffffffffu, v.tier_pages, d);
+		o.pinned_pages = __shfl_up_sync(0xffffffffu, v.pinned_pages, d);
+		o.stored_bytes = __shfl_up_sync(0xffffffffu, v.stored_bytes, d);
+		o.first_page = __shfl_up_sync(0xffffffffu, v.first_page, d);
+		o.last_page = __shfl_up_sync(0xffffffffu, v.last_page, d);
+		o.oldest_ts = __shfl_up_sync(0xffffffffu, v.oldest_ts, d);
+		o.newest_ts = __shfl_up_sync(0xffffffffu, v.newest_ts, d);
+		if (lane >= d && orid == me) usage_fold_into(v, o);
+	}
+	const uint32_t next = __shfl_down_sync(0xffffffffu, me, 1);
+	if (i >= n || (lane != 31 && next == me && i + 1 < n)) return;
+	UsageRow &r = out[me - 1];
+	atomicAdd(&r.pages, v.pages);
+	atomicAdd(&r.tier_pages, v.tier_pages);
+	atomicAdd(&r.pinned_pages, v.pinned_pages);
+	atomicAdd(&r.stored_bytes, v.stored_bytes);
+	atomicMin(&r.first_page, v.first_page);
+	atomicMax(&r.last_page, v.last_page);
+	atomicMin(&r.oldest_ts, v.oldest_ts);
+	atomicMax(&r.newest_ts, v.newest_ts);
+}
+__global__ void k_usage_okeys(const UsageRow *rows, uint32_t n, unsigned long long *okey, uint32_t *idx) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= n) return;
+	okey[i] = ~rows[i].stored_bytes;                      // ascending ~bytes = descending bytes
+	idx[i] = i;
+}
+__global__ void k_usage_take(const UsageRow *rows, const uint32_t *idx, uint32_t take, UsageRow *out) {
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < take) out[i] = rows[idx[i]];
+}
+
+int launch_residency(TableView t, unsigned long long u, unsigned long long l_first, unsigned long long l_last,
+    bool scan, ulonglong2 *hits, unsigned long long *cursor, uint64_t max_n, cudaStream_t st) {
+	if (scan) {
+		const uint64_t n = t.cap + 2;
+		k_residency_scan<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, u, l_first, l_last, hits, cursor, max_n);
+	} else {
+		const uint64_t n = l_last - l_first + 1;
+		k_residency_keys<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, u, l_first, n, hits, cursor, max_n);
+	}
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+int launch_usage_list(TableView t, PinView p, uint32_t bsize, UsageRec *recs, unsigned long long *cursor,
+    uint64_t max_n, cudaStream_t st) {
+	const uint64_t n = t.cap + 2;
+	k_usage_list<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(t, p, bsize, recs, cursor, max_n);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+// Scratch of a grouping of n items, each region 256-byte aligned: genid keys and indices, two buffers
+// each (the second genid buffer then holds the row numbers); u keys, two buffers; CUB's temporary storage.
+static size_t al256(size_t v) { return (v + 255) & ~(size_t)255; }
+static size_t usage_cub_bytes(uint32_t n) {
+	size_t a = 0, b = 0, c = 0;
+	cub::DoubleBuffer<uint32_t> k32(nullptr, nullptr), v32(nullptr, nullptr);
+	cub::DoubleBuffer<unsigned long long> k64(nullptr, nullptr);
+	cub::DeviceRadixSort::SortPairs(nullptr, a, k32, v32, (int)n, 0, 20);
+	cub::DeviceRadixSort::SortPairs(nullptr, b, k64, v32, (int)n, 0, 64);
+	cub::DeviceScan::InclusiveSum(nullptr, c, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)n);
+	return std::max(a, std::max(b, c));
+}
+size_t usage_group_bytes(uint64_t n) {
+	return 4 * al256(n * 4) + 2 * al256(n * 8) + al256(usage_cub_bytes((uint32_t)n));
+}
+
+int launch_usage_group(const UsageRec *recs, const UsageRow *rows_in, uint32_t n, UsageRow *rows_out,
+    unsigned long long *n_rows, void *scratch, cudaStream_t st) {
+	if (n == 0) {
+		CMB_CHECK(cudaMemsetAsync(n_rows, 0, sizeof(unsigned long long), st));
+		return 0;
+	}
+	uint8_t *p = (uint8_t *)scratch;
+	uint32_t *g0 = (uint32_t *)p, *g1 = (uint32_t *)(p + al256(n * 4));
+	uint32_t *i0 = (uint32_t *)(p + 2 * al256(n * 4)), *i1 = (uint32_t *)(p + 3 * al256(n * 4));
+	unsigned long long *u0 = (unsigned long long *)(p + 4 * al256(n * 4)), *u1 = u0 + al256(n * 8) / 8;
+	void *tmp = p + 4 * al256(n * 4) + 2 * al256(n * 8);
+	size_t tmp_bytes = usage_cub_bytes(n);
+	// stable LSD order: by genid, then by u
+	k_usage_gkeys<<<GRID1D(n), 0, st>>>(recs, rows_in, n, g0, i0);
+	CMB_CHECK(cudaGetLastError());
+	cub::DoubleBuffer<uint32_t> gk(g0, g1), ix(i0, i1);
+	CMB_CHECK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, gk, ix, (int)n, 0, 20, st));
+	k_usage_ukeys<<<GRID1D(n), 0, st>>>(recs, rows_in, n, ix.Current(), u0);
+	CMB_CHECK(cudaGetLastError());
+	cub::DoubleBuffer<unsigned long long> uk(u0, u1);
+	CMB_CHECK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, uk, ix, (int)n, 0, 64, st));
+	const uint32_t *idx = ix.Current();
+	uint32_t *head = g0, *rid = g1;
+	k_usage_heads<<<GRID1D(n), 0, st>>>(recs, rows_in, n, idx, head);
+	CMB_CHECK(cudaGetLastError());
+	CMB_CHECK(cub::DeviceScan::InclusiveSum(tmp, tmp_bytes, head, rid, (int)n, st));
+	k_usage_rows_init<<<GRID1D(n), 0, st>>>(recs, rows_in, n, idx, rid, rows_out, n_rows);
+	CMB_CHECK(cudaGetLastError());
+	k_usage_fold<<<GRID1D(n), 0, st>>>(recs, rows_in, n, idx, rid, rows_out);
+	CMB_CHECK(cudaGetLastError());
+	return 0;
+}
+
+int launch_usage_order(const UsageRow *rows, uint32_t n, UsageRow *out, uint32_t take, void *scratch,
+    cudaStream_t st) {
+	if (n == 0 || take == 0) return 0;
+	uint8_t *p = (uint8_t *)scratch;
+	uint32_t *i0 = (uint32_t *)(p + 2 * al256(n * 4)), *i1 = (uint32_t *)(p + 3 * al256(n * 4));
+	unsigned long long *k0 = (unsigned long long *)(p + 4 * al256(n * 4)), *k1 = k0 + al256(n * 8) / 8;
+	void *tmp = p + 4 * al256(n * 4) + 2 * al256(n * 8);
+	size_t tmp_bytes = usage_cub_bytes(n);
+	k_usage_okeys<<<GRID1D(n), 0, st>>>(rows, n, k0, i0);
+	CMB_CHECK(cudaGetLastError());
+	// stable: rows of equal bytes stay in (u, genid) order
+	cub::DoubleBuffer<unsigned long long> ok(k0, k1);
+	cub::DoubleBuffer<uint32_t> ix(i0, i1);
+	CMB_CHECK(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, ok, ix, (int)n, 0, 64, st));
+	k_usage_take<<<GRID1D(take), 0, st>>>(rows, ix.Current(), take, out);
 	CMB_CHECK(cudaGetLastError());
 	return 0;
 }

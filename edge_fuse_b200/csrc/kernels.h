@@ -301,6 +301,45 @@ int launch_sample(TableView t, PinView p, const unsigned long long *r, uint32_t 
 int launch_pin_select(TableView t, PinView p, uint64_t keyed_pages, unsigned long long *counts, ulonglong2 *list,
     unsigned long long *cursor, uint32_t max_n, cudaStream_t st);
 
+// ---- usage and residency (cmb200_residency, cmb200_usage_set): read-only scans of the table ----
+// cmb200_residency: every live local record of {u, l}, l_first <= l <= l_last, selected as
+// cmb200_invalidate selects (scan: k_residency_scan, one thread per slot; else k_residency_keys, one
+// thread per l), goes to hits[cursor[0]++] = {l, 1 arena | 2 host tier} while the index is below max_n;
+// cursor[0] ends at the number found.
+int launch_residency(TableView t, unsigned long long u, unsigned long long l_first, unsigned long long l_last,
+    bool scan, ulonglong2 *hits, unsigned long long *cursor, uint64_t max_n, cudaStream_t st);
+
+// One live local record as k_usage_list lists it.  flags: USAGE_TIER (in the host tier), USAGE_PINNED
+// (its address is in the pin list).
+struct UsageRec {
+	unsigned long long u, l, ts;
+	uint32_t len, flags;            // len: 24-byte prefix + LZ4 block or raw page
+};
+static_assert(sizeof(UsageRec) == 32, "usage record layout");
+constexpr uint32_t USAGE_TIER = 1u, USAGE_PINNED = 2u;
+// One object's row, laid out as cmb200_object_usage (engine.cu checks it).
+struct UsageRow {
+	unsigned long long u;
+	uint32_t genid, reserved;
+	unsigned long long pages, tier_pages, pinned_pages, stored_bytes;
+	unsigned long long first_page, last_page, oldest_ts, newest_ts;
+};
+static_assert(sizeof(UsageRow) == 80, "usage row layout");
+
+// k_usage_list: one thread per slot (cap + 2); every live local record goes to recs[cursor[0]++] while
+// the index is below max_n; cursor[0] ends at the number found.
+int launch_usage_list(TableView t, PinView p, uint32_t bsize, UsageRec *recs, unsigned long long *cursor,
+    uint64_t max_n, cudaStream_t st);
+// Groups n items, records (recs) or rows (rows_in; exactly one of the two is set), by (u, genid) into
+// rows_out, sorted by (u, genid); *n_rows (a device word) = the rows.  Scratch: usage_group_bytes(n).
+size_t usage_group_bytes(uint64_t n);
+int launch_usage_group(const UsageRec *recs, const UsageRow *rows_in, uint32_t n, UsageRow *rows_out,
+    unsigned long long *n_rows, void *scratch, cudaStream_t st);
+// The first `take` of n rows in the public order (stored_bytes descending, then u, then genid; rows must
+// be sorted by (u, genid)) go to out.  Scratch: usage_group_bytes(n).
+int launch_usage_order(const UsageRow *rows, uint32_t n, UsageRow *out, uint32_t take, void *scratch,
+    cudaStream_t st);
+
 int launch_read_fp(TableView t, const unsigned long long *addr, uint32_t n, uint64_t *fp_out, int32_t *ok,
     cudaStream_t st);
 // words_out[CKPT_WORDS i + k] = checkpoint word k of the key's slot (t.ckpt must be set); ok[i] = 1: a local

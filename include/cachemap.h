@@ -188,6 +188,46 @@ uint64_t cachemap_unpin(struct cachemap *cm, uint64_t nhid_small, uint32_t genid
 /* pinned = pages named by pins; in_hbm / in_tier = pinned pages cached in the arena / the host tier. */
 void cachemap_pin_stats(struct cachemap *cm, uint64_t *pinned, uint64_t *in_hbm, uint64_t *in_tier);
 
+/*
+ * What the cache holds, read off the key table on the GPU (DESIGN.md §2, *Usage and residency*).
+ * Both calls answer for every page cachemap_put accepted before the call (the write-behind rings are
+ * drained first), and count only records stored on this map's engines, in HBM or in the host tier.
+ * A page not loaded yet by a CMB200_LOAD=background load is not cached, as a get would answer.  A call
+ * before the first get starts the engines and answers for the loaded snapshot, as cachemap_invalidate
+ * does.  Neither call changes anything else: the request and hit counters, the frequency sketch, ghost
+ * entries, record timestamps, the host tier's hot log and promotion, and the checkpoint change count all
+ * stay as they were.  A small get that touches a record (CMB200_EVICT=access) while a usage scan runs may
+ * or may not show in newest_ts: the benign race of touches (cmb200_get_small).
+ *
+ * cachemap_residency: vec gets one byte per page of object (nhid_small, genid) that overlaps bytes
+ * [off, off + size), partial pages at both ends included, as cachemap_pin counts them: CACHEMAP_IN_HBM or
+ * CACHEMAP_IN_TIER if the page is cached, 0 if it is not, with CACHEMAP_PINNED ORed in when the address is
+ * pinned, cached or not.  Returns the pages cached, or -1, leaving vec untouched, when size is 0 or
+ * CACHEMAP_TO_END, when the first or the last page does not fit 44 bits, or when an engine cannot answer.
+ *
+ * cachemap_usage: returns the number of objects (nhid_small, genid) with at least one cached page, or -1
+ * if any engine cannot answer (nothing partial is returned).  out gets the first min(max, count) of them
+ * ordered by stored_bytes descending, then nhid_small ascending, then genid ascending; max = 0 counts
+ * only.
+ */
+#define CACHEMAP_IN_HBM  1u
+#define CACHEMAP_IN_TIER 2u
+#define CACHEMAP_PINNED  4u
+int64_t cachemap_residency(struct cachemap *cm, uint64_t nhid_small, uint32_t genid, uint64_t off, uint64_t size,
+    uint8_t *vec);
+
+struct cachemap_object_usage {
+	uint64_t nhid_small;
+	uint32_t genid, reserved;          /* reserved = 0 */
+	uint64_t pages;                    /* cached pages: HBM + host tier */
+	uint64_t tier_pages;               /* of those, in the host tier */
+	uint64_t pinned_pages;             /* of those, at pinned addresses */
+	uint64_t stored_bytes;             /* sum of record lengths: 24-byte prefix + LZ4 block or raw page */
+	uint64_t first_page, last_page;    /* lowest / highest cached page number */
+	uint64_t oldest_ts, newest_ts;     /* lowest / highest record ts (put time, or last hit under CMB200_EVICT=access) */
+};
+int64_t cachemap_usage(struct cachemap *cm, size_t max, struct cachemap_object_usage *out);
+
 /* requests / hits counters (cachemap.c:176,181) and the engine under the map. */
 void cachemap_get_counters(struct cachemap *cm, uint64_t *requests, uint64_t *hits);
 /* CMB200_ADMIT=freq: pages admitted over the victim they were paired with, and pages rejected (not stored,

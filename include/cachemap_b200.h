@@ -263,6 +263,31 @@ int cmb200_pin_set(cmb200_engine *e, size_t n, const cmb200_pin_range *r);
 int cmb200_pin_count(cmb200_engine *e, uint64_t *in_arena, uint64_t *in_tier);
 int cmb200_pin_promote(cmb200_engine *e, uint64_t *promoted_out);
 
+/* ---- usage and residency -----------------------------------------------------------------------
+ * Read-only views of the key table; nothing in it is written, nor any counter, sketch, ghost or stamp.
+ * cmb200_residency: out[l - l_first] = 1 for a record in the arena, 2 for one in the host tier, for every
+ * live local record stored at {u, l}, l_first <= l <= l_last; every other byte of out is left as it is (so
+ * one zeroed vector can gather several engines).  The records are selected as cmb200_invalidate selects
+ * them: key by key up to its threshold (a key that holds another object's address is not counted), by a
+ * scan of every slot, side slots included, above it.  The kernels list the records found; the device
+ * memory a call takes grows with them, not with the interval.
+ * cmb200_usage_set: one row per object {u, genid = l >> 44} with a live local record on any of the g
+ * engines (the rows of an object spread over the engines by key are summed), ordered by stored_bytes
+ * descending, then u, then genid.  *objects_out = the number of rows; out gets the first min(max, rows).
+ * pinned_pages counts records at addresses of the engine's pin list (cmb200_pin_set).  Each engine is
+ * scanned under its lock on its stream; scratch HBM is allocated for the call and freed before it returns
+ * (a failed allocation is -1 with the error set).  Both calls are -1 on an engine that has made a
+ * multi-GPU call, as cmb200_invalidate is. */
+typedef struct cmb200_object_usage {
+	uint64_t u;
+	uint32_t genid, reserved;
+	uint64_t pages, tier_pages, pinned_pages, stored_bytes;
+	uint64_t first_page, last_page, oldest_ts, newest_ts;
+} cmb200_object_usage;
+int cmb200_residency(cmb200_engine *e, uint64_t u, uint64_t l_first, uint64_t l_last, uint8_t *out);
+int cmb200_usage_set(cmb200_engine *const *engines, int g, size_t max, cmb200_object_usage *out,
+    uint64_t *objects_out);
+
 /* Copies the stored record of each address — the bytes the reference keeps in LMDB:
  * 24-byte data_prefix + payload (filemap.c:9-12,140-147) — into out (stride bytes apart) and its
  * total length into len_out (-1 = absent). */
